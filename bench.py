@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """bench.py — faces/sec of the SMIRK hot path (encode -> FLAME -> render @224^2, and the full cycle with
-SmirkGenerator) on N B200s.
+SmirkGenerator) on N H100s.
 
 Contract (see DESIGN.md §Measurement):
   python bench.py --gpus N --steps K --warmup W            product arm (under torchrun for N > 1)
@@ -13,8 +13,8 @@ workloads and prints ONE JSON line:
                 (`--full-batch`; `--no-full-cycle` skips it, `--generator` makes it the headline instead).
 For each workload:
   value     faces/s with the input batches resident in HBM: CUDA-graph replay over `--slots` pipeline lanes, CUDA events
-            around exactly K steps, repeated over `--windows` back-to-back windows; the reported figure is the MEDIAN
-            window (min / max / relative spread alongside), max over ranks per window.  Inputs rotate over a set of
+            around exactly K timed steps (`--windows R` > 1 repeats the K-step window R times and reports the MEDIAN
+            window, min / max / relative spread alongside), max over ranks per window.  Inputs rotate over a set of
             batches larger than L2.  For N > 1 the NCCL all-gather of the final outputs runs INSIDE the timed region
             (on a communication stream, overlapping the next batch); `no_gather` repeats the measurement without it.
   e2e       the same metric through SmirkPipeline.run_host(): pinned host images -> H2D -> graph -> D2H of rendered
@@ -26,6 +26,11 @@ For each workload:
   parity    max errors of the timed configuration against the CPU oracle, checked in-run on one batch.
   cpu_baseline: `bench.py --impl reference` run as a child process on the host cores (so both arms share one code path
             and one thread-count choice).
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step of each workload returned (rendered image,
+vertices, FLAME parameters, + reconstructed image for the full cycle) as DIR/<workload>_<name>.npy (float32); a workload
+whose outputs exceed 32 MB is cut to a fixed, seeded sample of faces (DIR/<workload>_faces.npy lists them).  Inputs and
+weights are seeded, so two builds run with the same arguments can be compared output for output.  With N > 1 GPUs rank 0
+writes its own shard (the outputs of its last batch, before the all-gather).
 """
 import argparse
 import json
@@ -48,16 +53,18 @@ CONSTANT_BYTES = {False: 38.0e6, True: 163.5e6}             # weights / FLAME co
 
 
 def load_peaks():
+    # NVIDIA's H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s — a ceiling, not a measurement
+    sheet = dict(hbm=3350.0, tensor=989.0, tensor_sustained=989.0, source="data sheet (H100 SXM)")
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return dict(hbm=float(d["hbm_gbs"]), tensor=float(d.get("bf16_tflops", 1590.0)),
-                    tensor_sustained=float(d.get("bf16_tflops_sustained", 1400.0)), source="measured")
-    return dict(hbm=6650.0, tensor=1590.0, tensor_sustained=1400.0, source="fallback")
+        return dict(hbm=float(d.get("hbm_gbs", sheet["hbm"])), tensor=float(d.get("bf16_tflops", sheet["tensor"])),
+                    tensor_sustained=float(d.get("bf16_tflops_sustained", sheet["tensor_sustained"])), source="measured")
+    return sheet
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -277,6 +284,26 @@ def window_stats(ms, K):
             "rel_spread": (max(ms) - min(ms)) / med if med > 0 else None}
 
 
+DUMP_BYTES_PER_WORKLOAD = 32 << 20
+
+
+def dump_outputs(dirpath, workload, out, keys):
+    """`out` = the output tensors of one timed step (batch-major).  Writes DIR/<workload>_<key>.npy in float32; if the step's
+    outputs exceed DUMP_BYTES_PER_WORKLOAD, a fixed seeded sample of faces (same for every run) is kept and listed."""
+    import numpy as np
+    import torch
+    torch.cuda.synchronize()
+    B = out[keys[0]].shape[0]
+    per_face = sum(out[k][0].numel() * 4 for k in keys)
+    n = max(1, min(B, DUMP_BYTES_PER_WORKLOAD // per_face))
+    faces = np.arange(B) if n == B else np.sort(np.random.default_rng(0).choice(B, n, replace=False))
+    idx = torch.as_tensor(faces, device=out[keys[0]].device)
+    for k in keys:
+        np.save(os.path.join(dirpath, "%s_%s.npy" % (workload, k)), out[k].index_select(0, idx).float().cpu().numpy())
+    if n < B:
+        np.save(os.path.join(dirpath, "%s_faces.npy" % workload), faces.astype(np.float32))
+
+
 def run_workload(cx, args, B, generator, slots, R, with_cpu):
     """Measure one workload (device-resident, e2e, ± gather for N > 1, kernel breakdown, parity).  Returns a dict."""
     import torch
@@ -302,7 +329,7 @@ def run_workload(cx, args, B, generator, slots, R, with_cpu):
         stage = MaskingStage(fl.faces_tensor, synth_inputs.face_probabilities(fl.faces_tensor.shape[0]), seed=1234 + rank)
     pipe = SmirkPipeline(enc, fl, rd, gen, device=dev, slots=slots, masking=stage)
 
-    # rotating input set larger than L2 (126 MB): Rset batches of B x 602 KB (x2 with the masked image)
+    # rotating input set larger than L2 (50 MB on H100): Rset batches of B x 602 KB (x2 with the masked image)
     per = B * 224 * 224 * 4 * (4 if generator else 3)
     Rset = max(2, -(-160_000_000 // per))
     host_imgs = [synth_inputs.images(B, 5000 + rank * 100 + i).pin_memory() for i in range(Rset)]
@@ -315,7 +342,7 @@ def run_workload(cx, args, B, generator, slots, R, with_cpu):
     keys = ("rendered_img", "vertices", "params") + (("reconstructed_img",) if generator else ())
 
     def dev_step(i):            # batch i goes to lane i % slots (own stream + graph replica): consecutive batches overlap
-        pipe.submit(i, dev_imgs[i % Rset], dev_masks[i % Rset] if generator else None)
+        cx.last_out = pipe.submit(i, dev_imgs[i % Rset], dev_masks[i % Rset] if generator else None)
 
     def host_step(i):
         cx.last = pipe.run_host(host_imgs[i % Rset], i, host_masks[i % Rset] if generator else None, keys)
@@ -331,8 +358,10 @@ def run_workload(cx, args, B, generator, slots, R, with_cpu):
     out["windows"] = window_stats(ms, K)
     out["ms_per_step"] = out["windows"]["median_ms"] / K
     out["value"] = faces / (out["windows"]["median_ms"] / 1e3)
+    if args.dump_outputs and rank == 0:             # the last timed step's outputs, before another pass reuses the lane
+        dump_outputs(args.dump_outputs, "full_cycle" if (generator and not args.generator) else "headline", cx.last_out, keys)
     h2d, d2h = pipe.bytes_per_step(B, keys)
-    ms2 = timed_windows(cx, host_step, pipe.join, K, W, max(3, R // 2))
+    ms2 = timed_windows(cx, host_step, pipe.join, K, W, R)
     out["e2e"] = {"value": faces / (statistics.median(ms2) / 1e3), "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                   "ms_per_step": statistics.median(ms2) / K, "windows": window_stats(ms2, K),
                   "api": "SmirkPipeline.run_host (pinned host in/out, %d lanes, copies on their own streams)" % pipe.slots,
@@ -347,8 +376,8 @@ def run_workload(cx, args, B, generator, slots, R, with_cpu):
         if pipe._gather_backend == "p2p" and isinstance(p2p, dict):
             out["gather"]["form"] = "packed: one staging copy, one push per peer, lane released after the pack" if p2p.get("pack") else "direct: one push per (output, peer)"
         pipe.enable_gather(())
-        ms3 = timed_windows(cx, dev_step, pipe.join, K, W, max(3, R // 2))
-        ms4 = timed_windows(cx, host_step, pipe.join, K, W, max(3, R // 2))
+        ms3 = timed_windows(cx, dev_step, pipe.join, K, W, R)
+        ms4 = timed_windows(cx, host_step, pipe.join, K, W, R)
         out["no_gather"] = {"value": faces / (statistics.median(ms3) / 1e3), "ms_per_step": statistics.median(ms3) / K,
                             "e2e_value": faces / (statistics.median(ms4) / 1e3)}
 
@@ -374,24 +403,17 @@ def run_workload(cx, args, B, generator, slots, R, with_cpu):
         v["gbs"] = v["bytes"] / v["ms"] / 1e6
         v["tflops"] = v["flops"] / v["ms"] / 1e9
     top_tag, top = max(breakdown.items(), key=lambda kv: kv[1]["ms"])
-    # Every tensor-core kernel here computes in TF32: its ceiling is HALF the measured bf16 GEMM peak (tcgen05 kind::tf32
-    # runs at half the kind::f16 rate), and the hbm/tensor ridge is judged against that.
+    # Every tensor-core kernel here computes in TF32: its ceiling is HALF the bf16 GEMM peak (wgmma TF32 runs at half the
+    # BF16 rate), and the hbm/tensor ridge is judged against that.
     tf32_peak = peaks["tensor"] / 2.0
     ai = top["flops"] / max(top["bytes"], 1.0)
     ridge = tf32_peak * 1e3 / peaks["hbm"]
     if "tc" in top_tag and ai > ridge:
         roof = {"bound": "tensor", "achieved": top["tflops"], "peak": tf32_peak, "unit": "TFLOP/s",
-                "peak_note": "TF32 = measured bf16 cuBLAS peak / 2"}
+                "peak_note": "TF32 = bf16 peak / 2"}
     else:
         roof = {"bound": "hbm", "achieved": top["gbs"], "peak": peaks["hbm"], "unit": "GB/s"}
-    traffic, step_traffic = None, None
-    tname = "r02_ncu_dram_traffic_%s_b%d_%s.json" % ("c3" if generator else "c2", B, args.precision)
-    tpath = os.path.join(ROOT, "profiles", tname)
-    if os.path.exists(tpath):
-        tj = json.load(open(tpath))
-        tk = tj.get("kernels", {}).get(top_tag.split(":")[0])
-        traffic = tk["traffic_bytes_per_launch"] if tk else None
-        step_traffic = tj.get("step_traffic_bytes")
+    traffic, step_traffic = None, None                 # measured DRAM traffic: not available without a hardware profiler
     roof.update(frac=roof["achieved"] / roof["peak"], traffic=traffic, kernel=top_tag, share_of_step=top["share"],
                 launches_per_step=top["launches"] / NP, us_per_launch=top["ms_per_launch"] * 1e3, peak_source=peaks["source"],
                 arithmetic_intensity=ai, ridge_flop_per_byte=ridge,
@@ -451,7 +473,10 @@ def main():
     ap.add_argument("--full-batch", type=int, default=256, help="faces per GPU per step of the full-cycle workload (configs[2]/[4] = 256)")
     ap.add_argument("--generator", action="store_true", help="make the full cycle (with SmirkGenerator) the headline workload at --batch")
     ap.add_argument("--no-full-cycle", action="store_true", help="skip the extra full_cycle block")
-    ap.add_argument("--windows", type=int, default=21, help="back-to-back repeats of the K-step timed window (median reported)")
+    ap.add_argument("--windows", type=int, default=1, help="back-to-back repeats of the K-step timed window (median reported)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs of each workload to DIR/<workload>_<name>.npy (float32, <= 64 MB in all; "
+                         "with N > 1 GPUs rank 0's own shard)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity", action="store_true")
     ap.add_argument("--no-gather", action="store_true", help="N > 1: leave the NCCL all-gather of the outputs out of the timed region")
@@ -462,12 +487,15 @@ def main():
     ap.add_argument("--full-slots", type=int, default=2)
     ap.add_argument("--profile-out", default=None, help="write the per-kernel breakdown JSON here (suffix _c2 / _c3 added)")
     ap.add_argument("--precision", default="tf32x3", choices=sorted(PRECISIONS),
-                    help="encoder arithmetic.  tf32x3: tcgen05 tensor cores with error-compensated 3xTF32 products (fp32-equivalent; "
+                    help="encoder arithmetic.  tf32x3: wgmma tensor cores with error-compensated 3xTF32 products (fp32-equivalent; "
                          "the parity path and the default); tf32: plain TF32 tensor cores (the reference's cuDNN default); "
-                         "fp32: exact fp32 CUDA cores.  The generator runs TF32 tcgen05 unless fp32 is chosen.")
+                         "fp32: exact fp32 CUDA cores.  The generator runs TF32 wgmma unless fp32 is chosen.")
     args = ap.parse_args()
     if args.profile_out:
         args.profile_out = os.path.abspath(args.profile_out)
+    if args.dump_outputs:
+        args.dump_outputs = os.path.abspath(args.dump_outputs)
+        os.makedirs(args.dump_outputs, exist_ok=True)
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -505,7 +533,7 @@ def main():
     head = run_workload(cx, args, args.batch, args.generator, args.slots, max(1, args.windows), with_cpu=(world == 1 and not args.no_cpu_baseline))
     full = None
     if not args.generator and not args.no_full_cycle:
-        full = run_workload(cx, args, args.full_batch, True, args.full_slots, max(1, min(args.windows, 5)), with_cpu=False)
+        full = run_workload(cx, args, args.full_batch, True, args.full_slots, max(1, args.windows), with_cpu=False)
 
     if rank == 0:
         B, K = args.batch, args.steps
@@ -515,13 +543,13 @@ def main():
             "dtype": {"tf32x3": "tf32x3", "tf32": "tf32", "tf32-unfused": "tf32", "fp32": "f32"}[args.precision],
             "data": "synthetic",
             "config": {"workload": workload_name(args.generator, B), "precision": args.precision,
-                       "arithmetic": {"tf32x3": "encoder convs: tcgen05 TF32 products, 3-term error-compensated (fp32-equivalent), fp32 accumulate; FLAME / rasteriser f32",
-                                      "tf32": "encoder convs: tcgen05 TF32, fp32 accumulate; FLAME / rasteriser f32",
-                                      "tf32-unfused": "encoder convs: tcgen05 TF32, fp32 accumulate; FLAME / rasteriser f32",
+                       "arithmetic": {"tf32x3": "encoder convs: wgmma TF32 products, 3-term error-compensated (fp32-equivalent), fp32 accumulate; FLAME / rasteriser f32",
+                                      "tf32": "encoder convs: wgmma TF32, fp32 accumulate; FLAME / rasteriser f32",
+                                      "tf32-unfused": "encoder convs: wgmma TF32, fp32 accumulate; FLAME / rasteriser f32",
                                       "fp32": "f32 CUDA cores throughout"}[args.precision],
                        "global_batch": B * world,
                        "faces_per_gpu_per_step": B, "image": "224x224 RGB fp32", "parallelism": "frame-shard dp%d" % world,
-                       "l2_policy": "inputs rotate over a set of batches > 126 MB L2 (160 MB)",
+                       "l2_policy": "inputs rotate over a set of batches (160 MB) larger than the 50 MB L2",
                        "timing": "median of %d back-to-back windows of exactly %d steps (CUDA events, max over ranks per window)" % (head["windows"]["n"], K),
                        "execution": "CUDA graph replay, %d kernels per step, %d-lane software pipeline over consecutive steps" % (head["launches_per_step"], args.slots),
                        "host_affinity": affinity},

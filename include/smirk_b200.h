@@ -1,5 +1,5 @@
 /*
- * smirk_b200 — C ABI of the B200-native SMIRK hot path (encode -> FLAME -> render -> generator).
+ * smirk_b200 — C ABI of the H100-native SMIRK hot path (encode -> FLAME -> render -> generator).
  *
  * The reference (georgeretsi/smirk) is pure Python and has no FFI of its own; its only native seams
  * on this path are third-party: `timm.create_model` (src/smirk_encoder.py:7-12), ATen/cuDNN ops, and
@@ -125,7 +125,7 @@ typedef struct {
     const float* head_b[3];
     int n_shape;               /* 300 */
     int n_exp;                 /* 50 */
-    int precision;             /* 0 = fp32 CUDA-core GEMMs, 1 = TF32 tcgen05 GEMMs for the 1x1 convs,
+    int precision;             /* 0 = fp32 CUDA-core GEMMs, 1 = TF32 wgmma GEMMs for the 1x1 convs,
                                   2 = 1 + inverted-residual blocks run expand-1x1 + depthwise-3x3 as one fused kernel,
                                   3 = 2 with error-compensated "3xTF32" tensor-core arithmetic (operands split into TF32
                                       head + tail, three products per term): fp32-equivalent results, the parity path */
@@ -149,7 +149,7 @@ typedef struct {
     /* fp32 tensors of the module's state_dict in state_dict order, `num_batches_tracked` removed.    */
     const float* const* tensors;
     int n_tensors;
-    int precision;             /* 0 = fp32 CUDA-core implicit GEMM, 1 = TF32 tcgen05 implicit GEMM */
+    int precision;             /* 0 = fp32 CUDA-core implicit GEMM, 1 = TF32 wgmma implicit GEMM */
 } SmkGeneratorDesc;
 
 int smk_generator_create(const SmkGeneratorDesc* desc, SmkGenerator** out);
@@ -239,7 +239,7 @@ int smk_peer_fan_push(SmkPeerFan* f, void* const* dsts, int n, const void* src, 
  * not part of the drop-in surface).  All pointers are device pointers.
  *   smk_debug_conv_f32: fp32 CUDA-core implicit GEMM.  w_kn is [K][N]; mode 0 = 1x1, 1 = 3x3 zero pad,
  *                       2 = 3x3 reflection pad; shuffle = 1 stores ConvTranspose2d(k2,s2) pixel-shuffled.
- *   smk_debug_conv_tc : TF32 tcgen05 implicit GEMM.  wt is [N][K]; mode 2 expects `in` to be a
+ *   smk_debug_conv_tc : TF32 wgmma implicit GEMM.  wt is [N][K]; mode 2 expects `in` to be a
  *                       [B,H+2,W+2,*] buffer whose halo was filled by smk_debug_reflect_halo;
  *                       store 0 plain, 1 pixel-shuffle, 2 interior of a padded [B,H+2,W+2,*] buffer.
  * ---------------------------------------------------------------------------------------------- */
@@ -250,14 +250,14 @@ int smk_debug_conv_tc(const float* in, int ld_in, int B, int H, int W, int Cin, 
                       const float* bias, int N, int K, int mode, int relu, const float* res, int ld_res, int res_pad,
                       float* out, int ld_out, int store, void* stream);
 int smk_debug_reflect_halo(float* buf, int B, int H, int W, int C, void* stream);
-/*   smk_debug_xdw: fused expand-1x1 (TF32 tcgen05) + BN + ReLU + depthwise-3x3 (fp32) + BN + ReLU of a
+/*   smk_debug_xdw: fused expand-1x1 (TF32 wgmma) + BN + ReLU + depthwise-3x3 (fp32) + BN + ReLU of a
  *                  MobileNetV3 inverted-residual block.  x [B,H,W,Cin] NHWC; w1t [mid][Cin]; wdw [9][mid];
  *                  out [B,ceil(H/stride),ceil(W/stride),mid]; TF-SAME padding.                            */
 int smk_debug_xdw(const float* x, int B, int H, int W, int Cin, const float* w1t, const float* scale1, const float* bias1,
                   int mid, const float* wdw, const float* scale2, const float* bias2, int stride, int round_out,
                   float* out, void* stream);
 
-/*   smk_debug_conv3_win: the persistent windowed TF32 tcgen05 3x3 convolution of the high-resolution narrow layers
+/*   smk_debug_conv3_win: the persistent windowed TF32 wgmma 3x3 convolution of the high-resolution narrow layers
  *                  (zero padding 1, N in {32, 64}, Cin % 32 == 0, W >= 56, resident weights <= 72 KB); wt is [N][9*Cin].      */
 int smk_debug_conv3_win(const float* in, int ld_in, int B, int H, int W, int Cin, const float* wt, const float* scale,
                         const float* bias, int N, int relu, float* out, int ld_out, void* stream);

@@ -1,7 +1,7 @@
-"""smirk_b200 — B200-native implementation of SMIRK's per-frame hot path
+"""smirk_b200 — H100-native implementation of SMIRK's per-frame hot path
 (SmirkEncoder -> FLAME -> Renderer -> SmirkGenerator) behind the reference's class signatures.
 
-All arithmetic runs in hand-written sm_100a CUDA (``csrc/``) behind the C ABI of
+All arithmetic runs in hand-written sm_90a CUDA (``csrc/``) behind the C ABI of
 ``include/smirk_b200.h``; PyTorch supplies device memory, streams and torch.distributed only.
 """
 from .flame import FLAME                    # noqa: F401

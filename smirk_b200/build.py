@@ -1,4 +1,4 @@
-"""Build recipe: smirk_b200/csrc/*.cu -> smirk_b200/libsmirk_b200.so (sm_100a only, in-tree).
+"""Build recipe: smirk_b200/csrc/*.cu -> smirk_b200/libsmirk_b200.so (sm_90a only, in-tree).
 
 nvcc cross-compiles without a GPU.  Objects are cached by mtime.  Per-file flags:
 render.cu is compiled with -fmad=false so the rasteriser's fp32 arithmetic is never contracted into
@@ -13,8 +13,8 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "csrc", "build")
 LIB = os.path.join(HERE, "libsmirk_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-BASE = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
-        "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+BASE = ARCH + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 PER_FILE = {"render.cu": ["-fmad=false"]}
 
 
@@ -42,7 +42,7 @@ def build(force=False, verbose=False):
                 fh.write(r.stdout + r.stderr)
             rebuilt = True
     if rebuilt or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+        cmd = [NVCC, "-shared", "-o", LIB] + objs + ARCH + ["-cudart", "static"]
         subprocess.check_call(cmd)
     return LIB
 

@@ -39,9 +39,18 @@ void prof_begin(const char* tag, double bytes, double flops, cudaStream_t st) {
     g_pending = true; g_pending_stream = st;
 }
 bool profiling() { return g_prof; }
+int num_sms() {
+    static int cached[64] = {0};
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) dev = 0;
+    if (dev < 64 && cached[dev]) return cached[dev];
+    int n = 0;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+    if (dev < 64) cached[dev] = n;
+    return n;
+}
 // Off by default: with 3 backbone streams x 4 batches in flight the launch gaps are already filled by other
-// kernels and programmatic edges measured neutral-to-slightly-negative end to end (profiles/r01_footprint_sweep.txt);
-// SMK_PDL=1 turns the launch attribute on (useful for a single low-latency stream: +3 % at one lane).
+// kernels; SMK_PDL=1 turns the launch attribute on (meant for a single low-latency stream).
 bool pdl_enabled() { static const bool on = []() { const char* e = getenv("SMK_PDL"); return e && atoi(e) != 0; }(); return on; }
 void prof_end() {
     if (!g_prof || !g_pending) return;

@@ -1,4 +1,4 @@
-// Shared helpers for the smirk_b200 CUDA library (sm_100a only).
+// Shared helpers for the smirk_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -69,12 +69,15 @@ static inline size_t ws_round(size_t bytes) { return (bytes + 255) & ~size_t(255
 
 static inline int cdiv(long a, long b) { return (int)((a + b - 1) / b); }
 
+// Streaming multiprocessors of the current device (cached per device ordinal): the size of a persistent grid.
+int num_sms();
+
 // ---- programmatic dependent launch (PDL) --------------------------------------------------------------
 // Every kernel of the library is launched with cudaLaunchAttributeProgrammaticStreamSerialization and starts
 // with pdl_sync(): `griddepcontrol.wait` blocks until the preceding kernel on the stream has completed and
 // flushed (so every global read AND write of this kernel stays ordered after it), `griddepcontrol.
 // launch_dependents` lets the following kernel's CTAs be scheduled as soon as all CTAs of this one have
-// started.  Net effect: launch latency, parameter/tensor-map fetch, barrier init and TMEM allocation of
+// started.  Net effect: launch latency, parameter/tensor-map fetch, barrier init and tensor-map prefetch of
 // kernel N+1 overlap the tail of kernel N — which is what a chain of ~100 short kernels per batch is bound
 // by.  Inside a stream capture these become programmatic graph edges.  The attribute is opt-in (SMK_PDL=1, see
 // common.cu); without it the device-side instructions are no-ops.
@@ -99,7 +102,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 
 // TF32 rounding (round-to-nearest, ties away: PTX cvt.rna).  The tensor cores read fp32 words from shared
 // memory and simply ignore the 13 low mantissa bits (truncation, a systematic bias); operands that feed
-// a tcgen05 layer are therefore rounded once, where they are produced: weights on the host at pack
+// a tensor-core layer are therefore rounded once, where they are produced: weights on the host at pack
 // time, activations in the epilogue of the kernel that writes them — what cuDNN/CUTLASS TF32 kernels
 // do with cvt.rna in registers before mma.
 #ifdef __CUDACC__
@@ -108,32 +111,15 @@ __device__ __forceinline__ float round_tf32(float x) {
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
     return __uint_as_float(u);
 }
-// Packed fp32 FMA (Blackwell FFMA2: two IEEE fused multiply-adds per instruction on 64-bit register pairs).
-// Same rounding as two scalar fmaf calls; halves the issue slots of the CUDA-core inner loops.
+// float4 fused multiply-adds (four IEEE fmaf each) of the CUDA-core inner loops.
 __device__ __forceinline__ void fma4_acc(float4& acc, const float4& x, const float4& k) {    // acc += x * k
-    uint64_t* a = reinterpret_cast<uint64_t*>(&acc);
-    const uint64_t* xx = reinterpret_cast<const uint64_t*>(&x);
-    const uint64_t* kk = reinterpret_cast<const uint64_t*>(&k);
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(a[0]) : "l"(xx[0]), "l"(kk[0]));
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(a[1]) : "l"(xx[1]), "l"(kk[1]));
+    acc.x = fmaf(x.x, k.x, acc.x); acc.y = fmaf(x.y, k.y, acc.y); acc.z = fmaf(x.z, k.z, acc.z); acc.w = fmaf(x.w, k.w, acc.w);
 }
 __device__ __forceinline__ void fma4_s(float4& acc, float x, const float4& k) {              // acc += x * k (scalar x)
-    uint64_t xx;
-    asm("mov.b64 %0, {%1, %1};" : "=l"(xx) : "f"(x));
-    uint64_t* a = reinterpret_cast<uint64_t*>(&acc);
-    const uint64_t* kk = reinterpret_cast<const uint64_t*>(&k);
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(a[0]) : "l"(xx), "l"(kk[0]));
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(a[1]) : "l"(xx), "l"(kk[1]));
+    acc.x = fmaf(x, k.x, acc.x); acc.y = fmaf(x, k.y, acc.y); acc.z = fmaf(x, k.z, acc.z); acc.w = fmaf(x, k.w, acc.w);
 }
 __device__ __forceinline__ float4 fma4(const float4& x, const float4& s, const float4& b) {  // x * s + b
-    float4 o;
-    uint64_t* oo = reinterpret_cast<uint64_t*>(&o);
-    const uint64_t* xx = reinterpret_cast<const uint64_t*>(&x);
-    const uint64_t* ss = reinterpret_cast<const uint64_t*>(&s);
-    const uint64_t* bb = reinterpret_cast<const uint64_t*>(&b);
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(oo[0]) : "l"(xx[0]), "l"(ss[0]), "l"(bb[0]));
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(oo[1]) : "l"(xx[1]), "l"(ss[1]), "l"(bb[1]));
-    return o;
+    return make_float4(fmaf(x.x, s.x, b.x), fmaf(x.y, s.y, b.y), fmaf(x.z, s.z, b.z), fmaf(x.w, s.w, b.w));
 }
 #endif
 static inline float round_tf32_host(float x) {

@@ -1,26 +1,26 @@
 // 3x3 stride-1 convolution for the generator's HIGH-RESOLUTION, NARROW layers (224^2 and 112^2, Cout = 32 / 64;
-// reference src/smirk_generator.py:56-60,73-76 -> `_block` :88-119) as a persistent "windowed" TF32 tcgen05 implicit GEMM.
+// reference src/smirk_generator.py:56-60,73-76 -> `_block` :88-119) as a persistent "windowed" TF32 wgmma implicit GEMM.
 //
 // Why a second 3x3 kernel.  gemm_tc.cu feeds the nine filter taps with nine im2col TMA loads per 32-channel chunk, so
 // every input pixel crosses L2 -> shared memory nine times, and every tile re-loads the layer's weights.  For the wide, deep
-// layers that hides behind the MMAs (14^2 x 512: 697 TFLOP/s).  With Cout = 32 the MMAs are tiny (128 x 32 x 8: 19 % tensor-pipe
-// activity in profiles/r02_ncu_full_c3_H224_K32_N32.txt) and a tile's life is a serial chain of short steps.  Here:
+// layers that hides behind the MMAs.  With Cout = 32 the MMAs are tiny (128 x 32 x 8) and a tile's life is a serial chain of
+// short steps.  Here:
 //
 //   output tile   4 x 30 pixels of one image
 //   patch         6 x 32 pixels x 32 channels = 192 rows of 128 bytes, one 4-D tiled TMA box (out-of-image halo zero
 //                 filled = the conv's zero padding), SWIZZLE_128B, row r = py * 32 + px — loaded ONCE per channel chunk
-//   tap (dy,dx)   A operand = the 128 consecutive patch rows starting at row dy*32 + dx: only the UMMA descriptor's start
-//                 address moves (the tensor core derives the swizzle phase from the absolute shared-memory address, as TMA
-//                 does when it writes).  GEMM row m <-> output pixel (m / 32, m % 32); columns 30, 31 of each row wrap
-//                 into the halo and are not stored (93.75 % useful rows).
+//   tap (dy,dx)   A operand = the 128 consecutive patch rows starting at row dy*32 + dx: only the wgmma descriptor's start
+//                 address moves (the swizzle follows the absolute shared-memory address, as TMA's does when it writes).
+//                 GEMM row m <-> output pixel (m / 32, m % 32); columns 30, 31 of each row wrap into the halo and are not
+//                 stored (93.75 % useful rows).
 //   weights       [N][9*Cin] K-major; the 9 * Cin/32 boxes of BN x 32 are loaded once per CTA and stay in shared memory
-//   two pipelines one CTA per SM runs TWO independent tile pipelines (each: TMA producer warp, MMA issuer warp, four epilogue
-//                 warps, a 2-deep patch ring, a double-buffered accumulator in TMEM) that share the resident weights.
-//                 Measured at B = 256, 224^2 x 32 -> 32: one pipeline per SM 1174 us (no better than im2col's 1079 us: a tile's
-//                 load -> 36 MMAs -> drain chain is latency-bound per pipeline, not L2-bound), two pipelines per SM 711 us.
+//   two pipelines one CTA per SM runs TWO independent tile pipelines (each: a TMA producer warp and one consumer warpgroup
+//                 that issues the wgmmas — two m64 halves of the 128-row tile — and runs the epilogue from its accumulator
+//                 registers, a 2-deep patch ring) that share the resident weights, so one pipeline's loads and epilogue
+//                 overlap the other's MMAs.
 // L2 -> SM traffic per output pixel drops from 9 x 128 B (+ the weights again for every tile) to 1.6 x 128 B.
 // Epilogue as in gemm_tc.cu (folded BN, ReLU, TF32 rounding, coalesced NHWC stores) plus the fused 1x1 head + sigmoid of
-// the network's last layer (store 3), computed per pixel right after tcgen05.ld.
+// the network's last layer (store 3).
 #include "gemm_tc.cuh"
 #include "tc_ptx.cuh"
 #include <cuda.h>
@@ -32,15 +32,16 @@ namespace {
 using namespace ptx;
 
 constexpr int PIPES = 2;
-constexpr int PIPE_THREADS = 192;                    // warp 0 TMA, warp 1 MMA, warps 2..5 epilogue
-constexpr int NUM_THREADS = PIPES * PIPE_THREADS;
+constexpr int NUM_THREADS = PIPES * 128 + PIPES * 32;   // warps 0..7: consumer warpgroups (pipeline = warp / 4); warps 8, 9: TMA producers
 constexpr int PW = 32, TH = 4, TW = 30;              // patch width, output tile height / width
 constexpr int PATCH_BYTES = (TH + 2) * PW * 128;     // 24 KiB
 constexpr int STAGES = 2;                            // patch ring depth per pipeline
-constexpr int SLAB_BYTES = 4 * 4096;                 // per pipeline
+constexpr int SLAB_BYTES = 4 * 2048;                 // per pipeline: 16 rows x 128 B per consumer warp
 constexpr int TAIL_BYTES = 1024;                     // the last tap view reads 2 rows past its patch: keep that inside the allocation
-constexpr int PIPE_BYTES = STAGES * PATCH_BYTES + TAIL_BYTES + SLAB_BYTES;      // 66 560 B
+constexpr int PIPE_BYTES = STAGES * PATCH_BYTES + TAIL_BYTES + SLAB_BYTES;      // 58 368 B
 constexpr int NB = 4;                                // weight-ring depth per pipeline (layers whose weights do not fit resident)
+constexpr int BAR_BYTES = 512;
+constexpr int HEAD_PAR_BYTES = 1088;                 // per pipeline, store 3: [32][8] per-channel constants + 4 head biases
 
 struct WinArgs {
     int H, W, N;
@@ -60,40 +61,32 @@ template <int BN, bool RES>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv3_win_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, const WinArgs a) {
     constexpr int B_BYTES = BN * 128;                      // one (chunk, tap) weight box
-    constexpr uint32_t TMEM_COLS = PIPES * 2 * BN;         // 128 / 256
-    constexpr uint32_t IDESC = make_idesc_tf32(128, BN);
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int pipe = warp / 6, pw = warp - pipe * 6;       // pipeline of this warp, role within it
+    const bool producer = warp >= PIPES * 4;
+    const int pipe = producer ? warp - PIPES * 4 : warp >> 2;      // pipeline of this warp
     uint8_t* sP = smem + pipe * PIPE_BYTES;                // this pipeline's patch ring (+ tail) ...
     uint8_t* slabs = sP + STAGES * PATCH_BYTES + TAIL_BYTES;      // ... and epilogue staging
     // weights: resident [chunk][tap][BN x 128 B] shared by both pipelines, or one NB-deep ring of boxes per pipeline
     const int w_bytes = RES ? a.nchunks * 9 * B_BYTES : PIPES * NB * B_BYTES;
     uint8_t* sW = smem + PIPES * PIPE_BYTES + (RES ? 0 : pipe * NB * B_BYTES);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + PIPES * PIPE_BYTES + w_bytes);
-    constexpr int PER_PIPE_BARS = 2 * STAGES + 4 + 2 * NB;
+    constexpr int PER_PIPE_BARS = 2 * STAGES + 2 * NB;
     uint64_t* w_full = bars;                               // [1]
-    uint64_t* p_full = bars + 1 + pipe * PER_PIPE_BARS;    // per pipeline: p_full[STAGES], p_empty[STAGES], acc_full[2], acc_empty[2], b_full[NB], b_empty[NB]
+    uint64_t* p_full = bars + 1 + pipe * PER_PIPE_BARS;    // per pipeline: p_full[STAGES], p_empty[STAGES], b_full[NB], b_empty[NB]
     uint64_t* p_empty = p_full + STAGES;
-    uint64_t* acc_full = p_empty + STAGES;
-    uint64_t* acc_empty = acc_full + 2;
-    uint64_t* b_full = acc_empty + 2;
+    uint64_t* b_full = p_empty + STAGES;
     uint64_t* b_empty = b_full + NB;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 1 + PIPES * PER_PIPE_BARS);
+    float* hpar = reinterpret_cast<float*>(smem + PIPES * PIPE_BYTES + w_bytes + BAR_BYTES + pipe * HEAD_PAR_BYTES);
 
-    if (pw == 0 && lane == 0) {
+    if (producer && lane == 0) {
         if (pipe == 0) { prefetch_tensormap(&tmX); prefetch_tensormap(&tmW); mbar_init(w_full, 1); }
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&p_full[s], 1); mbar_init(&p_empty[s], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 4); }
-        for (int i = 0; i < NB; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 1); }
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&p_full[s], 1); mbar_init(&p_empty[s], 4); }
+        for (int i = 0; i < NB; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 4); }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc<TMEM_COLS>(tmem_slot);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot + (uint32_t)(pipe * 2 * BN);       // this pipeline's two accumulators
     pdl_sync();
 
     auto decode = [&](int t, int& img, int& h0, int& w0) {
@@ -104,7 +97,7 @@ conv3_win_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
     // tiles are strided over (CTA, pipeline) pairs
     const int t_first = blockIdx.x * PIPES + pipe, t_step = gridDim.x * PIPES;
 
-    if (pw == 0) {
+    if (producer) {
         if (lane == 0) {
             // ===== TMA producer: (pipeline 0) the weights once; then one patch per (tile, channel chunk) =====
             if (RES && pipe == 0) {
@@ -133,91 +126,95 @@ conv3_win_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
                 }
             }
         }
-    } else if (pw == 1) {
-        if (lane == 0) {
-            // ===== MMA issuer =====
-            if (RES) { mbar_wait(w_full, 0); tcgen05_fence_after(); }
-            const uint32_t w_base = smem_u32(sW);
-            int it = 0, tc = 0, itb = 0;
-            for (int t = t_first; t < a.n_tiles; t += t_step, ++tc) {
-                const int buf = tc & 1;
-                mbar_wait(&acc_empty[buf], ((uint32_t)(tc >> 1) & 1u) ^ 1u);
-                tcgen05_fence_after();
-                const uint32_t d = tmem_base + (uint32_t)(buf * BN);
-                for (int c = 0; c < a.nchunks; ++c, ++it) {
-                    const int s = it % STAGES;
-                    mbar_wait(&p_full[s], (uint32_t)(it / STAGES) & 1u);
-                    tcgen05_fence_after();
-                    const uint32_t p_base = smem_u32(sP + s * PATCH_BYTES);
+        return;
+    }
+
+    // ===== consumer warpgroup of this pipeline: MMAs, then the epilogue from the accumulator registers =====
+    const int wq = warp & 3;
+    uint8_t* slab = slabs + wq * 2048;
+    const int sub = lane >> 3, jj = lane & 7;
+    if (BN == 32 && a.store == 3) {                      // head constants of channel `lane` (see gemm_tc.cu)
+        if (wq == 0) {
+            hpar[lane * 8 + 0] = __ldg(a.scale + lane); hpar[lane * 8 + 1] = __ldg(a.bias + lane);
 #pragma unroll
-                    for (int tap = 0; tap < 9; ++tap) {
-                        const uint32_t a_tap = p_base + (uint32_t)(((tap / 3) * PW + (tap % 3)) * 128);
-                        uint32_t b_tap;
-                        int sb = 0;
-                        if (RES) {
-                            b_tap = w_base + (uint32_t)((c * 9 + tap) * B_BYTES);
-                        } else {
-                            sb = itb % NB;
-                            mbar_wait(&b_full[sb], (uint32_t)(itb / NB) & 1u);
-                            tcgen05_fence_after();
-                            b_tap = w_base + (uint32_t)(sb * B_BYTES);
-                            ++itb;
-                        }
+            for (int co = 0; co < 4; ++co) hpar[lane * 8 + 2 + co] = co < a.head_c ? __ldg(a.head_w + (size_t)lane * a.head_c + co) : 0.f;
+            if (lane < 4) hpar[256 + lane] = lane < a.head_c ? __ldg(a.head_b + lane) : 0.f;
+        }
+        named_barrier(1 + pipe, 128);
+    }
+    if (RES) mbar_wait(w_full, 0);
+    const uint32_t w_base = smem_u32(sW);
+    int it = 0, itb = 0;
+    for (int t = t_first; t < a.n_tiles; t += t_step) {
+        int img, h0, w0;
+        decode(t, img, h0, w0);
+        float acc[2][BN / 2];
 #pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            umma_tf32(d, make_smem_desc(a_tap + k * 32), make_smem_desc(b_tap + k * 32), IDESC, (c | tap | k) != 0 ? 1u : 0u);
-                        if (!RES) tcgen05_commit(&b_empty[sb]);
-                    }
-                    tcgen05_commit(&p_empty[s]);             // the patch may be overwritten once these MMAs have read it
+        for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[mb][i] = 0.f;
+        for (int c = 0; c < a.nchunks; ++c, ++it) {
+            const int s = it % STAGES;
+            mbar_wait(&p_full[s], (uint32_t)(it / STAGES) & 1u);
+            const uint32_t p_base = smem_u32(sP + s * PATCH_BYTES);
+#pragma unroll
+            for (int tap = 0; tap < 9; ++tap) {
+                const uint32_t a_tap = p_base + (uint32_t)(((tap / 3) * PW + (tap % 3)) * 128);
+                uint32_t b_tap;
+                int sb = 0;
+                if (RES) {
+                    b_tap = w_base + (uint32_t)((c * 9 + tap) * B_BYTES);
+                } else {
+                    sb = itb % NB;
+                    mbar_wait(&b_full[sb], (uint32_t)(itb / NB) & 1u);
+                    b_tap = w_base + (uint32_t)(sb * B_BYTES);
+                    ++itb;
                 }
-                tcgen05_commit(&acc_full[buf]);
-            }
-        }
-    } else {
-        // ===== epilogue: four warps per pipeline, TMEM lane quarter = warp % 4 =====
-        const int quarter = warp & 3;
-        uint8_t* slab = slabs + (pw - 2) * 4096;
-        const int sub = lane >> 3, jj = lane & 7;
-        if (BN == 32 && a.store == 3) {                      // head constants of channel `lane` -> this warp's slab (see gemm_tc.cu)
-            float* par = reinterpret_cast<float*>(slab);
-            par[lane * 8 + 0] = __ldg(a.scale + lane); par[lane * 8 + 1] = __ldg(a.bias + lane);
+                wgmma_fence();
 #pragma unroll
-            for (int co = 0; co < 4; ++co) par[lane * 8 + 2 + co] = co < a.head_c ? __ldg(a.head_w + (size_t)lane * a.head_c + co) : 0.f;
-            if (lane < 4) par[256 + lane] = lane < a.head_c ? __ldg(a.head_b + lane) : 0.f;
-            __syncwarp();
-        }
-        int tc = 0;
-        for (int t = t_first; t < a.n_tiles; t += t_step, ++tc) {
-            int img, h0, w0;
-            decode(t, img, h0, w0);
-            const int buf = tc & 1;
-            mbar_wait(&acc_full[buf], (uint32_t)(tc >> 1) & 1u);
-            tcgen05_fence_after();
-#pragma unroll 1
-            for (int c0 = 0; c0 < BN; c0 += 32) {
-                float v[32];
-                tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * BN + c0), v);
-                if (c0 + 32 >= BN) {                         // last read of this accumulator: hand it back to the MMA warp
-                    tcgen05_fence_before();
+                for (int k = 0; k < 4; ++k)
+#pragma unroll
+                    for (int mb = 0; mb < 2; ++mb)
+                        Wgmma<BN>::ss(acc[mb], make_smem_desc(a_tap + mb * 64 * 128 + k * 32), make_smem_desc(b_tap + k * 32), 1u);
+                wgmma_commit();
+                if (!RES) {                                  // the weight box may be overwritten once these MMAs have read it
+                    wgmma_wait<0>();
                     __syncwarp();
-                    if (lane == 0) mbar_arrive(&acc_empty[buf]);
+                    if (lane == 0) mbar_arrive(&b_empty[sb]);
                 }
-                if (BN == 32 && a.store == 3) {
-                    // fused 1x1 head + sigmoid (smirk_generator.py:77-78 -> :86), N == BN == 32: lane = tile row = one pixel with all 32
-                    // accumulators in registers; constants by broadcast LDS from the slab; NCHW stores
-                    const float* par = reinterpret_cast<const float*>(slab);
-                    float a0 = par[256], a1 = par[257], a2 = par[258], a3 = par[259];
+            }
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&p_empty[s]);         // the patch may be overwritten
+        }
 #pragma unroll
-                    for (int nn = 0; nn < 32; ++nn) {
-                        const float4 p0 = *reinterpret_cast<const float4*>(par + nn * 8);
-                        const float2 p1 = *reinterpret_cast<const float2*>(par + nn * 8 + 4);
-                        float x = fmaf(v[nn], p0.x, p0.y);
-                        if (a.relu) x = fmaxf(x, 0.f);
-                        a0 = fmaf(x, p0.z, a0); a1 = fmaf(x, p0.w, a1); a2 = fmaf(x, p1.x, a2); a3 = fmaf(x, p1.y, a3);
-                    }
-                    const int m = quarter * 32 + lane, oy = m / PW, ox = m - oy * PW;
+        for (int mb = 0; mb < 2; ++mb) {
+            const int mrow = mb * 64 + wq * 16;              // first tile row of this warp's slab
+#pragma unroll
+            for (int c0 = 0; c0 < BN; c0 += 32) {
+                stage32<BN>(slab, acc[mb], c0, lane);
+                __syncwarp();
+                if (BN == 32 && a.store == 3) {
+                    // fused 1x1 head + sigmoid (smirk_generator.py:77-78 -> :86), N == BN == 32: lane r < 16 = slab row r = one
+                    // pixel with all 32 accumulators; constants by broadcast LDS; NCHW stores
+                    const int m = mrow + lane, oy = m / PW, ox = m - oy * PW;
                     const int oh = h0 + oy, ow = w0 + ox;
-                    if (ox < TW && oh < a.H && ow < a.W) {
+                    if (lane < 16 && ox < TW && oh < a.H && ow < a.W) {
+                        float a0 = hpar[256], a1 = hpar[257], a2 = hpar[258], a3 = hpar[259];
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {
+                            const float4 x4 = slab_chunk(slab, lane, j);
+                            const float xs[4] = {x4.x, x4.y, x4.z, x4.w};
+#pragma unroll
+                            for (int e = 0; e < 4; ++e) {
+                                const int nn = 4 * j + e;
+                                const float4 p0 = *reinterpret_cast<const float4*>(hpar + nn * 8);
+                                const float2 p1 = *reinterpret_cast<const float2*>(hpar + nn * 8 + 4);
+                                float x = fmaf(xs[e], p0.x, p0.y);
+                                if (a.relu) x = fmaxf(x, 0.f);
+                                a0 = fmaf(x, p0.z, a0); a1 = fmaf(x, p0.w, a1); a2 = fmaf(x, p1.x, a2); a3 = fmaf(x, p1.y, a3);
+                            }
+                        }
                         const int hw_px = a.H * a.W;
                         float* dst = a.out + (size_t)img * a.head_c * hw_px + (size_t)oh * a.W + ow;
                         dst[0] = 1.f / (1.f + __expf(-a0));
@@ -225,23 +222,20 @@ conv3_win_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
                         if (a.head_c > 2) dst[2 * (size_t)hw_px] = 1.f / (1.f + __expf(-a2));
                         if (a.head_c > 3) dst[3 * (size_t)hw_px] = 1.f / (1.f + __expf(-a3));
                     }
+                    __syncwarp();
                     continue;
                 }
-#pragma unroll
-                for (int j = 0; j < 8; ++j)
-                    *reinterpret_cast<float4*>(slab + lane * 128 + ((j ^ (lane & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                __syncwarp();
                 const int nc = c0 + jj * 4;
                 if (nc < a.N) {
                     const float4 sc = __ldg(reinterpret_cast<const float4*>(a.scale + nc));
                     const float4 bi = __ldg(reinterpret_cast<const float4*>(a.bias + nc));
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) {
+                    for (int i = 0; i < 4; ++i) {
                         const int r = 4 * i + sub;
-                        const int m = quarter * 32 + r, oy = m / PW, ox = m - oy * PW;
+                        const int m = mrow + r, oy = m / PW, ox = m - oy * PW;
                         const int oh = h0 + oy, ow = w0 + ox;
                         if (!(ox < TW && oh < a.H && ow < a.W)) continue;
-                        const float4 x = *reinterpret_cast<const float4*>(slab + r * 128 + ((jj ^ (r & 7)) << 4));
+                        const float4 x = slab_chunk(slab, r, jj);
                         float4 o;
                         o.x = fmaf(x.x, sc.x, bi.x); o.y = fmaf(x.y, sc.y, bi.y); o.z = fmaf(x.z, sc.z, bi.z); o.w = fmaf(x.w, sc.w, bi.w);
                         if (a.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
@@ -252,12 +246,6 @@ conv3_win_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
                 __syncwarp();
             }
         }
-        tcgen05_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc<TMEM_COLS>(*tmem_slot);
     }
 }
 
@@ -277,7 +265,7 @@ int load_encoder() {
 }
 
 size_t win_smem_bytes(int nchunks, int BN, bool res) {
-    return (size_t)PIPES * PIPE_BYTES + (res ? (size_t)nchunks * 9 * BN * 128 : (size_t)PIPES * NB * BN * 128) + 512 + 1024;
+    return (size_t)PIPES * PIPE_BYTES + (res ? (size_t)nchunks * 9 * BN * 128 : (size_t)PIPES * NB * BN * 128) + BAR_BYTES + PIPES * HEAD_PAR_BYTES + 1024;
 }
 bool win_resident(int nchunks, int BN) { return win_smem_bytes(nchunks, BN, true) <= 227 * 1024; }
 
@@ -292,7 +280,7 @@ int launch(const CUtensorMap& tmX, const CUtensorMap& tmW, const WinArgs& a, cud
         SMK_CHECK_CUDA(cudaFuncSetAttribute((conv3_win_kernel<BN, RES>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         if (dev < 64) configured_mask |= 1ull << dev;
     }
-    SMK_LAUNCH((conv3_win_kernel<BN, RES>), dim3((unsigned)std::min(cdiv(a.n_tiles, PIPES), 148)), dim3(NUM_THREADS), smem, st, tmX, tmW, a);
+    SMK_LAUNCH((conv3_win_kernel<BN, RES>), dim3((unsigned)std::min(cdiv(a.n_tiles, PIPES), num_sms())), dim3(NUM_THREADS), smem, st, tmX, tmW, a);
     SMK_CHECK_LAUNCH();
     return 0;
 }

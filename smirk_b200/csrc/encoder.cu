@@ -17,7 +17,7 @@ using smk::ConvProblem;
 
 constexpr float kBnEps = 1e-3f;
 
-struct ConvW { float* w = nullptr; float* wt = nullptr; float* wt_lo = nullptr; float* scale = nullptr; float* bias = nullptr; int cin = 0, cout = 0; };   // w: [K][N] fp32 path, wt: [N][K] tcgen05 path (TF32 heads), wt_lo: TF32 tails (3xTF32 path)
+struct ConvW { float* w = nullptr; float* wt = nullptr; float* wt_lo = nullptr; float* scale = nullptr; float* bias = nullptr; int cin = 0, cout = 0; };   // w: [K][N] fp32 path, wt: [N][K] tensor-core path (TF32 heads), wt_lo: TF32 tails (3xTF32 path)
 enum Kind { DS = 0, IR = 1, CN = 2 };
 struct BlockDef { Kind kind; int stride; float exp; int cout; };
 struct Block { Kind kind; int stride, cin, mid, cout; bool skip; ConvW pw, dw, pwl; ConvW pw_f32; };   // pw_f32: fp32 [K][N] copy of a DS block's 1x1 (fused stem path)
@@ -123,7 +123,7 @@ struct SmkEncoder {
 extern "C" int smk_encoder_create(const SmkEncoderDesc* desc, SmkEncoder** out) {
     SMK_REQUIRE(desc && out, "smk_encoder_create: null argument");
     SMK_REQUIRE(desc->precision >= 0 && desc->precision <= 3,
-                "smk_encoder_create: precision must be 0 (fp32 CUDA cores), 1 (tf32 tcgen05 1x1 convs), 2 (1 + fused expand/depthwise blocks) or "
+                "smk_encoder_create: precision must be 0 (fp32 CUDA cores), 1 (tf32 wgmma 1x1 convs), 2 (1 + fused expand/depthwise blocks) or "
                 "3 (2 with 3xTF32 error-compensated tensor-core arithmetic: fp32-equivalent results)");
     if (desc->precision >= 1) { if (int rc = smk::tc_init()) return rc; }
     const bool tc = desc->precision >= 1;
@@ -311,8 +311,8 @@ extern "C" int smk_encoder_forward(const SmkEncoder* h, const float* img, int B,
                     rc = smk::dwconv3x3(x[k], B, res, res, b[k]->cin, b[k]->stride, b[k]->dw.w, b[k]->dw.scale, b[k]->dw.bias, d[k], st, rnd);
                 if (!rc) rc = pointwise(n, pw, d, B, ro, ro, false, b0.skip ? x : nullptr, y, st);
             } else if (b0.kind == IR) {
-                // The 7x7 layers (a 16x16 window holds 81 useful pixels, 49 outputs) run 3 % faster end to end as
-                // 1x1 GEMM + depthwise kernels; every other resolution wins fused (profiles/r01_footprint_sweep.txt).
+                // The 7x7 layers (a 16x16 window holds 81 useful pixels, 49 outputs) run as 1x1 GEMM + depthwise kernels:
+                // most of a window would be halo; every other resolution runs fused.
                 static const int xdw_min_res = []() { const char* e = getenv("SMK_XDW_MIN_RES"); return e ? atoi(e) : 8; }();
                 if (h->fuse_xdw && b0.pw.wt && res >= xdw_min_res) {
                     // expand 1x1 + depthwise 3x3 in one kernel: the expanded tensor never leaves the SM

@@ -1,4 +1,4 @@
-// FLAME forward on sm_100a: blendshapes + pose correctives + linear blend skinning + eyelids + landmarks.
+// FLAME forward on sm_90a: blendshapes + pose correctives + linear blend skinning + eyelids + landmarks.
 //
 // Replaces FLAME.forward (reference src/FLAME/FLAME.py:232-315) and lbs() (src/FLAME/lbs.py:140-227).
 // Three launches per batch, all fp32 FMA (this stage is memory/latency bound; tensor cores would

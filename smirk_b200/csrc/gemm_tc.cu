@@ -1,4 +1,4 @@
-// TF32 tcgen05 implicit-GEMM convolution for sm_100a:  C[M,N] = epi( A[M,K] * W[N,K]^T ).
+// TF32 tensor-core implicit-GEMM convolution for sm_90a (Hopper wgmma):  C[M,N] = epi( A[M,K] * W[N,K]^T ).
 //
 // This is the tensor-core path of the generator's 3x3 convolutions / transposed convolutions and of
 // the encoder's 1x1 convolutions (precision = 1).  The reference executes these layers as cuDNN
@@ -11,16 +11,16 @@
 //     fills the padding halo, writing a 128 x 32-channel (128-byte rows) SWIZZLE_128B tile into
 //     shared memory.  No im2col matrix is ever materialised.
 //   * W ([N][K], K-major, K ordered (tap, channel)) comes in through a 2-D TMA box of BN x 32.
-//   * One elected thread issues `tcgen05.mma.cta_group::1.kind::tf32` (M=128, N=BN, K=8 per
-//     instruction, 4 per 128-byte k-block); the fp32 accumulator lives in TMEM (BN columns).
-//   * A STAGES-deep mbarrier ring decouples the TMA producer warp from the MMA warp;
-//     `tcgen05.commit` releases shared-memory stages and finally signals the epilogue warps, which
-//     read the accumulator with `tcgen05.ld.32x32b`, apply folded BatchNorm scale/bias, optional
-//     residual and ReLU, and store NHWC rows — plain, into a channel slice of a concat buffer, into
-//     the interior of a reflection-padded buffer, or pixel-shuffled (ConvTranspose2d k2 s2).
+//   * Two consumer warpgroups each own 64 rows of the 128-row tile and issue
+//     `wgmma.mma_async.m64nBNk8.f32.tf32.tf32` from shared-memory descriptors (4 per 128-byte k-block); the fp32
+//     accumulators live in registers (BN / 2 per thread).
+//   * A STAGES-deep mbarrier ring decouples the TMA producer warp from the consumers; a consumer releases a stage
+//     as soon as the wgmma group that read it has retired (one group stays in flight).  The epilogue — folded
+//     BatchNorm scale/bias, optional residual and ReLU, NHWC stores plain, into a channel slice of a concat buffer,
+//     into the interior of a reflection-padded buffer, or pixel-shuffled (ConvTranspose2d k2 s2) — runs in the same
+//     warps, straight from the accumulator registers through a per-warp staging slab.
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer,
-// warps 2..5 = epilogue (warp_id % 4 selects the TMEM lane quarter each may access).
+// Threads (288): warps 0..7 = consumers (warpgroups 0 and 1), warp 8 = TMA producer.
 #include "gemm_tc.cuh"
 #include "tc_ptx.cuh"
 #include <cuda.h>
@@ -31,13 +31,15 @@ namespace {
 constexpr int BM = 128;
 constexpr int BKB = 128;                  // bytes of K per k-block = one SWIZZLE_128B row = 32 fp32
 constexpr int BK = 32;
-constexpr int UMMA_K = 8;                 // tf32
+constexpr int MMA_K = 8;                  // tf32
 constexpr int A_STAGE_BYTES = BM * BKB;   // 16 KiB
-constexpr int NUM_THREADS = 192;
-constexpr int SLAB_BYTES = 4 * 4096;      // epilogue staging: 32 rows x 128 B per epilogue warp
+constexpr int CONSUMER_WARPS = 8;
+constexpr int NUM_THREADS = CONSUMER_WARPS * 32 + 32;
+constexpr int SLAB_BYTES = CONSUMER_WARPS * 2048;     // epilogue staging: 16 rows x 128 B per consumer warp
+constexpr int BAR_BYTES = 256;
+constexpr int HEAD_PAR_BYTES = 1088;                  // store 3: [32][8] per-channel constants + 4 head biases
 
-using namespace ptx;                      // PTX wrappers shared by the tcgen05 kernels (tc_ptx.cuh)
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) { return make_idesc_tf32(M, N); }
+using namespace ptx;                      // PTX wrappers shared by the tensor-core kernels (tc_ptx.cuh)
 
 struct TcArgs {
     int M, N, nkb;                 // nkb = number of 32-wide k-blocks
@@ -58,8 +60,6 @@ struct TcArgs {
     int store;                     // 0 plain, 1 pixel-shuffle (N = 4*Cout), 2 interior of a (H+2)x(W+2) padded buffer,
                                    // 3 fused head: out[b, co, h, w] = sigmoid(head_b[co] + sum_n act[m, n] * head_w[n][co]) (NCHW, N <= 32)
     int round_out;                 // 1: round the stored activations to TF32 (round-to-nearest) for the next tensor-core layer
-    int x3_trunc;                  // 3xTF32, tails in TMEM: 1 = rely on the tensor core TRUNCATING fp32 words to TF32 (head = a & ~0x1fff is
-                                   // implicit, nothing is written back to shared memory); 0 = rewrite the heads (round-to-nearest) in place
     const float* head_w; const float* head_b; int head_c;      // store 3: 1x1 head weights [N][head_c], bias [head_c], head_c <= 4
 };
 
@@ -69,67 +69,46 @@ template <int BN, int STAGES, int MINB, bool PERSIST, int X3>
 __global__ void __launch_bounds__(NUM_THREADS, MINB)
 gemm_tc_kernel(const __grid_constant__ TcMaps mp, const TcArgs a) {
     // Output tiles (128 rows x BN columns) are strided over the grid.
-    //   PERSIST = true : grid = resident CTAs; the smem ring runs across tile boundaries and the accumulator is
-    //                    double-buffered in TMEM, so the TMA loads and MMAs of tile i+1 overlap the epilogue of
-    //                    tile i.  Wins for the deep-K 3x3 convolutions (measured, profiles/r01_gemm_tc_persist.txt).
-    //   PERSIST = false: grid = tiles, one tile per CTA, the epilogue staging slab aliases the (by then idle)
-    //                    first ring stage and TMEM holds one accumulator: smaller footprint -> 3-5 CTAs per SM,
-    //                    which is what the shallow-K streaming 1x1 layers want (more epilogue warps in flight).
+    //   PERSIST = true : grid = resident CTAs; the smem ring runs across tile boundaries, so the TMA loads of tile i+1
+    //                    are in flight while the consumers run the epilogue of tile i.
+    //   PERSIST = false: grid = tiles, one tile per CTA, and each consumer warp's staging slab aliases the A rows of ring
+    //                    stage 0 that only its own warpgroup reads (and has finished reading when the epilogue starts):
+    //                    a smaller footprint, so more CTAs of this kernel and of the concurrent pipeline's other kernels
+    //                    share an SM, which is what the shallow-K streaming 1x1 layers want.
     //   X3 = 2         : error-compensated "3xTF32" arithmetic (fp32-equivalent results on the tensor cores).  Every fp32
     //                    operand is split into a TF32 head and a TF32 tail, a = a_hi + a_lo, and three products are
     //                    accumulated: a_hi*w_hi + a_lo*w_hi + a_hi*w_lo (the dropped a_lo*w_lo term is ~2^-22 relative).
-    //                    Weights are split on the host (TcMaps::blo maps the tails).  The activation tile is split after TMA has
-    //                    landed it, by the epilogue warps — otherwise idle during the main loop of a single-tile CTA: thread =
-    //                    tile row = TMEM lane; the tails go to TENSOR MEMORY (32 columns per ring stage next to the
-    //                    accumulator) and are multiplied with the A-from-TMEM form of tcgen05.mma; the heads are what the
-    //                    tensor core reads from the fp32 words itself (it truncates to TF32; x3_trunc = 0 rewrites them in
-    //                    place, round to nearest).  The shared-memory footprint is that of the plain TF32 kernel plus the
-    //                    weight tails, so as many CTAs share an SM as before — which is what the concurrent pipeline's
-    //                    throughput hangs on (DESIGN.md "footprint beats per-kernel speed").  A first cut with the tails in a
-    //                    second shared-memory tile cost 10 % end to end (27.2k vs 30.2k faces/s) and was removed.
-    static_assert(!X3 || !PERSIST, "the 3xTF32 split borrows the epilogue warps: single-tile CTAs only");
+    //                    Weights are split on the host (TcMaps::blo maps the tails).  The activation tile is split in
+    //                    registers by the consumers (A fragments of the register form of wgmma), so shared memory holds
+    //                    only the plain kernel's tiles plus the weight tails.
+    static_assert(!X3 || !PERSIST, "3xTF32 runs single-tile CTAs");
     constexpr int B_STAGE_BYTES = BN * BKB;
     constexpr int HALF_STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
     constexpr int STAGE_BYTES = X3 ? HALF_STAGE_BYTES + B_STAGE_BYTES : HALF_STAGE_BYTES;         // [A][B] (+ [B tails])
     constexpr int BLO_OFF = HALF_STAGE_BYTES;                                                       // weight tails within a stage
-    constexpr uint32_t ALO_COL = PERSIST ? 2 * BN : BN;                                            // X3 == 2: first TMEM column of the A tails
-    constexpr uint32_t TMEM_NEED = (PERSIST ? 2 * BN : BN) + (X3 == 2 ? STAGES * 32 : 0);
-    constexpr uint32_t TMEM_COLS = TMEM_NEED <= 32 ? 32 : TMEM_NEED <= 64 ? 64 : TMEM_NEED <= 128 ? 128 : TMEM_NEED <= 256 ? 256 : 512;
-    constexpr uint32_t IDESC = make_idesc(BM, BN);
     extern __shared__ uint8_t smem_raw[];
     // 1024-byte alignment for SWIZZLE_128B; offset arithmetic keeps the shared address space visible to the
     // compiler (LDS/STS for the staging slab instead of generic LD/ST).
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* slabs = PERSIST ? smem + STAGES * STAGE_BYTES : smem;      // 4 x 4 KiB epilogue staging, one per epilogue warp
+    uint8_t* slabs = PERSIST ? smem + STAGES * STAGE_BYTES : smem;      // 8 x 2 KiB epilogue staging, one per consumer warp
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + (PERSIST ? SLAB_BYTES : 0));
     uint64_t* empty = full + STAGES;
-    uint64_t* acc_full = empty + STAGES;
-    uint64_t* acc_empty = acc_full + 2;
-    uint64_t* split = acc_empty + 2;                                    // X3: "stage s has been split" (4 epilogue warps arrive)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(split + STAGES);
+    float* hpar = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + BAR_BYTES);   // store 3 constants
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == CONSUMER_WARPS && lane == 0) {
         const int g0 = (!PERSIST && (int)blockIdx.x >= a.n_tiles_g) ? 1 : 0;
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&mp.a[g0]) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&mp.b[g0]) : "memory");
-        if (X3) asm volatile("prefetch.tensormap [%0];" ::"l"(&mp.blo[g0]) : "memory");
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); mbar_init(&split[s], 4); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 4); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        prefetch_tensormap(&mp.a[g0]);
+        prefetch_tensormap(&mp.b[g0]);
+        if (X3) prefetch_tensormap(&mp.blo[g0]);
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], CONSUMER_WARPS); }
+        fence_barrier_init();
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    pdl_sync();                                // barriers, tensor maps and TMEM are set up; now wait for the producer layer
+    pdl_sync();                                // barriers and tensor maps are set up; now wait for the producer layer
 
-    if (warp == 0) {
+    if (warp == CONSUMER_WARPS) {
         if (lane == 0) {
             // ===== TMA producer =====
             int it = 0;
@@ -158,192 +137,160 @@ gemm_tc_kernel(const __grid_constant__ TcMaps mp, const TcArgs a) {
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ===== MMA issuer =====
-            int it = 0, tc = 0;
-            for (int t = blockIdx.x; t < a.n_tiles; t += gridDim.x, ++tc) {
-                const int buf = tc & 1;
-                mbar_wait(&acc_empty[buf], ((uint32_t)(tc >> 1) & 1u) ^ 1u);      // epilogue has drained this accumulator
-                tcgen05_fence_after();
-                for (int kb = 0; kb < a.nkb; ++kb, ++it) {
-                    const int s = it % STAGES;
-                    mbar_wait(X3 ? &split[s] : &full[s], (uint32_t)(it / STAGES) & 1u);
-                    tcgen05_fence_after();
-                    const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
-                    const uint32_t sb = sa + A_STAGE_BYTES;
+        return;
+    }
+
+    // ===== consumers: warpgroup wg owns tile rows [64 wg, 64 wg + 64); warp wq of it rows [64 wg + 16 wq, +16) =====
+    const int wg = warp >> 2, wq = warp & 3;
+    if (a.store == 3) {                                    // head constants of channel `lane` (read-only, shared by all warps)
+        if (warp == 0) {
+            hpar[lane * 8 + 0] = __ldg(a.scale[0] + lane); hpar[lane * 8 + 1] = __ldg(a.bias[0] + lane);
 #pragma unroll
-                    for (int k = 0; k < BK / UMMA_K; ++k) {
-                        uint64_t da = make_smem_desc(sa + k * UMMA_K * 4);
-                        uint64_t db = make_smem_desc(sb + k * UMMA_K * 4);
-                        umma_tf32(tmem_base + (uint32_t)(buf * BN), da, db, IDESC, (kb | k) != 0 ? 1u : 0u);
-                        if (X3) {
-                            uint64_t dbl = make_smem_desc(sa + BLO_OFF + k * UMMA_K * 4);
-                            umma_tf32_ts(tmem_base + (uint32_t)(buf * BN), tmem_base + ALO_COL + (uint32_t)(s * 32 + k * UMMA_K), db, IDESC, 1u);
-                            umma_tf32(tmem_base + (uint32_t)(buf * BN), da, dbl, IDESC, 1u);      // a_hi * w_lo
+            for (int co = 0; co < 4; ++co) hpar[lane * 8 + 2 + co] = co < a.head_c ? __ldg(a.head_w + (size_t)lane * a.head_c + co) : 0.f;
+            if (lane < 4) hpar[256 + lane] = lane < a.head_c ? __ldg(a.head_b + lane) : 0.f;
+        }
+        named_barrier(1, CONSUMER_WARPS * 32);
+    }
+    uint8_t* slab = slabs + warp * 2048;
+    const int sub = lane >> 3, jj = lane & 7;              // phase-2 role: row-in-group, 16-byte chunk
+    int it = 0;
+    for (int t = blockIdx.x; t < a.n_tiles; t += gridDim.x) {
+        const int g = t >= a.n_tiles_g ? 1 : 0, tt = t - g * a.n_tiles_g;
+        const int tm = tt / a.tiles_n, tn = tt - tm * a.tiles_n;
+        const int m0 = tm * BM, n0 = tn * BN;
+        float d[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+        int prev = -1;
+        for (int kb = 0; kb < a.nkb; ++kb, ++it) {
+            const int s = it % STAGES;
+            mbar_wait(&full[s], (uint32_t)(it / STAGES) & 1u);
+            uint8_t* st = smem + s * STAGE_BYTES;
+            const uint32_t sa = smem_u32(st) + (uint32_t)(wg * 64 * BKB);
+            const uint32_t sb = smem_u32(st) + A_STAGE_BYTES;
+            if constexpr (X3 != 0) {
+                uint32_t hi[BK / MMA_K][4], lo[BK / MMA_K][4];
+#pragma unroll
+                for (int k = 0; k < BK / MMA_K; ++k) {
+                    float v[4];
+                    load_a_frag(st, wg * 64, k * MMA_K, wq, lane, v);
+                    split_frag(v, hi[k], lo[k]);
+                }
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / MMA_K; ++k) {
+                    const uint64_t db = make_smem_desc(sb + k * MMA_K * 4);
+                    const uint64_t dbl = make_smem_desc(smem_u32(st) + BLO_OFF + k * MMA_K * 4);
+                    Wgmma<BN>::rs(d, hi[k], db, 1u);                 // a_hi * w_hi
+                    Wgmma<BN>::rs(d, lo[k], db, 1u);                 // a_lo * w_hi
+                    Wgmma<BN>::rs(d, hi[k], dbl, 1u);                // a_hi * w_lo
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[s]);
+            } else {
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / MMA_K; ++k)
+                    Wgmma<BN>::ss(d, make_smem_desc(sa + k * MMA_K * 4), make_smem_desc(sb + k * MMA_K * 4), 1u);
+                wgmma_commit();
+                wgmma_wait<1>();                               // the previous k-block's group has retired: release its stage
+                __syncwarp();
+                if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+                prev = s;
+            }
+        }
+        if constexpr (X3 == 0) {
+            wgmma_wait<0>();
+            __syncwarp();
+            if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+        }
+
+        // ===== epilogue: per 32-column chunk, (1) accumulators -> this warp's slab, (2) 8 lanes per row, 4 rows per
+        // instruction: scale/bias (+residual) (+ReLU) (+TF32 rounding) and whole-128-byte-line stores =====
+        const float* __restrict__ g_scale = a.scale[g]; const float* __restrict__ g_bias = a.bias[g];
+        const float* __restrict__ g_res = a.res[g]; float* __restrict__ g_out = a.out[g];
+        const int row0 = m0 + wg * 64 + wq * 16;           // first tile row of this warp
+        int opix[4], rpix[4];                              // destination / residual pixel of my 4 phase-2 rows (-1: past M)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int m = row0 + 4 * i + sub;
+            int o = -1, r = -1;
+            if (m < a.M) {
+                o = r = m;
+                if (a.store != 0 || a.res_pad) {
+                    const int hw = a.H * a.W, b = m / hw, rem = m - b * hw, h = rem / a.W, w = rem - h * a.W;
+                    const int padded = (b * (a.H + 2) + h + 1) * (a.W + 2) + w + 1;
+                    if (a.store == 2) o = padded;
+                    else if (a.store == 1) o = (b * (2 * a.H) + 2 * h) * (2 * a.W) + 2 * w;
+                    if (a.res_pad) r = padded;
+                }
+            }
+            opix[i] = o; rpix[i] = r;
+        }
+#pragma unroll
+        for (int c0 = 0; c0 < BN; c0 += 32) {
+            const int n = n0 + c0;
+            if (n >= a.N) break;                           // warp-uniform
+            stage32<BN>(slab, d, c0, lane);
+            __syncwarp();
+            if (a.store == 3) {
+                // Fused 1x1 head + sigmoid (smirk_generator.py:77-78 -> :86), N == BN == 32: lane r < 16 takes slab row r = one
+                // pixel with all 32 accumulators; per-channel constants by broadcast LDS; the activation tensor is never written.
+                const int m = row0 + lane;
+                if (lane < 16 && m < a.M) {
+                    float a0 = hpar[256], a1 = hpar[257], a2 = hpar[258], a3 = hpar[259];       // head bias
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) {
+                        const float4 x4 = slab_chunk(slab, lane, j);
+                        const float xs[4] = {x4.x, x4.y, x4.z, x4.w};
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) {
+                            const int nn = 4 * j + e;
+                            const float4 p0 = *reinterpret_cast<const float4*>(hpar + nn * 8);
+                            const float2 p1 = *reinterpret_cast<const float2*>(hpar + nn * 8 + 4);
+                            float x = fmaf(xs[e], p0.x, p0.y);
+                            if (a.relu) x = fmaxf(x, 0.f);
+                            a0 = fmaf(x, p0.z, a0); a1 = fmaf(x, p0.w, a1); a2 = fmaf(x, p1.x, a2); a3 = fmaf(x, p1.y, a3);
                         }
                     }
-                    tcgen05_commit(&empty[s]);          // frees this smem stage once the MMAs above have read it
+                    const int hw_px = a.H * a.W, b = m / hw_px, rem = m - b * hw_px;
+                    float* dst = g_out + (size_t)b * a.head_c * hw_px + rem;
+                    dst[0] = 1.f / (1.f + __expf(-a0));
+                    if (a.head_c > 1) dst[hw_px] = 1.f / (1.f + __expf(-a1));
+                    if (a.head_c > 2) dst[2 * (size_t)hw_px] = 1.f / (1.f + __expf(-a2));
+                    if (a.head_c > 3) dst[3 * (size_t)hw_px] = 1.f / (1.f + __expf(-a3));
                 }
-                tcgen05_commit(&acc_full[buf]);         // accumulator complete
-            }
-        }
-    } else {
-        // ===== epilogue: warps 2..5, TMEM lane quarter = warp % 4 =====
-        // Two phases per 32-column chunk, both private to the warp (it owns TMEM lanes / tile rows
-        // [32*quarter, +32)), so only __syncwarp separates them:
-        //   1. lane = row: tcgen05.ld 32 accumulator columns and park them in a 32 x 128-byte staging
-        //      slab in shared memory (16-byte chunks XOR-swizzled by row: conflict-free both ways);
-        //   2. 8 lanes per row, 4 rows per instruction: read the slab back transposed, apply
-        //      scale/bias (+residual) (+ReLU) (+TF32 rounding) and store — every global access of the
-        //      warp now covers whole 128-byte lines of 4 output rows instead of 16 bytes of 32 rows.
-        const int quarter = warp & 3;
-        if (X3 == 2) {
-            // ===== 3xTF32, tails in tensor memory: thread = tile row (its TMEM lane); heads rewritten in place =====
-            const int r = quarter * 32 + lane;
-            for (int kb = 0; kb < a.nkb; ++kb) {
-                const int s = kb % STAGES;
-                mbar_wait(&full[s], (uint32_t)(kb / STAGES) & 1u);
-                uint8_t* row = smem + s * STAGE_BYTES + r * 128;
-                float lo[32];
-                if (a.x3_trunc) {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const float4 v = *reinterpret_cast<const float4*>(row + ((j ^ (r & 7)) << 4));
-                        lo[4 * j] = v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u); lo[4 * j + 1] = v.y - __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
-                        lo[4 * j + 2] = v.z - __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u); lo[4 * j + 3] = v.w - __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
-                    }
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        float4* p = reinterpret_cast<float4*>(row + ((j ^ (r & 7)) << 4));       // 16-byte chunk j of the row (SWIZZLE_128B)
-                        const float4 v = *p;
-                        float4 hi;
-                        hi.x = smk::round_tf32(v.x); hi.y = smk::round_tf32(v.y); hi.z = smk::round_tf32(v.z); hi.w = smk::round_tf32(v.w);
-                        lo[4 * j] = v.x - hi.x; lo[4 * j + 1] = v.y - hi.y; lo[4 * j + 2] = v.z - hi.z; lo[4 * j + 3] = v.w - hi.w;
-                        *p = hi;
-                    }
-                }
-                tmem_st32(tmem_base + ((uint32_t)(quarter * 32) << 16) + ALO_COL + (uint32_t)(s * 32), lo);   // warp-collective, waits for completion
-                if (!a.x3_trunc) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                tcgen05_fence_before();
                 __syncwarp();
-                if (lane == 0) mbar_arrive(&split[s]);
+                continue;
             }
-            tcgen05_fence_after();
-        }
-        uint8_t* slab = slabs + quarter * 4096;
-        const int sub = lane >> 3, jj = lane & 7;              // phase-2 role: row-in-group, 16-byte chunk
-        if (a.store == 3) {                                    // head constants of channel `lane` -> this warp's slab (PERSIST layout: slabs are private)
-            float* par = reinterpret_cast<float*>(slab);
-            par[lane * 8 + 0] = __ldg(a.scale[0] + lane); par[lane * 8 + 1] = __ldg(a.bias[0] + lane);
+            const int nc = n + jj * 4;                     // my 4 columns
+            if (nc < a.N) {
+                const float4 sc = __ldg(reinterpret_cast<const float4*>(g_scale + nc));
+                const float4 bi = __ldg(reinterpret_cast<const float4*>(g_bias + nc));
+                int col = nc, pix_off = 0;
+                if (a.store == 1) {                        // ConvTranspose2d k2 s2: n = (dy*2+dx)*Cout + co
+                    const int cout = a.N >> 2, q = nc / cout;
+                    col = nc - q * cout; pix_off = (q >> 1) * (2 * a.W) + (q & 1);
+                }
 #pragma unroll
-            for (int co = 0; co < 4; ++co) par[lane * 8 + 2 + co] = co < a.head_c ? __ldg(a.head_w + (size_t)lane * a.head_c + co) : 0.f;
-            if (lane < 4) par[256 + lane] = lane < a.head_c ? __ldg(a.head_b + lane) : 0.f;
+                for (int i = 0; i < 4; ++i) {
+                    if (opix[i] < 0) continue;
+                    const float4 x = slab_chunk(slab, 4 * i + sub, jj);
+                    float4 o;
+                    o.x = fmaf(x.x, sc.x, bi.x); o.y = fmaf(x.y, sc.y, bi.y); o.z = fmaf(x.z, sc.z, bi.z); o.w = fmaf(x.w, sc.w, bi.w);
+                    if (g_res) {
+                        const float4 r4 = __ldg(reinterpret_cast<const float4*>(g_res + (size_t)rpix[i] * a.ld_res + nc));
+                        o.x += r4.x; o.y += r4.y; o.z += r4.z; o.w += r4.w;
+                    }
+                    if (a.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
+                    if (a.round_out) { o.x = smk::round_tf32(o.x); o.y = smk::round_tf32(o.y); o.z = smk::round_tf32(o.z); o.w = smk::round_tf32(o.w); }
+                    *reinterpret_cast<float4*>(g_out + (size_t)(opix[i] + pix_off) * a.ld_out + col) = o;
+                }
+            }
             __syncwarp();
         }
-        int tc = 0;
-        for (int t = blockIdx.x; t < a.n_tiles; t += gridDim.x, ++tc) {
-            const int g = t >= a.n_tiles_g ? 1 : 0, tt = t - g * a.n_tiles_g;
-            const float* __restrict__ g_scale = a.scale[g]; const float* __restrict__ g_bias = a.bias[g];
-            const float* __restrict__ g_res = a.res[g]; float* __restrict__ g_out = a.out[g];
-            const int tm = tt / a.tiles_n, tn = tt - tm * a.tiles_n;
-            const int m0 = tm * BM, n0 = tn * BN;
-            const int buf = tc & 1;
-            int opix[8], rpix[8];                              // destination / residual pixel of my 8 phase-2 rows (-1: past M)
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const int m = m0 + quarter * 32 + 4 * i + sub;
-                int o = -1, r = -1;
-                if (m < a.M) {
-                    o = r = m;
-                    if (a.store != 0 || a.res_pad) {
-                        const int hw = a.H * a.W, b = m / hw, rem = m - b * hw, h = rem / a.W, w = rem - h * a.W;
-                        const int padded = (b * (a.H + 2) + h + 1) * (a.W + 2) + w + 1;
-                        if (a.store == 2) o = padded;
-                        else if (a.store == 1) o = (b * (2 * a.H) + 2 * h) * (2 * a.W) + 2 * w;
-                        if (a.res_pad) r = padded;
-                    }
-                }
-                opix[i] = o; rpix[i] = r;
-            }
-            mbar_wait(&acc_full[buf], (uint32_t)(tc >> 1) & 1u);
-            tcgen05_fence_after();
-#pragma unroll 1
-            for (int c0 = 0; c0 < BN; c0 += 32) {
-                const int n = n0 + c0;
-                if (n >= a.N) break;                           // warp-uniform
-                float v[32];
-                tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * BN + c0), v);     // warp-collective
-                if (c0 + 32 >= BN || n + 32 >= a.N) {          // last read of this accumulator: hand it back to the MMA warp
-                    tcgen05_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&acc_empty[buf]);
-                }
-                if (a.store == 3) {
-                    // Fused 1x1 head + sigmoid (smirk_generator.py:77-78 -> :86), N == BN == 32: right after tcgen05.ld every lane holds
-                    // ALL 32 accumulators of its own pixel, so BN + ReLU + the 32 -> head_c dot products need no exchange between
-                    // lanes; per-channel constants come from this warp's slab (filled once, broadcast LDS), consecutive lanes are
-                    // consecutive pixels -> coalesced NCHW stores.  The activation tensor itself is never written.
-                    const float* par = reinterpret_cast<const float*>(slab);       // [32][8]: scale, bias, w0..w3, pad
-                    float a0 = par[256], a1 = par[257], a2 = par[258], a3 = par[259];       // head bias
-#pragma unroll
-                    for (int nn = 0; nn < 32; ++nn) {
-                        const float4 p0 = *reinterpret_cast<const float4*>(par + nn * 8);
-                        const float2 p1 = *reinterpret_cast<const float2*>(par + nn * 8 + 4);
-                        float x = fmaf(v[nn], p0.x, p0.y);
-                        if (a.relu) x = fmaxf(x, 0.f);
-                        a0 = fmaf(x, p0.z, a0); a1 = fmaf(x, p0.w, a1); a2 = fmaf(x, p1.x, a2); a3 = fmaf(x, p1.y, a3);
-                    }
-                    const int m = m0 + quarter * 32 + lane;
-                    if (m < a.M) {
-                        const int hw_px = a.H * a.W, b = m / hw_px, rem = m - b * hw_px;
-                        float* dst = g_out + (size_t)b * a.head_c * hw_px + rem;
-                        dst[0] = 1.f / (1.f + __expf(-a0));
-                        if (a.head_c > 1) dst[hw_px] = 1.f / (1.f + __expf(-a1));
-                        if (a.head_c > 2) dst[2 * (size_t)hw_px] = 1.f / (1.f + __expf(-a2));
-                        if (a.head_c > 3) dst[3 * (size_t)hw_px] = 1.f / (1.f + __expf(-a3));
-                    }
-                    continue;
-                }
-#pragma unroll
-                for (int j = 0; j < 8; ++j)
-                    *reinterpret_cast<float4*>(slab + lane * 128 + ((j ^ (lane & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                __syncwarp();
-                const int nc = n + jj * 4;                     // my 4 columns
-                if (nc < a.N) {
-                    const float4 sc = __ldg(reinterpret_cast<const float4*>(g_scale + nc));
-                    const float4 bi = __ldg(reinterpret_cast<const float4*>(g_bias + nc));
-                    int col = nc, pix_off = 0;
-                    if (a.store == 1) {                        // ConvTranspose2d k2 s2: n = (dy*2+dx)*Cout + co
-                        const int cout = a.N >> 2, q = nc / cout;
-                        col = nc - q * cout; pix_off = (q >> 1) * (2 * a.W) + (q & 1);
-                    }
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        if (opix[i] < 0) continue;
-                        const int r = 4 * i + sub;
-                        const float4 x = *reinterpret_cast<const float4*>(slab + r * 128 + ((jj ^ (r & 7)) << 4));
-                        float4 o;
-                        o.x = fmaf(x.x, sc.x, bi.x); o.y = fmaf(x.y, sc.y, bi.y); o.z = fmaf(x.z, sc.z, bi.z); o.w = fmaf(x.w, sc.w, bi.w);
-                        if (g_res) {
-                            const float4 r4 = __ldg(reinterpret_cast<const float4*>(g_res + (size_t)rpix[i] * a.ld_res + nc));
-                            o.x += r4.x; o.y += r4.y; o.z += r4.z; o.w += r4.w;
-                        }
-                        if (a.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-                        if (a.round_out) { o.x = smk::round_tf32(o.x); o.y = smk::round_tf32(o.y); o.z = smk::round_tf32(o.z); o.w = smk::round_tf32(o.w); }
-                        *reinterpret_cast<float4*>(g_out + (size_t)(opix[i] + pix_off) * a.ld_out + col) = o;
-                    }
-                }
-                __syncwarp();
-            }
-        }
-        tcgen05_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
     }
 }
 
@@ -424,9 +371,9 @@ int encode_im2col(CUtensorMap* map, const float* base, int B, int Hin, int Win, 
 template <int BN, int STAGES, int MINB, bool PERSIST, int X3 = 0>
 int launch(const TcMaps& mp, const TcArgs& a_in, cudaStream_t st, int groups) {
     constexpr size_t stage = X3 ? A_STAGE_BYTES + 2 * BN * BKB : A_STAGE_BYTES + BN * BKB;
-    constexpr size_t smem = (size_t)STAGES * stage + (PERSIST ? SLAB_BYTES : 0) + 1024 + 256;
+    constexpr size_t smem = (size_t)STAGES * stage + (PERSIST ? SLAB_BYTES : 0) + BAR_BYTES + HEAD_PAR_BYTES + 1024;
+    static_assert(PERSIST || (size_t)STAGES * stage >= SLAB_BYTES, "single-tile CTAs stage the epilogue in ring stage 0");
     static_assert(MINB * (smem + 1024) <= 228 * 1024, "shared memory budget of MINB resident CTAs");
-    static_assert(MINB * ((PERSIST ? 2 : 1) * BN + (X3 == 2 ? STAGES * 32 : 0)) <= 512, "TMEM budget of MINB resident CTAs");
     // The attribute is per device and per function; set it once per (device, instantiation).  One bit per
     // device ordinal; a benign race (two threads setting it twice) is harmless.
     static unsigned long long configured_mask = 0;
@@ -440,7 +387,7 @@ int launch(const TcMaps& mp, const TcArgs& a_in, cudaStream_t st, int groups) {
     a.tiles_n = cdiv(a.N, BN);
     a.n_tiles_g = cdiv(a.M, BM) * a.tiles_n;
     a.n_tiles = groups * a.n_tiles_g;
-    dim3 grid((unsigned)(PERSIST ? std::min(a.n_tiles, MINB * 148) : a.n_tiles));
+    dim3 grid((unsigned)(PERSIST ? std::min(a.n_tiles, MINB * num_sms()) : a.n_tiles));
     SMK_LAUNCH((gemm_tc_kernel<BN, STAGES, MINB, PERSIST, X3>), dim3(grid), dim3(NUM_THREADS), smem, st, mp, a);
     SMK_CHECK_LAUNCH();
     return 0;
@@ -463,28 +410,12 @@ int tc_conv(const TcConv& p, cudaStream_t st, const TcConv* p2) {
                         p2->res_pad == p.res_pad && p2->round_out == p.round_out && !p2->wt_lo == !p.wt_lo && !p2->res == !p.res && p.store != 3),
                 "tc_conv: paired problems must have identical shapes and epilogue options");
     int BN = p.N <= 32 ? 32 : (p.N <= 64 ? 64 : 128);
-    // Wide layers (N >= 256: the generator's 28^2 / 14^2 convolutions, 75 % of its FLOPs): a 128 x 256 tile halves the
-    // A-operand bytes the tensor core pulls from shared memory per FLOP.  TF32 operands are 4 bytes, so at BN = 128 the
-    // MMA reads (A 4 KB + B 4 KB per 64-cycle instruction) plus the TMA fill already ask for ~2x the 128 B/clk an SM's
-    // shared memory delivers; at BN = 256 the demand drops to ~1.5x.  One persistent CTA per SM, 4-stage ring (192 KB),
-    // both accumulators (2 x 256 columns) fill the SM's tensor memory.  SMK_TC_BN256=0 restores 128-wide tiles.
+    // Wide 3x3 layers (N a multiple of 256: the generator's 28^2 / 14^2 convolutions, most of its FLOPs): a 128 x 256 tile
+    // halves the A-operand bytes wgmma pulls from shared memory per FLOP (TF32 operands are 4 bytes; at BN = 128 the
+    // operand reads ask for more than an SM's shared-memory bandwidth).  One persistent CTA per SM, 4-stage ring.
+    // SMK_TC_BN256=0 keeps 128-wide tiles.
     static const int bn256 = []() { const char* e = getenv("SMK_TC_BN256"); return e ? atoi(e) : 1; }();
     if (bn256 && p.mode != 0 && p.N % 256 == 0 && !p.wt_lo) BN = 256;
-    // Few-tile, deep-K problems (the encoder's 7x7 / 14x14 projections: M = 1568..6272, K up to 960) are a serial
-    // chain of k-blocks on a handful of SMs: narrower N tiles put more CTAs to work.  An 8-stage ring with one
-    // CTA per SM (SMK_TC_DEEP_SMALL=1) makes such a kernel ~20 % faster when it runs ALONE, but its 177 KB of
-    // shared memory evict every other kernel from the SM; the pipeline runs three backbones x several batches
-    // concurrently, where the small-footprint configuration is worth +11 % end to end (profiles/r01_footprint_sweep.txt).
-    const int nkb_all = cdiv(p.K, BK);
-    bool deep_small = false;
-    if (nkb_all >= 6 && p.store != 1) {
-        // (narrowing is off by default: fewer, wider tiles re-read A less often, and in the concurrent pipeline idle SMs
-        //  are filled by other kernels anyway; SMK_TC_NARROW=148 restores the latency-oriented choice.)
-        static const int narrow_target = []() { const char* e = getenv("SMK_TC_NARROW"); return e ? atoi(e) : 0; }();
-        while (BN > 32 && (long)groups * cdiv(M, BM) * cdiv(p.N, BN) < narrow_target) BN >>= 1;
-        static const int deep_small_on = []() { const char* e = getenv("SMK_TC_DEEP_SMALL"); return e ? atoi(e) : 0; }();
-        deep_small = deep_small_on && (long)groups * cdiv(M, BM) * cdiv(p.N, BN) <= 2 * 148;
-    }
     TcMaps mp;
     TcArgs a{};
     a.M = M; a.N = p.N; a.nkb = cdiv(p.K, BK); a.mode = p.mode == 0 ? 0 : 1; a.H = p.H; a.W = p.W;
@@ -492,10 +423,6 @@ int tc_conv(const TcConv& p, cudaStream_t st, const TcConv* p2) {
     a.ld_res = p.ld_res; a.res_pad = p.res_pad; a.relu = p.relu;
     a.ld_out = p.ld_out; a.store = p.store; a.round_out = p.round_out;
     a.head_w = p.head_w; a.head_b = p.head_b; a.head_c = p.head_c;
-    {
-        static const int x3_trunc = []() { const char* e = getenv("SMK_X3_TRUNC"); return e ? atoi(e) : 1; }();
-        a.x3_trunc = x3_trunc;
-    }
     SMK_REQUIRE(p.store != 3 || (p.N == 32 && p.mode != 0 && p.head_w && p.head_b && p.head_c >= 1 && p.head_c <= 4 && !p.res && !p2),
                 "tc_conv: the fused 1x1 head needs a 3x3 conv with N == 32 (persistent kernel, one full column tile) and 1..4 head channels");
     SMK_REQUIRE(!p.wt_lo || (p.mode == 0 && p.store == 0), "tc_conv: the 3xTF32 path covers plain 1x1 convolutions / GEMMs");
@@ -523,48 +450,38 @@ int tc_conv(const TcConv& p, cudaStream_t st, const TcConv* p2) {
                 groups * 4.0 * ((double)M * cin_eff + (double)p.K * p.N + (double)M * p.N * (p.res ? 2 : 1) + 2.0 * p.N),
                 groups * 2.0 * (double)M * p.N * p.K, st);
     }
+    // MINB (third template argument) trades registers for co-resident CTAs: ptxas budgets the 288-thread block as three
+    // warpgroups, so MINB = 1 / 2 / 3 cap a thread at 168 / 96 / 72 registers.  At these budgets <256,4,1>, <128,2,2> and
+    // <64,2,3> spill (16-220 B) and the 3xTF32 <32,2,3> serialises its wgmmas; spill-free budgets (lower MINB) were measured
+    // slower end to end on H100 (fewer CTAs of the concurrent pipeline share an SM), and 128-wide tiles in place of
+    // <256,...> much slower, so the spills stay.
     if (p.wt_lo) {                                      // 3xTF32: fp32-equivalent arithmetic (encoder precision 3)
-        // deep-K layers (the 14x14 / 7x7 projections, K = 480..960): per k-block the chain TMA -> split -> MMA -> free is
-        // ~1.5 us with a 2-stage ring (measured: 47 us for K = 960); a 4-stage ring keeps three loads in flight and is
-        // faster alone, but its footprint costs the concurrent pipeline 3 % (29.8k vs 30.6k faces/s): opt-in, SMK_X3_DEEP=1
-        static const int x3_deep = []() { const char* e = getenv("SMK_X3_DEEP"); return e ? atoi(e) : 0; }();
-        if (x3_deep && a.nkb >= 8) {
-            if (BN == 32) return launch<32, 4, 2, false, 2>(mp, a, st, groups);
-            if (BN == 64) return launch<64, 4, 1, false, 2>(mp, a, st, groups);
-            return launch<128, 4, 1, false, 2>(mp, a, st, groups);
-        }
-        if (BN == 32) return launch<32, 2, 4, false, 2>(mp, a, st, groups);
-        if (BN == 64) return launch<64, 2, 3, false, 2>(mp, a, st, groups);
-        return launch<128, 2, 2, false, 2>(mp, a, st, groups);
+        if (BN == 32) return launch<32, 2, 3, false, 2>(mp, a, st, groups);
+        if (BN == 64) return launch<64, 2, 2, false, 2>(mp, a, st, groups);
+        return launch<128, 2, 1, false, 2>(mp, a, st, groups);
     }
-    if (deep_small && BN == 32) return launch<32, 8, 1, false>(mp, a, st, groups);
-    if (deep_small && BN == 64) return launch<64, 8, 1, false>(mp, a, st, groups);
     static const int persist_mode = []() { const char* e = getenv("SMK_TC_PERSIST"); return e ? atoi(e) : -1; }();   // -1 auto, 0 never, 1 always
     const long n_tiles = (long)groups * cdiv(M, BM) * cdiv(p.N, BN);
-    // 3x3 convolutions (deep K): persistent CTAs for the narrow-N layers and for the few-tile 14x14 layers;
-    // the wide-N layers are bound by the shared-memory fill rate either way and keep two single-tile CTAs per SM.
-    const bool persist = p.store == 3 || (persist_mode >= 0 ? persist_mode != 0 : (p.mode != 0 && (BN <= 64 || n_tiles <= 2 * 148)));   // (the fused head lives in the persistent layout: private slabs)
+    // 3x3 convolutions (deep K): persistent CTAs for the narrow-N layers and for the few-tile 14x14 layers; the fused head
+    // always (its constants are loaded once per CTA).  Everything else runs one tile per CTA with a 2-stage ring: a small
+    // footprint, so several CTAs of this kernel — or of the other backbones' and batches' kernels — share an SM and hide
+    // each other's prologue / epilogue.
+    const bool persist = p.store == 3 || (persist_mode >= 0 ? persist_mode != 0 : (p.mode != 0 && (BN <= 64 || n_tiles <= 2 * num_sms())));
     if (BN == 256) return launch<256, 4, 1, true>(mp, a, st, groups);
     if (persist) {
         if (BN == 32) return launch<32, 4, 2, true>(mp, a, st, groups);
         if (BN == 64) return launch<64, 3, 2, true>(mp, a, st, groups);
         return a.nkb > 8 ? launch<128, 5, 1, true>(mp, a, st, groups) : launch<128, 2, 2, true>(mp, a, st, groups);
     }
-    // One tile per CTA, 2-stage ring: 41-66 KB per CTA, so 3-5 CTAs of this kernel — or CTAs of the other
-    // backbones' and batches' kernels — share an SM and hide each other's prologue/epilogue.  Deeper rings
-    // (SMK_TC_SHALLOW_NKB=2 restores them for K > 64) win a few percent per kernel in isolation and lose
-    // 5 % end to end for the same co-residency reason as above.
-    static const int shallow_nkb = []() { const char* e = getenv("SMK_TC_SHALLOW_NKB"); return e ? atoi(e) : (1 << 30); }();
-    const bool shallow = a.nkb <= shallow_nkb;
-    if (BN == 32) return shallow ? launch<32, 2, 5, false>(mp, a, st, groups) : launch<32, 4, 2, false>(mp, a, st, groups);
-    if (BN == 64) return shallow ? launch<64, 2, 4, false>(mp, a, st, groups) : launch<64, 4, 2, false>(mp, a, st, groups);
-    return shallow ? launch<128, 2, 3, false>(mp, a, st, groups) : launch<128, 3, 2, false>(mp, a, st, groups);
+    if (BN == 32) return launch<32, 2, 3, false>(mp, a, st, groups);
+    if (BN == 64) return launch<64, 2, 3, false>(mp, a, st, groups);
+    return launch<128, 2, 2, false>(mp, a, st, groups);
 }
 
 int reflect_halo(float* buf, int B, int H, int W, int C, cudaStream_t st) {
     long total = (long)B * (2 * (W + 2) + 2 * H) * (C / 4);
     SMK_TAG("reflect_halo", 8.0 * (double)total * 4, 0.0, st);
-    SMK_LAUNCH(reflect_halo_kernel, dim3((int)std::min<long>((total + 255) / 256, 148L * 8)), dim3(256), 0, st, buf, B, H, W, C);
+    SMK_LAUNCH(reflect_halo_kernel, dim3((int)std::min<long>((total + 255) / 256, 8L * num_sms())), dim3(256), 0, st, buf, B, H, W, C);
     SMK_CHECK_LAUNCH();
     return 0;
 }

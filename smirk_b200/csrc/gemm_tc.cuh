@@ -1,4 +1,4 @@
-// TF32 tcgen05 implicit-GEMM convolution (see gemm_tc.cu).
+// TF32 wgmma implicit-GEMM convolution (see gemm_tc.cu).
 #pragma once
 #include "common.cuh"
 

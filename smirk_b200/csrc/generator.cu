@@ -8,7 +8,7 @@
 //
 // precision 0: every convolution runs on the fp32 CUDA-core implicit GEMM (nn_kernels.cu); reflection
 //              padding (:147-171) is resolved in the A-operand loader.
-// precision 1: every convolution runs on the TF32 tcgen05 implicit GEMM (gemm_tc.cu); the very first one (Cin = 6)
+// precision 1: every convolution runs on the TF32 wgmma implicit GEMM (gemm_tc.cu); the very first one (Cin = 6)
 //              reads an input whose channels are zero-padded to 32 by the layout-conversion kernel (one 128-byte
 //              SWIZZLE_128B row per pixel: the im2col TMA path as is; 2.3x faster than the fp32 CUDA-core kernel it
 //              replaces even though 26 of the 32 K-columns per tap multiply zeros).  The ResNet blocks keep their activations in
@@ -93,10 +93,10 @@ struct SmkGenerator {
 
 extern "C" int smk_generator_create(const SmkGeneratorDesc* desc, SmkGenerator** out) {
     SMK_REQUIRE(desc && out && desc->tensors, "smk_generator_create: null argument");
-    SMK_REQUIRE(desc->precision == 0 || desc->precision == 1, "smk_generator_create: precision must be 0 (fp32) or 1 (tf32 tcgen05)");
+    SMK_REQUIRE(desc->precision == 0 || desc->precision == 1, "smk_generator_create: precision must be 0 (fp32) or 1 (tf32 wgmma)");
     SMK_REQUIRE(desc->init_features % 8 == 0 && desc->out_channels <= 4 && desc->in_channels >= 1,
                 "smk_generator_create: need init_features %% 8 == 0 and out_channels <= 4");
-    SMK_REQUIRE(desc->precision == 0 || desc->init_features % 32 == 0, "smk_generator_create: the tcgen05 path needs init_features %% 32 == 0");
+    SMK_REQUIRE(desc->precision == 0 || desc->init_features % 32 == 0, "smk_generator_create: the tensor-core path needs init_features %% 32 == 0");
     if (desc->precision == 1) { if (int rc = smk::tc_init()) return rc; }
     SmkGenerator* h = new SmkGenerator();
     h->cin = desc->in_channels; h->cout = desc->out_channels;
@@ -237,7 +237,7 @@ extern "C" int smk_generator_forward(const SmkGenerator* h, const float* x, int 
         }
         bott = cur;
     } else {
-        // tcgen05 path: residual stream lives in reflection-padded buffers  xa -> (xt) -> xb
+        // tensor-core path: residual stream lives in reflection-padded buffers  xa -> (xt) -> xb
         float *xa = pad[0], *xt = pad[1], *xb = pad[2];
         if ((rc = conv3(h, h->enc[4][1], tb, cb, B, Sb, false, true, nullptr, 0, xa, cb, 2, st))) return rc;
         if ((rc = smk::reflect_halo(xa, B, Sb, Sb, cb, st))) return rc;

@@ -360,8 +360,7 @@ stem_conv_kernel(const float* __restrict__ img, int B, int H, int W, int Ho, int
 struct Stem3 { const float* w[3]; const float* scale[3]; const float* bias[3]; float* out[3]; };
 
 // CTA = one output row (b, oh): the 3 channels x 3 input rows it needs are staged in shared memory with
-// coalesced 16-byte loads (the direct version issued 27 strided 4-byte loads per thread and was
-// latency-bound at 22 % occupancy); thread = output pixel, 48 accumulators.
+// coalesced 16-byte loads (instead of 27 strided 4-byte loads per thread); thread = output pixel, 48 accumulators.
 constexpr int STEM_MAXW = 512;                     // staged row length (floats), >= W + 2
 __global__ void __launch_bounds__(128)
 stem_conv3_kernel(const float* __restrict__ img, int B, int H, int W, int Ho, int Wo, int pad, Stem3 p) {

@@ -2,7 +2,7 @@
 //
 // These are the exact-fp32 path (precision = 0): a tiled implicit-GEMM convolution with fused
 // BN / ReLU / residual / pixel-shuffle epilogues, depthwise 3x3, stem conv, 2x2 max-pool, layout
-// conversion, the final 1x1+sigmoid and the pooled linear heads.  The TF32 tcgen05 GEMM in
+// conversion, the final 1x1+sigmoid and the pooled linear heads.  The TF32 wgmma GEMM in
 // gemm_tc.cu replaces `conv_gemm` for the tensor-bound layers when precision = 1.
 #pragma once
 #include "common.cuh"

@@ -1,9 +1,8 @@
 // Peer-mapped gather buffers: the multi-GPU all-gather of the final outputs (SURVEY.md 8e; the reference itself has no
 // multi-GPU code) done with copy-engine pushes over NVLink instead of a collective kernel.
 //
-// Why not only NCCL: the compute kernels of this library are persistent (148 CTAs striding over their work items, one per
-// SM).  A collective kernel that occupies a few SMs while they run turns every concurrent persistent launch into two waves
-// (measured on 8 x B200: 0.85 end-to-end efficiency with the NCCL all-gather in the timed region, 0.99 without it).  A push
+// Why not only NCCL: the compute kernels of this library are persistent (one CTA per SM striding over their work items).
+// A collective kernel that occupies a few SMs while they run turns every concurrent persistent launch into two waves.  A push
 // from the copy engines takes no SM: each rank owns one gather buffer [world][shard], maps every peer's buffer through CUDA
 // IPC once, and after each batch copies its packed shard into slot `rank` of every peer's buffer on a communication stream.
 #include "common.cuh"
@@ -43,8 +42,7 @@ extern "C" int smk_peer_close(void* ptr) {
 }
 
 // One copy per destination, spread over the fan's own streams so that several copy engines (and NVLink ports) work at once:
-// a single stream moved 21 MB shards at ~160 GB/s, which at 8 GPUs made the pushes of one batch (8 x 21 MB) as long as the
-// batch itself.  Ordered after the work already on `stream`; `stream` continues only after every copy (device-side waits).
+// on one stream the pushes to all peers would run one after another.  Ordered after the work already on `stream`; `stream` continues only after every copy (device-side waits).
 struct SmkPeerFan {
     std::vector<cudaStream_t> streams;
     std::vector<cudaEvent_t> done;

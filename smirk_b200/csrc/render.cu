@@ -1,4 +1,4 @@
-// Mesh renderer on sm_100a: orthographic vertex stage, deterministic vertex normals, tiled
+// Mesh renderer on sm_90a: orthographic vertex stage, deterministic vertex normals, tiled
 // edge-function rasteriser with shared-memory triangle binning, barycentric attribute interpolation
 // and directional-light shading — one pass, no [B,F,3,6] attribute tensor, no atomics.
 //

@@ -130,7 +130,7 @@ int launch_warp(const uint8_t* src, int B, int Hs, int Ws, const double* M, int 
     SMK_CHECK_LAUNCH();
     const size_t n = (size_t)Hs * Ws * 3;
     SMK_TAG("warp_minmax", 0.0, 0.0, st);
-    SMK_LAUNCH(u8_minmax_kernel, dim3((unsigned)std::min<size_t>((n / 16 + 255) / 256 + 1, 296), B), dim3(256), 0, st, src, n, mm);
+    SMK_LAUNCH(u8_minmax_kernel, dim3((unsigned)std::min<size_t>((n / 16 + 255) / 256 + 1, 2 * (size_t)smk::num_sms()), B), dim3(256), 0, st, src, n, mm);
     SMK_CHECK_LAUNCH();
     SMK_TAG("warp_bilinear", (double)B * Hd * Wd * (out_f32 ? 12.0 : 3.0) + (double)B * Hd * Wd * 12.0, 30.0 * B * Hd * Wd, st);
     dim3 grid(smk::cdiv(Wd, 32), smk::cdiv(Hd, 8), B);
@@ -165,7 +165,7 @@ extern "C" int smk_f32chw_to_u8hwc(const float* in, int B, int S, uint8_t* out, 
     SMK_REQUIRE(in && out && B > 0 && S > 0, "smk_f32chw_to_u8hwc: bad argument");
     cudaStream_t st = (cudaStream_t)stream;
     SMK_TAG("f32chw_to_u8hwc", 15.0 * B * S * S, 0.0, st);
-    SMK_LAUNCH(f32chw_to_u8hwc_kernel, dim3((unsigned)std::min<size_t>(((size_t)B * S * S + 255) / 256, 148 * 8)), dim3(256), 0, st, in, B, S, out);
+    SMK_LAUNCH(f32chw_to_u8hwc_kernel, dim3((unsigned)std::min<size_t>(((size_t)B * S * S + 255) / 256, 8 * (size_t)smk::num_sms())), dim3(256), 0, st, in, B, S, out);
     SMK_CHECK_LAUNCH();
     return 0;
 }

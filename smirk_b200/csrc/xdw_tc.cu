@@ -3,19 +3,19 @@
 //
 // The expanded tensor e = ReLU(BN(conv_pw(x))) is the largest activation of every block (4-6x the block's
 // input) and in the unfused path is written to HBM by the 1x1 GEMM and read back by the depthwise kernel.
-// Here it only ever exists in TMEM and shared memory:
+// Here it only ever exists in registers and shared memory:
 //
 //   CTA = one 16x16-pixel window of e for one image (a 14x14 tile of outputs + halo for stride 1, a 7x7
 //         tile for stride 2) x one group of 32-channel chunks of the expanded tensor (the depthwise conv
-//         makes channel chunks independent, so low-resolution layers still fill the GPU).  The kernel fits 2
-//         CTAs per SM; the launcher aims for one per SM (148 persistent CTAs), which leaves half of every SM to
-//         the other kernels of the concurrent pipeline (measured +4 % end to end, see xdw_conv below).
-//   warp 0      TMA producer: two 16x8-pixel boxes of x (4-D tiled tensor map over NHWC, halo pixels
+//         makes channel chunks independent, so low-resolution layers still fill the GPU).  Persistent CTAs,
+//         two per SM fit; the launcher aims for one per SM, which leaves room on every SM for the other kernels
+//         of the concurrent pipeline.
+//   warp 8      TMA producer: two 16x8-pixel boxes of x (4-D tiled tensor map over NHWC, halo pixels
 //               outside the image zero-filled by the hardware) + a 32-row box of the 1x1 weights per k-block.
-//   warp 1      tcgen05.mma kind::tf32, M = 2 x 128 window pixels, N = 32 channels, accumulators
-//               double-buffered in TMEM (4 x 32 columns) so chunk c+1 is multiplied while chunk c drains.
-//   warps 2-9   (a) TMEM -> BN1 + ReLU (+ zero outside the image, which is what the depthwise conv's zero
-//               padding of e means) -> shared-memory window E[256][32];
+//   warps 0-7   two warpgroups; warpgroup h multiplies window half h (128 pixels x 32 channels) with
+//               wgmma.m64n32k8 TF32 (two per k-step), then
+//               (a) accumulator registers -> BN1 + ReLU (+ zero outside the image, which is what the depthwise
+//               conv's zero padding of e means) -> shared-memory window E[256][32];
 //               (b) depthwise 3x3 over E on the CUDA cores (float4 over channels), BN2 + ReLU, optional
 //               TF32 rounding, coalesced 256-byte stores of d.
 //
@@ -28,28 +28,22 @@
 namespace smk {
 namespace {
 
-constexpr int BKB = 128, BK = 32, UMMA_K = 8;
+constexpr int BKB = 128, BK = 32, MMA_K = 8;
 constexpr int WIN = 16;                         // window edge (pixels of e)
 constexpr int HALF_BYTES = 128 * BKB;           // one 16x8-pixel box, 32 channels: 16 KiB
 constexpr int NC = 32;                          // expanded channels per chunk
 constexpr int B_BYTES = NC * BKB;               // 4 KiB
-constexpr int STAGE_BYTES = 2 * HALF_BYTES + B_BYTES;   // 36 KiB (x2 in the 3xTF32 variant: heads + tails)
-#ifndef SMK_XDW_STAGES
-#define SMK_XDW_STAGES 2
-#endif
-constexpr int STAGES = SMK_XDW_STAGES;
+constexpr int STAGE_BYTES = 2 * HALF_BYTES + B_BYTES;   // 36 KiB (+ the weight tails in the 3xTF32 variant)
+constexpr int STAGES = 2;
 constexpr int E_PITCH = NC + 4;                 // floats; 144-byte rows (odd multiple of 16 B): conflict-free 16-byte column writes
 constexpr int E_BYTES = 256 * E_PITCH * 4;      // 36 864 B
 constexpr int PAR_ROWS = 13;                     // scale1, bias1, 9 depthwise taps, scale2, bias2
 constexpr int PAR_BYTES = 2 * PAR_ROWS * NC * 4;  // double-buffered: 3328 B
 constexpr int NUM_WORKERS = 256;
-constexpr int NUM_THREADS = 64 + NUM_WORKERS;
-constexpr int NUM_SPLITTERS = 128;              // 3xTF32 variant: four more warps split the landed x window into TF32 heads / tails
-constexpr uint32_t TMEM_COLS = 128;             // (2 buffers) x (2 halves) x 32 columns; the 3xTF32 variant adds STAGES x 2 x 32 for the x tails
+constexpr int NUM_THREADS = NUM_WORKERS + 32;
 
-using namespace ptx;                            // PTX wrappers shared by the tcgen05 kernels (tc_ptx.cuh)
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) { return make_idesc_tf32(M, N); }
-__device__ __forceinline__ void worker_barrier() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+using namespace ptx;                            // PTX wrappers shared by the tensor-core kernels (tc_ptx.cuh)
+__device__ __forceinline__ void worker_barrier() { named_barrier(1, NUM_WORKERS); }
 
 struct XdwMaps { CUtensorMap x[2], w[2], wlo[2]; };      // per problem: activations, 1x1 weights (TF32 heads), weight tails
 
@@ -67,26 +61,17 @@ struct XdwArgs {
     const float* scale2[2]; const float* bias2[2];  // folded BN of the depthwise conv   [mid]
     float* out[2];                                  // d: [B, Ho, Wo, mid]
     int round_out;
-    int x3_trunc;                  // see gemm_tc.cu: 1 = the tensor core's own truncation of fp32 words is the head
 };
 
-// X3 != 0: error-compensated 3xTF32 expand GEMM (fp32-equivalent e): x = x_hi + x_lo, w1 = w_hi + w_lo (split on the host, tmWlo),
-// e = x_hi*w_hi + x_lo*w_hi + x_hi*w_lo accumulated in the same TMEM columns.  The tails of x live in TENSOR MEMORY (64 columns
-// per ring stage next to the accumulators) and are multiplied with the A-from-TMEM form of tcgen05.mma, so shared memory stays
-// at the plain kernel's 113 KB + the weight tails.  Four dedicated splitter warps (448 threads) split each landed x window;
-// letting the eight worker warps do it instead (320 threads, tried for Cin <= 64) measured 2 % slower end to end and 6-8 % slower
-// per layer (profiles/r02_xdw_worker_split_ab.txt), so that variant is gone.
+// X3 != 0: error-compensated 3xTF32 expand GEMM (fp32-equivalent e): x = x_hi + x_lo, w1 = w_hi + w_lo (split on the host, wlo),
+// e = x_hi*w_hi + x_lo*w_hi + x_hi*w_lo accumulated in the same registers.  The workers split their own A fragments of x in
+// registers and use the register-A form of wgmma, so shared memory only grows by the weight tails.
 template <int STRIDE, int X3>
-__global__ void __launch_bounds__(NUM_THREADS + (X3 ? NUM_SPLITTERS : 0), X3 ? 1 : 2) __maxnreg__(X3 ? 96 : 102)
+__global__ void __launch_bounds__(NUM_THREADS, X3 ? 1 : 2)
 xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
     constexpr int TO = STRIDE == 1 ? 14 : 7;                    // output tile edge
     constexpr int STAGE_BYTES = X3 ? smk::STAGE_BYTES + B_BYTES : smk::STAGE_BYTES;      // [x half 0][x half 1][w] (+ [w tails])
     constexpr int WLO = smk::STAGE_BYTES;                       // offset of the weight tails within a stage
-    constexpr uint32_t XLO_COL = smk::TMEM_COLS;                // first TMEM column of the x tails (stage s, half h -> + (2 s + h) * 32)
-    constexpr uint32_t TMEM_COLS = X3 ? 256u : smk::TMEM_COLS;
-    constexpr int SPLIT_ARRIVALS = NUM_SPLITTERS / 32;
-    static_assert(!X3 || 128 + STAGES * 64 <= 256, "TMEM columns");
-    constexpr uint32_t IDESC = make_idesc(128, NC);
     extern __shared__ uint8_t smem_raw[];
     // 1024-byte alignment for SWIZZLE_128B; offset arithmetic (not an integer round-trip of the pointer) keeps
     // the shared address space visible to the compiler, so E is accessed with LDS/STS instead of generic LD/ST.
@@ -95,19 +80,13 @@ xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
     float* PAR = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES + E_BYTES);        // [2][PAR_ROWS][NC]
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + E_BYTES + PAR_BYTES);
     uint64_t* empty = full + STAGES;
-    uint64_t* acc_full = empty + STAGES;
-    uint64_t* acc_empty = acc_full + 2;
-    uint64_t* split = acc_empty + 2;                            // X3: stage s has been split (one arrival per splitting warp)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(split + STAGES);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // Persistent CTA: work item = (image, output tile, channel-chunk group), items strided over the grid.
-    // All three roles walk the same item sequence; the smem ring and the TMEM double buffer run across
-    // item boundaries, so the x window / weights of item i+1 are in flight (and multiplied) while the
-    // workers are still busy with item i.
+    // Both roles walk the same item sequence; the smem ring runs across item boundaries, so the x window / weights
+    // of item i+1 are in flight while the workers are still busy with item i.
     // The item sequence of a CTA advances by gridDim.x; the (group, tile x, tile y, image) digits of the item index are
-    // carried along incrementally — one runtime decomposition per thread at kernel start instead of four integer divisions per
-    // item (which cost the workers ~16 % of their time on the two-chunk 112^2 block, profiles/r02_ncu_full_xdw3x_*.txt).
+    // carried along incrementally — one runtime decomposition per thread at kernel start instead of four integer divisions per item.
     struct Item { int prob, img, oh0, ow0, c_begin, c_end; };
     struct ItemIter { int item, grp, tx, ty, img2; };          // img2: image index over both problems
     auto iter_begin = [&]() {
@@ -131,53 +110,17 @@ xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
         return w;
     };
 
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&mp.x[0]) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&mp.w[0]) : "memory");
-        if (X3) asm volatile("prefetch.tensormap [%0];" ::"l"(&mp.wlo[0]) : "memory");
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); mbar_init(&split[s], SPLIT_ARRIVALS); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], NUM_WORKERS / 32); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    if (warp == NUM_WORKERS / 32 && lane == 0) {
+        prefetch_tensormap(&mp.x[0]);
+        prefetch_tensormap(&mp.w[0]);
+        if (X3) prefetch_tensormap(&mp.wlo[0]);
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], NUM_WORKERS / 32); }
+        fence_barrier_init();
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     pdl_sync();
 
-    // 3xTF32: split 32 rows x 32 channels of one half of the x window in stage s — thread = window row r of its warp's TMEM lane
-    // quarter (a warp may only touch lanes [32 * (warp % 4), +32)).  Tails -> tensor memory; heads either implicit (the tensor core
-    // truncates fp32 words to TF32: x3_trunc) or rewritten in place (round to nearest).
-    auto split_rows = [&](int s, int half) {
-        const int r = (warp & 3) * 32 + lane;
-        uint8_t* row = smem + s * STAGE_BYTES + half * HALF_BYTES + r * 128;
-        float lo[32];
-        if (a.x3_trunc) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const float4 v = *reinterpret_cast<const float4*>(row + ((j ^ (r & 7)) << 4));
-                lo[4 * j] = v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u); lo[4 * j + 1] = v.y - __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
-                lo[4 * j + 2] = v.z - __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u); lo[4 * j + 3] = v.w - __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
-            }
-        } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                float4* p = reinterpret_cast<float4*>(row + ((j ^ (r & 7)) << 4));
-                const float4 v = *p;
-                float4 hi;
-                hi.x = round_tf32(v.x); hi.y = round_tf32(v.y); hi.z = round_tf32(v.z); hi.w = round_tf32(v.w);
-                lo[4 * j] = v.x - hi.x; lo[4 * j + 1] = v.y - hi.y; lo[4 * j + 2] = v.z - hi.z; lo[4 * j + 3] = v.w - hi.w;
-                *p = hi;
-            }
-        }
-        tmem_st32(tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + XLO_COL + (uint32_t)((s * 2 + half) * 32), lo);
-    };
-
-    if (warp == 0) {
+    if (warp == NUM_WORKERS / 32) {
         if (lane == 0) {
             // ===== TMA producer: (x window, W1 chunk) per k-block, for every channel chunk =====
             int it = 0;
@@ -197,218 +140,199 @@ xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
                     }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ===== MMA issuer =====
-            int it = 0, cc = 0;                             // ring iteration / accumulator-buffer use counters
-            for (ItemIter ii = iter_begin(); ii.item < a.n_items; iter_next(ii)) {
-              const Item w = decode(ii);
-              for (int c = w.c_begin; c < w.c_end; ++c, ++cc) {
-                const int buf = cc & 1;
-                mbar_wait(&acc_empty[buf], ((uint32_t)(cc >> 1) & 1u) ^ 1u);
-                tcgen05_fence_after();
-                for (int kb = 0; kb < a.nkb; ++kb, ++it) {
-                    const int s = it % STAGES;
-                    mbar_wait(X3 ? &split[s] : &full[s], (uint32_t)(it / STAGES) & 1u);
-                    tcgen05_fence_after();
-                    const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
-                    const uint32_t sb = sa + 2 * HALF_BYTES;
+        return;
+    }
+
+    // ===== workers: 8 warps =====
+    const int half = warp >> 2, wq = warp & 3;         // warpgroup = window half (rows 128 half ..), warp within it
+    const int t = threadIdx.x;                         // 0..255
+    const int cq = t & 7, slot = t >> 3;               // depthwise role: channel quad within the chunk, output slot (0..31)
+    // Per-chunk parameters (BN1 scale/bias, nine depthwise taps, BN2 scale/bias: 13 rows of 32 channels) are
+    // staged through a double-buffered shared-memory block: thread t < 208 owns one float2 of the block, loads
+    // it for chunk i+1 before it starts its MMAs for chunk i and parks it after phase (a) —
+    // the global-load latency is off the critical path and phases (a)/(b) read parameters with LDS.
+    const int prow = t >> 4, pcol = (t & 15) * 2;
+    const bool par_owner = t < PAR_ROWS * 16;
+    const float* psrc[2] = {nullptr, nullptr};
+    if (par_owner) {
 #pragma unroll
-                    for (int half = 0; half < 2; ++half)
+        for (int q = 0; q < 2; ++q)
+            psrc[q] = (prow == 0 ? a.scale1[q] : prow == 1 ? a.bias1[q] : prow == 11 ? a.scale2[q] : prow == 12 ? a.bias2[q]
+                                                                                   : a.wdw[q] + (size_t)(prow - 2) * a.mid) + pcol;
+    }
+    auto load_par = [&](int prob, int c) {
+        float2 v = make_float2(0.f, 0.f);
+        if (par_owner && c * NC + pcol < a.mid) v = __ldg(reinterpret_cast<const float2*>(psrc[prob] + c * NC));
+        return v;
+    };
+    auto park_par = [&](int slot_idx, const float2& v) {
+        if (par_owner) *reinterpret_cast<float2*>(PAR + slot_idx * (PAR_ROWS * NC) + prow * NC + pcol) = v;
+    };
+    ItemIter ii = iter_begin();
+    if (ii.item < a.n_items) { const Item w0 = decode(ii); park_par(0, load_par(w0.prob, w0.c_begin)); }
+    worker_barrier();
+    // Depthwise role of this thread: output column dw_ox and row group dw_rg of the tile's valid columns x as many row groups
+    // as fit in the 32 slots.  A tile has TO columns / rows except in the last tile column / row: the thread's role for both
+    // column counts is worked out once here (bytes of `role`: ox full, rg full, ox edge, rg edge), the row grouping of the four
+    // tile kinds comes from the host (a.geom); the item loop only selects.
+    const int ncols_e = a.Wo - (a.tiles_x - 1) * TO, nrows_e = a.Ho - (a.tiles_y - 1) * TO;
+    const unsigned role = (unsigned)(slot % TO) | (unsigned)(slot / TO) << 8 | (unsigned)(slot % ncols_e) << 16 | (unsigned)(slot / ncols_e) << 24;
+    int cc = 0, it = 0;
+    for (; ii.item < a.n_items;) {
+      const Item w = decode(ii);
+      const int img = w.img, oh0 = w.oh0, ow0 = w.ow0;
+      const int ey0 = oh0 * STRIDE - a.pad, ex0 = ow0 * STRIDE - a.pad;
+      // this thread's output column dw_ox and output rows [dw_oy0, dw_oy1) of the tile
+      const bool col_e = ii.tx == a.tiles_x - 1, row_e = ii.ty == a.tiles_y - 1;
+      const int nrows = row_e ? nrows_e : TO;
+      const unsigned g8 = a.geom >> ((col_e ? 16 : 0) + (row_e ? 8 : 0));
+      const int rpt = (int)(g8 & 15u), n_rg = (int)((g8 >> 4) & 15u);
+      const unsigned r16 = role >> (col_e ? 16 : 0);
+      const int dw_ox = (int)(r16 & 255u), dw_rg = (int)((r16 >> 8) & 255u);
+      const int dw_oy0 = dw_rg * rpt, dw_oy1 = dw_rg < n_rg ? min(nrows, dw_oy0 + rpt) : 0;
+      int next_first = -1, next_prob = 0;              // first chunk (and problem) of this CTA's next item (-1: none)
+      iter_next(ii);
+      if (ii.item < a.n_items) { const Item wn = decode(ii); next_first = wn.c_begin; next_prob = wn.prob; }
+      for (int c = w.c_begin; c < w.c_end; ++c, ++cc) {
+        const int buf = cc & 1;
+        const int ch0 = c * NC;
+        const float* par = PAR + buf * (PAR_ROWS * NC);
+        const int c_next = c + 1 < w.c_end ? c + 1 : next_first;
+        float2 pf = make_float2(0.f, 0.f);
+        if (c_next >= 0) pf = load_par(c + 1 < w.c_end ? w.prob : next_prob, c_next);
+        // expand GEMM of this chunk: rows [64 mb, 64 mb + 64) of window half `half`, 32 channels
+        float acc[2][NC / 2];
 #pragma unroll
-                        for (int k = 0; k < BK / UMMA_K; ++k) {
-                            const uint32_t d = tmem_base + (uint32_t)((buf * 2 + half) * NC);
-                            const uint64_t da = make_smem_desc(sa + half * HALF_BYTES + k * UMMA_K * 4);
-                            const uint64_t db = make_smem_desc(sb + k * UMMA_K * 4);
-                            umma_tf32(d, da, db, IDESC, (kb | k) != 0 ? 1u : 0u);
-                            if (X3) {
-                                umma_tf32_ts(d, tmem_base + XLO_COL + (uint32_t)((s * 2 + half) * 32 + k * UMMA_K), db, IDESC, 1u);   // x_lo * w_hi
-                                umma_tf32(d, da, make_smem_desc(sa + WLO + k * UMMA_K * 4), IDESC, 1u);                               // x_hi * w_lo
-                            }
-                        }
-                    tcgen05_commit(&empty[s]);
+        for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+            for (int i = 0; i < NC / 2; ++i) acc[mb][i] = 0.f;
+        for (int kb = 0; kb < a.nkb; ++kb, ++it) {
+            const int s = it % STAGES;
+            mbar_wait(&full[s], (uint32_t)(it / STAGES) & 1u);
+            const uint8_t* st = smem + s * STAGE_BYTES;
+            const uint32_t sa = smem_u32(st) + (uint32_t)(half * HALF_BYTES);
+            const uint32_t sb = smem_u32(st) + 2 * HALF_BYTES;
+            if constexpr (X3 != 0) {
+                uint32_t hi[2][BK / MMA_K][4], lo[2][BK / MMA_K][4];
+#pragma unroll
+                for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+                    for (int k = 0; k < BK / MMA_K; ++k) {
+                        float v[4];
+                        load_a_frag(st + half * HALF_BYTES, mb * 64, k * MMA_K, wq, lane, v);
+                        split_frag(v, hi[mb][k], lo[mb][k]);
+                    }
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / MMA_K; ++k) {
+                    const uint64_t db = make_smem_desc(sb + k * MMA_K * 4);
+                    const uint64_t dbl = make_smem_desc(smem_u32(st) + WLO + k * MMA_K * 4);
+#pragma unroll
+                    for (int mb = 0; mb < 2; ++mb) {
+                        Wgmma<NC>::rs(acc[mb], hi[mb][k], db, 1u);       // x_hi * w_hi
+                        Wgmma<NC>::rs(acc[mb], lo[mb][k], db, 1u);       // x_lo * w_hi
+                        Wgmma<NC>::rs(acc[mb], hi[mb][k], dbl, 1u);      // x_hi * w_lo
+                    }
                 }
-                tcgen05_commit(&acc_full[buf]);
-              }
+            } else {
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / MMA_K; ++k) {
+                    const uint64_t db = make_smem_desc(sb + k * MMA_K * 4);
+#pragma unroll
+                    for (int mb = 0; mb < 2; ++mb)
+                        Wgmma<NC>::ss(acc[mb], make_smem_desc(sa + mb * 64 * BKB + k * MMA_K * 4), db, 1u);
+                }
             }
+            wgmma_commit();
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[s]);
         }
-    } else if (X3 && warp >= 2 + NUM_WORKERS / 32) {
-        // ===== dedicated splitters: both halves of every landed x window, one ring stage at a time =====
-        int it = 0;
-        for (ItemIter ii = iter_begin(); ii.item < a.n_items; iter_next(ii)) {
-            const Item w = decode(ii);
-            for (int c = w.c_begin; c < w.c_end; ++c)
-                for (int kb = 0; kb < a.nkb; ++kb, ++it) {
-                    const int s = it % STAGES;
-                    mbar_wait(&full[s], (uint32_t)(it / STAGES) & 1u);
-                    split_rows(s, 0); split_rows(s, 1);
-                    if (!a.x3_trunc) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    tcgen05_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&split[s]);
-                }
-        }
-    } else {
-        // ===== workers: 8 warps =====
-        const int wid = warp - 2;                          // 0..7
-        const int quarter = warp & 3;                      // TMEM lane quarter this warp may read
-        const int half = wid >> 2;                         // warps {2..5} drain the upper 16x8 pixels, {6..9} the lower
-        const int t = threadIdx.x - 64;                    // 0..255
-        const int cq = t & 7, slot = t >> 3;               // depthwise role: channel quad within the chunk, output slot (0..31)
-        // Per-chunk parameters (BN1 scale/bias, nine depthwise taps, BN2 scale/bias: 13 rows of 32 channels) are
-        // staged through a double-buffered shared-memory block: thread t < 208 owns one float2 of the block, loads
-        // it for chunk i+1 before it starts waiting for the accumulator of chunk i and parks it after phase (a) —
-        // the global-load latency is off the critical path and phases (a)/(b) read parameters with LDS.
-        const int prow = t >> 4, pcol = (t & 15) * 2;
-        const bool par_owner = t < PAR_ROWS * 16;
-        const float* psrc[2] = {nullptr, nullptr};
-        if (par_owner) {
+        // (a) accumulators -> BN1 + ReLU -> E.  Channels past `mid` have zero scale and bias in the parameter block, pixels
+        // outside the image are zeroed: that is the zero padding of e the depthwise conv expects.
 #pragma unroll
-            for (int q = 0; q < 2; ++q)
-                psrc[q] = (prow == 0 ? a.scale1[q] : prow == 1 ? a.bias1[q] : prow == 11 ? a.scale2[q] : prow == 12 ? a.bias2[q]
-                                                                                       : a.wdw[q] + (size_t)(prow - 2) * a.mid) + pcol;
-        }
-        auto load_par = [&](int prob, int c) {
-            float2 v = make_float2(0.f, 0.f);
-            if (par_owner && c * NC + pcol < a.mid) v = __ldg(reinterpret_cast<const float2*>(psrc[prob] + c * NC));
-            return v;
-        };
-        auto park_par = [&](int slot_idx, const float2& v) {
-            if (par_owner) *reinterpret_cast<float2*>(PAR + slot_idx * (PAR_ROWS * NC) + prow * NC + pcol) = v;
-        };
-        ItemIter ii = iter_begin();
-        if (ii.item < a.n_items) { const Item w0 = decode(ii); park_par(0, load_par(w0.prob, w0.c_begin)); }
-        worker_barrier();
-        // Depthwise role of this thread: output column dw_ox and row group dw_rg of the tile's valid columns x as many row groups
-        // as fit in the 32 slots.  A tile has TO columns / rows except in the last tile column / row: the thread's role for both
-        // column counts is worked out once here (bytes of `role`: ox full, rg full, ox edge, rg edge), the row grouping of the four
-        // tile kinds comes from the host (a.geom); the item loop only selects.
-        const int ncols_e = a.Wo - (a.tiles_x - 1) * TO, nrows_e = a.Ho - (a.tiles_y - 1) * TO;
-        const unsigned role = (unsigned)(slot % TO) | (unsigned)(slot / TO) << 8 | (unsigned)(slot % ncols_e) << 16 | (unsigned)(slot / ncols_e) << 24;
-        int cc = 0;
-        for (; ii.item < a.n_items;) {
-          const Item w = decode(ii);
-          const int img = w.img, oh0 = w.oh0, ow0 = w.ow0;
-          const int ey0 = oh0 * STRIDE - a.pad, ex0 = ow0 * STRIDE - a.pad;
-          // this thread's output column dw_ox and output rows [dw_oy0, dw_oy1) of the tile
-          const bool col_e = ii.tx == a.tiles_x - 1, row_e = ii.ty == a.tiles_y - 1;
-          const int nrows = row_e ? nrows_e : TO;
-          const unsigned g8 = a.geom >> ((col_e ? 16 : 0) + (row_e ? 8 : 0));
-          const int rpt = (int)(g8 & 15u), n_rg = (int)((g8 >> 4) & 15u);
-          const unsigned r16 = role >> (col_e ? 16 : 0);
-          const int dw_ox = (int)(r16 & 255u), dw_rg = (int)((r16 >> 8) & 255u);
-          const int dw_oy0 = dw_rg * rpt, dw_oy1 = dw_rg < n_rg ? min(nrows, dw_oy0 + rpt) : 0;
-          int next_first = -1, next_prob = 0;              // first chunk (and problem) of this CTA's next item (-1: none)
-          iter_next(ii);
-          if (ii.item < a.n_items) { const Item wn = decode(ii); next_first = wn.c_begin; next_prob = wn.prob; }
-          for (int c = w.c_begin; c < w.c_end; ++c, ++cc) {
-            const int buf = cc & 1;
-            const int ch0 = c * NC;
-            const float* par = PAR + buf * (PAR_ROWS * NC);
-            const int c_next = c + 1 < w.c_end ? c + 1 : next_first;
-            float2 pf = make_float2(0.f, 0.f);
-            if (c_next >= 0) pf = load_par(c + 1 < w.c_end ? w.prob : next_prob, c_next);
-            mbar_wait(&acc_full[buf], (uint32_t)(cc >> 1) & 1u);
-            tcgen05_fence_after();
-            // (a) TMEM -> BN1 + ReLU -> E   (rows = window pixels, lane = pixel).  Channels past `mid` have zero
-            // scale and bias in the parameter block, pixels outside the image are zeroed: that is the zero
-            // padding of e the depthwise conv expects.
-            {
-                float4 v[8];
-                tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)((buf * 2 + half) * NC), reinterpret_cast<float*>(v));
-                const int r = quarter * 32 + lane;                       // row within the half: r = hh*16 + ww
+        for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+                const int r = mb * 64 + wq * 16 + (lane >> 2) + 8 * hr;      // row within the half: r = hh*16 + ww
                 const int ey = ey0 + half * 8 + (r >> 4), ex = ex0 + (r & 15);
                 const bool inside = ey >= 0 && ey < a.H && ex >= 0 && ex < a.W;
                 float* erow = E + (size_t)(half * 128 + r) * E_PITCH;
-                const int nquads = (min(NC, a.mid - ch0) + 3) >> 2;      // channel quads of this chunk that exist (phase (b) reads no others)
-                if (inside) {
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        if (j >= nquads) break;
-                        const float4 sc = *reinterpret_cast<const float4*>(par + 4 * j);
-                        const float4 bi = *reinterpret_cast<const float4*>(par + NC + 4 * j);
-                        float4 o = fma4(v[j], sc, bi);
-                        o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
-                        *reinterpret_cast<float4*>(erow + 4 * j) = o;
+                for (int j = 0; j < NC / 8; ++j) {
+                    const int ch = 8 * j + 2 * (lane & 3);
+                    float2 o = make_float2(0.f, 0.f);
+                    if (inside) {
+                        const float2 sc = *reinterpret_cast<const float2*>(par + ch);
+                        const float2 bi = *reinterpret_cast<const float2*>(par + NC + ch);
+                        o.x = fmaxf(fmaf(acc[mb][4 * j + 2 * hr], sc.x, bi.x), 0.f);
+                        o.y = fmaxf(fmaf(acc[mb][4 * j + 2 * hr + 1], sc.y, bi.y), 0.f);
                     }
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        if (j >= nquads) break;
-                        *reinterpret_cast<float4*>(erow + 4 * j) = make_float4(0.f, 0.f, 0.f, 0.f);
-                    }
+                    *reinterpret_cast<float2*>(erow + ch) = o;
                 }
             }
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[buf]);   // this warp has drained its part of the accumulator
-            if (c_next >= 0) park_par(buf ^ 1, pf);        // slot buf^1 was last read in the previous chunk's phase (b)
-            worker_barrier();
-            // (b) depthwise 3x3 over E.  One thread owns one output column of one channel quad and walks down
-            // its rows, so every E row it reads is shared by the (up to three) output rows it feeds: 3 LDS.128
-            // per input row instead of 9 per output.  Tap order per output stays (ky, kx) ascending -> same
-            // rounding as the unfused path.
-            if (cq * 4 < a.mid - ch0 && dw_oy0 < dw_oy1) {
-                const int ch = ch0 + cq * 4;
-                float4 k[9];
+        if (c_next >= 0) park_par(buf ^ 1, pf);        // slot buf^1 was last read in the previous chunk's phase (b)
+        worker_barrier();
+        // (b) depthwise 3x3 over E.  One thread owns one output column of one channel quad and walks down
+        // its rows, so every E row it reads is shared by the (up to three) output rows it feeds: 3 LDS.128
+        // per input row instead of 9 per output.  Tap order per output stays (ky, kx) ascending -> same
+        // rounding as the unfused path.
+        if (cq * 4 < a.mid - ch0 && dw_oy0 < dw_oy1) {
+            const int ch = ch0 + cq * 4;
+            float4 k[9];
 #pragma unroll
-                for (int q = 0; q < 9; ++q) k[q] = *reinterpret_cast<const float4*>(par + (2 + q) * NC + cq * 4);
-                const float4 s2 = *reinterpret_cast<const float4*>(par + 11 * NC + cq * 4);
-                const float4 b2 = *reinterpret_cast<const float4*>(par + 12 * NC + cq * 4);
-                float* orow = a.out[w.prob] + (((size_t)img * a.Ho + oh0 + dw_oy0) * a.Wo + ow0 + dw_ox) * a.mid + ch;
-                const size_t orow_stride = (size_t)a.Wo * a.mid;
-                auto emit = [&](const float4& acc) {
-                    float4 o = fma4(acc, s2, b2);
-                    o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
-                    if (a.round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
-                    *reinterpret_cast<float4*>(orow) = o;
-                    orow += orow_stride;
-                };
-                const float* e = E + (size_t)((dw_oy0 * STRIDE) * WIN + dw_ox * STRIDE) * E_PITCH + cq * 4;
-                const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (STRIDE == 1) {
-                    float4 acc0 = zero, acc1 = zero, acc2 = zero;          // outputs r-2 (gets ky=2), r-1 (ky=1), r (ky=0)
-                    const int n_in = dw_oy1 - dw_oy0 + 2;
+            for (int q = 0; q < 9; ++q) k[q] = *reinterpret_cast<const float4*>(par + (2 + q) * NC + cq * 4);
+            const float4 s2 = *reinterpret_cast<const float4*>(par + 11 * NC + cq * 4);
+            const float4 b2 = *reinterpret_cast<const float4*>(par + 12 * NC + cq * 4);
+            float* orow = a.out[w.prob] + (((size_t)img * a.Ho + oh0 + dw_oy0) * a.Wo + ow0 + dw_ox) * a.mid + ch;
+            const size_t orow_stride = (size_t)a.Wo * a.mid;
+            auto emit = [&](const float4& acc4) {
+                float4 o = fma4(acc4, s2, b2);
+                o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
+                if (a.round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
+                *reinterpret_cast<float4*>(orow) = o;
+                orow += orow_stride;
+            };
+            const float* e = E + (size_t)((dw_oy0 * STRIDE) * WIN + dw_ox * STRIDE) * E_PITCH + cq * 4;
+            const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (STRIDE == 1) {
+                float4 acc0 = zero, acc1 = zero, acc2 = zero;          // outputs r-2 (gets ky=2), r-1 (ky=1), r (ky=0)
+                const int n_in = dw_oy1 - dw_oy0 + 2;
 #pragma unroll 3
-                    for (int r = 0; r < n_in; ++r, e += WIN * E_PITCH) {
-                        const float4 x0 = *reinterpret_cast<const float4*>(e);
-                        const float4 x1 = *reinterpret_cast<const float4*>(e + E_PITCH);
-                        const float4 x2 = *reinterpret_cast<const float4*>(e + 2 * E_PITCH);
-                        fma4_acc(acc0, x0, k[6]); fma4_acc(acc0, x1, k[7]); fma4_acc(acc0, x2, k[8]);
-                        fma4_acc(acc1, x0, k[3]); fma4_acc(acc1, x1, k[4]); fma4_acc(acc1, x2, k[5]);
-                        fma4_acc(acc2, x0, k[0]); fma4_acc(acc2, x1, k[1]); fma4_acc(acc2, x2, k[2]);
-                        if (r >= 2) emit(acc0);
-                        acc0 = acc1; acc1 = acc2; acc2 = zero;
-                    }
-                } else {
-                    float4 p0 = *reinterpret_cast<const float4*>(e);
-                    float4 p1 = *reinterpret_cast<const float4*>(e + E_PITCH);
-                    float4 p2 = *reinterpret_cast<const float4*>(e + 2 * E_PITCH);
-                    for (int oy = dw_oy0; oy < dw_oy1; ++oy) {
-                        e += WIN * E_PITCH;
-                        float4 acc = zero;
-                        fma4_acc(acc, p0, k[0]); fma4_acc(acc, p1, k[1]); fma4_acc(acc, p2, k[2]);
-                        const float4 m0 = *reinterpret_cast<const float4*>(e);
-                        const float4 m1 = *reinterpret_cast<const float4*>(e + E_PITCH);
-                        const float4 m2 = *reinterpret_cast<const float4*>(e + 2 * E_PITCH);
-                        fma4_acc(acc, m0, k[3]); fma4_acc(acc, m1, k[4]); fma4_acc(acc, m2, k[5]);
-                        e += WIN * E_PITCH;
-                        p0 = *reinterpret_cast<const float4*>(e);
-                        p1 = *reinterpret_cast<const float4*>(e + E_PITCH);
-                        p2 = *reinterpret_cast<const float4*>(e + 2 * E_PITCH);
-                        fma4_acc(acc, p0, k[6]); fma4_acc(acc, p1, k[7]); fma4_acc(acc, p2, k[8]);
-                        emit(acc);
-                    }
+                for (int r = 0; r < n_in; ++r, e += WIN * E_PITCH) {
+                    const float4 x0 = *reinterpret_cast<const float4*>(e);
+                    const float4 x1 = *reinterpret_cast<const float4*>(e + E_PITCH);
+                    const float4 x2 = *reinterpret_cast<const float4*>(e + 2 * E_PITCH);
+                    fma4_acc(acc0, x0, k[6]); fma4_acc(acc0, x1, k[7]); fma4_acc(acc0, x2, k[8]);
+                    fma4_acc(acc1, x0, k[3]); fma4_acc(acc1, x1, k[4]); fma4_acc(acc1, x2, k[5]);
+                    fma4_acc(acc2, x0, k[0]); fma4_acc(acc2, x1, k[1]); fma4_acc(acc2, x2, k[2]);
+                    if (r >= 2) emit(acc0);
+                    acc0 = acc1; acc1 = acc2; acc2 = zero;
+                }
+            } else {
+                float4 p0 = *reinterpret_cast<const float4*>(e);
+                float4 p1 = *reinterpret_cast<const float4*>(e + E_PITCH);
+                float4 p2 = *reinterpret_cast<const float4*>(e + 2 * E_PITCH);
+                for (int oy = dw_oy0; oy < dw_oy1; ++oy) {
+                    e += WIN * E_PITCH;
+                    float4 acc4 = zero;
+                    fma4_acc(acc4, p0, k[0]); fma4_acc(acc4, p1, k[1]); fma4_acc(acc4, p2, k[2]);
+                    const float4 m0 = *reinterpret_cast<const float4*>(e);
+                    const float4 m1 = *reinterpret_cast<const float4*>(e + E_PITCH);
+                    const float4 m2 = *reinterpret_cast<const float4*>(e + 2 * E_PITCH);
+                    fma4_acc(acc4, m0, k[3]); fma4_acc(acc4, m1, k[4]); fma4_acc(acc4, m2, k[5]);
+                    e += WIN * E_PITCH;
+                    p0 = *reinterpret_cast<const float4*>(e);
+                    p1 = *reinterpret_cast<const float4*>(e + E_PITCH);
+                    p2 = *reinterpret_cast<const float4*>(e + 2 * E_PITCH);
+                    fma4_acc(acc4, p0, k[6]); fma4_acc(acc4, p1, k[7]); fma4_acc(acc4, p2, k[8]);
+                    emit(acc4);
                 }
             }
-            worker_barrier();                              // E and the parameter slot are free for the next chunk
-          }
         }
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
+        worker_barrier();                              // E and the parameter slot are free for the next chunk
+      }
     }
 }
 
@@ -473,15 +397,10 @@ int xdw_conv(const XdwConv& p, cudaStream_t st, const XdwConv* p2) {
         mp.x[1] = mp.x[0]; mp.w[1] = mp.w[0]; mp.wlo[1] = mp.wlo[0];
         a.scale1[1] = a.scale1[0]; a.bias1[1] = a.bias1[0]; a.wdw[1] = a.wdw[0]; a.scale2[1] = a.scale2[0]; a.bias2[1] = a.bias2[0]; a.out[1] = a.out[0];
     }
-    // Resident CTAs to aim for.  Round 1 (plain TF32, 2 CTAs/SM possible): one per SM leaves half of every SM to the concurrent
-    // kernels (+4 % end to end vs 296).  The 3xTF32 variant owns most of an SM's registers and half its tensor memory, so in the
-    // small-batch regime (many short kernels of 3 backbones x 4 lanes in flight) it pays to leave half of the SMs entirely to
-    // the other kernels: 74 CTAs measured +3.4 % (34.6k vs 33.5k faces/s at B = 32); large batches are throughput-bound and
-    // take every SM.
+    // Resident CTAs to aim for: one per SM (two would fit) leaves room on every SM for the other backbones' and batches'
+    // kernels of the concurrent pipeline.  SMK_XDW_SLOTS overrides the target.
     static const int slots_env = []() { const char* e = getenv("SMK_XDW_SLOTS"); return e ? atoi(e) : 0; }();
-    const int slots_lo = slots_env > 0 ? slots_env : ((p.w1t_lo && p.B <= 64) ? 74 : 148);
-    static const int slots_hi = []() { const char* e = getenv("SMK_XDW_SLOTS_HI"); return e ? atoi(e) : 0; }();  // layers with >= 296 output tiles (0: same as SMK_XDW_SLOTS)
-    const int slots = (slots_hi > 0 && (long)nprob * cdiv(Wo, TO) * cdiv(Ho, TO) * p.B >= 296) ? slots_hi : slots_lo;
+    const int slots = slots_env > 0 ? slots_env : num_sms();
     a.H = p.H; a.W = p.W; a.Ho = Ho; a.Wo = Wo; a.mid = p.mid; a.nkb = cdiv(p.Cin, BK); a.nchunks = cdiv(p.mid, NC);
     {   // split the channel chunks over enough CTAs to fill the resident slots
         const long tiles = (long)nprob * cdiv(Wo, TO) * cdiv(Ho, TO) * p.B;
@@ -492,10 +411,6 @@ int xdw_conv(const XdwConv& p, cudaStream_t st, const XdwConv* p2) {
     a.pad = p.stride == 1 ? 1 : 0;
     a.tiles_x = cdiv(Wo, TO); a.tiles_y = cdiv(Ho, TO);
     a.round_out = p.round_out;
-    {
-        static const int x3_trunc = []() { const char* e = getenv("SMK_X3_TRUNC"); return e ? atoi(e) : 1; }();
-        a.x3_trunc = x3_trunc;
-    }
     constexpr size_t smem = (size_t)STAGES * STAGE_BYTES + E_BYTES + PAR_BYTES + 1024 + 256;
     constexpr size_t smem3t = (size_t)STAGES * (STAGE_BYTES + B_BYTES) + E_BYTES + PAR_BYTES + 1024 + 256;  // 3xTF32: + the weight tails
     static_assert(2 * (smem + 1024) <= 228 * 1024, "two CTAs per SM");
@@ -522,11 +437,11 @@ int xdw_conv(const XdwConv& p, cudaStream_t st, const XdwConv* p2) {
         auto group = [](int ncols, int nrows) { const int n_rg = std::min(32 / ncols, nrows); return (unsigned)((nrows + n_rg - 1) / n_rg) | (unsigned)n_rg << 4; };
         a.geom = group(TO, TO) | group(TO, nrows_e) << 8 | group(ncols_e, TO) << 16 | group(ncols_e, nrows_e) << 24;
     }
-    dim3 grid((unsigned)std::min(a.n_items, p.w1t_lo ? std::min(slots, 148) : slots));            // persistent: (up to) 2 CTAs per SM
+    dim3 grid((unsigned)std::min(a.n_items, p.w1t_lo ? std::min(slots, num_sms()) : slots));      // persistent: (up to) 2 CTAs per SM
     { int v = (int)grid.x; a.d_grp = v % a.groups; v /= a.groups; a.d_tx = v % a.tiles_x; v /= a.tiles_x; a.d_ty = v % a.tiles_y; a.d_img = v / a.tiles_y; }
     if (p.w1t_lo) {
-        if (p.stride == 1) SMK_LAUNCH((xdw_kernel<1, 2>), dim3(grid), dim3(NUM_THREADS + NUM_SPLITTERS), smem3t, st, mp, a);
-        else SMK_LAUNCH((xdw_kernel<2, 2>), dim3(grid), dim3(NUM_THREADS + NUM_SPLITTERS), smem3t, st, mp, a);
+        if (p.stride == 1) SMK_LAUNCH((xdw_kernel<1, 2>), dim3(grid), dim3(NUM_THREADS), smem3t, st, mp, a);
+        else SMK_LAUNCH((xdw_kernel<2, 2>), dim3(grid), dim3(NUM_THREADS), smem3t, st, mp, a);
     } else {
         if (p.stride == 1) SMK_LAUNCH((xdw_kernel<1, 0>), dim3(grid), dim3(NUM_THREADS), smem, st, mp, a);
         else SMK_LAUNCH((xdw_kernel<2, 0>), dim3(grid), dim3(NUM_THREADS), smem, st, mp, a);

@@ -255,9 +255,8 @@ class SmirkPipeline:
         output tensor until ``gathered()`` is called.  A slot of
         a peer's buffer is rewritten ``slots`` batches later; ``gather_sync()`` (stream join + group barrier) makes a batch's
         gathered tensors safe to read.
-        backend "nccl": ``all_gather_into_tensor`` over NVLink 5 / NVSwitch.  NCCL's kernels occupy SMs while the compute
-        kernels (148 persistent CTAs each) run, which splits every overlapped launch into two waves: measured 0.85 (B = 32) /
-        0.89 (full cycle, B = 256) of the no-gather throughput at 8 GPUs (profiles/r02_bench_n8_nccl_gather.json)."""
+        backend "nccl": ``all_gather_into_tensor`` over NVLink / NVSwitch.  NCCL's kernels occupy SMs while the compute
+        kernels (one persistent CTA per SM each) run, which splits every overlapped launch into two waves."""
         import torch.distributed as dist
         self._gather_keys = tuple(keys) if (dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1) else ()
         self._gather_group = group
@@ -324,12 +323,9 @@ class SmirkPipeline:
         if self._gather_backend == "p2p":
             # Copy-engine copies into slot `rank` of each PEER's buffer on the fan's streams; the own shard is never copied.
             #   direct (one peer): every output goes from where the kernels wrote it, one copy per (output, peer) — device-local
-            #     copies are what hurts the concurrent compute kernels (tools/bench_peer_load.py: 7 x 21 MB inside the GPU cost
-            #     the B = 32 pipeline 42 %, the same bytes pushed to a peer 3.8 %): 0.999 of the no-gather throughput at 2 GPUs
-            #     against 0.972 with a pack copy first.
-            #   packed (more peers): the outputs are first packed into one staging buffer and each peer gets ONE copy.  At
-            #     8 GPUs the 21 copies per batch of the direct form measured 226k faces/s end to end against 260k packed
-            #     (device-resident: 250k vs 249k); profiles/r02_bench_n8_*.json.
+            #     copies are what hurts the concurrent compute kernels (tools/bench_peer_load.py measures it), so none is made.
+            #   packed (more peers): the outputs are first packed into one staging buffer and each peer gets ONE copy instead of
+            #     one per (output, peer).
             with torch.cuda.stream(self._comm):
                 self._comm.wait_event(L.computed)
                 if self._p2p["pack"]:
@@ -337,8 +333,7 @@ class SmirkPipeline:
                         L.p2p_stage[off:off + n].copy_(rec["out"][k].reshape(-1).view(torch.uint8), non_blocking=True)
                     # The lane may overwrite its outputs as soon as they are PACKED: the pushes read the staging buffer only, and
                     # its reuse is ordered by this stream (a fan push ends with the stream waiting for every copy).  Releasing
-                    # the lane after the pushes instead idles it for their whole duration — with 7 peers 0.3 of the 3.6 ms a
-                    # B = 32 batch spends on its lane, which is the 11 % the 8-GPU runs lost (DESIGN.md 6).
+                    # the lane after the pushes instead idles it for their whole duration.
                     L.gathered.record(self._comm)
                     _lib.check(_lib.lib().smk_peer_fan_push(self._fan, L.p2p.dsts[0], ws - 1, L.p2p_stage.data_ptr(), self._p2p["shard"],
                                                             self._comm.cuda_stream), "smk_peer_fan_push")

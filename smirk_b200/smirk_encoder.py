@@ -112,7 +112,7 @@ class _NativeEncoder(nn.Module):
     ``_parts()`` (slot 0 = pose / small, 1 = shape / large, 2 = expression / large; None = not part of this module),
     re-packed whenever a parameter / buffer is modified or moved, and the raw forward through the C ABI.
 
-    ``precision``: 0 fp32 CUDA cores | 1 TF32 tcgen05 1x1 convs | 2 = 1 + fused expand/depthwise blocks |
+    ``precision``: 0 fp32 CUDA cores | 1 TF32 wgmma 1x1 convs | 2 = 1 + fused expand/depthwise blocks |
     3 = 2 with error-compensated 3xTF32 arithmetic (fp32-equivalent; the parity path)."""
 
     def _init_native(self, n_exp=50, n_shape=300):

@@ -1,8 +1,7 @@
 """TEST INFRASTRUCTURE — the single-image flow of the reference's ``demo.py`` restated for machines that have a GPU but
 no reference checkout (the GPU box): same steps, same module names — it imports the hot-path classes from the names the
 reference uses (``src.smirk_encoder`` ...), which ``python -m smirk_b200.dropin`` aliases to smirk_b200 — and writes the
-same grid image.  Each block cites the demo.py lines it follows.  The unmodified script itself is exercised in the build
-container by tests/test_dropin_demo.py::test_unmodified_demo_script_runs_on_the_dropin_classes.
+same grid image.  Each block cites the demo.py lines it follows.  The image the unmodified script wrote is tests/golden/demo.npz.
 
     python -m smirk_b200.dropin tests/demo_flow.py --input_path x.png --checkpoint ck.pt --out_path out [--use_smirk_generator]
 """

@@ -1,5 +1,5 @@
 """GPU suite (-m gpu): single convolution kernels through the C ABI's test entry points against
-torch fp32 on the same inputs.  fp32 CUDA-core path: 1e-5 relative.  TF32 tcgen05 path: TF32 operand
+torch fp32 on the same inputs.  fp32 CUDA-core path: 1e-5 relative.  TF32 wgmma path: TF32 operand
 truncation (10-bit mantissa) bounds the error at ~1e-3 of the output scale; the torch reference for
 that path is computed in fp64 so the comparison isolates the kernel's own rounding."""
 import ctypes as C
@@ -111,7 +111,7 @@ TC_CASES = [
     (2, 14, 14, 64, 128, 1),        # 3x3, tiles cross rows and images, partial tail
     (3, 14, 14, 32, 96, 2),         # 3x3 over a reflection-padded buffer
     (2, 28, 28, 128, 256, 1),       # 3x3, two N tiles, 36 k-blocks (ring wraps many times)
-    (2, 160, 160, 32, 32, 1),       # 3x3 persistent path: 400 tiles on 296 CTAs -> CTAs own 1 or 2 tiles (TMEM double buffer)
+    (2, 160, 160, 32, 32, 1),       # 3x3 persistent path: 400 tiles on 2 CTAs per SM -> CTAs own 1 or 2 tiles
     (3, 120, 120, 64, 64, 2),       # 3x3 persistent, BN = 64, reflection-padded input, 338 tiles
     (1, 300, 300, 32, 24, 1),       # 3x3 persistent, 704 tiles -> 2-3 tiles per CTA, N < BN, partial last tile
 ]
@@ -312,8 +312,8 @@ def test_gemm_tc3x_matches_fp64(native_lib, M, K, N, relu, use_res):
     got = out.cpu()
     assert torch.isfinite(got).all()
     err = (got - ref).abs().max().item()
-    # measured on B200: 8e-6 of the output scale at K = 960 (the dropped a_lo*w_lo products and the tensor core's own
-    # accumulation), 100x below plain TF32; bound it at 4e-6 * sqrt(K / 64)
+    # the error left is the dropped a_lo*w_lo products and the tensor core's own accumulation, ~100x below plain TF32;
+    # bound it at 4e-6 * sqrt(K / 64) of the output scale
     assert err <= 4e-6 * ref.abs().max().item() * max(1.0, (K / 64) ** 0.5), "max err %.3g vs scale %.3g" % (err, ref.abs().max().item())
 
 

@@ -257,7 +257,7 @@ def test_generator_batch_independence(generator):
 
 
 # ------------------------------------------------------------------------- TF32 tensor-core precision
-# precision = 1 runs the 1x1 / 3x3 / transposed convolutions on tcgen05 with TF32 operands (10-bit
+# precision = 1 runs the 1x1 / 3x3 / transposed convolutions on wgmma with TF32 operands (10-bit
 # mantissa, fp32 accumulate) — the arithmetic the reference itself gets from cuDNN on Ampere+ GPUs
 # (torch.backends.cudnn.allow_tf32 defaults to True).  Tolerance: 5e-3 of the output scale through
 # the ~50-layer encoder and the 27-conv generator, stated here; the fp32 path above stays at 1e-4.
@@ -296,7 +296,7 @@ def test_encoder_tf32_tensor_core_path(encoder):
 
 
 def test_encoder_fused_blocks_path(encoder):
-    """precision = 2: inverted-residual blocks run expand+depthwise as one tcgen05 kernel."""
+    """precision = 2: inverted-residual blocks run expand+depthwise as one wgmma kernel."""
     import copy
     from oracle import encoder_ref
     ef = copy.deepcopy(encoder)

@@ -1,4 +1,4 @@
-"""Micro-benchmark of the TF32 tcgen05 GEMM kernel (gemm_tc.cu) on the encoder's 1x1 projection shapes and the
+"""Micro-benchmark of the TF32 wgmma GEMM kernel (gemm_tc.cu) on the encoder's 1x1 projection shapes and the
 generator's 3x3 convolution shapes.
 
     python tools/bench_pw.py [--batch 32] [--reps 20] [--only K72] [--gen]
