@@ -1,7 +1,6 @@
 // Error channel + version for the smirk_b200 C ABI.
 #include "common.cuh"
 #include <stdarg.h>
-#include <stdlib.h>
 
 namespace smk {
 static thread_local char g_err[512] = "";
@@ -49,9 +48,6 @@ int num_sms() {
     if (dev < 64) cached[dev] = n;
     return n;
 }
-// Off by default: with 3 backbone streams x 4 batches in flight the launch gaps are already filled by other
-// kernels; SMK_PDL=1 turns the launch attribute on (meant for a single low-latency stream).
-bool pdl_enabled() { static const bool on = []() { const char* e = getenv("SMK_PDL"); return e && atoi(e) != 0; }(); return on; }
 void prof_end() {
     if (!g_prof || !g_pending) return;
     cudaEventRecord(g_entries.back().b, g_pending_stream);

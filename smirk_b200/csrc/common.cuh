@@ -72,32 +72,24 @@ static inline int cdiv(long a, long b) { return (int)((a + b - 1) / b); }
 // Streaming multiprocessors of the current device (cached per device ordinal): the size of a persistent grid.
 int num_sms();
 
-// ---- programmatic dependent launch (PDL) --------------------------------------------------------------
-// Every kernel of the library is launched with cudaLaunchAttributeProgrammaticStreamSerialization and starts
-// with pdl_sync(): `griddepcontrol.wait` blocks until the preceding kernel on the stream has completed and
-// flushed (so every global read AND write of this kernel stays ordered after it), `griddepcontrol.
-// launch_dependents` lets the following kernel's CTAs be scheduled as soon as all CTAs of this one have
-// started.  Net effect: launch latency, parameter/tensor-map fetch, barrier init and tensor-map prefetch of
-// kernel N+1 overlap the tail of kernel N — which is what a chain of ~100 short kernels per batch is bound
-// by.  Inside a stream capture these become programmatic graph edges.  The attribute is opt-in (SMK_PDL=1, see
-// common.cu); without it the device-side instructions are no-ops.
-bool pdl_enabled();
 #ifdef __CUDACC__
-__device__ __forceinline__ void pdl_sync() {
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+// Launch errors surface through cudaGetLastError in SMK_CHECK_LAUNCH.
+#define SMK_LAUNCH(kernel, grid, block, smem, st, ...) kernel<<<grid, block, smem, st>>>(__VA_ARGS__)
+
+// cudaFuncAttributeMaxDynamicSharedMemorySize is per device and per function: set it the first time Kernel is
+// launched on a device.  One bit per device ordinal (ordinals >= 64 set it on every call).
+template <auto Kernel>
+cudaError_t set_max_dynamic_smem(int bytes) {
+    static unsigned long long configured_mask = 0;
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    const unsigned long long bit = dev < 64 ? 1ull << dev : 0;
+    if (bit && (__atomic_load_n(&configured_mask, __ATOMIC_RELAXED) & bit)) return cudaSuccess;
+    e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) __atomic_fetch_or(&configured_mask, bit, __ATOMIC_RELAXED);
+    return e;
 }
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, kernel, KArgs(static_cast<Args&&>(args))...);
-}
-#define SMK_LAUNCH(kernel, grid, block, smem, st, ...) (void)smk::launch_pdl(kernel, grid, block, smem, st, __VA_ARGS__)
 #endif
 
 // TF32 rounding (round-to-nearest, ties away: PTX cvt.rna).  The tensor cores read fp32 words from shared

@@ -23,8 +23,6 @@
 // the network's last layer (store 3).
 #include "gemm_tc.cuh"
 #include "tc_ptx.cuh"
-#include <cuda.h>
-#include <stdlib.h>
 
 namespace smk {
 namespace {
@@ -87,7 +85,6 @@ conv3_win_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
         fence_barrier_init();
     }
     __syncthreads();
-    pdl_sync();
 
     auto decode = [&](int t, int& img, int& h0, int& w0) {
         const int tx = t % a.tiles_x; t /= a.tiles_x;
@@ -249,21 +246,6 @@ conv3_win_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
     }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn g_encode = nullptr;
-
-int load_encoder() {
-    if (g_encode) return 0;
-    cudaDriverEntryPointQueryResult q;
-    void* fn = nullptr;
-    SMK_CHECK_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q));
-    SMK_REQUIRE(fn && q == cudaDriverEntryPointSuccess, "cuTensorMapEncodeTiled not available from the driver");
-    g_encode = (EncodeTiledFn)fn;
-    return 0;
-}
-
 size_t win_smem_bytes(int nchunks, int BN, bool res) {
     return (size_t)PIPES * PIPE_BYTES + (res ? (size_t)nchunks * 9 * BN * 128 : (size_t)PIPES * NB * BN * 128) + BAR_BYTES + PIPES * HEAD_PAR_BYTES + 1024;
 }
@@ -273,13 +255,7 @@ template <int BN, bool RES>
 int launch(const CUtensorMap& tmX, const CUtensorMap& tmW, const WinArgs& a, cudaStream_t st) {
     const size_t smem = win_smem_bytes(a.nchunks, BN, RES);
     SMK_REQUIRE(smem <= 227 * 1024, "conv3_win: shared-memory budget exceeded (%zu bytes)", smem);
-    static unsigned long long configured_mask = 0;
-    int dev = 0;
-    SMK_CHECK_CUDA(cudaGetDevice(&dev));
-    if (dev >= 64 || !(configured_mask & (1ull << dev))) {
-        SMK_CHECK_CUDA(cudaFuncSetAttribute((conv3_win_kernel<BN, RES>), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        if (dev < 64) configured_mask |= 1ull << dev;
-    }
+    SMK_CHECK_CUDA((set_max_dynamic_smem<conv3_win_kernel<BN, RES>>(227 * 1024)));
     SMK_LAUNCH((conv3_win_kernel<BN, RES>), dim3((unsigned)std::min(cdiv(a.n_tiles, PIPES), num_sms())), dim3(NUM_THREADS), smem, st, tmX, tmW, a);
     SMK_CHECK_LAUNCH();
     return 0;
@@ -288,40 +264,20 @@ int launch(const CUtensorMap& tmX, const CUtensorMap& tmW, const WinArgs& a, cud
 }  // namespace
 
 bool conv3_win_supported(const TcConv& p) {
-    static const int on = []() { const char* e = getenv("SMK_CONV3_WIN"); return e ? atoi(e) : 1; }();
-    if (!on || p.mode != 1 || p.res || p.wt_lo || (p.store != 0 && p.store != 3) || (p.store == 3 && p.N != 32)) return false;
+    if (p.mode != 1 || p.res || p.wt_lo || (p.store != 0 && p.store != 3) || (p.store == 3 && p.N != 32)) return false;
     if (p.Cin % 32 != 0 || p.K != 9 * p.Cin || (p.N != 32 && p.N != 64)) return false;
-    if (p.W < 56) return false;                                   // low-resolution layers are MMA-bound: gemm_tc's wide tiles win there
-    static const int ring_on = []() { const char* e = getenv("SMK_CONV3_WIN_RING"); return e ? atoi(e) : 1; }();
-    return ring_on || win_resident(p.Cin / 32, p.N <= 32 ? 32 : 64);   // resident weights: 36 KB (32->32), 72 KB (64->32, 32->64); else a ring
+    return p.W >= 56;                                             // low-resolution layers are MMA-bound: gemm_tc's wide tiles win there
 }
 
 // p uses TcConv semantics: mode 1 (3x3, zero padding 1), store 0 or 3, no residual.
 int conv3_win(const TcConv& p, cudaStream_t st) {
-    if (int rc = load_encoder()) return rc;
     SMK_REQUIRE(conv3_win_supported(p), "conv3_win: unsupported problem (needs 3x3 zero-pad, Cin %% 32 == 0, N in {32, 64}, W >= 56)");
     SMK_REQUIRE(p.N % 4 == 0 && p.ld_in % 4 == 0 && p.ld_out % 4 == 0, "conv3_win: N and strides must be multiples of 4");
     SMK_REQUIRE(p.store != 3 || (p.N == 32 && p.head_w && p.head_b && p.head_c >= 1 && p.head_c <= 4), "conv3_win: the fused head needs N == 32");
     const int BN = p.N <= 32 ? 32 : 64;
     CUtensorMap tmX, tmW;
-    {
-        cuuint64_t dims[4] = {(cuuint64_t)p.Cin, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.B};
-        cuuint64_t strides[3] = {(cuuint64_t)p.ld_in * 4, (cuuint64_t)p.W * p.ld_in * 4, (cuuint64_t)p.H * p.W * p.ld_in * 4};
-        cuuint32_t box[4] = {32, (cuuint32_t)PW, (cuuint32_t)(TH + 2), 1};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult r = g_encode(&tmX, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)p.in, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        SMK_REQUIRE(r == CUDA_SUCCESS, "conv3_win: cuTensorMapEncodeTiled(x) failed (%d)", (int)r);
-    }
-    {
-        cuuint64_t dims[2] = {(cuuint64_t)p.K, (cuuint64_t)p.N};
-        cuuint64_t strides[1] = {(cuuint64_t)p.K * 4};
-        cuuint32_t box[2] = {32, (cuuint32_t)BN};
-        cuuint32_t estr[2] = {1, 1};
-        CUresult r = g_encode(&tmW, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)p.wt, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        SMK_REQUIRE(r == CUDA_SUCCESS, "conv3_win: cuTensorMapEncodeTiled(w) failed (%d)", (int)r);
-    }
+    if (int rc = encode_nhwc(&tmX, p.in, p.B, p.H, p.W, p.Cin, p.ld_in, PW, TH + 2, "conv3_win(x)")) return rc;
+    if (int rc = encode_2d(&tmW, p.wt, (uint64_t)p.N, (uint64_t)p.K, (uint64_t)p.K, (uint32_t)BN, "conv3_win(w)")) return rc;
     WinArgs a{};
     a.H = p.H; a.W = p.W; a.N = p.N; a.nchunks = p.Cin / 32;
     a.tiles_x = cdiv(p.W, TW); a.tiles_y = cdiv(p.H, TH); a.n_tiles = a.tiles_x * a.tiles_y * p.B;
@@ -333,6 +289,7 @@ int conv3_win(const TcConv& p, cudaStream_t st) {
         if (g_prof_detail) tag = prof_shape_tag(tag, (long)M, p.K, p.N);
         SMK_TAG(tag, 4.0 * (M * p.Cin + (double)p.K * p.N + M * (p.store == 3 ? p.head_c : p.N) + 2.0 * p.N), 2.0 * M * p.N * p.K, st);
     }
+    // resident weights: 36 KB (32->32), 72 KB (64->32, 32->64); larger layers stream them through a ring
     if (win_resident(a.nchunks, BN)) return BN == 32 ? launch<32, true>(tmX, tmW, a, st) : launch<64, true>(tmX, tmW, a, st);
     return BN == 32 ? launch<32, false>(tmX, tmW, a, st) : launch<64, false>(tmX, tmW, a, st);
 }

@@ -9,7 +9,6 @@
 #include "gemm_tc.cuh"
 #include "xdw_tc.cuh"
 #include <math.h>
-#include <stdlib.h>
 
 namespace {
 
@@ -253,8 +252,7 @@ extern "C" int smk_encoder_forward(const SmkEncoder* h, const float* img, int B,
     const SmkEncoder::ForkSet& fk = h->forks[__atomic_fetch_add(&h->next_fork, 1u, __ATOMIC_RELAXED) % SmkEncoder::kForkSets];
     // precision 2: stem + block 0 (depthwise-separable, 16 channels at 112 x 112) run as one kernel per backbone —
     // the three largest activations never reach HBM.
-    static const int fuse_stem_env = []() { const char* e = getenv("SMK_FUSE_STEM"); return e ? atoi(e) : 1; }();
-    const bool fuse_stem = h->fuse_xdw && fuse_stem_env;                           // every backbone starts with a DS block
+    const bool fuse_stem = h->fuse_xdw;                           // every backbone starts with a DS block
     if (!fuse_stem && n_present == 3) {   // all three stems in one pass over the image (it is the only tensor the backbones share)
         const float* sw[3]; const float* ss[3]; const float* sb[3]; float* so[3];
         for (int i = 0; i < 3; ++i) { sw[i] = h->bb[i].stem.w; ss[i] = h->bb[i].stem.scale; sb[i] = h->bb[i].stem.bias; so[i] = bufs[i][0]; }
@@ -270,8 +268,7 @@ extern "C" int smk_encoder_forward(const SmkEncoder* h, const float* img, int B,
     int rc = 0;                                   // first error; the side streams are joined on every path
     // Work units: the two "large" backbones (shape, expression) have the same layer list, so on the tensor-core path they
     // advance in lock step and every layer of the pair is ONE launch; the small (pose) backbone is its own unit.
-    static const int pair_env = []() { const char* e = getenv("SMK_ENC_PAIR"); return e ? atoi(e) : 1; }();
-    const bool pair = pair_env && h->precision >= 1 && h->present[1] && h->present[2];
+    const bool pair = h->precision >= 1 && h->present[1] && h->present[2];
     struct Unit { int n; int idx[2]; cudaStream_t st; };
     Unit units[3]; int n_units = 0;
     if (h->present[0]) units[n_units++] = Unit{1, {0, 0}, main_st};
@@ -313,8 +310,8 @@ extern "C" int smk_encoder_forward(const SmkEncoder* h, const float* img, int B,
             } else if (b0.kind == IR) {
                 // The 7x7 layers (a 16x16 window holds 81 useful pixels, 49 outputs) run as 1x1 GEMM + depthwise kernels:
                 // most of a window would be halo; every other resolution runs fused.
-                static const int xdw_min_res = []() { const char* e = getenv("SMK_XDW_MIN_RES"); return e ? atoi(e) : 8; }();
-                if (h->fuse_xdw && b0.pw.wt && res >= xdw_min_res) {
+                constexpr int kXdwMinRes = 8;
+                if (h->fuse_xdw && b0.pw.wt && res >= kXdwMinRes) {
                     // expand 1x1 + depthwise 3x3 in one kernel: the expanded tensor never leaves the SM
                     smk::XdwConv q[2];
                     for (int k = 0; k < n; ++k) {

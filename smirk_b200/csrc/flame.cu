@@ -73,7 +73,6 @@ flame_pose_kernel(FlameDev d, const float* __restrict__ betas, const float* __re
                   float* __restrict__ joints_out /*[B][5][3] or null*/, int32_t* __restrict__ dyn_out /*[B]*/) {
     __shared__ float sJ[15];
     __shared__ float sR[kJ][9];
-    smk::pdl_sync();
     const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const float* beta = betas + (size_t)b * d.L;
     // J = J0 + JS * beta : 15 dot products of length L, one warp per row (lbs.py:188 pre-contracted)
@@ -154,7 +153,6 @@ flame_verts_kernel(FlameDev d, const float* __restrict__ betas, const float* __r
     float* sE = sA + BT * 60;               // [BT][2]
     const int b0 = blockIdx.y * BT;
     const int tid = threadIdx.x;
-    smk::pdl_sync();
     for (int i = tid; i < d.L * BT; i += 128) {
         int l = i / BT, t = i % BT;
         int b = min(b0 + t, B - 1);
@@ -259,7 +257,6 @@ flame_landmarks_kernel(FlameDev d, const float* __restrict__ verts, const int32_
     const int n_fan = d.n_dyn + d.n_static;
     const int total = n_fan + d.n_full + d.n_mp;
     const float* vb = verts + (size_t)b * d.V * 3;
-    smk::pdl_sync();
     const int row = dyn_idx[b];
     for (int i = threadIdx.x; i < total; i += blockDim.x) {
         int f; const float* bc; float* out;
@@ -377,8 +374,8 @@ extern "C" int smk_flame_forward(const SmkFlame* h, const float* betas, const fl
     SMK_LAUNCH(flame_pose_kernel, dim3(B), dim3(128), 0, st, d, betas, full_pose, B, A, pf, joints, dyn);
     SMK_CHECK_LAUNCH();
     int rc;
-    static const int bt8_from = []() { const char* e = getenv("SMK_FLAME_BT8_FROM"); return e ? atoi(e) : 96; }();
-    if (B >= bt8_from) rc = launch_verts<8>(d, betas, eyelid, A, pf, B, verts, st);
+    constexpr int kBt8From = 96;               // batch size from which flame_verts keeps 8 (instead of 4) faces per thread
+    if (B >= kBt8From) rc = launch_verts<8>(d, betas, eyelid, A, pf, B, verts, st);
     else if (B >= 8) rc = launch_verts<4>(d, betas, eyelid, A, pf, B, verts, st);
     else if (B >= 2) rc = launch_verts<2>(d, betas, eyelid, A, pf, B, verts, st);
     else rc = launch_verts<1>(d, betas, eyelid, A, pf, B, verts, st);

@@ -23,7 +23,6 @@
 // Threads (288): warps 0..7 = consumers (warpgroups 0 and 1), warp 8 = TMA producer.
 #include "gemm_tc.cuh"
 #include "tc_ptx.cuh"
-#include <cuda.h>
 
 namespace smk {
 namespace {
@@ -106,7 +105,6 @@ gemm_tc_kernel(const __grid_constant__ TcMaps mp, const TcArgs a) {
         fence_barrier_init();
     }
     __syncthreads();
-    pdl_sync();                                // barriers and tensor maps are set up; now wait for the producer layer
 
     if (warp == CONSUMER_WARPS) {
         if (lane == 0) {
@@ -297,7 +295,6 @@ gemm_tc_kernel(const __grid_constant__ TcMaps mp, const TcArgs a) {
 // ---- reflection halo of a [B, H+2, W+2, C] buffer whose interior has been written -------------------
 __global__ void __launch_bounds__(256)
 reflect_halo_kernel(float* __restrict__ buf, int B, int H, int W, int C) {
-    pdl_sync();
     const int Hp = H + 2, Wp = W + 2, C4 = C >> 2;
     const int halo = 2 * Wp + 2 * H;                       // halo pixels per image
     long total = (long)B * halo * C4;
@@ -324,49 +321,73 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                    const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*, CUtensorMapInterleave,
                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn g_encode_tiled = nullptr;
-EncodeIm2colFn g_encode_im2col = nullptr;
+struct DriverFns { EncodeTiledFn tiled; EncodeIm2colFn im2col; };
 
-int load_driver_fns() {
-    if (g_encode_tiled && g_encode_im2col) return 0;
-    cudaDriverEntryPointQueryResult q;
-    void* fn = nullptr;
-    SMK_CHECK_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q));
-    SMK_REQUIRE(fn && q == cudaDriverEntryPointSuccess, "cuTensorMapEncodeTiled not available from the driver");
-    g_encode_tiled = (EncodeTiledFn)fn;
-    SMK_CHECK_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &fn, cudaEnableDefault, &q));
-    SMK_REQUIRE(fn && q == cudaDriverEntryPointSuccess, "cuTensorMapEncodeIm2col not available from the driver");
-    g_encode_im2col = (EncodeIm2colFn)fn;
+// Resolved once per process (thread-safe static initialisation); null where the driver lacks an entry point.
+const DriverFns& driver_fns() {
+    static const DriverFns fns = [] {
+        auto get = [](const char* name) -> void* {
+            void* fn = nullptr;
+            cudaDriverEntryPointQueryResult q;
+            return cudaGetDriverEntryPoint(name, &fn, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess ? fn : nullptr;
+        };
+        return DriverFns{(EncodeTiledFn)get("cuTensorMapEncodeTiled"), (EncodeIm2colFn)get("cuTensorMapEncodeIm2col")};
+    }();
+    return fns;
+}
+
+}  // namespace
+
+int tc_init() {
+    SMK_REQUIRE(driver_fns().tiled && driver_fns().im2col, "cuTensorMapEncodeTiled / cuTensorMapEncodeIm2col not available from the driver");
     return 0;
 }
 
-int encode_2d(CUtensorMap* map, const float* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows) {
+int encode_2d(CUtensorMap* map, const float* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows, const char* what) {
+    if (int rc = tc_init()) return rc;
     cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {ld_elems * sizeof(float)};
+    cuuint64_t strides[1] = {ld * sizeof(float)};
     cuuint32_t box[2] = {(cuuint32_t)BK, box_rows};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = g_encode_tiled(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)base, dims, strides, box, estr,
-                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    SMK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d): rows=%llu cols=%llu ld=%llu box_rows=%u", (int)r,
-                (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld_elems, box_rows);
+    CUresult r = driver_fns().tiled(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)base, dims, strides, box, estr,
+                                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    SMK_REQUIRE(r == CUDA_SUCCESS, "%s: cuTensorMapEncodeTiled failed (%d): rows=%llu cols=%llu ld=%llu box_rows=%u", what, (int)r,
+                (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld, box_rows);
     return 0;
 }
 
-// NHWC activation tensor [B][Hin][Win][C] (pixel stride ld) read as 3x3 windows; lower/upper corner per CUTLASS
-// conventions: lower = -pad, upper = pad - (3-1).
-int encode_im2col(CUtensorMap* map, const float* base, int B, int Hin, int Win, int C, int ld, int pad) {
-    cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)Win, (cuuint64_t)Hin, (cuuint64_t)B};
-    cuuint64_t strides[3] = {(cuuint64_t)ld * 4, (cuuint64_t)Win * ld * 4, (cuuint64_t)Hin * Win * ld * 4};
+int encode_nhwc(CUtensorMap* map, const float* base, int B, int H, int W, int C, int ld, int box_w, int box_h, const char* what) {
+    if (int rc = tc_init()) return rc;
+    cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+    cuuint64_t strides[3] = {(cuuint64_t)ld * 4, (cuuint64_t)W * ld * 4, (cuuint64_t)H * W * ld * 4};
+    cuuint32_t box[4] = {(cuuint32_t)BK, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    CUresult r = driver_fns().tiled(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)base, dims, strides, box, estr,
+                                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    SMK_REQUIRE(r == CUDA_SUCCESS, "%s: cuTensorMapEncodeTiled failed (%d): B=%d H=%d W=%d C=%d ld=%d box=%dx%d", what, (int)r,
+                B, H, W, C, ld, box_h, box_w);
+    return 0;
+}
+
+// Lower / upper corner of the 3x3 window per CUTLASS conventions: lower = -pad, upper = pad - (3-1).
+int encode_im2col(CUtensorMap* map, const float* base, int B, int H, int W, int C, int ld, int pad, const char* what) {
+    if (int rc = tc_init()) return rc;
+    cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+    cuuint64_t strides[3] = {(cuuint64_t)ld * 4, (cuuint64_t)W * ld * 4, (cuuint64_t)H * W * ld * 4};
     int lower[2] = {-pad, -pad};
     int upper[2] = {pad - 2, pad - 2};
     cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = g_encode_im2col(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)base, dims, strides, lower, upper,
-                                 (cuuint32_t)BK, (cuuint32_t)BM, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                 CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    SMK_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeIm2col failed (%d): B=%d H=%d W=%d C=%d ld=%d pad=%d", (int)r, B, Hin, Win, C, ld, pad);
+    CUresult r = driver_fns().im2col(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)base, dims, strides, lower, upper,
+                                     (cuuint32_t)BK, (cuuint32_t)BM, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                                     CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    SMK_REQUIRE(r == CUDA_SUCCESS, "%s: cuTensorMapEncodeIm2col failed (%d): B=%d H=%d W=%d C=%d ld=%d pad=%d", what, (int)r,
+                B, H, W, C, ld, pad);
     return 0;
 }
+
+namespace {
 
 template <int BN, int STAGES, int MINB, bool PERSIST, int X3 = 0>
 int launch(const TcMaps& mp, const TcArgs& a_in, cudaStream_t st, int groups) {
@@ -374,15 +395,7 @@ int launch(const TcMaps& mp, const TcArgs& a_in, cudaStream_t st, int groups) {
     constexpr size_t smem = (size_t)STAGES * stage + (PERSIST ? SLAB_BYTES : 0) + BAR_BYTES + HEAD_PAR_BYTES + 1024;
     static_assert(PERSIST || (size_t)STAGES * stage >= SLAB_BYTES, "single-tile CTAs stage the epilogue in ring stage 0");
     static_assert(MINB * (smem + 1024) <= 228 * 1024, "shared memory budget of MINB resident CTAs");
-    // The attribute is per device and per function; set it once per (device, instantiation).  One bit per
-    // device ordinal; a benign race (two threads setting it twice) is harmless.
-    static unsigned long long configured_mask = 0;
-    int dev = 0;
-    SMK_CHECK_CUDA(cudaGetDevice(&dev));
-    if (dev >= 64 || !(configured_mask & (1ull << dev))) {
-        SMK_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, STAGES, MINB, PERSIST, X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        if (dev < 64) configured_mask |= 1ull << dev;
-    }
+    SMK_CHECK_CUDA((set_max_dynamic_smem<gemm_tc_kernel<BN, STAGES, MINB, PERSIST, X3>>((int)smem)));
     TcArgs a = a_in;
     a.tiles_n = cdiv(a.N, BN);
     a.n_tiles_g = cdiv(a.M, BM) * a.tiles_n;
@@ -395,10 +408,7 @@ int launch(const TcMaps& mp, const TcArgs& a_in, cudaStream_t st, int groups) {
 
 }  // namespace
 
-int tc_init() { return load_driver_fns(); }
-
 int tc_conv(const TcConv& p, cudaStream_t st, const TcConv* p2) {
-    if (int rc = load_driver_fns()) return rc;
     if (!p2 && conv3_win_supported(p)) return conv3_win(p, st);       // 224^2 / 112^2, Cout 32 / 64: one patch load per chunk, resident weights
     const int M = p.B * p.H * p.W;
     const int groups = p2 ? 2 : 1;
@@ -413,9 +423,7 @@ int tc_conv(const TcConv& p, cudaStream_t st, const TcConv* p2) {
     // Wide 3x3 layers (N a multiple of 256: the generator's 28^2 / 14^2 convolutions, most of its FLOPs): a 128 x 256 tile
     // halves the A-operand bytes wgmma pulls from shared memory per FLOP (TF32 operands are 4 bytes; at BN = 128 the
     // operand reads ask for more than an SM's shared-memory bandwidth).  One persistent CTA per SM, 4-stage ring.
-    // SMK_TC_BN256=0 keeps 128-wide tiles.
-    static const int bn256 = []() { const char* e = getenv("SMK_TC_BN256"); return e ? atoi(e) : 1; }();
-    if (bn256 && p.mode != 0 && p.N % 256 == 0 && !p.wt_lo) BN = 256;
+    if (p.mode != 0 && p.N % 256 == 0 && !p.wt_lo) BN = 256;
     TcMaps mp;
     TcArgs a{};
     a.M = M; a.N = p.N; a.nkb = cdiv(p.K, BK); a.mode = p.mode == 0 ? 0 : 1; a.H = p.H; a.W = p.W;
@@ -430,14 +438,14 @@ int tc_conv(const TcConv& p, cudaStream_t st, const TcConv* p2) {
         const TcConv& q = g ? *p2 : p;
         a.scale[g] = q.scale; a.bias[g] = q.bias; a.res[g] = q.res; a.out[g] = q.out;
         if (q.mode == 0) {
-            if (int rc = encode_2d(&mp.a[g], q.in, (uint64_t)M, (uint64_t)q.K, (uint64_t)q.ld_in, BM)) return rc;
+            if (int rc = encode_2d(&mp.a[g], q.in, (uint64_t)M, (uint64_t)q.K, (uint64_t)q.ld_in, BM, "tc_conv(A)")) return rc;
         } else if (q.mode == 1) {
-            if (int rc = encode_im2col(&mp.a[g], q.in, q.B, q.H, q.W, q.Cin, q.ld_in, 1)) return rc;
+            if (int rc = encode_im2col(&mp.a[g], q.in, q.B, q.H, q.W, q.Cin, q.ld_in, 1, "tc_conv(A)")) return rc;
         } else {                                            // input buffer is [B, H+2, W+2, C], already reflection padded
-            if (int rc = encode_im2col(&mp.a[g], q.in, q.B, q.H + 2, q.W + 2, q.Cin, q.ld_in, 0)) return rc;
+            if (int rc = encode_im2col(&mp.a[g], q.in, q.B, q.H + 2, q.W + 2, q.Cin, q.ld_in, 0, "tc_conv(A)")) return rc;
         }
-        if (int rc = encode_2d(&mp.b[g], q.wt, (uint64_t)q.N, (uint64_t)q.K, (uint64_t)q.K, (uint32_t)BN)) return rc;
-        if (q.wt_lo) { if (int rc = encode_2d(&mp.blo[g], q.wt_lo, (uint64_t)q.N, (uint64_t)q.K, (uint64_t)q.K, (uint32_t)BN)) return rc; }
+        if (int rc = encode_2d(&mp.b[g], q.wt, (uint64_t)q.N, (uint64_t)q.K, (uint64_t)q.K, (uint32_t)BN, "tc_conv(W)")) return rc;
+        if (q.wt_lo) { if (int rc = encode_2d(&mp.blo[g], q.wt_lo, (uint64_t)q.N, (uint64_t)q.K, (uint64_t)q.K, (uint32_t)BN, "tc_conv(W tails)")) return rc; }
         else mp.blo[g] = mp.b[g];
     }
     if (groups == 1) { mp.a[1] = mp.a[0]; mp.b[1] = mp.b[0]; mp.blo[1] = mp.blo[0]; a.scale[1] = a.scale[0]; a.bias[1] = a.bias[0]; a.res[1] = a.res[0]; a.out[1] = a.out[0]; }
@@ -460,13 +468,12 @@ int tc_conv(const TcConv& p, cudaStream_t st, const TcConv* p2) {
         if (BN == 64) return launch<64, 2, 2, false, 2>(mp, a, st, groups);
         return launch<128, 2, 1, false, 2>(mp, a, st, groups);
     }
-    static const int persist_mode = []() { const char* e = getenv("SMK_TC_PERSIST"); return e ? atoi(e) : -1; }();   // -1 auto, 0 never, 1 always
     const long n_tiles = (long)groups * cdiv(M, BM) * cdiv(p.N, BN);
     // 3x3 convolutions (deep K): persistent CTAs for the narrow-N layers and for the few-tile 14x14 layers; the fused head
     // always (its constants are loaded once per CTA).  Everything else runs one tile per CTA with a 2-stage ring: a small
     // footprint, so several CTAs of this kernel — or of the other backbones' and batches' kernels — share an SM and hide
     // each other's prologue / epilogue.
-    const bool persist = p.store == 3 || (persist_mode >= 0 ? persist_mode != 0 : (p.mode != 0 && (BN <= 64 || n_tiles <= 2 * num_sms())));
+    const bool persist = p.store == 3 || (p.mode != 0 && (BN <= 64 || n_tiles <= 2 * num_sms()));
     if (BN == 256) return launch<256, 4, 1, true>(mp, a, st, groups);
     if (persist) {
         if (BN == 32) return launch<32, 4, 2, true>(mp, a, st, groups);

@@ -1,6 +1,7 @@
 // TF32 wgmma implicit-GEMM convolution (see gemm_tc.cu).
 #pragma once
 #include "common.cuh"
+#include <cuda.h>
 
 namespace smk {
 
@@ -22,6 +23,16 @@ struct TcConv {
 };
 
 int tc_init();                                              // resolves the driver's tensor-map encoders
+
+// TMA descriptors over fp32 tensors as the wgmma kernels read them: boxes of 32 elements (128 bytes) in the innermost
+// dimension, SWIZZLE_128B, L2 promotion 128 B, zero fill out of bounds.  `what` names the operand in the error message.
+// [rows][cols] matrix with a row stride of ld elements, boxes of box_rows x 32.
+int encode_2d(CUtensorMap* map, const float* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows, const char* what);
+// NHWC tensor [B][H][W][C] with a pixel stride of ld elements, boxes of box_h x box_w pixels x 32 channels of one image.
+int encode_nhwc(CUtensorMap* map, const float* base, int B, int H, int W, int C, int ld, int box_w, int box_h, const char* what);
+// The same tensor read as 3x3 windows with `pad` pixels of zero padding (im2col), boxes of 128 pixels x 32 channels.
+int encode_im2col(CUtensorMap* map, const float* base, int B, int H, int W, int C, int ld, int pad, const char* what);
+
 // p2 (optional): a second problem of identical shape sharing the launch (tiles of both in one grid).
 int tc_conv(const TcConv& p, cudaStream_t st, const TcConv* p2 = nullptr);
 int reflect_halo(float* buf, int B, int H, int W, int C, cudaStream_t st);

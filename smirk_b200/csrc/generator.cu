@@ -18,7 +18,6 @@
 #include "nn_kernels.cuh"
 #include "gemm_tc.cuh"
 #include <math.h>
-#include <stdlib.h>
 
 namespace {
 
@@ -271,8 +270,7 @@ extern "C" int smk_generator_forward(const SmkGenerator* h, const float* x, int 
         if ((rc = conv3(h, h->dec[l][0], cat[lvl], 2 * u.cout, B, dS, false, true, nullptr, 0, t[lvl], u.cout, 0, st))) return rc;
         // last layer of the tensor-core path: the 1x1 conv + sigmoid (smirk_generator.py:77-78,86) rides in the epilogue of
         // dec1conv2 — the [B,224,224,32] activation (6.4 MB per face) is neither written nor read back
-        static const int fuse_head_env = []() { const char* e = getenv("SMK_FUSE_HEAD"); return e ? atoi(e) : 1; }();
-        const bool fuse_head = l == 3 && tc && fuse_head_env && u.cout <= 32;
+        const bool fuse_head = l == 3 && tc && u.cout <= 32;
         if (fuse_head) return conv3(h, h->dec[l][1], t[lvl], u.cout, B, dS, false, true, nullptr, 0, y, u.cout, 3, st, true);
         if ((rc = conv3(h, h->dec[l][1], t[lvl], u.cout, B, dS, false, true, nullptr, 0, d[lvl], u.cout, 0, st))) return rc;
         din = d[lvl];

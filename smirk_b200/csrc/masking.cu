@@ -37,7 +37,6 @@ struct MaskDev {
 // vertex normals of the full mesh (util.vertex_normals), one thread per vertex, fixed accumulation order
 __global__ void __launch_bounds__(128)
 mask_normals_kernel(MaskDev d, const float* __restrict__ tv, int B, float* __restrict__ normals) {
-    smk::pdl_sync();
     const int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
     if (i >= d.V) return;
     const float* vb = tv + (size_t)b * d.V * 3;
@@ -63,7 +62,6 @@ mask_normals_kernel(MaskDev d, const float* __restrict__ tv, int B, float* __res
 __global__ void __launch_bounds__(128)
 mask_face_weights_kernel(MaskDev d, const float* __restrict__ tv, const float* __restrict__ normals,
                          const float* __restrict__ base_prob, int B, float* __restrict__ w) {
-    smk::pdl_sync();
     const int f = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
     if (f >= d.F) return;
     const int32_t* tri = d.faces + (size_t)f * 3;
@@ -85,7 +83,6 @@ mask_face_weights_kernel(MaskDev d, const float* __restrict__ tv, const float* _
 __global__ void __launch_bounds__(256)
 mask_points_kernel(MaskDev d, const float* __restrict__ tv, const int64_t* __restrict__ fidx, const float* __restrict__ bary,
                    int B, int N, int S, int64_t* __restrict__ npoints) {
-    smk::pdl_sync();
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long)B * N) return;
     const int b = (int)(i / N);
@@ -106,7 +103,6 @@ mask_points_kernel(MaskDev d, const float* __restrict__ tv, const int64_t* __res
 
 __global__ void __launch_bounds__(256)
 mask_scatter_kernel(const int64_t* __restrict__ npoints, const int64_t* __restrict__ rbound, int B, int N, int S, uint8_t* __restrict__ pm) {
-    smk::pdl_sync();
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long)B * N) return;
     const int b = (int)(i / N), j = (int)(i - (long)b * N);
@@ -119,7 +115,6 @@ mask_scatter_kernel(const int64_t* __restrict__ npoints, const int64_t* __restri
 __global__ void __launch_bounds__(256)
 mask_hmax_kernel(const float* __restrict__ hull, const float* __restrict__ centres, int B, int S, int wr,
                  float* __restrict__ th, float* __restrict__ tc) {
-    smk::pdl_sync();
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long)B * S * S) return;
     const int x = (int)(i % S);
@@ -140,7 +135,6 @@ __global__ void __launch_bounds__(256)
 mask_compose_kernel(const float* __restrict__ img, const float* __restrict__ th, const float* __restrict__ tc,
                     const uint8_t* __restrict__ pm, const float* __restrict__ extra, const float* __restrict__ rendered_mask,
                     const float* __restrict__ noise_mult, int B, int S, int wr, float* __restrict__ out) {
-    smk::pdl_sync();
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long)B * S * S) return;
     const int b = (int)(i / ((long)S * S));
@@ -190,7 +184,6 @@ __device__ __forceinline__ float u01(uint32_t r) { return (float)(r >> 8) * (1.0
 __global__ void __launch_bounds__(512)
 mask_sample_kernel(const float* __restrict__ w, int F, int N, float ratio_mul, const uint64_t* __restrict__ rng,
                    int64_t* __restrict__ fidx, float* __restrict__ bary, int64_t* __restrict__ rbound) {
-    smk::pdl_sync();
     extern __shared__ float cdf[];                      // [F]
     __shared__ float part[512];
     const int b = blockIdx.x, t = threadIdx.x, nt = blockDim.x;
@@ -240,7 +233,6 @@ mask_sample_kernel(const float* __restrict__ w, int F, int N, float ratio_mul, c
 // noise_mult[b,c,y,x] = N(0,1) * 0.05 + 1 (masking.py:84-86); centres[b,0,y,x] ~ Bernoulli(p) (masking.py:89-92)
 __global__ void __launch_bounds__(256)
 mask_rng_fill_kernel(int B, int S, float p_centre, const uint64_t* __restrict__ rng, float* __restrict__ noise, float* __restrict__ centres) {
-    smk::pdl_sync();
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     const long npx = (long)B * S * S;
     if (i >= npx) return;
@@ -260,7 +252,6 @@ mask_rng_fill_kernel(int B, int S, float p_centre, const uint64_t* __restrict__ 
 // rendered_mask = 1 - all(rendered == 0 over channels)   (demo.py:146)
 __global__ void __launch_bounds__(256)
 mask_rendered_kernel(const float* __restrict__ rendered, int B, int S, float* __restrict__ rmask) {
-    smk::pdl_sync();
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long)B * S * S) return;
     const int b = (int)(i / ((long)S * S)); const long pix = i - (long)b * S * S;
@@ -269,14 +260,13 @@ mask_rendered_kernel(const float* __restrict__ rendered, int B, int S, float* __
     rmask[i] = bg ? 0.f : 1.f;
 }
 
-__global__ void mask_rng_advance_kernel(uint64_t* rng) { smk::pdl_sync(); if (threadIdx.x == 0) rng[1] += 1; }
+__global__ void mask_rng_advance_kernel(uint64_t* rng) { if (threadIdx.x == 0) rng[1] += 1; }
 
 // transfer_pixels (masking.py:116-129): out[b, :, p2.y, p2.x] = img[b, :, p1.y, p1.x] for the first rbound[b] (or all) point
 // pairs; with duplicate targets the LAST pair in index order wins (the sequential semantics of the reference's indexed
 // assignment).  Pass 1: winner[target pixel] = max pair index (atomicMax); pass 2: every pixel copies from its winner.
 __global__ void __launch_bounds__(256)
 mask_transfer_winner_kernel(const int64_t* __restrict__ p2, const int64_t* __restrict__ rbound, int B, int N, int S, int* __restrict__ winner) {
-    smk::pdl_sync();
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long)B * N) return;
     const int b = (int)(i / N), j = (int)(i - (long)b * N);
@@ -288,7 +278,6 @@ mask_transfer_winner_kernel(const int64_t* __restrict__ p2, const int64_t* __res
 __global__ void __launch_bounds__(256)
 mask_transfer_copy_kernel(const float* __restrict__ img, const int64_t* __restrict__ p1, const int* __restrict__ winner, int B, int N, int S,
                           float* __restrict__ out) {
-    smk::pdl_sync();
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long)B * S * S) return;
     const int b = (int)(i / ((long)S * S)); const long pix = i - (long)b * S * S;
@@ -447,15 +436,7 @@ extern "C" int smk_masking_forward(const SmkMasking* h, const float* img, const 
     float* rmask = w.take<float>((size_t)npx);
     SMK_REQUIRE(rmask != nullptr, "smk_masking_forward: workspace carve-up failed");
     if (int rc = smk_masking_face_weights(h, trans_verts, base_prob, B, weights, ws, base, stream)) return rc;
-    {
-        static unsigned long long configured_mask = 0;
-        int dev = 0;
-        SMK_CHECK_CUDA(cudaGetDevice(&dev));
-        if (dev >= 64 || !(configured_mask & (1ull << dev))) {
-            SMK_CHECK_CUDA(cudaFuncSetAttribute(mask_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-            if (dev < 64) configured_mask |= 1ull << dev;
-        }
-    }
+    SMK_CHECK_CUDA(smk::set_max_dynamic_smem<mask_sample_kernel>(160 * 1024));
     SMK_TAG("mask_sample", 4.0 * B * d.F + 36.0 * B * N, 0.0, st);
     SMK_LAUNCH(mask_sample_kernel, dim3(B), dim3(512), (size_t)d.F * sizeof(float), st, (const float*)weights, d.F, N, ratio_mul,
                (const uint64_t*)rng_state, fidx, bary, rbound);

@@ -22,7 +22,6 @@ conv_gemm_kernel(ConvProblem p, int M) {
     const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
     const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
     const int HW = p.H * p.W;
-    pdl_sync();
 
     // per-thread A rows: r = tid/4 + 64*j, k-quad kq = tid%4
     const int kq = tid & 3;
@@ -143,7 +142,6 @@ __global__ void __launch_bounds__(256)
 dwconv3x3_kernel(const float* __restrict__ in, int B, int H, int W, int C, int stride, int pad, int Ho, int Wo,
                  const float* __restrict__ w9c, const float* __restrict__ scale, const float* __restrict__ bias,
                  float* __restrict__ out) {
-    pdl_sync();
     const int C4 = C >> 2;
     const long total = (long)B * Ho * Wo * C4;
     for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -182,7 +180,6 @@ dwconv3x3_px4_kernel(const float* __restrict__ in, int B, int H, int W, int C, i
     constexpr int PX = 4, NC = 3 + (PX - 1) * STRIDE;
     const int C4 = C >> 2, WG = (Wo + PX - 1) / PX;
     const long total = (long)B * Ho * WG * C4;
-    pdl_sync();
     for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
         int c4 = (int)(i % C4); long t = i / C4;
         int wg = (int)(t % WG); t /= WG; int oh = (int)(t % Ho); int b = (int)(t / Ho);
@@ -232,7 +229,6 @@ dwconv3x3_px4_kernel(const float* __restrict__ in, int B, int H, int W, int C, i
 __global__ void __launch_bounds__(256)
 gap_kernel(const float* __restrict__ feat, int HW, int C, float* __restrict__ pooled) {
     __shared__ float part[4][64];
-    pdl_sync();
     const int b = blockIdx.x, c = blockIdx.y * 64 + (threadIdx.x & 63), pl = threadIdx.x >> 6;
     float s = 0.f;
     if (c < C) {
@@ -249,7 +245,6 @@ gap_kernel(const float* __restrict__ feat, int HW, int C, float* __restrict__ po
 __global__ void __launch_bounds__(256)
 head_linear_kernel(const float* __restrict__ pooled, int C, const float* __restrict__ w, const float* __restrict__ bias,
                    int n_out, const uint8_t* __restrict__ codes, float* __restrict__ out) {
-    pdl_sync();
     const int b = blockIdx.x, lane = threadIdx.x & 31, o = blockIdx.y * 8 + (threadIdx.x >> 5);
     if (o >= n_out) return;
     const float* wr = w + (size_t)o * C;
@@ -276,7 +271,6 @@ struct GapHead { const float* feat[2]; const float* w[2]; const float* bias[2]; 
 __global__ void __launch_bounds__(256)
 gap_head_kernel(const __grid_constant__ GapHead g, int HW, int C) {
     extern __shared__ float pooled[];                 // [C]
-    pdl_sync();
     const int q = blockIdx.z, b = blockIdx.x;
     const int n_out = g.n_out[q];
     if ((int)blockIdx.y * 32 >= n_out) return;
@@ -323,7 +317,6 @@ stem_conv_kernel(const float* __restrict__ img, int B, int H, int W, int Ho, int
     for (int i = threadIdx.x; i < 27 * 16; i += blockDim.x) sw[i] = w[i];
     if (threadIdx.x < 16) { ss[threadIdx.x] = scale[threadIdx.x]; sb[threadIdx.x] = bias[threadIdx.x]; }
     __syncthreads();
-    pdl_sync();
     long pix = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (pix >= (long)B * Ho * Wo) return;
     int ow = (int)(pix % Wo); long t = pix / Wo; int oh = (int)(t % Ho); int b = (int)(t / Ho);
@@ -370,7 +363,6 @@ stem_conv3_kernel(const float* __restrict__ img, int B, int H, int W, int Ho, in
     const int oh = blockIdx.x % Ho, b = blockIdx.x / Ho;
     for (int i = threadIdx.x; i < 27 * 48; i += blockDim.x) { int tap = i / 48, gc = i % 48; sw[i] = p.w[gc / 16][tap * 16 + gc % 16]; }
     if (threadIdx.x < 48) { ss[threadIdx.x] = p.scale[threadIdx.x / 16][threadIdx.x % 16]; sb[threadIdx.x] = p.bias[threadIdx.x / 16][threadIdx.x % 16]; }
-    pdl_sync();                                    // weights are constants; the image and the outputs are not
     {   // stage rows: element iw of row (c,ky) lands at sin_[c*3+ky][4 + iw] so 16-byte stores stay aligned; halo columns zeroed
         const int W4 = W >> 2;
         for (int i = threadIdx.x; i < 9 * W4; i += blockDim.x) {
@@ -419,7 +411,6 @@ __global__ void __launch_bounds__(256)
 maxpool2x2_kernel(const float* __restrict__ in, int ld_in, int B, int H, int W, int C, float* __restrict__ out) {
     const int Ho = H >> 1, Wo = W >> 1, C4 = C >> 2;
     const long total = (long)B * Ho * Wo * C4;
-    pdl_sync();
     for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
         int c4 = (int)(i % C4); long pix = i / C4;
         int ow = (int)(pix % Wo); long t = pix / Wo; int oh = (int)(t % Ho); int b = (int)(t / Ho);
@@ -436,7 +427,6 @@ maxpool2x2_kernel(const float* __restrict__ in, int ld_in, int B, int H, int W, 
 __global__ void __launch_bounds__(256)
 nchw_to_nhwc_pad_kernel(const float* __restrict__ in, int B, int C, int HW, int Cp, int round, float* __restrict__ out) {
     // thread = (pixel, channel quad), quads of a pixel in adjacent lanes: every warp stores 512 contiguous bytes
-    pdl_sync();
     const int Q = Cp >> 2;
     long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long)B * HW * Q) return;
@@ -459,7 +449,6 @@ conv1x1_sigmoid_kernel(const float* __restrict__ in, int B, int HW, int Cin, con
     for (int i = threadIdx.x; i < Cin * Cout; i += blockDim.x) sw[i] = w[i];
     for (int i = threadIdx.x; i < Cout; i += blockDim.x) sw[Cin * Cout + i] = bias[i];
     __syncthreads();
-    pdl_sync();
     long pix = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (pix >= (long)B * HW) return;
     int b = (int)(pix / HW); int r = (int)(pix - (long)b * HW);
@@ -599,7 +588,6 @@ stem_ds_kernel(const float* __restrict__ img, int H, int W, int Hs, int Ws, int 
         sB[tid] = p.stem_s[tid]; sB[16 + tid] = p.stem_b[tid]; sB[32 + tid] = p.dw_s[tid]; sB[48 + tid] = p.dw_b[tid];
         sB[64 + tid] = p.pw_s[tid]; sB[80 + tid] = p.pw_b[tid];
     }
-    pdl_sync();                                            // weights are constants; the image and the outputs are not
     // ix0 and W are even: one 8-byte load fetches an (even, odd) column pair — exactly the de-interleaved layout.
     // 19 pairs per row cover the 37 columns (the odd half of the last pair is never read).
     constexpr int SD_PAIRS = (SD_PR + 1) / 2;

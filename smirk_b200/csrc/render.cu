@@ -43,7 +43,6 @@ __device__ __forceinline__ float pix_to_ndc(int i, int S) {
 __global__ void __launch_bounds__(256)
 project_kernel(const float* __restrict__ pts, const float* __restrict__ cam, int B, int L, int out_dim,
                float* __restrict__ out) {
-    smk::pdl_sync();
     long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long)B * L) return;
     int b = (int)(i / L);
@@ -60,7 +59,6 @@ project_kernel(const float* __restrict__ pts, const float* __restrict__ cam, int
 __global__ void __launch_bounds__(128)
 submesh_kernel(RenderDev d, const float* __restrict__ verts, const float* __restrict__ tverts, int B,
                float* __restrict__ rv /*[B][NM][3]*/, float* __restrict__ normals /*[B][NM][3]*/) {
-    smk::pdl_sync();
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     int b = blockIdx.y;
     if (i >= d.NM) return;
@@ -92,7 +90,6 @@ submesh_kernel(RenderDev d, const float* __restrict__ verts, const float* __rest
 __global__ void __launch_bounds__(128)
 tri_setup_kernel(RenderDev d, const float* __restrict__ rv, int B, float* __restrict__ recs /*[B][F][REC]*/,
                  uint32_t* __restrict__ ranges /*[B][F]*/) {
-    smk::pdl_sync();
     int f = blockIdx.x * blockDim.x + threadIdx.x;
     int b = blockIdx.y;
     if (f >= d.F) return;
@@ -144,7 +141,6 @@ raster_tile_kernel(RenderDev d, const float* __restrict__ recs, const uint32_t* 
     const uint32_t tx = blockIdx.x, ty = blockIdx.y;
     if (tid == 0) s_count = 0;
     __syncthreads();
-    smk::pdl_sync();
     // -- bin: compact the ids of triangles whose conservative tile range covers this tile
     //    (4 packed ranges per thread per pass: one 16-byte load, one shared atomic per warp)
     const uint4* rg4 = reinterpret_cast<const uint4*>(ranges + (size_t)b * d.F);

@@ -31,7 +31,6 @@ struct MinMax { unsigned int mn, mx; };
 // per-frame min / max of the uint8 source over all channels (skimage clips per warp() call = per whole image)
 __global__ void __launch_bounds__(256)
 u8_minmax_kernel(const uint8_t* __restrict__ src, size_t n_per_frame, MinMax* __restrict__ mm) {
-    smk::pdl_sync();
     const int b = blockIdx.y;
     const uint8_t* s = src + (size_t)b * n_per_frame;
     unsigned int mn = 255u, mx = 0u;
@@ -55,7 +54,6 @@ u8_minmax_kernel(const uint8_t* __restrict__ src, size_t n_per_frame, MinMax* __
 }
 
 __global__ void minmax_init_kernel(MinMax* mm, int B) {
-    smk::pdl_sync();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < B) { mm[i].mn = 255u; mm[i].mx = 0u; }
 }
@@ -63,7 +61,6 @@ __global__ void minmax_init_kernel(MinMax* mm, int B) {
 // rendered float [B,3,S,S] -> uint8 [B,S,S,3]: (x * 255.0f).astype(uint8) in float32 like numpy (demo_video.py:148)
 __global__ void __launch_bounds__(256)
 f32chw_to_u8hwc_kernel(const float* __restrict__ in, int B, int S, uint8_t* __restrict__ out) {
-    smk::pdl_sync();
     const size_t n = (size_t)B * S * S;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
         const size_t b = i / ((size_t)S * S), p = i - b * (size_t)S * S;
@@ -82,7 +79,6 @@ template <bool OUT_F32>
 __global__ void __launch_bounds__(256)
 warp_bilinear_kernel(const uint8_t* __restrict__ src, int Hs, int Ws, const double* __restrict__ M, const MinMax* __restrict__ mm,
                      int Hd, int Wd, int swap_rb, void* __restrict__ dst) {
-    smk::pdl_sync();
     const int b = blockIdx.z;
     const int tfc = blockIdx.x * 32 + (threadIdx.x & 31), tfr = blockIdx.y * 8 + (threadIdx.x >> 5);
     if (tfc >= Wd || tfr >= Hd) return;

@@ -23,7 +23,6 @@
 #include "gemm_tc.cuh"
 #include "xdw_tc.cuh"
 #include "tc_ptx.cuh"
-#include <cuda.h>
 
 namespace smk {
 namespace {
@@ -118,7 +117,6 @@ xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
         fence_barrier_init();
     }
     __syncthreads();
-    pdl_sync();
 
     if (warp == NUM_WORKERS / 32) {
         if (lane == 0) {
@@ -336,25 +334,19 @@ xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
     }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn g_encode = nullptr;
-
-int load_encoder() {
-    if (g_encode) return 0;
-    cudaDriverEntryPointQueryResult q;
-    void* fn = nullptr;
-    SMK_CHECK_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q));
-    SMK_REQUIRE(fn && q == cudaDriverEntryPointSuccess, "cuTensorMapEncodeTiled not available from the driver");
-    g_encode = (EncodeTiledFn)fn;
+template <int STRIDE, int X3>
+int launch(const XdwMaps& mp, const XdwArgs& a, int grid, cudaStream_t st) {
+    constexpr size_t smem = (size_t)STAGES * (STAGE_BYTES + (X3 ? B_BYTES : 0)) + E_BYTES + PAR_BYTES + 1024 + 256;  // 3xTF32: + the weight tails
+    static_assert(X3 || 2 * (smem + 1024) <= 228 * 1024, "two CTAs per SM");
+    SMK_CHECK_CUDA((set_max_dynamic_smem<xdw_kernel<STRIDE, X3>>((int)smem)));
+    SMK_LAUNCH((xdw_kernel<STRIDE, X3>), dim3(grid), dim3(NUM_THREADS), smem, st, mp, a);
+    SMK_CHECK_LAUNCH();
     return 0;
 }
 
 }  // namespace
 
 int xdw_conv(const XdwConv& p, cudaStream_t st, const XdwConv* p2) {
-    if (int rc = load_encoder()) return rc;
     const int nprob = p2 ? 2 : 1;
     SMK_REQUIRE(p.stride == 1 || p.stride == 2, "xdw_conv: stride must be 1 or 2");
     SMK_REQUIRE(p.Cin % 4 == 0 && p.mid % 4 == 0, "xdw_conv: Cin and mid must be multiples of 4");
@@ -367,30 +359,10 @@ int xdw_conv(const XdwConv& p, cudaStream_t st, const XdwConv* p2) {
     XdwArgs a{};
     for (int g = 0; g < nprob; ++g) {
         const XdwConv& q = g ? *p2 : p;
-        {
-            cuuint64_t dims[4] = {(cuuint64_t)q.Cin, (cuuint64_t)q.W, (cuuint64_t)q.H, (cuuint64_t)q.B};
-            cuuint64_t strides[3] = {(cuuint64_t)q.Cin * 4, (cuuint64_t)q.W * q.Cin * 4, (cuuint64_t)q.H * q.W * q.Cin * 4};
-            cuuint32_t box[4] = {(cuuint32_t)BK, (cuuint32_t)WIN, 8, 1};
-            cuuint32_t estr[4] = {1, 1, 1, 1};
-            CUresult r = g_encode(&mp.x[g], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)q.x, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            SMK_REQUIRE(r == CUDA_SUCCESS, "xdw_conv: cuTensorMapEncodeTiled(x) failed (%d): B=%d H=%d W=%d Cin=%d", (int)r, q.B, q.H, q.W, q.Cin);
-        }
-        {
-            cuuint64_t dims[2] = {(cuuint64_t)q.Cin, (cuuint64_t)q.mid};
-            cuuint64_t strides[1] = {(cuuint64_t)q.Cin * 4};
-            cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)NC};
-            cuuint32_t estr[2] = {1, 1};
-            CUresult r = g_encode(&mp.w[g], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)q.w1t, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            SMK_REQUIRE(r == CUDA_SUCCESS, "xdw_conv: cuTensorMapEncodeTiled(w1) failed (%d): mid=%d Cin=%d", (int)r, q.mid, q.Cin);
-            mp.wlo[g] = mp.w[g];
-            if (q.w1t_lo) {
-                r = g_encode(&mp.wlo[g], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)q.w1t_lo, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-                SMK_REQUIRE(r == CUDA_SUCCESS, "xdw_conv: cuTensorMapEncodeTiled(w1 tails) failed (%d)", (int)r);
-            }
-        }
+        if (int rc = encode_nhwc(&mp.x[g], q.x, q.B, q.H, q.W, q.Cin, q.Cin, WIN, 8, "xdw_conv(x)")) return rc;
+        if (int rc = encode_2d(&mp.w[g], q.w1t, (uint64_t)q.mid, (uint64_t)q.Cin, (uint64_t)q.Cin, NC, "xdw_conv(w1)")) return rc;
+        mp.wlo[g] = mp.w[g];
+        if (q.w1t_lo) { if (int rc = encode_2d(&mp.wlo[g], q.w1t_lo, (uint64_t)q.mid, (uint64_t)q.Cin, (uint64_t)q.Cin, NC, "xdw_conv(w1 tails)")) return rc; }
         a.scale1[g] = q.scale1; a.bias1[g] = q.bias1; a.wdw[g] = q.wdw; a.scale2[g] = q.scale2; a.bias2[g] = q.bias2; a.out[g] = q.out;
     }
     if (nprob == 1) {
@@ -398,9 +370,8 @@ int xdw_conv(const XdwConv& p, cudaStream_t st, const XdwConv* p2) {
         a.scale1[1] = a.scale1[0]; a.bias1[1] = a.bias1[0]; a.wdw[1] = a.wdw[0]; a.scale2[1] = a.scale2[0]; a.bias2[1] = a.bias2[0]; a.out[1] = a.out[0];
     }
     // Resident CTAs to aim for: one per SM (two would fit) leaves room on every SM for the other backbones' and batches'
-    // kernels of the concurrent pipeline.  SMK_XDW_SLOTS overrides the target.
-    static const int slots_env = []() { const char* e = getenv("SMK_XDW_SLOTS"); return e ? atoi(e) : 0; }();
-    const int slots = slots_env > 0 ? slots_env : num_sms();
+    // kernels of the concurrent pipeline.
+    const int slots = num_sms();
     a.H = p.H; a.W = p.W; a.Ho = Ho; a.Wo = Wo; a.mid = p.mid; a.nkb = cdiv(p.Cin, BK); a.nchunks = cdiv(p.mid, NC);
     {   // split the channel chunks over enough CTAs to fill the resident slots
         const long tiles = (long)nprob * cdiv(Wo, TO) * cdiv(Ho, TO) * p.B;
@@ -411,19 +382,6 @@ int xdw_conv(const XdwConv& p, cudaStream_t st, const XdwConv* p2) {
     a.pad = p.stride == 1 ? 1 : 0;
     a.tiles_x = cdiv(Wo, TO); a.tiles_y = cdiv(Ho, TO);
     a.round_out = p.round_out;
-    constexpr size_t smem = (size_t)STAGES * STAGE_BYTES + E_BYTES + PAR_BYTES + 1024 + 256;
-    constexpr size_t smem3t = (size_t)STAGES * (STAGE_BYTES + B_BYTES) + E_BYTES + PAR_BYTES + 1024 + 256;  // 3xTF32: + the weight tails
-    static_assert(2 * (smem + 1024) <= 228 * 1024, "two CTAs per SM");
-    static unsigned long long configured_mask = 0;       // per-device attribute, see gemm_tc.cu
-    int dev = 0;
-    SMK_CHECK_CUDA(cudaGetDevice(&dev));
-    if (dev >= 64 || !(configured_mask & (1ull << dev))) {
-        SMK_CHECK_CUDA(cudaFuncSetAttribute(xdw_kernel<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        SMK_CHECK_CUDA(cudaFuncSetAttribute(xdw_kernel<2, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        SMK_CHECK_CUDA(cudaFuncSetAttribute(xdw_kernel<1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3t));
-        SMK_CHECK_CUDA(cudaFuncSetAttribute(xdw_kernel<2, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3t));
-        if (dev < 64) configured_mask |= 1ull << dev;
-    }
     {
         const double px_in = (double)nprob * p.B * p.H * p.W, px_out = (double)nprob * p.B * Ho * Wo;
         const char* tag = p.w1t_lo ? "xdw_fused_tc3x" : "xdw_fused_tc";
@@ -437,17 +395,10 @@ int xdw_conv(const XdwConv& p, cudaStream_t st, const XdwConv* p2) {
         auto group = [](int ncols, int nrows) { const int n_rg = std::min(32 / ncols, nrows); return (unsigned)((nrows + n_rg - 1) / n_rg) | (unsigned)n_rg << 4; };
         a.geom = group(TO, TO) | group(TO, nrows_e) << 8 | group(ncols_e, TO) << 16 | group(ncols_e, nrows_e) << 24;
     }
-    dim3 grid((unsigned)std::min(a.n_items, p.w1t_lo ? std::min(slots, num_sms()) : slots));      // persistent: (up to) 2 CTAs per SM
-    { int v = (int)grid.x; a.d_grp = v % a.groups; v /= a.groups; a.d_tx = v % a.tiles_x; v /= a.tiles_x; a.d_ty = v % a.tiles_y; a.d_img = v / a.tiles_y; }
-    if (p.w1t_lo) {
-        if (p.stride == 1) SMK_LAUNCH((xdw_kernel<1, 2>), dim3(grid), dim3(NUM_THREADS), smem3t, st, mp, a);
-        else SMK_LAUNCH((xdw_kernel<2, 2>), dim3(grid), dim3(NUM_THREADS), smem3t, st, mp, a);
-    } else {
-        if (p.stride == 1) SMK_LAUNCH((xdw_kernel<1, 0>), dim3(grid), dim3(NUM_THREADS), smem, st, mp, a);
-        else SMK_LAUNCH((xdw_kernel<2, 0>), dim3(grid), dim3(NUM_THREADS), smem, st, mp, a);
-    }
-    SMK_CHECK_LAUNCH();
-    return 0;
+    const int grid = std::min(a.n_items, slots);         // persistent
+    { int v = grid; a.d_grp = v % a.groups; v /= a.groups; a.d_tx = v % a.tiles_x; v /= a.tiles_x; a.d_ty = v % a.tiles_y; a.d_img = v / a.tiles_y; }
+    if (p.w1t_lo) return p.stride == 1 ? launch<1, 2>(mp, a, grid, st) : launch<2, 2>(mp, a, grid, st);
+    return p.stride == 1 ? launch<1, 0>(mp, a, grid, st) : launch<2, 0>(mp, a, grid, st);
 }
 
 }  // namespace smk

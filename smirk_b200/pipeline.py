@@ -23,7 +23,6 @@ Captured graphs snapshot the packed weights and workspaces they were recorded wi
 (``rec["keep"]``); after changing weights, ``precision`` or devices call ``refresh()`` to re-capture.
 """
 import copy
-import os
 
 import torch
 
@@ -273,7 +272,7 @@ class SmirkPipeline:
         import torch.distributed as dist
         ws, rank = dist.get_world_size(self._gather_group), dist.get_rank(self._gather_group)
         ok, sizes, offsets, shard, mine, bufs = True, [], [], 0, None, []
-        pack = int(os.environ.get("SMK_GATHER_PACK", "1" if ws > 2 else "0")) != 0
+        pack = ws > 2
         try:
             rec = self.capture(B)
             assert all(rec["out"][k].is_contiguous() for k in self._gather_keys)
