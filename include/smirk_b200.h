@@ -79,6 +79,16 @@ size_t smk_flame_workspace_bytes(const SmkFlame* h, int B);
 int smk_flame_forward(const SmkFlame* h, const float* betas, const float* full_pose, const float* eyelid,
                       int B, float* verts, float* lmk_fan, float* lmk_fan3d, float* lmk_mp,
                       float* joints, int32_t* dyn_idx, void* ws, size_t ws_bytes, void* stream);
+/* Backward of smk_flame_forward: the gradient torch autograd takes through FLAME.forward for betas,
+ * full_pose and eyelid.  dyn_idx is the forward's contour row (required).  Upstream gradients g_verts
+ * [B,V,3], g_lmk_fan [B,68,3], g_lmk_fan3d [B,68,3], g_lmk_mp [B,105,3]: each may be NULL (= zero).
+ * Outputs are written, not accumulated: g_betas [B,n_betas], g_full_pose [B,15], g_eyelid [B,2] (may be
+ * NULL).  eyelid may be NULL.  Deterministic (no atomics).  Needs n_betas <= 350.                    */
+size_t smk_flame_backward_workspace_bytes(const SmkFlame* h, int B);
+int smk_flame_backward(const SmkFlame* h, const float* betas, const float* full_pose, const float* eyelid,
+                       int B, const int32_t* dyn_idx,
+                       const float* g_verts, const float* g_lmk_fan, const float* g_lmk_fan3d, const float* g_lmk_mp,
+                       float* g_betas, float* g_full_pose, float* g_eyelid, void* ws, size_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Renderer — replaces Renderer.forward/render/rasterize (src/renderer/renderer.py:100-207,239-250),
@@ -107,6 +117,18 @@ int smk_renderer_forward(const SmkRenderer* h, const float* verts, const float* 
                          float* normals, void* ws, size_t ws_bytes, void* stream);
 /* Orthographic projection of landmark sets (renderer.py:104-108): pts [B,L,3] -> out [B,L,2]. */
 int smk_project_points(const float* pts, const float* cam, int B, int L, float* out_xy, void* stream);
+/* Backward of smk_renderer_forward for verts and cam, from the forward's pix_to_face, bary and normals.
+ * The rasteriser part is pytorch3d's rasterize_meshes backward (blur 0, K = 1, no perspective
+ * correction, no zbuf / dists gradient).  g_rendered [B,3,S,S] and g_tverts [B,n_verts,3] may be NULL
+ * (= zero).  Outputs are written: g_verts [B,n_verts,3], g_cam [B,3].  Deterministic (no atomics).   */
+size_t smk_renderer_backward_workspace_bytes(const SmkRenderer* h, int B);
+int smk_renderer_backward(const SmkRenderer* h, const float* verts, const float* cam, int B,
+                          const int64_t* pix_to_face, const float* bary, const float* normals,
+                          const float* g_rendered, const float* g_tverts, float* g_verts, float* g_cam,
+                          void* ws, size_t ws_bytes, void* stream);
+/* Backward of smk_project_points: g_xy [B,L,2] -> g_pts [B,L,3], g_cam [B,3] (written). */
+int smk_project_points_backward(const float* pts, const float* cam, int B, int L, const float* g_xy,
+                                float* g_pts, float* g_cam, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * SmirkEncoder — replaces SmirkEncoder.forward (src/smirk_encoder.py:123-133): three timm

@@ -49,6 +49,8 @@ SYMBOLS = ["smk_version", "smk_last_error", "smk_launch_count", "smk_profiler_en
            "smk_flame_create", "smk_flame_destroy", "smk_flame_workspace_bytes", "smk_flame_forward",
            "smk_renderer_create", "smk_renderer_destroy", "smk_renderer_workspace_bytes", "smk_renderer_forward",
            "smk_project_points",
+           "smk_flame_backward_workspace_bytes", "smk_flame_backward", "smk_renderer_backward_workspace_bytes",
+           "smk_renderer_backward", "smk_project_points_backward",
            "smk_encoder_create", "smk_encoder_destroy", "smk_encoder_workspace_bytes", "smk_encoder_forward",
            "smk_generator_create", "smk_generator_destroy", "smk_generator_workspace_bytes", "smk_generator_forward",
            "smk_debug_conv_f32", "smk_debug_conv_tc", "smk_debug_reflect_halo", "smk_debug_xdw", "smk_debug_stem_ds", "smk_debug_gemm_tc3x", "smk_debug_xdw3x", "smk_debug_conv3_win",
@@ -90,6 +92,11 @@ def lib():
     L.smk_renderer_workspace_bytes.argtypes = [vp, i]
     L.smk_renderer_forward.argtypes = [vp, vp, vp, i, vp, vp, vp, vp, vp, vp, vp, sz, vp]
     L.smk_project_points.argtypes = [vp, vp, i, i, vp, vp]
+    L.smk_flame_backward_workspace_bytes.argtypes = [vp, i]
+    L.smk_flame_backward.argtypes = [vp, vp, vp, vp, i, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
+    L.smk_renderer_backward_workspace_bytes.argtypes = [vp, i]
+    L.smk_renderer_backward.argtypes = [vp, vp, vp, i, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
+    L.smk_project_points_backward.argtypes = [vp, vp, i, i, vp, vp, vp, vp]
     L.smk_encoder_create.argtypes = [C.POINTER(SmkEncoderDesc), C.POINTER(vp)]
     L.smk_encoder_destroy.argtypes = [vp]
     L.smk_encoder_workspace_bytes.argtypes = [vp, i]

@@ -266,11 +266,300 @@ raster_tile_kernel(RenderDev d, const float* __restrict__ recs, const uint32_t* 
     }
 }
 
+// =================================================================================================
+// Backward: the gradient torch autograd takes through Renderer.forward (renderer.py:100-207,239-250,
+// util.py:30-78) for verts and cam, with pytorch3d's rasterize_meshes backward for blur 0, K = 1, no
+// perspective correction and no clipping (zbuf / dists carry no gradient: the reference uses neither).
+// Four launches, no atomics, fixed-order sums:
+//   render_bwd_face_kernel    one warp per face scans the face's conservative pixel range against the
+//                             forward's pix_to_face: shading -> barycentrics -> raster-space x/y of the
+//                             three corners, and the interpolated-normal gradient of the three corners.
+//   render_bwd_normal_kernel  per sub-mesh vertex: gathers those over the CSR vertex -> face adjacency and
+//                             backpropagates F.normalize(eps=1e-6) (util.py:62).
+//   render_bwd_vertex_kernel  per mesh vertex: the cross products of util.py:52-57, the raster-space and
+//                             transformed_vertices gradients through batch_orth_proj (util.py:64-78).
+//   render_bwd_cam_kernel     per face: fixed-order reduction of the camera gradient.
+constexpr int kFG = 15;                     // per-face gradient: x,y of 3 corners + normal of 3 corners
+
+__device__ __forceinline__ void tri_raster_xy(const RenderDev& d, const float* vb, const int32_t* mask_ids,
+                                              float s, float tx, float ty, int f, float* x, float* y) {
+    // raster-space (pytorch3d NDC) x/y of the face's corners, bitwise as project_kernel + submesh_kernel
+    for (int k = 0; k < 3; ++k) {
+        const float* p = vb + (size_t)mask_ids[d.faces[(size_t)f * 3 + k]] * 3;
+        x[k] = -__fmul_rn(s, __fadd_rn(p[0], tx));
+        y[k] = __fmul_rn(s, __fadd_rn(p[1], ty));
+    }
+}
+
+__global__ void __launch_bounds__(128)
+render_bwd_face_kernel(RenderDev d, Lights lights, const float* __restrict__ verts, const float* __restrict__ cam,
+                       const int64_t* __restrict__ p2f, const float* __restrict__ bary, const float* __restrict__ normals,
+                       const float* __restrict__ g_rendered, int B, float* __restrict__ gface /*[B][F][15]*/) {
+    const int lane = threadIdx.x & 31;
+    const int f = blockIdx.x * 4 + (threadIdx.x >> 5), b = blockIdx.y;
+    if (f >= d.F) return;
+    float acc[kFG];
+#pragma unroll
+    for (int q = 0; q < kFG; ++q) acc[q] = 0.f;
+    const float s = cam[b * 3], tx = cam[b * 3 + 1], ty = cam[b * 3 + 2];
+    float x[3], y[3];
+    tri_raster_xy(d, verts + (size_t)b * d.V * 3, d.mask_ids, s, tx, ty, f, x, y);
+    const float xmin = fminf(x[0], fminf(x[1], x[2])), xmax = fmaxf(x[0], fmaxf(x[1], x[2]));
+    const float ymin = fminf(y[0], fminf(y[1], y[2])), ymax = fmaxf(y[0], fmaxf(y[1], y[2]));
+    const float hs = 0.5f * d.S;                 // the pixel range of tri_setup_kernel (a superset of the coverage)
+    const float fx_lo = floorf((1.f - xmax) * hs - 0.5f) - 1.f, fx_hi = ceilf((1.f - xmin) * hs - 0.5f) + 1.f;
+    const float fy_lo = floorf((1.f - ymax) * hs - 0.5f) - 1.f, fy_hi = ceilf((1.f - ymin) * hs - 0.5f) + 1.f;
+    if (g_rendered && isfinite(xmin) && isfinite(xmax) && isfinite(ymin) && isfinite(ymax) &&
+        fx_hi >= 0.f && fy_hi >= 0.f && fx_lo <= d.S - 1 && fy_lo <= d.S - 1) {
+        const int xl = (int)fmaxf(fx_lo, 0.f), xh = (int)fminf(fx_hi, (float)(d.S - 1));
+        const int yl = (int)fmaxf(fy_lo, 0.f), yh = (int)fminf(fy_hi, (float)(d.S - 1));
+        const int nx = xh - xl + 1, npx = nx * (yh - yl + 1);
+        const int64_t me = (int64_t)b * d.F + f;
+        const size_t plane = (size_t)d.S * d.S;
+        const float* nb = normals + (size_t)b * d.NM * 3;
+        const int32_t* tri = d.faces + (size_t)f * 3;
+        float n[3][3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+#pragma unroll
+            for (int c = 0; c < 3; ++c) n[k][c] = nb[(size_t)tri[k] * 3 + c];
+        // den = edge(v2; v0, v1) + 1e-8, as tri_setup_kernel
+        const float den = __fadd_rn(edge_nf(x[2], y[2], x[0], y[0], x[1], y[1]), kEps);
+        const float col = 180.0f / 255.0f;
+        for (int q = lane; q < npx; q += 32) {
+            const int xi = xl + q % nx, yi = yl + q / nx;
+            const size_t pix = (size_t)yi * d.S + xi;
+            if (p2f[(size_t)b * plane + pix] != me) continue;
+            const float* gr = g_rendered + (size_t)b * 3 * plane + pix;
+            const float G = (gr[0] + gr[plane]) + gr[2 * plane];          // the three channels are the same value
+            const float* bw = bary + ((size_t)b * plane + pix) * 3;
+            const float w[3] = {bw[0], bw[1], bw[2]};
+            // forward recomputed in raster_tile_kernel's order (so the clamp masks match)
+            const float alb = __fadd_rn(__fadd_rn(__fmul_rn(w[0], col), __fmul_rn(w[1], col)), __fmul_rn(w[2], col));
+            float nn[3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) nn[c] = __fadd_rn(__fadd_rn(__fmul_rn(w[0], n[0][c]), __fmul_rn(w[1], n[1][c])), __fmul_rn(w[2], n[2][c]));
+            float sum = 0.f, gnn[3] = {0.f, 0.f, 0.f};
+            bool pass[5];
+#pragma unroll
+            for (int l = 0; l < 5; ++l) {
+                float dot = __fadd_rn(__fadd_rn(__fmul_rn(nn[0], lights.dir[l][0]), __fmul_rn(nn[1], lights.dir[l][1])),
+                                      __fmul_rn(nn[2], lights.dir[l][2]));
+                pass[l] = dot >= 0.f && dot <= 1.f;               // torch.clamp passes the gradient on [0, 1] inclusive
+                dot = fminf(fmaxf(dot, 0.f), 1.f);
+                sum = __fadd_rn(sum, __fmul_rn(dot, 1.7f));
+            }
+            // rendered = albedo * shading, shading = mean_l(1.7 clamp(n.l))           renderer.py:158-166,239-250
+            const float g_alb = G * (sum / 5.0f);
+            const float g_dot = G * alb * (1.7f / 5.0f);
+#pragma unroll
+            for (int l = 0; l < 5; ++l)
+                if (pass[l])
+#pragma unroll
+                    for (int c = 0; c < 3; ++c) gnn[c] += g_dot * lights.dir[l][c];
+            // interpolation (renderer.py:194-207): the albedo is the constant 180/255 at every corner
+            float gw[3];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                gw[k] = g_alb * col + ((gnn[0] * n[k][0] + gnn[1] * n[k][1]) + gnn[2] * n[k][2]);
+#pragma unroll
+                for (int c = 0; c < 3; ++c) acc[6 + 3 * k + c] += w[k] * gnn[c];
+            }
+            // w_k = e_k / den with e0 = edge(p; v1, v2), e1 = edge(p; v2, v0), e2 = edge(p; v0, v1)
+            // edge(p; a, b) = (px-ax)(by-ay) - (py-ay)(bx-ax): d/da = (py-by, bx-px), d/db = (ay-py, px-ax)
+            const float xf = pix_to_ndc(d.S - 1 - xi, d.S), yf = pix_to_ndc(d.S - 1 - yi, d.S);
+            const float ge[3] = {gw[0] / den, gw[1] / den, gw[2] / den};
+            const float gden = -((gw[0] * w[0] + gw[1] * w[1]) + gw[2] * w[2]) / den;
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                const int a = (k + 1) % 3, c = (k + 2) % 3;            // e_k = edge(p; v_a, v_c)
+                acc[2 * a + 0] += ge[k] * (yf - y[c]);
+                acc[2 * a + 1] += ge[k] * (x[c] - xf);
+                acc[2 * c + 0] += ge[k] * (y[a] - yf);
+                acc[2 * c + 1] += ge[k] * (xf - x[a]);
+            }
+            // den = edge(v2; v0, v1): d/dv2 = (y1-y0, x0-x1), d/dv0 = (y2-y1, x1-x2), d/dv1 = (y0-y2, x2-x0)
+            acc[4] += gden * (y[1] - y[0]); acc[5] += gden * (x[0] - x[1]);
+            acc[0] += gden * (y[2] - y[1]); acc[1] += gden * (x[1] - x[2]);
+            acc[2] += gden * (y[0] - y[2]); acc[3] += gden * (x[2] - x[0]);
+        }
+    }
+#pragma unroll
+    for (int q = 0; q < kFG; ++q) {
+        float v = acc[q];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        acc[q] = v;
+    }
+    if (lane < kFG) {
+        float v = acc[0];
+#pragma unroll
+        for (int q = 1; q < kFG; ++q) if (lane == q) v = acc[q];
+        gface[((size_t)b * d.F + f) * kFG + lane] = v;
+    }
+}
+
+// raw (un-normalised) vertex normal of sub-mesh vertex i, as submesh_kernel
+__device__ __forceinline__ void raw_normal(const RenderDev& d, const float* vb, int i, float* n) {
+    float nx = 0.f, ny = 0.f, nz = 0.f;
+    for (int e = d.adj_ptr[i]; e < d.adj_ptr[i + 1]; ++e) {
+        int code = d.adj[e], f = code >> 2, c = code & 3;
+        const int32_t* tri = d.faces + (size_t)f * 3;
+        const float* p = vb + (size_t)d.mask_ids[tri[c]] * 3;
+        const float* q1 = vb + (size_t)d.mask_ids[tri[(c + 1) % 3]] * 3;
+        const float* q2 = vb + (size_t)d.mask_ids[tri[(c + 2) % 3]] * 3;
+        float ax = q1[0] - p[0], ay = q1[1] - p[1], az = q1[2] - p[2];
+        float bx = q2[0] - p[0], by = q2[1] - p[1], bz = q2[2] - p[2];
+        nx += __fsub_rn(__fmul_rn(ay, bz), __fmul_rn(az, by));
+        ny += __fsub_rn(__fmul_rn(az, bx), __fmul_rn(ax, bz));
+        nz += __fsub_rn(__fmul_rn(ax, by), __fmul_rn(ay, bx));
+    }
+    n[0] = nx; n[1] = ny; n[2] = nz;
+}
+
+__global__ void __launch_bounds__(128)
+render_bwd_normal_kernel(RenderDev d, const float* __restrict__ verts, const float* __restrict__ gface, int B,
+                         float* __restrict__ graw /*[B][NM][3]*/, float* __restrict__ grv /*[B][NM][2]*/) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+    if (i >= d.NM) return;
+    float gxy[2] = {0.f, 0.f}, gn[3] = {0.f, 0.f, 0.f};
+    for (int e = d.adj_ptr[i]; e < d.adj_ptr[i + 1]; ++e) {
+        const int code = d.adj[e], f = code >> 2, c = code & 3;
+        const float* g = gface + ((size_t)b * d.F + f) * kFG;
+        gxy[0] += g[2 * c]; gxy[1] += g[2 * c + 1];
+        gn[0] += g[6 + 3 * c]; gn[1] += g[6 + 3 * c + 1]; gn[2] += g[6 + 3 * c + 2];
+    }
+    grv[((size_t)b * d.NM + i) * 2 + 0] = gxy[0];
+    grv[((size_t)b * d.NM + i) * 2 + 1] = gxy[1];
+    // y = x / max(||x||, 1e-6): g_x = g/den - x (x.g) / (den^2 ||x||) while ||x|| >= 1e-6
+    float n[3];
+    raw_normal(d, verts + (size_t)b * d.V * 3, i, n);
+    const float len = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(n[0], n[0]), __fmul_rn(n[1], n[1])), __fmul_rn(n[2], n[2])));
+    const float den = fmaxf(len, 1e-6f);
+    const float xg = (n[0] * gn[0] + n[1] * gn[1]) + n[2] * gn[2];
+    const float k = len >= 1e-6f ? xg / (den * den * len) : 0.f;
+    float* o = graw + ((size_t)b * d.NM + i) * 3;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[c] = gn[c] / den - n[c] * k;
+}
+
+__global__ void __launch_bounds__(128)
+render_bwd_vertex_kernel(RenderDev d, const int32_t* __restrict__ inv_ptr, const int32_t* __restrict__ inv,
+                         const float* __restrict__ verts, const float* __restrict__ cam, const float* __restrict__ graw,
+                         const float* __restrict__ grv, const float* __restrict__ g_tverts, int B,
+                         float* __restrict__ g_verts, float* __restrict__ gcam_v /*[B][V][3]*/) {
+    const int v = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+    if (v >= d.V) return;
+    const float* vb = verts + (size_t)b * d.V * 3;
+    float gt[3] = {0.f, 0.f, 0.f}, gp[3] = {0.f, 0.f, 0.f};
+    if (g_tverts) {
+        const float* g = g_tverts + ((size_t)b * d.V + v) * 3;
+        gt[0] = g[0]; gt[1] = g[1]; gt[2] = g[2];
+    }
+    for (int m = inv_ptr[v]; m < inv_ptr[v + 1]; ++m) {
+        const int i = inv[m];
+        // raster x, y = -tverts x, y (renderer.py:172-173); z only shifts and carries no gradient
+        gt[0] -= grv[((size_t)b * d.NM + i) * 2 + 0];
+        gt[1] -= grv[((size_t)b * d.NM + i) * 2 + 1];
+        // util.py:52-57: corner c' adds cross(q1 - p, q2 - p) with p = c', q1 = c'+1, q2 = c'+2;
+        // d cross(a, b) . G = da . (b x G) + db . (G x a)
+        for (int e = d.adj_ptr[i]; e < d.adj_ptr[i + 1]; ++e) {
+            const int code = d.adj[e], f = code >> 2, c = code & 3;
+            const int32_t* tri = d.faces + (size_t)f * 3;
+            float P[3][3], Gc[3][3];
+#pragma unroll
+            for (int k = 0; k < 3; ++k)
+#pragma unroll
+                for (int q = 0; q < 3; ++q) {
+                    P[k][q] = vb[(size_t)d.mask_ids[tri[k]] * 3 + q];
+                    Gc[k][q] = graw[((size_t)b * d.NM + tri[k]) * 3 + q];
+                }
+#pragma unroll
+            for (int cp = 0; cp < 3; ++cp) {
+                const int q1 = (cp + 1) % 3, q2 = (cp + 2) % 3;
+                if (c != cp && c != q1 && c != q2) continue;
+                float a[3], bb[3];
+#pragma unroll
+                for (int q = 0; q < 3; ++q) { a[q] = P[q1][q] - P[cp][q]; bb[q] = P[q2][q] - P[cp][q]; }
+                const float* G = Gc[cp];
+                const float ga[3] = {bb[1] * G[2] - bb[2] * G[1], bb[2] * G[0] - bb[0] * G[2], bb[0] * G[1] - bb[1] * G[0]};
+                const float gb[3] = {G[1] * a[2] - G[2] * a[1], G[2] * a[0] - G[0] * a[2], G[0] * a[1] - G[1] * a[0]};
+#pragma unroll
+                for (int q = 0; q < 3; ++q)
+                    gp[q] += c == cp ? -(ga[q] + gb[q]) : (c == q1 ? ga[q] : gb[q]);
+            }
+        }
+    }
+    // tverts = (s (x + tx), -s (y + ty), -s z)                                      util.py:64-78, renderer.py:102
+    const float s = cam[b * 3], tx = cam[b * 3 + 1], ty = cam[b * 3 + 2];
+    float* o = g_verts + ((size_t)b * d.V + v) * 3;
+    o[0] = s * gt[0] + gp[0];
+    o[1] = -s * gt[1] + gp[1];
+    o[2] = -s * gt[2] + gp[2];
+    float* gc = gcam_v + ((size_t)b * d.V + v) * 3;
+    gc[0] = ((vb[v * 3] + tx) * gt[0] - (vb[v * 3 + 1] + ty) * gt[1]) - vb[v * 3 + 2] * gt[2];
+    gc[1] = s * gt[0];
+    gc[2] = -s * gt[1];
+}
+
+// out[b][k] = sum_i in[b][i][k], i < n, in a fixed order (strided per-thread sums, then a shared-memory tree)
+__global__ void __launch_bounds__(256)
+render_bwd_cam_kernel(const float* __restrict__ in, int n, float* __restrict__ out) {
+    __shared__ float sR[3][256];
+    const int b = blockIdx.x, tid = threadIdx.x;
+    float a[3] = {0.f, 0.f, 0.f};
+    for (int i = tid; i < n; i += 256)
+#pragma unroll
+        for (int k = 0; k < 3; ++k) a[k] += in[((size_t)b * n + i) * 3 + k];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) sR[k][tid] = a[k];
+    __syncthreads();
+    for (int w = 128; w > 0; w >>= 1) {
+        if (tid < w)
+#pragma unroll
+            for (int k = 0; k < 3; ++k) sR[k][tid] += sR[k][tid + w];
+        __syncthreads();
+    }
+    if (tid < 3) out[b * 3 + tid] = sR[tid][0];
+}
+
+// landmark projection backward (renderer.py:104-108): one CTA per face, x = s (px + tx), y = -s (py + ty);
+// the camera gradient is summed over the points in a fixed order
+__global__ void __launch_bounds__(128)
+project_bwd_kernel(const float* __restrict__ pts, const float* __restrict__ cam, int L, const float* __restrict__ g_xy,
+                   float* __restrict__ g_pts, float* __restrict__ g_cam) {
+    __shared__ float sR[3][128];
+    const int b = blockIdx.x, tid = threadIdx.x;
+    const float s = cam[b * 3], tx = cam[b * 3 + 1], ty = cam[b * 3 + 2];
+    float a[3] = {0.f, 0.f, 0.f};
+    for (int l = tid; l < L; l += 128) {
+        const size_t i = (size_t)b * L + l;
+        const float* p = pts + i * 3;
+        const float gx = g_xy[i * 2], gy = g_xy[i * 2 + 1];
+        g_pts[i * 3] = s * gx; g_pts[i * 3 + 1] = -s * gy; g_pts[i * 3 + 2] = 0.f;
+        a[0] += (p[0] + tx) * gx - (p[1] + ty) * gy;
+        a[1] += s * gx;
+        a[2] -= s * gy;
+    }
+#pragma unroll
+    for (int k = 0; k < 3; ++k) sR[k][tid] = a[k];
+    __syncthreads();
+    for (int w = 64; w > 0; w >>= 1) {
+        if (tid < w)
+#pragma unroll
+            for (int k = 0; k < 3; ++k) sR[k][tid] += sR[k][tid + w];
+        __syncthreads();
+    }
+    if (tid < 3) g_cam[b * 3 + tid] = sR[tid][0];
+}
+
 }  // namespace
 
 struct SmkRenderer {
     RenderDev d;
     Lights lights;
+    int32_t* inv_ptr;      // [V+1] CSR mesh vertex -> sub-mesh ids (the inverse of mask_ids), for the backward
+    int32_t* inv;          // [NM]
     smk::DeviceArena arena;
 };
 
@@ -303,6 +592,15 @@ extern "C" int smk_renderer_create(const SmkRendererDesc* desc, SmkRenderer** ou
     if (e == cudaSuccess) e = h->arena.upload(desc->faces, (size_t)d.F * 3, &d.faces);
     if (e == cudaSuccess) e = h->arena.upload(ptr, &d.adj_ptr);
     if (e == cudaSuccess) e = h->arena.upload(adj, &d.adj);
+    {   // backward: mesh vertex -> sub-mesh ids
+        std::vector<int32_t> iptr(d.V + 1, 0), inv(std::max(d.NM, 1), 0);
+        for (int i = 0; i < d.NM; ++i) iptr[desc->mask_ids[i] + 1]++;
+        for (int v = 0; v < d.V; ++v) iptr[v + 1] += iptr[v];
+        std::vector<int32_t> ifill(iptr.begin(), iptr.end() - 1);
+        for (int i = 0; i < d.NM; ++i) inv[ifill[desc->mask_ids[i]]++] = i;
+        if (e == cudaSuccess) e = h->arena.upload(iptr, &h->inv_ptr);
+        if (e == cudaSuccess) e = h->arena.upload(inv, &h->inv);
+    }
     if (e != cudaSuccess) { smk::set_error("smk_renderer_create: upload failed: %s", cudaGetErrorString(e)); delete h; return (int)e; }
     // light directions, F.normalize(dir) = dir / max(||dir||, 1e-12)      renderer.py:127-135,247
     const float dirs[5][3] = {{-1, 1, 1}, {1, 1, 1}, {-1, -1, 1}, {1, -1, 1}, {0, 0, 1}};
@@ -359,6 +657,61 @@ extern "C" int smk_renderer_forward(const SmkRenderer* h, const float* verts, co
     dim3 grid(d.S / TILE_W, d.S / TILE_H, B);
     SMK_TAG("raster_tile", 4.0 * B * ((double)d.F * (REC + 1) + 3.0 * d.NM + (double)d.S * d.S * (3 + (pix_to_face ? 2 : 0) + (bary ? 3 : 0) + (zbuf ? 1 : 0))), 0.0, st);
     SMK_LAUNCH(raster_tile_kernel, dim3(grid), dim3(dim3(TILE_W, TILE_H)), smem, st, d, recs, ranges, nrm, h->lights, B, rendered, pix_to_face, bary, zbuf);
+    SMK_CHECK_LAUNCH();
+    return 0;
+}
+
+// ---- backward ------------------------------------------------------------------------------------
+extern "C" size_t smk_renderer_backward_workspace_bytes(const SmkRenderer* h, int B) {
+    if (!h || B <= 0) return 0;
+    const RenderDev& d = h->d;
+    return smk::ws_round((size_t)B * d.F * kFG * 4) + smk::ws_round((size_t)B * d.NM * 3 * 4) +
+           smk::ws_round((size_t)B * d.NM * 2 * 4) + smk::ws_round((size_t)B * d.V * 3 * 4);
+}
+
+extern "C" int smk_renderer_backward(const SmkRenderer* h, const float* verts, const float* cam, int B,
+                                     const int64_t* pix_to_face, const float* bary, const float* normals,
+                                     const float* g_rendered, const float* g_tverts, float* g_verts, float* g_cam,
+                                     void* ws, size_t ws_bytes, void* stream) {
+    if (B == 0) return 0;
+    SMK_REQUIRE(h && verts && cam && pix_to_face && bary && normals && g_verts && g_cam, "smk_renderer_backward: null argument");
+    SMK_REQUIRE(B > 0, "smk_renderer_backward: negative batch");
+    SMK_REQUIRE(ws && ws_bytes >= smk_renderer_backward_workspace_bytes(h, B), "smk_renderer_backward: workspace too small");
+    const RenderDev& d = h->d;
+    cudaStream_t st = (cudaStream_t)stream;
+    smk::Workspace w(ws, ws_bytes);
+    float* gface = w.take<float>((size_t)B * d.F * kFG);
+    float* graw = w.take<float>((size_t)B * d.NM * 3);
+    float* grv = w.take<float>((size_t)B * d.NM * 2);
+    float* gcam_v = w.take<float>((size_t)B * d.V * 3);
+    const double plane = (double)d.S * d.S;
+    SMK_TAG("render_bwd_face", 4.0 * B * ((double)d.F * (kFG + 6) + 9.0 * d.NM + (g_rendered ? plane * (2 + 3 + 3) : 0.0)),
+            g_rendered ? 120.0 * B * plane : 0.0, st);
+    SMK_LAUNCH(render_bwd_face_kernel, dim3(smk::cdiv(d.F, 4), B), dim3(128), 0, st, d, h->lights, verts, cam,
+               pix_to_face, bary, normals, g_rendered, B, gface);
+    SMK_CHECK_LAUNCH();
+    SMK_TAG("render_bwd_normal", 4.0 * B * ((double)d.F * kFG + 3.0 * d.NM + 5.0 * d.NM) + 4.0 * (4.0 * d.F + 2.0 * d.NM),
+            B * (30.0 * 3.0 * d.F + 20.0 * d.NM), st);
+    SMK_LAUNCH(render_bwd_normal_kernel, dim3(smk::cdiv(d.NM, 128), B), dim3(128), 0, st, d, verts, gface, B, graw, grv);
+    SMK_CHECK_LAUNCH();
+    SMK_TAG("render_bwd_vertex", 4.0 * B * (3.0 * d.V * (g_tverts ? 4 : 3) + 5.0 * d.NM + 6.0 * d.V) + 4.0 * (d.V + 1 + d.NM),
+            B * (60.0 * 3.0 * d.F + 12.0 * d.V), st);
+    SMK_LAUNCH(render_bwd_vertex_kernel, dim3(smk::cdiv(d.V, 128), B), dim3(128), 0, st, d, h->inv_ptr, h->inv, verts, cam,
+               graw, grv, g_tverts, B, g_verts, gcam_v);
+    SMK_CHECK_LAUNCH();
+    SMK_TAG("render_bwd_cam", 4.0 * B * (3.0 * d.V + 3), 3.0 * B * d.V, st);
+    SMK_LAUNCH(render_bwd_cam_kernel, dim3(B), dim3(256), 0, st, gcam_v, d.V, g_cam);
+    SMK_CHECK_LAUNCH();
+    return 0;
+}
+
+extern "C" int smk_project_points_backward(const float* pts, const float* cam, int B, int L, const float* g_xy,
+                                           float* g_pts, float* g_cam, void* stream) {
+    if (B == 0 || L == 0) return 0;            // empty batch: nothing to do (pointers may be null)
+    SMK_REQUIRE(pts && cam && g_xy && g_pts && g_cam, "smk_project_points_backward: null argument");
+    SMK_REQUIRE(B > 0 && L > 0, "smk_project_points_backward: negative size");
+    SMK_TAG("project_points_bwd", 4.0 * B * (8.0 * L + 6), 12.0 * B * L, (cudaStream_t)stream);
+    SMK_LAUNCH(project_bwd_kernel, dim3(B), dim3(128), 0, (cudaStream_t)stream, pts, cam, L, g_xy, g_pts, g_cam);
     SMK_CHECK_LAUNCH();
     return 0;
 }

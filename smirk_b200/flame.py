@@ -1,7 +1,9 @@
-"""``FLAME`` — drop-in for the reference class ``src/FLAME/FLAME.py:44-315`` (forward only).
+"""``FLAME`` — drop-in for the reference class ``src/FLAME/FLAME.py:44-315``.
 
 Same constructor arguments, buffer names (so ``state_dict`` keys match), ``forward`` signature and
-output dict; the arithmetic runs in ``csrc/flame.cu`` through ``smk_flame_forward``.
+output dict; the arithmetic runs in ``csrc/flame.cu`` through ``smk_flame_forward``.  When grad mode is
+on and a parameter requires grad, ``forward`` is differentiable for shape, expression, pose, jaw, neck,
+eye pose and eyelid parameters (``smk_flame_backward``); otherwise it is the plain forward.
 """
 import ctypes as C
 import pickle
@@ -100,7 +102,7 @@ class FLAME(nn.Module):
         self.register_buffer("mp_lmk_bary_coords", torch.from_numpy(mp["lmk_b_coords"]).to(self.dtype))
         if self.parents.tolist() != [-1, 0, 1, 1, 1]:
             raise RuntimeError("smirk_b200.FLAME: unsupported kinematic tree %s" % self.parents.tolist())
-        self._handle, self._handle_dev, self._ws = None, None, _lib.Workspace()
+        self._handle, self._handle_dev, self._ws, self._bws = None, None, _lib.Workspace(), _lib.Workspace()
 
     # -- native handle (re-packed when a buffer is replaced / edited in place / moved) ---------------
     def _native(self, device):
@@ -142,9 +144,9 @@ class FLAME(nn.Module):
         new = self.__class__.__new__(self.__class__)
         nn.Module.__init__(new)
         for k, v in self.__dict__.items():
-            if k not in ("_handle", "_handle_dev", "_ws"):
+            if k not in ("_handle", "_handle_dev", "_ws", "_bws"):
                 new.__dict__[k] = copy.deepcopy(v, memo)
-        new._handle, new._handle_dev, new._ws = None, None, _lib.Workspace()
+        new._handle, new._handle_dev, new._ws, new._bws = None, None, _lib.Workspace(), _lib.Workspace()
         return new
 
     # -- forward --------------------------------------------------------------------------------------
@@ -204,5 +206,41 @@ class FLAME(nn.Module):
             neck_pose_params = self.neck_pose.expand(B, -1)
         betas = torch.cat([shape_params, expression_params], 1)
         full_pose = torch.cat([pose_params, neck_pose_params.to(dev), jaw_params, eye_pose_params.to(dev)], 1)
+        keys = ("vertices", "landmarks_fan", "landmarks_fan_3d", "landmarks_mp")
+        if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (betas, full_pose, eyelid_params)):
+            return dict(zip(keys, _FlameFunction.apply(self, betas, full_pose, eyelid_params)))
         r = self.run_lbs(betas, full_pose, eyelid_params)
-        return {k: r[k] for k in ("vertices", "landmarks_fan", "landmarks_fan_3d", "landmarks_mp")}
+        return {k: r[k] for k in keys}
+
+
+class _FlameFunction(torch.autograd.Function):
+    """betas, full_pose, eyelid -> (vertices, landmarks_fan, landmarks_fan_3d, landmarks_mp); the backward is
+    ``smk_flame_backward``.  Concatenation, zero padding and the ``zero_*`` switches stay in torch autograd."""
+
+    @staticmethod
+    def forward(ctx, module, betas, full_pose, eyelid):
+        r = module.run_lbs(betas, full_pose, eyelid)
+        ctx.module, ctx.has_eyelid = module, eyelid is not None
+        ctx.dtypes = (betas.dtype, full_pose.dtype, eyelid.dtype if eyelid is not None else None)
+        ctx.save_for_backward(_lib.dev_f32(betas, "betas"), _lib.dev_f32(full_pose, "full_pose"), r["dyn_idx"])
+        return r["vertices"], r["landmarks_fan"], r["landmarks_fan_3d"], r["landmarks_mp"]
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_verts, g_fan, g_fan3d, g_mp):
+        betas, full_pose, dyn = ctx.saved_tensors
+        m, dev, B = ctx.module, betas.device, betas.shape[0]
+        L = _lib.lib()
+        h = m._native(dev)
+        gs = [None if g is None else g.to(torch.float32).contiguous() for g in (g_verts, g_fan, g_fan3d, g_mp)]
+        g_betas = torch.empty_like(betas)
+        g_pose = torch.empty_like(full_pose)
+        g_eyelid = torch.empty(B, 2, dtype=torch.float32, device=dev) if ctx.has_eyelid else None
+        with torch.cuda.device(dev):
+            ws = m._bws.get(L.smk_flame_backward_workspace_bytes(h, B), dev)
+            _lib.check(L.smk_flame_backward(h, _lib.ptr(betas), _lib.ptr(full_pose), None, B, _lib.ptr(dyn),
+                                            *[_lib.ptr(g) for g in gs], _lib.ptr(g_betas), _lib.ptr(g_pose),
+                                            _lib.ptr(g_eyelid), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev)),
+                       "smk_flame_backward")
+        return (None, g_betas.to(ctx.dtypes[0]), g_pose.to(ctx.dtypes[1]),
+                g_eyelid.to(ctx.dtypes[2]) if g_eyelid is not None else None)

@@ -1,9 +1,11 @@
-"""``Renderer`` — drop-in for the reference class ``src/renderer/renderer.py:49-207`` (forward only).
+"""``Renderer`` — drop-in for the reference class ``src/renderer/renderer.py:49-207``.
 
 Same constructor arguments, registered buffers (``state_dict`` keys: faces, face_colors, raw_uvcoords,
 uvcoords, uvfaces, face_uvcoords, constant_factor) and ``forward`` output dict; the vertex stage,
 normals, rasterisation (pytorch3d's ``rasterize_meshes`` in the reference) and shading run in
-``csrc/render.cu`` through ``smk_renderer_forward``.
+``csrc/render.cu`` through ``smk_renderer_forward``.  When grad mode is on and an input requires grad,
+``forward`` is differentiable for the vertices, the camera and the landmark sets (``smk_renderer_backward``,
+``smk_project_points_backward``); otherwise it is the plain forward.
 """
 import ctypes as C
 import pickle
@@ -80,7 +82,7 @@ class Renderer(nn.Module):
              ((2 * pi) / 3) * (np.sqrt(3 / (4 * pi))), (pi / 4) * (3) * (np.sqrt(5 / (12 * pi))),
              (pi / 4) * (3) * (np.sqrt(5 / (12 * pi))), (pi / 4) * (3) * (np.sqrt(5 / (12 * pi))),
              (pi / 4) * (3 / 2) * (np.sqrt(5 / (12 * pi))), (pi / 4) * (1 / 2) * (np.sqrt(5 / (4 * pi)))]).float())
-        self._handle, self._handle_dev, self._ws = None, None, _lib.Workspace()
+        self._handle, self._handle_dev, self._ws, self._bws = None, None, _lib.Workspace(), _lib.Workspace()
 
     def _native(self, device):
         sig = (str(device), self.faces._version, self.faces.data_ptr(), self.image_size)
@@ -107,14 +109,27 @@ class Renderer(nn.Module):
         new = self.__class__.__new__(self.__class__)
         nn.Module.__init__(new)
         for k, v in self.__dict__.items():
-            if k not in ("_handle", "_handle_dev", "_ws"):
+            if k not in ("_handle", "_handle_dev", "_ws", "_bws"):
                 new.__dict__[k] = copy.deepcopy(v, memo)
-        new._handle, new._handle_dev, new._ws = None, None, _lib.Workspace()
+        new._handle, new._handle_dev, new._ws, new._bws = None, None, _lib.Workspace(), _lib.Workspace()
         return new
 
-    @torch.no_grad()
     def forward(self, vertices, cam_params, **landmarks):
+        if torch.is_grad_enabled() and any(torch.is_tensor(t) and t.requires_grad
+                                           for t in (vertices, cam_params, *landmarks.values())):
+            return self._forward_autograd(vertices, cam_params, **landmarks)
         return self.render_full(vertices, cam_params, raw=False, **landmarks)
+
+    def _forward_autograd(self, vertices, cam_params, **landmarks):
+        """forward() with gradients for vertices, cam_params and every landmark set (smk_renderer_backward,
+        smk_project_points_backward).  Saves the rasteriser's pix_to_face, bary and the vertex normals."""
+        if self.render_full_head:
+            raise RuntimeError("smirk_b200.Renderer: gradients are not implemented for render_full_head=True")
+        rendered, tverts = _RenderFunction.apply(self, vertices, cam_params)
+        out = {"rendered_img": rendered, "transformed_vertices": tverts}
+        for k, pts in landmarks.items():
+            out[k] = _ProjectFunction.apply(pts, cam_params)
+        return out
 
     @torch.no_grad()
     def render_full(self, vertices, cam_params, raw=True, **landmarks):
@@ -153,3 +168,65 @@ class Renderer(nn.Module):
         if raw:
             out.update(pix_to_face=p2f, bary=bary, zbuf=zbuf, normals=normals)
         return out
+
+
+def _grad_f32(g):
+    return None if g is None else g.to(torch.float32).contiguous()
+
+
+class _RenderFunction(torch.autograd.Function):
+    """vertices, cam -> (rendered_img, transformed_vertices) through ``render_full(raw=True)``; the backward is
+    ``smk_renderer_backward`` from the saved pix_to_face / bary / normals."""
+
+    @staticmethod
+    def forward(ctx, module, vertices, cam):
+        r = module.render_full(vertices, cam, raw=True)
+        ctx.module, ctx.dtypes = module, (vertices.dtype, cam.dtype)
+        ctx.save_for_backward(_lib.dev_f32(vertices, "vertices"), _lib.dev_f32(cam, "cam_params"),
+                              r["pix_to_face"], r["bary"], r["normals"])
+        return r["rendered_img"], r["transformed_vertices"]
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_rendered, g_tverts):
+        verts, cam, p2f, bary, normals = ctx.saved_tensors
+        m, dev, B = ctx.module, verts.device, verts.shape[0]
+        L = _lib.lib()
+        h = m._native(dev)
+        g_verts, g_cam = torch.empty_like(verts), torch.empty_like(cam)
+        g_rendered, g_tverts = _grad_f32(g_rendered), _grad_f32(g_tverts)
+        with torch.cuda.device(dev):
+            ws = m._bws.get(L.smk_renderer_backward_workspace_bytes(h, B), dev)
+            _lib.check(L.smk_renderer_backward(h, _lib.ptr(verts), _lib.ptr(cam), B, _lib.ptr(p2f), _lib.ptr(bary),
+                                               _lib.ptr(normals), _lib.ptr(g_rendered), _lib.ptr(g_tverts),
+                                               _lib.ptr(g_verts), _lib.ptr(g_cam), _lib.ptr(ws), ws.numel(),
+                                               _lib.stream_ptr(dev)), "smk_renderer_backward")
+        return None, g_verts.to(ctx.dtypes[0]), g_cam.to(ctx.dtypes[1])
+
+
+class _ProjectFunction(torch.autograd.Function):
+    """Landmark projection (renderer.py:104-108): pts [B,L,3], cam [B,3] -> [B,L,2]."""
+
+    @staticmethod
+    def forward(ctx, pts, cam):
+        p, c = _lib.dev_f32(pts, "landmarks"), _lib.dev_f32(cam, "cam_params")
+        B, n = p.shape[0], p.shape[1]
+        xy = torch.empty(B, n, 2, dtype=torch.float32, device=p.device)
+        with torch.cuda.device(p.device):
+            _lib.check(_lib.lib().smk_project_points(_lib.ptr(p), _lib.ptr(c), B, n, _lib.ptr(xy),
+                                                     _lib.stream_ptr(p.device)), "smk_project_points")
+        ctx.dtypes = (pts.dtype, cam.dtype)
+        ctx.save_for_backward(p, c)
+        return xy
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_xy):
+        p, c = ctx.saved_tensors
+        B, n = p.shape[0], p.shape[1]
+        g_pts, g_cam, g_xy = torch.empty_like(p), torch.empty_like(c), _grad_f32(g_xy)
+        with torch.cuda.device(p.device):
+            _lib.check(_lib.lib().smk_project_points_backward(_lib.ptr(p), _lib.ptr(c), B, n, _lib.ptr(g_xy),
+                                                              _lib.ptr(g_pts), _lib.ptr(g_cam), _lib.stream_ptr(p.device)),
+                       "smk_project_points_backward")
+        return g_pts.to(ctx.dtypes[0]), g_cam.to(ctx.dtypes[1])
