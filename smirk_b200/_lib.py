@@ -3,6 +3,7 @@
 There is deliberately no fallback: if the shared library is missing or a call fails, the product
 path raises.  Build with ``python -m smirk_b200.build`` (or ``__graft_entry__.build()``).
 """
+import copy
 import ctypes as C
 import os
 
@@ -44,21 +45,76 @@ class SmkGeneratorDesc(C.Structure):
                 ("precision", C.c_int)]
 
 
-SYMBOLS = ["smk_version", "smk_last_error", "smk_launch_count", "smk_profiler_enable", "smk_profiler_reset",
-           "smk_profiler_report",
-           "smk_flame_create", "smk_flame_destroy", "smk_flame_workspace_bytes", "smk_flame_forward",
-           "smk_renderer_create", "smk_renderer_destroy", "smk_renderer_workspace_bytes", "smk_renderer_forward",
-           "smk_project_points",
-           "smk_flame_backward_workspace_bytes", "smk_flame_backward", "smk_renderer_backward_workspace_bytes",
-           "smk_renderer_backward", "smk_project_points_backward",
-           "smk_encoder_create", "smk_encoder_destroy", "smk_encoder_workspace_bytes", "smk_encoder_forward",
-           "smk_generator_create", "smk_generator_destroy", "smk_generator_workspace_bytes", "smk_generator_forward",
-           "smk_debug_conv_f32", "smk_debug_conv_tc", "smk_debug_reflect_halo", "smk_debug_xdw", "smk_debug_stem_ds", "smk_debug_gemm_tc3x", "smk_debug_xdw3x", "smk_debug_conv3_win",
-           "smk_warp_workspace_bytes", "smk_crop_warp", "smk_warp_u8", "smk_f32chw_to_u8hwc",
-           "smk_masking_create", "smk_masking_destroy", "smk_masking_workspace_bytes", "smk_masking_face_weights",
-           "smk_masking_points", "smk_masking_compose", "smk_masking_forward_workspace_bytes", "smk_masking_forward", "smk_masking_transfer_pixels",
-           "smk_peer_alloc", "smk_peer_free", "smk_peer_open", "smk_peer_close", "smk_peer_push",
-           "smk_peer_fan_create", "smk_peer_fan_destroy", "smk_peer_fan_push"]
+class SmkMaskingDesc(C.Structure):
+    _fields_ = [("n_verts", C.c_int), ("n_faces", C.c_int), ("faces", c_i32p)]
+
+
+# The binding table: one (name, return type, argument types) row per entry point of include/smirk_b200.h, in the
+# header's order.  STREAM marks a trailing `void* stream`, which `call` fills in with the current stream.  An `int`
+# result is a status code, except for smk_version and smk_profiler_report, which only this file calls.
+STREAM = "stream"
+_vp, _i, _sz, _f, _vpp = C.c_void_p, C.c_int, C.c_size_t, C.c_float, C.POINTER(C.c_void_p)
+BINDINGS = [
+    ("smk_version", _i, []),
+    ("smk_last_error", C.c_char_p, []),
+    ("smk_launch_count", C.c_ulonglong, []),
+    ("smk_profiler_enable", None, [_i]),
+    ("smk_profiler_reset", None, []),
+    ("smk_profiler_report", _i, [C.c_char_p, _sz]),
+    ("smk_flame_create", _i, [C.POINTER(SmkFlameDesc), _vpp]),
+    ("smk_flame_destroy", None, [_vp]),
+    ("smk_flame_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_flame_forward", _i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_flame_backward_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_flame_backward", _i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_renderer_create", _i, [C.POINTER(SmkRendererDesc), _vpp]),
+    ("smk_renderer_destroy", None, [_vp]),
+    ("smk_renderer_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_renderer_forward", _i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_project_points", _i, [_vp, _vp, _i, _i, _vp, STREAM]),
+    ("smk_renderer_backward_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_renderer_backward", _i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_project_points_backward", _i, [_vp, _vp, _i, _i, _vp, _vp, _vp, STREAM]),
+    ("smk_encoder_create", _i, [C.POINTER(SmkEncoderDesc), _vpp]),
+    ("smk_encoder_destroy", None, [_vp]),
+    ("smk_encoder_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_encoder_forward", _i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_generator_create", _i, [C.POINTER(SmkGeneratorDesc), _vpp]),
+    ("smk_generator_destroy", None, [_vp]),
+    ("smk_generator_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_generator_forward", _i, [_vp, _vp, _i, _vp, _vp, _sz, STREAM]),
+    ("smk_warp_workspace_bytes", _sz, [_i]),
+    ("smk_crop_warp", _i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _sz, STREAM]),
+    ("smk_warp_u8", _i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _sz, STREAM]),
+    ("smk_f32chw_to_u8hwc", _i, [_vp, _i, _i, _vp, STREAM]),
+    ("smk_masking_create", _i, [C.POINTER(SmkMaskingDesc), _vpp]),
+    ("smk_masking_destroy", None, [_vp]),
+    ("smk_masking_workspace_bytes", _sz, [_vp, _i, _i]),
+    ("smk_masking_face_weights", _i, [_vp, _vp, _vp, _i, _vp, _vp, _sz, STREAM]),
+    ("smk_masking_points", _i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, STREAM]),
+    ("smk_masking_compose", _i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _sz, STREAM]),
+    ("smk_masking_transfer_pixels", _i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _sz, STREAM]),
+    ("smk_masking_forward_workspace_bytes", _sz, [_vp, _i, _i, _i]),
+    ("smk_masking_forward", _i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _f, _i, _vp, _vp, _vp, _vp, _vp, _vp,
+                                 _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_peer_alloc", _i, [_sz, _vpp, C.c_char_p]),
+    ("smk_peer_free", _i, [_vp]),
+    ("smk_peer_open", _i, [C.c_char_p, _vpp]),
+    ("smk_peer_close", _i, [_vp]),
+    ("smk_peer_push", _i, [_vp, _vp, _sz, STREAM]),
+    ("smk_peer_fan_create", _i, [_i, _vpp]),
+    ("smk_peer_fan_destroy", None, [_vp]),
+    ("smk_peer_fan_push", _i, [_vp, _vpp, _i, _vp, _sz, STREAM]),
+    ("smk_debug_conv_f32", _i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _i, _vp, _i, _i, STREAM]),
+    ("smk_debug_conv_tc", _i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, STREAM]),
+    ("smk_debug_reflect_halo", _i, [_vp, _i, _i, _i, _i, STREAM]),
+    ("smk_debug_xdw", _i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _i, _vp, STREAM]),
+    ("smk_debug_conv3_win", _i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _vp, _i, STREAM]),
+    ("smk_debug_gemm_tc3x", _i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _vp, _i, STREAM]),
+    ("smk_debug_xdw3x", _i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _vp, STREAM]),
+    ("smk_debug_stem_ds", _i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, STREAM]),
+]
+_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS if args[-1:] == [STREAM])
 
 
 def lib():
@@ -70,72 +126,9 @@ def lib():
         raise RuntimeError("smirk_b200: %s not found — build it with `python -m smirk_b200.build` "
                            "(there is no CPU / PyTorch fallback)" % LIB_PATH)
     L = C.CDLL(LIB_PATH)
-    L.smk_last_error.restype = C.c_char_p
-    for name in SYMBOLS:
+    for name, restype, argtypes in BINDINGS:
         fn = getattr(L, name)
-        if name.endswith("_workspace_bytes"):
-            fn.restype = C.c_size_t
-        elif name.endswith("_destroy"):
-            fn.restype = None
-    vp, i, sz = C.c_void_p, C.c_int, C.c_size_t
-    L.smk_launch_count.restype = C.c_ulonglong
-    L.smk_profiler_enable.argtypes = [i]
-    L.smk_profiler_enable.restype = None
-    L.smk_profiler_reset.restype = None
-    L.smk_profiler_report.argtypes = [C.c_char_p, sz]
-    L.smk_flame_create.argtypes = [C.POINTER(SmkFlameDesc), C.POINTER(vp)]
-    L.smk_flame_destroy.argtypes = [vp]
-    L.smk_flame_workspace_bytes.argtypes = [vp, i]
-    L.smk_flame_forward.argtypes = [vp, vp, vp, vp, i, vp, vp, vp, vp, vp, vp, vp, sz, vp]
-    L.smk_renderer_create.argtypes = [C.POINTER(SmkRendererDesc), C.POINTER(vp)]
-    L.smk_renderer_destroy.argtypes = [vp]
-    L.smk_renderer_workspace_bytes.argtypes = [vp, i]
-    L.smk_renderer_forward.argtypes = [vp, vp, vp, i, vp, vp, vp, vp, vp, vp, vp, sz, vp]
-    L.smk_project_points.argtypes = [vp, vp, i, i, vp, vp]
-    L.smk_flame_backward_workspace_bytes.argtypes = [vp, i]
-    L.smk_flame_backward.argtypes = [vp, vp, vp, vp, i, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
-    L.smk_renderer_backward_workspace_bytes.argtypes = [vp, i]
-    L.smk_renderer_backward.argtypes = [vp, vp, vp, i, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
-    L.smk_project_points_backward.argtypes = [vp, vp, i, i, vp, vp, vp, vp]
-    L.smk_encoder_create.argtypes = [C.POINTER(SmkEncoderDesc), C.POINTER(vp)]
-    L.smk_encoder_destroy.argtypes = [vp]
-    L.smk_encoder_workspace_bytes.argtypes = [vp, i]
-    L.smk_encoder_forward.argtypes = [vp, vp, i, vp, vp, vp, vp, sz, vp]
-    L.smk_generator_create.argtypes = [C.POINTER(SmkGeneratorDesc), C.POINTER(vp)]
-    L.smk_generator_destroy.argtypes = [vp]
-    L.smk_generator_workspace_bytes.argtypes = [vp, i]
-    L.smk_generator_forward.argtypes = [vp, vp, i, vp, vp, sz, vp]
-    L.smk_debug_conv_f32.argtypes = [vp, i, i, i, i, i, vp, vp, vp, i, i, i, i, vp, i, vp, i, i, vp]
-    L.smk_debug_conv_tc.argtypes = [vp, i, i, i, i, i, vp, vp, vp, i, i, i, i, vp, i, i, vp, i, i, vp]
-    L.smk_debug_reflect_halo.argtypes = [vp, i, i, i, i, vp]
-    L.smk_debug_xdw.argtypes = [vp, i, i, i, i, vp, vp, vp, i, vp, vp, vp, i, i, vp, vp]
-    L.smk_masking_create.argtypes = [vp, vp]
-    L.smk_masking_destroy.argtypes = [vp]
-    L.smk_masking_workspace_bytes.argtypes = [vp, i, i]
-    L.smk_masking_face_weights.argtypes = [vp, vp, vp, i, vp, vp, sz, vp]
-    L.smk_masking_points.argtypes = [vp, vp, vp, vp, i, i, i, vp, vp]
-    L.smk_masking_forward_workspace_bytes.argtypes = [vp, i, i, i]
-    L.smk_masking_forward.argtypes = [vp, vp, vp, vp, vp, vp, i, i, i, i, C.c_float, C.c_float, i, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
-    L.smk_masking_compose.argtypes = [vp, vp, vp, vp, vp, i, vp, vp, vp, vp, i, i, i, vp, vp, sz, vp]
-    L.smk_masking_transfer_pixels.argtypes = [vp, vp, vp, vp, i, i, i, vp, vp, sz, vp]
-    L.smk_peer_alloc.argtypes = [sz, C.POINTER(vp), C.c_char_p]
-    L.smk_peer_free.argtypes = [vp]
-    L.smk_peer_open.argtypes = [C.c_char_p, C.POINTER(vp)]
-    L.smk_peer_close.argtypes = [vp]
-    L.smk_peer_push.argtypes = [vp, vp, sz, vp]
-    L.smk_peer_fan_create.argtypes = [i, C.POINTER(vp)]
-    L.smk_peer_fan_destroy.argtypes = [vp]
-    L.smk_peer_fan_destroy.restype = None
-    L.smk_peer_fan_push.argtypes = [vp, C.POINTER(vp), i, vp, sz, vp]
-    L.smk_debug_conv3_win.argtypes = [vp, i, i, i, i, i, vp, vp, vp, i, i, vp, i, vp]
-    L.smk_debug_gemm_tc3x.argtypes = [vp, i, i, vp, vp, vp, vp, i, i, i, vp, i, vp, i, vp]
-    L.smk_debug_xdw3x.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, i, vp, vp, vp, i, vp, vp]
-    L.smk_warp_workspace_bytes.argtypes = [i]
-    L.smk_warp_workspace_bytes.restype = C.c_size_t
-    L.smk_crop_warp.argtypes = [vp, i, i, i, vp, i, i, vp, vp, C.c_size_t, vp]
-    L.smk_warp_u8.argtypes = [vp, i, i, i, vp, i, i, vp, vp, C.c_size_t, vp]
-    L.smk_f32chw_to_u8hwc.argtypes = [vp, i, i, vp, vp]
-    L.smk_debug_stem_ds.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp, vp, vp, vp, vp, i, i, vp, vp]
+        fn.restype, fn.argtypes = restype, [_vp if a is STREAM else a for a in argtypes]
     if L.smk_version() != 100:
         raise RuntimeError("smirk_b200: library/header version mismatch (%d)" % L.smk_version())
     _lib = L
@@ -146,6 +139,22 @@ def check(rc, what):
     if rc != 0:
         msg = lib().smk_last_error().decode("utf-8", "replace")
         raise RuntimeError("smirk_b200: %s failed (rc=%d): %s" % (what, rc, msg))
+
+
+def call(name, device, *args):
+    """Run entry point ``name`` for tensors on ``device``: under that device (launches go to the tensors' device, not
+    the current one) and, for an entry point that takes a stream, on that device's current stream, which is appended
+    to ``args``.  Tensors are passed as their data pointers, None as NULL.  An ``int`` result is a status code and
+    raises through ``check``; any other result (a workspace size, a launch count) is returned."""
+    fn = getattr(lib(), name)
+    args = [a.data_ptr() if torch.is_tensor(a) else a for a in args]
+    with torch.cuda.device(device):
+        if name in _TAKES_STREAM:
+            args.append(torch.cuda.current_stream(device).cuda_stream)
+        r = fn(*args)
+    if fn.restype is not _i:
+        return r
+    check(r, name)
 
 
 def f32(a):
@@ -173,14 +182,6 @@ def dev_f32(t, name):
     return t.detach().to(torch.float32).contiguous()
 
 
-def ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
-
-
-def stream_ptr(device):
-    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-
-
 class NativeHandle:
     """Owner of one ``Smk*`` handle.  Passed to the C ABI like a ``c_void_p`` (``_as_parameter_``); the native
     object is destroyed when the last Python reference goes away.  Modules drop their reference when their weights
@@ -198,6 +199,13 @@ class NativeHandle:
         except Exception:
             pass
         self._as_parameter_ = None
+
+
+def create(kind, desc, device):
+    """``smk_<kind>_create(&desc, &h)`` on ``device`` -> the handle, destroyed by ``smk_<kind>_destroy``."""
+    h = C.c_void_p()
+    call("smk_%s_create" % kind, device, C.byref(desc), C.byref(h))
+    return NativeHandle(h, "smk_%s_destroy" % kind)
 
 
 class Workspace:
@@ -221,6 +229,62 @@ def buffers_signature(module, device, *extra):
         s.append(t._version)
         s.append(t.data_ptr())
     return tuple(s)
+
+
+class NativeState:
+    """Everything native one module owns: the handle and the key it was created for, named workspaces, and tensors
+    the module keeps per device."""
+
+    def __init__(self):
+        self.handle, self.key, self.workspaces, self.per_device = None, None, {}, {}
+
+
+class NativeModule:
+    """Base of every module that wraps a native handle.  A subclass implements ``_native_create(device)`` (build the
+    descriptor, return ``create(...)``); the handle is created lazily and again whenever ``_native_key(device)``
+    changes.  All of it lives in one ``NativeState``, which a deep copy does not share."""
+
+    @property
+    def _native(self):
+        st = self.__dict__.get("_native_state")
+        if st is None:
+            st = self.__dict__["_native_state"] = NativeState()
+        return st
+
+    def _native_key(self, device):
+        return buffers_signature(self, device, *self._native_extras())
+
+    def _native_extras(self):
+        """Settings besides the parameters and buffers that the handle is packed for."""
+        return ()
+
+    def _native_create(self, device):
+        raise NotImplementedError
+
+    def _native_handle(self, device):
+        st, key = self._native, self._native_key(device)
+        if st.handle is None or st.key != key:
+            st.handle = None                   # the native object dies with its last reference (NativeHandle)
+            st.handle, st.key = self._native_create(device), key
+        return st.handle
+
+    def _native_workspace(self, name, nbytes, device):
+        return self._native.workspaces.setdefault(name, Workspace()).get(nbytes, device)
+
+    def graph_keep_alive(self):
+        """What a CUDA graph captured over this module must keep alive: the handle (packed weights) and the forward
+        workspace it was recorded with."""
+        ws = self._native.workspaces.get("forward")
+        return self._native.handle, ws.buf if ws is not None else None
+
+    def __deepcopy__(self, memo):
+        """Same parameter and buffer values; the copy builds its own native state on first use."""
+        new = self.__class__.__new__(self.__class__)
+        memo[id(self)] = new
+        for k, v in self.__dict__.items():
+            if k != "_native_state":
+                new.__dict__[k] = copy.deepcopy(v, memo)
+        return new
 
 
 def profiler_report():

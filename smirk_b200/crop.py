@@ -98,9 +98,8 @@ def _matrices(tforms, invert, device):
     return host.to(device, non_blocking=True), host
 
 
-def _workspace(L, B, device):
-    n = int(L.smk_warp_workspace_bytes(B))
-    return torch.empty(n, dtype=torch.uint8, device=device), n
+def _workspace(B, device):
+    return torch.empty(_lib.call("smk_warp_workspace_bytes", device, B), dtype=torch.uint8, device=device)
 
 
 def crop_to_tensor(frames, tforms, image_size=224, bgr=True):
@@ -113,15 +112,12 @@ def crop_to_tensor(frames, tforms, image_size=224, bgr=True):
     B, H, W, _ = frames.shape
     if len(tforms) != B:
         raise ValueError("one transform per frame expected")
-    L = _lib.lib()
     out = torch.empty(B, 3, image_size, image_size, dtype=torch.float32, device=frames.device)
     if B == 0:
         return out
-    with torch.cuda.device(frames.device):                 # launches go to the frames' device, not the current one
-        m, _pinned = _matrices(tforms, True, frames.device)
-        ws, n = _workspace(L, B, frames.device)
-        _lib.check(L.smk_crop_warp(frames.data_ptr(), B, H, W, m.data_ptr(), image_size, 1 if bgr else 0, out.data_ptr(),
-                                   ws.data_ptr(), n, _lib.stream_ptr(frames.device)), "smk_crop_warp")
+    m, _pinned = _matrices(tforms, True, frames.device)
+    ws = _workspace(B, frames.device)
+    _lib.call("smk_crop_warp", frames.device, frames, B, H, W, m, image_size, 1 if bgr else 0, out, ws, ws.numel())
     return out
 
 
@@ -136,15 +132,13 @@ def warp_back(rendered, tforms, out_hw):
     H, W = int(out_hw[0]), int(out_hw[1])
     if len(tforms) != B:
         raise ValueError("one transform per frame expected")
-    L = _lib.lib()
-    out = torch.empty(B, H, W, 3, dtype=torch.uint8, device=rendered.device)
+    dev = rendered.device
+    out = torch.empty(B, H, W, 3, dtype=torch.uint8, device=dev)
     if B == 0:
         return out
-    with torch.cuda.device(rendered.device):
-        st = _lib.stream_ptr(rendered.device)
-        u8 = torch.empty(B, S, S, 3, dtype=torch.uint8, device=rendered.device)
-        _lib.check(L.smk_f32chw_to_u8hwc(rendered.data_ptr(), B, S, u8.data_ptr(), st), "smk_f32chw_to_u8hwc")
-        m, _pinned = _matrices(tforms, False, rendered.device)
-        ws, n = _workspace(L, B, rendered.device)
-        _lib.check(L.smk_warp_u8(u8.data_ptr(), B, S, S, m.data_ptr(), H, W, out.data_ptr(), ws.data_ptr(), n, st), "smk_warp_u8")
+    u8 = torch.empty(B, S, S, 3, dtype=torch.uint8, device=dev)
+    _lib.call("smk_f32chw_to_u8hwc", dev, rendered, B, S, u8)
+    m, _pinned = _matrices(tforms, False, dev)
+    ws = _workspace(B, dev)
+    _lib.call("smk_warp_u8", dev, u8, B, S, S, m, H, W, out, ws, ws.numel())
     return out

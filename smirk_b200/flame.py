@@ -5,7 +5,6 @@ output dict; the arithmetic runs in ``csrc/flame.cu`` through ``smk_flame_forwar
 on and a parameter requires grad, ``forward`` is differentiable for shape, expression, pose, jaw, neck,
 eye pose and eyelid parameters (``smk_flame_backward``); otherwise it is the plain forward.
 """
-import ctypes as C
 import pickle
 import sys
 import types
@@ -62,7 +61,7 @@ def _load_flame_pickle(path):
                 sys.modules[k] = v
 
 
-class FLAME(nn.Module):
+class FLAME(_lib.NativeModule, nn.Module):
     def __init__(self, flame_model_path="assets/FLAME2020/generic_model.pkl",
                  flame_lmk_embedding_path="assets/landmark_embedding.npy", n_shape=300, n_exp=50):
         super().__init__()
@@ -102,15 +101,9 @@ class FLAME(nn.Module):
         self.register_buffer("mp_lmk_bary_coords", torch.from_numpy(mp["lmk_b_coords"]).to(self.dtype))
         if self.parents.tolist() != [-1, 0, 1, 1, 1]:
             raise RuntimeError("smirk_b200.FLAME: unsupported kinematic tree %s" % self.parents.tolist())
-        self._handle, self._handle_dev, self._ws, self._bws = None, None, _lib.Workspace(), _lib.Workspace()
 
     # -- native handle (re-packed when a buffer is replaced / edited in place / moved) ---------------
-    def _native(self, device):
-        sig = _lib.buffers_signature(self, device)
-        if self._handle is not None and self._handle_dev == sig:
-            return self._handle
-        self._release()
-        L = _lib.lib()
+    def _native_create(self, device):
         keep = []
 
         def F(x):
@@ -130,24 +123,7 @@ class FLAME(nn.Module):
         d.dyn_faces, d.dyn_bary = I(self.dynamic_lmk_faces_idx), F(self.dynamic_lmk_bary_coords)
         d.n_full, d.full_faces, d.full_bary = self.full_lmk_faces_idx.numel(), I(self.full_lmk_faces_idx), F(self.full_lmk_bary_coords)
         d.n_mp, d.mp_faces, d.mp_bary = self.mp_lmk_faces_idx.numel(), I(self.mp_lmk_faces_idx), F(self.mp_lmk_bary_coords)
-        h = C.c_void_p()
-        with torch.cuda.device(device):
-            _lib.check(L.smk_flame_create(C.byref(d), C.byref(h)), "smk_flame_create")
-        self._handle, self._handle_dev = _lib.NativeHandle(h, "smk_flame_destroy"), sig
-        return self._handle
-
-    def _release(self):
-        self._handle = None                    # the native object dies with its last reference (_lib.NativeHandle)
-
-    def __deepcopy__(self, memo):
-        import copy
-        new = self.__class__.__new__(self.__class__)
-        nn.Module.__init__(new)
-        for k, v in self.__dict__.items():
-            if k not in ("_handle", "_handle_dev", "_ws", "_bws"):
-                new.__dict__[k] = copy.deepcopy(v, memo)
-        new._handle, new._handle_dev, new._ws, new._bws = None, None, _lib.Workspace(), _lib.Workspace()
-        return new
+        return _lib.create("flame", d, device)
 
     # -- forward --------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -155,8 +131,7 @@ class FLAME(nn.Module):
         """betas [B,350], full_pose [B,15], eyelid [B,2]|None -> dict incl. joints and LUT row."""
         dev = betas.device
         _lib.require_cuda(betas, "betas")
-        L = _lib.lib()
-        h = self._native(dev)
+        h = self._native_handle(dev)
         B = betas.shape[0]
         betas, full_pose = _lib.dev_f32(betas, "betas"), _lib.dev_f32(full_pose, "full_pose")
         eyelid = _lib.dev_f32(eyelid, "eyelid_params") if eyelid is not None else None
@@ -165,13 +140,8 @@ class FLAME(nn.Module):
         verts, fan, fan3d, mp = o(B, V, 3), o(B, 68, 3), o(B, self.full_lmk_faces_idx.numel(), 3), o(B, self.mp_lmk_faces_idx.numel(), 3)
         joints = o(B, 5, 3)
         dyn = torch.empty(B, dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            nws = L.smk_flame_workspace_bytes(h, B)
-            ws = self._ws.get(nws, dev)
-            _lib.check(L.smk_flame_forward(h, _lib.ptr(betas), _lib.ptr(full_pose), _lib.ptr(eyelid), B,
-                                           _lib.ptr(verts), _lib.ptr(fan), _lib.ptr(fan3d), _lib.ptr(mp),
-                                           _lib.ptr(joints), _lib.ptr(dyn), _lib.ptr(ws), ws.numel(),
-                                           _lib.stream_ptr(dev)), "smk_flame_forward")
+        ws = self._native_workspace("forward", _lib.call("smk_flame_workspace_bytes", dev, h, B), dev)
+        _lib.call("smk_flame_forward", dev, h, betas, full_pose, eyelid, B, verts, fan, fan3d, mp, joints, dyn, ws, ws.numel())
         return {"vertices": verts, "landmarks_fan": fan, "landmarks_fan_3d": fan3d, "landmarks_mp": mp,
                 "joints": joints, "dyn_idx": dyn}
 
@@ -230,17 +200,12 @@ class _FlameFunction(torch.autograd.Function):
     def backward(ctx, g_verts, g_fan, g_fan3d, g_mp):
         betas, full_pose, dyn = ctx.saved_tensors
         m, dev, B = ctx.module, betas.device, betas.shape[0]
-        L = _lib.lib()
-        h = m._native(dev)
+        h = m._native_handle(dev)
         gs = [None if g is None else g.to(torch.float32).contiguous() for g in (g_verts, g_fan, g_fan3d, g_mp)]
         g_betas = torch.empty_like(betas)
         g_pose = torch.empty_like(full_pose)
         g_eyelid = torch.empty(B, 2, dtype=torch.float32, device=dev) if ctx.has_eyelid else None
-        with torch.cuda.device(dev):
-            ws = m._bws.get(L.smk_flame_backward_workspace_bytes(h, B), dev)
-            _lib.check(L.smk_flame_backward(h, _lib.ptr(betas), _lib.ptr(full_pose), None, B, _lib.ptr(dyn),
-                                            *[_lib.ptr(g) for g in gs], _lib.ptr(g_betas), _lib.ptr(g_pose),
-                                            _lib.ptr(g_eyelid), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev)),
-                       "smk_flame_backward")
+        ws = m._native_workspace("backward", _lib.call("smk_flame_backward_workspace_bytes", dev, h, B), dev)
+        _lib.call("smk_flame_backward", dev, h, betas, full_pose, None, B, dyn, *gs, g_betas, g_pose, g_eyelid, ws, ws.numel())
         return (None, g_betas.to(ctx.dtypes[0]), g_pose.to(ctx.dtypes[1]),
                 g_eyelid.to(ctx.dtypes[2]) if g_eyelid is not None else None)

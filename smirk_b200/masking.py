@@ -4,42 +4,31 @@ Mirrors ``src/utils/masking.py``: ``mesh_based_mask_uniform_faces`` and ``maskin
 arguments and return values.  Random draws (multinomial, rand, randn, bernoulli) are made with torch on the tensors'
 device, exactly where the reference makes them; the deterministic parts run in ``csrc/masking.cu``.
 """
-import ctypes as C
-
 import torch
 
 from . import _lib
 
 
-class SmkMaskingDesc(C.Structure):
-    _fields_ = [("n_verts", C.c_int), ("n_faces", C.c_int), ("faces", C.c_void_p)]
-
-
 class MaskingContext:
-    """Native handle for one mesh topology (the reference passes ``flame.faces_tensor`` on every call)."""
+    """Native handle for one mesh topology on one device (the reference passes ``flame.faces_tensor`` on every call)."""
 
-    def __init__(self, faces, n_verts):
-        f = faces.detach().to("cpu", torch.int32).contiguous()
-        self._faces_host = f
+    def __init__(self, faces, n_verts, device):
+        f, fp = _lib.i32(faces)
         self.n_verts, self.n_faces = int(n_verts), int(f.shape[0])
-        L = _lib.lib()
-        h = C.c_void_p()
-        desc = SmkMaskingDesc(self.n_verts, self.n_faces, f.data_ptr())
-        _lib.check(L.smk_masking_create(C.byref(desc), C.byref(h)), "smk_masking_create")
-        self._h = _lib.NativeHandle(h, "smk_masking_destroy")
+        self.handle = _lib.create("masking", _lib.SmkMaskingDesc(self.n_verts, self.n_faces, fp), device)
 
     def workspace(self, B, S, device):
-        n = int(_lib.lib().smk_masking_workspace_bytes(self._h, B, S))
-        return torch.empty(n, dtype=torch.uint8, device=device), n
+        n = _lib.call("smk_masking_workspace_bytes", device, self.handle, B, S)
+        return torch.empty(n, dtype=torch.uint8, device=device)
 
 
 _CTX = {}
 
 
-def _context(flame_faces, n_verts):
-    key = (flame_faces.data_ptr(), int(flame_faces.shape[0]), int(n_verts))
+def _context(flame_faces, n_verts, device):
+    key = (flame_faces.data_ptr(), int(flame_faces.shape[0]), int(n_verts), device)
     if key not in _CTX:
-        _CTX[key] = MaskingContext(flame_faces, n_verts)
+        _CTX[key] = MaskingContext(flame_faces, n_verts, device)
     return _CTX[key]
 
 
@@ -56,15 +45,13 @@ def face_weights(flame_trans_verts, flame_faces, face_probabilities):
     _lib.require_cuda(flame_trans_verts, "flame_trans_verts")
     tv = flame_trans_verts.float().contiguous()
     B, V = tv.shape[:2]
-    ctx = _context(flame_faces, V)
-    L = _lib.lib()
+    ctx = _context(flame_faces, V, tv.device)
     w = torch.empty(B, ctx.n_faces, dtype=torch.float32, device=tv.device)
     if B == 0:
         return w
-    ws, n = ctx.workspace(B, 224, tv.device)
+    ws = ctx.workspace(B, 224, tv.device)
     bp = face_probabilities.to(tv.device, torch.float32).contiguous()
-    _lib.check(L.smk_masking_face_weights(ctx._h, tv.data_ptr(), bp.data_ptr(), B, w.data_ptr(), ws.data_ptr(), n,
-                                          _lib.stream_ptr(tv.device)), "smk_masking_face_weights")
+    _lib.call("smk_masking_face_weights", tv.device, ctx.handle, tv, bp, B, w, ws, ws.numel())
     return w
 
 
@@ -82,11 +69,10 @@ def mesh_based_mask_uniform_faces(flame_trans_verts, flame_faces, face_probabili
         idx, bary = coords["sampled_faces_indices"], coords["barycentric_coords"]
     idx = idx.to(tv.device, torch.int64).contiguous()
     bary = bary.to(tv.device, torch.float32).contiguous()
-    ctx = _context(flame_faces, V)
+    ctx = _context(flame_faces, V, tv.device)
     npoints = torch.empty(B, idx.shape[1], 2, dtype=torch.int64, device=tv.device)
     if B and idx.shape[1]:
-        _lib.check(_lib.lib().smk_masking_points(ctx._h, tv.data_ptr(), idx.data_ptr(), bary.data_ptr(), B, idx.shape[1], IMAGE_SIZE,
-                                                 npoints.data_ptr(), _lib.stream_ptr(tv.device)), "smk_masking_points")
+        _lib.call("smk_masking_points", tv.device, ctx.handle, tv, idx, bary, B, idx.shape[1], IMAGE_SIZE, npoints)
     return npoints, {"sampled_faces_indices": idx, "barycentric_coords": bary}
 
 
@@ -96,19 +82,17 @@ def masking_from_points(img, mask, npoints, rbound, wr=15, rendered_mask=None, n
     _lib.require_cuda(img, "img")
     img = img.float().contiguous()
     B, _, S, _ = img.shape
-    ctx = _context(flame_faces, n_verts) if flame_faces is not None else next(iter(_CTX.values()))
+    ctx = _context(flame_faces, n_verts, img.device) if flame_faces is not None else next(iter(_CTX.values()))
     out = torch.empty_like(img)
     if B == 0:
         return out
-    P = lambda t: 0 if t is None else t.to(img.device, torch.float32).contiguous().data_ptr()
-    keep = [t.to(img.device, torch.float32).contiguous() if t is not None else None for t in (mask, rendered_mask, noise_mult, random_centres)]
+    hull, rmask, noise, centres = [t.to(img.device, torch.float32).contiguous() if t is not None else None
+                                   for t in (mask, rendered_mask, noise_mult, random_centres)]
     npts = npoints[..., :2].to(img.device, torch.int64).contiguous()      # the reference's npoints may carry a third (z) column
     rb = rbound.to(img.device, torch.int64).contiguous()
-    ws, n = ctx.workspace(B, S, img.device)
-    ptr = lambda t: 0 if t is None else t.data_ptr()
-    _lib.check(_lib.lib().smk_masking_compose(ctx._h, img.data_ptr(), ptr(keep[0]), npts.data_ptr(), rb.data_ptr(), npts.shape[1], 0,
-                                              ptr(keep[1]), ptr(keep[2]), ptr(keep[3]), int(wr), B, S, out.data_ptr(),
-                                              ws.data_ptr(), n, _lib.stream_ptr(img.device)), "smk_masking_compose")
+    ws = ctx.workspace(B, S, img.device)
+    _lib.call("smk_masking_compose", img.device, ctx.handle, img, hull, npts, rb, npts.shape[1], None, rmask, noise, centres,
+              int(wr), B, S, out, ws, ws.numel())
     return out
 
 
@@ -124,10 +108,7 @@ def transfer_pixels(img, points1, points2, rbound=None):
     if B == 0:
         return out
     ws = torch.empty(B * S * S, dtype=torch.int32, device=img.device)
-    with torch.cuda.device(img.device):
-        _lib.check(_lib.lib().smk_masking_transfer_pixels(img.data_ptr(), p1.data_ptr(), p2.data_ptr(), rb.data_ptr() if rb is not None else 0,
-                                                          B, p1.shape[1], S, out.data_ptr(), ws.data_ptr(), ws.numel() * 4,
-                                                          _lib.stream_ptr(img.device)), "smk_masking_transfer_pixels")
+    _lib.call("smk_masking_transfer_pixels", img.device, img, p1, p2, rb, B, p1.shape[1], S, out, ws, ws.numel() * 4)
     return out
 
 
@@ -137,7 +118,7 @@ def masking(img, mask, extra_points, wr=15, rendered_mask=None, extra_noise=True
     _lib.require_cuda(img, "img")
     img = img.float().contiguous()
     B, _, S, _ = img.shape
-    ctx = _context(flame_faces, n_verts) if flame_faces is not None else (next(iter(_CTX.values())) if _CTX else MaskingContext(torch.tensor([[0, 1, 2]]), 3))
+    ctx = _context(flame_faces, n_verts, img.device) if flame_faces is not None else (next(iter(_CTX.values())) if _CTX else MaskingContext(torch.tensor([[0, 1, 2]]), 3, img.device))
     noise = (torch.randn_like(img) * 0.05 + 1) if extra_noise else None
     centres = torch.bernoulli(torch.ones((B, 1, S, S), device=img.device) * random_mask) if random_mask > 0 else None
     f = lambda t: None if t is None else t.to(img.device, torch.float32).contiguous()
@@ -145,15 +126,13 @@ def masking(img, mask, extra_points, wr=15, rendered_mask=None, extra_noise=True
     out = torch.empty_like(img)
     if B == 0:
         return out
-    ptr = lambda t: 0 if t is None else t.data_ptr()
-    with torch.cuda.device(img.device):
-        ws, n = ctx.workspace(B, S, img.device)
-        _lib.check(_lib.lib().smk_masking_compose(ctx._h, img.data_ptr(), hull.data_ptr(), 0, 0, 0, extra.data_ptr(), ptr(rmask), ptr(noise), ptr(centres),
-                                                  int(wr), B, S, out.data_ptr(), ws.data_ptr(), n, _lib.stream_ptr(img.device)), "smk_masking_compose")
+    ws = ctx.workspace(B, S, img.device)
+    _lib.call("smk_masking_compose", img.device, ctx.handle, img, hull, None, None, 0, extra, rmask, noise, centres,
+              int(wr), B, S, out, ws, ws.numel())
     return out
 
 
-class MaskingStage:
+class MaskingStage(_lib.NativeModule):
     """The masking step of the full cycle (``demo.py:138-165``) as one capturable device call:
     ``rendered_img, transformed_vertices, img, hull_mask -> masked_img`` with every random draw made on the device by a
     counter-based generator (``csrc/masking.cu``, Philox4x32-10).  ``rng_state`` = (seed, call counter) lives in device
@@ -170,30 +149,23 @@ class MaskingStage:
         self.ratio_mul, self.wr = float(mask_ratio_mul), int(mask_dilation_radius)
         self.N = int(mask_ratio * mask_ratio_mul * image_size * image_size)
         self.extra_noise, self.p_centre, self.seed = bool(extra_noise), float(random_mask), int(seed)
-        self._ctx, self._dev, self._ws = None, {}, _lib.Workspace()
 
-    def __deepcopy__(self, memo):
-        new = MaskingStage.__new__(MaskingStage)
-        new.__dict__.update(self.__dict__)
-        new._ctx, new._dev, new._ws = None, {}, _lib.Workspace()
-        return new
+    def _native_key(self, device):              # one topology handle, made on the device of the first call
+        return ()
 
-    @property
-    def _handle(self):                          # for SmirkPipeline's keep-alive list
-        return self._ctx
+    def _native_create(self, device):
+        return MaskingContext(self.faces, self.n_verts, device)
 
     def _state(self, device):
-        if self._ctx is None:
-            with torch.cuda.device(device):
-                self._ctx = MaskingContext(self.faces, self.n_verts)
-        if device not in self._dev:
+        ctx, per_device = self._native_handle(device), self._native.per_device
+        if device not in per_device:
             rng = torch.tensor([self.seed, 0], dtype=torch.int64, device=device)
-            self._dev[device] = (self.base_prob_host.to(device), rng)
-        return self._dev[device]
+            per_device[device] = (self.base_prob_host.to(device), rng)
+        return (ctx,) + per_device[device]
 
     def reseed(self, seed, counter=0):
         self.seed = int(seed)
-        for _, rng in self._dev.values():
+        for _, rng in self._native.per_device.values():
             rng.copy_(torch.tensor([self.seed, int(counter)], dtype=torch.int64))
 
     @torch.no_grad()
@@ -205,7 +177,7 @@ class MaskingStage:
         B, S, N = img.shape[0], self.S, self.N
         if tuple(img.shape[1:]) != (3, S, S) or tuple(rend.shape) != tuple(img.shape) or hull.numel() != B * S * S or tuple(tv.shape) != (B, self.n_verts, 3):
             raise RuntimeError("smirk_b200.MaskingStage: expected img/rendered [B,3,%d,%d], hull [B,1,%d,%d], transformed_vertices [B,%d,3]" % (S, S, S, S, self.n_verts))
-        base_prob, rng = self._state(dev)
+        ctx, base_prob, rng = self._state(dev)
         out = torch.empty_like(img)
         dbg = {}
         if debug:
@@ -213,16 +185,11 @@ class MaskingStage:
             f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
             dbg = dict(sampled_faces_indices=i64(B, N), barycentric_coords=f32(B, N, 3), npoints=i64(B, N, 2), rbound=i64(B),
                        noise_mult=f32(B, 3, S, S), random_centres=f32(B, 1, S, S))
-        L = _lib.lib()
-        P = lambda k: _lib.ptr(dbg.get(k))
-        with torch.cuda.device(dev):
-            n = int(L.smk_masking_forward_workspace_bytes(self._ctx._h, B, S, N))
-            ws = self._ws.get(n, dev)
-            _lib.check(L.smk_masking_forward(self._ctx._h, _lib.ptr(img), _lib.ptr(hull), _lib.ptr(tv), _lib.ptr(rend), _lib.ptr(base_prob),
-                                             B, S, N, self.wr, self.ratio_mul, self.p_centre, 1 if self.extra_noise else 0, _lib.ptr(rng),
-                                             _lib.ptr(out), P("sampled_faces_indices"), P("barycentric_coords"), P("npoints"), P("rbound"),
-                                             P("noise_mult"), P("random_centres"), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev)),
-                       "smk_masking_forward")
+        ws = self._native_workspace("forward", _lib.call("smk_masking_forward_workspace_bytes", dev, ctx.handle, B, S, N), dev)
+        _lib.call("smk_masking_forward", dev, ctx.handle, img, hull, tv, rend, base_prob, B, S, N, self.wr, self.ratio_mul,
+                  self.p_centre, 1 if self.extra_noise else 0, rng, out,
+                  *[dbg.get(k) for k in ("sampled_faces_indices", "barycentric_coords", "npoints", "rbound", "noise_mult", "random_centres")],
+                  ws, ws.numel())
         return (out, dbg) if debug else out
 
     __call__ = forward

@@ -83,9 +83,8 @@ class _PeerBuffer:
 
     def __init__(self, nbytes, device):
         import ctypes as C
-        L = _lib.lib()
         ptr, handle = C.c_void_p(), C.create_string_buffer(64)
-        _lib.check(L.smk_peer_alloc(nbytes, C.byref(ptr), handle), "smk_peer_alloc")
+        _lib.call("smk_peer_alloc", device, nbytes, C.byref(ptr), handle)
         self.ptr, self.nbytes, self.handle, self.ptrs, self._mapped = ptr.value, nbytes, handle.raw, [], []
         self.__cuda_array_interface__ = {"shape": (nbytes,), "typestr": "|u1", "data": (self.ptr, False), "version": 2}
         self.local = torch.as_tensor(self, device=device)
@@ -94,13 +93,12 @@ class _PeerBuffer:
         """Open every peer's handle; ``dsts[j]`` = where part j (byte offset ``offsets[j]``) of this rank's shard goes in each
         PEER's buffer (slot ``rank``), starting with the next rank.  The own slot is not a destination: see ``SmirkPipeline.gathered``."""
         import ctypes as C
-        L = _lib.lib()
         for r, h in enumerate(handles):
             if r == rank:
                 self.ptrs.append(self.ptr)
                 continue
             p = C.c_void_p()
-            _lib.check(L.smk_peer_open(h, C.byref(p)), "smk_peer_open")
+            _lib.call("smk_peer_open", self.local.device, h, C.byref(p))
             self._mapped.append(p.value)
             self.ptrs.append(p.value)
         self.local = self.local.view(len(handles), -1)
@@ -113,9 +111,8 @@ class _PeerBuffer:
         # it is left to process teardown (a gather set-up is made once per pipeline; bench.py's two pipelines hold 0.7 + 5.9 GB
         # at 8 GPUs).  A host that re-creates pipelines can call smk_peer_free itself after a barrier.
         try:
-            L = _lib.lib()
             for p in self._mapped:
-                L.smk_peer_close(p)
+                _lib.call("smk_peer_close", self.local.device, p)
             self._mapped = []
         except Exception:
             pass
@@ -192,15 +189,15 @@ class SmirkPipeline:
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
         g = torch.cuda.CUDAGraph()
-        n0 = _lib.lib().smk_launch_count()
+        n0 = _lib.call("smk_launch_count", dev)
         with torch.cuda.graph(g):
             static_out = self.forward(static_in, static_mask, lane)
-        launches = _lib.lib().smk_launch_count() - n0
+        launches = _lib.call("smk_launch_count", dev) - n0
         # The graph holds raw pointers into each module's packed weights (native handle) and workspace: keep both
         # alive for as long as the graph exists, whatever the modules do afterwards (re-pack, grow their workspace
         # for a larger batch, ...).  A workspace that grows allocates a NEW buffer, so graphs of different batch
         # sizes on one lane never alias a freed one.
-        keep = [(m._handle, m._ws.buf) for m in L.modules()]
+        keep = [m.graph_keep_alive() for m in L.modules()]
         rec = dict(graph=g, img=static_in, mask=static_mask, out=static_out, launches=int(launches), keep=keep)
         L.graphs[B] = rec
         return rec
@@ -297,7 +294,7 @@ class SmirkPipeline:
                         L.p2p_stage = torch.empty(shard, dtype=torch.uint8, device=self.device) if pack else None
                     import ctypes as C
                     fan = C.c_void_p()
-                    _lib.check(_lib.lib().smk_peer_fan_create(min(ws, 8), C.byref(fan)), "smk_peer_fan_create")
+                    _lib.call("smk_peer_fan_create", self.device, min(ws, 8), C.byref(fan))
                     self._fan = _lib.NativeHandle(fan, "smk_peer_fan_destroy")
                 torch.cuda.synchronize(self.device)
             except Exception:
@@ -334,12 +331,10 @@ class SmirkPipeline:
                     # its reuse is ordered by this stream (a fan push ends with the stream waiting for every copy).  Releasing
                     # the lane after the pushes instead idles it for their whole duration.
                     L.gathered.record(self._comm)
-                    _lib.check(_lib.lib().smk_peer_fan_push(self._fan, L.p2p.dsts[0], ws - 1, L.p2p_stage.data_ptr(), self._p2p["shard"],
-                                                            self._comm.cuda_stream), "smk_peer_fan_push")
+                    _lib.call("smk_peer_fan_push", self.device, self._fan, L.p2p.dsts[0], ws - 1, L.p2p_stage, self._p2p["shard"])
                 else:
                     for j, (k, n) in enumerate(zip(self._gather_keys, self._p2p["sizes"])):
-                        _lib.check(_lib.lib().smk_peer_fan_push(self._fan, L.p2p.dsts[j], ws - 1, rec["out"][k].data_ptr(), n,
-                                                                self._comm.cuda_stream), "smk_peer_fan_push")
+                        _lib.call("smk_peer_fan_push", self.device, self._fan, L.p2p.dsts[j], ws - 1, rec["out"][k], n)
                     L.gathered.record(self._comm)
             return
         with torch.cuda.stream(self._comm):

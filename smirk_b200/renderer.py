@@ -7,7 +7,6 @@ normals, rasterisation (pytorch3d's ``rasterize_meshes`` in the reference) and s
 ``forward`` is differentiable for the vertices, the camera and the landmark sets (``smk_renderer_backward``,
 ``smk_project_points_backward``); otherwise it is the plain forward.
 """
-import ctypes as C
 import pickle
 
 import numpy as np
@@ -50,7 +49,7 @@ def _face_vertices(vertices, faces):
     return vertices.reshape(bs * nv, -1)[(faces + (torch.arange(bs) * nv)[:, None, None]).long()]
 
 
-class Renderer(nn.Module):
+class Renderer(_lib.NativeModule, nn.Module):
     def __init__(self, render_full_head=False, obj_filename="assets/head_template.obj"):
         super().__init__()
         self.image_size = 224
@@ -82,37 +81,17 @@ class Renderer(nn.Module):
              ((2 * pi) / 3) * (np.sqrt(3 / (4 * pi))), (pi / 4) * (3) * (np.sqrt(5 / (12 * pi))),
              (pi / 4) * (3) * (np.sqrt(5 / (12 * pi))), (pi / 4) * (3) * (np.sqrt(5 / (12 * pi))),
              (pi / 4) * (3 / 2) * (np.sqrt(5 / (12 * pi))), (pi / 4) * (1 / 2) * (np.sqrt(5 / (4 * pi)))]).float())
-        self._handle, self._handle_dev, self._ws, self._bws = None, None, _lib.Workspace(), _lib.Workspace()
 
-    def _native(self, device):
-        sig = (str(device), self.faces._version, self.faces.data_ptr(), self.image_size)
-        if self._handle is not None and self._handle_dev == sig:
-            return self._handle
-        self._release()
-        L = _lib.lib()
+    def _native_key(self, device):              # the handle packs only the topology and the image size
+        return str(device), self.faces._version, self.faces.data_ptr(), self.image_size
+
+    def _native_create(self, device):
         mask_np, mask_p = _lib.i32(np.asarray(self.final_mask))
         faces_np, faces_p = _lib.i32(self.faces[0])
         d = _lib.SmkRendererDesc()
         d.n_verts, d.n_mask, d.mask_ids = self.n_verts, len(self.final_mask), mask_p
         d.n_faces, d.faces, d.image_size = faces_np.shape[0], faces_p, self.image_size
-        h = C.c_void_p()
-        with torch.cuda.device(device):
-            _lib.check(L.smk_renderer_create(C.byref(d), C.byref(h)), "smk_renderer_create")
-        self._handle, self._handle_dev = _lib.NativeHandle(h, "smk_renderer_destroy"), sig
-        return self._handle
-
-    def _release(self):
-        self._handle = None                    # the native object dies with its last reference (_lib.NativeHandle)
-
-    def __deepcopy__(self, memo):
-        import copy
-        new = self.__class__.__new__(self.__class__)
-        nn.Module.__init__(new)
-        for k, v in self.__dict__.items():
-            if k not in ("_handle", "_handle_dev", "_ws", "_bws"):
-                new.__dict__[k] = copy.deepcopy(v, memo)
-        new._handle, new._handle_dev, new._ws, new._bws = None, None, _lib.Workspace(), _lib.Workspace()
-        return new
+        return _lib.create("renderer", d, device)
 
     def forward(self, vertices, cam_params, **landmarks):
         if torch.is_grad_enabled() and any(torch.is_tensor(t) and t.requires_grad
@@ -137,8 +116,7 @@ class Renderer(nn.Module):
         packed like pytorch3d, bary [B,S,S,3], zbuf [B,S,S]) and the vertex normals [B,n_mask,3]."""
         _lib.require_cuda(vertices, "vertices")
         dev = vertices.device
-        L = _lib.lib()
-        h = self._native(dev)
+        h = self._native_handle(dev)
         verts, cam = _lib.dev_f32(vertices, "vertices"), _lib.dev_f32(cam_params, "cam_params")
         B, S = verts.shape[0], self.image_size
         if verts.shape[1] != self.n_verts or cam.shape != (B, 3):
@@ -149,18 +127,13 @@ class Renderer(nn.Module):
         bary, zbuf = (o(B, S, S, 3), o(B, S, S)) if raw else (None, None)
         normals = o(B, len(self.final_mask), 3) if raw else None
         out = {"rendered_img": rendered, "transformed_vertices": tverts}
-        with torch.cuda.device(dev):
-            st = _lib.stream_ptr(dev)
-            ws = self._ws.get(L.smk_renderer_workspace_bytes(h, B), dev)
-            _lib.check(L.smk_renderer_forward(h, _lib.ptr(verts), _lib.ptr(cam), B, _lib.ptr(rendered), _lib.ptr(tverts),
-                                              _lib.ptr(p2f), _lib.ptr(bary), _lib.ptr(zbuf), _lib.ptr(normals),
-                                              _lib.ptr(ws), ws.numel(), st), "smk_renderer_forward")
-            for k, pts in landmarks.items():                                     # renderer.py:104-108
-                pts = _lib.dev_f32(pts, k)
-                xy = o(B, pts.shape[1], 2)
-                _lib.check(L.smk_project_points(_lib.ptr(pts), _lib.ptr(cam), B, pts.shape[1], _lib.ptr(xy), st),
-                           "smk_project_points")
-                out[k] = xy
+        ws = self._native_workspace("forward", _lib.call("smk_renderer_workspace_bytes", dev, h, B), dev)
+        _lib.call("smk_renderer_forward", dev, h, verts, cam, B, rendered, tverts, p2f, bary, zbuf, normals, ws, ws.numel())
+        for k, pts in landmarks.items():                                         # renderer.py:104-108
+            pts = _lib.dev_f32(pts, k)
+            xy = o(B, pts.shape[1], 2)
+            _lib.call("smk_project_points", dev, pts, cam, B, pts.shape[1], xy)
+            out[k] = xy
         if self.render_full_head:
             # renderer.py:140-144: with the full head the fancy-index is skipped, so the in-place `z += 10` of render()
             # also lands in the tensor the reference returns as `transformed_vertices`
@@ -191,16 +164,12 @@ class _RenderFunction(torch.autograd.Function):
     def backward(ctx, g_rendered, g_tverts):
         verts, cam, p2f, bary, normals = ctx.saved_tensors
         m, dev, B = ctx.module, verts.device, verts.shape[0]
-        L = _lib.lib()
-        h = m._native(dev)
+        h = m._native_handle(dev)
         g_verts, g_cam = torch.empty_like(verts), torch.empty_like(cam)
         g_rendered, g_tverts = _grad_f32(g_rendered), _grad_f32(g_tverts)
-        with torch.cuda.device(dev):
-            ws = m._bws.get(L.smk_renderer_backward_workspace_bytes(h, B), dev)
-            _lib.check(L.smk_renderer_backward(h, _lib.ptr(verts), _lib.ptr(cam), B, _lib.ptr(p2f), _lib.ptr(bary),
-                                               _lib.ptr(normals), _lib.ptr(g_rendered), _lib.ptr(g_tverts),
-                                               _lib.ptr(g_verts), _lib.ptr(g_cam), _lib.ptr(ws), ws.numel(),
-                                               _lib.stream_ptr(dev)), "smk_renderer_backward")
+        ws = m._native_workspace("backward", _lib.call("smk_renderer_backward_workspace_bytes", dev, h, B), dev)
+        _lib.call("smk_renderer_backward", dev, h, verts, cam, B, p2f, bary, normals, g_rendered, g_tverts, g_verts, g_cam,
+                  ws, ws.numel())
         return None, g_verts.to(ctx.dtypes[0]), g_cam.to(ctx.dtypes[1])
 
 
@@ -212,9 +181,7 @@ class _ProjectFunction(torch.autograd.Function):
         p, c = _lib.dev_f32(pts, "landmarks"), _lib.dev_f32(cam, "cam_params")
         B, n = p.shape[0], p.shape[1]
         xy = torch.empty(B, n, 2, dtype=torch.float32, device=p.device)
-        with torch.cuda.device(p.device):
-            _lib.check(_lib.lib().smk_project_points(_lib.ptr(p), _lib.ptr(c), B, n, _lib.ptr(xy),
-                                                     _lib.stream_ptr(p.device)), "smk_project_points")
+        _lib.call("smk_project_points", p.device, p, c, B, n, xy)
         ctx.dtypes = (pts.dtype, cam.dtype)
         ctx.save_for_backward(p, c)
         return xy
@@ -225,8 +192,5 @@ class _ProjectFunction(torch.autograd.Function):
         p, c = ctx.saved_tensors
         B, n = p.shape[0], p.shape[1]
         g_pts, g_cam, g_xy = torch.empty_like(p), torch.empty_like(c), _grad_f32(g_xy)
-        with torch.cuda.device(p.device):
-            _lib.check(_lib.lib().smk_project_points_backward(_lib.ptr(p), _lib.ptr(c), B, n, _lib.ptr(g_xy),
-                                                              _lib.ptr(g_pts), _lib.ptr(g_cam), _lib.stream_ptr(p.device)),
-                       "smk_project_points_backward")
+        _lib.call("smk_project_points_backward", p.device, p, c, B, n, g_xy, g_pts, g_cam)
         return g_pts.to(ctx.dtypes[0]), g_cam.to(ctx.dtypes[1])

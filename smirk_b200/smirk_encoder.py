@@ -107,7 +107,7 @@ def create_backbone(backbone_name, pretrained=True):
     return bb, bb.feature_dim
 
 
-class _NativeEncoder(nn.Module):
+class _NativeEncoder(_lib.NativeModule, nn.Module):
     """Shared machinery of SmirkEncoder and its three sub-encoders: a native handle over the backbones returned by
     ``_parts()`` (slot 0 = pose / small, 1 = shape / large, 2 = expression / large; None = not part of this module),
     re-packed whenever a parameter / buffer is modified or moved, and the raw forward through the C ABI.
@@ -118,17 +118,14 @@ class _NativeEncoder(nn.Module):
     def _init_native(self, n_exp=50, n_shape=300):
         self.n_exp, self.n_shape = n_exp, n_shape
         self.precision = 0
-        self._handle, self._sig, self._ws = None, None, _lib.Workspace()
 
     def _parts(self):
         raise NotImplementedError
 
-    def _native(self, device):
-        sig = _lib.buffers_signature(self, device, self.precision)
-        if self._handle is not None and self._sig == sig:
-            return self._handle
-        self._release()
-        L = _lib.lib()
+    def _native_extras(self):
+        return (self.precision,)
+
+    def _native_create(self, device):
         keep = []
         d = _lib.SmkEncoderDesc()
         for i, part in enumerate(self._parts()):
@@ -148,24 +145,7 @@ class _NativeEncoder(nn.Module):
             a, p = _lib.f32(head.weight); keep.append(a); d.head_w[i] = p
             a, p = _lib.f32(head.bias); keep.append(a); d.head_b[i] = p
         d.n_shape, d.n_exp, d.precision = self.n_shape, self.n_exp, int(self.precision)
-        h = C.c_void_p()
-        with torch.cuda.device(device):
-            _lib.check(L.smk_encoder_create(C.byref(d), C.byref(h)), "smk_encoder_create")
-        self._handle, self._sig = _lib.NativeHandle(h, "smk_encoder_destroy"), sig
-        return self._handle
-
-    def _release(self):
-        self._handle = None                    # the native object dies with its last reference (_lib.NativeHandle)
-
-    def __deepcopy__(self, memo):               # base_trainer.py:237 deep-copies the encoder
-        import copy
-        new = self.__class__.__new__(self.__class__)
-        nn.Module.__init__(new)
-        for k, v in self.__dict__.items():
-            if k not in ("_handle", "_sig", "_ws"):
-                new.__dict__[k] = copy.deepcopy(v, memo)
-        new._handle, new._sig, new._ws = None, None, _lib.Workspace()
-        return new
+        return _lib.create("encoder", d, device)
 
     @torch.no_grad()
     def _run(self, img):
@@ -174,8 +154,7 @@ class _NativeEncoder(nn.Module):
         if self.training:                      # checked on every call: .train() after the first forward must not silently run eval BN
             raise RuntimeError("smirk_b200.%s: train-mode BatchNorm is not implemented (forward/eval only)" % type(self).__name__)
         dev = img.device
-        L = _lib.lib()
-        h = self._native(dev)
+        h = self._native_handle(dev)
         x = _lib.dev_f32(img, "img")
         if x.dim() != 4 or tuple(x.shape[1:]) != (3, 224, 224):
             raise RuntimeError("smirk_b200.%s: expected img [B,3,224,224], got %s" % (type(self).__name__, tuple(x.shape)))
@@ -183,10 +162,8 @@ class _NativeEncoder(nn.Module):
         widths = (6, self.n_shape, self.n_exp + 5)
         outs = [torch.empty(B, w, dtype=torch.float32, device=dev) if part is not None else None
                 for w, part in zip(widths, self._parts())]
-        with torch.cuda.device(dev):
-            ws = self._ws.get(L.smk_encoder_workspace_bytes(h, B), dev)
-            _lib.check(L.smk_encoder_forward(h, _lib.ptr(x), B, _lib.ptr(outs[0]), _lib.ptr(outs[1]), _lib.ptr(outs[2]),
-                                             _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev)), "smk_encoder_forward")
+        ws = self._native_workspace("forward", _lib.call("smk_encoder_workspace_bytes", dev, h, B), dev)
+        _lib.call("smk_encoder_forward", dev, h, x, B, *outs, ws, ws.numel())
         return outs
 
 

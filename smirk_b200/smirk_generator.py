@@ -25,7 +25,7 @@ class ResnetBlock(nn.Module):
             nn.ReflectionPad2d(1), nn.Conv2d(dim, dim, 3, padding=0, bias=use_bias), norm_layer(dim))
 
 
-class SmirkGenerator(nn.Module):
+class SmirkGenerator(_lib.NativeModule, nn.Module):
     def __init__(self, in_channels=3, out_channels=1, init_features=16, res_blocks=3):
         super().__init__()
         f = init_features
@@ -50,7 +50,6 @@ class SmirkGenerator(nn.Module):
         self.conv = nn.Conv2d(in_channels=f, out_channels=out_channels, kernel_size=1)
         self._cfg = (in_channels, out_channels, init_features, res_blocks)
         self.precision = 0
-        self._handle, self._sig, self._ws = None, None, _lib.Workspace()
 
     @staticmethod
     def _block(in_channels, features, name):
@@ -63,19 +62,10 @@ class SmirkGenerator(nn.Module):
             (name + "relu2", nn.ReLU(inplace=True)),
         ]))
 
-    def _signature(self, device):
-        s = [str(device), self.precision]
-        for t in list(self.parameters()) + list(self.buffers()):
-            s.append(t._version)
-            s.append(t.data_ptr())
-        return tuple(s)
+    def _native_extras(self):
+        return (self.precision,)
 
-    def _native(self, device):
-        sig = self._signature(device)
-        if self._handle is not None and self._sig == sig:
-            return self._handle
-        self._release()
-        L = _lib.lib()
+    def _native_create(self, device):
         keep = []
         ts = [v for k, v in self.state_dict().items() if not k.endswith("num_batches_tracked")]
         arr = (_lib.c_f32p * len(ts))()
@@ -86,24 +76,7 @@ class SmirkGenerator(nn.Module):
         d = _lib.SmkGeneratorDesc()
         d.in_channels, d.out_channels, d.init_features, d.res_blocks = self._cfg
         d.tensors, d.n_tensors, d.precision = C.cast(arr, C.POINTER(_lib.c_f32p)), len(ts), self.precision
-        h = C.c_void_p()
-        with torch.cuda.device(device):
-            _lib.check(L.smk_generator_create(C.byref(d), C.byref(h)), "smk_generator_create")
-        self._handle, self._sig = _lib.NativeHandle(h, "smk_generator_destroy"), sig
-        return self._handle
-
-    def _release(self):
-        self._handle = None                    # the native object dies with its last reference (_lib.NativeHandle)
-
-    def __deepcopy__(self, memo):
-        import copy
-        new = self.__class__.__new__(self.__class__)
-        nn.Module.__init__(new)
-        for k, v in self.__dict__.items():
-            if k not in ("_handle", "_sig", "_ws"):
-                new.__dict__[k] = copy.deepcopy(v, memo)
-        new._handle, new._sig, new._ws = None, None, _lib.Workspace()
-        return new
+        return _lib.create("generator", d, device)
 
     @torch.no_grad()
     def forward(self, x):
@@ -111,16 +84,13 @@ class SmirkGenerator(nn.Module):
         if self.training:                      # checked on every call: .train() after the first forward must not silently run eval BN
             raise RuntimeError("smirk_b200.SmirkGenerator: train-mode BatchNorm is not implemented (forward/eval only)")
         dev = x.device
-        L = _lib.lib()
-        h = self._native(dev)
+        h = self._native_handle(dev)
         x = _lib.dev_f32(x, "x")
         cin, cout = self._cfg[0], self._cfg[1]
         if x.dim() != 4 or tuple(x.shape[1:]) != (cin, 224, 224):
             raise RuntimeError("smirk_b200.SmirkGenerator: expected x [B,%d,224,224], got %s" % (cin, tuple(x.shape)))
         B = x.shape[0]
         y = torch.empty(B, cout, 224, 224, dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            ws = self._ws.get(L.smk_generator_workspace_bytes(h, B), dev)
-            _lib.check(L.smk_generator_forward(h, _lib.ptr(x), B, _lib.ptr(y), _lib.ptr(ws), ws.numel(),
-                                               _lib.stream_ptr(dev)), "smk_generator_forward")
+        ws = self._native_workspace("forward", _lib.call("smk_generator_workspace_bytes", dev, h, B), dev)
+        _lib.call("smk_generator_forward", dev, h, x, B, y, ws, ws.numel())
         return y

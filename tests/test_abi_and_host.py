@@ -1,6 +1,6 @@
-"""CPU suite: the C-ABI library loads and exports every symbol include/smirk_b200.h declares, the
-reference-compatible modules construct with the reference's state_dict keys, and the product path
-fails loudly (no CPU fallback)."""
+"""CPU suite: the C-ABI library loads and exports every symbol include/smirk_b200.h declares, the ctypes binding
+table matches the header, the reference-compatible modules construct with the reference's state_dict keys, and the
+product path fails loudly (no CPU fallback)."""
 import copy
 import os
 import re
@@ -11,16 +11,36 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_library_exports_every_declared_symbol(native_lib):
+def test_library_exports_and_binds_every_declared_symbol(native_lib):
+    """The library exports every prototype in include/smirk_b200.h, and each has one row in _lib.BINDINGS with the same
+    return type and the same parameters: count, pointer / value kind, and the trailing stream where the header has one."""
+    import ctypes as C
+    from smirk_b200 import _lib
     hdr = open(os.path.join(ROOT, "include", "smirk_b200.h")).read()
     hdr = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
     declared = set(re.findall(r"\b(smk_[a-z_0-9]+)\s*\(", hdr))
     assert len(declared) >= 19
     for name in sorted(declared):
         assert hasattr(native_lib, name), "missing export: " + name
-    from smirk_b200 import _lib
-    assert set(_lib.SYMBOLS) == declared
     assert native_lib.smk_version() == 100
+    protos = re.findall(r"^\s*([A-Za-z_][\w ]*?\**)\s*\b(smk_\w+)\s*\(([^)]*)\)\s*;", hdr, flags=re.M)
+    table = {name: (restype, args) for name, restype, args in _lib.BINDINGS}
+    assert len(protos) == 57 and len(table) == len(_lib.BINDINGS)
+    assert {name for _, name, _ in protos} == set(table)
+    returns = {"int": C.c_int, "size_t": C.c_size_t, "void": None, "const char*": C.c_char_p, "unsigned long long": C.c_ulonglong}
+    values = {"int": C.c_int, "size_t": C.c_size_t, "float": C.c_float}
+    for ret, name, params in protos:
+        restype, args = table[name]
+        assert restype is returns[ret.strip()], name
+        params = [q.strip() for q in params.split(",") if q.strip() not in ("", "void")]
+        assert len(args) == len(params), name
+        for q, a in zip(params, args):
+            if q.endswith("stream"):
+                assert a is _lib.STREAM, (name, q)
+            elif "*" in q:
+                assert a in (C.c_void_p, C.c_char_p) or issubclass(a, C._Pointer), (name, q)
+            else:
+                assert a is values[q.rsplit(None, 1)[0]], (name, q)
 
 
 def test_create_rejects_bad_arguments_without_gpu(native_lib):
@@ -57,7 +77,16 @@ def test_modules_construct_with_reference_keys(asset_root):
     gk = list(gen.state_dict())
     assert len(gk) == 178 and gk[0] == "encoder1.enc1conv1.weight" and "resnet_blocks.4.conv_block.6.running_var" in gk
     assert gen.upconv4.weight.shape == (512, 256, 2, 2)
-    copy.deepcopy(enc)                                                          # base_trainer.py:237
+    from smirk_b200.masking import MaskingStage
+    stage = MaskingStage(fl.faces_tensor, torch.ones(fl.faces_tensor.shape[0]))
+    for m in (enc, fl, rd, gen, stage):                                         # base_trainer.py:237 deep-copies the encoder
+        m._native.handle = handle = object()                                    # stands in for a packed native handle
+        c = copy.deepcopy(m)
+        assert "_native_state" not in c.__dict__, type(m).__name__
+        assert c._native is not m._native and c._native.handle is None and m._native.handle is handle
+        if isinstance(m, torch.nn.Module):
+            for a, b in zip(m.state_dict().values(), c.state_dict().values()):
+                assert torch.equal(a, b) and (a.numel() == 0 or a.data_ptr() != b.data_ptr())
     assert len(list(enc.pose_encoder.parameters())) > 0
 
 

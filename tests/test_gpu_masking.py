@@ -70,6 +70,28 @@ def test_compose_matches_reference(native_lib, g, faces):
     assert torch.equal(out, ref)
 
 
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs")
+def test_free_functions_launch_on_the_tensors_device(native_lib, g, faces):
+    """face_weights, mesh_based_mask_uniform_faces and masking_from_points run on their tensors' device, not the current
+    one: on cuda:1 tensors while cuda:0 is current they return what the same calls return on cuda:0."""
+    from smirk_b200 import masking
+    tv, bp = T(g["trans_verts"]), T(g["base_prob"])
+    coords = {"sampled_faces_indices": T(g["sampled_faces_indices"], torch.long), "barycentric_coords": T(g["barycentric_coords"])}
+    npoints, rbound = T(g["npoints"], torch.long), T(g["rbound"])
+    img, hull = synth_inputs.images(npoints.shape[0], int(g["seeds"][2])), T(g["hull"], torch.float32)
+
+    def run(dev):
+        w = masking.face_weights(tv.to(dev), faces, bp)
+        pts, _ = masking.mesh_based_mask_uniform_faces(tv.to(dev), faces, bp, mask_ratio=0.05, coords=coords)
+        out = masking.masking_from_points(img.to(dev), hull, npoints, rbound, wr=10, flame_faces=faces)
+        return [t.cpu() for t in (w, pts, out)]
+
+    with torch.cuda.device(0):
+        on0, on1 = run("cuda:0"), run("cuda:1")
+    for a, b in zip(on0, on1):
+        assert torch.equal(a, b)
+
+
 # ------------------------------------------------------------------------------ MaskingStage: draws made on the device
 def _stage(g, faces, **kw):
     from smirk_b200 import masking

@@ -425,7 +425,7 @@ def test_encoder_and_generator_at_batch_256(mods, encoder, generator, asset_root
 
 
 # ----------------------------------------------------------------------- graph lifetime, sub-encoders, masking in the pipeline
-def test_graphs_of_different_batch_sizes_keep_their_own_workspaces(mods, encoder):
+def test_graphs_of_different_batch_sizes_keep_their_workspaces_alive(mods, encoder):
     """ADVICE r1 (medium): capture B = 2, then B = 8 (the module workspaces grow -> new buffers), then re-pack the
     encoder; the B = 2 graph must still replay correctly: it keeps the workspace and the packed weights it was recorded
     with alive (rec['keep'])."""
@@ -439,10 +439,10 @@ def test_graphs_of_different_batch_sizes_keep_their_own_workspaces(mods, encoder
     x2, x8 = synth_inputs.images(2, 801).to(DEV), synth_inputs.images(8, 802).to(DEV)
     eager2 = {k: v.clone() for k, v in pipe.forward(x2).items()}
     pipe.capture(2)
-    ws_before = enc._ws.buf.data_ptr()
+    ws_before = enc.graph_keep_alive()[1].data_ptr()
     eager8 = {k: v.clone() for k, v in pipe.forward(x8).items()}
     pipe.capture(8)
-    assert enc._ws.buf.data_ptr() != ws_before, "the workspace was expected to grow into a new buffer"
+    assert enc.graph_keep_alive()[1].data_ptr() != ws_before, "the workspace was expected to grow into a new buffer"
     with torch.no_grad():
         enc.shape_encoder.shape_layers[0].bias += 0.0           # bumps the version: the next eager forward re-packs the weights
     pipe.forward(x8)
