@@ -302,4 +302,8 @@ int smk_debug_stem_ds(const float* img, int B, int H, int W, const float* stem_w
 #ifdef __cplusplus
 }
 #endif
+
+/* The generator's input-gradient entry points. */
+#include "smirk_b200_grad.h"
+
 #endif /* SMIRK_B200_H */

@@ -114,7 +114,15 @@ BINDINGS = [
     ("smk_debug_xdw3x", _i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _vp, STREAM]),
     ("smk_debug_stem_ds", _i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, STREAM]),
 ]
-_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS if args[-1:] == [STREAM])
+# The same for include/smirk_b200_grad.h (the generator's input gradient), which smirk_b200.h includes at its end.
+GRAD_BINDINGS = [
+    ("smk_generator_saved_bytes", _sz, [_vp, _i]),
+    ("smk_generator_forward_saved", _i, [_vp, _vp, _i, _vp, _vp, _sz, _vp, _sz, STREAM]),
+    ("smk_generator_saved_tensor", _i, [_vp, _i, _i, C.POINTER(C.c_char_p), C.POINTER(_sz), C.POINTER(C.c_int)]),
+    ("smk_generator_backward_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_generator_backward", _i, [_vp, _i, _vp, _vp, _sz, _vp, _vp, _vp, _sz, STREAM]),
+]
+_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS + GRAD_BINDINGS if args[-1:] == [STREAM])
 
 
 def lib():
@@ -126,7 +134,7 @@ def lib():
         raise RuntimeError("smirk_b200: %s not found — build it with `python -m smirk_b200.build` "
                            "(there is no CPU / PyTorch fallback)" % LIB_PATH)
     L = C.CDLL(LIB_PATH)
-    for name, restype, argtypes in BINDINGS:
+    for name, restype, argtypes in BINDINGS + GRAD_BINDINGS:
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, [_vp if a is STREAM else a for a in argtypes]
     if L.smk_version() != 100:

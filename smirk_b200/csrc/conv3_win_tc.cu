@@ -50,12 +50,16 @@ struct WinArgs {
     float* out; int ld_out;
     int store;                   // 0 plain NHWC, 3 fused 1x1 head + sigmoid (NCHW)
     const float* head_w; const float* head_b; int head_c;
+    const float* mask; int ld_mask;   // store 0: zero outputs whose mask[pixel, n] <= 0 (ReLU backward)
+    float* out2; int ld_out2;         // the stored activations again, compact NHWC (store 3: the activations it does not store)
 };
 
 // RES = true : the layer's whole weight matrix stays in shared memory, shared by both pipelines (<= 72 KB);
 // RES = false: each pipeline streams the (chunk, tap) weight boxes through its own NB-deep ring (the 112^2 Cout-64 layers with
 //              147 - 295 KB of weights): the input window is still loaded once per chunk instead of nine times.
-template <int BN, bool RES>
+// EXTRA = true: the epilogue also applies `mask` and writes `out2` (backward / grad-mode forward); the forward-only
+//               instantiations are compiled without them.
+template <int BN, bool RES, bool EXTRA>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv3_win_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, const WinArgs a) {
     constexpr int B_BYTES = BN * 128;                      // one (chunk, tap) weight box
@@ -201,7 +205,7 @@ conv3_win_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
 #pragma unroll
                         for (int j = 0; j < 8; ++j) {
                             const float4 x4 = slab_chunk(slab, lane, j);
-                            const float xs[4] = {x4.x, x4.y, x4.z, x4.w};
+                            float xs[4] = {x4.x, x4.y, x4.z, x4.w};
 #pragma unroll
                             for (int e = 0; e < 4; ++e) {
                                 const int nn = 4 * j + e;
@@ -209,8 +213,11 @@ conv3_win_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
                                 const float2 p1 = *reinterpret_cast<const float2*>(hpar + nn * 8 + 4);
                                 float x = fmaf(xs[e], p0.x, p0.y);
                                 if (a.relu) x = fmaxf(x, 0.f);
+                                xs[e] = x;
                                 a0 = fmaf(x, p0.z, a0); a1 = fmaf(x, p0.w, a1); a2 = fmaf(x, p1.x, a2); a3 = fmaf(x, p1.y, a3);
                             }
+                            if (EXTRA && a.out2)
+                                *reinterpret_cast<float4*>(a.out2 + ((size_t)(img * a.H + oh) * a.W + ow) * a.ld_out2 + 4 * j) = make_float4(xs[0], xs[1], xs[2], xs[3]);
                         }
                         const int hw_px = a.H * a.W;
                         float* dst = a.out + (size_t)img * a.head_c * hw_px + (size_t)oh * a.W + ow;
@@ -236,8 +243,14 @@ conv3_win_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
                         float4 o;
                         o.x = fmaf(x.x, sc.x, bi.x); o.y = fmaf(x.y, sc.y, bi.y); o.z = fmaf(x.z, sc.z, bi.z); o.w = fmaf(x.w, sc.w, bi.w);
                         if (a.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
+                        const size_t pix = (size_t)(img * a.H + oh) * a.W + ow;
+                        if (EXTRA && a.mask) {
+                            const float4 k4 = __ldg(reinterpret_cast<const float4*>(a.mask + pix * a.ld_mask + nc));
+                            o.x = k4.x > 0.f ? o.x : 0.f; o.y = k4.y > 0.f ? o.y : 0.f; o.z = k4.z > 0.f ? o.z : 0.f; o.w = k4.w > 0.f ? o.w : 0.f;
+                        }
                         if (a.round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
-                        *reinterpret_cast<float4*>(a.out + ((size_t)(img * a.H + oh) * a.W + ow) * a.ld_out + nc) = o;
+                        *reinterpret_cast<float4*>(a.out + pix * a.ld_out + nc) = o;
+                        if (EXTRA && a.out2) *reinterpret_cast<float4*>(a.out2 + pix * a.ld_out2 + nc) = o;
                     }
                 }
                 __syncwarp();
@@ -251,20 +264,26 @@ size_t win_smem_bytes(int nchunks, int BN, bool res) {
 }
 bool win_resident(int nchunks, int BN) { return win_smem_bytes(nchunks, BN, true) <= 227 * 1024; }
 
-template <int BN, bool RES>
-int launch(const CUtensorMap& tmX, const CUtensorMap& tmW, const WinArgs& a, cudaStream_t st) {
+template <int BN, bool RES, bool EXTRA>
+int launch_kernel(const CUtensorMap& tmX, const CUtensorMap& tmW, const WinArgs& a, cudaStream_t st) {
     const size_t smem = win_smem_bytes(a.nchunks, BN, RES);
     SMK_REQUIRE(smem <= 227 * 1024, "conv3_win: shared-memory budget exceeded (%zu bytes)", smem);
-    SMK_CHECK_CUDA((set_max_dynamic_smem<conv3_win_kernel<BN, RES>>(227 * 1024)));
-    SMK_LAUNCH((conv3_win_kernel<BN, RES>), dim3((unsigned)std::min(cdiv(a.n_tiles, PIPES), num_sms())), dim3(NUM_THREADS), smem, st, tmX, tmW, a);
+    SMK_CHECK_CUDA((set_max_dynamic_smem<conv3_win_kernel<BN, RES, EXTRA>>(227 * 1024)));
+    SMK_LAUNCH((conv3_win_kernel<BN, RES, EXTRA>), dim3((unsigned)std::min(cdiv(a.n_tiles, PIPES), num_sms())), dim3(NUM_THREADS), smem, st, tmX, tmW, a);
     SMK_CHECK_LAUNCH();
     return 0;
+}
+
+template <int BN, bool RES>
+int launch(const CUtensorMap& tmX, const CUtensorMap& tmW, const WinArgs& a, cudaStream_t st) {
+    if (a.mask || a.out2) return launch_kernel<BN, RES, true>(tmX, tmW, a, st);
+    return launch_kernel<BN, RES, false>(tmX, tmW, a, st);
 }
 
 }  // namespace
 
 bool conv3_win_supported(const TcConv& p) {
-    if (p.mode != 1 || p.res || p.wt_lo || (p.store != 0 && p.store != 3) || (p.store == 3 && p.N != 32)) return false;
+    if (p.mode != 1 || p.res || p.wt_lo || (p.store != 0 && p.store != 3) || (p.store == 3 && (p.N != 32 || p.mask))) return false;
     if (p.Cin % 32 != 0 || p.K != 9 * p.Cin || (p.N != 32 && p.N != 64)) return false;
     return p.W >= 56;                                             // low-resolution layers are MMA-bound: gemm_tc's wide tiles win there
 }
@@ -283,11 +302,13 @@ int conv3_win(const TcConv& p, cudaStream_t st) {
     a.tiles_x = cdiv(p.W, TW); a.tiles_y = cdiv(p.H, TH); a.n_tiles = a.tiles_x * a.tiles_y * p.B;
     a.scale = p.scale; a.bias = p.bias; a.relu = p.relu; a.round_out = p.round_out;
     a.out = p.out; a.ld_out = p.ld_out; a.store = p.store; a.head_w = p.head_w; a.head_b = p.head_b; a.head_c = p.head_c;
+    a.mask = p.mask; a.ld_mask = p.ld_mask; a.out2 = p.out2; a.ld_out2 = p.ld_out2;
     {
         const double M = (double)p.B * p.H * p.W;
-        const char* tag = p.store == 3 ? "conv3x3_win_head_tc" : "conv3x3_win_tc";
+        const char* tag = p.tag ? p.tag : p.store == 3 ? "conv3x3_win_head_tc" : "conv3x3_win_tc";
         if (g_prof_detail) tag = prof_shape_tag(tag, (long)M, p.K, p.N);
-        SMK_TAG(tag, 4.0 * (M * p.Cin + (double)p.K * p.N + M * (p.store == 3 ? p.head_c : p.N) + 2.0 * p.N), 2.0 * M * p.N * p.K, st);
+        SMK_TAG(tag, 4.0 * (M * p.Cin + (double)p.K * p.N + M * (p.store == 3 ? p.head_c : p.N) + M * p.N * (!!p.mask + !!p.out2) + 2.0 * p.N),
+                2.0 * M * p.N * p.K, st);
     }
     // resident weights: 36 KB (32->32), 72 KB (64->32, 32->64); larger layers stream them through a ring
     if (win_resident(a.nchunks, BN)) return BN == 32 ? launch<32, true>(tmX, tmW, a, st) : launch<64, true>(tmX, tmW, a, st);

@@ -60,11 +60,13 @@ struct TcArgs {
                                    // 3 fused head: out[b, co, h, w] = sigmoid(head_b[co] + sum_n act[m, n] * head_w[n][co]) (NCHW, N <= 32)
     int round_out;                 // 1: round the stored activations to TF32 (round-to-nearest) for the next tensor-core layer
     const float* head_w; const float* head_b; int head_c;      // store 3: 1x1 head weights [N][head_c], bias [head_c], head_c <= 4
+    const float* mask; int ld_mask;    // zero outputs whose mask[m, n] <= 0 (single problem, store 0)
+    float* out2; int ld_out2;          // second store of the activations, compact at pixel m (single problem, store 0 / 2 / 3)
 };
 
 struct TcMaps { CUtensorMap a[2], b[2], blo[2]; };       // per problem: activations, weights (TF32 heads), weight tails (3xTF32)
 
-template <int BN, int STAGES, int MINB, bool PERSIST, int X3>
+template <int BN, int STAGES, int MINB, bool PERSIST, int X3, bool EXTRA>
 __global__ void __launch_bounds__(NUM_THREADS, MINB)
 gemm_tc_kernel(const __grid_constant__ TcMaps mp, const TcArgs a) {
     // Output tiles (128 rows x BN columns) are strided over the grid.
@@ -80,6 +82,8 @@ gemm_tc_kernel(const __grid_constant__ TcMaps mp, const TcArgs a) {
     //                    Weights are split on the host (TcMaps::blo maps the tails).  The activation tile is split in
     //                    registers by the consumers (A fragments of the register form of wgmma), so shared memory holds
     //                    only the plain kernel's tiles plus the weight tails.
+    //   EXTRA = true     : the epilogue also applies `mask` and writes `out2` (backward / grad-mode forward); the forward-only
+    //                    instantiations are compiled without them.
     static_assert(!X3 || !PERSIST, "3xTF32 runs single-tile CTAs");
     constexpr int B_STAGE_BYTES = BN * BKB;
     constexpr int HALF_STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
@@ -242,7 +246,7 @@ gemm_tc_kernel(const __grid_constant__ TcMaps mp, const TcArgs a) {
 #pragma unroll
                     for (int j = 0; j < 8; ++j) {
                         const float4 x4 = slab_chunk(slab, lane, j);
-                        const float xs[4] = {x4.x, x4.y, x4.z, x4.w};
+                        float xs[4] = {x4.x, x4.y, x4.z, x4.w};
 #pragma unroll
                         for (int e = 0; e < 4; ++e) {
                             const int nn = 4 * j + e;
@@ -250,8 +254,10 @@ gemm_tc_kernel(const __grid_constant__ TcMaps mp, const TcArgs a) {
                             const float2 p1 = *reinterpret_cast<const float2*>(hpar + nn * 8 + 4);
                             float x = fmaf(xs[e], p0.x, p0.y);
                             if (a.relu) x = fmaxf(x, 0.f);
+                            xs[e] = x;
                             a0 = fmaf(x, p0.z, a0); a1 = fmaf(x, p0.w, a1); a2 = fmaf(x, p1.x, a2); a3 = fmaf(x, p1.y, a3);
                         }
+                        if (EXTRA && a.out2) *reinterpret_cast<float4*>(a.out2 + (size_t)m * a.ld_out2 + 4 * j) = make_float4(xs[0], xs[1], xs[2], xs[3]);
                     }
                     const int hw_px = a.H * a.W, b = m / hw_px, rem = m - b * hw_px;
                     float* dst = g_out + (size_t)b * a.head_c * hw_px + rem;
@@ -283,8 +289,14 @@ gemm_tc_kernel(const __grid_constant__ TcMaps mp, const TcArgs a) {
                         o.x += r4.x; o.y += r4.y; o.z += r4.z; o.w += r4.w;
                     }
                     if (a.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
+                    const size_t mc = (size_t)(row0 + 4 * i + sub);            // compact pixel (mask, second store)
+                    if (EXTRA && a.mask) {
+                        const float4 k4 = __ldg(reinterpret_cast<const float4*>(a.mask + mc * a.ld_mask + nc));
+                        o.x = k4.x > 0.f ? o.x : 0.f; o.y = k4.y > 0.f ? o.y : 0.f; o.z = k4.z > 0.f ? o.z : 0.f; o.w = k4.w > 0.f ? o.w : 0.f;
+                    }
                     if (a.round_out) { o.x = smk::round_tf32(o.x); o.y = smk::round_tf32(o.y); o.z = smk::round_tf32(o.z); o.w = smk::round_tf32(o.w); }
                     *reinterpret_cast<float4*>(g_out + (size_t)(opix[i] + pix_off) * a.ld_out + col) = o;
+                    if (EXTRA && a.out2) *reinterpret_cast<float4*>(a.out2 + mc * a.ld_out2 + nc) = o;
                 }
             }
             __syncwarp();
@@ -389,21 +401,29 @@ int encode_im2col(CUtensorMap* map, const float* base, int B, int H, int W, int 
 
 namespace {
 
-template <int BN, int STAGES, int MINB, bool PERSIST, int X3 = 0>
-int launch(const TcMaps& mp, const TcArgs& a_in, cudaStream_t st, int groups) {
+template <int BN, int STAGES, int MINB, bool PERSIST, int X3, bool EXTRA>
+int launch_kernel(const TcMaps& mp, const TcArgs& a_in, cudaStream_t st, int groups) {
     constexpr size_t stage = X3 ? A_STAGE_BYTES + 2 * BN * BKB : A_STAGE_BYTES + BN * BKB;
     constexpr size_t smem = (size_t)STAGES * stage + (PERSIST ? SLAB_BYTES : 0) + BAR_BYTES + HEAD_PAR_BYTES + 1024;
     static_assert(PERSIST || (size_t)STAGES * stage >= SLAB_BYTES, "single-tile CTAs stage the epilogue in ring stage 0");
     static_assert(MINB * (smem + 1024) <= 228 * 1024, "shared memory budget of MINB resident CTAs");
-    SMK_CHECK_CUDA((set_max_dynamic_smem<gemm_tc_kernel<BN, STAGES, MINB, PERSIST, X3>>((int)smem)));
+    SMK_CHECK_CUDA((set_max_dynamic_smem<gemm_tc_kernel<BN, STAGES, MINB, PERSIST, X3, EXTRA>>((int)smem)));
     TcArgs a = a_in;
     a.tiles_n = cdiv(a.N, BN);
     a.n_tiles_g = cdiv(a.M, BM) * a.tiles_n;
     a.n_tiles = groups * a.n_tiles_g;
     dim3 grid((unsigned)(PERSIST ? std::min(a.n_tiles, MINB * num_sms()) : a.n_tiles));
-    SMK_LAUNCH((gemm_tc_kernel<BN, STAGES, MINB, PERSIST, X3>), dim3(grid), dim3(NUM_THREADS), smem, st, mp, a);
+    SMK_LAUNCH((gemm_tc_kernel<BN, STAGES, MINB, PERSIST, X3, EXTRA>), dim3(grid), dim3(NUM_THREADS), smem, st, mp, a);
     SMK_CHECK_LAUNCH();
     return 0;
+}
+
+template <int BN, int STAGES, int MINB, bool PERSIST, int X3 = 0>
+int launch(const TcMaps& mp, const TcArgs& a, cudaStream_t st, int groups) {
+    if constexpr (X3 == 0) {
+        if (a.mask || a.out2) return launch_kernel<BN, STAGES, MINB, PERSIST, X3, true>(mp, a, st, groups);
+    }
+    return launch_kernel<BN, STAGES, MINB, PERSIST, X3, false>(mp, a, st, groups);
 }
 
 }  // namespace
@@ -434,6 +454,9 @@ int tc_conv(const TcConv& p, cudaStream_t st, const TcConv* p2) {
     SMK_REQUIRE(p.store != 3 || (p.N == 32 && p.mode != 0 && p.head_w && p.head_b && p.head_c >= 1 && p.head_c <= 4 && !p.res && !p2),
                 "tc_conv: the fused 1x1 head needs a 3x3 conv with N == 32 (persistent kernel, one full column tile) and 1..4 head channels");
     SMK_REQUIRE(!p.wt_lo || (p.mode == 0 && p.store == 0), "tc_conv: the 3xTF32 path covers plain 1x1 convolutions / GEMMs");
+    SMK_REQUIRE((!p.mask || p.store == 0) && (!p.out2 || p.store != 1) && (!(p.mask || p.out2) || (!p2 && !p.wt_lo)),
+                "tc_conv: the mask needs store 0, the second store a non-shuffled store, both a single TF32 problem");
+    a.mask = p.mask; a.ld_mask = p.ld_mask; a.out2 = p.out2; a.ld_out2 = p.ld_out2;
     for (int g = 0; g < groups; ++g) {
         const TcConv& q = g ? *p2 : p;
         a.scale[g] = q.scale; a.bias[g] = q.bias; a.res[g] = q.res; a.out[g] = q.out;
@@ -451,11 +474,11 @@ int tc_conv(const TcConv& p, cudaStream_t st, const TcConv* p2) {
     if (groups == 1) { mp.a[1] = mp.a[0]; mp.b[1] = mp.b[0]; mp.blo[1] = mp.blo[0]; a.scale[1] = a.scale[0]; a.bias[1] = a.bias[0]; a.res[1] = a.res[0]; a.out[1] = a.out[0]; }
     {
         const double cin_eff = p.mode == 0 ? p.K : p.Cin;
-        const char* tag = p.mode == 0 ? (p.store == 1 ? "upconv_gemm_tc" : (p.wt_lo ? "pw_gemm_tc3x" : "pw_gemm_tc"))
+        const char* tag = p.tag ? p.tag : p.mode == 0 ? (p.store == 1 ? "upconv_gemm_tc" : (p.wt_lo ? "pw_gemm_tc3x" : "pw_gemm_tc"))
                                       : (p.store == 3 ? "conv3x3_head_gemm_tc" : "conv3x3_gemm_tc");
         if (g_prof_detail) tag = prof_shape_tag(tag, (long)groups * M, p.K, p.N);
         SMK_TAG(tag,
-                groups * 4.0 * ((double)M * cin_eff + (double)p.K * p.N + (double)M * p.N * (p.res ? 2 : 1) + 2.0 * p.N),
+                groups * 4.0 * ((double)M * cin_eff + (double)p.K * p.N + (double)M * p.N * (1 + !!p.res + !!p.mask + !!p.out2) + 2.0 * p.N),
                 groups * 2.0 * (double)M * p.N * p.K, st);
     }
     // MINB (third template argument) trades registers for co-resident CTAs: ptxas budgets the 288-thread block as three

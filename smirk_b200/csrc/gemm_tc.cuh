@@ -20,6 +20,9 @@ struct TcConv {
                                          // 3 fused 1x1 head + sigmoid: out is [B, head_c, H, W] NCHW, the activations are not stored
     const float* head_w; const float* head_b; int head_c;     // store 3: head weights [N][head_c], bias [head_c]
     int round_out;                       // 1: round stored activations to TF32 (RN) — they feed another tensor-core layer
+    const float* mask; int ld_mask;      // optional (store 0): zero output (m, n) where mask[m*ld_mask + n] <= 0 (ReLU backward)
+    float* out2; int ld_out2;            // optional (store 0, 2, 3): the stored activations again, compact NHWC at pixel m
+    const char* tag;                     // profiler tag (null: derived from the problem)
 };
 
 int tc_init();                                              // resolves the driver's tensor-map encoders

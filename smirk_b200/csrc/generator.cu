@@ -15,9 +15,18 @@
 //              reflection-padded [B,16,16,512] buffers: each conv's epilogue writes the interior, a
 //              tiny kernel mirrors the 1-pixel halo, and the next conv's im2col TMA reads it with no
 //              padding — the hardware cannot reflect, so the halo is made explicit once per layer.
+//
+// Input gradient (frozen weights, eval BN): smk_generator_forward_saved runs the same launches with the post-ReLU outputs
+// of every block conv and ResNet conv1 written to a caller-owned `saved` buffer (by redirecting the store, or by a second
+// store of the same epilogue), and smk_generator_backward walks the network backwards.  Every dgrad is an ordinary
+// convolution on the forward's GEMM kernels: a 3x3 conv's g_x = conv3x3(g, W') with W'[ci][8 - tap][co] = s[co] W[co][ci][tap]
+// (the folded BN scale rides in W', packed at create time next to the forward weights), the ReLU mask [a > 0] is applied
+// by the epilogue of the kernel that produces g, and ConvTranspose2d's dgrad is a GEMM over a space-to-depth copy of g.
 #include "nn_kernels.cuh"
 #include "gemm_tc.cuh"
 #include <math.h>
+#include <algorithm>
+#include <string>
 
 namespace {
 
@@ -25,8 +34,10 @@ using smk::ConvProblem;
 using smk::TcConv;
 constexpr float kBnEps = 1e-5f;
 
-struct Conv3 { float* w; float* wt; float* scale; float* bias; int cin, cin_p, cout; };  // w: [9*cin_p][cout]; wt: [cout][9*cin_p]
-struct UpConv { float* w; float* wt; float* scale; float* bias; int cin, cout; };         // w: [cin][4*cout];   wt: [4*cout][cin]
+// dw: dgrad weights, W' scaled by the folded BN scale: [9*cout][cin_p] (fp32) or [cin_p][9*cout] (TF32), k = tap' * cout + co
+struct Conv3 { float* w; float* wt; float* scale; float* bias; float* dw; int cin, cin_p, cout; };  // w: [9*cin_p][cout]; wt: [cout][9*cin_p]
+// dw: [4*cout][cin] (fp32) or [cin][4*cout] (TF32), k = (dy*2+dx) * cout + co
+struct UpConv { float* w; float* wt; float* scale; float* bias; float* dw; int cin, cout; };         // w: [cin][4*cout];   wt: [4*cout][cin]
 
 struct TensorCursor {
     const float* const* t; int n; int i = 0;
@@ -37,21 +48,26 @@ bool fold_conv3(TensorCursor& cur, int cin, int cin_p, int cout, bool tc, smk::D
     const float* w = cur.next(); const float* g = cur.next(); const float* b = cur.next();
     const float* mu = cur.next(); const float* var = cur.next();
     if (!w || !g || !b || !mu || !var) return false;
-    const size_t K = (size_t)9 * cin_p;
-    std::vector<float> W(K * cout, 0.f), S(cout), Bi(cout);
+    const size_t K = (size_t)9 * cin_p, Kd = (size_t)9 * cout;
+    std::vector<float> W(K * cout, 0.f), D(Kd * cin_p, 0.f), S(cout), Bi(cout);
+    for (int o = 0; o < cout; ++o) {
+        float s = g[o] / sqrtf(var[o] + kBnEps);
+        S[o] = s; Bi[o] = b[o] - mu[o] * s;
+    }
     for (int o = 0; o < cout; ++o)
         for (int c = 0; c < cin; ++c)
             for (int k = 0; k < 9; ++k) {
                 float v = w[((size_t)o * cin + c) * 9 + k];
                 if (tc) W[(size_t)o * K + (size_t)k * cin_p + c] = smk::round_tf32_host(v);   // [N][K], TF32-rounded
                 else W[((size_t)k * cin_p + c) * cout + o] = v;                // [K][N]
+                const float vd = v * S[o];
+                const size_t kd = (size_t)(8 - k) * cout + o;                  // rotated tap
+                if (tc) D[(size_t)c * Kd + kd] = smk::round_tf32_host(vd);
+                else D[kd * cin_p + c] = vd;
             }
-    for (int o = 0; o < cout; ++o) {
-        float s = g[o] / sqrtf(var[o] + kBnEps);
-        S[o] = s; Bi[o] = b[o] - mu[o] * s;
-    }
     out->cin = cin; out->cin_p = cin_p; out->cout = cout; out->w = out->wt = nullptr;
     cudaError_t e = arena.upload(W, tc ? &out->wt : &out->w);
+    if (e == cudaSuccess) e = arena.upload(D, &out->dw);
     if (e == cudaSuccess) e = arena.upload(S, &out->scale);
     if (e == cudaSuccess) e = arena.upload(Bi, &out->bias);
     *err = e;
@@ -61,17 +77,20 @@ bool fold_conv3(TensorCursor& cur, int cin, int cin_p, int cout, bool tc, smk::D
 bool fold_upconv(TensorCursor& cur, int cin, int cout, bool tc, smk::DeviceArena& arena, UpConv* out, cudaError_t* err) {
     const float* w = cur.next(); const float* b = cur.next();        // weight [cin, cout, 2, 2], bias [cout]
     if (!w || !b) return false;
-    std::vector<float> W((size_t)cin * 4 * cout), S((size_t)4 * cout, 1.f), Bi((size_t)4 * cout);
+    std::vector<float> W((size_t)cin * 4 * cout), D((size_t)cin * 4 * cout), S((size_t)4 * cout, 1.f), Bi((size_t)4 * cout);
     for (int c = 0; c < cin; ++c)
         for (int o = 0; o < cout; ++o)
             for (int q = 0; q < 4; ++q) {
                 float v = w[((size_t)c * cout + o) * 4 + q];
                 if (tc) W[((size_t)q * cout + o) * cin + c] = smk::round_tf32_host(v);   // [N = 4*cout][K = cin]
                 else W[(size_t)c * 4 * cout + q * cout + o] = v;               // [K][N]
+                if (tc) D[(size_t)c * 4 * cout + q * cout + o] = smk::round_tf32_host(v);  // dgrad [N = cin][K = 4*cout]
+                else D[((size_t)q * cout + o) * cin + c] = v;                  // dgrad [K][N]
             }
     for (int q = 0; q < 4; ++q) for (int o = 0; o < cout; ++o) Bi[q * cout + o] = b[o];
     out->cin = cin; out->cout = cout; out->w = out->wt = nullptr;
     cudaError_t e = arena.upload(W, tc ? &out->wt : &out->w);
+    if (e == cudaSuccess) e = arena.upload(D, &out->dw);
     if (e == cudaSuccess) e = arena.upload(S, &out->scale);
     if (e == cudaSuccess) e = arena.upload(Bi, &out->bias);
     *err = e;
@@ -87,6 +106,12 @@ struct SmkGenerator {
     UpConv up[4];                    // upconv4..1  (index 0 = level 4)
     Conv3 dec[4][2];                 // decoder4..1
     float *fw = nullptr, *fb = nullptr;   // final 1x1: W[f][cout], bias
+    float *ones = nullptr, *zeros = nullptr;   // unit scale / zero bias of the dgrad epilogues
+    // saved activations of the grad-mode forward (forward order): name, per-image float offset, H, W, C
+    std::vector<std::string> sv_name;
+    std::vector<size_t> sv_off;
+    std::vector<int> sv_hwc;
+    size_t sv_total = 0;                  // floats per image
     smk::DeviceArena arena;
 };
 
@@ -128,6 +153,9 @@ extern "C" int smk_generator_create(const SmkGeneratorDesc* desc, SmkGenerator**
             for (int o = 0; o < h->cout; ++o) for (int c = 0; c < f; ++c) W[(size_t)c * h->cout + o] = w[(size_t)o * f + c];
             e = h->arena.upload(W, &h->fw);
             if (e == cudaSuccess) e = h->arena.upload(b, (size_t)h->cout, &h->fb);
+            const std::vector<float> one((size_t)std::max(16 * f, h->cin_p), 1.f), zero(one.size(), 0.f);
+            if (e == cudaSuccess) e = h->arena.upload(one, &h->ones);
+            if (e == cudaSuccess) e = h->arena.upload(zero, &h->zeros);
             ok = e == cudaSuccess;
         }
     }
@@ -136,6 +164,17 @@ extern "C" int smk_generator_create(const SmkGeneratorDesc* desc, SmkGenerator**
         else smk::set_error("smk_generator_create: consumed %d tensors but %d were given (state_dict order, num_batches_tracked removed)", cur.i, cur.n);
         delete h; return e != cudaSuccess ? (int)e : -1;
     }
+    auto add = [h](const std::string& name, int S, int C) {
+        h->sv_name.push_back(name); h->sv_off.push_back(h->sv_total);
+        h->sv_hwc.insert(h->sv_hwc.end(), {S, S, C});
+        h->sv_total += (size_t)S * S * C;                                  // a multiple of 64 floats: tensors stay 256-byte aligned
+    };
+    for (int l = 0; l < 4; ++l)
+        for (int j = 1; j <= 2; ++j) add("enc" + std::to_string(l + 1) + "conv" + std::to_string(j), 224 >> l, f << l);
+    add("bottleneckconv1", 14, 16 * f); add("bottleneckconv2", 14, 16 * f);
+    for (int r = 0; r < h->nres; ++r) add("res" + std::to_string(r) + "conv1", 14, 16 * f);
+    for (int l = 3; l >= 0; --l)
+        for (int j = 1; j <= 2; ++j) add("dec" + std::to_string(l + 1) + "conv" + std::to_string(j), 224 >> l, f << l);
     *out = h;
     return 0;
 }
@@ -169,39 +208,42 @@ Plan make_plan(const SmkGenerator* h) {
 // One 3x3 convolution, dispatched on the handle's precision.
 //   refl   : reflection padding (ResNet blocks).  At precision 1 `in` must then be a padded buffer.
 //   store  : 0 plain / slice, 2 interior of a padded buffer (precision 1 only)
+//   out2   : optional second, compact [B,S,S,cout] store of the activations (the grad-mode forward's saved copy)
 int conv3(const SmkGenerator* h, const Conv3& c, const float* in, int ld_in, int B, int S, bool refl, bool relu,
-          const float* res, int res_pad, float* out, int ld_out, int store, cudaStream_t st, bool fuse_head = false) {
+          const float* res, int res_pad, float* out, int ld_out, int store, cudaStream_t st, bool fuse_head = false,
+          float* out2 = nullptr) {
     if (c.wt) {
         TcConv p{};
         if (fuse_head) { p.head_w = h->fw; p.head_b = h->fb; p.head_c = h->cout; }
         p.in = in; p.ld_in = ld_in; p.B = B; p.H = S; p.W = S; p.Cin = c.cin_p; p.wt = c.wt; p.scale = c.scale; p.bias = c.bias;
         p.N = c.cout; p.K = 9 * c.cin_p; p.mode = refl ? 2 : 1; p.relu = relu ? 1 : 0;
         p.res = res; p.ld_res = c.cout; p.res_pad = res_pad; p.out = out; p.ld_out = ld_out; p.store = store; p.round_out = 1;
+        p.out2 = out2; p.ld_out2 = c.cout;
         return smk::tc_conv(p, st);
     }
     ConvProblem p{};
     p.in = in; p.ld_in = ld_in; p.B = B; p.H = S; p.W = S; p.Cin = c.cin_p;
     p.w = c.w; p.scale = c.scale; p.bias = c.bias; p.N = c.cout; p.K = 9 * c.cin_p; p.mode = refl ? 2 : 1; p.relu = relu ? 1 : 0;
     p.res = res; p.ld_res = c.cout; p.out = out; p.ld_out = ld_out; p.shuffle = 0; p.round_out = h->precision == 1 ? 1 : 0;
+    p.out2 = out2; p.ld_out2 = c.cout;
     return smk::conv_gemm(p, st);
 }
-}  // namespace
 
-extern "C" size_t smk_generator_workspace_bytes(const SmkGenerator* h, int B) {
-    return (make_plan(h).total() * (size_t)B * sizeof(float)) + 40 * 256;
-}
+// Index of a saved tensor (forward order, see smk_generator_create).
+int sv_enc(int l, int j) { return 2 * l + j; }                              // encoder level l (0 = 224^2), conv j (0, 1)
+int sv_bott(int j) { return 8 + j; }
+int sv_res(int r) { return 10 + r; }
+int sv_dec(const SmkGenerator* h, int lvl, int j) { return 10 + h->nres + 2 * (3 - lvl) + j; }
 
-extern "C" int smk_generator_forward(const SmkGenerator* h, const float* x, int B, float* y,
-                                     void* ws, size_t ws_bytes, void* stream) {
-    if (B == 0) return 0;                      // empty batch: nothing to do (pointers may be null)
-    SMK_REQUIRE(h && x && y, "smk_generator_forward: null argument");
-    SMK_REQUIRE(B > 0, "smk_generator_forward: negative batch");
-    SMK_REQUIRE(ws && ws_bytes >= smk_generator_workspace_bytes(h, B), "smk_generator_forward: workspace too small");
-    cudaStream_t st = (cudaStream_t)stream;
+// The forward.  sv == null: the forward-only path.  Otherwise every saved activation is written to sv as well: the
+// layers whose output feeds only the next layer write straight into sv, the others (the skips, the padded ResNet
+// stream and the fused head's input) store it a second time from the same epilogue.  The arithmetic is the same.
+int generator_forward(const SmkGenerator* h, const float* x, int B, float* y, float* sv, void* ws, size_t ws_bytes, cudaStream_t st) {
     smk::Workspace w(ws, ws_bytes);
     const Plan P = make_plan(h);
     const int f = h->f;
     const bool tc = h->precision == 1;
+    auto SV = [&](int i) -> float* { return sv ? sv + (size_t)B * h->sv_off[i] : nullptr; };
     float* x8 = w.take<float>(P.x8 * B);
     float *cat[4], *t[4], *d[4], *p[4];
     for (int l = 0; l < 4; ++l) {
@@ -218,31 +260,36 @@ extern "C" int smk_generator_forward(const SmkGenerator* h, const float* x, int 
     const float* in = x8; int ld = h->cin_p;
     for (int l = 0; l < 4; ++l) {
         int S = 224 >> l, c = f << l;
-        if ((rc = conv3(h, h->enc[l][0], in, ld, B, S, false, true, nullptr, 0, t[l], c, 0, st))) return rc;
-        if ((rc = conv3(h, h->enc[l][1], t[l], c, B, S, false, true, nullptr, 0, cat[l] + c, 2 * c, 0, st))) return rc;
+        float* e1 = sv ? SV(sv_enc(l, 0)) : t[l];
+        if ((rc = conv3(h, h->enc[l][0], in, ld, B, S, false, true, nullptr, 0, e1, c, 0, st))) return rc;
+        if ((rc = conv3(h, h->enc[l][1], e1, c, B, S, false, true, nullptr, 0, cat[l] + c, 2 * c, 0, st, false, SV(sv_enc(l, 1))))) return rc;
         if ((rc = smk::maxpool2x2(cat[l] + c, 2 * c, B, S, S, c, p[l], st))) return rc;
         in = p[l]; ld = c;
     }
     const int Sb = 14, cb = 16 * f;
-    if ((rc = conv3(h, h->enc[4][0], p[3], 8 * f, B, Sb, false, true, nullptr, 0, tb, cb, 0, st))) return rc;
+    float* tbo = sv ? SV(sv_bott(0)) : tb;
+    if ((rc = conv3(h, h->enc[4][0], p[3], 8 * f, B, Sb, false, true, nullptr, 0, tbo, cb, 0, st))) return rc;
     const float* bott;                              // plain [B,14,14,cb] tensor feeding the first upconv
     if (!tc || h->nres == 0) {
-        if ((rc = conv3(h, h->enc[4][1], tb, cb, B, Sb, false, true, nullptr, 0, b0, cb, 0, st))) return rc;
-        float *cur = b0, *nxt = b1;
+        float* b0o = sv ? SV(sv_bott(1)) : b0;
+        if ((rc = conv3(h, h->enc[4][1], tbo, cb, B, Sb, false, true, nullptr, 0, b0o, cb, 0, st))) return rc;
+        float* cur = b0o;
+        float* const nxt[2] = {b1, b0};
         for (int r = 0; r < h->nres && !tc; ++r) {  // x + BN(conv(reflpad(ReLU(BN(conv(reflpad(x)))))))
-            if ((rc = conv3(h, h->res[2 * r], cur, cb, B, Sb, true, true, nullptr, 0, tb, cb, 0, st))) return rc;
-            if ((rc = conv3(h, h->res[2 * r + 1], tb, cb, B, Sb, true, false, cur, 0, nxt, cb, 0, st))) return rc;
-            std::swap(cur, nxt);
+            float* u = sv ? SV(sv_res(r)) : tb;
+            if ((rc = conv3(h, h->res[2 * r], cur, cb, B, Sb, true, true, nullptr, 0, u, cb, 0, st))) return rc;
+            if ((rc = conv3(h, h->res[2 * r + 1], u, cb, B, Sb, true, false, cur, 0, nxt[r & 1], cb, 0, st))) return rc;
+            cur = nxt[r & 1];
         }
         bott = cur;
     } else {
         // tensor-core path: residual stream lives in reflection-padded buffers  xa -> (xt) -> xb
         float *xa = pad[0], *xt = pad[1], *xb = pad[2];
-        if ((rc = conv3(h, h->enc[4][1], tb, cb, B, Sb, false, true, nullptr, 0, xa, cb, 2, st))) return rc;
+        if ((rc = conv3(h, h->enc[4][1], tbo, cb, B, Sb, false, true, nullptr, 0, xa, cb, 2, st, false, SV(sv_bott(1))))) return rc;
         if ((rc = smk::reflect_halo(xa, B, Sb, Sb, cb, st))) return rc;
         for (int r = 0; r < h->nres; ++r) {
             const bool last = r == h->nres - 1;
-            if ((rc = conv3(h, h->res[2 * r], xa, cb, B, Sb, true, true, nullptr, 0, xt, cb, 2, st))) return rc;
+            if ((rc = conv3(h, h->res[2 * r], xa, cb, B, Sb, true, true, nullptr, 0, xt, cb, 2, st, false, SV(sv_res(r))))) return rc;
             if ((rc = smk::reflect_halo(xt, B, Sb, Sb, cb, st))) return rc;
             if ((rc = conv3(h, h->res[2 * r + 1], xt, cb, B, Sb, true, false, xa, 1, last ? b0 : xb, cb, last ? 0 : 2, st))) return rc;
             if (!last) { if ((rc = smk::reflect_halo(xb, B, Sb, Sb, cb, st))) return rc; std::swap(xa, xb); }
@@ -267,13 +314,331 @@ extern "C" int smk_generator_forward(const SmkGenerator* h, const float* x, int 
             if ((rc = smk::conv_gemm(q, st))) return rc;
         }
         dS *= 2;
-        if ((rc = conv3(h, h->dec[l][0], cat[lvl], 2 * u.cout, B, dS, false, true, nullptr, 0, t[lvl], u.cout, 0, st))) return rc;
+        float* dt = sv ? SV(sv_dec(h, lvl, 0)) : t[lvl];
+        if ((rc = conv3(h, h->dec[l][0], cat[lvl], 2 * u.cout, B, dS, false, true, nullptr, 0, dt, u.cout, 0, st))) return rc;
         // last layer of the tensor-core path: the 1x1 conv + sigmoid (smirk_generator.py:77-78,86) rides in the epilogue of
-        // dec1conv2 — the [B,224,224,32] activation (6.4 MB per face) is neither written nor read back
+        // dec1conv2 — the [B,224,224,32] activation (6.4 MB per face) is neither written nor read back (the grad-mode forward
+        // stores it once, for the backward's ReLU mask)
         const bool fuse_head = l == 3 && tc && u.cout <= 32;
-        if (fuse_head) return conv3(h, h->dec[l][1], t[lvl], u.cout, B, dS, false, true, nullptr, 0, y, u.cout, 3, st, true);
-        if ((rc = conv3(h, h->dec[l][1], t[lvl], u.cout, B, dS, false, true, nullptr, 0, d[lvl], u.cout, 0, st))) return rc;
-        din = d[lvl];
+        if (fuse_head) return conv3(h, h->dec[l][1], dt, u.cout, B, dS, false, true, nullptr, 0, y, u.cout, 3, st, true, SV(sv_dec(h, lvl, 1)));
+        float* dd = sv ? SV(sv_dec(h, lvl, 1)) : d[lvl];
+        if ((rc = conv3(h, h->dec[l][1], dt, u.cout, B, dS, false, true, nullptr, 0, dd, u.cout, 0, st))) return rc;
+        din = dd;
     }
-    return smk::conv1x1_sigmoid_nchw(d[0], B, 224 * 224, f, h->fw, h->fb, h->cout, y, st);
+    return smk::conv1x1_sigmoid_nchw(din, B, 224 * 224, f, h->fw, h->fb, h->cout, y, st);
+}
+
+// ---- backward kernels ----------------------------------------------------------------------------------------------
+// Head: g_d[b,p,c] = (sum_j W_h[c][j] * g_y[b,j,p] * y (1 - y)) * [d > 0], NCHW g_y / y -> NHWC [B,HW,f].
+__global__ void __launch_bounds__(256)
+head_bwd_kernel(const float* __restrict__ gy, const float* __restrict__ y, int B, int HW, int cout, const float* __restrict__ w,
+                const float* __restrict__ d, int f, int round, float* __restrict__ out) {
+    const int F4 = f >> 2;
+    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long)B * HW * F4) return;
+    const int q = (int)(i % F4); const long pix = i / F4;
+    const int b = (int)(pix / HW), r = (int)(pix - (long)b * HW);
+    float t[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        t[j] = 0.f;
+        if (j < cout) { const size_t o = ((size_t)b * cout + j) * HW + r; const float yv = __ldg(y + o); t[j] = __ldg(gy + o) * (yv * (1.f - yv)); }
+    }
+    const float4 m = __ldg(reinterpret_cast<const float4*>(d + (size_t)pix * f) + q);
+    const float mk[4] = {m.x, m.y, m.z, m.w};
+    float o[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+        const int c = 4 * q + e;
+        float acc = 0.f;
+        for (int j = 0; j < cout; ++j) acc = fmaf(__ldg(w + (size_t)c * cout + j), t[j], acc);
+        acc = mk[e] > 0.f ? acc : 0.f;
+        o[e] = round ? smk::round_tf32(acc) : acc;
+    }
+    reinterpret_cast<float4*>(out + (size_t)pix * f)[q] = make_float4(o[0], o[1], o[2], o[3]);
+}
+
+// MaxPool 2x2 backward + skip gradient + ReLU mask of the pool input e (= the encoder's conv2 output = the skip):
+// g_e = (g_skip + [first maximum of the window, row-major] * g_p) * [e > 0].
+__global__ void __launch_bounds__(256)
+pool_bwd_kernel(const float* __restrict__ e, const float* __restrict__ gp, const float* __restrict__ gskip, int ld_skip,
+                int B, int S, int C, int round, float* __restrict__ out) {
+    const int Ho = S >> 1, C4 = C >> 2;
+    const long total = (long)B * Ho * Ho * C4;
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+        const int c4 = (int)(i % C4); const long pix = i / C4;
+        const int ow = (int)(pix % Ho); const long t = pix / Ho; const int oh = (int)(t % Ho); const int b = (int)(t / Ho);
+        const size_t p00 = ((size_t)b * S + 2 * oh) * S + 2 * ow;
+        const size_t px[4] = {p00, p00 + 1, p00 + S, p00 + S + 1};
+        float v[4][4], g[4][4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const float4 a = __ldg(reinterpret_cast<const float4*>(e + px[k] * C) + c4);
+            const float4 s = __ldg(reinterpret_cast<const float4*>(gskip + px[k] * ld_skip) + c4);
+            v[k][0] = a.x; v[k][1] = a.y; v[k][2] = a.z; v[k][3] = a.w;
+            g[k][0] = s.x; g[k][1] = s.y; g[k][2] = s.z; g[k][3] = s.w;
+        }
+        const float4 gq = __ldg(reinterpret_cast<const float4*>(gp + (size_t)pix * C) + c4);
+        const float gv[4] = {gq.x, gq.y, gq.z, gq.w};
+#pragma unroll
+        for (int ch = 0; ch < 4; ++ch) {
+            const float mx = fmaxf(fmaxf(v[0][ch], v[1][ch]), fmaxf(v[2][ch], v[3][ch]));
+            const int arg = v[0][ch] == mx ? 0 : v[1][ch] == mx ? 1 : v[2][ch] == mx ? 2 : 3;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                float r = k == arg ? g[k][ch] + gv[ch] : g[k][ch];
+                r = v[k][ch] > 0.f ? r : 0.f;
+                g[k][ch] = round ? smk::round_tf32(r) : r;
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+            reinterpret_cast<float4*>(out + px[k] * C)[c4] = make_float4(g[k][0], g[k][1], g[k][2], g[k][3]);
+    }
+}
+
+// Space-to-depth of the up-convolution's output gradient: out[b,h,w,(dy*2+dx)*C + c] = in[b,2h+dy,2w+dx,c] (S = out size).
+__global__ void __launch_bounds__(256)
+s2d_kernel(const float* __restrict__ in, int ld_in, int B, int S, int C, float* __restrict__ out) {
+    const int C4 = C >> 2;
+    const long total = (long)B * S * S * 4 * C4;
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+        const int c4 = (int)(i % C4); long t = i / C4; const int q = (int)(t % 4); const long pix = t / 4;
+        const int w = (int)(pix % S); t = pix / S; const int h = (int)(t % S); const int b = (int)(t / S);
+        const size_t src = ((size_t)b * 2 * S + 2 * h + (q >> 1)) * 2 * S + 2 * w + (q & 1);
+        reinterpret_cast<float4*>(out + (size_t)pix * 4 * C + (size_t)q * C)[c4] = __ldg(reinterpret_cast<const float4*>(in + src * ld_in) + c4);
+    }
+}
+
+// Adjoint of ReflectionPad2d(1) (the transpose of reflect_halo): g[h,w] = sum of gP over the padded pixels that mirror
+// onto (h,w), fixed order; + res (plain or the interior of a padded buffer); * [mask > 0].  gP may be null (g = res).
+// out_pad: write [B,H+2,W+2,C] with a zero halo (the next dgrad's zero padding over the padded domain), else [B,H,W,C].
+__global__ void __launch_bounds__(256)
+fold_kernel(const float* __restrict__ gP, const float* __restrict__ res, int res_pad, const float* __restrict__ mask,
+            int B, int H, int W, int C, int round, float* __restrict__ out, int out_pad) {
+    const int C4 = C >> 2, Ho = H + 2 * out_pad, Wo = W + 2 * out_pad, Hp = H + 2, Wp = W + 2;
+    const long total = (long)B * Ho * Wo * C4;
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+        const int c4 = (int)(i % C4); const long pix = i / C4;
+        const int ow = (int)(pix % Wo); const long t = pix / Wo; const int oh = (int)(t % Ho); const int b = (int)(t / Ho);
+        const int h = oh - out_pad, w = ow - out_pad;
+        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (h >= 0 && h < H && w >= 0 && w < W) {
+            if (gP) {
+                const int rows[2] = {h + 1, h == 1 ? 0 : (h == H - 2 ? H + 1 : -1)};
+                const int cols[2] = {w + 1, w == 1 ? 0 : (w == W - 2 ? W + 1 : -1)};
+#pragma unroll
+                for (int a = 0; a < 2; ++a)
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        if (rows[a] < 0 || cols[c] < 0) continue;
+                        const float4 v = __ldg(reinterpret_cast<const float4*>(gP + (((size_t)b * Hp + rows[a]) * Wp + cols[c]) * C) + c4);
+                        acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+                    }
+            }
+            if (res) {
+                const size_t rp = res_pad ? ((size_t)b * Hp + h + 1) * Wp + w + 1 : ((size_t)b * H + h) * W + w;
+                const float4 v = __ldg(reinterpret_cast<const float4*>(res + rp * C) + c4);
+                acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+            }
+            if (mask) {
+                const float4 m = __ldg(reinterpret_cast<const float4*>(mask + (((size_t)b * H + h) * W + w) * C) + c4);
+                acc.x = m.x > 0.f ? acc.x : 0.f; acc.y = m.y > 0.f ? acc.y : 0.f; acc.z = m.z > 0.f ? acc.z : 0.f; acc.w = m.w > 0.f ? acc.w : 0.f;
+            }
+            if (round) { acc.x = smk::round_tf32(acc.x); acc.y = smk::round_tf32(acc.y); acc.z = smk::round_tf32(acc.z); acc.w = smk::round_tf32(acc.w); }
+        }
+        reinterpret_cast<float4*>(out + (size_t)pix * C)[c4] = acc;
+    }
+}
+
+// First C of Cp channels, NHWC [B,HW,Cp] -> NCHW [B,C,HW].
+__global__ void __launch_bounds__(256)
+nhwc_to_nchw_kernel(const float* __restrict__ in, int B, int HW, int Cp, int C, float* __restrict__ out) {
+    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long)B * C * HW) return;
+    const int r = (int)(i % HW); const long t = i / HW; const int c = (int)(t % C); const int b = (int)(t / C);
+    out[i] = __ldg(in + ((size_t)b * HW + r) * Cp + c);
+}
+
+int grid_of(long total) { return (int)std::min<long>((total + 255) / 256, 16L * smk::num_sms()); }
+
+// dgrad of a 3x3 conv (zero padding 1): g_in = conv3x3(g, W') over S x S, * [mask > 0] (mask: the saved input activation).
+int dgrad3(const SmkGenerator* h, const Conv3& c, const float* g, int B, int S, const float* mask, float* out, int ld_out, bool round,
+           cudaStream_t st) {
+    if (h->precision == 1) {
+        TcConv p{};
+        p.in = g; p.ld_in = c.cout; p.B = B; p.H = S; p.W = S; p.Cin = c.cout; p.wt = c.dw; p.scale = h->ones; p.bias = h->zeros;
+        p.N = c.cin_p; p.K = 9 * c.cout; p.mode = 1; p.out = out; p.ld_out = ld_out; p.store = 0; p.round_out = round ? 1 : 0;
+        p.mask = mask; p.ld_mask = c.cin_p; p.tag = "conv3x3_dgrad_tc";
+        return smk::tc_conv(p, st);
+    }
+    ConvProblem p{};
+    p.in = g; p.ld_in = c.cout; p.B = B; p.H = S; p.W = S; p.Cin = c.cout; p.w = c.dw; p.scale = h->ones; p.bias = h->zeros;
+    p.N = c.cin_p; p.K = 9 * c.cout; p.mode = 1; p.out = out; p.ld_out = ld_out; p.mask = mask; p.ld_mask = c.cin_p;
+    p.tag = "conv3x3_dgrad_f32";
+    return smk::conv_gemm(p, st);
+}
+
+// dgrad of ConvTranspose2d(k2, s2): g_in[S x S, cin] = s2d(g_out)[S x S, 4 cout] . W'^T, * [mask > 0].
+int dgrad_up(const SmkGenerator* h, const UpConv& u, const float* s2d, int B, int S, const float* mask, float* out, bool round, cudaStream_t st) {
+    const int K = 4 * u.cout;
+    if (h->precision == 1) {
+        TcConv p{};
+        p.in = s2d; p.ld_in = K; p.B = B; p.H = S; p.W = S; p.Cin = K; p.wt = u.dw; p.scale = h->ones; p.bias = h->zeros;
+        p.N = u.cin; p.K = K; p.mode = 0; p.out = out; p.ld_out = u.cin; p.store = 0; p.round_out = round ? 1 : 0;
+        p.mask = mask; p.ld_mask = u.cin; p.tag = "upconv_dgrad_tc";
+        return smk::tc_conv(p, st);
+    }
+    ConvProblem p{};
+    p.in = s2d; p.ld_in = K; p.B = B; p.H = S; p.W = S; p.Cin = K; p.w = u.dw; p.scale = h->ones; p.bias = h->zeros;
+    p.N = u.cin; p.K = K; p.mode = 0; p.out = out; p.ld_out = u.cin; p.mask = mask; p.ld_mask = u.cin; p.tag = "upconv_dgrad_f32";
+    return smk::conv_gemm(p, st);
+}
+
+int fold(const float* gP, const float* res, int res_pad, const float* mask, int B, int C, bool round, float* out, int out_pad, cudaStream_t st) {
+    const int H = 14, Ho = H + 2 * out_pad;
+    const long total = (long)B * Ho * Ho * (C / 4);
+    SMK_TAG("reflect_fold", 4.0 * B * C * ((gP ? 16.0 * 16 : 0.0) + (res ? 196.0 : 0.0) + (mask ? 196.0 : 0.0) + Ho * Ho), (gP ? 1.0 : 0.0) * B * C * 256, st);
+    SMK_LAUNCH(fold_kernel, dim3(grid_of(total)), dim3(256), 0, st, gP, res, res_pad, mask, B, H, H, C, round ? 1 : 0, out, out_pad);
+    SMK_CHECK_LAUNCH();
+    return 0;
+}
+
+// floats per image of the backward's workspace buffers
+struct GradPlan {
+    size_t g, gcat[4], s2d, pad;
+    size_t total() const { return 2 * g + gcat[0] + gcat[1] + gcat[2] + gcat[3] + s2d + 4 * pad; }
+};
+GradPlan make_grad_plan(const SmkGenerator* h) {
+    GradPlan P{};
+    P.g = (size_t)224 * 224 * std::max(h->f, h->cin_p);
+    for (int l = 0; l < 4; ++l) { const size_t S = 224 >> l; P.gcat[l] = S * S * 2 * ((size_t)h->f << l); }
+    P.s2d = (size_t)112 * 112 * 4 * h->f;
+    P.pad = h->nres > 0 ? (size_t)16 * 16 * 16 * h->f : 0;
+    return P;
+}
+}  // namespace
+
+extern "C" size_t smk_generator_workspace_bytes(const SmkGenerator* h, int B) {
+    return (make_plan(h).total() * (size_t)B * sizeof(float)) + 40 * 256;
+}
+
+extern "C" int smk_generator_forward(const SmkGenerator* h, const float* x, int B, float* y,
+                                     void* ws, size_t ws_bytes, void* stream) {
+    if (B == 0) return 0;                      // empty batch: nothing to do (pointers may be null)
+    SMK_REQUIRE(h && x && y, "smk_generator_forward: null argument");
+    SMK_REQUIRE(B > 0, "smk_generator_forward: negative batch");
+    SMK_REQUIRE(ws && ws_bytes >= smk_generator_workspace_bytes(h, B), "smk_generator_forward: workspace too small");
+    return generator_forward(h, x, B, y, nullptr, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+extern "C" size_t smk_generator_saved_bytes(const SmkGenerator* h, int B) {
+    return h && B > 0 ? h->sv_total * (size_t)B * sizeof(float) : 0;
+}
+
+extern "C" int smk_generator_saved_tensor(const SmkGenerator* h, int B, int i, const char** name, size_t* offset, int* dims) {
+    SMK_REQUIRE(h && name && offset && dims, "smk_generator_saved_tensor: null argument");
+    SMK_REQUIRE(B >= 0, "smk_generator_saved_tensor: negative batch");
+    SMK_REQUIRE(i >= 0 && i < (int)h->sv_name.size(), "smk_generator_saved_tensor: index %d out of range (%d tensors)", i, (int)h->sv_name.size());
+    *name = h->sv_name[i].c_str();
+    *offset = h->sv_off[i] * (size_t)B;
+    dims[0] = B; dims[1] = h->sv_hwc[3 * i]; dims[2] = h->sv_hwc[3 * i + 1]; dims[3] = h->sv_hwc[3 * i + 2];
+    return 0;
+}
+
+extern "C" int smk_generator_forward_saved(const SmkGenerator* h, const float* x, int B, float* y, float* saved, size_t saved_bytes,
+                                           void* ws, size_t ws_bytes, void* stream) {
+    SMK_REQUIRE(h, "smk_generator_forward_saved: null handle");
+    SMK_REQUIRE(B >= 0, "smk_generator_forward_saved: negative batch");
+    if (B == 0) return 0;
+    SMK_REQUIRE(x && y && saved, "smk_generator_forward_saved: null argument");
+    SMK_REQUIRE(saved_bytes > 0 && saved_bytes >= smk_generator_saved_bytes(h, B), "smk_generator_forward_saved: saved buffer too small");
+    SMK_REQUIRE(ws && ws_bytes > 0 && ws_bytes >= smk_generator_workspace_bytes(h, B), "smk_generator_forward_saved: workspace too small");
+    return generator_forward(h, x, B, y, saved, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+extern "C" size_t smk_generator_backward_workspace_bytes(const SmkGenerator* h, int B) {
+    return h && B > 0 ? make_grad_plan(h).total() * (size_t)B * sizeof(float) + 16 * 256 : 0;
+}
+
+extern "C" int smk_generator_backward(const SmkGenerator* h, int B, const float* y, const float* saved, size_t saved_bytes,
+                                      const float* g_y, float* g_x, void* ws, size_t ws_bytes, void* stream) {
+    SMK_REQUIRE(h, "smk_generator_backward: null handle");
+    SMK_REQUIRE(B >= 0, "smk_generator_backward: negative batch");
+    if (B == 0) return 0;
+    SMK_REQUIRE(y && saved && g_y && g_x, "smk_generator_backward: null argument");
+    SMK_REQUIRE(saved_bytes > 0 && saved_bytes >= smk_generator_saved_bytes(h, B), "smk_generator_backward: saved buffer too small");
+    SMK_REQUIRE(ws && ws_bytes > 0 && ws_bytes >= smk_generator_backward_workspace_bytes(h, B), "smk_generator_backward: workspace too small");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int f = h->f, cb = 16 * f;
+    const bool tc = h->precision == 1;
+    auto SV = [&](int i) -> const float* { return saved + (size_t)B * h->sv_off[i]; };
+    const GradPlan P = make_grad_plan(h);
+    smk::Workspace w(ws, ws_bytes);
+    float* A = w.take<float>(P.g * B); float* Bf = w.take<float>(P.g * B);
+    float* gcat[4];
+    for (int l = 0; l < 4; ++l) gcat[l] = w.take<float>(P.gcat[l] * B);
+    float* s2d = w.take<float>(P.s2d * B);
+    float* pad[4] = {nullptr, nullptr, nullptr, nullptr};
+    if (h->nres > 0) for (int i = 0; i < 4; ++i) pad[i] = w.take<float>(P.pad * B);
+    SMK_REQUIRE(s2d && (h->nres == 0 || pad[3]), "smk_generator_backward: workspace carve-up failed");
+    int rc;
+    // head: sigmoid and the 1x1 conv, through dec1conv2's ReLU
+    {
+        const long total = (long)B * 224 * 224 * (f / 4);
+        SMK_TAG("head_dgrad", 4.0 * B * 224.0 * 224.0 * (2.0 * h->cout + 2.0 * f), 2.0 * B * 224.0 * 224.0 * f * h->cout, st);
+        SMK_LAUNCH(head_bwd_kernel, dim3(smk::cdiv(total, 256)), dim3(256), 0, st, g_y, y, B, 224 * 224, h->cout, h->fw,
+                   SV(sv_dec(h, 0, 1)), f, tc ? 1 : 0, A);
+        SMK_CHECK_LAUNCH();
+    }
+    // decoder levels 1..4: conv2, conv1 (both halves of the concat), up-convolution
+    for (int lvl = 0; lvl < 4; ++lvl) {
+        const int i = 3 - lvl, S = 224 >> lvl, c = f << lvl;
+        if ((rc = dgrad3(h, h->dec[i][1], A, B, S, SV(sv_dec(h, lvl, 0)), Bf, c, tc, st))) return rc;
+        if ((rc = dgrad3(h, h->dec[i][0], Bf, B, S, nullptr, gcat[lvl], 2 * c, tc, st))) return rc;
+        {
+            const long total = (long)B * (S / 2) * (S / 2) * 4 * (c / 4);
+            SMK_TAG("upconv_s2d", 8.0 * B * S * S * c, 0.0, st);
+            SMK_LAUNCH(s2d_kernel, dim3(grid_of(total)), dim3(256), 0, st, gcat[lvl], 2 * c, B, S / 2, c, s2d);
+            SMK_CHECK_LAUNCH();
+        }
+        const float* m = lvl < 3 ? SV(sv_dec(h, lvl + 1, 1)) : (h->nres == 0 ? SV(sv_bott(1)) : nullptr);
+        if ((rc = dgrad_up(h, h->up[i], s2d, B, S / 2, m, A, tc, st))) return rc;
+    }
+    // ResNet blocks, last to first, over zero-haloed 16 x 16 gradient buffers: g_x = fold(conv(G(fold(conv(G(g)) * [u > 0])))) + g
+    float* g = A;                                    // gradient of the bottleneck's conv2 output, [B,14,14,cb]
+    if (h->nres > 0) {
+        float *cur = pad[0], *nxt = pad[1], *gP = pad[2], *gu = pad[3];
+        if ((rc = fold(nullptr, A, 0, nullptr, B, cb, tc, cur, 1, st))) return rc;
+        for (int r = h->nres - 1; r >= 0; --r) {
+            if ((rc = dgrad3(h, h->res[2 * r + 1], cur, B, 16, nullptr, gP, cb, tc, st))) return rc;
+            if ((rc = fold(gP, nullptr, 0, SV(sv_res(r)), B, cb, tc, gu, 1, st))) return rc;
+            if ((rc = dgrad3(h, h->res[2 * r], gu, B, 16, nullptr, gP, cb, tc, st))) return rc;
+            if (r == 0) { if ((rc = fold(gP, cur, 1, SV(sv_bott(1)), B, cb, tc, Bf, 0, st))) return rc; }
+            else { if ((rc = fold(gP, cur, 1, nullptr, B, cb, tc, nxt, 1, st))) return rc; std::swap(cur, nxt); }
+        }
+        g = Bf;
+    }
+    float* o = g == A ? Bf : A;
+    if ((rc = dgrad3(h, h->enc[4][1], g, B, 14, SV(sv_bott(0)), o, cb, tc, st))) return rc;
+    if ((rc = dgrad3(h, h->enc[4][0], o, B, 14, nullptr, g, 8 * f, tc, st))) return rc;
+    // encoder levels 4..1: pool (+ skip gradient), conv2, conv1
+    for (int lvl = 3; lvl >= 0; --lvl) {
+        const int S = 224 >> lvl, c = f << lvl;
+        {
+            const long total = (long)B * (S / 2) * (S / 2) * (c / 4);
+            SMK_TAG("maxpool_dgrad", 4.0 * B * ((double)S * S * c * 3 + (S / 2.0) * (S / 2.0) * c), 0.0, st);
+            SMK_LAUNCH(pool_bwd_kernel, dim3(grid_of(total)), dim3(256), 0, st, SV(sv_enc(lvl, 1)), g, gcat[lvl] + c, 2 * c, B, S, c, tc ? 1 : 0, o);
+            SMK_CHECK_LAUNCH();
+        }
+        if ((rc = dgrad3(h, h->enc[lvl][1], o, B, S, SV(sv_enc(lvl, 0)), g, c, tc, st))) return rc;
+        const int n_in = lvl > 0 ? c / 2 : h->cin_p;
+        if ((rc = dgrad3(h, h->enc[lvl][0], g, B, S, nullptr, o, n_in, tc && lvl > 0, st))) return rc;
+        std::swap(g, o);
+    }
+    const long total = (long)B * h->cin * 224 * 224;
+    SMK_TAG("nhwc_to_nchw", 4.0 * (double)B * 224 * 224 * (h->cin + h->cin_p), 0.0, st);
+    SMK_LAUNCH(nhwc_to_nchw_kernel, dim3(smk::cdiv(total, 256)), dim3(256), 0, st, g, B, 224 * 224, h->cin_p, h->cin, g_x);
+    SMK_CHECK_LAUNCH();
+    return 0;
 }

@@ -124,7 +124,9 @@ conv_gemm_kernel(ConvProblem p, int M) {
             float v = fmaf(acc[i][j], p.scale[n], p.bias[n]);
             if (p.res) v += p.res[(size_t)m * p.ld_res + n];
             if (p.relu) v = fmaxf(v, 0.f);
+            if (p.mask && !(p.mask[(size_t)m * p.ld_mask + n] > 0.f)) v = 0.f;
             if (p.round_out) v = round_tf32(v);
+            if (p.out2) p.out2[(size_t)m * p.ld_out2 + n] = v;
             if (p.shuffle) {
                 int cout = p.N >> 2, q = n / cout, co = n - q * cout;
                 int b = m / HW, r = m - b * HW, h = r / p.W, w = r - h * p.W;
@@ -473,12 +475,13 @@ int conv_gemm(const ConvProblem& p, cudaStream_t st) {
     const int M = p.B * p.H * p.W;
     SMK_REQUIRE(p.K % 4 == 0 && p.N % 4 == 0 && p.ld_in % 4 == 0, "conv_gemm: K, N, ld_in must be multiples of 4");
     SMK_REQUIRE(p.mode == 0 || p.Cin % 4 == 0, "conv_gemm: Cin must be a multiple of 4");
+    SMK_REQUIRE(!p.out2 || !p.shuffle, "conv_gemm: the second store does not support the pixel-shuffle layout");
     {
         const double cin_eff = p.mode == 0 ? p.K : p.Cin;       // unique input bytes (not im2col-expanded)
-        const char* tag = p.mode == 0 ? (p.shuffle ? "upconv_gemm_f32" : "pw_gemm_f32") : "conv3x3_gemm_f32";
+        const char* tag = p.tag ? p.tag : p.mode == 0 ? (p.shuffle ? "upconv_gemm_f32" : "pw_gemm_f32") : "conv3x3_gemm_f32";
         if (g_prof_detail) tag = prof_shape_tag(tag, M, p.K, p.N);
         SMK_TAG(tag,
-                4.0 * ((double)M * cin_eff + (double)p.K * p.N + (double)M * p.N * (p.res ? 2 : 1) + 2.0 * p.N),
+                4.0 * ((double)M * cin_eff + (double)p.K * p.N + (double)M * p.N * (1 + !!p.res + !!p.mask + !!p.out2) + 2.0 * p.N),
                 2.0 * (double)M * p.N * p.K, st);
     }
     if (p.N <= 32) {

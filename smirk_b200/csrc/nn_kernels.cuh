@@ -25,6 +25,9 @@ struct ConvProblem {
     float* out; int ld_out;              // pixel stride of the output (>= N; lets us write a concat slice)
     int shuffle;                         // 1: n = (dy*2+dx)*Cout + co  ->  pixel (2h+dy, 2w+dx), channel co
     int round_out;                       // 1: round outputs to TF32 (they feed a tensor-core layer)
+    const float* mask; int ld_mask;      // optional: zero output (m, n) where mask[m*ld_mask + n] <= 0 (ReLU backward)
+    float* out2; int ld_out2;            // optional second store of the output at pixel m (no shuffle)
+    const char* tag;                     // profiler tag (null: derived from the problem)
 };
 
 int conv_gemm(const ConvProblem& p, cudaStream_t st);

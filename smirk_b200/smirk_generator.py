@@ -1,8 +1,13 @@
-"""``SmirkGenerator`` — drop-in for the reference ``src/smirk_generator.py`` (forward only, eval BN).
+"""``SmirkGenerator`` — drop-in for the reference ``src/smirk_generator.py`` (eval BN).
 
 Same constructor, sub-module names (``state_dict`` keys such as ``encoder1.enc1conv1.weight``,
 ``resnet_blocks.0.conv_block.1.weight``, ``upconv4.bias``) and forward signature.  The torch modules are
 parameter containers; the forward pass runs in ``csrc/generator.cu`` through ``smk_generator_forward``.
+
+With grad mode on and an input that requires grad, a frozen (``requires_grad_(False)``) eval-mode generator passes the
+gradient to its input, as the reference trainer's emotion loss and photometric fitting need: the forward then keeps
+its activations (``smk_generator_forward_saved``) and the backward runs ``smk_generator_backward``.  Weight gradients
+are not implemented.
 """
 import ctypes as C
 from collections import OrderedDict
@@ -78,19 +83,81 @@ class SmirkGenerator(_lib.NativeModule, nn.Module):
         d.tensors, d.n_tensors, d.precision = C.cast(arr, C.POINTER(_lib.c_f32p)), len(ts), self.precision
         return _lib.create("generator", d, device)
 
-    @torch.no_grad()
+    def _check_input(self, x):
+        cin = self._cfg[0]
+        if x.dim() != 4 or tuple(x.shape[1:]) != (cin, 224, 224):
+            raise RuntimeError("smirk_b200.SmirkGenerator: expected x [B,%d,224,224], got %s" % (cin, tuple(x.shape)))
+
     def forward(self, x):
         _lib.require_cuda(x, "x")
         if self.training:                      # checked on every call: .train() after the first forward must not silently run eval BN
             raise RuntimeError("smirk_b200.SmirkGenerator: train-mode BatchNorm is not implemented (forward/eval only)")
+        if torch.is_grad_enabled() and x.requires_grad:
+            if any(p.requires_grad for p in self.parameters()):
+                raise RuntimeError("smirk_b200.SmirkGenerator: weight gradients are not implemented; to pass a gradient to the "
+                                   "input, freeze the generator with .requires_grad_(False)")
+            self._check_input(x)
+            return _GeneratorFunction.apply(x, self)
+        with torch.no_grad():
+            dev = x.device
+            h = self._native_handle(dev)
+            x = _lib.dev_f32(x, "x")
+            self._check_input(x)
+            B = x.shape[0]
+            y = torch.empty(B, self._cfg[1], 224, 224, dtype=torch.float32, device=dev)
+            ws = self._native_workspace("forward", _lib.call("smk_generator_workspace_bytes", dev, h, B), dev)
+            _lib.call("smk_generator_forward", dev, h, x, B, y, ws, ws.numel())
+            return y
+
+    def _forward_saved(self, x):
+        """-> (handle, y, saved): the grad-mode forward, its activations in a buffer of their own."""
         dev = x.device
         h = self._native_handle(dev)
         x = _lib.dev_f32(x, "x")
-        cin, cout = self._cfg[0], self._cfg[1]
-        if x.dim() != 4 or tuple(x.shape[1:]) != (cin, 224, 224):
-            raise RuntimeError("smirk_b200.SmirkGenerator: expected x [B,%d,224,224], got %s" % (cin, tuple(x.shape)))
         B = x.shape[0]
-        y = torch.empty(B, cout, 224, 224, dtype=torch.float32, device=dev)
+        y = torch.empty(B, self._cfg[1], 224, 224, dtype=torch.float32, device=dev)
+        nbytes = _lib.call("smk_generator_saved_bytes", dev, h, B)
+        saved = torch.empty(nbytes // 4, dtype=torch.float32, device=dev)
         ws = self._native_workspace("forward", _lib.call("smk_generator_workspace_bytes", dev, h, B), dev)
-        _lib.call("smk_generator_forward", dev, h, x, B, y, ws, ws.numel())
+        _lib.call("smk_generator_forward_saved", dev, h, x, B, y, saved, nbytes, ws, ws.numel())
+        return h, y, saved
+
+    @torch.no_grad()
+    def saved_activations(self, x):
+        """The activations the backward of ``self(x)`` uses, {reference layer name: [B,C,H,W] tensor}: the post-ReLU
+        output of every block conv (``enc1conv1`` ... ``dec1conv2``) and of every ResNet block's first conv
+        (``res0conv1`` ...).  The forward is deterministic and batch-independent, so these are the tensors an autograd
+        context of the same input holds."""
+        _lib.require_cuda(x, "x")
+        self._check_input(x)
+        h, _, saved = self._forward_saved(x)
+        B, out = x.shape[0], {}
+        name, off, dims = C.c_char_p(), C.c_size_t(), (C.c_int * 4)()
+        for i in range(18 + self._cfg[3]):
+            _lib.call("smk_generator_saved_tensor", x.device, h, B, i, C.byref(name), C.byref(off), dims)
+            b, hh, ww, c = dims
+            out[name.value.decode()] = saved[off.value:off.value + b * hh * ww * c].view(b, hh, ww, c).permute(0, 3, 1, 2)
+        return out
+
+
+class _GeneratorFunction(torch.autograd.Function):
+    """Frozen generator: y = G(x), and the gradient with respect to x only.  The activations are saved per call, so
+    several forwards may share one backward."""
+
+    @staticmethod
+    def forward(ctx, x, module):
+        h, y, saved = module._forward_saved(x)
+        ctx.handle, ctx.module, ctx.dtype = h, module, x.dtype    # the handle the activations were computed with
+        ctx.save_for_backward(y, saved)
         return y
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_y):
+        y, saved = ctx.saved_tensors
+        m, dev, B = ctx.module, y.device, y.shape[0]
+        g_y = _lib.dev_f32(g_y, "g_y")
+        g_x = torch.empty(B, m._cfg[0], 224, 224, dtype=torch.float32, device=dev)
+        ws = m._native_workspace("backward", _lib.call("smk_generator_backward_workspace_bytes", dev, ctx.handle, B), dev)
+        _lib.call("smk_generator_backward", dev, ctx.handle, B, y, saved, saved.numel() * 4, g_y, g_x, ws, ws.numel())
+        return g_x.to(ctx.dtype), None
