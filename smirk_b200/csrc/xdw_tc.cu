@@ -7,19 +7,27 @@
 //
 //   CTA = one 16x16-pixel window of e for one image (a 14x14 tile of outputs + halo for stride 1, a 7x7
 //         tile for stride 2) x one group of 32-channel chunks of the expanded tensor (the depthwise conv
-//         makes channel chunks independent, so low-resolution layers still fill the GPU).  Persistent CTAs,
-//         two per SM fit; the launcher aims for one per SM, which leaves room on every SM for the other kernels
-//         of the concurrent pipeline.
-//   warp 8      TMA producer: two 16x8-pixel boxes of x (4-D tiled tensor map over NHWC, halo pixels
-//               outside the image zero-filled by the hardware) + a 32-row box of the 1x1 weights per k-block.
-//   warps 0-7   two warpgroups; warpgroup h multiplies window half h (128 pixels x 32 channels) with
-//               wgmma.m64n32k8 TF32 (two per k-step), then
+//         makes channel chunks independent, so low-resolution layers still fill the GPU).  Persistent CTAs;
+//         the launcher aims for one per SM, which leaves room on every SM for the other kernels of the
+//         concurrent pipeline.
+//   warp 8      TMA producer: per work item, the whole x window once — two 16x8-pixel boxes per 32-channel
+//               k-block (4-D tiled tensor map over NHWC, halo pixels outside the image zero-filled by the hardware)
+//               into a window region that stays resident for the item; then only the 1x1 weights (a 32-row box
+//               per (chunk, k-block), plus its tails in the 3xTF32 variant) through a small mbarrier ring.
+//   warps 0-7   two warpgroups; warpgroup h multiplies window half h (128 pixels x Cin) with wgmma.m64n32k8 TF32
+//               (two per k-step, ceil(Cin / 8) k-steps: none over the zero-filled channels past Cin), then
 //               (a) accumulator registers -> BN1 + ReLU (+ zero outside the image, which is what the depthwise
 //               conv's zero padding of e means) -> shared-memory window E[256][32];
 //               (b) depthwise 3x3 over E on the CUDA cores (float4 over channels), BN2 + ReLU, optional
 //               TF32 rounding, coalesced 256-byte stores of d.
 //
-// Algorithmic HBM traffic per block drops from  x + 2e + d  to  x + d.
+// Shared memory: [window 0 (, window 1)][weight ring][E][parameters][barriers].  The window holds NKB = ceil(Cin / 32)
+// k-blocks of 32 KiB (the kernel is instantiated per NKB, Cin <= 160); it is double-buffered where that fits the
+// per-SM budget (so the next item's window lands while this item computes), otherwise the producer refills it as soon
+// as the item's last chunk has finished its MMAs, during that chunk's phases (a)/(b).
+//
+// Algorithmic HBM traffic per block drops from  x + 2e + d  to  x + d.  L2 -> shared memory per item: the window
+// once (NKB x 32 KiB) + the weights of its chunks (NKB x 4 KiB per chunk, x2 for 3xTF32).
 #include "gemm_tc.cuh"
 #include "xdw_tc.cuh"
 #include "tc_ptx.cuh"
@@ -30,16 +38,39 @@ namespace {
 constexpr int BKB = 128, BK = 32, MMA_K = 8;
 constexpr int WIN = 16;                         // window edge (pixels of e)
 constexpr int HALF_BYTES = 128 * BKB;           // one 16x8-pixel box, 32 channels: 16 KiB
+constexpr int KB_BYTES = 2 * HALF_BYTES;        // both halves of the window, one 32-channel k-block: 32 KiB
 constexpr int NC = 32;                          // expanded channels per chunk
 constexpr int B_BYTES = NC * BKB;               // 4 KiB
-constexpr int STAGE_BYTES = 2 * HALF_BYTES + B_BYTES;   // 36 KiB (+ the weight tails in the 3xTF32 variant)
-constexpr int STAGES = 2;
 constexpr int E_PITCH = NC + 4;                 // floats; 144-byte rows (odd multiple of 16 B): conflict-free 16-byte column writes
 constexpr int E_BYTES = 256 * E_PITCH * 4;      // 36 864 B
 constexpr int PAR_ROWS = 13;                     // scale1, bias1, 9 depthwise taps, scale2, bias2
 constexpr int PAR_BYTES = 2 * PAR_ROWS * NC * 4;  // double-buffered: 3328 B
 constexpr int NUM_WORKERS = 256;
 constexpr int NUM_THREADS = NUM_WORKERS + 32;
+constexpr int MAX_NKB = 5;                      // Cin <= 160
+constexpr int SMEM_PER_SM = 228 * 1024, SMEM_PER_CTA = 227 * 1024, SMEM_RESERVED = 1024;   // sm_90 limits
+
+// Shared-memory plan of one window size.  MINB: resident CTAs per SM the kernel is built for — two for plain TF32
+// wherever a single window leaves room for them, one for 3xTF32 (register-bound) and for the deep plain-TF32 windows.
+// STAGES: weight stages; NKB where they fit, so the next chunk's weights all load during this chunk's phases (a)/(b).
+// WBUF: windows, two where they fit beside MINB CTAs.
+template <int NKB, int X3> struct XdwSmem {
+    static constexpr int WIN_BYTES = NKB * KB_BYTES;
+    static constexpr int STAGE_BYTES = X3 ? 2 * B_BYTES : B_BYTES;      // [w heads] (+ [w tails])
+    static constexpr size_t bytes(int wbuf, int stages) {
+        return (size_t)wbuf * WIN_BYTES + stages * STAGE_BYTES + E_BYTES + PAR_BYTES + 256 + 1024;   // + barriers, alignment slack
+    }
+    static constexpr bool fits(int wbuf, int stages, int minb) {
+        return bytes(wbuf, stages) <= SMEM_PER_CTA && minb * (bytes(wbuf, stages) + SMEM_RESERVED) <= SMEM_PER_SM;
+    }
+    static constexpr int MINB = !X3 && fits(1, 2, 2) ? 2 : 1;
+    static constexpr int STAGES = NKB > 2 && fits(1, NKB, MINB) ? NKB : 2;
+    static constexpr int WBUF = fits(2, STAGES, MINB) ? 2 : 1;
+    static constexpr size_t SMEM = bytes(WBUF, STAGES);
+    static constexpr int RING = WBUF * WIN_BYTES, E_OFF = RING + STAGES * STAGE_BYTES, PAR_OFF = E_OFF + E_BYTES,
+                         BAR_OFF = PAR_OFF + PAR_BYTES;
+    static_assert(fits(WBUF, STAGES, MINB), "shared-memory budget");
+};
 
 using namespace ptx;                            // PTX wrappers shared by the tensor-core kernels (tc_ptx.cuh)
 __device__ __forceinline__ void worker_barrier() { named_barrier(1, NUM_WORKERS); }
@@ -48,7 +79,7 @@ struct XdwMaps { CUtensorMap x[2], w[2], wlo[2]; };      // per problem: activat
 
 struct XdwArgs {
     int H, W, Ho, Wo;              // e (= x) resolution and output resolution
-    int mid, nkb, nchunks;         // expanded channels, 32-wide k-blocks of Cin, 32-wide channel chunks
+    int mid, nchunks;              // expanded channels, 32-wide channel chunks
     int groups, chunks_per_group;  // a group owns chunks [g*cpg, min((g+1)*cpg, nchunks)); item = ((img*tiles_y + ty)*tiles_x + tx)*groups + g
     int n_items, B;                // items of the launch (two identically shaped problems may share one, like gemm_tc.cu: image index B.. = problem 1)
     int d_grp, d_tx, d_ty, d_img;  // (group, tile x, tile y, image) digits of the grid size: the item stride of a persistent CTA
@@ -65,25 +96,30 @@ struct XdwArgs {
 // X3 != 0: error-compensated 3xTF32 expand GEMM (fp32-equivalent e): x = x_hi + x_lo, w1 = w_hi + w_lo (split on the host, wlo),
 // e = x_hi*w_hi + x_lo*w_hi + x_hi*w_lo accumulated in the same registers.  The workers split their own A fragments of x in
 // registers and use the register-A form of wgmma, so shared memory only grows by the weight tails.
-template <int STRIDE, int X3>
-__global__ void __launch_bounds__(NUM_THREADS, X3 ? 1 : 2)
+// NKB: 32-channel k-blocks of Cin (window size), KSL: wgmma k-steps of 8 channels in the last one (Cin = 32 (NKB - 1) + 8 KSL,
+// rounded up to a multiple of 8).
+template <int STRIDE, int X3, int NKB, int KSL>
+__global__ void __launch_bounds__(NUM_THREADS, XdwSmem<NKB, X3>::MINB)
 xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
+    using L = XdwSmem<NKB, X3>;
     constexpr int TO = STRIDE == 1 ? 14 : 7;                    // output tile edge
-    constexpr int STAGE_BYTES = X3 ? smk::STAGE_BYTES + B_BYTES : smk::STAGE_BYTES;      // [x half 0][x half 1][w] (+ [w tails])
-    constexpr int WLO = smk::STAGE_BYTES;                       // offset of the weight tails within a stage
+    constexpr int STAGES = L::STAGES, STAGE_BYTES = L::STAGE_BYTES, WBUF = L::WBUF;
     extern __shared__ uint8_t smem_raw[];
     // 1024-byte alignment for SWIZZLE_128B; offset arithmetic (not an integer round-trip of the pointer) keeps
     // the shared address space visible to the compiler, so E is accessed with LDS/STS instead of generic LD/ST.
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    float* E = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
-    float* PAR = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES + E_BYTES);        // [2][PAR_ROWS][NC]
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + E_BYTES + PAR_BYTES);
+    uint8_t* ring = smem + L::RING;                              // stage s: [w heads] (+ [w tails])
+    float* E = reinterpret_cast<float*>(smem + L::E_OFF);
+    float* PAR = reinterpret_cast<float*>(smem + L::PAR_OFF);   // [2][PAR_ROWS][NC]
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
     uint64_t* empty = full + STAGES;
+    uint64_t* wfull = empty + STAGES;                            // window b loaded (TMA transaction count)
+    uint64_t* wempty = wfull + WBUF;                             // window b free: its item's last chunk has finished its MMAs
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // Persistent CTA: work item = (image, output tile, channel-chunk group), items strided over the grid.
-    // Both roles walk the same item sequence; the smem ring runs across item boundaries, so the x window / weights
-    // of item i+1 are in flight while the workers are still busy with item i.
+    // Both roles walk the same item sequence; the weight ring runs across item boundaries and the window is
+    // refilled as soon as it is free, so the loads of item i+1 are in flight while the workers are still busy with item i.
     // The item sequence of a CTA advances by gridDim.x; the (group, tile x, tile y, image) digits of the item index are
     // carried along incrementally — one runtime decomposition per thread at kernel start instead of four integer divisions per item.
     struct Item { int prob, img, oh0, ow0, c_begin, c_end; };
@@ -114,27 +150,35 @@ xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
         prefetch_tensormap(&mp.w[0]);
         if (X3) prefetch_tensormap(&mp.wlo[0]);
         for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], NUM_WORKERS / 32); }
+        for (int b = 0; b < WBUF; ++b) { mbar_init(&wfull[b], 1); mbar_init(&wempty[b], NUM_WORKERS / 32); }
         fence_barrier_init();
     }
     __syncthreads();
 
     if (warp == NUM_WORKERS / 32) {
         if (lane == 0) {
-            // ===== TMA producer: (x window, W1 chunk) per k-block, for every channel chunk =====
-            int it = 0;
-            for (ItemIter ii = iter_begin(); ii.item < a.n_items; iter_next(ii)) {
+            // ===== TMA producer: the x window once per item, then the W1 rows of every (chunk, k-block) =====
+            int it = 0, n = 0;
+            for (ItemIter ii = iter_begin(); ii.item < a.n_items; iter_next(ii), ++n) {
                 const Item w = decode(ii);
                 const int ey0 = w.oh0 * STRIDE - a.pad, ex0 = w.ow0 * STRIDE - a.pad;     // window origin in e / x coordinates
+                const int b = n % WBUF;
+                mbar_wait(&wempty[b], ((uint32_t)(n / WBUF) & 1u) ^ 1u);
+                uint8_t* win = smem + b * L::WIN_BYTES;                                     // [k-block][half][128 pixels][32 channels]
+                mbar_expect_tx(&wfull[b], (uint32_t)L::WIN_BYTES);
+#pragma unroll
+                for (int kb = 0; kb < NKB; ++kb) {
+                    tma_load_4d(&mp.x[w.prob], win + kb * KB_BYTES, &wfull[b], kb * BK, ex0, ey0, w.img);
+                    tma_load_4d(&mp.x[w.prob], win + kb * KB_BYTES + HALF_BYTES, &wfull[b], kb * BK, ex0, ey0 + 8, w.img);
+                }
                 for (int c = w.c_begin; c < w.c_end; ++c)
-                    for (int kb = 0; kb < a.nkb; ++kb, ++it) {
+                    for (int kb = 0; kb < NKB; ++kb, ++it) {
                         const int s = it % STAGES;
                         mbar_wait(&empty[s], ((uint32_t)(it / STAGES) & 1u) ^ 1u);
-                        uint8_t* st = smem + s * STAGE_BYTES;
-                        mbar_expect_tx(&full[s], (uint32_t)(smk::STAGE_BYTES + (X3 ? B_BYTES : 0)));
-                        tma_load_4d(&mp.x[w.prob], st, &full[s], kb * BK, ex0, ey0, w.img);
-                        tma_load_4d(&mp.x[w.prob], st + HALF_BYTES, &full[s], kb * BK, ex0, ey0 + 8, w.img);
-                        tma_load_2d(&mp.w[w.prob], st + 2 * HALF_BYTES, &full[s], kb * BK, c * NC);
-                        if (X3) tma_load_2d(&mp.wlo[w.prob], st + WLO, &full[s], kb * BK, c * NC);
+                        uint8_t* st = ring + s * STAGE_BYTES;
+                        mbar_expect_tx(&full[s], (uint32_t)STAGE_BYTES);
+                        tma_load_2d(&mp.w[w.prob], st, &full[s], kb * BK, c * NC);
+                        if (X3) tma_load_2d(&mp.wlo[w.prob], st + B_BYTES, &full[s], kb * BK, c * NC);
                     }
             }
         }
@@ -176,8 +220,11 @@ xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
     const int ncols_e = a.Wo - (a.tiles_x - 1) * TO, nrows_e = a.Ho - (a.tiles_y - 1) * TO;
     const unsigned role = (unsigned)(slot % TO) | (unsigned)(slot / TO) << 8 | (unsigned)(slot % ncols_e) << 16 | (unsigned)(slot / ncols_e) << 24;
     int cc = 0, it = 0;
-    for (; ii.item < a.n_items;) {
+    for (int n = 0; ii.item < a.n_items; ++n) {
       const Item w = decode(ii);
+      const int wb = n % WBUF;
+      const uint8_t* win = smem + wb * L::WIN_BYTES + half * HALF_BYTES;     // this warpgroup's half of k-block 0
+      mbar_wait(&wfull[wb], (uint32_t)(n / WBUF) & 1u);
       const int img = w.img, oh0 = w.oh0, ow0 = w.ow0;
       const int ey0 = oh0 * STRIDE - a.pad, ex0 = ow0 * STRIDE - a.pad;
       // this thread's output column dw_ox and output rows [dw_oy0, dw_oy1) of the tile
@@ -204,27 +251,30 @@ xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
         for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
             for (int i = 0; i < NC / 2; ++i) acc[mb][i] = 0.f;
-        for (int kb = 0; kb < a.nkb; ++kb, ++it) {
+#pragma unroll
+        for (int kb = 0; kb < NKB; ++kb, ++it) {
+            // k-steps of this k-block: all four, except KSL in the last one, where the steps over the channels past Cin
+            // (zero-filled by TMA) would only add zeros.  Known at compile time, so no wgmma sits behind a branch.
+            const int nks = kb + 1 < NKB ? BK / MMA_K : KSL;
             const int s = it % STAGES;
             mbar_wait(&full[s], (uint32_t)(it / STAGES) & 1u);
-            const uint8_t* st = smem + s * STAGE_BYTES;
-            const uint32_t sa = smem_u32(st) + (uint32_t)(half * HALF_BYTES);
-            const uint32_t sb = smem_u32(st) + 2 * HALF_BYTES;
+            const uint8_t* xa = win + kb * KB_BYTES;
+            const uint32_t sb = smem_u32(ring + s * STAGE_BYTES);
             if constexpr (X3 != 0) {
                 uint32_t hi[2][BK / MMA_K][4], lo[2][BK / MMA_K][4];
 #pragma unroll
                 for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
-                    for (int k = 0; k < BK / MMA_K; ++k) {
+                    for (int k = 0; k < nks; ++k) {
                         float v[4];
-                        load_a_frag(st + half * HALF_BYTES, mb * 64, k * MMA_K, wq, lane, v);
+                        load_a_frag(xa, mb * 64, k * MMA_K, wq, lane, v);
                         split_frag(v, hi[mb][k], lo[mb][k]);
                     }
                 wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < BK / MMA_K; ++k) {
+                for (int k = 0; k < nks; ++k) {
                     const uint64_t db = make_smem_desc(sb + k * MMA_K * 4);
-                    const uint64_t dbl = make_smem_desc(smem_u32(st) + WLO + k * MMA_K * 4);
+                    const uint64_t dbl = make_smem_desc(sb + B_BYTES + k * MMA_K * 4);
 #pragma unroll
                     for (int mb = 0; mb < 2; ++mb) {
                         Wgmma<NC>::rs(acc[mb], hi[mb][k], db, 1u);       // x_hi * w_hi
@@ -233,9 +283,10 @@ xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
                     }
                 }
             } else {
+                const uint32_t sa = smem_u32(xa);
                 wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < BK / MMA_K; ++k) {
+                for (int k = 0; k < nks; ++k) {
                     const uint64_t db = make_smem_desc(sb + k * MMA_K * 4);
 #pragma unroll
                     for (int mb = 0; mb < 2; ++mb)
@@ -245,8 +296,9 @@ xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
             wgmma_commit();
             wgmma_wait<0>();
             __syncwarp();
-            if (lane == 0) mbar_arrive(&empty[s]);
+            mbar_arrive_if(&empty[s], lane == 0);
         }
+        mbar_arrive_if(&wempty[wb], lane == 0 && c + 1 == w.c_end);     // the item's last MMAs have read the window
         // (a) accumulators -> BN1 + ReLU -> E.  Channels past `mid` have zero scale and bias in the parameter block, pixels
         // outside the image are zeroed: that is the zero padding of e the depthwise conv expects.
 #pragma unroll
@@ -334,14 +386,37 @@ xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
     }
 }
 
-template <int STRIDE, int X3>
+template <int STRIDE, int X3, int NKB, int KSL>
 int launch(const XdwMaps& mp, const XdwArgs& a, int grid, cudaStream_t st) {
-    constexpr size_t smem = (size_t)STAGES * (STAGE_BYTES + (X3 ? B_BYTES : 0)) + E_BYTES + PAR_BYTES + 1024 + 256;  // 3xTF32: + the weight tails
-    static_assert(X3 || 2 * (smem + 1024) <= 228 * 1024, "two CTAs per SM");
-    SMK_CHECK_CUDA((set_max_dynamic_smem<xdw_kernel<STRIDE, X3>>((int)smem)));
-    SMK_LAUNCH((xdw_kernel<STRIDE, X3>), dim3(grid), dim3(NUM_THREADS), smem, st, mp, a);
+    constexpr size_t smem = XdwSmem<NKB, X3>::SMEM;
+    SMK_CHECK_CUDA((set_max_dynamic_smem<xdw_kernel<STRIDE, X3, NKB, KSL>>((int)smem)));
+    SMK_LAUNCH((xdw_kernel<STRIDE, X3, NKB, KSL>), dim3(grid), dim3(NUM_THREADS), smem, st, mp, a);
     SMK_CHECK_LAUNCH();
     return 0;
+}
+
+template <int STRIDE, int X3, int NKB>
+int launch_ksl(int ksl, const XdwMaps& mp, const XdwArgs& a, int grid, cudaStream_t st) {
+    switch (ksl) {
+        case 1: return launch<STRIDE, X3, NKB, 1>(mp, a, grid, st);
+        case 2: return launch<STRIDE, X3, NKB, 2>(mp, a, grid, st);
+        case 3: return launch<STRIDE, X3, NKB, 3>(mp, a, grid, st);
+        default: return launch<STRIDE, X3, NKB, 4>(mp, a, grid, st);
+    }
+}
+
+// instantiation by window size: Cin = 32 (nkb - 1) + 8 ksl (rounded up to a multiple of 8), nkb <= MAX_NKB
+template <int STRIDE, int X3>
+int launch_cin(int Cin, const XdwMaps& mp, const XdwArgs& a, int grid, cudaStream_t st) {
+    static_assert(MAX_NKB == 5, "one case per window size");
+    const int nkb = cdiv(Cin, BK), ksl = cdiv(Cin, MMA_K) - (nkb - 1) * (BK / MMA_K);
+    switch (nkb) {
+        case 1: return launch_ksl<STRIDE, X3, 1>(ksl, mp, a, grid, st);
+        case 2: return launch_ksl<STRIDE, X3, 2>(ksl, mp, a, grid, st);
+        case 3: return launch_ksl<STRIDE, X3, 3>(ksl, mp, a, grid, st);
+        case 4: return launch_ksl<STRIDE, X3, 4>(ksl, mp, a, grid, st);
+        default: return launch_ksl<STRIDE, X3, 5>(ksl, mp, a, grid, st);
+    }
 }
 
 }  // namespace
@@ -350,6 +425,7 @@ int xdw_conv(const XdwConv& p, cudaStream_t st, const XdwConv* p2) {
     const int nprob = p2 ? 2 : 1;
     SMK_REQUIRE(p.stride == 1 || p.stride == 2, "xdw_conv: stride must be 1 or 2");
     SMK_REQUIRE(p.Cin % 4 == 0 && p.mid % 4 == 0, "xdw_conv: Cin and mid must be multiples of 4");
+    SMK_REQUIRE(p.Cin > 0 && p.Cin <= MAX_NKB * BK, "xdw_conv: Cin must be at most 160 (the whole input window stays in shared memory)");
     SMK_REQUIRE(p.stride == 1 || (p.H % 2 == 0 && p.W % 2 == 0), "xdw_conv: stride 2 expects even input sizes (TF-SAME pad_begin 0)");
     SMK_REQUIRE(!p2 || (p2->B == p.B && p2->H == p.H && p2->W == p.W && p2->Cin == p.Cin && p2->mid == p.mid && p2->stride == p.stride &&
                         p2->round_out == p.round_out && !p2->w1t_lo == !p.w1t_lo), "xdw_conv: paired problems must have identical shapes");
@@ -369,10 +445,10 @@ int xdw_conv(const XdwConv& p, cudaStream_t st, const XdwConv* p2) {
         mp.x[1] = mp.x[0]; mp.w[1] = mp.w[0]; mp.wlo[1] = mp.wlo[0];
         a.scale1[1] = a.scale1[0]; a.bias1[1] = a.bias1[0]; a.wdw[1] = a.wdw[0]; a.scale2[1] = a.scale2[0]; a.bias2[1] = a.bias2[0]; a.out[1] = a.out[0];
     }
-    // Resident CTAs to aim for: one per SM (two would fit) leaves room on every SM for the other backbones' and batches'
+    // Resident CTAs to aim for: one per SM (two fit for plain TF32 with Cin <= 64) leaves room on every SM for the other backbones' and batches'
     // kernels of the concurrent pipeline.
     const int slots = num_sms();
-    a.H = p.H; a.W = p.W; a.Ho = Ho; a.Wo = Wo; a.mid = p.mid; a.nkb = cdiv(p.Cin, BK); a.nchunks = cdiv(p.mid, NC);
+    a.H = p.H; a.W = p.W; a.Ho = Ho; a.Wo = Wo; a.mid = p.mid; a.nchunks = cdiv(p.mid, NC);
     {   // split the channel chunks over enough CTAs to fill the resident slots
         const long tiles = (long)nprob * cdiv(Wo, TO) * cdiv(Ho, TO) * p.B;
         int groups = (int)std::min<long>(a.nchunks, std::max<long>(1, (slots + tiles - 1) / tiles));
@@ -397,8 +473,8 @@ int xdw_conv(const XdwConv& p, cudaStream_t st, const XdwConv* p2) {
     }
     const int grid = std::min(a.n_items, slots);         // persistent
     { int v = grid; a.d_grp = v % a.groups; v /= a.groups; a.d_tx = v % a.tiles_x; v /= a.tiles_x; a.d_ty = v % a.tiles_y; a.d_img = v / a.tiles_y; }
-    if (p.w1t_lo) return p.stride == 1 ? launch<1, 2>(mp, a, grid, st) : launch<2, 2>(mp, a, grid, st);
-    return p.stride == 1 ? launch<1, 0>(mp, a, grid, st) : launch<2, 0>(mp, a, grid, st);
+    if (p.w1t_lo) return p.stride == 1 ? launch_cin<1, 2>(p.Cin, mp, a, grid, st) : launch_cin<2, 2>(p.Cin, mp, a, grid, st);
+    return p.stride == 1 ? launch_cin<1, 0>(p.Cin, mp, a, grid, st) : launch_cin<2, 0>(p.Cin, mp, a, grid, st);
 }
 
 }  // namespace smk
