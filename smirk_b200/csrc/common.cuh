@@ -1,6 +1,7 @@
 // Shared helpers for the smirk_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
@@ -66,6 +67,20 @@ struct Workspace {
     }
 };
 static inline size_t ws_round(size_t bytes) { return (bytes + 255) & ~size_t(255); }
+
+// Walks the host tensor list of a create call (state_dict order); null past the end.
+struct TensorCursor {
+    const float* const* t; int n; int i = 0;
+    const float* next() { return i < n ? t[i++] : nullptr; }
+};
+
+// Eval-mode BatchNorm folded into a per-channel scale and bias: s = g / sqrt(var + eps), b' = beta - mu * s.
+static inline void fold_bn(const float* g, const float* beta, const float* mu, const float* var, int n, float eps, float* s, float* b) {
+    for (int o = 0; o < n; ++o) {
+        const float so = g[o] / sqrtf(var[o] + eps);
+        s[o] = so; b[o] = beta[o] - mu[o] * so;
+    }
+}
 
 static inline int cdiv(long a, long b) { return (int)((a + b - 1) / b); }
 

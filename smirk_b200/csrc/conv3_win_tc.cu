@@ -282,14 +282,14 @@ int launch(const CUtensorMap& tmX, const CUtensorMap& tmW, const WinArgs& a, cud
 
 }  // namespace
 
-bool conv3_win_supported(const TcConv& p) {
+bool conv3_win_supported(const Conv& p) {
     if (p.mode != 1 || p.res || p.wt_lo || (p.store != 0 && p.store != 3) || (p.store == 3 && (p.N != 32 || p.mask))) return false;
     if (p.Cin % 32 != 0 || p.K != 9 * p.Cin || (p.N != 32 && p.N != 64)) return false;
     return p.W >= 56;                                             // low-resolution layers are MMA-bound: gemm_tc's wide tiles win there
 }
 
-// p uses TcConv semantics: mode 1 (3x3, zero padding 1), store 0 or 3, no residual.
-int conv3_win(const TcConv& p, cudaStream_t st) {
+// mode 1 (3x3, zero padding 1), store 0 or 3, no residual.
+int conv3_win(const Conv& p, cudaStream_t st) {
     SMK_REQUIRE(conv3_win_supported(p), "conv3_win: unsupported problem (needs 3x3 zero-pad, Cin %% 32 == 0, N in {32, 64}, W >= 56)");
     SMK_REQUIRE(p.N % 4 == 0 && p.ld_in % 4 == 0 && p.ld_out % 4 == 0, "conv3_win: N and strides must be multiples of 4");
     SMK_REQUIRE(p.store != 3 || (p.N == 32 && p.head_w && p.head_b && p.head_c >= 1 && p.head_c <= 4), "conv3_win: the fused head needs N == 32");
@@ -319,7 +319,7 @@ int conv3_win(const TcConv& p, cudaStream_t st) {
 
 extern "C" int smk_debug_conv3_win(const float* in, int ld_in, int B, int H, int W, int Cin, const float* wt, const float* scale,
                                    const float* bias, int N, int relu, float* out, int ld_out, void* stream) {
-    smk::TcConv p{};
+    smk::Conv p{};
     p.in = in; p.ld_in = ld_in; p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.wt = wt; p.scale = scale; p.bias = bias; p.N = N; p.K = 9 * Cin;
     p.mode = 1; p.relu = relu; p.out = out; p.ld_out = ld_out; p.store = 0;
     return smk::conv3_win(p, (cudaStream_t)stream);

@@ -12,7 +12,7 @@
 
 namespace {
 
-using smk::ConvProblem;
+using smk::TensorCursor;
 
 constexpr float kBnEps = 1e-3f;
 
@@ -53,11 +53,6 @@ int make_divisible(double v, int divisor = 8) {
 }
 
 // Consumes (conv weight, bn gamma, beta, mean, var) from the tensor list.
-struct TensorCursor {
-    const float* const* t; int n; int i = 0;
-    const float* next() { return i < n ? t[i++] : nullptr; }
-};
-
 // kind: 0 = 1x1 [Cout,Cin,1,1] -> W[Cin][Cout]; 1 = depthwise [C,1,3,3] -> W[9][C]; 2 = stem [16,3,3,3] -> W[27][16]
 bool fold_conv(TensorCursor& cur, int kind, int cin, int cout, bool tc, smk::DeviceArena& arena, ConvW* out, cudaError_t* err, bool x3 = false) {
     const float* w = cur.next(); const float* g = cur.next(); const float* b = cur.next();
@@ -81,10 +76,7 @@ bool fold_conv(TensorCursor& cur, int kind, int cin, int cout, bool tc, smk::Dev
         W.resize((size_t)27 * cout);
         for (int o = 0; o < cout; ++o) for (int k = 0; k < 27; ++k) W[(size_t)k * cout + o] = w[(size_t)o * 27 + k];
     }
-    for (int o = 0; o < cout; ++o) {
-        float s = g[o] / sqrtf(var[o] + kBnEps);
-        S[o] = s; Bi[o] = b[o] - mu[o] * s;
-    }
+    smk::fold_bn(g, b, mu, var, cout, kBnEps, S.data(), Bi.data());
     out->cin = cin; out->cout = cout;
     cudaError_t e = arena.upload(W, (kind == 0 && tc) ? &out->wt : &out->w);
     if (e == cudaSuccess && !Wlo.empty()) e = arena.upload(Wlo, &out->wt_lo);
@@ -201,32 +193,20 @@ extern "C" size_t smk_encoder_workspace_bytes(const SmkEncoder* h, int B) {
     return 12 * smk::ws_round((size_t)B * h->max_act * sizeof(float));      // 4 buffers per backbone, 3 concurrent backbones
 }
 
-static smk::TcConv tc_problem(const ConvW& c, const float* in, int B, int H, int W, bool relu, const float* res, float* out) {
-    smk::TcConv q{};
-    q.in = in; q.ld_in = c.cin; q.B = B; q.H = H; q.W = W; q.Cin = c.cin; q.wt = c.wt; q.wt_lo = c.wt_lo; q.scale = c.scale; q.bias = c.bias;
-    q.N = c.cout; q.K = c.cin; q.mode = 0; q.relu = relu ? 1 : 0; q.res = res; q.ld_res = c.cout; q.res_pad = 0;
-    q.out = out; q.ld_out = c.cout; q.store = 0; q.round_out = c.wt_lo ? 0 : 1;       // 3xTF32 consumers split full fp32 activations themselves
-    return q;
-}
-
 // One 1x1 convolution for n = 1 or 2 backbones of identical structure (c[k], in[k], res[k], out[k]).  On the tensor-core
 // path a pair shares ONE launch (gemm_tc.cu, TcMaps): half the launches and twice the tiles per launch for layers that
-// sit on the launch/latency floor.
+// sit on the launch/latency floor.  Backbones are paired only on the tensor-core path.
 static int pointwise(int n, const ConvW* const* c, float* const* in, int B, int H, int W, bool relu, float* const* res, float* const* out, cudaStream_t st) {
-    if (c[0]->wt) {
-        smk::TcConv q0 = tc_problem(*c[0], in[0], B, H, W, relu, res ? res[0] : nullptr, out[0]);
-        if (n == 1) return smk::tc_conv(q0, st);
-        smk::TcConv q1 = tc_problem(*c[1], in[1], B, H, W, relu, res ? res[1] : nullptr, out[1]);
-        return smk::tc_conv(q0, st, &q1);
-    }
+    smk::Conv q[2];
     for (int k = 0; k < n; ++k) {
-        ConvProblem p{};
-        p.in = in[k]; p.ld_in = c[k]->cin; p.B = B; p.H = H; p.W = W; p.Cin = c[k]->cin;
-        p.w = c[k]->w; p.scale = c[k]->scale; p.bias = c[k]->bias; p.N = c[k]->cout; p.K = c[k]->cin; p.mode = 0; p.relu = relu ? 1 : 0;
-        p.res = res ? res[k] : nullptr; p.ld_res = c[k]->cout; p.out = out[k]; p.ld_out = c[k]->cout; p.shuffle = 0;
-        if (int rc = smk::conv_gemm(p, st)) return rc;
+        q[k] = smk::Conv{};
+        q[k].in = in[k]; q[k].ld_in = c[k]->cin; q[k].B = B; q[k].H = H; q[k].W = W; q[k].Cin = c[k]->cin;
+        q[k].w = c[k]->w; q[k].wt = c[k]->wt; q[k].wt_lo = c[k]->wt_lo; q[k].scale = c[k]->scale; q[k].bias = c[k]->bias;
+        q[k].N = c[k]->cout; q[k].K = c[k]->cin; q[k].mode = 0; q[k].relu = relu ? 1 : 0;
+        q[k].res = res ? res[k] : nullptr; q[k].ld_res = c[k]->cout; q[k].out = out[k]; q[k].ld_out = c[k]->cout;
+        q[k].round_out = c[k]->wt && !c[k]->wt_lo;      // 3xTF32 consumers split full fp32 activations themselves
     }
-    return 0;
+    return smk::conv(q[0], st, n == 2 ? &q[1] : nullptr);
 }
 
 extern "C" int smk_encoder_forward(const SmkEncoder* h, const float* img, int B, float* pose_cam, float* shape,

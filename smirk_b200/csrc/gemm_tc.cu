@@ -428,7 +428,7 @@ int launch(const TcMaps& mp, const TcArgs& a, cudaStream_t st, int groups) {
 
 }  // namespace
 
-int tc_conv(const TcConv& p, cudaStream_t st, const TcConv* p2) {
+int tc_conv(const Conv& p, cudaStream_t st, const Conv* p2) {
     if (!p2 && conv3_win_supported(p)) return conv3_win(p, st);       // 224^2 / 112^2, Cout 32 / 64: one patch load per chunk, resident weights
     const int M = p.B * p.H * p.W;
     const int groups = p2 ? 2 : 1;
@@ -458,7 +458,7 @@ int tc_conv(const TcConv& p, cudaStream_t st, const TcConv* p2) {
                 "tc_conv: the mask needs store 0, the second store a non-shuffled store, both a single TF32 problem");
     a.mask = p.mask; a.ld_mask = p.ld_mask; a.out2 = p.out2; a.ld_out2 = p.ld_out2;
     for (int g = 0; g < groups; ++g) {
-        const TcConv& q = g ? *p2 : p;
+        const Conv& q = g ? *p2 : p;
         a.scale[g] = q.scale; a.bias[g] = q.bias; a.res[g] = q.res; a.out[g] = q.out;
         if (q.mode == 0) {
             if (int rc = encode_2d(&mp.a[g], q.in, (uint64_t)M, (uint64_t)q.K, (uint64_t)q.ld_in, BM, "tc_conv(A)")) return rc;
@@ -522,7 +522,7 @@ int reflect_halo(float* buf, int B, int H, int W, int C, cudaStream_t st) {
 extern "C" int smk_debug_conv_tc(const float* in, int ld_in, int B, int H, int W, int Cin, const float* wt, const float* scale,
                                  const float* bias, int N, int K, int mode, int relu, const float* res, int ld_res, int res_pad,
                                  float* out, int ld_out, int store, void* stream) {
-    smk::TcConv p{};
+    smk::Conv p{};
     p.in = in; p.ld_in = ld_in; p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.wt = wt; p.scale = scale; p.bias = bias; p.N = N; p.K = K;
     p.mode = mode; p.relu = relu; p.res = res; p.ld_res = ld_res; p.res_pad = res_pad; p.out = out; p.ld_out = ld_out; p.store = store;
     return smk::tc_conv(p, (cudaStream_t)stream);
@@ -530,7 +530,7 @@ extern "C" int smk_debug_conv_tc(const float* in, int ld_in, int B, int H, int W
 // 1x1 conv / GEMM on the 3xTF32 path: wt_hi / wt_lo are the TF32 heads and tails of the [N][K] weights.
 extern "C" int smk_debug_gemm_tc3x(const float* in, int ld_in, int M, const float* wt_hi, const float* wt_lo, const float* scale,
                                    const float* bias, int N, int K, int relu, const float* res, int ld_res, float* out, int ld_out, void* stream) {
-    smk::TcConv p{};
+    smk::Conv p{};
     p.in = in; p.ld_in = ld_in; p.B = 1; p.H = 1; p.W = M; p.Cin = K; p.wt = wt_hi; p.wt_lo = wt_lo; p.scale = scale; p.bias = bias; p.N = N; p.K = K;
     p.mode = 0; p.relu = relu; p.res = res; p.ld_res = ld_res; p.res_pad = 0; p.out = out; p.ld_out = ld_out; p.store = 0; p.round_out = 0;
     return smk::tc_conv(p, (cudaStream_t)stream);

@@ -30,8 +30,7 @@
 
 namespace {
 
-using smk::ConvProblem;
-using smk::TcConv;
+using smk::TensorCursor;
 constexpr float kBnEps = 1e-5f;
 
 // dw: dgrad weights, W' scaled by the folded BN scale: [9*cout][cin_p] (fp32) or [cin_p][9*cout] (TF32), k = tap' * cout + co
@@ -39,21 +38,13 @@ struct Conv3 { float* w; float* wt; float* scale; float* bias; float* dw; int ci
 // dw: [4*cout][cin] (fp32) or [cin][4*cout] (TF32), k = (dy*2+dx) * cout + co
 struct UpConv { float* w; float* wt; float* scale; float* bias; float* dw; int cin, cout; };         // w: [cin][4*cout];   wt: [4*cout][cin]
 
-struct TensorCursor {
-    const float* const* t; int n; int i = 0;
-    const float* next() { return i < n ? t[i++] : nullptr; }
-};
-
 bool fold_conv3(TensorCursor& cur, int cin, int cin_p, int cout, bool tc, smk::DeviceArena& arena, Conv3* out, cudaError_t* err) {
     const float* w = cur.next(); const float* g = cur.next(); const float* b = cur.next();
     const float* mu = cur.next(); const float* var = cur.next();
     if (!w || !g || !b || !mu || !var) return false;
     const size_t K = (size_t)9 * cin_p, Kd = (size_t)9 * cout;
     std::vector<float> W(K * cout, 0.f), D(Kd * cin_p, 0.f), S(cout), Bi(cout);
-    for (int o = 0; o < cout; ++o) {
-        float s = g[o] / sqrtf(var[o] + kBnEps);
-        S[o] = s; Bi[o] = b[o] - mu[o] * s;
-    }
+    smk::fold_bn(g, b, mu, var, cout, kBnEps, S.data(), Bi.data());
     for (int o = 0; o < cout; ++o)
         for (int c = 0; c < cin; ++c)
             for (int k = 0; k < 9; ++k) {
@@ -212,21 +203,13 @@ Plan make_plan(const SmkGenerator* h) {
 int conv3(const SmkGenerator* h, const Conv3& c, const float* in, int ld_in, int B, int S, bool refl, bool relu,
           const float* res, int res_pad, float* out, int ld_out, int store, cudaStream_t st, bool fuse_head = false,
           float* out2 = nullptr) {
-    if (c.wt) {
-        TcConv p{};
-        if (fuse_head) { p.head_w = h->fw; p.head_b = h->fb; p.head_c = h->cout; }
-        p.in = in; p.ld_in = ld_in; p.B = B; p.H = S; p.W = S; p.Cin = c.cin_p; p.wt = c.wt; p.scale = c.scale; p.bias = c.bias;
-        p.N = c.cout; p.K = 9 * c.cin_p; p.mode = refl ? 2 : 1; p.relu = relu ? 1 : 0;
-        p.res = res; p.ld_res = c.cout; p.res_pad = res_pad; p.out = out; p.ld_out = ld_out; p.store = store; p.round_out = 1;
-        p.out2 = out2; p.ld_out2 = c.cout;
-        return smk::tc_conv(p, st);
-    }
-    ConvProblem p{};
-    p.in = in; p.ld_in = ld_in; p.B = B; p.H = S; p.W = S; p.Cin = c.cin_p;
-    p.w = c.w; p.scale = c.scale; p.bias = c.bias; p.N = c.cout; p.K = 9 * c.cin_p; p.mode = refl ? 2 : 1; p.relu = relu ? 1 : 0;
-    p.res = res; p.ld_res = c.cout; p.out = out; p.ld_out = ld_out; p.shuffle = 0; p.round_out = h->precision == 1 ? 1 : 0;
+    smk::Conv p{};
+    if (fuse_head) { p.head_w = h->fw; p.head_b = h->fb; p.head_c = h->cout; }
+    p.in = in; p.ld_in = ld_in; p.B = B; p.H = S; p.W = S; p.Cin = c.cin_p; p.w = c.w; p.wt = c.wt; p.scale = c.scale; p.bias = c.bias;
+    p.N = c.cout; p.K = 9 * c.cin_p; p.mode = refl ? 2 : 1; p.relu = relu ? 1 : 0;
+    p.res = res; p.ld_res = c.cout; p.res_pad = res_pad; p.out = out; p.ld_out = ld_out; p.store = store; p.round_out = c.wt ? 1 : 0;
     p.out2 = out2; p.ld_out2 = c.cout;
-    return smk::conv_gemm(p, st);
+    return smk::conv(p, st);
 }
 
 // Index of a saved tensor (forward order, see smk_generator_create).
@@ -301,18 +284,10 @@ int generator_forward(const SmkGenerator* h, const float* x, int B, float* y, fl
     for (int l = 0; l < 4; ++l) {
         int lvl = 3 - l;                            // index into cat/t/d (3 = 28x28 ... 0 = 224x224)
         const UpConv& u = h->up[l];
-        if (u.wt) {
-            TcConv q{};
-            q.in = din; q.ld_in = u.cin; q.B = B; q.H = dS; q.W = dS; q.Cin = u.cin; q.wt = u.wt; q.scale = u.scale; q.bias = u.bias;
-            q.N = 4 * u.cout; q.K = u.cin; q.mode = 0; q.relu = 0; q.res = nullptr; q.out = cat[lvl]; q.ld_out = 2 * u.cout; q.store = 1; q.round_out = 1;
-            if ((rc = smk::tc_conv(q, st))) return rc;
-        } else {
-            ConvProblem q{};
-            q.in = din; q.ld_in = u.cin; q.B = B; q.H = dS; q.W = dS; q.Cin = u.cin; q.w = u.w; q.scale = u.scale; q.bias = u.bias;
-            q.N = 4 * u.cout; q.K = u.cin; q.mode = 0; q.relu = 0; q.res = nullptr; q.ld_res = 0;
-            q.out = cat[lvl]; q.ld_out = 2 * u.cout; q.shuffle = 1;
-            if ((rc = smk::conv_gemm(q, st))) return rc;
-        }
+        smk::Conv q{};
+        q.in = din; q.ld_in = u.cin; q.B = B; q.H = dS; q.W = dS; q.Cin = u.cin; q.w = u.w; q.wt = u.wt; q.scale = u.scale; q.bias = u.bias;
+        q.N = 4 * u.cout; q.K = u.cin; q.mode = 0; q.out = cat[lvl]; q.ld_out = 2 * u.cout; q.store = 1; q.round_out = u.wt ? 1 : 0;
+        if ((rc = smk::conv(q, st))) return rc;
         dS *= 2;
         float* dt = sv ? SV(sv_dec(h, lvl, 0)) : t[lvl];
         if ((rc = conv3(h, h->dec[l][0], cat[lvl], 2 * u.cout, B, dS, false, true, nullptr, 0, dt, u.cout, 0, st))) return rc;
@@ -465,34 +440,23 @@ int grid_of(long total) { return (int)std::min<long>((total + 255) / 256, 16L * 
 // dgrad of a 3x3 conv (zero padding 1): g_in = conv3x3(g, W') over S x S, * [mask > 0] (mask: the saved input activation).
 int dgrad3(const SmkGenerator* h, const Conv3& c, const float* g, int B, int S, const float* mask, float* out, int ld_out, bool round,
            cudaStream_t st) {
-    if (h->precision == 1) {
-        TcConv p{};
-        p.in = g; p.ld_in = c.cout; p.B = B; p.H = S; p.W = S; p.Cin = c.cout; p.wt = c.dw; p.scale = h->ones; p.bias = h->zeros;
-        p.N = c.cin_p; p.K = 9 * c.cout; p.mode = 1; p.out = out; p.ld_out = ld_out; p.store = 0; p.round_out = round ? 1 : 0;
-        p.mask = mask; p.ld_mask = c.cin_p; p.tag = "conv3x3_dgrad_tc";
-        return smk::tc_conv(p, st);
-    }
-    ConvProblem p{};
-    p.in = g; p.ld_in = c.cout; p.B = B; p.H = S; p.W = S; p.Cin = c.cout; p.w = c.dw; p.scale = h->ones; p.bias = h->zeros;
-    p.N = c.cin_p; p.K = 9 * c.cout; p.mode = 1; p.out = out; p.ld_out = ld_out; p.mask = mask; p.ld_mask = c.cin_p;
-    p.tag = "conv3x3_dgrad_f32";
-    return smk::conv_gemm(p, st);
+    const bool tc = h->precision == 1;
+    smk::Conv p{};
+    p.in = g; p.ld_in = c.cout; p.B = B; p.H = S; p.W = S; p.Cin = c.cout; p.w = tc ? nullptr : c.dw; p.wt = tc ? c.dw : nullptr; p.scale = h->ones; p.bias = h->zeros;
+    p.N = c.cin_p; p.K = 9 * c.cout; p.mode = 1; p.out = out; p.ld_out = ld_out; p.round_out = round ? 1 : 0;
+    p.mask = mask; p.ld_mask = c.cin_p; p.tag = tc ? "conv3x3_dgrad_tc" : "conv3x3_dgrad_f32";
+    return smk::conv(p, st);
 }
 
 // dgrad of ConvTranspose2d(k2, s2): g_in[S x S, cin] = s2d(g_out)[S x S, 4 cout] . W'^T, * [mask > 0].
 int dgrad_up(const SmkGenerator* h, const UpConv& u, const float* s2d, int B, int S, const float* mask, float* out, bool round, cudaStream_t st) {
+    const bool tc = h->precision == 1;
     const int K = 4 * u.cout;
-    if (h->precision == 1) {
-        TcConv p{};
-        p.in = s2d; p.ld_in = K; p.B = B; p.H = S; p.W = S; p.Cin = K; p.wt = u.dw; p.scale = h->ones; p.bias = h->zeros;
-        p.N = u.cin; p.K = K; p.mode = 0; p.out = out; p.ld_out = u.cin; p.store = 0; p.round_out = round ? 1 : 0;
-        p.mask = mask; p.ld_mask = u.cin; p.tag = "upconv_dgrad_tc";
-        return smk::tc_conv(p, st);
-    }
-    ConvProblem p{};
-    p.in = s2d; p.ld_in = K; p.B = B; p.H = S; p.W = S; p.Cin = K; p.w = u.dw; p.scale = h->ones; p.bias = h->zeros;
-    p.N = u.cin; p.K = K; p.mode = 0; p.out = out; p.ld_out = u.cin; p.mask = mask; p.ld_mask = u.cin; p.tag = "upconv_dgrad_f32";
-    return smk::conv_gemm(p, st);
+    smk::Conv p{};
+    p.in = s2d; p.ld_in = K; p.B = B; p.H = S; p.W = S; p.Cin = K; p.w = tc ? nullptr : u.dw; p.wt = tc ? u.dw : nullptr; p.scale = h->ones; p.bias = h->zeros;
+    p.N = u.cin; p.K = K; p.mode = 0; p.out = out; p.ld_out = u.cin; p.round_out = round ? 1 : 0;
+    p.mask = mask; p.ld_mask = u.cin; p.tag = tc ? "upconv_dgrad_tc" : "upconv_dgrad_f32";
+    return smk::conv(p, st);
 }
 
 int fold(const float* gP, const float* res, int res_pad, const float* mask, int B, int C, bool round, float* out, int out_pad, cudaStream_t st) {

@@ -12,7 +12,7 @@ constexpr int NT = 256;
 // register tiles; global->register prefetch of the next k-slab overlaps the FMAs of the current one.
 template <int BM, int BN>
 __global__ void __launch_bounds__(NT)
-conv_gemm_kernel(ConvProblem p, int M) {
+conv_gemm_kernel(Conv p, int M) {
     constexpr int TM = BM / 16, TN = BN / 16;
     constexpr int A_LD = BM + 4, B_LD = BN + 4;
     constexpr int A_PER = BM / 64;                 // float4 loads of A per thread per slab (BM*BK/4/NT)
@@ -127,7 +127,7 @@ conv_gemm_kernel(ConvProblem p, int M) {
             if (p.mask && !(p.mask[(size_t)m * p.ld_mask + n] > 0.f)) v = 0.f;
             if (p.round_out) v = round_tf32(v);
             if (p.out2) p.out2[(size_t)m * p.ld_out2 + n] = v;
-            if (p.shuffle) {
+            if (p.store == 1) {
                 int cout = p.N >> 2, q = n / cout, co = n - q * cout;
                 int b = m / HW, r = m - b * HW, h = r / p.W, w = r - h * p.W;
                 size_t dp = ((size_t)b * (2 * p.H) + 2 * h + (q >> 1)) * (2 * p.W) + 2 * w + (q & 1);
@@ -140,38 +140,6 @@ conv_gemm_kernel(ConvProblem p, int M) {
 }
 
 // ---------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-dwconv3x3_kernel(const float* __restrict__ in, int B, int H, int W, int C, int stride, int pad, int Ho, int Wo,
-                 const float* __restrict__ w9c, const float* __restrict__ scale, const float* __restrict__ bias,
-                 float* __restrict__ out) {
-    const int C4 = C >> 2;
-    const long total = (long)B * Ho * Wo * C4;
-    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-        int c4 = (int)(i % C4); long pix = i / C4;
-        int ow = (int)(pix % Wo); long t = pix / Wo; int oh = (int)(t % Ho); int b = (int)(t / Ho);
-        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-        for (int ky = 0; ky < 3; ++ky) {
-            int ih = oh * stride + ky - pad;
-            if (ih < 0 || ih >= H) continue;
-#pragma unroll
-            for (int kx = 0; kx < 3; ++kx) {
-                int iw = ow * stride + kx - pad;
-                if (iw < 0 || iw >= W) continue;
-                float4 x = *reinterpret_cast<const float4*>(in + (((size_t)b * H + ih) * W + iw) * C + c4 * 4);
-                float4 k = *reinterpret_cast<const float4*>(w9c + (size_t)(ky * 3 + kx) * C + c4 * 4);
-                acc.x = fmaf(x.x, k.x, acc.x); acc.y = fmaf(x.y, k.y, acc.y);
-                acc.z = fmaf(x.z, k.z, acc.z); acc.w = fmaf(x.w, k.w, acc.w);
-            }
-        }
-        float4 s = *reinterpret_cast<const float4*>(scale + c4 * 4), bb = *reinterpret_cast<const float4*>(bias + c4 * 4);
-        float4 o;
-        o.x = fmaxf(fmaf(acc.x, s.x, bb.x), 0.f); o.y = fmaxf(fmaf(acc.y, s.y, bb.y), 0.f);
-        o.z = fmaxf(fmaf(acc.z, s.z, bb.z), 0.f); o.w = fmaxf(fmaf(acc.w, s.w, bb.w), 0.f);
-        *reinterpret_cast<float4*>(out + (size_t)pix * C + c4 * 4) = o;
-    }
-}
-
 // Depthwise 3x3, 4 output pixels along W x 4 channels per thread: the 3 x (3 + 3*STRIDE) input window is
 // loaded once (float4 per pixel) and reused by the 4 outputs; weights stay in registers.
 template <int STRIDE>
@@ -226,49 +194,9 @@ dwconv3x3_px4_kernel(const float* __restrict__ in, int B, int H, int W, int C, i
     }
 }
 
-// Global average pool, split over channel chunks so the grid fills the machine: block = 64 channels x 4
-// pixel lanes; pooled[b][c] = mean over HW.
-__global__ void __launch_bounds__(256)
-gap_kernel(const float* __restrict__ feat, int HW, int C, float* __restrict__ pooled) {
-    __shared__ float part[4][64];
-    const int b = blockIdx.x, c = blockIdx.y * 64 + (threadIdx.x & 63), pl = threadIdx.x >> 6;
-    float s = 0.f;
-    if (c < C) {
-        const float* f = feat + (size_t)b * HW * C + c;
-        for (int p = pl; p < HW; p += 4) s += f[(size_t)p * C];
-    }
-    part[pl][threadIdx.x & 63] = s;
-    __syncthreads();
-    if (pl == 0 && c < C)
-        pooled[(size_t)b * C + c] = (part[0][threadIdx.x] + part[1][threadIdx.x] + part[2][threadIdx.x] + part[3][threadIdx.x]) * (1.f / (float)HW);
-}
-
-// out[b][o] = clamp(bias[o] + pooled[b] . w[o]); one warp per output, 8 outputs per block.
-__global__ void __launch_bounds__(256)
-head_linear_kernel(const float* __restrict__ pooled, int C, const float* __restrict__ w, const float* __restrict__ bias,
-                   int n_out, const uint8_t* __restrict__ codes, float* __restrict__ out) {
-    const int b = blockIdx.x, lane = threadIdx.x & 31, o = blockIdx.y * 8 + (threadIdx.x >> 5);
-    if (o >= n_out) return;
-    const float* wr = w + (size_t)o * C;
-    const float* pb = pooled + (size_t)b * C;
-    float acc = 0.f;
-    for (int c = lane; c < C; c += 32) acc = fmaf(pb[c], wr[c], acc);
-#pragma unroll
-    for (int s = 16; s > 0; s >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, s);
-    if (lane == 0) {
-        float v = acc + bias[o];
-        int code = codes ? codes[o] : 0;
-        if (code == 1) v = fminf(fmaxf(v, 0.f), 1.f);
-        else if (code == 2) v = fmaxf(v, 0.f);
-        else if (code == 3) v = fminf(fmaxf(v, -0.2f), 0.2f);
-        out[(size_t)b * n_out + o] = v;
-    }
-}
-
 // Global average pool + linear head + clamps in ONE launch for one or two backbones (blockIdx.z): every CTA pools its
 // image's feature map into shared memory (the map is L2-resident: 188 KB at 7x7x960) and computes 32 head outputs, one
-// warp per output (smirk_encoder.py:34-45,66-73,95-110).  Replaces gap_kernel + head_linear_kernel: 6 launches per
-// encoder pass become 2.
+// warp per output (smirk_encoder.py:34-45,66-73,95-110).
 struct GapHead { const float* feat[2]; const float* w[2]; const float* bias[2]; const uint8_t* codes[2]; float* out[2]; int n_out[2]; };
 __global__ void __launch_bounds__(256)
 gap_head_kernel(const __grid_constant__ GapHead g, int HW, int C) {
@@ -471,14 +399,16 @@ conv1x1_sigmoid_kernel(const float* __restrict__ in, int B, int HW, int Cin, con
 
 }  // namespace
 
-int conv_gemm(const ConvProblem& p, cudaStream_t st) {
+int conv_gemm(const Conv& p, cudaStream_t st) {
     const int M = p.B * p.H * p.W;
+    SMK_REQUIRE(!p.wt && !p.wt_lo, "conv_gemm: TF32 weights need tc_conv");
+    SMK_REQUIRE(!p.res_pad && (p.store == 0 || p.store == 1), "conv_gemm: padded residuals and stores 2 / 3 need tc_conv");
     SMK_REQUIRE(p.K % 4 == 0 && p.N % 4 == 0 && p.ld_in % 4 == 0, "conv_gemm: K, N, ld_in must be multiples of 4");
     SMK_REQUIRE(p.mode == 0 || p.Cin % 4 == 0, "conv_gemm: Cin must be a multiple of 4");
-    SMK_REQUIRE(!p.out2 || !p.shuffle, "conv_gemm: the second store does not support the pixel-shuffle layout");
+    SMK_REQUIRE(!p.out2 || p.store != 1, "conv_gemm: the second store does not support the pixel-shuffle layout");
     {
         const double cin_eff = p.mode == 0 ? p.K : p.Cin;       // unique input bytes (not im2col-expanded)
-        const char* tag = p.tag ? p.tag : p.mode == 0 ? (p.shuffle ? "upconv_gemm_f32" : "pw_gemm_f32") : "conv3x3_gemm_f32";
+        const char* tag = p.tag ? p.tag : p.mode == 0 ? (p.store == 1 ? "upconv_gemm_f32" : "pw_gemm_f32") : "conv3x3_gemm_f32";
         if (g_prof_detail) tag = prof_shape_tag(tag, M, p.K, p.N);
         SMK_TAG(tag,
                 4.0 * ((double)M * cin_eff + (double)p.K * p.N + (double)M * p.N * (1 + !!p.res + !!p.mask + !!p.out2) + 2.0 * p.N),
@@ -714,12 +644,6 @@ int stem_ds(const float* img, int B, int H, int W, const StemDsProblem* probs, i
     SMK_CHECK_LAUNCH();
     return 0;
 }
-int stem_ds(const float* img, int B, int H, int W, const float* stem_w, const float* stem_s, const float* stem_b,
-            const float* dw_w, const float* dw_s, const float* dw_b, const float* pw_w, const float* pw_s, const float* pw_b,
-            int stride, int round_out, float* out, cudaStream_t st) {
-    StemDsProblem q{stem_w, stem_s, stem_b, dw_w, dw_s, dw_b, pw_w, pw_s, pw_b, out};
-    return stem_ds(img, B, H, W, &q, 1, stride, round_out, st);
-}
 
 int maxpool2x2(const float* in, int ld_in, int B, int H, int W, int C, float* out, cudaStream_t st) {
     long total = (long)B * (H / 2) * (W / 2) * (C / 4);
@@ -748,17 +672,6 @@ int conv1x1_sigmoid_nchw(const float* in, int B, int HW, int Cin, const float* w
     return 0;
 }
 
-int gap_linear(const float* feat, int B, int HW, int C, const float* w, const float* bias, int n_out, const uint8_t* codes,
-               float* pooled_scratch, float* out, cudaStream_t st) {
-    SMK_TAG("gap_pool", 4.0 * ((double)B * HW * C + (double)B * C), (double)B * C * HW, st);
-    SMK_LAUNCH(gap_kernel, dim3(dim3(B, cdiv(C, 64))), dim3(256), 0, st, feat, HW, C, pooled_scratch);
-    SMK_CHECK_LAUNCH();
-    SMK_TAG("head_linear", 4.0 * ((double)B * C + (double)n_out * C + (double)B * n_out), 2.0 * (double)B * C * n_out, st);
-    SMK_LAUNCH(head_linear_kernel, dim3(dim3(B, cdiv(n_out, 8))), dim3(256), 0, st, pooled_scratch, C, w, bias, n_out, codes, out);
-    SMK_CHECK_LAUNCH();
-    return 0;
-}
-
 int gap_head(const GapHeadProblem* probs, int n, int B, int HW, int C, cudaStream_t st) {
     SMK_REQUIRE(n == 1 || n == 2, "gap_head: one or two backbones per launch");
     SMK_REQUIRE((size_t)C * 4 <= 48 * 1024, "gap_head: feature width too large for the shared-memory pool");
@@ -782,9 +695,9 @@ int gap_head(const GapHeadProblem* probs, int n, int B, int HW, int C, cudaStrea
 extern "C" int smk_debug_conv_f32(const float* in, int ld_in, int B, int H, int W, int Cin, const float* w_kn, const float* scale,
                                   const float* bias, int N, int K, int mode, int relu, const float* res, int ld_res,
                                   float* out, int ld_out, int shuffle, void* stream) {
-    smk::ConvProblem p{};
+    smk::Conv p{};
     p.in = in; p.ld_in = ld_in; p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.w = w_kn; p.scale = scale; p.bias = bias; p.N = N; p.K = K;
-    p.mode = mode; p.relu = relu; p.res = res; p.ld_res = ld_res; p.out = out; p.ld_out = ld_out; p.shuffle = shuffle;
+    p.mode = mode; p.relu = relu; p.res = res; p.ld_res = ld_res; p.out = out; p.ld_out = ld_out; p.store = shuffle;
     return smk::conv_gemm(p, (cudaStream_t)stream);
 }
 
@@ -793,5 +706,6 @@ extern "C" int smk_debug_stem_ds(const float* img, int B, int H, int W, const fl
                                  const float* pw_b, int stride, int round_out, float* out, void* stream) {
     if (B == 0) return 0;
     SMK_REQUIRE(img && stem_w && stem_s && stem_b && dw_w && dw_s && dw_b && pw_w && pw_s && pw_b && out, "smk_debug_stem_ds: null argument");
-    return smk::stem_ds(img, B, H, W, stem_w, stem_s, stem_b, dw_w, dw_s, dw_b, pw_w, pw_s, pw_b, stride, round_out, out, (cudaStream_t)stream);
+    const smk::StemDsProblem q{stem_w, stem_s, stem_b, dw_w, dw_s, dw_b, pw_w, pw_s, pw_b, out};
+    return smk::stem_ds(img, B, H, W, &q, 1, stride, round_out, (cudaStream_t)stream);
 }

@@ -25,7 +25,7 @@ TAGS = [
     (r"dwconv3x3", "dwconv3x3"), (r"conv_gemm_kernel", "conv_gemm_f32"), (r"raster_tile_kernel", "raster_tile"),
     (r"flame_verts_kernel", "flame_verts"), (r"flame_pose_kernel", "flame_pose"), (r"flame_landmarks_kernel", "flame_landmarks"),
     (r"tri_setup_kernel", "tri_setup"), (r"submesh_kernel", "submesh_normals"), (r"project_kernel", "project"),
-    (r"gap_kernel", "gap_pool"), (r"head_linear_kernel", "head_linear"), (r"reflect_halo_kernel", "reflect_halo"),
+    (r"reflect_halo_kernel", "reflect_halo"),
     (r"maxpool2x2_kernel", "maxpool2x2"), (r"nchw_to_nhwc_pad_kernel", "nchw_to_nhwc"), (r"conv1x1_sigmoid_kernel", "conv1x1_sigmoid"),
 ]
 UNIT = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9, "ns": 1e-3, "us": 1.0, "usecond": 1.0, "nsecond": 1e-3, "ms": 1e3, "msecond": 1e3}
