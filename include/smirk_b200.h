@@ -305,5 +305,7 @@ int smk_debug_stem_ds(const float* img, int B, int H, int W, const float* stem_w
 
 /* The generator's input-gradient entry points. */
 #include "smirk_b200_grad.h"
+/* The encoder's input-gradient entry points. */
+#include "smirk_b200_encoder_grad.h"
 
 #endif /* SMIRK_B200_H */

@@ -122,7 +122,16 @@ GRAD_BINDINGS = [
     ("smk_generator_backward_workspace_bytes", _sz, [_vp, _i]),
     ("smk_generator_backward", _i, [_vp, _i, _vp, _vp, _sz, _vp, _vp, _vp, _sz, STREAM]),
 ]
-_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS + GRAD_BINDINGS if args[-1:] == [STREAM])
+# The same for include/smirk_b200_encoder_grad.h (the encoder's input gradient), included after smirk_b200_grad.h.
+ENCODER_GRAD_BINDINGS = [
+    ("smk_encoder_saved_bytes", _sz, [_vp, _i]),
+    ("smk_encoder_forward_saved", _i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp, _sz, STREAM]),
+    ("smk_encoder_saved_tensor", _i, [_vp, _i, _i, C.POINTER(C.c_char_p), C.POINTER(_sz), C.POINTER(C.c_int)]),
+    ("smk_encoder_backward_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_encoder_backward", _i, [_vp, _i, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, STREAM]),
+]
+_ALL_BINDINGS = BINDINGS + GRAD_BINDINGS + ENCODER_GRAD_BINDINGS
+_TAKES_STREAM = frozenset(name for name, _, args in _ALL_BINDINGS if args[-1:] == [STREAM])
 
 
 def lib():
@@ -134,7 +143,7 @@ def lib():
         raise RuntimeError("smirk_b200: %s not found — build it with `python -m smirk_b200.build` "
                            "(there is no CPU / PyTorch fallback)" % LIB_PATH)
     L = C.CDLL(LIB_PATH)
-    for name, restype, argtypes in BINDINGS + GRAD_BINDINGS:
+    for name, restype, argtypes in _ALL_BINDINGS:
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, [_vp if a is STREAM else a for a in argtypes]
     if L.smk_version() != 100:

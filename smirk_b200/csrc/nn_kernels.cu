@@ -197,7 +197,9 @@ dwconv3x3_px4_kernel(const float* __restrict__ in, int B, int H, int W, int C, i
 // Global average pool + linear head + clamps in ONE launch for one or two backbones (blockIdx.z): every CTA pools its
 // image's feature map into shared memory (the map is L2-resident: 188 KB at 7x7x960) and computes 32 head outputs, one
 // warp per output (smirk_encoder.py:34-45,66-73,95-110).
-struct GapHead { const float* feat[2]; const float* w[2]; const float* bias[2]; const uint8_t* codes[2]; float* out[2]; int n_out[2]; };
+// SAVE: also store the pre-clamp head values (raw) for the backward's clamp masks.
+struct GapHead { const float* feat[2]; const float* w[2]; const float* bias[2]; const uint8_t* codes[2]; float* out[2]; int n_out[2]; float* raw[2]; };
+template <bool SAVE>
 __global__ void __launch_bounds__(256)
 gap_head_kernel(const __grid_constant__ GapHead g, int HW, int C) {
     extern __shared__ float pooled[];                 // [C]
@@ -229,6 +231,7 @@ gap_head_kernel(const __grid_constant__ GapHead g, int HW, int C) {
         for (int s = 16; s > 0; s >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, s);
         if (lane == 0) {
             float v = acc + bias[o];
+            if (SAVE) g.raw[q][(size_t)b * n_out + o] = v;
             const int code = codes ? codes[o] : 0;
             if (code == 1) v = fminf(fmaxf(v, 0.f), 1.f);
             else if (code == 2) v = fmaxf(v, 0.f);
@@ -493,14 +496,17 @@ struct StemDs {                              // one or two backbones share a lau
     int round_out;
 };
 
-template <int STRIDE>
+// SAVE: also store the stem output of the tile's own 16 x 16 pixels (s_out) and the depthwise output (d_out), the ReLU
+// outputs the backward masks with.
+template <int STRIDE, bool SAVE>
 __global__ void __launch_bounds__(256, 3)
 stem_ds_kernel(const float* __restrict__ img, int H, int W, int Hs, int Ws, int pad, const __grid_constant__ StemDs pp) {
-    struct { const float *stem_w, *stem_s, *stem_b, *dw_w, *dw_s, *dw_b, *pw_w, *pw_s, *pw_b; float* out; int round_out; } p;
+    struct { const float *stem_w, *stem_s, *stem_b, *dw_w, *dw_s, *dw_b, *pw_w, *pw_s, *pw_b; float* out; int round_out; float *s_out, *d_out; } p;
     {
         const StemDsProblem& q = pp.q[blockIdx.z];
         p.stem_w = q.stem_w; p.stem_s = q.stem_s; p.stem_b = q.stem_b; p.dw_w = q.dw_w; p.dw_s = q.dw_s; p.dw_b = q.dw_b;
         p.pw_w = q.pw_w; p.pw_s = q.pw_s; p.pw_b = q.pw_b; p.out = q.out; p.round_out = pp.round_out;
+        if (SAVE) { p.s_out = q.s_out; p.d_out = q.d_out; }
     }
     constexpr int PADO = STRIDE == 1 ? 1 : 0;              // depthwise TF-SAME pad_begin on an even-sized map
     constexpr int TO = SD_T / STRIDE;                      // output tile edge
@@ -565,6 +571,13 @@ stem_ds_kernel(const float* __restrict__ img, int H, int W, int Hs, int Ws, int 
             o0.x = v0 ? fmaxf(o0.x, 0.f) : 0.f; o0.y = v0 ? fmaxf(o0.y, 0.f) : 0.f; o0.z = v0 ? fmaxf(o0.z, 0.f) : 0.f; o0.w = v0 ? fmaxf(o0.w, 0.f) : 0.f;
             o1.x = v1 ? fmaxf(o1.x, 0.f) : 0.f; o1.y = v1 ? fmaxf(o1.y, 0.f) : 0.f; o1.z = v1 ? fmaxf(o1.z, 0.f) : 0.f; o1.w = v1 ? fmaxf(o1.w, 0.f) : 0.f;
             s0[q] = o0; s1[q] = o1;
+            if (SAVE) {                                    // the tile's own pixels: stem rows / columns [PADO, PADO + 16) of S
+                const bool own_x = sx >= PADO && sx < PADO + SD_T;
+                if (own_x && syp >= PADO)
+                    reinterpret_cast<float4*>(p.s_out + (((size_t)b * Hs + sy0 + syp) * Ws + sx0 + sx) * 16)[q] = o0;
+                if (own_x && syp + SD_ST / 2 < PADO + SD_T)
+                    reinterpret_cast<float4*>(p.s_out + (((size_t)b * Hs + sy0 + syp + SD_ST / 2) * Ws + sx0 + sx) * 16)[q] = o1;
+            }
         }
     }
     __syncthreads();
@@ -589,6 +602,8 @@ stem_ds_kernel(const float* __restrict__ img, int H, int W, int Hs, int Ws, int 
             float4 o = fma4(acc, sc, bi);
             o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
             *reinterpret_cast<float4*>(sD + px * 16 + 4 * q) = o;
+            if (SAVE)
+                *reinterpret_cast<float4*>(p.d_out + (((size_t)b * (Hs / STRIDE) + ty * TO + oy) * (Ws / STRIDE) + tx * TO + ox) * 16 + 4 * q) = o;
         }
     }
     __syncthreads();
@@ -633,14 +648,22 @@ int stem_ds(const float* img, int B, int H, int W, const StemDsProblem* probs, i
     SMK_REQUIRE(stride == 1 || stride == 2, "stem_ds: stride must be 1 or 2");
     SMK_REQUIRE(H % 2 == 0 && W % 2 == 0 && Hs % SD_T == 0 && Ws % SD_T == 0, "stem_ds: image size %dx%d must be a multiple of 32", H, W);
     SMK_REQUIRE(((uintptr_t)img & 7) == 0, "stem_ds: image pointer must be 8-byte aligned");
+    const bool save = probs[0].s_out != nullptr;
+    SMK_REQUIRE(((probs[0].s_out && probs[0].d_out) || (!probs[0].s_out && !probs[0].d_out)) &&
+                (!probs[n - 1].s_out == !save) && (!probs[n - 1].d_out == !save), "stem_ds: s_out and d_out are given together, for every problem or none");
     StemDs p{};
     p.q[0] = probs[0]; p.q[1] = probs[n - 1]; p.round_out = round_out;
     const double px_o = (double)B * (Hs / stride) * (Ws / stride);
     SMK_TAG("stem_ds_fused", 4.0 * ((double)B * 3 * H * W + n * (px_o * 16 + 27 * 16 + 9 * 16 + 256 + 96)),
             n * 2.0 * ((double)B * Hs * Ws * 16 * 27 + px_o * 16 * (9 + 16)), st);
     dim3 grid((Hs / SD_T) * (Ws / SD_T), B, n);
-    if (stride == 1) SMK_LAUNCH((stem_ds_kernel<1>), grid, dim3(256), 0, st, img, H, W, Hs, Ws, same_pad_begin(H, 2), p);
-    else SMK_LAUNCH((stem_ds_kernel<2>), grid, dim3(256), 0, st, img, H, W, Hs, Ws, same_pad_begin(H, 2), p);
+    if (save) {
+        if (stride == 1) SMK_LAUNCH((stem_ds_kernel<1, true>), grid, dim3(256), 0, st, img, H, W, Hs, Ws, same_pad_begin(H, 2), p);
+        else SMK_LAUNCH((stem_ds_kernel<2, true>), grid, dim3(256), 0, st, img, H, W, Hs, Ws, same_pad_begin(H, 2), p);
+    } else {
+        if (stride == 1) SMK_LAUNCH((stem_ds_kernel<1, false>), grid, dim3(256), 0, st, img, H, W, Hs, Ws, same_pad_begin(H, 2), p);
+        else SMK_LAUNCH((stem_ds_kernel<2, false>), grid, dim3(256), 0, st, img, H, W, Hs, Ws, same_pad_begin(H, 2), p);
+    }
     SMK_CHECK_LAUNCH();
     return 0;
 }
@@ -677,15 +700,18 @@ int gap_head(const GapHeadProblem* probs, int n, int B, int HW, int C, cudaStrea
     SMK_REQUIRE((size_t)C * 4 <= 48 * 1024, "gap_head: feature width too large for the shared-memory pool");
     GapHead g{};
     int max_out = 0;
+    const bool save = probs[0].raw != nullptr;
+    SMK_REQUIRE(!probs[n - 1].raw == !save, "gap_head: raw is given for every problem or none");
     for (int k = 0; k < 2; ++k) {
         const GapHeadProblem& q = probs[k < n ? k : n - 1];
-        g.feat[k] = q.feat; g.w[k] = q.w; g.bias[k] = q.bias; g.codes[k] = q.codes; g.out[k] = q.out; g.n_out[k] = q.n_out;
+        g.feat[k] = q.feat; g.w[k] = q.w; g.bias[k] = q.bias; g.codes[k] = q.codes; g.out[k] = q.out; g.n_out[k] = q.n_out; g.raw[k] = q.raw;
         max_out = std::max(max_out, q.n_out);
     }
     double by = 0, fl = 0;
     for (int k = 0; k < n; ++k) { by += 4.0 * ((double)B * HW * C + (double)probs[k].n_out * C + (double)B * probs[k].n_out); fl += (double)B * C * HW + 2.0 * B * C * probs[k].n_out; }
     SMK_TAG("gap_head", by, fl, st);
-    SMK_LAUNCH(gap_head_kernel, dim3(B, cdiv(max_out, 32), n), dim3(256), (size_t)C * 4, st, g, HW, C);
+    if (save) SMK_LAUNCH(gap_head_kernel<true>, dim3(B, cdiv(max_out, 32), n), dim3(256), (size_t)C * 4, st, g, HW, C);
+    else SMK_LAUNCH(gap_head_kernel<false>, dim3(B, cdiv(max_out, 32), n), dim3(256), (size_t)C * 4, st, g, HW, C);
     SMK_CHECK_LAUNCH();
     return 0;
 }

@@ -24,6 +24,7 @@ struct StemDsProblem {
     const float* dw_w; const float* dw_s; const float* dw_b;            // [9][16]
     const float* pw_w; const float* pw_s; const float* pw_b;            // [16 ci][16 co]
     float* out;
+    float* s_out; float* d_out;          // optional, together: also store the stem output [B,112,112,16] and the depthwise output
 };
 // n = 1 or 2 backbones of the same block-0 stride in one launch (they read the same image).
 int stem_ds(const float* img_nchw, int B, int H, int W, const StemDsProblem* probs, int n, int stride, int round_out, cudaStream_t st);
@@ -35,8 +36,9 @@ int conv1x1_sigmoid_nchw(const float* in, int B, int HW, int Cin, const float* w
                          int Cout, float* out, cudaStream_t st);
 // Global average pool over HW pixels + Linear(C -> n_out) + clamp codes per output column (0 none, 1 clamp[0,1], 2 relu,
 // 3 clamp[-0.2,0.2]) in one launch, for one or two backbones with the same feature shape [B, HW, C] (different head widths
-// allowed).  w is [n_out][C]; codes (device) may be null.
-struct GapHeadProblem { const float* feat; const float* w; const float* bias; const uint8_t* codes; float* out; int n_out; };
+// allowed).  w is [n_out][C]; codes (device) may be null.  raw (optional, for every problem or none): also store the
+// pre-clamp values [B, n_out].
+struct GapHeadProblem { const float* feat; const float* w; const float* bias; const uint8_t* codes; float* out; int n_out; float* raw; };
 int gap_head(const GapHeadProblem* probs, int n, int B, int HW, int C, cudaStream_t st);
 
 }  // namespace smk

@@ -91,14 +91,16 @@ struct XdwArgs {
     const float* scale2[2]; const float* bias2[2];  // folded BN of the depthwise conv   [mid]
     float* out[2];                                  // d: [B, Ho, Wo, mid]
     int round_out;
+    float* e_out[2];                                // SAVE: e [B, H, W, mid] (per problem)
 };
 
 // X3 != 0: error-compensated 3xTF32 expand GEMM (fp32-equivalent e): x = x_hi + x_lo, w1 = w_hi + w_lo (split on the host, wlo),
 // e = x_hi*w_hi + x_lo*w_hi + x_hi*w_lo accumulated in the same registers.  The workers split their own A fragments of x in
 // registers and use the register-A form of wgmma, so shared memory only grows by the weight tails.
 // NKB: 32-channel k-blocks of Cin (window size), KSL: wgmma k-steps of 8 channels in the last one (Cin = 32 (NKB - 1) + 8 KSL,
-// rounded up to a multiple of 8).
-template <int STRIDE, int X3, int NKB, int KSL>
+// rounded up to a multiple of 8).  SAVE: phase (a) also stores e for the pixels the item owns (rows / columns
+// [o0 * STRIDE, (o0 + TO) * STRIDE) of e: every pixel of e belongs to one tile) — the backward's ReLU mask.
+template <int STRIDE, int X3, int NKB, int KSL, bool SAVE>
 __global__ void __launch_bounds__(NUM_THREADS, XdwSmem<NKB, X3>::MINB)
 xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
     using L = XdwSmem<NKB, X3>;
@@ -309,6 +311,12 @@ xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
                 const int ey = ey0 + half * 8 + (r >> 4), ex = ex0 + (r & 15);
                 const bool inside = ey >= 0 && ey < a.H && ex >= 0 && ex < a.W;
                 float* erow = E + (size_t)(half * 128 + r) * E_PITCH;
+                bool own = false;
+                float* esave = nullptr;
+                if constexpr (SAVE) {
+                    own = inside && ey >= oh0 * STRIDE && ey < (oh0 + TO) * STRIDE && ex >= ow0 * STRIDE && ex < (ow0 + TO) * STRIDE;
+                    esave = a.e_out[w.prob] + (((size_t)img * a.H + ey) * a.W + ex) * a.mid + ch0;
+                }
 #pragma unroll
                 for (int j = 0; j < NC / 8; ++j) {
                     const int ch = 8 * j + 2 * (lane & 3);
@@ -320,6 +328,7 @@ xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
                         o.y = fmaxf(fmaf(acc[mb][4 * j + 2 * hr + 1], sc.y, bi.y), 0.f);
                     }
                     *reinterpret_cast<float2*>(erow + ch) = o;
+                    if (SAVE && own && ch0 + ch < a.mid) *reinterpret_cast<float2*>(esave + ch) = o;
                 }
             }
         if (c_next >= 0) park_par(buf ^ 1, pf);        // slot buf^1 was last read in the previous chunk's phase (b)
@@ -386,22 +395,27 @@ xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
     }
 }
 
-template <int STRIDE, int X3, int NKB, int KSL>
+template <int STRIDE, int X3, int NKB, int KSL, bool SAVE>
 int launch(const XdwMaps& mp, const XdwArgs& a, int grid, cudaStream_t st) {
     constexpr size_t smem = XdwSmem<NKB, X3>::SMEM;
-    SMK_CHECK_CUDA((set_max_dynamic_smem<xdw_kernel<STRIDE, X3, NKB, KSL>>((int)smem)));
-    SMK_LAUNCH((xdw_kernel<STRIDE, X3, NKB, KSL>), dim3(grid), dim3(NUM_THREADS), smem, st, mp, a);
+    SMK_CHECK_CUDA((set_max_dynamic_smem<xdw_kernel<STRIDE, X3, NKB, KSL, SAVE>>((int)smem)));
+    SMK_LAUNCH((xdw_kernel<STRIDE, X3, NKB, KSL, SAVE>), dim3(grid), dim3(NUM_THREADS), smem, st, mp, a);
     SMK_CHECK_LAUNCH();
     return 0;
+}
+
+template <int STRIDE, int X3, int NKB, int KSL>
+int launch_save(const XdwMaps& mp, const XdwArgs& a, int grid, cudaStream_t st) {
+    return a.e_out[0] ? launch<STRIDE, X3, NKB, KSL, true>(mp, a, grid, st) : launch<STRIDE, X3, NKB, KSL, false>(mp, a, grid, st);
 }
 
 template <int STRIDE, int X3, int NKB>
 int launch_ksl(int ksl, const XdwMaps& mp, const XdwArgs& a, int grid, cudaStream_t st) {
     switch (ksl) {
-        case 1: return launch<STRIDE, X3, NKB, 1>(mp, a, grid, st);
-        case 2: return launch<STRIDE, X3, NKB, 2>(mp, a, grid, st);
-        case 3: return launch<STRIDE, X3, NKB, 3>(mp, a, grid, st);
-        default: return launch<STRIDE, X3, NKB, 4>(mp, a, grid, st);
+        case 1: return launch_save<STRIDE, X3, NKB, 1>(mp, a, grid, st);
+        case 2: return launch_save<STRIDE, X3, NKB, 2>(mp, a, grid, st);
+        case 3: return launch_save<STRIDE, X3, NKB, 3>(mp, a, grid, st);
+        default: return launch_save<STRIDE, X3, NKB, 4>(mp, a, grid, st);
     }
 }
 
@@ -428,7 +442,8 @@ int xdw_conv(const XdwConv& p, cudaStream_t st, const XdwConv* p2) {
     SMK_REQUIRE(p.Cin > 0 && p.Cin <= MAX_NKB * BK, "xdw_conv: Cin must be at most 160 (the whole input window stays in shared memory)");
     SMK_REQUIRE(p.stride == 1 || (p.H % 2 == 0 && p.W % 2 == 0), "xdw_conv: stride 2 expects even input sizes (TF-SAME pad_begin 0)");
     SMK_REQUIRE(!p2 || (p2->B == p.B && p2->H == p.H && p2->W == p.W && p2->Cin == p.Cin && p2->mid == p.mid && p2->stride == p.stride &&
-                        p2->round_out == p.round_out && !p2->w1t_lo == !p.w1t_lo), "xdw_conv: paired problems must have identical shapes");
+                        p2->round_out == p.round_out && !p2->w1t_lo == !p.w1t_lo && !p2->e_out == !p.e_out),
+                "xdw_conv: paired problems must have identical shapes");
     const int Ho = (p.H + p.stride - 1) / p.stride, Wo = (p.W + p.stride - 1) / p.stride;
     const int TO = p.stride == 1 ? 14 : 7;
     XdwMaps mp;
@@ -440,10 +455,12 @@ int xdw_conv(const XdwConv& p, cudaStream_t st, const XdwConv* p2) {
         mp.wlo[g] = mp.w[g];
         if (q.w1t_lo) { if (int rc = encode_2d(&mp.wlo[g], q.w1t_lo, (uint64_t)q.mid, (uint64_t)q.Cin, (uint64_t)q.Cin, NC, "xdw_conv(w1 tails)")) return rc; }
         a.scale1[g] = q.scale1; a.bias1[g] = q.bias1; a.wdw[g] = q.wdw; a.scale2[g] = q.scale2; a.bias2[g] = q.bias2; a.out[g] = q.out;
+        a.e_out[g] = q.e_out;
     }
     if (nprob == 1) {
         mp.x[1] = mp.x[0]; mp.w[1] = mp.w[0]; mp.wlo[1] = mp.wlo[0];
         a.scale1[1] = a.scale1[0]; a.bias1[1] = a.bias1[0]; a.wdw[1] = a.wdw[0]; a.scale2[1] = a.scale2[0]; a.bias2[1] = a.bias2[0]; a.out[1] = a.out[0];
+        a.e_out[1] = a.e_out[0];
     }
     // Resident CTAs to aim for: one per SM (two fit for plain TF32 with Cin <= 64) leaves room on every SM for the other backbones' and batches'
     // kernels of the concurrent pipeline.

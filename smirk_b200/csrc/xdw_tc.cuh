@@ -16,6 +16,7 @@ struct XdwConv {
     int stride;                           // 1 or 2, TF-"SAME" padding
     int round_out;                        // round d to TF32 (it feeds the projection GEMM)
     float* out;                           // d: [B,Ho,Wo,mid]
+    float* e_out;                         // optional: also store e [B,H,W,mid] (the backward's ReLU mask)
 };
 
 // p2 (optional): a second problem of identical shape sharing the launch.

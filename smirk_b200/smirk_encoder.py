@@ -1,9 +1,14 @@
-"""``SmirkEncoder`` — drop-in for the reference ``src/smirk_encoder.py`` (forward only).
+"""``SmirkEncoder`` — drop-in for the reference ``src/smirk_encoder.py`` (eval BN).
 
 Same class names, constructor arguments, sub-module / parameter names (``state_dict`` keys follow the
 timm ``features_only`` MobileNetV3 layout the reference checkpoints use) and output dicts.  The
 ``nn.Conv2d`` / ``nn.BatchNorm2d`` objects below are parameter containers only — they are never
 called; the forward pass runs in ``csrc/encoder.cu`` through ``smk_encoder_forward``.
+
+With grad mode on and an image that requires grad, a frozen (``requires_grad_(False)``) encoder whose BatchNorms are in
+eval mode passes the gradient to its input, as the reference trainer's cycle loss (its encoder frozen by
+``utils.freeze_module``) and analysis-by-synthesis fitting need: the forward then keeps its activations
+(``smk_encoder_forward_saved``) and the backward runs ``smk_encoder_backward``.  Weight gradients are not implemented.
 """
 import ctypes as C
 
@@ -147,24 +152,104 @@ class _NativeEncoder(_lib.NativeModule, nn.Module):
         d.n_shape, d.n_exp, d.precision = self.n_shape, self.n_exp, int(self.precision)
         return _lib.create("encoder", d, device)
 
-    @torch.no_grad()
+    def _check(self, img):
+        """Device, shape and mode checks of every call.  The mode is that of the BatchNorms the call runs, as in the
+        reference (whose parent module owns none): a parent in train mode over frozen, eval-mode sub-encoders runs."""
+        _lib.require_cuda(img, "img")
+        for part in self._parts():            # checked on every call: .train() after the first forward must not silently run eval BN
+            if part is not None and any(m.training for m in part[0].encoder.modules() if isinstance(m, nn.BatchNorm2d)):
+                raise RuntimeError("smirk_b200.%s: train-mode BatchNorm is not implemented (forward/eval only)" % type(self).__name__)
+        if img.dim() != 4 or tuple(img.shape[1:]) != (3, 224, 224):
+            raise RuntimeError("smirk_b200.%s: expected img [B,3,224,224], got %s" % (type(self).__name__, tuple(img.shape)))
+
+    def _outputs(self, B, dev):
+        widths = (6, self.n_shape, self.n_exp + 5)
+        return [torch.empty(B, w, dtype=torch.float32, device=dev) if part is not None else None
+                for w, part in zip(widths, self._parts())]
+
     def _run(self, img):
         """img [B,3,224,224] -> (pose_cam [B,6] | None, shape [B,n_shape] | None, expr [B,n_exp+5] | None)."""
-        _lib.require_cuda(img, "img")
-        if self.training:                      # checked on every call: .train() after the first forward must not silently run eval BN
-            raise RuntimeError("smirk_b200.%s: train-mode BatchNorm is not implemented (forward/eval only)" % type(self).__name__)
+        self._check(img)
+        if torch.is_grad_enabled() and img.requires_grad:
+            parts = [p for p in self._parts() if p is not None]
+            if any(t.requires_grad for enc, head in parts for t in list(enc.encoder.parameters()) + list(head.parameters())):
+                raise RuntimeError("smirk_b200.%s: weight gradients are not implemented; to pass a gradient to the input, "
+                                   "freeze the encoder with .requires_grad_(False)" % type(self).__name__)
+            raw = _EncoderFunction.apply(img, self)
+            it = iter(raw)
+            return [next(it) if p is not None else None for p in self._parts()]
+        with torch.no_grad():
+            dev = img.device
+            h = self._native_handle(dev)
+            x = _lib.dev_f32(img, "img")
+            B = x.shape[0]
+            outs = self._outputs(B, dev)
+            ws = self._native_workspace("forward", _lib.call("smk_encoder_workspace_bytes", dev, h, B), dev)
+            _lib.call("smk_encoder_forward", dev, h, x, B, *outs, ws, ws.numel())
+            return outs
+
+    def _forward_saved(self, img):
+        """-> (handle, [raw outputs | None], saved): the grad-mode forward, its activations in a buffer of their own."""
         dev = img.device
         h = self._native_handle(dev)
         x = _lib.dev_f32(img, "img")
-        if x.dim() != 4 or tuple(x.shape[1:]) != (3, 224, 224):
-            raise RuntimeError("smirk_b200.%s: expected img [B,3,224,224], got %s" % (type(self).__name__, tuple(x.shape)))
         B = x.shape[0]
-        widths = (6, self.n_shape, self.n_exp + 5)
-        outs = [torch.empty(B, w, dtype=torch.float32, device=dev) if part is not None else None
-                for w, part in zip(widths, self._parts())]
+        outs = self._outputs(B, dev)
+        nbytes = _lib.call("smk_encoder_saved_bytes", dev, h, B)
+        saved = torch.empty(max(nbytes // 4, 1), dtype=torch.float32, device=dev)
         ws = self._native_workspace("forward", _lib.call("smk_encoder_workspace_bytes", dev, h, B), dev)
-        _lib.call("smk_encoder_forward", dev, h, x, B, *outs, ws, ws.numel())
-        return outs
+        _lib.call("smk_encoder_forward_saved", dev, h, x, B, *outs, saved, nbytes, ws, ws.numel())
+        return h, outs, saved
+
+    @torch.no_grad()
+    def saved_activations(self, img):
+        """The tensors the backward of ``self(img)`` uses, {name: tensor}, names being the reference's module paths: the
+        output of every ReLU as a [B,C,H,W] view of the NHWC buffer (``shape_encoder.encoder.bn1`` for the stem,
+        ``….blocks.<stage>.<i>.bn1`` / ``.bn2`` ...) and each head's pre-clamp output [B,n_out]
+        (``expression_encoder.expression_layers.0`` ...).  The forward is deterministic and batch-independent, so these
+        are the tensors an autograd context of the same input holds."""
+        self._check(img)
+        h, _, saved = self._forward_saved(img)
+        B, out, i = img.shape[0], {}, 0
+        name, off, dims = C.c_char_p(), C.c_size_t(), (C.c_int * 4)()
+        while True:
+            try:
+                _lib.call("smk_encoder_saved_tensor", img.device, h, B, i, C.byref(name), C.byref(off), dims)
+            except RuntimeError:
+                break
+            b, hh, ww, c = dims
+            t = saved[off.value:off.value + b * hh * ww * c].view(b, hh, ww, c)
+            out[name.value.decode()] = t.view(b, c) if hh == ww == 1 else t.permute(0, 3, 1, 2)
+            i += 1
+        return out
+
+
+class _EncoderFunction(torch.autograd.Function):
+    """Frozen encoder: the raw outputs (pose_cam, shape, expr: those the module holds) of img, and the gradient with
+    respect to img only.  An output that receives no gradient arrives as None and its backbone's backward launches
+    nothing.  The activations are saved per call, so several forwards may share one backward."""
+
+    @staticmethod
+    def forward(ctx, img, module):
+        h, outs, saved = module._forward_saved(img)
+        ctx.set_materialize_grads(False)
+        ctx.handle, ctx.module, ctx.dtype, ctx.B = h, module, img.dtype, img.shape[0]
+        ctx.present = [o is not None for o in outs]
+        ctx.save_for_backward(saved)
+        return tuple(o for o in outs if o is not None)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, *grads):
+        saved, = ctx.saved_tensors
+        m, dev, B = ctx.module, saved.device, ctx.B
+        it = iter(grads)
+        g = [next(it) if p else None for p in ctx.present]
+        g = [None if t is None else _lib.dev_f32(t, "grad") for t in g]
+        g_img = torch.empty(B, 3, 224, 224, dtype=torch.float32, device=dev)
+        ws = m._native_workspace("backward", _lib.call("smk_encoder_backward_workspace_bytes", dev, ctx.handle, B), dev)
+        _lib.call("smk_encoder_backward", dev, ctx.handle, B, saved, saved.numel() * 4, *g, g_img, ws, ws.numel())
+        return g_img.to(ctx.dtype), None
 
 
 class PoseEncoder(_NativeEncoder):
