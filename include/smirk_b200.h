@@ -307,5 +307,7 @@ int smk_debug_stem_ds(const float* img, int B, int H, int W, const float* stem_w
 #include "smirk_b200_grad.h"
 /* The encoder's input-gradient entry points. */
 #include "smirk_b200_encoder_grad.h"
+/* The video demo's output grid. */
+#include "smirk_b200_video.h"
 
 #endif /* SMIRK_B200_H */

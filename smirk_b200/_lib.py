@@ -130,7 +130,13 @@ ENCODER_GRAD_BINDINGS = [
     ("smk_encoder_backward_workspace_bytes", _sz, [_vp, _i]),
     ("smk_encoder_backward", _i, [_vp, _i, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, STREAM]),
 ]
-_ALL_BINDINGS = BINDINGS + GRAD_BINDINGS + ENCODER_GRAD_BINDINGS
+# The same for include/smirk_b200_video.h (the video demo's output grid), included after smirk_b200_encoder_grad.h.
+VIDEO_BINDINGS = [
+    ("smk_hull_mask", _i, [_vp, _i, _i, _i, _vp, STREAM]),
+    ("smk_video_workspace_bytes", _sz, [_i, _i]),
+    ("smk_video_compose", _i, [_vp, _i, _i, _i, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _sz, STREAM]),
+]
+_ALL_BINDINGS = BINDINGS + GRAD_BINDINGS + ENCODER_GRAD_BINDINGS + VIDEO_BINDINGS
 _TAKES_STREAM = frozenset(name for name, _, args in _ALL_BINDINGS if args[-1:] == [STREAM])
 
 

@@ -21,6 +21,7 @@
 // integer shifts, scipy cross-check away from the border): "parity unpinned" for the border/clip rules.
 // HBM traffic: the gather touches each source texel it needs once through L2; output 150 KB (crop) or H*W*3 (back).
 #include "common.cuh"
+#include "warp_sample.cuh"
 #include <math.h>
 #include <algorithm>
 
@@ -65,10 +66,7 @@ f32chw_to_u8hwc_kernel(const float* __restrict__ in, int B, int S, uint8_t* __re
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
         const size_t b = i / ((size_t)S * S), p = i - b * (size_t)S * S;
 #pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            const float v = __fmul_rn(in[(b * 3 + c) * (size_t)S * S + p], 255.0f);
-            out[i * 3 + c] = (uint8_t)(int)v;                      // C cast: truncation, values are in [0, 255]
-        }
+        for (int c = 0; c < 3; ++c) out[i * 3 + c] = smk::unit_to_u8(in[(b * 3 + c) * (size_t)S * S + p]);
     }
 }
 
@@ -82,31 +80,10 @@ warp_bilinear_kernel(const uint8_t* __restrict__ src, int Hs, int Ws, const doub
     const int b = blockIdx.z;
     const int tfc = blockIdx.x * 32 + (threadIdx.x & 31), tfr = blockIdx.y * 8 + (threadIdx.x >> 5);
     if (tfc >= Wd || tfr >= Hd) return;
-    const double* m = M + (size_t)b * 9;
-    // _transform_affine: c = M00 x + M01 y + M02 (left to right, no contraction)
-    const double c = __dadd_rn(__dadd_rn(__dmul_rn(m[0], (double)tfc), __dmul_rn(m[1], (double)tfr)), m[2]);
-    const double r = __dadd_rn(__dadd_rn(__dmul_rn(m[3], (double)tfc), __dmul_rn(m[4], (double)tfr)), m[5]);
-    const double fr = floor(r), fc = floor(c);
-    const long long minr = (long long)fr, minc = (long long)fc, maxr = (long long)ceil(r), maxc = (long long)ceil(c);
-    const double dr = __dsub_rn(r, (double)minr), dc = __dsub_rn(c, (double)minc);
     const uint8_t* s = src + (size_t)b * Hs * Ws * 3;
-    const bool r0 = minr >= 0 && minr < Hs, r1 = maxr >= 0 && maxr < Hs, c0 = minc >= 0 && minc < Ws, c1 = maxc >= 0 && maxc < Ws;
-    const double lo = (double)mm[b].mn, hi = (double)mm[b].mx;
-    const bool keep_cval = !(lo <= 0.0 && 0.0 <= hi);              // cval = 0 outside the source's range: exact zeros survive the clip
     uint8_t res[3];
-#pragma unroll
-    for (int ch = 0; ch < 3; ++ch) {
-        const double tl = (r0 && c0) ? (double)s[((size_t)minr * Ws + minc) * 3 + ch] : 0.0;
-        const double tr = (r0 && c1) ? (double)s[((size_t)minr * Ws + maxc) * 3 + ch] : 0.0;
-        const double bl = (r1 && c0) ? (double)s[((size_t)maxr * Ws + minc) * 3 + ch] : 0.0;
-        const double br = (r1 && c1) ? (double)s[((size_t)maxr * Ws + maxc) * 3 + ch] : 0.0;
-        const double omc = __dsub_rn(1.0, dc), omr = __dsub_rn(1.0, dr);
-        const double top = __dadd_rn(__dmul_rn(omc, tl), __dmul_rn(dc, tr));
-        const double bot = __dadd_rn(__dmul_rn(omc, bl), __dmul_rn(dc, br));
-        double v = __dadd_rn(__dmul_rn(omr, top), __dmul_rn(dr, bot));
-        if (!(keep_cval && v == 0.0)) v = fmin(fmax(v, lo), hi);
-        res[ch] = (uint8_t)(int)v;
-    }
+    smk::skimage_bilinear3(M + (size_t)b * 9, tfc, tfr, Hs, Ws, (double)mm[b].mn, (double)mm[b].mx,
+                           [s, Ws](int ch, int row, int col) { return (double)s[((size_t)row * Ws + col) * 3 + ch]; }, res);
     if (OUT_F32) {
         float* o = reinterpret_cast<float*>(dst) + (size_t)b * 3 * Hd * Wd + (size_t)tfr * Wd + tfc;
 #pragma unroll

@@ -15,6 +15,9 @@ This is the public entry point ``bench.py`` and the demos use for batched work:
                               the copies of one batch overlap the kernels of the other;
 * ``shard_bounds`` / ``all_gather_frames``  frame-shard data parallelism (one process per GPU, contiguous
                               split of the batch; a single NCCL all-gather of the final outputs — SURVEY.md §8e);
+* ``video=VideoStage(...)``  uint8 frames in, the video demo's output grid out (``smirk_b200.video``): the batch's
+                              crop, the hot path and the grid in one call / one graph; the auxiliary input is the
+                              ``VideoBatch`` of ``VideoStage.prepare``;
 * ``enable_gather(keys)``     puts that all-gather INTO the pipeline: after every batch the lane's outputs are gathered
                               over all ranks on a communication stream (NCCL over NVLink / NVSwitch), overlapping the
                               kernels of the next batches on the other lanes.
@@ -61,7 +64,7 @@ class _Lane:
     """One pipeline lane: a set of modules, a compute stream, a copy stream, per-batch-size graphs."""
 
     def __init__(self, modules, device, own_stream):
-        self.encoder, self.flame, self.renderer, self.generator, self.masking = modules
+        self.encoder, self.flame, self.renderer, self.generator, self.masking, self.video = modules
         self.stream = torch.cuda.Stream(device=device) if own_stream else None
         self.graphs = {}
         self.host = {}
@@ -73,7 +76,7 @@ class _Lane:
         self.gather_out = {}
 
     def modules(self):
-        return [m for m in (self.encoder, self.flame, self.renderer, self.generator, self.masking) if m is not None]
+        return [m for m in (self.encoder, self.flame, self.renderer, self.generator, self.masking, self.video) if m is not None]
 
 
 class _PeerBuffer:
@@ -121,36 +124,69 @@ class _PeerBuffer:
 class SmirkPipeline:
     OUT_KEYS = ("rendered_img", "vertices", "transformed_vertices", "landmarks_fan", "landmarks_mp", "params")
 
-    def __init__(self, encoder, flame, renderer, generator=None, device="cuda:0", slots=2, masking=None):
+    def __init__(self, encoder, flame, renderer, generator=None, device="cuda:0", slots=2, masking=None, video=None):
         """``masking``: a ``smirk_b200.masking.MaskingStage``.  With it the full cycle computes the generator's second
         input itself (demo.py:138-165) and the auxiliary input of forward/replay/submit/run_host is the landmark hull mask
-        [B,1,224,224]; without it the auxiliary input is a ready-made ``masked_img`` [B,3,224,224]."""
+        [B,1,224,224]; without it the auxiliary input is a ready-made ``masked_img`` [B,3,224,224].
+        ``video``: a ``smirk_b200.video.VideoStage``.  With it the first input of forward/replay/submit/run_host is a
+        batch of uint8 BGR frames [B,H,W,3], the auxiliary input the ``VideoBatch`` of ``video.prepare``, and the outputs
+        gain ``cropped_img`` and ``grid`` (and, with a generator, ``hull_mask``; the generator then needs ``masking``)."""
+        if video is not None and generator is not None and masking is None:
+            raise ValueError("SmirkPipeline: the video stage's generator panel needs masking=MaskingStage(...) "
+                             "(the hull mask goes through the masking step, demo_video.py:177-197)")
         self.device = torch.device(device)
         self.encoder, self.flame, self.renderer, self.generator, self.masking = encoder, flame, renderer, generator, masking
+        self.video = video
         self.slots = max(1, int(slots))
-        self._lanes = [_Lane((encoder, flame, renderer, generator, masking), self.device, own_stream=False)]
+        self._lanes = [_Lane(self._modules(), self.device, own_stream=False)]
         self._h2d = self._d2h = None
         self._gather_keys, self._gather_group, self._comm, self._gather_backend, self._p2p = (), None, None, None, None
+
+    def _modules(self):
+        return (self.encoder, self.flame, self.renderer, self.generator, self.masking, self.video)
 
     def refresh(self):
         """Drop every captured graph (and the weights / workspaces they kept alive) and the lane replicas, so the next
         call re-captures from the current state of the caller's modules."""
         torch.cuda.synchronize(self.device)
-        self._lanes = [_Lane((self.encoder, self.flame, self.renderer, self.generator, self.masking), self.device, own_stream=False)]
+        self._lanes = [_Lane(self._modules(), self.device, own_stream=False)]
 
     def _lane(self, i):
         """Lane 0 runs the caller's modules on the caller's stream; lanes >= 1 are replicas (deep copies:
         same parameter values, separate native handles / workspaces) on their own streams."""
         while len(self._lanes) <= i:
-            mods = tuple(copy.deepcopy(m) if m is not None else None
-                         for m in (self.encoder, self.flame, self.renderer, self.generator, self.masking))
+            mods = tuple(copy.deepcopy(m) if m is not None else None for m in self._modules())
             self._lanes.append(_Lane(mods, self.device, own_stream=True))
         return self._lanes[i]
 
     # ---- plain forward (device in, device out) -----------------------------------------------------
     @torch.no_grad()
     def forward(self, img, masked_img=None, lane=0):
+        if self.video is not None:                  # img = uint8 frames, masked_img = the VideoBatch
+            self.video.check(img, masked_img)
+            aux = [masked_img[k].to(img.device, non_blocking=True) for k in self._video_keys()]
+            return self._forward_video(img, aux, lane)
+        return self._forward(self._lane(lane), img, masked_img)
+
+    def _forward_video(self, frames, aux, lane):
+        """Crop, the hot path, the output grid (smirk_b200/video.py); aux = the device tensors of ``_video_keys()``: crop /
+        back matrices [B,9] (+ the int32 crop landmarks [B,L,2] with a generator)."""
         L = self._lane(lane)
+        img = L.video.crop(frames, aux[0])
+        hull = L.video.hull_mask(aux[2]) if L.generator is not None else None
+        out = self._forward(L, img, hull)
+        out["cropped_img"] = img
+        panels = [out["rendered_img"]]
+        if hull is not None:
+            out["hull_mask"] = hull
+            panels.append(out["reconstructed_img"])
+        out["grid"] = L.video.compose(frames, img, panels, aux[1])
+        return out
+
+    def _video_keys(self):
+        return ("crop_m", "back_m", "kpt") if self.generator is not None else ("crop_m", "back_m")
+
+    def _forward(self, L, img, masked_img):
         p = L.encoder(img)
         fo = L.flame.forward(p)
         ro = L.renderer.forward(fo["vertices"], p["cam"], landmarks_fan=fo["landmarks_fan"],
@@ -179,35 +215,49 @@ class SmirkPipeline:
         if B in L.graphs:
             return L.graphs[B]
         dev = self.device
-        static_in = torch.zeros(B, 3, 224, 224, device=dev)
-        static_mask = torch.zeros(B, 1 if self.masking is not None else 3, 224, 224, device=dev) if self.generator is not None else None
+        static_aux = []
+        static_mask = None                                  # the video stage draws its hull mask inside the graph
+        if self.generator is not None and self.video is None:
+            static_mask = torch.zeros(B, 1 if self.masking is not None else 3, 224, 224, device=dev)
+        if self.video is not None:                          # frames + the two [B,9] matrices of the VideoBatch
+            static_in = torch.zeros((B,) + self.video.frame_hw + (3,), dtype=torch.uint8, device=dev)
+            static_aux = [torch.zeros(B, 9, dtype=torch.float64, device=dev) for _ in range(2)]
+            if self.generator is not None:
+                static_aux.append(torch.zeros(B, self.video.L, 2, dtype=torch.int32, device=dev))
+            run = lambda: self._forward_video(static_in, static_aux, lane)
+        else:
+            static_in = torch.zeros(B, 3, 224, 224, device=dev)
+            run = lambda: self.forward(static_in, static_mask, lane)
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):                       # warm-up: builds handles, sizes workspaces
             for _ in range(2):
-                self.forward(static_in, static_mask, lane)
+                run()
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
         g = torch.cuda.CUDAGraph()
         n0 = _lib.call("smk_launch_count", dev)
         with torch.cuda.graph(g):
-            static_out = self.forward(static_in, static_mask, lane)
+            static_out = run()
         launches = _lib.call("smk_launch_count", dev) - n0
         # The graph holds raw pointers into each module's packed weights (native handle) and workspace: keep both
         # alive for as long as the graph exists, whatever the modules do afterwards (re-pack, grow their workspace
         # for a larger batch, ...).  A workspace that grows allocates a NEW buffer, so graphs of different batch
         # sizes on one lane never alias a freed one.
         keep = [m.graph_keep_alive() for m in L.modules()]
-        rec = dict(graph=g, img=static_in, mask=static_mask, out=static_out, launches=int(launches), keep=keep)
+        rec = dict(graph=g, img=static_in, mask=static_mask, aux=static_aux, out=static_out, launches=int(launches), keep=keep)
         L.graphs[B] = rec
         return rec
 
     def replay(self, img, masked_img=None):
         """Lane 0, caller's stream: copy the inputs into the graph's static buffers and replay."""
+        if self.video is not None:
+            self.video.check(img, masked_img)
         rec = self.capture(img.shape[0])
         rec["img"].copy_(img, non_blocking=True)
         if rec["mask"] is not None:
             rec["mask"].copy_(masked_img, non_blocking=True)
+        self._copy_aux(rec["aux"], self._upload_aux(masked_img, torch.cuda.current_stream(self.device)))
         rec["graph"].replay()
         return rec["out"]
 
@@ -217,6 +267,8 @@ class SmirkPipeline:
         must already be valid on the caller's current stream.  Outputs live in the lane's static buffers
         until that lane is used again; call ``join()`` before reading them from the caller's stream."""
         lane = i % self.slots
+        if self.video is not None:
+            self.video.check(img, masked_img)
         rec = self.capture(img.shape[0], lane)
         L = self._lanes[lane]
         cur = torch.cuda.current_stream(self.device)
@@ -228,16 +280,42 @@ class SmirkPipeline:
             self._gather(L, rec)
             return rec["out"]
         L.stream.wait_stream(cur)                           # inputs ready
+        aux = self._upload_aux(masked_img, L.stream)
         with torch.cuda.stream(L.stream):
             if self._gather_keys:
                 L.stream.wait_event(L.gathered)             # the previous all-gather of this lane has read the outputs
             rec["img"].copy_(img, non_blocking=True)
             if rec["mask"] is not None:
                 rec["mask"].copy_(masked_img, non_blocking=True)
+            self._copy_aux(rec["aux"], aux)
             rec["graph"].replay()
             L.computed.record(L.stream)
         self._gather(L, rec)
         return rec["out"]
+
+    def _upload_aux(self, batch, consumer):
+        """The video stage's graph inputs besides the frames (``_video_keys()`` of a VideoBatch), on the device and valid on
+        ``consumer``: host tensors are uploaded on the H2D stream, device tensors are used as they are.  None without the
+        video stage."""
+        if self.video is None:
+            return None
+        src = [batch[k] for k in self._video_keys()]
+        if all(t.is_cuda for t in src):
+            return src
+        if self._h2d is None:
+            self._h2d, self._d2h = torch.cuda.Stream(device=self.device), torch.cuda.Stream(device=self.device)
+        with torch.cuda.stream(self._h2d):
+            dev = [t.to(self.device, non_blocking=True) for t in src]
+        consumer.wait_stream(self._h2d)
+        for t in dev:
+            t.record_stream(consumer)
+        return dev
+
+    @staticmethod
+    def _copy_aux(static_aux, src):
+        """Copy the video stage's graph inputs (a list of device tensors) into the graph's static buffers."""
+        for s, t in zip(static_aux, src or ()):
+            s.copy_(t, non_blocking=True)
 
     # ---- all-gather of the final outputs inside the pipeline (frame-shard data parallelism) ----------------
     def enable_gather(self, keys=("rendered_img", "vertices", "params"), group=None, backend="auto"):
@@ -400,6 +478,7 @@ class SmirkPipeline:
                 out={k: torch.empty(rec["out"][k].shape, dtype=rec["out"][k].dtype).pin_memory() for k in keys},
                 dev_in=torch.empty_like(rec["img"]),
                 dev_mask=torch.empty_like(rec["mask"]) if rec["mask"] is not None else None,
+                dev_aux=[torch.empty_like(a) for a in rec["aux"]],
                 dev_out={k: torch.empty_like(rec["out"][k]) for k in keys})
             if getattr(self, "_h2d", None) is None:
                 self._h2d = torch.cuda.Stream(device=self.device)
@@ -415,6 +494,8 @@ class SmirkPipeline:
         batch i.  Returns the lane's pinned output dict — ``join()`` (or ``lane_done(i).synchronize()``)
         before reading it."""
         B = img_pinned.shape[0]
+        if self.video is not None:
+            self.video.check(img_pinned, masked_pinned)
         lane = i % self.slots
         hb = self.host_buffers(B, lane, keys)
         rec = self.capture(B, lane)
@@ -426,6 +507,8 @@ class SmirkPipeline:
             hb["dev_in"].copy_(img_pinned, non_blocking=True)
             if hb["dev_mask"] is not None:
                 hb["dev_mask"].copy_(masked_pinned, non_blocking=True)
+            if hb["dev_aux"]:
+                self._copy_aux(hb["dev_aux"], [masked_pinned[k] for k in self._video_keys()])
             L.staged.record(self._h2d)
         with torch.cuda.stream(compute):
             compute.wait_event(L.staged)
@@ -435,6 +518,7 @@ class SmirkPipeline:
             rec["img"].copy_(hb["dev_in"], non_blocking=True)
             if rec["mask"] is not None:
                 rec["mask"].copy_(hb["dev_mask"], non_blocking=True)
+            self._copy_aux(rec["aux"], hb["dev_aux"])
             L.consumed.record(compute)
             rec["graph"].replay()
             for k in keys:
@@ -454,6 +538,8 @@ class SmirkPipeline:
     def bytes_per_step(self, B, keys=("rendered_img", "vertices", "params")):
         rec = self.capture(B)
         h2d = B * 3 * 224 * 224 * 4 + (rec["mask"].numel() * 4 if rec["mask"] is not None else 0)
+        if self.video is not None:
+            h2d = sum(t.numel() * t.element_size() for t in [rec["img"]] + rec["aux"])
         d2h = sum(rec["out"][k].numel() * rec["out"][k].element_size() for k in keys)
         return h2d, d2h
 
