@@ -160,6 +160,27 @@ size_t smk_encoder_workspace_bytes(const SmkEncoder* h, int B);
  * with the clamps of smirk_encoder.py:105-108 already applied to columns n_exp..n_exp+4.           */
 int smk_encoder_forward(const SmkEncoder* h, const float* img, int B, float* pose_cam, float* shape,
                         float* expr, void* ws, size_t ws_bytes, void* stream);
+/* Input gradient (frozen weights, eval-mode BN).  An empty batch (B = 0) is a no-op; the backward is deterministic: no
+ * atomics, fixed summation order.
+ * Grad-mode forward: the same launches and bitwise the same outputs as smk_encoder_forward at every precision, plus what
+ * the backward needs (the output of every ReLU, fp32 NHWC, and the pre-clamp head outputs) written into `saved`
+ * (caller-owned, >= smk_encoder_saved_bytes; one buffer per forward whose gradient will be taken).
+ * ws / ws_bytes: the forward workspace (smk_encoder_workspace_bytes). */
+size_t smk_encoder_saved_bytes(const SmkEncoder* h, int B);
+int smk_encoder_forward_saved(const SmkEncoder* h, const float* img, int B, float* pose_cam, float* shape, float* expr,
+                              float* saved, size_t saved_bytes, void* ws, size_t ws_bytes, void* stream);
+/* Layout of tensor i of `saved`: its name (the reference's module path of the ReLU's BatchNorm, e.g.
+ * "shape_encoder.encoder.bn1" for the stem, "shape_encoder.encoder.blocks.2.1.bn1" / ".bn2" for an inverted-residual
+ * block's expand / depthwise output, or the head, "expression_encoder.expression_layers.0", for its pre-clamp output),
+ * float offset, and dims [4] = B,H,W,C of the NHWC tensor (a head is 1 x 1 x n_out).  Forward order within each backbone,
+ * backbones in slot order (pose, shape, expression).  Returns non-zero past the last tensor. */
+int smk_encoder_saved_tensor(const SmkEncoder* h, int B, int i, const char** name, size_t* offset, int* dims);
+/* Input gradient: upstream gradients of the raw outputs (pose_cam [B,6], shape [B,n_shape], expr [B,n_exp+5]; each may
+ * be NULL, meaning zero, and then its backbone launches nothing) -> g_img [B,3,224,224] NCHW (written, not accumulated;
+ * zero-filled when every upstream gradient is NULL).  ws >= smk_encoder_backward_workspace_bytes. */
+size_t smk_encoder_backward_workspace_bytes(const SmkEncoder* h, int B);
+int smk_encoder_backward(const SmkEncoder* h, int B, const float* saved, size_t saved_bytes, const float* g_pose_cam,
+                         const float* g_shape, const float* g_expr, float* g_img, void* ws, size_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * SmirkGenerator — replaces SmirkGenerator.forward (src/smirk_generator.py:51-86), eval-mode BN.
@@ -180,6 +201,23 @@ size_t smk_generator_workspace_bytes(const SmkGenerator* h, int B);
 /* x [B,in_channels,224,224] NCHW -> y [B,out_channels,224,224] NCHW in (0,1). */
 int smk_generator_forward(const SmkGenerator* h, const float* x, int B, float* y,
                           void* ws, size_t ws_bytes, void* stream);
+/* Input gradient (frozen weights, eval-mode BN).  An empty batch (B = 0) is a no-op; the backward is deterministic: no
+ * atomics, fixed summation order.
+ * Grad-mode forward: the same launches and bitwise the same y as smk_generator_forward, plus the activations the backward
+ * needs (the post-ReLU output of every block conv and every ResNet conv1, fp32 NHWC) written into `saved`
+ * (caller-owned, >= smk_generator_saved_bytes; one buffer per forward whose gradient will be taken).
+ * ws / ws_bytes: the forward workspace (smk_generator_workspace_bytes). */
+size_t smk_generator_saved_bytes(const SmkGenerator* h, int B);
+int smk_generator_forward_saved(const SmkGenerator* h, const float* x, int B, float* y, float* saved, size_t saved_bytes,
+                                void* ws, size_t ws_bytes, void* stream);
+/* Layout of tensor i of `saved`: its name (the reference's layer name, e.g. "enc1conv2", "res0conv1", "dec1conv2"),
+ * float offset, and dims [4] = B,H,W,C of the NHWC tensor.  Returns non-zero past the last tensor. */
+int smk_generator_saved_tensor(const SmkGenerator* h, int B, int i, const char** name, size_t* offset, int* dims);
+/* Input gradient: y (the forward's output) and g_y [B,out_channels,224,224] NCHW -> g_x [B,in_channels,224,224] NCHW
+ * (written, not accumulated).  ws >= smk_generator_backward_workspace_bytes. */
+size_t smk_generator_backward_workspace_bytes(const SmkGenerator* h, int B);
+int smk_generator_backward(const SmkGenerator* h, int B, const float* y, const float* saved, size_t saved_bytes,
+                           const float* g_y, float* g_x, void* ws, size_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Crop / warp front and back end (SURVEY.md 8f #2) — replaces the CPU `skimage.transform.warp` calls of
@@ -197,6 +235,25 @@ int smk_crop_warp(const uint8_t* frames, int B, int H, int W, const double* minv
 int smk_warp_u8(const uint8_t* src, int B, int Hs, int Ws, const double* m, int Hd, int Wd, uint8_t* dst,
                 void* ws, size_t ws_bytes, void* stream);
 int smk_f32chw_to_u8hwc(const float* in, int B, int S, uint8_t* out, void* stream);
+
+/* The output grid of the video demo (demo_video.py --crop [--render_orig] [--use_smirk_generator]).  An empty batch
+ * (B = 0) is a no-op.
+ * create_mask(cropped_kpt, (S, S)) of the reference (datasets/base_dataset.py:9-15) for each frame: pts [B,L,2] int32
+ * points in crop pixels (1 <= L <= 1024), mask [B,1,S,S] float, 0 inside cv2.convexHull(pts) filled by
+ * cv2.fillConvexPoly (lineType 8, shift 0) and 1 outside, bit for bit (points outside the crop, repeated or collinear
+ * points included); S <= 256. */
+int smk_hull_mask(const int32_t* pts, int B, int L, int S, float* mask, void* stream);
+/* Workspace of smk_video_compose with render_orig (the per-panel clip range); without render_orig none is needed. */
+size_t smk_video_workspace_bytes(int B, int n_panels);
+/* grid [B, Hout, (n_panels + 1) * Wout, 3] uint8 BGR, one row of panels per frame: what demo_video.py:211-214 writes.
+ *   render_orig != 0: Hout x Wout = H x W; panel 0 = frames [B,H,W,3] (BGR); panel k = panels[k-1] [B,3,S,S] (RGB in
+ *                     [0,1]) converted to uint8 ((x * 255).astype(uint8)) and warped back to the frame with m [B,9]
+ *                     (float64, row-major crop -> frame similarity, tform.params), skimage warp semantics; crop unused.
+ *   render_orig == 0: Hout x Wout = S x S; panel 0 = crop [B,3,S,S] (the encoder's RGB input in [0,1]), panel k =
+ *                     panels[k-1], both converted to uint8; frames and m unused (may be NULL).
+ * panels: host array of n_panels (1 or 2) device pointers.  ws >= smk_video_workspace_bytes(B, n_panels) with render_orig. */
+int smk_video_compose(const uint8_t* frames, int B, int H, int W, const float* crop, const float* const* panels, int n_panels,
+                      int S, const double* m, int render_orig, uint8_t* grid, void* ws, size_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Masking between Renderer and SmirkGenerator (SURVEY.md 8f #1; src/utils/masking.py, demo.py:138-167).
@@ -302,12 +359,5 @@ int smk_debug_stem_ds(const float* img, int B, int H, int W, const float* stem_w
 #ifdef __cplusplus
 }
 #endif
-
-/* The generator's input-gradient entry points. */
-#include "smirk_b200_grad.h"
-/* The encoder's input-gradient entry points. */
-#include "smirk_b200_encoder_grad.h"
-/* The video demo's output grid. */
-#include "smirk_b200_video.h"
 
 #endif /* SMIRK_B200_H */

@@ -79,14 +79,27 @@ BINDINGS = [
     ("smk_encoder_destroy", None, [_vp]),
     ("smk_encoder_workspace_bytes", _sz, [_vp, _i]),
     ("smk_encoder_forward", _i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_encoder_saved_bytes", _sz, [_vp, _i]),
+    ("smk_encoder_forward_saved", _i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp, _sz, STREAM]),
+    ("smk_encoder_saved_tensor", _i, [_vp, _i, _i, C.POINTER(C.c_char_p), C.POINTER(_sz), C.POINTER(C.c_int)]),
+    ("smk_encoder_backward_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_encoder_backward", _i, [_vp, _i, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, STREAM]),
     ("smk_generator_create", _i, [C.POINTER(SmkGeneratorDesc), _vpp]),
     ("smk_generator_destroy", None, [_vp]),
     ("smk_generator_workspace_bytes", _sz, [_vp, _i]),
     ("smk_generator_forward", _i, [_vp, _vp, _i, _vp, _vp, _sz, STREAM]),
+    ("smk_generator_saved_bytes", _sz, [_vp, _i]),
+    ("smk_generator_forward_saved", _i, [_vp, _vp, _i, _vp, _vp, _sz, _vp, _sz, STREAM]),
+    ("smk_generator_saved_tensor", _i, [_vp, _i, _i, C.POINTER(C.c_char_p), C.POINTER(_sz), C.POINTER(C.c_int)]),
+    ("smk_generator_backward_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_generator_backward", _i, [_vp, _i, _vp, _vp, _sz, _vp, _vp, _vp, _sz, STREAM]),
     ("smk_warp_workspace_bytes", _sz, [_i]),
     ("smk_crop_warp", _i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _sz, STREAM]),
     ("smk_warp_u8", _i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _sz, STREAM]),
     ("smk_f32chw_to_u8hwc", _i, [_vp, _i, _i, _vp, STREAM]),
+    ("smk_hull_mask", _i, [_vp, _i, _i, _i, _vp, STREAM]),
+    ("smk_video_workspace_bytes", _sz, [_i, _i]),
+    ("smk_video_compose", _i, [_vp, _i, _i, _i, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _sz, STREAM]),
     ("smk_masking_create", _i, [C.POINTER(SmkMaskingDesc), _vpp]),
     ("smk_masking_destroy", None, [_vp]),
     ("smk_masking_workspace_bytes", _sz, [_vp, _i, _i]),
@@ -114,30 +127,7 @@ BINDINGS = [
     ("smk_debug_xdw3x", _i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _vp, STREAM]),
     ("smk_debug_stem_ds", _i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, STREAM]),
 ]
-# The same for include/smirk_b200_grad.h (the generator's input gradient), which smirk_b200.h includes at its end.
-GRAD_BINDINGS = [
-    ("smk_generator_saved_bytes", _sz, [_vp, _i]),
-    ("smk_generator_forward_saved", _i, [_vp, _vp, _i, _vp, _vp, _sz, _vp, _sz, STREAM]),
-    ("smk_generator_saved_tensor", _i, [_vp, _i, _i, C.POINTER(C.c_char_p), C.POINTER(_sz), C.POINTER(C.c_int)]),
-    ("smk_generator_backward_workspace_bytes", _sz, [_vp, _i]),
-    ("smk_generator_backward", _i, [_vp, _i, _vp, _vp, _sz, _vp, _vp, _vp, _sz, STREAM]),
-]
-# The same for include/smirk_b200_encoder_grad.h (the encoder's input gradient), included after smirk_b200_grad.h.
-ENCODER_GRAD_BINDINGS = [
-    ("smk_encoder_saved_bytes", _sz, [_vp, _i]),
-    ("smk_encoder_forward_saved", _i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp, _sz, STREAM]),
-    ("smk_encoder_saved_tensor", _i, [_vp, _i, _i, C.POINTER(C.c_char_p), C.POINTER(_sz), C.POINTER(C.c_int)]),
-    ("smk_encoder_backward_workspace_bytes", _sz, [_vp, _i]),
-    ("smk_encoder_backward", _i, [_vp, _i, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, STREAM]),
-]
-# The same for include/smirk_b200_video.h (the video demo's output grid), included after smirk_b200_encoder_grad.h.
-VIDEO_BINDINGS = [
-    ("smk_hull_mask", _i, [_vp, _i, _i, _i, _vp, STREAM]),
-    ("smk_video_workspace_bytes", _sz, [_i, _i]),
-    ("smk_video_compose", _i, [_vp, _i, _i, _i, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _sz, STREAM]),
-]
-_ALL_BINDINGS = BINDINGS + GRAD_BINDINGS + ENCODER_GRAD_BINDINGS + VIDEO_BINDINGS
-_TAKES_STREAM = frozenset(name for name, _, args in _ALL_BINDINGS if args[-1:] == [STREAM])
+_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS if args[-1:] == [STREAM])
 
 
 def lib():
@@ -149,7 +139,7 @@ def lib():
         raise RuntimeError("smirk_b200: %s not found — build it with `python -m smirk_b200.build` "
                            "(there is no CPU / PyTorch fallback)" % LIB_PATH)
     L = C.CDLL(LIB_PATH)
-    for name, restype, argtypes in _ALL_BINDINGS:
+    for name, restype, argtypes in BINDINGS:
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, [_vp if a is STREAM else a for a in argtypes]
     if L.smk_version() != 100:
@@ -229,6 +219,28 @@ def create(kind, desc, device):
     h = C.c_void_p()
     call("smk_%s_create" % kind, device, C.byref(desc), C.byref(h))
     return NativeHandle(h, "smk_%s_destroy" % kind)
+
+
+def saved_buffer(kind, handle, B, device):
+    """A buffer of ``smk_<kind>_saved_bytes`` for the activations of one grad-mode forward (pass ``numel() * 4`` bytes)."""
+    nbytes = call("smk_%s_saved_bytes" % kind, device, handle, B)
+    return torch.empty(max(nbytes // 4, 1), dtype=torch.float32, device=device)
+
+
+def saved_views(kind, handle, saved, B):
+    """{name: view of ``saved``} for every tensor ``smk_<kind>_saved_tensor`` lays out in it, in layout order: [B,C,H,W]
+    views of the NHWC tensors, [B,C] for 1 x 1 ones (the encoder's head outputs)."""
+    fn = getattr(lib(), "smk_%s_saved_tensor" % kind)
+    name, off, dims = C.c_char_p(), C.c_size_t(), (C.c_int * 4)()
+    out, i = {}, 0
+    while (rc := fn(handle, B, i, C.byref(name), C.byref(off), dims)) == 0:       # non-zero past the last tensor
+        b, h, w, c = dims
+        t = saved[off.value:off.value + b * h * w * c].view(b, h, w, c)
+        out[name.value.decode()] = t.view(b, c) if h == w == 1 else t.permute(0, 3, 1, 2)
+        i += 1
+    if not out:                                 # not even tensor 0: raise with the library's message
+        check(rc, "smk_%s_saved_tensor" % kind)
+    return out
 
 
 class Workspace:

@@ -25,8 +25,7 @@ def sources():
 def build(force=False, verbose=False):
     os.makedirs(OBJ, exist_ok=True)
     hdrs = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
-    hdrs += [os.path.join(HERE, "..", "include", h) for h in ("smirk_b200.h", "smirk_b200_grad.h", "smirk_b200_encoder_grad.h",
-                                                           "smirk_b200_video.h")]
+    hdrs.append(os.path.join(HERE, "..", "include", "smirk_b200.h"))
     hdr_m = max(os.path.getmtime(h) for h in hdrs)
     objs, rebuilt = [], False
     for s in sources():

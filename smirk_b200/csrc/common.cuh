@@ -5,6 +5,8 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
+#include <algorithm>
+#include <string>
 #include <vector>
 #include "../../include/smirk_b200.h"
 
@@ -86,6 +88,43 @@ static inline int cdiv(long a, long b) { return (int)((a + b - 1) / b); }
 
 // Streaming multiprocessors of the current device (cached per device ordinal): the size of a persistent grid.
 int num_sms();
+
+// Blocks of 256 threads for a grid-stride loop over `total` items: one item per thread, at most 16 blocks per SM.
+static inline int grid_of(long total) { return (int)std::min<long>((total + 255) / 256, 16L * num_sms()); }
+
+// TF-SAME padding of a 3x3 window: zero rows / columns before the first input pixel (TensorFlow pads the odd one after).
+static inline int same_pad_begin(int H, int stride) {
+    const int out = (H + stride - 1) / stride;
+    return std::max((out - 1) * stride + 3 - H, 0) / 2;
+}
+
+// Where a grad-mode forward keeps the activations its backward needs: named [B,H,W,C] fp32 tensors in one caller-owned
+// buffer, in the order they were added.  A tensor's offset is B times its per-image offset, and every tensor starts on a
+// 64-float boundary so float4 / TMA access to it stays aligned whatever B is.
+struct SavedLayout {
+    std::vector<std::string> name;
+    std::vector<size_t> off;           // per-image float offset of each tensor
+    std::vector<int> hwc;              // H, W, C of each tensor
+    size_t total = 0;                  // floats per image
+
+    int add(const std::string& n, int H, int W, int C) {      // -> the tensor's index
+        name.push_back(n); off.push_back(total); hwc.insert(hwc.end(), {H, W, C});
+        total += ((size_t)H * W * C + 63) / 64 * 64;
+        return (int)name.size() - 1;
+    }
+    size_t bytes(int B) const { return B > 0 ? total * (size_t)B * sizeof(float) : 0; }
+};
+
+// The `smk_*_saved_tensor` query of a handle's layout L (null for a null handle); fn names the entry point in errors.
+static inline int saved_tensor(const SavedLayout* L, const char* fn, int B, int i, const char** name, size_t* offset, int* dims) {
+    SMK_REQUIRE(L && name && offset && dims, "%s: null argument", fn);
+    SMK_REQUIRE(B >= 0, "%s: negative batch", fn);
+    SMK_REQUIRE(i >= 0 && i < (int)L->name.size(), "%s: index %d out of range (%d tensors)", fn, i, (int)L->name.size());
+    *name = L->name[i].c_str();
+    *offset = L->off[i] * (size_t)B;
+    dims[0] = B; dims[1] = L->hwc[3 * i]; dims[2] = L->hwc[3 * i + 1]; dims[3] = L->hwc[3 * i + 2];
+    return 0;
+}
 
 #ifdef __CUDACC__
 // Launch errors surface through cudaGetLastError in SMK_CHECK_LAUNCH.

@@ -22,6 +22,8 @@
 namespace {
 
 using smk::TensorCursor;
+using smk::grid_of;
+using smk::same_pad_begin;
 
 constexpr float kBnEps = 1e-3f;
 
@@ -136,12 +138,7 @@ struct SmkEncoder {
     bool x3 = false;             // precision 3: 3xTF32 error-compensated tensor-core arithmetic (fp32-equivalent), no TF32 rounding of activations
     bool present[3] = {false, false, false};   // a handle may hold a subset of the backbones (PoseEncoder / ShapeEncoder / ExpressionEncoder alone)
     float *ones = nullptr, *zeros = nullptr;   // unit scale / zero bias of the dgrad GEMM epilogues
-    // saved tensors of the grad-mode forward (forward order within a backbone, backbones in slot order): name, per-image
-    // float offset, H, W, C
-    std::vector<std::string> sv_name;
-    std::vector<size_t> sv_off;
-    std::vector<int> sv_hwc;
-    size_t sv_total = 0;                       // floats per image
+    smk::SavedLayout saved;                    // of the grad-mode forward: forward order within a backbone, backbones in slot order
     smk::DeviceArena arena;
     // Fork/join plumbing for running the backbones as parallel branches of the caller's stream.  A forward takes the
     // next set of a small pool (atomic round-robin), so up to kForkSets forwards of one handle may be in flight on
@@ -231,12 +228,7 @@ extern "C" int smk_encoder_create(const SmkEncoderDesc* desc, SmkEncoder** out) 
         static const char* const kEnc[3] = {"pose_encoder", "shape_encoder", "expression_encoder"};
         static const char* const kHead[3] = {"pose_cam_layers.0", "shape_layers.0", "expression_layers.0"};
         static const int kStageLarge[] = {1, 2, 3, 4, 2, 3, 1}, kStageSmall[] = {1, 2, 3, 2, 3, 1};
-        auto add = [&](const std::string& name, int H, int W, int C) {
-            h->sv_name.push_back(name); h->sv_off.push_back(h->sv_total);
-            h->sv_hwc.push_back(H); h->sv_hwc.push_back(W); h->sv_hwc.push_back(C);
-            h->sv_total += ((size_t)H * W * C + 63) / 64 * 64;       // every tensor starts 256-byte aligned (float4 / TMA access)
-            return (int)h->sv_name.size() - 1;
-        };
+        auto add = [h](const std::string& name, int H, int W, int C) { return h->saved.add(name, H, W, C); };
         for (int i = 0; i < 3; ++i) {
             if (!h->present[i]) continue;
             Backbone& bb = h->bb[i];
@@ -290,6 +282,40 @@ static int pointwise(int n, const ConvW* const* c, float* const* in, int B, int 
     return smk::conv(q[0], st, n == 2 ? &q[1] : nullptr);
 }
 
+// One unit of work: n = 1 backbone, or the pair idx = {1, 2}, on stream st.
+struct Unit { int n; int idx[2]; cudaStream_t st; };
+
+// Runs run(unit) (-> status; the first error stops the walk) over the backbones with use[i] set.  The three backbones
+// are independent (smirk_encoder.py:123-133 merely runs them one after another): with more than one in use, the units
+// fork from main_st onto the side streams of one of the handle's fork sets, so their many small, latency-bound layers
+// overlap, and join back into main_st — even after an error, so a capturing stream is left consistent.  Event
+// record/wait on other streams is legal under stream capture, so a CUDA graph of the caller's stream gets parallel
+// branches.  The two "large" backbones (shape, expression) have the same layer list, so on the tensor-core path they
+// advance in lock step as one unit and every layer of the pair is ONE launch; the small (pose) backbone is its own unit.
+template <typename Run>
+static int for_each_unit(const SmkEncoder* h, const bool use[3], cudaStream_t main_st, const char* what, Run&& run) {
+    const int n_use = (int)use[0] + (int)use[1] + (int)use[2];
+    const bool concurrent = !smk::profiling() && n_use > 1;       // the event profiler wants one kernel at a time
+    const SmkEncoder::ForkSet& fk = h->forks[__atomic_fetch_add(&h->next_fork, 1u, __ATOMIC_RELAXED) % SmkEncoder::kForkSets];
+    Unit units[3]; int n_units = 0;
+    if (use[0]) units[n_units++] = Unit{1, {0, 0}, main_st};
+    if (h->precision >= 1 && use[1] && use[2]) units[n_units++] = Unit{2, {1, 2}, concurrent ? fk.side[0] : main_st};
+    else for (int i = 1; i < 3; ++i) if (use[i]) units[n_units++] = Unit{1, {i, i}, concurrent ? fk.side[i - 1] : main_st};
+    if (!use[0] && n_units > 0) units[0].st = main_st;                             // without pose, the first unit takes the caller's stream
+    if (concurrent) {
+        SMK_CHECK_CUDA(cudaEventRecord(fk.fork, main_st));
+        for (int s = 0; s < 2; ++s) SMK_CHECK_CUDA(cudaStreamWaitEvent(fk.side[s], fk.fork, 0));
+    }
+    int rc = 0;
+    for (int u = 0; u < n_units && !rc; ++u) rc = run(units[u]);
+    for (int s = 0; s < 2 && concurrent; ++s) {
+        cudaError_t e1 = cudaEventRecord(fk.join[s], fk.side[s]);
+        cudaError_t e2 = e1 == cudaSuccess ? cudaStreamWaitEvent(main_st, fk.join[s], 0) : e1;
+        if (!rc && e2 != cudaSuccess) { smk::set_error("%s: stream join failed: %s", what, cudaGetErrorString(e2)); rc = (int)e2; }
+    }
+    return rc;
+}
+
 // The forward; sv (grad mode, may be null): the saved buffer.  With sv the launches and arithmetic are those of the
 // forward-only path: the ReLU outputs the forward writes to HBM anyway (stem, unfused e / d, cn) go to their saved slot
 // instead of a workspace buffer, the fused kernels and the head store a second copy.
@@ -300,16 +326,10 @@ static int encoder_forward(const SmkEncoder* h, const float* img, int B, float* 
     for (int i = 0; i < 3; ++i) for (int j = 0; j < 4; ++j) bufs[i][j] = w.take<float>((size_t)B * h->max_act);
     SMK_REQUIRE(bufs[2][3] != nullptr, "smk_encoder_forward: workspace carve-up failed");
     float* outs[3] = {pose_cam, shape, expr};
-    auto SV = [&](int i) -> float* { return sv ? sv + (size_t)B * h->sv_off[i] : nullptr; };
+    auto SV = [&](int i) -> float* { return sv ? sv + (size_t)B * h->saved.off[i] : nullptr; };
     float* stem_out[3];                                           // where each backbone's stem writes
     for (int i = 0; i < 3; ++i) stem_out[i] = sv && h->present[i] ? SV(h->bb[i].sv_stem) : bufs[i][0];
-    // The three backbones are independent (smirk_encoder.py:123-133 merely runs them one after another):
-    // fork the two large ones onto the handle's side streams so their many small, latency-bound layers
-    // overlap; join before returning.  Event record/wait on other streams is legal under stream capture,
-    // so a CUDA graph of the caller's stream gets three parallel branches.
     const int n_present = (int)h->present[0] + (int)h->present[1] + (int)h->present[2];
-    const bool concurrent = !smk::profiling() && n_present > 1;   // the event profiler wants one kernel at a time
-    const SmkEncoder::ForkSet& fk = h->forks[__atomic_fetch_add(&h->next_fork, 1u, __ATOMIC_RELAXED) % SmkEncoder::kForkSets];
     // precision 2: stem + block 0 (depthwise-separable, 16 channels at 112 x 112) run as one kernel per backbone —
     // the three largest activations never reach HBM.
     const bool fuse_stem = h->fuse_xdw;                           // every backbone starts with a DS block
@@ -321,27 +341,15 @@ static int encoder_forward(const SmkEncoder* h, const float* img, int B, float* 
         for (int i = 0; i < 3; ++i)
             if (h->present[i]) { if (int rc = smk::stem_conv(img, B, 224, 224, h->bb[i].stem.w, h->bb[i].stem.scale, h->bb[i].stem.bias, stem_out[i], main_st)) return rc; }
     }
-    if (concurrent) {
-        SMK_CHECK_CUDA(cudaEventRecord(fk.fork, main_st));
-        for (int s = 0; s < 2; ++s) SMK_CHECK_CUDA(cudaStreamWaitEvent(fk.side[s], fk.fork, 0));
-    }
-    int rc = 0;                                   // first error; the side streams are joined on every path
-    // Work units: the two "large" backbones (shape, expression) have the same layer list, so on the tensor-core path they
-    // advance in lock step and every layer of the pair is ONE launch; the small (pose) backbone is its own unit.
-    const bool pair = h->precision >= 1 && h->present[1] && h->present[2];
-    struct Unit { int n; int idx[2]; cudaStream_t st; };
-    Unit units[3]; int n_units = 0;
-    if (h->present[0]) units[n_units++] = Unit{1, {0, 0}, main_st};
-    if (pair) units[n_units++] = Unit{2, {1, 2}, concurrent ? fk.side[0] : main_st};
-    else for (int i = 1; i < 3; ++i) if (h->present[i]) units[n_units++] = Unit{1, {i, i}, concurrent ? fk.side[i - 1] : main_st};
-    if (!h->present[0] && n_units > 0) units[0].st = main_st;                        // a lone unit runs on the caller's stream
-    for (int u = 0; u < n_units && !rc; ++u) {
-        const int n = units[u].n;
-        cudaStream_t st = units[u].st;
+    // the stems above run on main_st before the fork
+    return for_each_unit(h, h->present, main_st, "smk_encoder_forward", [&](const Unit& unit) {
+        const int n = unit.n;
+        cudaStream_t st = unit.st;
+        int rc = 0;
         // x / y: the workspace ping-pong pair; cur: the current block's input (x, or a saved tensor)
         const Backbone* bb[2]; float *x[2], *y[2], *e[2], *d[2], *cur[2];
         for (int k = 0; k < n; ++k) {
-            const int i = units[u].idx[k];
+            const int i = unit.idx[k];
             bb[k] = &h->bb[i]; x[k] = bufs[i][0]; y[k] = bufs[i][1]; e[k] = bufs[i][2]; d[k] = bufs[i][3]; cur[k] = stem_out[i];
         }
         int res = 112;
@@ -411,17 +419,12 @@ static int encoder_forward(const SmkEncoder* h, const float* img, int B, float* 
         if (!rc) {                              // global average pool + head + clamps: one launch per unit
             smk::GapHeadProblem gp[2];
             for (int k = 0; k < n; ++k)
-                gp[k] = smk::GapHeadProblem{cur[k], bb[k]->head_w, bb[k]->head_b, bb[k]->codes, outs[units[u].idx[k]], bb[k]->n_out,
+                gp[k] = smk::GapHeadProblem{cur[k], bb[k]->head_w, bb[k]->head_b, bb[k]->codes, outs[unit.idx[k]], bb[k]->n_out,
                                             SV(bb[k]->sv_head)};
             rc = smk::gap_head(gp, n, B, res * res, bb[0]->feat, st);
         }
-    }
-    for (int s = 0; s < 2 && concurrent; ++s) {   // join even after an error so a capturing stream is left consistent
-        cudaError_t e1 = cudaEventRecord(fk.join[s], fk.side[s]);
-        cudaError_t e2 = e1 == cudaSuccess ? cudaStreamWaitEvent(main_st, fk.join[s], 0) : e1;
-        if (!rc && e2 != cudaSuccess) { smk::set_error("smk_encoder_forward: stream join failed: %s", cudaGetErrorString(e2)); rc = (int)e2; }
-    }
-    return rc;
+        return rc;
+    });
 }
 
 extern "C" int smk_encoder_forward(const SmkEncoder* h, const float* img, int B, float* pose_cam, float* shape,
@@ -556,13 +559,6 @@ stem_dgrad_kernel(const __grid_constant__ StemDgrad p, int B, int H, int W, int 
     for (int c = 0; c < 3; ++c) out[(((size_t)b * 3 + c) * H + ih) * W + iw] = acc[c];
 }
 
-int grid_of(long total) { return (int)std::min<long>((total + 255) / 256, 16L * smk::num_sms()); }
-
-int same_pad_begin(int H, int stride) {
-    const int out = (H + stride - 1) / stride;
-    return std::max((out - 1) * stride + 3 - H, 0) / 2;
-}
-
 // 1x1 dgrad of n = 1 or 2 backbones: out[m, :N] = g[m, :K] . Wd (+ res), K = the conv's cout, N = its cin.
 int dgrad_pw(const SmkEncoder* h, int n, const ConvW* const* c, const float* const* g, int B, int H, int W, const float* const* res,
              float* const* out, bool round, const char* tag, cudaStream_t st) {
@@ -598,18 +594,10 @@ int dgrad_dw(int n, const Block* const* b, const float* const* g, const float* c
 
 }  // namespace
 
-extern "C" size_t smk_encoder_saved_bytes(const SmkEncoder* h, int B) {
-    return h && B > 0 ? h->sv_total * (size_t)B * sizeof(float) : 0;
-}
+extern "C" size_t smk_encoder_saved_bytes(const SmkEncoder* h, int B) { return h ? h->saved.bytes(B) : 0; }
 
 extern "C" int smk_encoder_saved_tensor(const SmkEncoder* h, int B, int i, const char** name, size_t* offset, int* dims) {
-    SMK_REQUIRE(h && name && offset && dims, "smk_encoder_saved_tensor: null argument");
-    SMK_REQUIRE(B >= 0, "smk_encoder_saved_tensor: negative batch");
-    SMK_REQUIRE(i >= 0 && i < (int)h->sv_name.size(), "smk_encoder_saved_tensor: index %d out of range (%d tensors)", i, (int)h->sv_name.size());
-    *name = h->sv_name[i].c_str();
-    *offset = h->sv_off[i] * (size_t)B;
-    dims[0] = B; dims[1] = h->sv_hwc[3 * i]; dims[2] = h->sv_hwc[3 * i + 1]; dims[3] = h->sv_hwc[3 * i + 2];
-    return 0;
+    return smk::saved_tensor(h ? &h->saved : nullptr, "smk_encoder_saved_tensor", B, i, name, offset, dims);
 }
 
 extern "C" int smk_encoder_forward_saved(const SmkEncoder* h, const float* img, int B, float* pose_cam, float* shape, float* expr,
@@ -645,32 +633,19 @@ extern "C" int smk_encoder_backward(const SmkEncoder* h, int B, const float* sav
     float* bufs[3][3];
     for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) bufs[i][j] = w.take<float>((size_t)B * h->max_act);
     SMK_REQUIRE(bufs[2][2] != nullptr, "smk_encoder_backward: workspace carve-up failed");
-    auto SV = [&](int i) -> const float* { return saved + (size_t)B * h->sv_off[i]; };
+    auto SV = [&](int i) -> const float* { return saved + (size_t)B * h->saved.off[i]; };
     const bool tc = h->precision >= 1;
     const bool rnd = tc && !h->x3;                  // gradients that feed a TF32 GEMM are rounded (3xTF32 splits them itself)
     const float* g_stem[3] = {nullptr, nullptr, nullptr};
-    // work units and streams as in the forward
     const int n_active = (int)active[0] + (int)active[1] + (int)active[2];
-    const bool concurrent = !smk::profiling() && n_active > 1;
-    const SmkEncoder::ForkSet& fk = h->forks[__atomic_fetch_add(&h->next_fork, 1u, __ATOMIC_RELAXED) % SmkEncoder::kForkSets];
-    if (concurrent) {
-        SMK_CHECK_CUDA(cudaEventRecord(fk.fork, main_st));
-        for (int s = 0; s < 2; ++s) SMK_CHECK_CUDA(cudaStreamWaitEvent(fk.side[s], fk.fork, 0));
-    }
-    const bool pair = tc && active[1] && active[2];
-    struct Unit { int n; int idx[2]; cudaStream_t st; };
-    Unit units[3]; int n_units = 0;
-    if (active[0]) units[n_units++] = Unit{1, {0, 0}, main_st};
-    if (pair) units[n_units++] = Unit{2, {1, 2}, concurrent ? fk.side[0] : main_st};
-    else for (int i = 1; i < 3; ++i) if (active[i]) units[n_units++] = Unit{1, {i, i}, concurrent ? fk.side[i - 1] : main_st};
-    if (!active[0] && n_units > 0) units[0].st = main_st;
-    int rc = 0;
-    for (int u = 0; u < n_units && !rc; ++u) {
-        const int n = units[u].n;
-        cudaStream_t st = units[u].st;
+    // the stem dgrad after the join sums every backbone's stem gradient on main_st
+    int rc = for_each_unit(h, active, main_st, "smk_encoder_backward", [&](const Unit& unit) {
+        const int n = unit.n;
+        cudaStream_t st = unit.st;
+        int rc = 0;
         const Backbone* bb[2]; float *gy[2], *t1[2], *t2[2];
         for (int k = 0; k < n; ++k) {
-            const int i = units[u].idx[k];
+            const int i = unit.idx[k];
             bb[k] = &h->bb[i]; gy[k] = bufs[i][0]; t1[k] = bufs[i][1]; t2[k] = bufs[i][2];
         }
         const Backbone& b0b = *bb[0];
@@ -681,7 +656,7 @@ extern "C" int smk_encoder_backward(const SmkEncoder* h, int B, const float* sav
             for (int k = 0; k < 2; ++k) {
                 const int j = k < n ? k : n - 1;
                 const Block& cn = bb[j]->blocks.back();
-                p.g[k] = g_out[units[u].idx[j]]; p.raw[k] = SV(bb[j]->sv_head); p.codes[k] = bb[j]->codes; p.w[k] = bb[j]->head_w;
+                p.g[k] = g_out[unit.idx[j]]; p.raw[k] = SV(bb[j]->sv_head); p.codes[k] = bb[j]->codes; p.w[k] = bb[j]->head_w;
                 p.cn[k] = SV(cn.sv_a); p.out[k] = t1[j]; p.n_out[k] = bb[j]->n_out;
                 max_out = std::max(max_out, bb[j]->n_out);
             }
@@ -713,16 +688,12 @@ extern "C" int smk_encoder_backward(const SmkEncoder* h, int B, const float* sav
                 for (int k = 0; k < n; ++k) { dm[k] = SV(b[k]->sv_a); am[k] = SV(bb[k]->sv_stem); }
                 rc = dgrad_pw(h, n, cp, gy, B, ro, ro, nullptr, t1, false, tc ? "ds_pw_dgrad_tc" : "ds_pw_dgrad_f32", st);
                 if (!rc) rc = dgrad_dw(n, b, t1, dm, am, bk.skip ? gy : nullptr, B, ri, t2, false, st);
-                for (int k = 0; k < n; ++k) g_stem[units[u].idx[k]] = t2[k];
+                for (int k = 0; k < n; ++k) g_stem[unit.idx[k]] = t2[k];
             }
             res = ri;
         }
-    }
-    for (int s = 0; s < 2 && concurrent; ++s) {   // join even after an error so a capturing stream is left consistent
-        cudaError_t e1 = cudaEventRecord(fk.join[s], fk.side[s]);
-        cudaError_t e2 = e1 == cudaSuccess ? cudaStreamWaitEvent(main_st, fk.join[s], 0) : e1;
-        if (!rc && e2 != cudaSuccess) { smk::set_error("smk_encoder_backward: stream join failed: %s", cudaGetErrorString(e2)); rc = (int)e2; }
-    }
+        return rc;
+    });
     if (rc) return rc;
     StemDgrad p{};
     for (int i = 0; i < 3; ++i) { p.g[i] = g_stem[i]; p.w[i] = g_stem[i] ? h->bb[i].stem_d.w : nullptr; }

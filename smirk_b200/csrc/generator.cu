@@ -31,6 +31,7 @@
 namespace {
 
 using smk::TensorCursor;
+using smk::grid_of;
 constexpr float kBnEps = 1e-5f;
 
 // dw: dgrad weights, W' scaled by the folded BN scale: [9*cout][cin_p] (fp32) or [cin_p][9*cout] (TF32), k = tap' * cout + co
@@ -98,11 +99,7 @@ struct SmkGenerator {
     Conv3 dec[4][2];                 // decoder4..1
     float *fw = nullptr, *fb = nullptr;   // final 1x1: W[f][cout], bias
     float *ones = nullptr, *zeros = nullptr;   // unit scale / zero bias of the dgrad epilogues
-    // saved activations of the grad-mode forward (forward order): name, per-image float offset, H, W, C
-    std::vector<std::string> sv_name;
-    std::vector<size_t> sv_off;
-    std::vector<int> sv_hwc;
-    size_t sv_total = 0;                  // floats per image
+    smk::SavedLayout saved;          // activations of the grad-mode forward, forward order
     smk::DeviceArena arena;
 };
 
@@ -155,11 +152,8 @@ extern "C" int smk_generator_create(const SmkGeneratorDesc* desc, SmkGenerator**
         else smk::set_error("smk_generator_create: consumed %d tensors but %d were given (state_dict order, num_batches_tracked removed)", cur.i, cur.n);
         delete h; return e != cudaSuccess ? (int)e : -1;
     }
-    auto add = [h](const std::string& name, int S, int C) {
-        h->sv_name.push_back(name); h->sv_off.push_back(h->sv_total);
-        h->sv_hwc.insert(h->sv_hwc.end(), {S, S, C});
-        h->sv_total += (size_t)S * S * C;                                  // a multiple of 64 floats: tensors stay 256-byte aligned
-    };
+    // every size is a multiple of 64 floats (init_features % 8 == 0), so the tensors are packed with no gaps
+    auto add = [h](const std::string& name, int S, int C) { h->saved.add(name, S, S, C); };
     for (int l = 0; l < 4; ++l)
         for (int j = 1; j <= 2; ++j) add("enc" + std::to_string(l + 1) + "conv" + std::to_string(j), 224 >> l, f << l);
     add("bottleneckconv1", 14, 16 * f); add("bottleneckconv2", 14, 16 * f);
@@ -226,7 +220,7 @@ int generator_forward(const SmkGenerator* h, const float* x, int B, float* y, fl
     const Plan P = make_plan(h);
     const int f = h->f;
     const bool tc = h->precision == 1;
-    auto SV = [&](int i) -> float* { return sv ? sv + (size_t)B * h->sv_off[i] : nullptr; };
+    auto SV = [&](int i) -> float* { return sv ? sv + (size_t)B * h->saved.off[i] : nullptr; };
     float* x8 = w.take<float>(P.x8 * B);
     float *cat[4], *t[4], *d[4], *p[4];
     for (int l = 0; l < 4; ++l) {
@@ -435,8 +429,6 @@ nhwc_to_nchw_kernel(const float* __restrict__ in, int B, int HW, int Cp, int C, 
     out[i] = __ldg(in + ((size_t)b * HW + r) * Cp + c);
 }
 
-int grid_of(long total) { return (int)std::min<long>((total + 255) / 256, 16L * smk::num_sms()); }
-
 // dgrad of a 3x3 conv (zero padding 1): g_in = conv3x3(g, W') over S x S, * [mask > 0] (mask: the saved input activation).
 int dgrad3(const SmkGenerator* h, const Conv3& c, const float* g, int B, int S, const float* mask, float* out, int ld_out, bool round,
            cudaStream_t st) {
@@ -496,18 +488,10 @@ extern "C" int smk_generator_forward(const SmkGenerator* h, const float* x, int 
     return generator_forward(h, x, B, y, nullptr, ws, ws_bytes, (cudaStream_t)stream);
 }
 
-extern "C" size_t smk_generator_saved_bytes(const SmkGenerator* h, int B) {
-    return h && B > 0 ? h->sv_total * (size_t)B * sizeof(float) : 0;
-}
+extern "C" size_t smk_generator_saved_bytes(const SmkGenerator* h, int B) { return h ? h->saved.bytes(B) : 0; }
 
 extern "C" int smk_generator_saved_tensor(const SmkGenerator* h, int B, int i, const char** name, size_t* offset, int* dims) {
-    SMK_REQUIRE(h && name && offset && dims, "smk_generator_saved_tensor: null argument");
-    SMK_REQUIRE(B >= 0, "smk_generator_saved_tensor: negative batch");
-    SMK_REQUIRE(i >= 0 && i < (int)h->sv_name.size(), "smk_generator_saved_tensor: index %d out of range (%d tensors)", i, (int)h->sv_name.size());
-    *name = h->sv_name[i].c_str();
-    *offset = h->sv_off[i] * (size_t)B;
-    dims[0] = B; dims[1] = h->sv_hwc[3 * i]; dims[2] = h->sv_hwc[3 * i + 1]; dims[3] = h->sv_hwc[3 * i + 2];
-    return 0;
+    return smk::saved_tensor(h ? &h->saved : nullptr, "smk_generator_saved_tensor", B, i, name, offset, dims);
 }
 
 extern "C" int smk_generator_forward_saved(const SmkGenerator* h, const float* x, int B, float* y, float* saved, size_t saved_bytes,
@@ -536,7 +520,7 @@ extern "C" int smk_generator_backward(const SmkGenerator* h, int B, const float*
     cudaStream_t st = (cudaStream_t)stream;
     const int f = h->f, cb = 16 * f;
     const bool tc = h->precision == 1;
-    auto SV = [&](int i) -> const float* { return saved + (size_t)B * h->sv_off[i]; };
+    auto SV = [&](int i) -> const float* { return saved + (size_t)B * h->saved.off[i]; };
     const GradPlan P = make_grad_plan(h);
     smk::Workspace w(ws, ws_bytes);
     float* A = w.take<float>(P.g * B); float* Bf = w.take<float>(P.g * B);

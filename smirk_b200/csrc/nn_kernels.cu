@@ -428,13 +428,6 @@ int conv_gemm(const Conv& p, cudaStream_t st) {
     return 0;
 }
 
-static inline int same_pad_begin(int H, int stride) {
-    int out = (H + stride - 1) / stride;
-    int total = (out - 1) * stride + 3 - H;
-    if (total < 0) total = 0;
-    return total / 2;
-}
-
 int dwconv3x3(const float* in, int B, int H, int W, int C, int stride, const float* w9c, const float* scale,
               const float* bias, float* out, cudaStream_t st, bool round_out) {
     SMK_REQUIRE(C % 4 == 0, "dwconv3x3: C must be a multiple of 4");

@@ -195,10 +195,9 @@ class _NativeEncoder(_lib.NativeModule, nn.Module):
         x = _lib.dev_f32(img, "img")
         B = x.shape[0]
         outs = self._outputs(B, dev)
-        nbytes = _lib.call("smk_encoder_saved_bytes", dev, h, B)
-        saved = torch.empty(max(nbytes // 4, 1), dtype=torch.float32, device=dev)
+        saved = _lib.saved_buffer("encoder", h, B, dev)
         ws = self._native_workspace("forward", _lib.call("smk_encoder_workspace_bytes", dev, h, B), dev)
-        _lib.call("smk_encoder_forward_saved", dev, h, x, B, *outs, saved, nbytes, ws, ws.numel())
+        _lib.call("smk_encoder_forward_saved", dev, h, x, B, *outs, saved, saved.numel() * 4, ws, ws.numel())
         return h, outs, saved
 
     @torch.no_grad()
@@ -210,18 +209,7 @@ class _NativeEncoder(_lib.NativeModule, nn.Module):
         are the tensors an autograd context of the same input holds."""
         self._check(img)
         h, _, saved = self._forward_saved(img)
-        B, out, i = img.shape[0], {}, 0
-        name, off, dims = C.c_char_p(), C.c_size_t(), (C.c_int * 4)()
-        while True:
-            try:
-                _lib.call("smk_encoder_saved_tensor", img.device, h, B, i, C.byref(name), C.byref(off), dims)
-            except RuntimeError:
-                break
-            b, hh, ww, c = dims
-            t = saved[off.value:off.value + b * hh * ww * c].view(b, hh, ww, c)
-            out[name.value.decode()] = t.view(b, c) if hh == ww == 1 else t.permute(0, 3, 1, 2)
-            i += 1
-        return out
+        return _lib.saved_views("encoder", h, saved, img.shape[0])
 
 
 class _EncoderFunction(torch.autograd.Function):

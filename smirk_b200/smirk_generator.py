@@ -116,10 +116,9 @@ class SmirkGenerator(_lib.NativeModule, nn.Module):
         x = _lib.dev_f32(x, "x")
         B = x.shape[0]
         y = torch.empty(B, self._cfg[1], 224, 224, dtype=torch.float32, device=dev)
-        nbytes = _lib.call("smk_generator_saved_bytes", dev, h, B)
-        saved = torch.empty(nbytes // 4, dtype=torch.float32, device=dev)
+        saved = _lib.saved_buffer("generator", h, B, dev)
         ws = self._native_workspace("forward", _lib.call("smk_generator_workspace_bytes", dev, h, B), dev)
-        _lib.call("smk_generator_forward_saved", dev, h, x, B, y, saved, nbytes, ws, ws.numel())
+        _lib.call("smk_generator_forward_saved", dev, h, x, B, y, saved, saved.numel() * 4, ws, ws.numel())
         return h, y, saved
 
     @torch.no_grad()
@@ -131,13 +130,7 @@ class SmirkGenerator(_lib.NativeModule, nn.Module):
         _lib.require_cuda(x, "x")
         self._check_input(x)
         h, _, saved = self._forward_saved(x)
-        B, out = x.shape[0], {}
-        name, off, dims = C.c_char_p(), C.c_size_t(), (C.c_int * 4)()
-        for i in range(18 + self._cfg[3]):
-            _lib.call("smk_generator_saved_tensor", x.device, h, B, i, C.byref(name), C.byref(off), dims)
-            b, hh, ww, c = dims
-            out[name.value.decode()] = saved[off.value:off.value + b * hh * ww * c].view(b, hh, ww, c).permute(0, 3, 1, 2)
-        return out
+        return _lib.saved_views("generator", h, saved, x.shape[0])
 
 
 class _GeneratorFunction(torch.autograd.Function):

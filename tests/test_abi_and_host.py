@@ -11,9 +11,11 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_library_exports_and_binds_every_declared_symbol(native_lib):
-    """The library exports every prototype in include/smirk_b200.h, and each has one row in _lib.BINDINGS with the same
-    return type and the same parameters: count, pointer / value kind, and the trailing stream where the header has one."""
+def test_every_header_prototype_is_exported_and_bound(native_lib):
+    """The library exports every prototype in include/smirk_b200.h (all 70 entry points, the input gradients and the
+    video grid included), and each has exactly one row in _lib.BINDINGS with the same return type and the same
+    parameters: count, pointer / value kind, and the trailing stream where the header has one (which is what makes
+    `_lib.call` append the current stream)."""
     import ctypes as C
     from smirk_b200 import _lib
     hdr = open(os.path.join(ROOT, "include", "smirk_b200.h")).read()
@@ -25,7 +27,7 @@ def test_library_exports_and_binds_every_declared_symbol(native_lib):
     assert native_lib.smk_version() == 100
     protos = re.findall(r"^\s*([A-Za-z_][\w ]*?\**)\s*\b(smk_\w+)\s*\(([^)]*)\)\s*;", hdr, flags=re.M)
     table = {name: (restype, args) for name, restype, args in _lib.BINDINGS}
-    assert len(protos) == 57 and len(table) == len(_lib.BINDINGS)
+    assert len(protos) == 70 and len(table) == len(_lib.BINDINGS)
     assert {name for _, name, _ in protos} == set(table)
     returns = {"int": C.c_int, "size_t": C.c_size_t, "void": None, "const char*": C.c_char_p, "unsigned long long": C.c_ulonglong}
     values = {"int": C.c_int, "size_t": C.c_size_t, "float": C.c_float}
@@ -41,6 +43,7 @@ def test_library_exports_and_binds_every_declared_symbol(native_lib):
                 assert a in (C.c_void_p, C.c_char_p) or issubclass(a, C._Pointer), (name, q)
             else:
                 assert a is values[q.rsplit(None, 1)[0]], (name, q)
+        assert (name in _lib._TAKES_STREAM) == (args[-1:] == [_lib.STREAM]), name
 
 
 def test_create_rejects_bad_arguments_without_gpu(native_lib):

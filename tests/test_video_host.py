@@ -1,9 +1,7 @@
-"""CPU suite of the video stage (smirk_b200/video.py, include/smirk_b200_video.h): the header against
-_lib.VIDEO_BINDINGS, the byte round trip of the frame panel, the batched crop transforms against the one-frame helper, and
-the compose oracle (tests/video_ref.py) against a literal restatement of the video demo's per-frame grid."""
+"""CPU suite of the video stage (smirk_b200/video.py, smk_hull_mask / smk_video_* in include/smirk_b200.h): argument
+checking of the entry points, the byte round trip of the frame panel, the batched crop transforms against the one-frame
+helper, and the compose oracle (tests/video_ref.py) against a literal restatement of the video demo's per-frame grid."""
 import ctypes as C
-import os
-import re
 
 import numpy as np
 import pytest
@@ -12,44 +10,11 @@ import torch
 from smirk_b200 import crop, video
 import video_ref
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
 
 def _landmarks(rng, B, H=1080, W=1920, L=478):
     c = np.stack([rng.uniform(0.1 * W, 0.9 * W, B), rng.uniform(0.1 * H, 0.9 * H, B)], 1)[:, None]
     lm = c + rng.normal(0, 1, (B, L, 2)) * rng.uniform(10, 250, (B, 1, 1))
     return np.concatenate([lm, rng.normal(0, 1, (B, L, 1))], 2)                          # mediapipe's third (z) column
-
-
-def test_video_header_and_binding_table_agree(native_lib):
-    """include/smirk_b200_video.h is included by smirk_b200.h after smirk_b200_encoder_grad.h, and each of its prototypes
-    has one row in _lib.VIDEO_BINDINGS with the same return type, parameter count, pointer / value kinds and trailing
-    stream."""
-    from smirk_b200 import _lib
-    main = open(os.path.join(ROOT, "include", "smirk_b200.h")).read()
-    assert main.index('#include "smirk_b200_encoder_grad.h"') < main.index('#include "smirk_b200_video.h"')
-    hdr = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "smirk_b200_video.h")).read(), flags=re.S)
-    protos = re.findall(r"^\s*([A-Za-z_][\w ]*?\**)\s*\b(smk_\w+)\s*\(([^)]*)\)\s*;", hdr, flags=re.M)
-    table = {name: (restype, args) for name, restype, args in _lib.VIDEO_BINDINGS}
-    assert len(protos) == len(table) == len(_lib.VIDEO_BINDINGS) == 3
-    assert {name for _, name, _ in protos} == set(table)
-    assert not set(table) & {name for name, _, _ in _lib.BINDINGS + _lib.GRAD_BINDINGS + _lib.ENCODER_GRAD_BINDINGS}
-    assert native_lib.smk_version() == 100
-    types = {"int": C.c_int, "size_t": C.c_size_t}
-    for ret, name, params in protos:
-        assert hasattr(native_lib, name), name
-        restype, args = table[name]
-        assert restype is types[ret.strip()], name
-        params = [q.strip() for q in params.split(",") if q.strip()]
-        assert len(args) == len(params), name
-        for q, a in zip(params, args):
-            if q.endswith("stream"):
-                assert a is _lib.STREAM, (name, q)
-            elif "*" in q:
-                assert a in (C.c_void_p, C.c_char_p) or issubclass(a, C._Pointer), (name, q)
-            else:
-                assert a is types[q.rsplit(None, 1)[0]], (name, q)
-        assert (name in _lib._TAKES_STREAM) == (args[-1:] == [_lib.STREAM])
 
 
 def test_video_compose_rejects_bad_arguments(native_lib):
