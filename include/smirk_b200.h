@@ -226,7 +226,9 @@ int smk_generator_backward(const SmkGenerator* h, int B, const float* y, const f
  * arithmetic, truncation to uint8 — skimage's `_warp_fast` semantics.  m / minv: [B][9] row-major float64 3x3
  * maps from OUTPUT pixel (col,row,1) to INPUT (x,y,1) (affine rows only); ws >= smk_warp_workspace_bytes(B).
  *   smk_crop_warp      : frames uint8 [B,H,W,3] -> out float32 [B,3,S,S] = uint8 result / 255; swap_rb reverses the
- *                        channel order (BGR frame -> RGB tensor).
+ *                        channel order (BGR frame -> RGB tensor).  minv == NULL: no crop transform, the uint8 result
+ *                        is cv2.resize(frame, (S, S)) with INTER_LINEAR bit for bit (demo_video.py:130-136 without
+ *                        --crop; an exact 2x on both axes is cv2's INTER_AREA fast path); one launch, ws unused.
  *   smk_warp_u8        : src uint8 [B,Hs,Ws,3] -> dst uint8 [B,Hd,Wd,3].
  *   smk_f32chw_to_u8hwc: (x * 255.0f).astype(uint8) of a [B,3,S,S] float image -> [B,S,S,3] (demo_video.py:148).  */
 size_t smk_warp_workspace_bytes(int B);
@@ -236,22 +238,29 @@ int smk_warp_u8(const uint8_t* src, int B, int Hs, int Ws, const double* m, int 
                 void* ws, size_t ws_bytes, void* stream);
 int smk_f32chw_to_u8hwc(const float* in, int B, int S, uint8_t* out, void* stream);
 
-/* The output grid of the video demo (demo_video.py --crop [--render_orig] [--use_smirk_generator]).  An empty batch
+/* The output grid of the video demo (demo_video.py [--crop] [--render_orig] [--use_smirk_generator]).  An empty batch
  * (B = 0) is a no-op.
  * create_mask(cropped_kpt, (S, S)) of the reference (datasets/base_dataset.py:9-15) for each frame: pts [B,L,2] int32
- * points in crop pixels (1 <= L <= 1024), mask [B,1,S,S] float, 0 inside cv2.convexHull(pts) filled by
- * cv2.fillConvexPoly (lineType 8, shift 0) and 1 outside, bit for bit (points outside the crop, repeated or collinear
- * points included); S <= 256. */
+ * points in crop pixels, or in frame pixels without --crop (1 <= L <= 1024), mask [B,1,S,S] float, 0 inside
+ * cv2.convexHull(pts) filled by cv2.fillConvexPoly (lineType 8, shift 0) and 1 outside, bit for bit (points outside the
+ * mask, negative ones, repeated or collinear points included); S <= 256. */
 int smk_hull_mask(const int32_t* pts, int B, int L, int S, float* mask, void* stream);
-/* Workspace of smk_video_compose with render_orig (the per-panel clip range); without render_orig none is needed. */
+/* Workspace of smk_video_compose with render_orig == 1 (the per-panel clip range); the other modes need none. */
 size_t smk_video_workspace_bytes(int B, int n_panels);
 /* grid [B, Hout, (n_panels + 1) * Wout, 3] uint8 BGR, one row of panels per frame: what demo_video.py:211-214 writes.
- *   render_orig != 0: Hout x Wout = H x W; panel 0 = frames [B,H,W,3] (BGR); panel k = panels[k-1] [B,3,S,S] (RGB in
- *                     [0,1]) converted to uint8 ((x * 255).astype(uint8)) and warped back to the frame with m [B,9]
- *                     (float64, row-major crop -> frame similarity, tform.params), skimage warp semantics; crop unused.
+ *   render_orig == 1: (--crop --render_orig) Hout x Wout = H x W; panel 0 = frames [B,H,W,3] (BGR); panel k =
+ *                     panels[k-1] [B,3,S,S] (RGB in [0,1]) converted to uint8 ((x * 255).astype(uint8)) and warped back
+ *                     to the frame with m [B,9] (float64, row-major crop -> frame similarity, tform.params), skimage
+ *                     warp semantics; crop unused.
+ *   render_orig == 2: (--render_orig without --crop) Hout x Wout = H x W; panel 0 = frames; panel k =
+ *                     (F.interpolate(panels[k-1], (H, W), mode='bilinear') * 255).astype(uint8): torch's
+ *                     upsample_bilinear2d with align_corners = False, float32 without fused multiply-adds, evaluated per
+ *                     output byte; crop, m and ws unused (may be NULL).
  *   render_orig == 0: Hout x Wout = S x S; panel 0 = crop [B,3,S,S] (the encoder's RGB input in [0,1]), panel k =
  *                     panels[k-1], both converted to uint8; frames and m unused (may be NULL).
- * panels: host array of n_panels (1 or 2) device pointers.  ws >= smk_video_workspace_bytes(B, n_panels) with render_orig. */
+ * Any other render_orig is an error.
+ * panels: host array of n_panels (1 or 2) device pointers.  ws >= smk_video_workspace_bytes(B, n_panels) with
+ * render_orig == 1. */
 int smk_video_compose(const uint8_t* frames, int B, int H, int W, const float* crop, const float* const* panels, int n_panels,
                       int S, const double* m, int render_orig, uint8_t* grid, void* ws, size_t ws_bytes, void* stream);
 

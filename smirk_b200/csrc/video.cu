@@ -1,13 +1,18 @@
-// Output grid of the reference's video demo with --crop (demo_video.py:139-150,171,199-213), for a batch of frames on the
-// device: one row per frame, the panels side by side, uint8 BGR — the bytes demo_video.py hands to cv2.VideoWriter.
+// Output grid of the reference's video demo (demo_video.py:139-160,171,198-213), for a batch of frames on the device: one
+// row per frame, the panels side by side, uint8 BGR — the bytes demo_video.py hands to cv2.VideoWriter.
 //
-//   panel 0        render_orig: the frame itself (its u8 -> RGB -> /255 -> *255 -> u8 -> BGR round trip is the identity)
-//                  otherwise:   the 224x224 crop, (crop * 255).astype(uint8) of the float crop the encoder read (identity
-//                               on crop_to_tensor's u8 / 255 values), channels back to BGR
+//   panel 0        render_orig (1 or 2): the frame itself (its u8 -> RGB -> /255 -> *255 -> u8 -> BGR round trip is the
+//                               identity)
+//                  otherwise:   the 224x224 crop or resize, (crop * 255).astype(uint8) of the float image the encoder read
+//                               (identity on u8 / 255 values), channels back to BGR
 //   panel 1 (, 2)  the rendered (and reconstructed) image [3,S,S] in [0,1]:
-//                  render_orig: warp((x * 255).astype(uint8) HWC, tform, (H, W), preserve_range=True).astype(uint8)
+//                  render_orig == 1 (--crop --render_orig):
+//                               warp((x * 255).astype(uint8) HWC, tform, (H, W), preserve_range=True).astype(uint8)
 //                               — skimage's bilinear sample of warp_sample.cuh, the float -> u8 conversion done per tap,
 //                               clipped to the min / max of the converted panel (a small reduction launch first)
+//                  render_orig == 2 (--render_orig without --crop):
+//                               (F.interpolate(x, (H, W), mode='bilinear') * 255).astype(uint8) — torch's bilinear sample
+//                               of resize_sample.cuh evaluated per output byte, so no resized float panel reaches HBM
 //                  otherwise:   (x * 255).astype(uint8)
 //                  channels RGB -> BGR.
 // One launch writes the whole grid; no u8 intermediate of a panel reaches HBM.  Each thread owns one 16-byte-aligned
@@ -16,6 +21,7 @@
 #include "common.cuh"
 #include "warp_sample.cuh"
 #include "hull_mask.cuh"
+#include "resize_sample.cuh"
 #include <float.h>
 
 namespace {
@@ -53,7 +59,8 @@ __global__ void __launch_bounds__(512) panel_minmax_kernel(const float* __restri
     }
 }
 
-// The three BGR bytes of grid pixel (y, px) of frame b.
+// The three BGR bytes of grid pixel (y, px) of frame b.  RESIZE: render_orig == 2 (the panels resized to the frame).
+template <bool RESIZE>
 __device__ __forceinline__ void grid_pixel(const ComposeArgs& a, int b, int y, int px, uint8_t v[3]) {
     const int p = px / a.Wo, x = px - p * a.Wo;
     const size_t SS = (size_t)a.S * a.S;
@@ -63,6 +70,15 @@ __device__ __forceinline__ void grid_pixel(const ComposeArgs& a, int b, int y, i
         return;
     }
     const float* src = (p == 0 ? a.crop : p == 1 ? a.p1 : a.p2) + (size_t)b * 3 * SS;
+    if (RESIZE) {
+        const smk::resize::Lerp h = smk::resize::bilinear_index(y, a.S, a.Ho), w = smk::resize::bilinear_index(x, a.S, a.Wo);
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch) {
+            const float* c = src + (2 - ch) * SS;
+            v[ch] = smk::unit_to_u8(smk::resize::torch_bilinear(h, w, a.S, [c](int i) { return __ldg(c + i); }));
+        }
+        return;
+    }
     if (p == 0 || !a.render_orig) {
 #pragma unroll
         for (int ch = 0; ch < 3; ++ch) v[ch] = smk::unit_to_u8(__ldg(src + (2 - ch) * SS + (size_t)y * a.S + x));
@@ -76,6 +92,8 @@ __device__ __forceinline__ void grid_pixel(const ComposeArgs& a, int b, int y, i
                            }, v);
 }
 
+// RESIZE = false serves render_orig 0 and 1, RESIZE = true render_orig 2.
+template <bool RESIZE>
 __global__ void __launch_bounds__(256) video_compose_kernel(const ComposeArgs a) {
     const int y = blockIdx.y, b = blockIdx.z;
     uint8_t* row = a.grid + ((size_t)b * a.Ho + y) * a.pitch;
@@ -89,7 +107,7 @@ __global__ void __launch_bounds__(256) video_compose_kernel(const ComposeArgs a)
     const int px0 = (int)(o0 / 3), px1 = (int)((o1 - 1) / 3);
     for (int px = px0; px <= px1; ++px) {
         uint8_t v[3];
-        grid_pixel(a, b, y, px, v);
+        grid_pixel<RESIZE>(a, b, y, px, v);
 #pragma unroll
         for (int ch = 0; ch < 3; ++ch) {
             const long long j = 3LL * px + ch - o0;
@@ -167,9 +185,15 @@ extern "C" int smk_video_compose(const uint8_t* frames, int B, int H, int W, con
     SMK_REQUIRE(panels && grid, "smk_video_compose: null argument");
     SMK_REQUIRE(H > 0 && W > 0 && S > 0 && (n_panels == 1 || n_panels == 2), "smk_video_compose: bad sizes");
     SMK_REQUIRE(panels[0] && (n_panels == 1 || panels[1]), "smk_video_compose: null panel");
-    SMK_REQUIRE(render_orig ? (frames && m) : (crop != nullptr), "smk_video_compose: render_orig needs frames and m, "
-                "otherwise the crop is needed");
-    SMK_REQUIRE(!render_orig || (ws && ws_bytes >= smk_video_workspace_bytes(B, n_panels)), "smk_video_compose: workspace too small");
+    SMK_REQUIRE(render_orig >= 0 && render_orig <= 2, "smk_video_compose: render_orig must be 0, 1 or 2");
+    const bool resize = render_orig == 2;
+    if (resize) {
+        SMK_REQUIRE(frames, "smk_video_compose: render_orig == 2 needs frames");
+    } else {
+        SMK_REQUIRE(render_orig ? (frames && m) : (crop != nullptr), "smk_video_compose: render_orig needs frames and m, "
+                    "otherwise the crop is needed");
+        SMK_REQUIRE(!render_orig || (ws && ws_bytes >= smk_video_workspace_bytes(B, n_panels)), "smk_video_compose: workspace too small");
+    }
     cudaStream_t st = (cudaStream_t)stream;
     ComposeArgs a;
     a.frames = frames; a.crop = crop; a.p1 = panels[0]; a.p2 = n_panels > 1 ? panels[1] : nullptr; a.m = m;
@@ -180,7 +204,7 @@ extern "C" int smk_video_compose(const uint8_t* frames, int B, int H, int W, con
     a.grid = grid;
     SMK_REQUIRE(a.Ho <= 65535 && B <= 65535, "smk_video_compose: too many rows or frames");
     const double panel_bytes = (double)B * n_panels * 3 * S * S * 4;
-    if (render_orig) {
+    if (render_orig == 1) {
         SMK_TAG("video_minmax", panel_bytes, 0.0, st);
         SMK_LAUNCH(panel_minmax_kernel, dim3(B * n_panels), dim3(512), 0, st, a.p1, a.p2, S, n_panels, reinterpret_cast<unsigned*>(ws));
         SMK_CHECK_LAUNCH();
@@ -189,7 +213,9 @@ extern "C" int smk_video_compose(const uint8_t* frames, int B, int H, int W, con
     const double read = render_orig ? (double)B * H * W * 3 + panel_bytes : (double)B * 3 * S * S * 4 + panel_bytes;
     SMK_TAG("video_compose", (double)B * a.Ho * a.pitch + read, 0.0, st);
     const long long nseg = a.pitch / 16 + 2;
-    SMK_LAUNCH(video_compose_kernel, dim3(smk::cdiv(nseg, 256), a.Ho, B), dim3(256), 0, st, a);
+    const dim3 grid_dim(smk::cdiv(nseg, 256), a.Ho, B);
+    if (resize) SMK_LAUNCH(video_compose_kernel<true>, grid_dim, dim3(256), 0, st, a);
+    else SMK_LAUNCH(video_compose_kernel<false>, grid_dim, dim3(256), 0, st, a);
     SMK_CHECK_LAUNCH();
     return 0;
 }

@@ -7,7 +7,8 @@
 //   demo_video.py:148-149            rendered -> (x * 255).astype(uint8) -> warp(rendered, tform, output_shape=(H, W),
 //                                              preserve_range=True).astype(np.uint8)
 // The reference does this on the CPU per frame (skimage's Cython `_warp_fast`) between a D2H and an H2D copy; here
-// it is one gather-bilinear pass per direction.
+// it is one gather-bilinear pass per direction.  Without a crop (demo_video.py:130-136 without --crop) smk_crop_warp
+// resizes the whole frame with cv2.resize's rule instead (resize_sample.cuh).
 //
 // Arithmetic follows skimage 0.2x `_warp_fast` / `bilinear_interpolation` / `_clip_warp_output` for order = 1,
 // mode = 'constant', cval = 0, clip = True, evaluated in float64 like the reference (preserve_range=True converts
@@ -22,6 +23,7 @@
 // HBM traffic: the gather touches each source texel it needs once through L2; output 150 KB (crop) or H*W*3 (back).
 #include "common.cuh"
 #include "warp_sample.cuh"
+#include "resize_sample.cuh"
 #include <math.h>
 #include <algorithm>
 
@@ -94,6 +96,20 @@ warp_bilinear_kernel(const uint8_t* __restrict__ src, int Hs, int Ws, const doub
     }
 }
 
+// cv2.resize(frame, (S, S)) of whole frames (demo_video.py:134-136 without --crop): one thread per output pixel, float
+// [B,3,S,S] = uint8 result / 255, channels reversed when swap_rb.
+__global__ void __launch_bounds__(256)
+resize_kernel(const uint8_t* __restrict__ src, int H, int W, int S, int swap_rb, float* __restrict__ dst) {
+    const int b = blockIdx.z;
+    const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);
+    if (x >= S || y >= S) return;
+    uint8_t res[3];
+    smk::resize::cv2_resize3(src + (size_t)b * H * W * 3, H, W, S, x, y, res);
+    float* o = dst + (size_t)b * 3 * S * S + (size_t)y * S + x;
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) o[(size_t)(swap_rb ? 2 - ch : ch) * S * S] = __fdiv_rn((float)res[ch], 255.0f);
+}
+
 int launch_warp(const uint8_t* src, int B, int Hs, int Ws, const double* M, int Hd, int Wd, bool out_f32, int swap_rb, void* dst,
                 void* ws, size_t ws_bytes, cudaStream_t st) {
     SMK_REQUIRE(ws && ws_bytes >= (size_t)B * sizeof(MinMax), "warp: workspace too small");
@@ -120,8 +136,17 @@ extern "C" size_t smk_warp_workspace_bytes(int B) { return smk::ws_round((size_t
 extern "C" int smk_crop_warp(const uint8_t* frames, int B, int H, int W, const double* minv, int S, int swap_rb, float* out,
                              void* ws, size_t ws_bytes, void* stream) {
     if (B == 0) return 0;
-    SMK_REQUIRE(frames && minv && out, "smk_crop_warp: null argument");
+    SMK_REQUIRE(frames && out, "smk_crop_warp: null argument");
     SMK_REQUIRE(B > 0 && H > 0 && W > 0 && S > 0, "smk_crop_warp: bad sizes");
+    if (!minv) {                                    // no crop transform: cv2.resize of the whole frame, no workspace
+        SMK_REQUIRE(B <= 65535, "smk_crop_warp: too many frames");
+        cudaStream_t st = (cudaStream_t)stream;
+        // algorithmic bytes: the output, and the four 3-byte taps of each output pixel (at most the whole frame)
+        SMK_TAG("resize", (double)B * S * S * 12.0 + (double)B * std::min((double)H * W * 3, (double)S * S * 12), 0.0, st);
+        SMK_LAUNCH(resize_kernel, dim3(smk::cdiv(S, 32), smk::cdiv(S, 8), B), dim3(256), 0, st, frames, H, W, S, swap_rb ? 1 : 0, out);
+        SMK_CHECK_LAUNCH();
+        return 0;
+    }
     return launch_warp(frames, B, H, W, minv, S, S, true, swap_rb ? 1 : 0, out, ws, ws_bytes, (cudaStream_t)stream);
 }
 

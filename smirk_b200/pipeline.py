@@ -163,28 +163,38 @@ class SmirkPipeline:
     @torch.no_grad()
     def forward(self, img, masked_img=None, lane=0):
         if self.video is not None:                  # img = uint8 frames, masked_img = the VideoBatch
-            self.video.check(img, masked_img)
+            self._check_video(img, masked_img)
             aux = [masked_img[k].to(img.device, non_blocking=True) for k in self._video_keys()]
             return self._forward_video(img, aux, lane)
         return self._forward(self._lane(lane), img, masked_img)
 
     def _forward_video(self, frames, aux, lane):
-        """Crop, the hot path, the output grid (smirk_b200/video.py); aux = the device tensors of ``_video_keys()``: crop /
-        back matrices [B,9] (+ the int32 crop landmarks [B,L,2] with a generator)."""
+        """Crop (or resize), the hot path, the output grid (smirk_b200/video.py); aux = the device tensors of
+        ``_video_keys()``, in that order: crop / back matrices [B,9] with the crop, the int32 landmarks [B,L,2] with a
+        generator."""
         L = self._lane(lane)
-        img = L.video.crop(frames, aux[0])
-        hull = L.video.hull_mask(aux[2]) if L.generator is not None else None
+        aux = dict(zip(self._video_keys(), aux))
+        img = L.video.crop(frames, aux.get("crop_m"))
+        hull = L.video.hull_mask(aux["kpt"]) if L.generator is not None else None
         out = self._forward(L, img, hull)
         out["cropped_img"] = img
         panels = [out["rendered_img"]]
         if hull is not None:
             out["hull_mask"] = hull
             panels.append(out["reconstructed_img"])
-        out["grid"] = L.video.compose(frames, img, panels, aux[1])
+        out["grid"] = L.video.compose(frames, img, panels, aux.get("back_m"))
         return out
 
     def _video_keys(self):
-        return ("crop_m", "back_m", "kpt") if self.generator is not None else ("crop_m", "back_m")
+        keys = ("crop_m", "back_m") if self.video.use_crop else ()
+        return keys + ("kpt",) if self.generator is not None else keys
+
+    def _check_video(self, frames, batch):
+        self.video.check(frames, batch)
+        missing = [k for k in self._video_keys() if k not in batch]
+        if missing:
+            raise ValueError("SmirkPipeline: the VideoBatch lacks %s (the generator's hull mask needs the landmarks: "
+                             "VideoStage.prepare(landmarks))" % ", ".join(missing))
 
     def _forward(self, L, img, masked_img):
         p = L.encoder(img)
@@ -219,11 +229,11 @@ class SmirkPipeline:
         static_mask = None                                  # the video stage draws its hull mask inside the graph
         if self.generator is not None and self.video is None:
             static_mask = torch.zeros(B, 1 if self.masking is not None else 3, 224, 224, device=dev)
-        if self.video is not None:                          # frames + the two [B,9] matrices of the VideoBatch
+        if self.video is not None:                          # frames + the tensors of the VideoBatch
             static_in = torch.zeros((B,) + self.video.frame_hw + (3,), dtype=torch.uint8, device=dev)
-            static_aux = [torch.zeros(B, 9, dtype=torch.float64, device=dev) for _ in range(2)]
-            if self.generator is not None:
-                static_aux.append(torch.zeros(B, self.video.L, 2, dtype=torch.int32, device=dev))
+            shapes = {"crop_m": ((B, 9), torch.float64), "back_m": ((B, 9), torch.float64),
+                      "kpt": ((B, self.video.L, 2), torch.int32)}
+            static_aux = [torch.zeros(shapes[k][0], dtype=shapes[k][1], device=dev) for k in self._video_keys()]
             run = lambda: self._forward_video(static_in, static_aux, lane)
         else:
             static_in = torch.zeros(B, 3, 224, 224, device=dev)
@@ -252,7 +262,7 @@ class SmirkPipeline:
     def replay(self, img, masked_img=None):
         """Lane 0, caller's stream: copy the inputs into the graph's static buffers and replay."""
         if self.video is not None:
-            self.video.check(img, masked_img)
+            self._check_video(img, masked_img)
         rec = self.capture(img.shape[0])
         rec["img"].copy_(img, non_blocking=True)
         if rec["mask"] is not None:
@@ -268,7 +278,7 @@ class SmirkPipeline:
         until that lane is used again; call ``join()`` before reading them from the caller's stream."""
         lane = i % self.slots
         if self.video is not None:
-            self.video.check(img, masked_img)
+            self._check_video(img, masked_img)
         rec = self.capture(img.shape[0], lane)
         L = self._lanes[lane]
         cur = torch.cuda.current_stream(self.device)
@@ -495,7 +505,7 @@ class SmirkPipeline:
         before reading it."""
         B = img_pinned.shape[0]
         if self.video is not None:
-            self.video.check(img_pinned, masked_pinned)
+            self._check_video(img_pinned, masked_pinned)
         lane = i % self.slots
         hb = self.host_buffers(B, lane, keys)
         rec = self.capture(B, lane)

@@ -1,4 +1,4 @@
-"""The frame loop of the reference's video demo (``demo_video.py:107-214`` with ``--crop``) as a stage of ``SmirkPipeline``.
+"""The frame loop of the reference's video demo (``demo_video.py:107-214``) as a stage of ``SmirkPipeline``.
 
     stage = VideoStage(frame_hw=(1080, 1920), render_orig=True)        # demo_video.py --crop [--render_orig]
     pipe  = SmirkPipeline(enc, flame, renderer, video=stage, slots=2)
@@ -6,6 +6,9 @@
     out   = pipe.forward(frames_u8_cuda, batch)            # eager
     out   = pipe.submit(i, frames_u8_cuda, batch)          # graph replay on lane i % slots
     out   = pipe.run_host(frames_pinned, i, batch, keys=("grid",))
+
+    stage = VideoStage((512, 512), render_orig=True, crop=False)       # demo_video.py [--render_orig] without --crop
+    batch = stage.prepare(batch_size=B)       # or stage.prepare(landmarks) with a generator (the hull mask's points)
 
 Per batch of uint8 BGR frames [B,H,W,3] on the device the pipeline crops (``smk_crop_warp``: ``warp(image,
 tform.inverse, (224, 224))`` + BGR2RGB + /255), runs encoder -> FLAME -> renderer, and writes ``out["grid"]``, uint8 BGR
@@ -15,8 +18,13 @@ With a generator (``--use_smirk_generator``, which needs ``masking=MaskingStage(
 ``datasets/base_dataset.py:9-15`` is drawn on the device (``smk_hull_mask``) from the int32 crop landmarks, goes through
 the masking step into the generator, and the reconstruction is the third panel.  The crop transforms and landmarks are
 graph inputs, so one captured graph per (B, H, W) serves every batch.  The landmark detector and the video decode /
-encode stay on the host, as in the reference.  The reference's branch without ``--crop`` (a resize of the whole frame)
-is not provided.
+encode stay on the host, as in the reference.
+
+Without ``--crop`` (``crop=False``; the reference's branch for face-aligned clips) the encoder reads
+``cv2.resize(frame, (224, 224))`` (``smk_crop_warp`` without a matrix, bit for bit), and with ``render_orig`` each render
+panel is ``F.interpolate(x, (H, W), mode='bilinear')`` of the reference (``smk_video_compose`` mode 2).  The hull mask
+is drawn from the landmarks in frame pixels as the reference does (``create_mask(kpt, (224, 224))``: points outside the
+224 x 224 mask are clipped there, not rescaled), and the batch holds no transforms.
 """
 import numpy as np
 import torch
@@ -72,30 +80,32 @@ def crop_landmarks(landmarks, T):
 
 
 class VideoBatch(dict):
-    """The host side of one batch (``VideoStage.prepare``): ``crop_m`` / ``back_m``, pinned float64 [B,9], the maps
-    crop -> frame (inverse of the transform; what the crop warp samples with) and frame -> crop (``tform.params``; what
-    the warp back to the frame samples with); ``kpt``, pinned int32 [B,L,2], the landmarks in crop pixels (the hull
-    mask's input)."""
+    """The host side of one batch of ``size`` frames (``VideoStage.prepare``): ``crop_m`` / ``back_m``, pinned float64
+    [B,9], the maps crop -> frame (inverse of the transform; what the crop warp samples with) and frame -> crop
+    (``tform.params``; what the warp back to the frame samples with); ``kpt``, pinned int32 [B,L,2], the landmarks in
+    crop pixels (the hull mask's input).  Without the crop only ``kpt`` (in frame pixels), or nothing."""
 
-    @property
-    def size(self):
-        return int(self["crop_m"].shape[0])
+    def __init__(self, size, **tensors):
+        super().__init__(**tensors)
+        self.size = int(size)
 
 
 class VideoStage:
-    """Configuration and workspaces of the video stage; attach it with ``SmirkPipeline(..., video=stage)``."""
+    """Configuration and workspaces of the video stage; attach it with ``SmirkPipeline(..., video=stage)``.
+    ``crop=False``: the reference's branch without ``--crop``, the whole frame resized to the encoder's input."""
 
-    def __init__(self, frame_hw, render_orig=False, scale=1.4, image_size=224, n_landmarks=478):
+    def __init__(self, frame_hw, render_orig=False, scale=1.4, image_size=224, n_landmarks=478, crop=True):
         self.frame_hw = (int(frame_hw[0]), int(frame_hw[1]))
         if min(self.frame_hw) <= 0:
             raise ValueError("frame_hw must be positive")
         self.render_orig, self.scale, self.S, self.L = bool(render_orig), float(scale), int(image_size), int(n_landmarks)
+        self.use_crop = bool(crop)
         if not 1 <= self.L <= 1024:
             raise ValueError("n_landmarks must be in [1, 1024]")
         self._ws = {}
 
     def __deepcopy__(self, memo):
-        new = VideoStage(self.frame_hw, self.render_orig, self.scale, self.S, self.L)
+        new = VideoStage(self.frame_hw, self.render_orig, self.scale, self.S, self.L, self.use_crop)
         memo[id(self)] = new
         return new
 
@@ -108,15 +118,28 @@ class VideoStage:
         return (B, Ho, (n_panels + 1) * Wo, 3)
 
     # ---- host ------------------------------------------------------------------------------------------------------------
-    def prepare(self, landmarks):
-        """[B,L,2|3] landmarks (mediapipe's, in frame pixels) -> ``VideoBatch`` of pinned host tensors."""
+    def prepare(self, landmarks=None, batch_size=None):
+        """[B,L,2|3] landmarks (mediapipe's, in frame pixels) -> ``VideoBatch`` of pinned host tensors.  Without the crop
+        the landmarks are only the hull mask's input (``kpt = landmarks.astype(np.int32)[..., :2]``, demo_video.py:131,171);
+        a pipeline without a generator needs none: ``prepare(batch_size=B)`` gives an empty batch of B frames."""
+        if landmarks is None:
+            if self.use_crop:
+                raise ValueError("VideoStage: the crop needs landmarks")
+            if batch_size is None or int(batch_size) < 0:
+                raise ValueError("VideoStage: without landmarks give batch_size >= 0")
+            return VideoBatch(batch_size)
         lm = np.asarray(landmarks)
         if lm.ndim != 3 or lm.shape[1] != self.L:
             raise ValueError("VideoStage: expected landmarks [B,%d,2|3], got %s" % (self.L, lm.shape))
-        T = box_transforms(lm, self.scale, self.S)
+        if batch_size is not None and int(batch_size) != lm.shape[0]:
+            raise ValueError("VideoStage: batch_size %d but %d landmark sets" % (batch_size, lm.shape[0]))
         cuda = torch.cuda.is_available()             # page-locked memory needs the driver; a host without one gets plain tensors
         pin = lambda a: (lambda t: t.pin_memory() if cuda else t)(torch.from_numpy(np.ascontiguousarray(a)))
-        return VideoBatch(crop_m=pin(np.linalg.inv(T).reshape(-1, 9)), back_m=pin(T.reshape(-1, 9)), kpt=pin(crop_landmarks(lm, T)))
+        if not self.use_crop:
+            return VideoBatch(lm.shape[0], kpt=pin(lm.astype(np.int32)[..., :2]))
+        T = box_transforms(lm, self.scale, self.S)
+        return VideoBatch(lm.shape[0], crop_m=pin(np.linalg.inv(T).reshape(-1, 9)), back_m=pin(T.reshape(-1, 9)),
+                          kpt=pin(crop_landmarks(lm, T)))
 
     def check(self, frames, batch):
         if not (torch.is_tensor(frames) and frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[3] == 3):
@@ -134,17 +157,21 @@ class VideoStage:
         return self._ws.setdefault(name, _lib.Workspace()).get(nbytes, device)
 
     def crop(self, frames, crop_m):
-        """frames uint8 [B,H,W,3] BGR, crop_m float64 [B,9] on the device -> the encoder's input, float32 [B,3,S,S] RGB."""
+        """frames uint8 [B,H,W,3] BGR, crop_m float64 [B,9] on the device -> the encoder's input, float32 [B,3,S,S] RGB.
+        Without the crop (crop_m unused) the input is cv2.resize of the whole frame."""
         dev = frames.device
         B, H, W, _ = frames.shape
         out = torch.empty(B, 3, self.S, self.S, dtype=torch.float32, device=dev)
-        if B:
+        if B and not self.use_crop:
+            _lib.call("smk_crop_warp", dev, frames, B, H, W, None, self.S, 1, out, None, 0)
+        elif B:
             ws = self._workspace("crop", _lib.call("smk_warp_workspace_bytes", dev, B), dev)
             _lib.call("smk_crop_warp", dev, frames, B, H, W, crop_m, self.S, 1, out, ws, ws.numel())
         return out
 
     def hull_mask(self, kpt):
-        """kpt int32 [B,L,2] crop landmarks on the device -> create_mask(kpt, (S, S)) as float [B,1,S,S]."""
+        """kpt int32 [B,L,2] crop landmarks (frame landmarks without the crop) on the device -> create_mask(kpt, (S, S))
+        as float [B,1,S,S]."""
         dev = kpt.device
         B = kpt.shape[0]
         mask = torch.empty(B, 1, self.S, self.S, dtype=torch.float32, device=dev)
@@ -153,14 +180,19 @@ class VideoStage:
         return mask
 
     def compose(self, frames, crop, panels, back_m):
-        """The output grid: panel 0 = the frame (render_orig) or the crop, then each of ``panels`` ([B,3,S,S] in [0,1])."""
+        """The output grid: panel 0 = the frame (render_orig) or the crop, then each of ``panels`` ([B,3,S,S] in [0,1])
+        warped back (or, without the crop, resized) to the frame with render_orig."""
         import ctypes as C
         dev = frames.device
         B, H, W, _ = frames.shape
         panels = [p.contiguous() for p in panels]
         grid = torch.empty(self.grid_shape(B, len(panels)), dtype=torch.uint8, device=dev)
-        if B:
-            ptrs = (C.c_void_p * len(panels))(*[p.data_ptr() for p in panels])
+        if not B:
+            return grid
+        ptrs = (C.c_void_p * len(panels))(*[p.data_ptr() for p in panels])
+        if self.render_orig and not self.use_crop:              # mode 2: the panels resized to the frame, no workspace
+            _lib.call("smk_video_compose", dev, frames, B, H, W, None, ptrs, len(panels), self.S, None, 2, grid, None, 0)
+        else:
             ws = self._workspace("compose", _lib.call("smk_video_workspace_bytes", dev, B, len(panels)), dev)
             _lib.call("smk_video_compose", dev, frames, B, H, W, None if self.render_orig else crop, ptrs, len(panels),
                       self.S, back_m if self.render_orig else None, 1 if self.render_orig else 0, grid, ws, ws.numel())

@@ -1,5 +1,5 @@
-"""configs[3]: the video demo's frame loop (demo_video.py --crop [--render_orig] [--use_smirk_generator]) at 1080p, batch 64 frames per step,
-frame-sharded over the GPUs of a torchrun job (``shard_bounds``; each rank keeps its grids, no all-gather: their consumer
+"""configs[3]: the video demo's frame loop (demo_video.py [--crop] [--render_orig] [--use_smirk_generator]) at 1080p (or --frame-hw),
+batch 64 frames per step, frame-sharded over the GPUs of a torchrun job (``shard_bounds``; each rank keeps its grids, no all-gather: their consumer
 is the host video writer, and every GPU has its own PCIe link).  Prints one JSON line:
 
   device_fps     frames/s with the frames resident in HBM: graph replay over the lanes, CUDA events around exactly
@@ -9,9 +9,10 @@ is the host video writer, and every GPU has its own PCIe link).  Prints one JSON
                  the crop warp (warp_minmax + warp_bilinear) from their algorithmic bytes
   gpu            card name, power limit and SM clocks read in the same run (read-only nvidia-smi queries)
   cpu_baseline   the reference's per-frame loop on the host cores over --cpu-frames frames: crop and warp back with the
-                 scikit-image restatement (oracle/warp_ref.py), the oracle port of encoder -> FLAME -> renderer, the grid
+                 scikit-image restatement (oracle/warp_ref.py), or without the crop cv2.resize and torch's CPU F.interpolate;
+                 the oracle port of encoder -> FLAME -> renderer, the grid
 
-    python tools/bench_video.py [--render-orig] [--generator]
+    python tools/bench_video.py [--render-orig] [--generator] [--no-crop] [--frame-hw 512x512]
     torchrun --nproc-per-node 2 tools/bench_video.py [--render-orig] [--generator]
 
 The CPU baseline covers the loop without the generator (its hull mask and masking step are not timed there).
@@ -34,16 +35,16 @@ import smirk_b200  # noqa: E402
 from smirk_b200 import _lib, synth_assets, synth_inputs, video  # noqa: E402
 from smirk_b200.pipeline import SmirkPipeline, shard_bounds  # noqa: E402
 
-H, W = 1080, 1920
+
+def landmarks(rng, B, H, W):
+    """Face-sized landmark clouds, placed as in a 1080 x 1920 frame scaled to H x W."""
+    c = np.stack([rng.uniform(W * 500 / 1920, W * 1420 / 1920, B), rng.uniform(H * 300 / 1080, H * 780 / 1080, B)], 1)[:, None]
+    return c + rng.normal(0, 1, (B, 478, 2)) * rng.uniform(40, 110, (B, 1, 1)) * (min(H, W) / 1080)
 
 
-def landmarks(rng, B):
-    c = np.stack([rng.uniform(500, 1420, B), rng.uniform(300, 780, B)], 1)[:, None]
-    return c + rng.normal(0, 1, (B, 478, 2)) * rng.uniform(40, 110, (B, 1, 1))
-
-
-def cpu_baseline(root, frames, lm, render_orig):
+def cpu_baseline(root, frames, lm, render_orig, crop):
     """The reference's per-frame loop (demo_video.py:121-213) on the host: seconds per frame."""
+    import torch.nn.functional as F
     from oracle import warp_ref, encoder_ref, flame_ref, render_ref
     st = bench._CPU_STATE
     if "enc_sd" not in st:
@@ -51,15 +52,22 @@ def cpu_baseline(root, frames, lm, render_orig):
         st["fc"], st["rc"] = flame_ref.FlameConstants(root), render_ref.RenderConstants(root)
     t0 = time.perf_counter()
     for f, l in zip(frames, lm):
-        T = warp_ref.crop_face_ref(f.shape, l, 1.4, 224)
-        c = warp_ref.warp_ref(f, np.linalg.inv(T), (224, 224))
+        if crop:
+            T = warp_ref.crop_face_ref(f.shape, l, 1.4, 224)
+            c = warp_ref.warp_ref(f, np.linalg.inv(T), (224, 224))
+        else:
+            import cv2
+            c = cv2.resize(cv2.cvtColor(f, cv2.COLOR_BGR2RGB), (224, 224))[..., ::-1]
         img = torch.from_numpy(np.ascontiguousarray(c[..., ::-1].transpose(2, 0, 1)))[None].float() / 255.0
         with torch.no_grad():
             p = {k: v for k, v in encoder_ref.encoder_forward_ref(st["enc_sd"], img).items() if not k.startswith("_")}
             fo = flame_ref.flame_forward_ref(st["fc"], p)
             r = render_ref.render_forward_ref(st["rc"], fo["vertices"], p["cam"], landmarks_fan=fo["landmarks_fan"],
                                               landmarks_mp=fo["landmarks_mp"])["rendered_img"][0].numpy()
-        if render_orig:
+        if render_orig and not crop:
+            up = F.interpolate(torch.from_numpy(r)[None], f.shape[:2], mode='bilinear')[0].numpy()
+            np.concatenate([f, ((up.transpose(1, 2, 0) * np.float32(255.0)).astype(np.uint8))[..., ::-1]], 1)
+        elif render_orig:
             np.concatenate([f, warp_ref.warp_back_ref(r, T, f.shape[:2])[..., ::-1]], 1)
         else:
             np.concatenate([c, ((r.transpose(1, 2, 0) * np.float32(255.0)).astype(np.uint8))[..., ::-1]], 1)
@@ -74,8 +82,11 @@ def main():
     ap.add_argument("--slots", type=int, default=2)
     ap.add_argument("--render-orig", action="store_true")
     ap.add_argument("--generator", action="store_true", help="--use_smirk_generator: hull mask, masking step, generator panel")
+    ap.add_argument("--no-crop", action="store_true", help="demo_video.py without --crop: the whole frame resized")
+    ap.add_argument("--frame-hw", default="1080x1920", help="frame height x width, e.g. 512x512 for pre-cropped clips")
     ap.add_argument("--cpu-frames", type=int, default=2)
     a = ap.parse_args()
+    H, W = (int(v) for v in a.frame_hw.lower().split("x"))
     world, rank = int(os.environ.get("WORLD_SIZE", "1")), int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     dist = None
@@ -92,7 +103,7 @@ def main():
     enc.load_state_dict(synth_inputs.random_state_dict(enc.state_dict(), seed=7))
     enc = enc.eval().to(dev)
     enc.precision = 3
-    stage = video.VideoStage((H, W), render_orig=a.render_orig)
+    stage = video.VideoStage((H, W), render_orig=a.render_orig, crop=not a.no_crop)
     fl = smirk_b200.FLAME().to(dev)
     gen = masking = None
     if a.generator:
@@ -105,9 +116,9 @@ def main():
     pipe = SmirkPipeline(enc, fl, smirk_b200.Renderer().to(dev), gen, device=dev, slots=a.slots, masking=masking, video=stage)
     rng = np.random.default_rng(100 + rank)
     host = [torch.from_numpy(rng.integers(0, 256, (B, H, W, 3), dtype=np.uint8)).pin_memory() for _ in range(2)]
-    lms = [landmarks(rng, B) for _ in range(2)]
-    batches = [stage.prepare(l) for l in lms]
-    frames = [h.to(dev) for h in host]                  # two 400 MB sets: nothing of a step is still in the 50 MB L2
+    lms = [landmarks(rng, B, H, W) for _ in range(2)]
+    batches = [stage.prepare(l) if (a.generator or not a.no_crop) else stage.prepare(batch_size=B) for l in lms]
+    frames = [h.to(dev) for h in host]                  # two 400 MB sets at 1080p: nothing of a step is still in the 50 MB L2
     for lane in range(pipe.slots):
         pipe.capture(B, lane)
 
@@ -156,10 +167,11 @@ def main():
     if rank == 0:
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", str(local)],
                            capture_output=True, text=True).stdout.strip()
-        cpu_s = cpu_baseline(root, [h.numpy() for h in host[0][:a.cpu_frames]], lms[0][:a.cpu_frames], a.render_orig)
+        cpu_s = cpu_baseline(root, [h.numpy() for h in host[0][:a.cpu_frames]], lms[0][:a.cpu_frames], a.render_orig, not a.no_crop)
         out = {
-            "workload": "configs[3]: demo_video.py --crop%s%s, %dx%d frames, batch %d (%d per GPU), %d GPU(s)"
-                        % (" --render_orig" if a.render_orig else "", " --use_smirk_generator" if a.generator else "",
+            "workload": "configs[3]: demo_video.py%s%s%s, %dx%d frames, batch %d (%d per GPU), %d GPU(s)"
+                        % ("" if a.no_crop else " --crop", " --render_orig" if a.render_orig else "",
+                           " --use_smirk_generator" if a.generator else "",
                            W, H, a.batch, B, world),
             "device_fps": round(a.batch * a.steps / ms_dev * 1e3, 1),
             "device_ms_per_step": round(ms_dev / a.steps, 3),
@@ -170,12 +182,13 @@ def main():
             "stages_rank0_eager": stages,
             "video_compose_gbs": gbs(["video_minmax", "video_compose"]),
             "hull_mask_ms": round(rep["hull_mask"]["ms"], 4) if "hull_mask" in rep else None,
-            "crop_warp_gbs": gbs(["warp_minmax", "warp_bilinear"]),
+            "crop_warp_gbs": gbs(["warp_minmax", "warp_bilinear", "resize"]),
             "gpu": {"name_power_limit": q, "clocks": clocks},
             "command": " ".join(sys.argv),
             "cpu_baseline": {"frames_per_s": round(1.0 / cpu_s, 3), "frames": a.cpu_frames, "cores": os.cpu_count(),
                              "threads": torch.get_num_threads(),
-                             "what": "oracle port (torch CPU) + warp_ref crop / warp back, one frame at a time"},
+                             "what": "oracle port (torch CPU) + %s, one frame at a time"
+                                     % ("cv2.resize / F.interpolate" if a.no_crop else "warp_ref crop / warp back")},
             "steps": a.steps, "warmup": a.warmup, "slots": a.slots,
         }
     if dist is not None:
