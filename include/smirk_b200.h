@@ -104,6 +104,9 @@ typedef struct {
     int n_faces;               /* 3408; must be < 65536 and a multiple of 4 (packed tile ranges are read 4 at a time) */
     const int32_t* faces;      /* [n_faces,3] indices into the sub-mesh (renderer.py:74) */
     int image_size;            /* 224 */
+    float z_offset;            /* added to the z of the returned tverts, 0 or 10: 0 for the face mask; 10 for the full head,
+                                  where the reference's in-place `z + 10` (renderer.py:140-144) lands in transformed_vertices.
+                                  The rasteriser's depth is z + 10 either way. */
 } SmkRendererDesc;
 
 int smk_renderer_create(const SmkRendererDesc* desc, SmkRenderer** out);

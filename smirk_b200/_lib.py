@@ -30,7 +30,7 @@ class SmkFlameDesc(C.Structure):
 
 class SmkRendererDesc(C.Structure):
     _fields_ = [("n_verts", C.c_int), ("n_mask", C.c_int), ("mask_ids", c_i32p), ("n_faces", C.c_int),
-                ("faces", c_i32p), ("image_size", C.c_int)]
+                ("faces", c_i32p), ("image_size", C.c_int), ("z_offset", C.c_float)]
 
 
 class SmkEncoderDesc(C.Structure):

@@ -41,7 +41,7 @@ __device__ __forceinline__ float pix_to_ndc(int i, int S) {
 
 // ---- vertex stage: util.batch_orth_proj + sign flips (renderer.py:101-102) ------------------------
 __global__ void __launch_bounds__(256)
-project_kernel(const float* __restrict__ pts, const float* __restrict__ cam, int B, int L, int out_dim,
+project_kernel(const float* __restrict__ pts, const float* __restrict__ cam, int B, int L, int out_dim, float z_offset,
                float* __restrict__ out) {
     long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long)B * L) return;
@@ -52,12 +52,15 @@ project_kernel(const float* __restrict__ pts, const float* __restrict__ cam, int
     float y = -__fmul_rn(s, __fadd_rn(p[1], ty));
     float* o = out + i * out_dim;
     o[0] = x; o[1] = y;
-    if (out_dim == 3) o[2] = -__fmul_rn(s, p[2]);
+    if (out_dim == 3) {
+        const float z = -__fmul_rn(s, p[2]);
+        o[2] = z_offset != 0.f ? __fadd_rn(z, z_offset) : z;     // no add at 0: keeps -0 as -0
+    }
 }
 
 // ---- masked sub-mesh: raster-space positions + vertex normals (util.py:30-62) ---------------------
 __global__ void __launch_bounds__(128)
-submesh_kernel(RenderDev d, const float* __restrict__ verts, const float* __restrict__ tverts, int B,
+submesh_kernel(RenderDev d, const float* __restrict__ verts, const float* __restrict__ tverts, float raster_dz, int B,
                float* __restrict__ rv /*[B][NM][3]*/, float* __restrict__ normals /*[B][NM][3]*/) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     int b = blockIdx.y;
@@ -65,8 +68,9 @@ submesh_kernel(RenderDev d, const float* __restrict__ verts, const float* __rest
     const float* vb = verts + (size_t)b * d.V * 3;
     const float* tv = tverts + ((size_t)b * d.V + d.mask_ids[i]) * 3;
     float* r = rv + ((size_t)b * d.NM + i) * 3;
-    // renderer.py:144 (z += 10) and :172-173 (negate x,y) -> pytorch3d NDC, +X left, +Y up
-    r[0] = -tv[0]; r[1] = -tv[1]; r[2] = __fadd_rn(tv[2], 10.0f);
+    // renderer.py:144 (z + 10) and :172-173 (negate x,y) -> pytorch3d NDC, +X left, +Y up.  raster_dz = 10 - z_offset:
+    // 10 for the face mask; 0 for the full head, whose tverts already carry the + 10 (tv[2] + 0 is tv[2]: never -0).
+    r[0] = -tv[0]; r[1] = -tv[1]; r[2] = __fadd_rn(tv[2], raster_dz);
     float nx = 0.f, ny = 0.f, nz = 0.f;
     for (int e = d.adj_ptr[i]; e < d.adj_ptr[i + 1]; ++e) {
         int code = d.adj[e], f = code >> 2, c = code & 3;
@@ -558,6 +562,7 @@ project_bwd_kernel(const float* __restrict__ pts, const float* __restrict__ cam,
 struct SmkRenderer {
     RenderDev d;
     Lights lights;
+    float z_offset;        // added to the returned tverts' z (SmkRendererDesc::z_offset)
     int32_t* inv_ptr;      // [V+1] CSR mesh vertex -> sub-mesh ids (the inverse of mask_ids), for the backward
     int32_t* inv;          // [NM]
     smk::DeviceArena arena;
@@ -569,9 +574,12 @@ extern "C" int smk_renderer_create(const SmkRendererDesc* desc, SmkRenderer** ou
                 desc->image_size / TILE_H < 255, "smk_renderer_create: image_size must be a multiple of 32 (got %d)", desc->image_size);
     SMK_REQUIRE(desc->n_faces > 0 && desc->n_faces < 65536 && desc->n_faces % 4 == 0,
                 "smk_renderer_create: n_faces must be in (0, 65536) and a multiple of 4 (got %d)", desc->n_faces);
+    SMK_REQUIRE(desc->z_offset == 0.f || desc->z_offset == 10.f,            // the raster depth tv.z + (10 - z_offset) is z + 10
+                "smk_renderer_create: z_offset must be 0 (face mask) or 10 (full head), got %g", (double)desc->z_offset);
     SmkRenderer* h = new SmkRenderer();
     RenderDev& d = h->d;
     d.V = desc->n_verts; d.NM = desc->n_mask; d.F = desc->n_faces; d.S = desc->image_size;
+    h->z_offset = desc->z_offset;
     for (int i = 0; i < d.NM; ++i)
         if (desc->mask_ids[i] < 0 || desc->mask_ids[i] >= d.V) { delete h; smk::set_error("smk_renderer_create: mask id out of range"); return -1; }
     for (int i = 0; i < d.F * 3; ++i)
@@ -624,7 +632,7 @@ extern "C" int smk_project_points(const float* pts, const float* cam, int B, int
     SMK_REQUIRE(pts && cam && out_xy, "smk_project_points: null argument");
     if (B <= 0 || L <= 0) return 0;
     SMK_TAG("project_points", 4.0 * B * (5.0 * L + 3), 4.0 * B * L, (cudaStream_t)stream);
-    SMK_LAUNCH(project_kernel, dim3(smk::cdiv((long)B * L, 256)), dim3(256), 0, (cudaStream_t)stream, pts, cam, B, L, 2, out_xy);
+    SMK_LAUNCH(project_kernel, dim3(smk::cdiv((long)B * L, 256)), dim3(256), 0, (cudaStream_t)stream, pts, cam, B, L, 2, 0.f, out_xy);
     SMK_CHECK_LAUNCH();
     return 0;
 }
@@ -645,10 +653,11 @@ extern "C" int smk_renderer_forward(const SmkRenderer* h, const float* verts, co
     uint32_t* ranges = w.take<uint32_t>((size_t)B * d.F);
     float* nrm = normals_out ? normals_out : nrm_ws;
     SMK_TAG("project_verts", 4.0 * B * (6.0 * d.V + 3), 5.0 * B * d.V, st);
-    SMK_LAUNCH(project_kernel, dim3(smk::cdiv((long)B * d.V, 256)), dim3(256), 0, st, verts, cam, B, d.V, 3, tverts);
+    SMK_LAUNCH(project_kernel, dim3(smk::cdiv((long)B * d.V, 256)), dim3(256), 0, st, verts, cam, B, d.V, 3, h->z_offset, tverts);
     SMK_CHECK_LAUNCH();
     SMK_TAG("submesh_normals", 4.0 * B * (9.0 * d.NM) + 4.0 * (4.0 * d.F + 2.0 * d.NM), 30.0 * B * 3.0 * d.F, st);
-    SMK_LAUNCH(submesh_kernel, dim3(dim3(smk::cdiv(d.NM, 128), B)), dim3(128), 0, st, d, verts, tverts, B, rv, nrm);
+    SMK_LAUNCH(submesh_kernel, dim3(dim3(smk::cdiv(d.NM, 128), B)), dim3(128), 0, st, d, verts, tverts, 10.0f - h->z_offset, B,
+               rv, nrm);
     SMK_CHECK_LAUNCH();
     SMK_TAG("tri_setup", 4.0 * B * (3.0 * d.NM + (double)d.F * (REC + 1)) + 12.0 * d.F, 40.0 * B * d.F, st);
     SMK_LAUNCH(tri_setup_kernel, dim3(dim3(smk::cdiv(d.F, 128), B)), dim3(128), 0, st, d, rv, B, recs, ranges);

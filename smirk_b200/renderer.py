@@ -91,6 +91,9 @@ class Renderer(_lib.NativeModule, nn.Module):
         d = _lib.SmkRendererDesc()
         d.n_verts, d.n_mask, d.mask_ids = self.n_verts, len(self.final_mask), mask_p
         d.n_faces, d.faces, d.image_size = faces_np.shape[0], faces_p, self.image_size
+        # renderer.py:140-144: with the full head the fancy-index is skipped, so the in-place `z + 10` of render()
+        # also lands in the tensor the reference returns as `transformed_vertices`
+        d.z_offset = 10.0 if self.render_full_head else 0.0
         return _lib.create("renderer", d, device)
 
     def forward(self, vertices, cam_params, **landmarks):
@@ -102,8 +105,6 @@ class Renderer(_lib.NativeModule, nn.Module):
     def _forward_autograd(self, vertices, cam_params, **landmarks):
         """forward() with gradients for vertices, cam_params and every landmark set (smk_renderer_backward,
         smk_project_points_backward).  Saves the rasteriser's pix_to_face, bary and the vertex normals."""
-        if self.render_full_head:
-            raise RuntimeError("smirk_b200.Renderer: gradients are not implemented for render_full_head=True")
         rendered, tverts = _RenderFunction.apply(self, vertices, cam_params)
         out = {"rendered_img": rendered, "transformed_vertices": tverts}
         for k, pts in landmarks.items():
@@ -134,10 +135,6 @@ class Renderer(_lib.NativeModule, nn.Module):
             xy = o(B, pts.shape[1], 2)
             _lib.call("smk_project_points", dev, pts, cam, B, pts.shape[1], xy)
             out[k] = xy
-        if self.render_full_head:
-            # renderer.py:140-144: with the full head the fancy-index is skipped, so the in-place `z += 10` of render()
-            # also lands in the tensor the reference returns as `transformed_vertices`
-            tverts[..., 2] += 10.0
         if raw:
             out.update(pix_to_face=p2f, bary=bary, zbuf=zbuf, normals=normals)
         return out
@@ -149,7 +146,8 @@ def _grad_f32(g):
 
 class _RenderFunction(torch.autograd.Function):
     """vertices, cam -> (rendered_img, transformed_vertices) through ``render_full(raw=True)``; the backward is
-    ``smk_renderer_backward`` from the saved pix_to_face / bary / normals."""
+    ``smk_renderer_backward`` from the saved pix_to_face / bary / normals.  Serves the face mask and the full head;
+    the full head's z offset on transformed_vertices is a constant, so its gradient passes through unchanged."""
 
     @staticmethod
     def forward(ctx, module, vertices, cam):
