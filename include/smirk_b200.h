@@ -372,4 +372,7 @@ int smk_debug_stem_ds(const float* img, int B, int H, int W, const float* stem_w
 }
 #endif
 
+/* SmirkEncoder train mode (batch-statistics BatchNorm and parameter gradients): include/smirk_b200_train.h. */
+#include "smirk_b200_train.h"
+
 #endif /* SMIRK_B200_H */

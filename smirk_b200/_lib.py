@@ -1,4 +1,4 @@
-"""ctypes binding of libsmirk_b200.so (the C ABI declared in include/smirk_b200.h).
+"""ctypes binding of libsmirk_b200.so (the C ABI declared in include/smirk_b200.h and include/smirk_b200_train.h).
 
 There is deliberately no fallback: if the shared library is missing or a call fails, the product
 path raises.  Build with ``python -m smirk_b200.build`` (or ``__graft_entry__.build()``).
@@ -37,6 +37,16 @@ class SmkEncoderDesc(C.Structure):
     _fields_ = [("tensors", C.POINTER(c_f32p) * 3), ("n_tensors", C.c_int * 3),
                 ("head_w", c_f32p * 3), ("head_b", c_f32p * 3),
                 ("n_shape", C.c_int), ("n_exp", C.c_int), ("precision", C.c_int)]
+
+
+class SmkEncoderTrainArgs(C.Structure):
+    _fields_ = [("tensors", C.POINTER(c_f32p) * 3), ("n_tensors", C.c_int * 3),
+                ("num_batches_tracked", C.POINTER(C.POINTER(C.c_int64)) * 3),
+                ("head_w", c_f32p * 3), ("head_b", c_f32p * 3), ("momentum", C.c_float * 3), ("eps", C.c_float * 3)]
+
+
+class SmkEncoderTrainGrads(C.Structure):
+    _fields_ = [("tensors", C.POINTER(c_f32p) * 3), ("head_w", c_f32p * 3), ("head_b", c_f32p * 3)]
 
 
 class SmkGeneratorDesc(C.Structure):
@@ -127,7 +137,15 @@ BINDINGS = [
     ("smk_debug_xdw3x", _i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _vp, STREAM]),
     ("smk_debug_stem_ds", _i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, STREAM]),
 ]
-_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS if args[-1:] == [STREAM])
+# The same for include/smirk_b200_train.h (SmirkEncoder train mode), in that header's order.
+TRAIN_BINDINGS = [
+    ("smk_encoder_train_create", _i, [_i, _i, _i, _i, _vpp]),
+    ("smk_encoder_train_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_encoder_forward_train", _i, [_vp, C.POINTER(SmkEncoderTrainArgs), _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp, _sz, STREAM]),
+    ("smk_encoder_backward_train", _i, [_vp, C.POINTER(SmkEncoderTrainArgs), _vp, _i, _vp, _sz, _vp, _vp, _vp, _vp,
+                                        C.POINTER(SmkEncoderTrainGrads), _vp, _sz, STREAM]),
+]
+_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS + TRAIN_BINDINGS if args[-1:] == [STREAM])
 
 
 def lib():
@@ -139,7 +157,7 @@ def lib():
         raise RuntimeError("smirk_b200: %s not found — build it with `python -m smirk_b200.build` "
                            "(there is no CPU / PyTorch fallback)" % LIB_PATH)
     L = C.CDLL(LIB_PATH)
-    for name, restype, argtypes in BINDINGS:
+    for name, restype, argtypes in BINDINGS + TRAIN_BINDINGS:
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, [_vp if a is STREAM else a for a in argtypes]
     if L.smk_version() != 100:
@@ -272,6 +290,7 @@ class NativeState:
 
     def __init__(self):
         self.handle, self.key, self.workspaces, self.per_device = None, None, {}, {}
+        self.train_handle, self.train_key = None, None        # the encoder's train-mode handle (topology only)
 
 
 class NativeModule:

@@ -25,7 +25,8 @@ def sources():
 def build(force=False, verbose=False):
     os.makedirs(OBJ, exist_ok=True)
     hdrs = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
-    hdrs.append(os.path.join(HERE, "..", "include", "smirk_b200.h"))
+    inc = os.path.join(HERE, "..", "include")
+    hdrs += [os.path.join(inc, f) for f in os.listdir(inc) if f.endswith(".h")]
     hdr_m = max(os.path.getmtime(h) for h in hdrs)
     objs, rebuilt = [], False
     for s in sources():

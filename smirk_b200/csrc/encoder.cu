@@ -13,6 +13,7 @@
 // `cn` ReLU), 1x1 dgrads as ordinary GEMMs over weights (diag(s) W)^T packed at create time (the folded BN scale rides in
 // the weights), a CUDA-core depthwise dgrad that applies both ReLU masks of its block, and one transposed stem conv that
 // sums the backbones' gradients into the NCHW image gradient.
+#include "encoder.cuh"
 #include "nn_kernels.cuh"
 #include "gemm_tc.cuh"
 #include "xdw_tc.cuh"
@@ -21,50 +22,12 @@
 
 namespace {
 
+using namespace enc;
 using smk::TensorCursor;
 using smk::grid_of;
 using smk::same_pad_begin;
 
 constexpr float kBnEps = 1e-3f;
-
-struct ConvW { float* w = nullptr; float* wt = nullptr; float* wt_lo = nullptr; float* scale = nullptr; float* bias = nullptr; int cin = 0, cout = 0; };   // w: [K][N] fp32 path, wt: [N][K] tensor-core path (TF32 heads), wt_lo: TF32 tails (3xTF32 path)
-enum Kind { DS = 0, IR = 1, CN = 2 };
-struct BlockDef { Kind kind; int stride; float exp; int cout; };
-// pw_f32: fp32 [K][N] copy of a DS block's 1x1 (fused stem path).  *_d: dgrad weights (see fold_conv).
-// sv_a / sv_b: saved-tensor indices of the block's ReLU outputs (IR: expand, depthwise; DS: depthwise; CN: its output).
-struct Block { Kind kind; int stride, cin, mid, cout; bool skip; ConvW pw, dw, pwl; ConvW pw_f32; ConvW pw_d, dw_d, pwl_d; int sv_a = -1, sv_b = -1; };
-
-struct Backbone {
-    ConvW stem, stem_d;
-    std::vector<Block> blocks;
-    int feat = 0;
-    float *head_w = nullptr, *head_b = nullptr;
-    int n_out = 0;
-    uint8_t* codes = nullptr;
-    int sv_stem = -1, sv_head = -1;
-};
-
-const BlockDef kLarge[] = {
-    {DS, 1, 1.f, 16},
-    {IR, 2, 4.f, 24}, {IR, 1, 3.f, 24},
-    {IR, 2, 3.f, 40}, {IR, 1, 3.f, 40}, {IR, 1, 3.f, 40},
-    {IR, 2, 6.f, 80}, {IR, 1, 2.5f, 80}, {IR, 1, 2.3f, 80}, {IR, 1, 2.3f, 80},
-    {IR, 1, 6.f, 112}, {IR, 1, 6.f, 112},
-    {IR, 2, 6.f, 160}, {IR, 1, 6.f, 160}, {IR, 1, 6.f, 160},
-    {CN, 1, 1.f, 960}};
-const BlockDef kSmall[] = {
-    {DS, 2, 1.f, 16},
-    {IR, 2, 4.5f, 24}, {IR, 1, 3.67f, 24},
-    {IR, 2, 4.f, 40}, {IR, 1, 6.f, 40}, {IR, 1, 6.f, 40},
-    {IR, 1, 3.f, 48}, {IR, 1, 3.f, 48},
-    {IR, 2, 6.f, 96}, {IR, 1, 6.f, 96}, {IR, 1, 6.f, 96},
-    {CN, 1, 1.f, 576}};
-
-int make_divisible(double v, int divisor = 8) {
-    int nv = std::max(divisor, (int)(v + divisor / 2.0) / divisor * divisor);
-    if (nv < 0.9 * v) nv += divisor;
-    return nv;
-}
 
 // Consumes (conv weight, bn gamma, beta, mean, var) from the tensor list.
 // kind: 0 = 1x1 [Cout,Cin,1,1] -> W[Cin][Cout]; 1 = depthwise [C,1,3,3] -> W[9][C]; 2 = stem [16,3,3,3] -> W[27][16]
@@ -129,31 +92,6 @@ bool fold_conv(TensorCursor& cur, int kind, int cin, int cout, bool tc, smk::Dev
 }
 
 }  // namespace
-
-struct SmkEncoder {
-    Backbone bb[3];
-    int n_shape = 300, n_exp = 50, precision = 0;
-    size_t max_act = 0;          // floats per image of the largest activation
-    bool fuse_xdw = false;       // precision >= 2: inverted-residual blocks use the fused expand+depthwise kernel
-    bool x3 = false;             // precision 3: 3xTF32 error-compensated tensor-core arithmetic (fp32-equivalent), no TF32 rounding of activations
-    bool present[3] = {false, false, false};   // a handle may hold a subset of the backbones (PoseEncoder / ShapeEncoder / ExpressionEncoder alone)
-    float *ones = nullptr, *zeros = nullptr;   // unit scale / zero bias of the dgrad GEMM epilogues
-    smk::SavedLayout saved;                    // of the grad-mode forward: forward order within a backbone, backbones in slot order
-    smk::DeviceArena arena;
-    // Fork/join plumbing for running the backbones as parallel branches of the caller's stream.  A forward takes the
-    // next set of a small pool (atomic round-robin), so up to kForkSets forwards of one handle may be in flight on
-    // different streams (with distinct workspaces) without sharing an event or a side stream: the handle is re-entrant.
-    static constexpr int kForkSets = 8;
-    struct ForkSet { cudaStream_t side[2] = {nullptr, nullptr}; cudaEvent_t fork = nullptr, join[2] = {nullptr, nullptr}; };
-    ForkSet forks[kForkSets];
-    mutable unsigned next_fork = 0;
-    ~SmkEncoder() {
-        for (auto& f : forks) {
-            for (int s = 0; s < 2; ++s) { if (f.side[s]) cudaStreamDestroy(f.side[s]); if (f.join[s]) cudaEventDestroy(f.join[s]); }
-            if (f.fork) cudaEventDestroy(f.fork);
-        }
-    }
-};
 
 extern "C" int smk_encoder_create(const SmkEncoderDesc* desc, SmkEncoder** out) {
     SMK_REQUIRE(desc && out, "smk_encoder_create: null argument");
@@ -225,14 +163,11 @@ extern "C" int smk_encoder_create(const SmkEncoderDesc* desc, SmkEncoder** out) 
         e = h->arena.upload(ones, &h->ones);
         if (e == cudaSuccess) e = h->arena.upload(zeros, &h->zeros);
         if (e != cudaSuccess) { smk::set_error("smk_encoder_create: upload failed: %s", cudaGetErrorString(e)); delete h; return (int)e; }
-        static const char* const kEnc[3] = {"pose_encoder", "shape_encoder", "expression_encoder"};
-        static const char* const kHead[3] = {"pose_cam_layers.0", "shape_layers.0", "expression_layers.0"};
-        static const int kStageLarge[] = {1, 2, 3, 4, 2, 3, 1}, kStageSmall[] = {1, 2, 3, 2, 3, 1};
         auto add = [h](const std::string& name, int H, int W, int C) { return h->saved.add(name, H, W, C); };
         for (int i = 0; i < 3; ++i) {
             if (!h->present[i]) continue;
             Backbone& bb = h->bb[i];
-            const std::string enc = std::string(kEnc[i]) + ".encoder.";
+            const std::string enc = std::string(kEncName[i]) + ".encoder.";
             const int* stages = i == 0 ? kStageSmall : kStageLarge;
             bb.sv_stem = add(enc + "bn1", 112, 112, 16);
             int res = 112, stage = 0, in_stage = 0;
@@ -245,16 +180,10 @@ extern "C" int smk_encoder_create(const SmkEncoderDesc* desc, SmkEncoder** out) 
                 res = ro;
                 if (++in_stage == stages[stage]) { ++stage; in_stage = 0; }
             }
-            bb.sv_head = add(std::string(kEnc[i]) + "." + kHead[i], 1, 1, bb.n_out);
+            bb.sv_head = add(std::string(kEncName[i]) + "." + kHeadName[i], 1, 1, bb.n_out);
         }
     }
-    for (auto& f : h->forks) {
-        for (int s = 0; s < 2 && e == cudaSuccess; ++s) {
-            e = cudaStreamCreateWithFlags(&f.side[s], cudaStreamNonBlocking);
-            if (e == cudaSuccess) e = cudaEventCreateWithFlags(&f.join[s], cudaEventDisableTiming);
-        }
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&f.fork, cudaEventDisableTiming);
-    }
+    e = create_forks(h);
     if (e != cudaSuccess) { smk::set_error("smk_encoder_create: stream/event creation failed: %s", cudaGetErrorString(e)); delete h; return (int)e; }
     *out = h;
     return 0;
@@ -280,40 +209,6 @@ static int pointwise(int n, const ConvW* const* c, float* const* in, int B, int 
         q[k].round_out = c[k]->wt && !c[k]->wt_lo;      // 3xTF32 consumers split full fp32 activations themselves
     }
     return smk::conv(q[0], st, n == 2 ? &q[1] : nullptr);
-}
-
-// One unit of work: n = 1 backbone, or the pair idx = {1, 2}, on stream st.
-struct Unit { int n; int idx[2]; cudaStream_t st; };
-
-// Runs run(unit) (-> status; the first error stops the walk) over the backbones with use[i] set.  The three backbones
-// are independent (smirk_encoder.py:123-133 merely runs them one after another): with more than one in use, the units
-// fork from main_st onto the side streams of one of the handle's fork sets, so their many small, latency-bound layers
-// overlap, and join back into main_st — even after an error, so a capturing stream is left consistent.  Event
-// record/wait on other streams is legal under stream capture, so a CUDA graph of the caller's stream gets parallel
-// branches.  The two "large" backbones (shape, expression) have the same layer list, so on the tensor-core path they
-// advance in lock step as one unit and every layer of the pair is ONE launch; the small (pose) backbone is its own unit.
-template <typename Run>
-static int for_each_unit(const SmkEncoder* h, const bool use[3], cudaStream_t main_st, const char* what, Run&& run) {
-    const int n_use = (int)use[0] + (int)use[1] + (int)use[2];
-    const bool concurrent = !smk::profiling() && n_use > 1;       // the event profiler wants one kernel at a time
-    const SmkEncoder::ForkSet& fk = h->forks[__atomic_fetch_add(&h->next_fork, 1u, __ATOMIC_RELAXED) % SmkEncoder::kForkSets];
-    Unit units[3]; int n_units = 0;
-    if (use[0]) units[n_units++] = Unit{1, {0, 0}, main_st};
-    if (h->precision >= 1 && use[1] && use[2]) units[n_units++] = Unit{2, {1, 2}, concurrent ? fk.side[0] : main_st};
-    else for (int i = 1; i < 3; ++i) if (use[i]) units[n_units++] = Unit{1, {i, i}, concurrent ? fk.side[i - 1] : main_st};
-    if (!use[0] && n_units > 0) units[0].st = main_st;                             // without pose, the first unit takes the caller's stream
-    if (concurrent) {
-        SMK_CHECK_CUDA(cudaEventRecord(fk.fork, main_st));
-        for (int s = 0; s < 2; ++s) SMK_CHECK_CUDA(cudaStreamWaitEvent(fk.side[s], fk.fork, 0));
-    }
-    int rc = 0;
-    for (int u = 0; u < n_units && !rc; ++u) rc = run(units[u]);
-    for (int s = 0; s < 2 && concurrent; ++s) {
-        cudaError_t e1 = cudaEventRecord(fk.join[s], fk.side[s]);
-        cudaError_t e2 = e1 == cudaSuccess ? cudaStreamWaitEvent(main_st, fk.join[s], 0) : e1;
-        if (!rc && e2 != cudaSuccess) { smk::set_error("%s: stream join failed: %s", what, cudaGetErrorString(e2)); rc = (int)e2; }
-    }
-    return rc;
 }
 
 // The forward; sv (grad mode, may be null): the saved buffer.  With sv the launches and arithmetic are those of the
@@ -435,6 +330,7 @@ extern "C" int smk_encoder_forward(const SmkEncoder* h, const float* img, int B,
                 "smk_encoder_forward: null output for a backbone this handle holds");
     SMK_REQUIRE(B > 0, "smk_encoder_forward: negative batch");
     SMK_REQUIRE(ws && ws_bytes >= smk_encoder_workspace_bytes(h, B), "smk_encoder_forward: workspace too small");
+    SMK_REQUIRE(!h->train, "smk_encoder_forward: a train-mode handle runs smk_encoder_forward_train");
     return encoder_forward(h, img, B, pose_cam, shape, expr, nullptr, ws, ws_bytes, (cudaStream_t)stream);
 }
 
@@ -594,7 +490,9 @@ int dgrad_dw(int n, const Block* const* b, const float* const* g, const float* c
 
 }  // namespace
 
-extern "C" size_t smk_encoder_saved_bytes(const SmkEncoder* h, int B) { return h ? h->saved.bytes(B) : 0; }
+extern "C" size_t smk_encoder_saved_bytes(const SmkEncoder* h, int B) {
+    return h && B > 0 ? h->saved.bytes(B) + smk::ws_round(h->stats_floats * sizeof(float)) : 0;   // stats: train handles only
+}
 
 extern "C" int smk_encoder_saved_tensor(const SmkEncoder* h, int B, int i, const char** name, size_t* offset, int* dims) {
     return smk::saved_tensor(h ? &h->saved : nullptr, "smk_encoder_saved_tensor", B, i, name, offset, dims);
@@ -610,6 +508,7 @@ extern "C" int smk_encoder_forward_saved(const SmkEncoder* h, const float* img, 
     SMK_REQUIRE((pose_cam || !h->present[0]) && (shape || !h->present[1]) && (expr || !h->present[2]),
                 "smk_encoder_forward_saved: null output for a backbone this handle holds");
     SMK_REQUIRE(ws && ws_bytes >= smk_encoder_workspace_bytes(h, B), "smk_encoder_forward_saved: workspace too small");
+    SMK_REQUIRE(!h->train, "smk_encoder_forward_saved: a train-mode handle runs smk_encoder_forward_train");
     return encoder_forward(h, img, B, pose_cam, shape, expr, saved, ws, ws_bytes, (cudaStream_t)stream);
 }
 
@@ -625,6 +524,7 @@ extern "C" int smk_encoder_backward(const SmkEncoder* h, int B, const float* sav
     SMK_REQUIRE(saved && g_img, "smk_encoder_backward: null argument");
     SMK_REQUIRE(saved_bytes > 0 && saved_bytes >= smk_encoder_saved_bytes(h, B), "smk_encoder_backward: saved buffer too small");
     SMK_REQUIRE(ws && ws_bytes >= smk_encoder_backward_workspace_bytes(h, B), "smk_encoder_backward: workspace too small");
+    SMK_REQUIRE(!h->train, "smk_encoder_backward: a train-mode handle runs smk_encoder_backward_train");
     cudaStream_t main_st = (cudaStream_t)stream;
     const float* g_out[3] = {g_pose_cam, g_shape, g_expr};
     bool active[3];
@@ -637,7 +537,6 @@ extern "C" int smk_encoder_backward(const SmkEncoder* h, int B, const float* sav
     const bool tc = h->precision >= 1;
     const bool rnd = tc && !h->x3;                  // gradients that feed a TF32 GEMM are rounded (3xTF32 splits them itself)
     const float* g_stem[3] = {nullptr, nullptr, nullptr};
-    const int n_active = (int)active[0] + (int)active[1] + (int)active[2];
     // the stem dgrad after the join sums every backbone's stem gradient on main_st
     int rc = for_each_unit(h, active, main_st, "smk_encoder_backward", [&](const Unit& unit) {
         const int n = unit.n;
@@ -695,11 +594,18 @@ extern "C" int smk_encoder_backward(const SmkEncoder* h, int B, const float* sav
         return rc;
     });
     if (rc) return rc;
+    const float* w_stem[3];
+    for (int i = 0; i < 3; ++i) w_stem[i] = g_stem[i] ? h->bb[i].stem_d.w : nullptr;
+    return enc::stem_dgrad(g_stem, w_stem, B, g_img, main_st);
+}
+
+int enc::stem_dgrad(const float* const g[3], const float* const w[3], int B, float* g_img, cudaStream_t st) {
     StemDgrad p{};
-    for (int i = 0; i < 3; ++i) { p.g[i] = g_stem[i]; p.w[i] = g_stem[i] ? h->bb[i].stem_d.w : nullptr; }
+    int n_active = 0;
+    for (int i = 0; i < 3; ++i) { p.g[i] = g[i]; p.w[i] = g[i] ? w[i] : nullptr; n_active += g[i] != nullptr; }
     const long px = (long)B * 224 * 224;
-    SMK_TAG("stem_dgrad", 4.0 * ((double)B * 3 * 224 * 224 + n_active * ((double)B * 112 * 112 * 16 + 27 * 16)), n_active * 2.0 * 27 * 16 * B * 112.0 * 112.0, main_st);
-    SMK_LAUNCH(stem_dgrad_kernel, dim3(smk::cdiv(px, 128)), dim3(128), 0, main_st, p, B, 224, 224, 112, 112, same_pad_begin(224, 2), g_img);
+    SMK_TAG("stem_dgrad", 4.0 * ((double)B * 3 * 224 * 224 + n_active * ((double)B * 112 * 112 * 16 + 27 * 16)), n_active * 2.0 * 27 * 16 * B * 112.0 * 112.0, st);
+    SMK_LAUNCH(stem_dgrad_kernel, dim3(smk::cdiv(px, 128)), dim3(128), 0, st, p, B, 224, 224, 112, 112, same_pad_begin(224, 2), g_img);
     SMK_CHECK_LAUNCH();
     return 0;
 }

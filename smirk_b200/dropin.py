@@ -1,6 +1,11 @@
 """Run the reference's own entry scripts on smirk_b200 without modifying them.
 
     cd <reference checkout>;  python -m smirk_b200.dropin demo.py --input_path ... [script args]
+    cd <reference checkout>;  python -m smirk_b200.dropin --train train.py configs/config_pretrain.yaml
+
+``--train`` (before the script) turns on the encoder's train-mode opt-in for the whole process
+(``smirk_encoder.set_train_mode_default(True)``): the trainer's ``.train()`` encoder then runs with batch statistics
+and gets its weight gradients.  Without it a train-mode encoder raises, as before.
 
 ``install()`` registers our modules under the four names the reference imports its hot-path classes
 from (``demo.py:5-7,62``, ``src/smirk_trainer.py:3-6``):
@@ -62,8 +67,14 @@ def install(reference_root=None):
 
 def main(argv=None):
     argv = list(sys.argv[1:] if argv is None else argv)
+    train = argv[:1] == ["--train"]
+    if train:
+        argv = argv[1:]
     if not argv:
-        raise SystemExit("usage: python -m smirk_b200.dropin <reference script.py> [script args...]")
+        raise SystemExit("usage: python -m smirk_b200.dropin [--train] <reference script.py> [script args...]")
+    if train:
+        from . import smirk_encoder
+        smirk_encoder.set_train_mode_default(True)
     script = argv[0]
     install(os.path.dirname(os.path.abspath(script)) or os.getcwd())
     sys.argv = argv
