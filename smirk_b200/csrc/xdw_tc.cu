@@ -10,21 +10,28 @@
 //         makes channel chunks independent, so low-resolution layers still fill the GPU).  Persistent CTAs;
 //         the launcher aims for one per SM, which leaves room on every SM for the other kernels of the
 //         concurrent pipeline.
-//   warp 8      TMA producer: per work item, the whole x window once — two 16x8-pixel boxes per 32-channel
+//   producer    one TMA warp: per work item, the whole x window once — two 16x8-pixel boxes per 32-channel
 //               k-block (4-D tiled tensor map over NHWC, halo pixels outside the image zero-filled by the hardware)
 //               into a window region that stays resident for the item; then only the 1x1 weights (a 32-row box
 //               per (chunk, k-block), plus its tails in the 3xTF32 variant) through a small mbarrier ring.
-//   warps 0-7   two warpgroups; warpgroup h multiplies window half h (128 pixels x Cin) with wgmma.m64n32k8 TF32
+//   MMA         two warpgroups; warpgroup h multiplies window half h (128 pixels x Cin) with wgmma.m64n32k8 TF32
 //               (two per k-step, ceil(Cin / 8) k-steps: none over the zero-filled channels past Cin), then
 //               (a) accumulator registers -> BN1 + ReLU (+ zero outside the image, which is what the depthwise
 //               conv's zero padding of e means) -> shared-memory window E[256][32];
-//               (b) depthwise 3x3 over E on the CUDA cores (float4 over channels), BN2 + ReLU, optional
+//   depthwise   (b) depthwise 3x3 over E on the CUDA cores (float4 over channels), BN2 + ReLU, optional
 //               TF32 rounding, coalesced 256-byte stores of d.
 //
-// Shared memory: [window 0 (, window 1)][weight ring][E][parameters][barriers].  The window holds NKB = ceil(Cin / 32)
+// Two schedules.  Serial (xdw_kernel, plain TF32, 288 threads, two CTAs per SM for Cin <= 64): the 8 MMA warps also run
+// phase (b), with a CTA barrier after (a) and after (b), so the tensor cores and the FP32 pipes take turns.  Pipelined
+// (xdw_ws_kernel, 3xTF32, 512 threads, one CTA per SM): the MMA warpgroups fill a ring of two E slots while a third
+// warpgroup runs phase (b) on the slot filled before, so chunk i+1's wgmma and phase (a) overlap chunk i's depthwise
+// conv; setmaxnreg gives the MMA warpgroups 168 registers, the depthwise warpgroup 136 and the producer's 40.
+// The arithmetic (k-step order, accumulators, BN / ReLU, tap order, rounding) is the same in both, so d and e are too.
+//
+// Shared memory: [window 0 (, window 1)][weight ring][E slots][parameters][barriers].  The window holds NKB = ceil(Cin / 32)
 // k-blocks of 32 KiB (the kernel is instantiated per NKB, Cin <= 160); it is double-buffered where that fits the
 // per-SM budget (so the next item's window lands while this item computes), otherwise the producer refills it as soon
-// as the item's last chunk has finished its MMAs, during that chunk's phases (a)/(b).
+// as the item's last chunk has finished its MMAs, during that chunk's phases (a)/(b).  XdwSmem is the plan.
 //
 // Algorithmic HBM traffic per block drops from  x + 2e + d  to  x + d.  L2 -> shared memory per item: the window
 // once (NKB x 32 KiB) + the weights of its chunks (NKB x 4 KiB per chunk, x2 for 3xTF32).
@@ -42,35 +49,52 @@ constexpr int KB_BYTES = 2 * HALF_BYTES;        // both halves of the window, on
 constexpr int NC = 32;                          // expanded channels per chunk
 constexpr int B_BYTES = NC * BKB;               // 4 KiB
 constexpr int E_PITCH = NC + 4;                 // floats; 144-byte rows (odd multiple of 16 B): conflict-free 16-byte column writes
-constexpr int E_BYTES = 256 * E_PITCH * 4;      // 36 864 B
+constexpr int E_FLOATS = 256 * E_PITCH, E_BYTES = E_FLOATS * 4;    // 36 864 B
 constexpr int PAR_ROWS = 13;                     // scale1, bias1, 9 depthwise taps, scale2, bias2
-constexpr int PAR_BYTES = 2 * PAR_ROWS * NC * 4;  // double-buffered: 3328 B
-constexpr int NUM_WORKERS = 256;
-constexpr int NUM_THREADS = NUM_WORKERS + 32;
+constexpr int PAR_FLOATS = PAR_ROWS * NC, PAR_SLOT_BYTES = PAR_FLOATS * 4;   // one chunk's parameters: 1664 B
+constexpr int NUM_WORKERS = 256;                // serial schedule: 8 worker warps; pipelined: the 8 warps of the two MMA warpgroups
+constexpr int NUM_THREADS = NUM_WORKERS + 32;   // serial schedule: + the TMA producer warp
+// Pipelined schedule: warpgroups 0-1 expand GEMM + phase (a), warpgroup 2 depthwise (each thread plays DW_ROLES of the
+// serial schedule's 256 depthwise roles), warpgroup 3 the TMA producer (one warp works, three exit).  Every warp starts
+// with WS_LAUNCH_REGS; the producer warpgroup gives registers back (setmaxnreg.dec, which may only lower the count) and the
+// other three take them (setmaxnreg.inc, which may only raise it).  The budgets fill the 64 K register file exactly.
+constexpr int DW_THREADS = 128, DW_ROLES = NUM_WORKERS / DW_THREADS, WS_THREADS = NUM_WORKERS + DW_THREADS + 128;
+constexpr int WS_LAUNCH_REGS = 65536 / WS_THREADS, MMA_REGS = 168, DW_REGS = 136, PROD_REGS = 40;
+static_assert(NUM_WORKERS * MMA_REGS + DW_THREADS * DW_REGS + 128 * PROD_REGS == 65536, "register budgets of the pipelined schedule");
+static_assert(MMA_REGS >= WS_LAUNCH_REGS && DW_REGS >= WS_LAUNCH_REGS && PROD_REGS <= WS_LAUNCH_REGS,
+              "setmaxnreg directions: inc for the MMA and depthwise warpgroups, dec for the producer");
 constexpr int MAX_NKB = 5;                      // Cin <= 160
 constexpr int SMEM_PER_SM = 228 * 1024, SMEM_PER_CTA = 227 * 1024, SMEM_RESERVED = 1024;   // sm_90 limits
 
-// Shared-memory plan of one window size.  MINB: resident CTAs per SM the kernel is built for — two for plain TF32
-// wherever a single window leaves room for them, one for 3xTF32 (register-bound) and for the deep plain-TF32 windows.
+// Shared-memory plan of one window size.  3xTF32 (X3) runs the pipelined schedule, plain TF32 the serial one.
+// MINB: resident CTAs per SM the kernel is built for — two for plain TF32 wherever a single window leaves room for them, one for
+// 3xTF32 (the pipelined schedule takes the whole register file) and for the deep plain-TF32 windows.
+// NE: E slots (each with its parameter block).  Pipelined: two where they fit beside one window and a 2-stage weight ring, so
+// the MMA warpgroups fill one slot while the depthwise warpgroup drains the other; one for NKB = 5 (Cin 160).  Serial: one E,
+// two parameter blocks (chunk parity).
 // STAGES: weight stages; NKB where they fit, so the next chunk's weights all load during this chunk's phases (a)/(b).
 // WBUF: windows, two where they fit beside MINB CTAs.
 template <int NKB, int X3> struct XdwSmem {
     static constexpr int WIN_BYTES = NKB * KB_BYTES;
     static constexpr int STAGE_BYTES = X3 ? 2 * B_BYTES : B_BYTES;      // [w heads] (+ [w tails])
-    static constexpr size_t bytes(int wbuf, int stages) {
-        return (size_t)wbuf * WIN_BYTES + stages * STAGE_BYTES + E_BYTES + PAR_BYTES + 256 + 1024;   // + barriers, alignment slack
+    static constexpr size_t bytes(int wbuf, int stages, int ne) {
+        return (size_t)wbuf * WIN_BYTES + stages * STAGE_BYTES + ne * E_BYTES + (X3 ? ne : 2) * PAR_SLOT_BYTES + 256 + 1024;   // + barriers, alignment slack
     }
-    static constexpr bool fits(int wbuf, int stages, int minb) {
-        return bytes(wbuf, stages) <= SMEM_PER_CTA && minb * (bytes(wbuf, stages) + SMEM_RESERVED) <= SMEM_PER_SM;
+    static constexpr bool fits(int wbuf, int stages, int ne, int minb) {
+        return bytes(wbuf, stages, ne) <= SMEM_PER_CTA && minb * (bytes(wbuf, stages, ne) + SMEM_RESERVED) <= SMEM_PER_SM;
     }
-    static constexpr int MINB = !X3 && fits(1, 2, 2) ? 2 : 1;
-    static constexpr int STAGES = NKB > 2 && fits(1, NKB, MINB) ? NKB : 2;
-    static constexpr int WBUF = fits(2, STAGES, MINB) ? 2 : 1;
-    static constexpr size_t SMEM = bytes(WBUF, STAGES);
-    static constexpr int RING = WBUF * WIN_BYTES, E_OFF = RING + STAGES * STAGE_BYTES, PAR_OFF = E_OFF + E_BYTES,
-                         BAR_OFF = PAR_OFF + PAR_BYTES;
-    static_assert(fits(WBUF, STAGES, MINB), "shared-memory budget");
+    static constexpr int MINB = !X3 && fits(1, 2, 1, 2) ? 2 : 1;
+    static constexpr int NE = X3 && fits(1, 2, 2, 1) ? 2 : 1;
+    static constexpr int STAGES = NKB > 2 && fits(1, NKB, NE, MINB) ? NKB : 2;
+    static constexpr int WBUF = fits(2, STAGES, NE, MINB) ? 2 : 1;
+    static constexpr size_t SMEM = bytes(WBUF, STAGES, NE);
+    static constexpr int RING = WBUF * WIN_BYTES, E_OFF = RING + STAGES * STAGE_BYTES, PAR_OFF = E_OFF + NE * E_BYTES,
+                         BAR_OFF = PAR_OFF + (X3 ? NE : 2) * PAR_SLOT_BYTES;
+    static_assert(fits(WBUF, STAGES, NE, MINB), "shared-memory budget");
+    static_assert(2 * (STAGES + WBUF + NE) * 8 <= 256, "barrier block");
 };
+static_assert(XdwSmem<1, 2>::NE == 2 && XdwSmem<2, 2>::NE == 2 && XdwSmem<3, 2>::NE == 2 && XdwSmem<4, 2>::NE == 2,
+              "3xTF32: two E slots for every window the encoder launches (Cin <= 112)");
 
 using namespace ptx;                            // PTX wrappers shared by the tensor-core kernels (tc_ptx.cuh)
 __device__ __forceinline__ void worker_barrier() { named_barrier(1, NUM_WORKERS); }
@@ -94,312 +118,447 @@ struct XdwArgs {
     float* e_out[2];                                // SAVE: e [B, H, W, mid] (per problem)
 };
 
-// X3 != 0: error-compensated 3xTF32 expand GEMM (fp32-equivalent e): x = x_hi + x_lo, w1 = w_hi + w_lo (split on the host, wlo),
-// e = x_hi*w_hi + x_lo*w_hi + x_hi*w_lo accumulated in the same registers.  The workers split their own A fragments of x in
-// registers and use the register-A form of wgmma, so shared memory only grows by the weight tails.
-// NKB: 32-channel k-blocks of Cin (window size), KSL: wgmma k-steps of 8 channels in the last one (Cin = 32 (NKB - 1) + 8 KSL,
-// rounded up to a multiple of 8).  SAVE: phase (a) also stores e for the pixels the item owns (rows / columns
-// [o0 * STRIDE, (o0 + TO) * STRIDE) of e: every pixel of e belongs to one tile) — the backward's ReLU mask.
+// Persistent CTA: work item = (image, output tile, channel-chunk group), items strided over the grid.  Every role walks the
+// same item sequence; the weight ring (and in the pipelined schedule the E ring) runs across item boundaries and the window is
+// refilled as soon as it is free, so the loads of item i+1 are in flight while the workers are still busy with item i.
+// The item sequence of a CTA advances by gridDim.x; the (group, tile x, tile y, image) digits of the item index are carried
+// along incrementally — one runtime decomposition per thread at kernel start instead of four integer divisions per item.
+struct Item { int prob, img, oh0, ow0, c_begin, c_end; };
+struct ItemIter {
+    int item, grp, tx, ty, img2;                // img2: image index over both problems
+    __device__ explicit ItemIter(const XdwArgs& a) {
+        int v = item = blockIdx.x;
+        grp = v % a.groups; v /= a.groups; tx = v % a.tiles_x; v /= a.tiles_x; ty = v % a.tiles_y; img2 = v / a.tiles_y;
+    }
+    __device__ void next(const XdwArgs& a) {
+        item += gridDim.x;
+        grp += a.d_grp; if (grp >= a.groups) { grp -= a.groups; ++tx; }
+        tx += a.d_tx;   if (tx >= a.tiles_x) { tx -= a.tiles_x; ++ty; }
+        ty += a.d_ty;   if (ty >= a.tiles_y) { ty -= a.tiles_y; ++img2; }
+        img2 += a.d_img;
+    }
+    template <int TO> __device__ Item decode(const XdwArgs& a) const {
+        Item w;
+        w.prob = img2 >= a.B ? 1 : 0; w.img = img2 - w.prob * a.B;
+        w.oh0 = ty * TO; w.ow0 = tx * TO;
+        w.c_begin = grp * a.chunks_per_group; w.c_end = min(a.nchunks, w.c_begin + a.chunks_per_group);
+        return w;
+    }
+};
+
+// TMA producer: the x window once per item, then the W1 rows of every (chunk, k-block).
+template <int STRIDE, int X3, int NKB>
+__device__ __forceinline__ void produce(const XdwMaps& mp, const XdwArgs& a, uint8_t* smem, uint64_t* full, uint64_t* empty,
+                                        uint64_t* wfull, uint64_t* wempty) {
+    using L = XdwSmem<NKB, X3>;
+    constexpr int TO = STRIDE == 1 ? 14 : 7, STAGES = L::STAGES, WBUF = L::WBUF;
+    uint8_t* ring = smem + L::RING;
+    int it = 0, n = 0;
+    for (ItemIter ii(a); ii.item < a.n_items; ii.next(a), ++n) {
+        const Item w = ii.decode<TO>(a);
+        const int ey0 = w.oh0 * STRIDE - a.pad, ex0 = w.ow0 * STRIDE - a.pad;     // window origin in e / x coordinates
+        const int b = n % WBUF;
+        mbar_wait(&wempty[b], ((uint32_t)(n / WBUF) & 1u) ^ 1u);
+        uint8_t* win = smem + b * L::WIN_BYTES;                                     // [k-block][half][128 pixels][32 channels]
+        mbar_expect_tx(&wfull[b], (uint32_t)L::WIN_BYTES);
+#pragma unroll
+        for (int kb = 0; kb < NKB; ++kb) {
+            tma_load_4d(&mp.x[w.prob], win + kb * KB_BYTES, &wfull[b], kb * BK, ex0, ey0, w.img);
+            tma_load_4d(&mp.x[w.prob], win + kb * KB_BYTES + HALF_BYTES, &wfull[b], kb * BK, ex0, ey0 + 8, w.img);
+        }
+        for (int c = w.c_begin; c < w.c_end; ++c)
+            for (int kb = 0; kb < NKB; ++kb, ++it) {
+                const int s = it % STAGES;
+                mbar_wait(&empty[s], ((uint32_t)(it / STAGES) & 1u) ^ 1u);
+                uint8_t* st = ring + s * L::STAGE_BYTES;
+                mbar_expect_tx(&full[s], (uint32_t)L::STAGE_BYTES);
+                tma_load_2d(&mp.w[w.prob], st, &full[s], kb * BK, c * NC);
+                if (X3) tma_load_2d(&mp.wlo[w.prob], st + B_BYTES, &full[s], kb * BK, c * NC);
+            }
+    }
+}
+
+// Per-chunk parameters (BN1 scale/bias, nine depthwise taps, BN2 scale/bias: 13 rows of 32 channels) are staged through a
+// shared-memory block: worker t < 208 owns one float2 of it, loads it from global memory before it starts the chunk's MMAs
+// (or, serial schedule, the previous chunk's) and parks it once the block is free, so the global-load latency is off the
+// critical path and phases (a)/(b) read parameters with LDS.  Channels past `mid` get zero scale and bias.
+struct ParLoader {
+    const float* src[2];
+    int prow, pcol;
+    bool owner;
+    __device__ ParLoader(const XdwArgs& a, int t) : src{nullptr, nullptr}, prow(t >> 4), pcol((t & 15) * 2), owner(t < PAR_ROWS * 16) {
+        if (owner) {
+#pragma unroll
+            for (int q = 0; q < 2; ++q)
+                src[q] = (prow == 0 ? a.scale1[q] : prow == 1 ? a.bias1[q] : prow == 11 ? a.scale2[q] : prow == 12 ? a.bias2[q]
+                                                                                  : a.wdw[q] + (size_t)(prow - 2) * a.mid) + pcol;
+        }
+    }
+    __device__ float2 load(const XdwArgs& a, int prob, int c) const {
+        float2 v = make_float2(0.f, 0.f);
+        if (owner && c * NC + pcol < a.mid) v = __ldg(reinterpret_cast<const float2*>(src[prob] + c * NC));
+        return v;
+    }
+    __device__ void park(float* par, const float2& v) const {
+        if (owner) *reinterpret_cast<float2*>(par + prow * NC + pcol) = v;
+    }
+};
+
+// Expand GEMM of one chunk: rows [64 mb, 64 mb + 64) of this warpgroup's window half x the chunk's 32 weight rows, over the
+// NKB k-blocks of weights streamed through the ring (k-block `it` in stage it % STAGES).
+template <int X3, int NKB, int KSL>
+__device__ __forceinline__ void expand_gemm(float (&acc)[2][NC / 2], const uint8_t* win, uint8_t* ring, uint64_t* full, uint64_t* empty,
+                                            int& it, int wq, int lane) {
+    using L = XdwSmem<NKB, X3>;
+    constexpr int STAGES = L::STAGES;
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+        for (int i = 0; i < NC / 2; ++i) acc[mb][i] = 0.f;
+#pragma unroll
+    for (int kb = 0; kb < NKB; ++kb, ++it) {
+        // k-steps of this k-block: all four, except KSL in the last one, where the steps over the channels past Cin
+        // (zero-filled by TMA) would only add zeros.  Known at compile time, so no wgmma sits behind a branch.
+        const int nks = kb + 1 < NKB ? BK / MMA_K : KSL;
+        const int s = it % STAGES;
+        mbar_wait(&full[s], (uint32_t)(it / STAGES) & 1u);
+        const uint8_t* xa = win + kb * KB_BYTES;
+        const uint32_t sb = smem_u32(ring + s * L::STAGE_BYTES);
+        if constexpr (X3 != 0) {
+            uint32_t hi[2][BK / MMA_K][4], lo[2][BK / MMA_K][4];
+#pragma unroll
+            for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+                for (int k = 0; k < nks; ++k) {
+                    float v[4];
+                    load_a_frag(xa, mb * 64, k * MMA_K, wq, lane, v);
+                    split_frag(v, hi[mb][k], lo[mb][k]);
+                }
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < nks; ++k) {
+                const uint64_t db = make_smem_desc(sb + k * MMA_K * 4);
+                const uint64_t dbl = make_smem_desc(sb + B_BYTES + k * MMA_K * 4);
+#pragma unroll
+                for (int mb = 0; mb < 2; ++mb) {
+                    Wgmma<NC>::rs(acc[mb], hi[mb][k], db, 1u);       // x_hi * w_hi
+                    Wgmma<NC>::rs(acc[mb], lo[mb][k], db, 1u);       // x_lo * w_hi
+                    Wgmma<NC>::rs(acc[mb], hi[mb][k], dbl, 1u);      // x_hi * w_lo
+                }
+            }
+        } else {
+            const uint32_t sa = smem_u32(xa);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < nks; ++k) {
+                const uint64_t db = make_smem_desc(sb + k * MMA_K * 4);
+#pragma unroll
+                for (int mb = 0; mb < 2; ++mb)
+                    Wgmma<NC>::ss(acc[mb], make_smem_desc(sa + mb * 64 * BKB + k * MMA_K * 4), db, 1u);
+            }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        __syncwarp();
+        mbar_arrive_if(&empty[s], lane == 0);
+    }
+}
+
+// Phase (a): accumulators -> BN1 + ReLU -> E.  Channels past `mid` have zero scale and bias in the parameter block, pixels
+// outside the image are zeroed: that is the zero padding of e the depthwise conv expects.  SAVE: also store e for the pixels
+// the item owns.
+template <int STRIDE, bool SAVE>
+__device__ __forceinline__ void bn1_relu(const float (&acc)[2][NC / 2], float* E, const float* par, const XdwArgs& a, const Item& w,
+                                         int ch0, int half, int wq, int lane) {
+    constexpr int TO = STRIDE == 1 ? 14 : 7;
+    const int ey0 = w.oh0 * STRIDE - a.pad, ex0 = w.ow0 * STRIDE - a.pad;
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            const int r = mb * 64 + wq * 16 + (lane >> 2) + 8 * hr;      // row within the half: r = hh*16 + ww
+            const int ey = ey0 + half * 8 + (r >> 4), ex = ex0 + (r & 15);
+            const bool inside = ey >= 0 && ey < a.H && ex >= 0 && ex < a.W;
+            float* erow = E + (size_t)(half * 128 + r) * E_PITCH;
+            bool own = false;
+            float* esave = nullptr;
+            if constexpr (SAVE) {
+                own = inside && ey >= w.oh0 * STRIDE && ey < (w.oh0 + TO) * STRIDE && ex >= w.ow0 * STRIDE && ex < (w.ow0 + TO) * STRIDE;
+                esave = a.e_out[w.prob] + (((size_t)w.img * a.H + ey) * a.W + ex) * a.mid + ch0;
+            }
+#pragma unroll
+            for (int j = 0; j < NC / 8; ++j) {
+                const int ch = 8 * j + 2 * (lane & 3);
+                float2 o = make_float2(0.f, 0.f);
+                if (inside) {
+                    const float2 sc = *reinterpret_cast<const float2*>(par + ch);
+                    const float2 bi = *reinterpret_cast<const float2*>(par + NC + ch);
+                    o.x = fmaxf(fmaf(acc[mb][4 * j + 2 * hr], sc.x, bi.x), 0.f);
+                    o.y = fmaxf(fmaf(acc[mb][4 * j + 2 * hr + 1], sc.y, bi.y), 0.f);
+                }
+                *reinterpret_cast<float2*>(erow + ch) = o;
+                if (SAVE && own && ch0 + ch < a.mid) *reinterpret_cast<float2*>(esave + ch) = o;
+            }
+        }
+}
+
+// Depthwise role: output column ox and row group rg of the tile's valid columns x as many row groups as fit in the 32 slots.
+// A tile has TO columns / rows except in the last tile column / row: the role for both column counts is worked out once
+// (bytes: ox full, rg full, ox edge, rg edge), the row grouping of the four tile kinds comes from the host (a.geom); the item
+// loop only selects (dw_rows).
+template <int TO> __device__ __forceinline__ unsigned dw_role(const XdwArgs& a, int slot) {
+    const int ncols_e = a.Wo - (a.tiles_x - 1) * TO;
+    return (unsigned)(slot % TO) | (unsigned)(slot / TO) << 8 | (unsigned)(slot % ncols_e) << 16 | (unsigned)(slot / ncols_e) << 24;
+}
+struct DwRows { int ox, oy0, oy1; };            // output column and output rows [oy0, oy1) of the tile
+template <int TO> __device__ __forceinline__ DwRows dw_rows(const XdwArgs& a, const ItemIter& ii, unsigned role) {
+    const bool col_e = ii.tx == a.tiles_x - 1, row_e = ii.ty == a.tiles_y - 1;
+    const int nrows = row_e ? a.Ho - (a.tiles_y - 1) * TO : TO;
+    const unsigned g8 = a.geom >> ((col_e ? 16 : 0) + (row_e ? 8 : 0));
+    const int rpt = (int)(g8 & 15u), n_rg = (int)((g8 >> 4) & 15u);
+    const unsigned r16 = role >> (col_e ? 16 : 0);
+    const int rg = (int)((r16 >> 8) & 255u);
+    DwRows d;
+    d.ox = (int)(r16 & 255u); d.oy0 = rg * rpt; d.oy1 = rg < n_rg ? min(nrows, d.oy0 + rpt) : 0;
+    return d;
+}
+
+// Phase (b): depthwise 3x3 over E, BN2 + ReLU, optional TF32 rounding, store of d.  One thread owns one output column of one
+// channel quad and walks down its rows, so every E row it reads is shared by the (up to three) output rows it feeds: 3 LDS.128
+// per input row instead of 9 per output.  Tap order per output stays (ky, kx) ascending -> same rounding as the unfused path.
+template <int STRIDE>
+__device__ __forceinline__ void depthwise(const float* E, const float* par, const XdwArgs& a, const Item& w, int ch0, int cq, const DwRows& rows) {
+    if (cq * 4 < a.mid - ch0 && rows.oy0 < rows.oy1) {
+        const int ch = ch0 + cq * 4;
+        float4 k[9];
+#pragma unroll
+        for (int q = 0; q < 9; ++q) k[q] = *reinterpret_cast<const float4*>(par + (2 + q) * NC + cq * 4);
+        const float4 s2 = *reinterpret_cast<const float4*>(par + 11 * NC + cq * 4);
+        const float4 b2 = *reinterpret_cast<const float4*>(par + 12 * NC + cq * 4);
+        float* orow = a.out[w.prob] + (((size_t)w.img * a.Ho + w.oh0 + rows.oy0) * a.Wo + w.ow0 + rows.ox) * a.mid + ch;
+        const size_t orow_stride = (size_t)a.Wo * a.mid;
+        auto emit = [&](const float4& acc4) {
+            float4 o = fma4(acc4, s2, b2);
+            o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
+            if (a.round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
+            *reinterpret_cast<float4*>(orow) = o;
+            orow += orow_stride;
+        };
+        const float* e = E + (size_t)((rows.oy0 * STRIDE) * WIN + rows.ox * STRIDE) * E_PITCH + cq * 4;
+        const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (STRIDE == 1) {
+            float4 acc0 = zero, acc1 = zero, acc2 = zero;          // outputs r-2 (gets ky=2), r-1 (ky=1), r (ky=0)
+            const int n_in = rows.oy1 - rows.oy0 + 2;
+#pragma unroll 3
+            for (int r = 0; r < n_in; ++r, e += WIN * E_PITCH) {
+                const float4 x0 = *reinterpret_cast<const float4*>(e);
+                const float4 x1 = *reinterpret_cast<const float4*>(e + E_PITCH);
+                const float4 x2 = *reinterpret_cast<const float4*>(e + 2 * E_PITCH);
+                fma4_acc(acc0, x0, k[6]); fma4_acc(acc0, x1, k[7]); fma4_acc(acc0, x2, k[8]);
+                fma4_acc(acc1, x0, k[3]); fma4_acc(acc1, x1, k[4]); fma4_acc(acc1, x2, k[5]);
+                fma4_acc(acc2, x0, k[0]); fma4_acc(acc2, x1, k[1]); fma4_acc(acc2, x2, k[2]);
+                if (r >= 2) emit(acc0);
+                acc0 = acc1; acc1 = acc2; acc2 = zero;
+            }
+        } else {
+            float4 p0 = *reinterpret_cast<const float4*>(e);
+            float4 p1 = *reinterpret_cast<const float4*>(e + E_PITCH);
+            float4 p2 = *reinterpret_cast<const float4*>(e + 2 * E_PITCH);
+            for (int oy = rows.oy0; oy < rows.oy1; ++oy) {
+                e += WIN * E_PITCH;
+                float4 acc4 = zero;
+                fma4_acc(acc4, p0, k[0]); fma4_acc(acc4, p1, k[1]); fma4_acc(acc4, p2, k[2]);
+                const float4 m0 = *reinterpret_cast<const float4*>(e);
+                const float4 m1 = *reinterpret_cast<const float4*>(e + E_PITCH);
+                const float4 m2 = *reinterpret_cast<const float4*>(e + 2 * E_PITCH);
+                fma4_acc(acc4, m0, k[3]); fma4_acc(acc4, m1, k[4]); fma4_acc(acc4, m2, k[5]);
+                e += WIN * E_PITCH;
+                p0 = *reinterpret_cast<const float4*>(e);
+                p1 = *reinterpret_cast<const float4*>(e + E_PITCH);
+                p2 = *reinterpret_cast<const float4*>(e + 2 * E_PITCH);
+                fma4_acc(acc4, p0, k[6]); fma4_acc(acc4, p1, k[7]); fma4_acc(acc4, p2, k[8]);
+                emit(acc4);
+            }
+        }
+    }
+}
+
+// Shared-memory pointers of one CTA: [window 0 (, window 1)][weight ring][E slots][parameter blocks][barriers].
+template <int NKB, int X3> struct XdwShared {
+    using L = XdwSmem<NKB, X3>;
+    uint8_t* smem;
+    float* E;                   // [NE][256][E_PITCH]
+    float* PAR;                 // [X3 ? NE : 2][PAR_ROWS][NC]
+    uint64_t *full, *empty;     // weight stage s loaded / free
+    uint64_t *wfull, *wempty;   // window b loaded (TMA transaction count) / free: its item's last chunk has finished its MMAs
+    uint64_t *efull, *eempty;   // pipelined: E slot s written by phase (a) / drained by phase (b)
+    __device__ explicit XdwShared(uint8_t* raw) {
+        // 1024-byte alignment for SWIZZLE_128B; offset arithmetic (not an integer round-trip of the pointer) keeps the shared
+        // address space visible to the compiler, so E is accessed with LDS/STS instead of generic LD/ST.
+        smem = raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u);
+        E = reinterpret_cast<float*>(smem + L::E_OFF);
+        PAR = reinterpret_cast<float*>(smem + L::PAR_OFF);
+        full = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
+        empty = full + L::STAGES;
+        wfull = empty + L::STAGES;
+        wempty = wfull + L::WBUF;
+        efull = wempty + L::WBUF;
+        eempty = efull + L::NE;
+    }
+};
+
+// Serial schedule (plain TF32).  For each chunk all 8 worker warps run the expand MMAs, phase (a) into E, a barrier, phase
+// (b) from E, a barrier.  X3 != 0: see xdw_ws_kernel.
 template <int STRIDE, int X3, int NKB, int KSL, bool SAVE>
 __global__ void __launch_bounds__(NUM_THREADS, XdwSmem<NKB, X3>::MINB)
 xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
     using L = XdwSmem<NKB, X3>;
-    constexpr int TO = STRIDE == 1 ? 14 : 7;                    // output tile edge
-    constexpr int STAGES = L::STAGES, STAGE_BYTES = L::STAGE_BYTES, WBUF = L::WBUF;
+    constexpr int TO = STRIDE == 1 ? 14 : 7;
     extern __shared__ uint8_t smem_raw[];
-    // 1024-byte alignment for SWIZZLE_128B; offset arithmetic (not an integer round-trip of the pointer) keeps
-    // the shared address space visible to the compiler, so E is accessed with LDS/STS instead of generic LD/ST.
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* ring = smem + L::RING;                              // stage s: [w heads] (+ [w tails])
-    float* E = reinterpret_cast<float*>(smem + L::E_OFF);
-    float* PAR = reinterpret_cast<float*>(smem + L::PAR_OFF);   // [2][PAR_ROWS][NC]
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
-    uint64_t* empty = full + STAGES;
-    uint64_t* wfull = empty + STAGES;                            // window b loaded (TMA transaction count)
-    uint64_t* wempty = wfull + WBUF;                             // window b free: its item's last chunk has finished its MMAs
-
+    const XdwShared<NKB, X3> sh(smem_raw);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // Persistent CTA: work item = (image, output tile, channel-chunk group), items strided over the grid.
-    // Both roles walk the same item sequence; the weight ring runs across item boundaries and the window is
-    // refilled as soon as it is free, so the loads of item i+1 are in flight while the workers are still busy with item i.
-    // The item sequence of a CTA advances by gridDim.x; the (group, tile x, tile y, image) digits of the item index are
-    // carried along incrementally — one runtime decomposition per thread at kernel start instead of four integer divisions per item.
-    struct Item { int prob, img, oh0, ow0, c_begin, c_end; };
-    struct ItemIter { int item, grp, tx, ty, img2; };          // img2: image index over both problems
-    auto iter_begin = [&]() {
-        ItemIter it;
-        int v = it.item = blockIdx.x;
-        it.grp = v % a.groups; v /= a.groups; it.tx = v % a.tiles_x; v /= a.tiles_x; it.ty = v % a.tiles_y; it.img2 = v / a.tiles_y;
-        return it;
-    };
-    auto iter_next = [&](ItemIter& it) {
-        it.item += gridDim.x;
-        it.grp += a.d_grp; if (it.grp >= a.groups) { it.grp -= a.groups; ++it.tx; }
-        it.tx += a.d_tx;   if (it.tx >= a.tiles_x) { it.tx -= a.tiles_x; ++it.ty; }
-        it.ty += a.d_ty;   if (it.ty >= a.tiles_y) { it.ty -= a.tiles_y; ++it.img2; }
-        it.img2 += a.d_img;
-    };
-    auto decode = [&](const ItemIter& it) {
-        Item w;
-        w.prob = it.img2 >= a.B ? 1 : 0; w.img = it.img2 - w.prob * a.B;
-        w.oh0 = it.ty * TO; w.ow0 = it.tx * TO;
-        w.c_begin = it.grp * a.chunks_per_group; w.c_end = min(a.nchunks, w.c_begin + a.chunks_per_group);
-        return w;
-    };
-
     if (warp == NUM_WORKERS / 32 && lane == 0) {
         prefetch_tensormap(&mp.x[0]);
         prefetch_tensormap(&mp.w[0]);
-        if (X3) prefetch_tensormap(&mp.wlo[0]);
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], NUM_WORKERS / 32); }
-        for (int b = 0; b < WBUF; ++b) { mbar_init(&wfull[b], 1); mbar_init(&wempty[b], NUM_WORKERS / 32); }
+        for (int s = 0; s < L::STAGES; ++s) { mbar_init(&sh.full[s], 1); mbar_init(&sh.empty[s], NUM_WORKERS / 32); }
+        for (int b = 0; b < L::WBUF; ++b) { mbar_init(&sh.wfull[b], 1); mbar_init(&sh.wempty[b], NUM_WORKERS / 32); }
         fence_barrier_init();
     }
     __syncthreads();
 
     if (warp == NUM_WORKERS / 32) {
-        if (lane == 0) {
-            // ===== TMA producer: the x window once per item, then the W1 rows of every (chunk, k-block) =====
-            int it = 0, n = 0;
-            for (ItemIter ii = iter_begin(); ii.item < a.n_items; iter_next(ii), ++n) {
-                const Item w = decode(ii);
-                const int ey0 = w.oh0 * STRIDE - a.pad, ex0 = w.ow0 * STRIDE - a.pad;     // window origin in e / x coordinates
-                const int b = n % WBUF;
-                mbar_wait(&wempty[b], ((uint32_t)(n / WBUF) & 1u) ^ 1u);
-                uint8_t* win = smem + b * L::WIN_BYTES;                                     // [k-block][half][128 pixels][32 channels]
-                mbar_expect_tx(&wfull[b], (uint32_t)L::WIN_BYTES);
-#pragma unroll
-                for (int kb = 0; kb < NKB; ++kb) {
-                    tma_load_4d(&mp.x[w.prob], win + kb * KB_BYTES, &wfull[b], kb * BK, ex0, ey0, w.img);
-                    tma_load_4d(&mp.x[w.prob], win + kb * KB_BYTES + HALF_BYTES, &wfull[b], kb * BK, ex0, ey0 + 8, w.img);
-                }
-                for (int c = w.c_begin; c < w.c_end; ++c)
-                    for (int kb = 0; kb < NKB; ++kb, ++it) {
-                        const int s = it % STAGES;
-                        mbar_wait(&empty[s], ((uint32_t)(it / STAGES) & 1u) ^ 1u);
-                        uint8_t* st = ring + s * STAGE_BYTES;
-                        mbar_expect_tx(&full[s], (uint32_t)STAGE_BYTES);
-                        tma_load_2d(&mp.w[w.prob], st, &full[s], kb * BK, c * NC);
-                        if (X3) tma_load_2d(&mp.wlo[w.prob], st + B_BYTES, &full[s], kb * BK, c * NC);
-                    }
-            }
-        }
+        if (lane == 0) produce<STRIDE, X3, NKB>(mp, a, sh.smem, sh.full, sh.empty, sh.wfull, sh.wempty);
         return;
     }
 
     // ===== workers: 8 warps =====
     const int half = warp >> 2, wq = warp & 3;         // warpgroup = window half (rows 128 half ..), warp within it
     const int t = threadIdx.x;                         // 0..255
-    const int cq = t & 7, slot = t >> 3;               // depthwise role: channel quad within the chunk, output slot (0..31)
-    // Per-chunk parameters (BN1 scale/bias, nine depthwise taps, BN2 scale/bias: 13 rows of 32 channels) are
-    // staged through a double-buffered shared-memory block: thread t < 208 owns one float2 of the block, loads
-    // it for chunk i+1 before it starts its MMAs for chunk i and parks it after phase (a) —
-    // the global-load latency is off the critical path and phases (a)/(b) read parameters with LDS.
-    const int prow = t >> 4, pcol = (t & 15) * 2;
-    const bool par_owner = t < PAR_ROWS * 16;
-    const float* psrc[2] = {nullptr, nullptr};
-    if (par_owner) {
-#pragma unroll
-        for (int q = 0; q < 2; ++q)
-            psrc[q] = (prow == 0 ? a.scale1[q] : prow == 1 ? a.bias1[q] : prow == 11 ? a.scale2[q] : prow == 12 ? a.bias2[q]
-                                                                                   : a.wdw[q] + (size_t)(prow - 2) * a.mid) + pcol;
-    }
-    auto load_par = [&](int prob, int c) {
-        float2 v = make_float2(0.f, 0.f);
-        if (par_owner && c * NC + pcol < a.mid) v = __ldg(reinterpret_cast<const float2*>(psrc[prob] + c * NC));
-        return v;
-    };
-    auto park_par = [&](int slot_idx, const float2& v) {
-        if (par_owner) *reinterpret_cast<float2*>(PAR + slot_idx * (PAR_ROWS * NC) + prow * NC + pcol) = v;
-    };
-    ItemIter ii = iter_begin();
-    if (ii.item < a.n_items) { const Item w0 = decode(ii); park_par(0, load_par(w0.prob, w0.c_begin)); }
+    const int cq = t & 7;                              // depthwise role: channel quad within the chunk, output slot t >> 3
+    // Parameters of chunk i+1 are loaded before the MMAs of chunk i and parked (slot (i+1) & 1) after its phase (a).
+    const ParLoader pl(a, t);
+    ItemIter ii(a);
+    if (ii.item < a.n_items) { const Item w0 = ii.decode<TO>(a); pl.park(sh.PAR, pl.load(a, w0.prob, w0.c_begin)); }
     worker_barrier();
-    // Depthwise role of this thread: output column dw_ox and row group dw_rg of the tile's valid columns x as many row groups
-    // as fit in the 32 slots.  A tile has TO columns / rows except in the last tile column / row: the thread's role for both
-    // column counts is worked out once here (bytes of `role`: ox full, rg full, ox edge, rg edge), the row grouping of the four
-    // tile kinds comes from the host (a.geom); the item loop only selects.
-    const int ncols_e = a.Wo - (a.tiles_x - 1) * TO, nrows_e = a.Ho - (a.tiles_y - 1) * TO;
-    const unsigned role = (unsigned)(slot % TO) | (unsigned)(slot / TO) << 8 | (unsigned)(slot % ncols_e) << 16 | (unsigned)(slot / ncols_e) << 24;
+    const unsigned role = dw_role<TO>(a, t >> 3);
     int cc = 0, it = 0;
     for (int n = 0; ii.item < a.n_items; ++n) {
-      const Item w = decode(ii);
-      const int wb = n % WBUF;
-      const uint8_t* win = smem + wb * L::WIN_BYTES + half * HALF_BYTES;     // this warpgroup's half of k-block 0
-      mbar_wait(&wfull[wb], (uint32_t)(n / WBUF) & 1u);
-      const int img = w.img, oh0 = w.oh0, ow0 = w.ow0;
-      const int ey0 = oh0 * STRIDE - a.pad, ex0 = ow0 * STRIDE - a.pad;
-      // this thread's output column dw_ox and output rows [dw_oy0, dw_oy1) of the tile
-      const bool col_e = ii.tx == a.tiles_x - 1, row_e = ii.ty == a.tiles_y - 1;
-      const int nrows = row_e ? nrows_e : TO;
-      const unsigned g8 = a.geom >> ((col_e ? 16 : 0) + (row_e ? 8 : 0));
-      const int rpt = (int)(g8 & 15u), n_rg = (int)((g8 >> 4) & 15u);
-      const unsigned r16 = role >> (col_e ? 16 : 0);
-      const int dw_ox = (int)(r16 & 255u), dw_rg = (int)((r16 >> 8) & 255u);
-      const int dw_oy0 = dw_rg * rpt, dw_oy1 = dw_rg < n_rg ? min(nrows, dw_oy0 + rpt) : 0;
+      const Item w = ii.decode<TO>(a);
+      const int wb = n % L::WBUF;
+      const uint8_t* win = sh.smem + wb * L::WIN_BYTES + half * HALF_BYTES;     // this warpgroup's half of k-block 0
+      mbar_wait(&sh.wfull[wb], (uint32_t)(n / L::WBUF) & 1u);
+      const DwRows rows = dw_rows<TO>(a, ii, role);
       int next_first = -1, next_prob = 0;              // first chunk (and problem) of this CTA's next item (-1: none)
-      iter_next(ii);
-      if (ii.item < a.n_items) { const Item wn = decode(ii); next_first = wn.c_begin; next_prob = wn.prob; }
+      ii.next(a);
+      if (ii.item < a.n_items) { const Item wn = ii.decode<TO>(a); next_first = wn.c_begin; next_prob = wn.prob; }
       for (int c = w.c_begin; c < w.c_end; ++c, ++cc) {
         const int buf = cc & 1;
-        const int ch0 = c * NC;
-        const float* par = PAR + buf * (PAR_ROWS * NC);
+        const float* par = sh.PAR + buf * PAR_FLOATS;
         const int c_next = c + 1 < w.c_end ? c + 1 : next_first;
         float2 pf = make_float2(0.f, 0.f);
-        if (c_next >= 0) pf = load_par(c + 1 < w.c_end ? w.prob : next_prob, c_next);
-        // expand GEMM of this chunk: rows [64 mb, 64 mb + 64) of window half `half`, 32 channels
+        if (c_next >= 0) pf = pl.load(a, c + 1 < w.c_end ? w.prob : next_prob, c_next);
         float acc[2][NC / 2];
-#pragma unroll
-        for (int mb = 0; mb < 2; ++mb)
-#pragma unroll
-            for (int i = 0; i < NC / 2; ++i) acc[mb][i] = 0.f;
-#pragma unroll
-        for (int kb = 0; kb < NKB; ++kb, ++it) {
-            // k-steps of this k-block: all four, except KSL in the last one, where the steps over the channels past Cin
-            // (zero-filled by TMA) would only add zeros.  Known at compile time, so no wgmma sits behind a branch.
-            const int nks = kb + 1 < NKB ? BK / MMA_K : KSL;
-            const int s = it % STAGES;
-            mbar_wait(&full[s], (uint32_t)(it / STAGES) & 1u);
-            const uint8_t* xa = win + kb * KB_BYTES;
-            const uint32_t sb = smem_u32(ring + s * STAGE_BYTES);
-            if constexpr (X3 != 0) {
-                uint32_t hi[2][BK / MMA_K][4], lo[2][BK / MMA_K][4];
-#pragma unroll
-                for (int mb = 0; mb < 2; ++mb)
-#pragma unroll
-                    for (int k = 0; k < nks; ++k) {
-                        float v[4];
-                        load_a_frag(xa, mb * 64, k * MMA_K, wq, lane, v);
-                        split_frag(v, hi[mb][k], lo[mb][k]);
-                    }
-                wgmma_fence();
-#pragma unroll
-                for (int k = 0; k < nks; ++k) {
-                    const uint64_t db = make_smem_desc(sb + k * MMA_K * 4);
-                    const uint64_t dbl = make_smem_desc(sb + B_BYTES + k * MMA_K * 4);
-#pragma unroll
-                    for (int mb = 0; mb < 2; ++mb) {
-                        Wgmma<NC>::rs(acc[mb], hi[mb][k], db, 1u);       // x_hi * w_hi
-                        Wgmma<NC>::rs(acc[mb], lo[mb][k], db, 1u);       // x_lo * w_hi
-                        Wgmma<NC>::rs(acc[mb], hi[mb][k], dbl, 1u);      // x_hi * w_lo
-                    }
-                }
-            } else {
-                const uint32_t sa = smem_u32(xa);
-                wgmma_fence();
-#pragma unroll
-                for (int k = 0; k < nks; ++k) {
-                    const uint64_t db = make_smem_desc(sb + k * MMA_K * 4);
-#pragma unroll
-                    for (int mb = 0; mb < 2; ++mb)
-                        Wgmma<NC>::ss(acc[mb], make_smem_desc(sa + mb * 64 * BKB + k * MMA_K * 4), db, 1u);
-                }
-            }
-            wgmma_commit();
-            wgmma_wait<0>();
-            __syncwarp();
-            mbar_arrive_if(&empty[s], lane == 0);
-        }
-        mbar_arrive_if(&wempty[wb], lane == 0 && c + 1 == w.c_end);     // the item's last MMAs have read the window
-        // (a) accumulators -> BN1 + ReLU -> E.  Channels past `mid` have zero scale and bias in the parameter block, pixels
-        // outside the image are zeroed: that is the zero padding of e the depthwise conv expects.
-#pragma unroll
-        for (int mb = 0; mb < 2; ++mb)
-#pragma unroll
-            for (int hr = 0; hr < 2; ++hr) {
-                const int r = mb * 64 + wq * 16 + (lane >> 2) + 8 * hr;      // row within the half: r = hh*16 + ww
-                const int ey = ey0 + half * 8 + (r >> 4), ex = ex0 + (r & 15);
-                const bool inside = ey >= 0 && ey < a.H && ex >= 0 && ex < a.W;
-                float* erow = E + (size_t)(half * 128 + r) * E_PITCH;
-                bool own = false;
-                float* esave = nullptr;
-                if constexpr (SAVE) {
-                    own = inside && ey >= oh0 * STRIDE && ey < (oh0 + TO) * STRIDE && ex >= ow0 * STRIDE && ex < (ow0 + TO) * STRIDE;
-                    esave = a.e_out[w.prob] + (((size_t)img * a.H + ey) * a.W + ex) * a.mid + ch0;
-                }
-#pragma unroll
-                for (int j = 0; j < NC / 8; ++j) {
-                    const int ch = 8 * j + 2 * (lane & 3);
-                    float2 o = make_float2(0.f, 0.f);
-                    if (inside) {
-                        const float2 sc = *reinterpret_cast<const float2*>(par + ch);
-                        const float2 bi = *reinterpret_cast<const float2*>(par + NC + ch);
-                        o.x = fmaxf(fmaf(acc[mb][4 * j + 2 * hr], sc.x, bi.x), 0.f);
-                        o.y = fmaxf(fmaf(acc[mb][4 * j + 2 * hr + 1], sc.y, bi.y), 0.f);
-                    }
-                    *reinterpret_cast<float2*>(erow + ch) = o;
-                    if (SAVE && own && ch0 + ch < a.mid) *reinterpret_cast<float2*>(esave + ch) = o;
-                }
-            }
-        if (c_next >= 0) park_par(buf ^ 1, pf);        // slot buf^1 was last read in the previous chunk's phase (b)
+        expand_gemm<X3, NKB, KSL>(acc, win, sh.smem + L::RING, sh.full, sh.empty, it, wq, lane);
+        mbar_arrive_if(&sh.wempty[wb], lane == 0 && c + 1 == w.c_end);     // the item's last MMAs have read the window
+        bn1_relu<STRIDE, SAVE>(acc, sh.E, par, a, w, c * NC, half, wq, lane);
+        if (c_next >= 0) pl.park(sh.PAR + (buf ^ 1) * PAR_FLOATS, pf);     // slot buf^1 was last read in the previous chunk's phase (b)
         worker_barrier();
-        // (b) depthwise 3x3 over E.  One thread owns one output column of one channel quad and walks down
-        // its rows, so every E row it reads is shared by the (up to three) output rows it feeds: 3 LDS.128
-        // per input row instead of 9 per output.  Tap order per output stays (ky, kx) ascending -> same
-        // rounding as the unfused path.
-        if (cq * 4 < a.mid - ch0 && dw_oy0 < dw_oy1) {
-            const int ch = ch0 + cq * 4;
-            float4 k[9];
-#pragma unroll
-            for (int q = 0; q < 9; ++q) k[q] = *reinterpret_cast<const float4*>(par + (2 + q) * NC + cq * 4);
-            const float4 s2 = *reinterpret_cast<const float4*>(par + 11 * NC + cq * 4);
-            const float4 b2 = *reinterpret_cast<const float4*>(par + 12 * NC + cq * 4);
-            float* orow = a.out[w.prob] + (((size_t)img * a.Ho + oh0 + dw_oy0) * a.Wo + ow0 + dw_ox) * a.mid + ch;
-            const size_t orow_stride = (size_t)a.Wo * a.mid;
-            auto emit = [&](const float4& acc4) {
-                float4 o = fma4(acc4, s2, b2);
-                o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
-                if (a.round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
-                *reinterpret_cast<float4*>(orow) = o;
-                orow += orow_stride;
-            };
-            const float* e = E + (size_t)((dw_oy0 * STRIDE) * WIN + dw_ox * STRIDE) * E_PITCH + cq * 4;
-            const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (STRIDE == 1) {
-                float4 acc0 = zero, acc1 = zero, acc2 = zero;          // outputs r-2 (gets ky=2), r-1 (ky=1), r (ky=0)
-                const int n_in = dw_oy1 - dw_oy0 + 2;
-#pragma unroll 3
-                for (int r = 0; r < n_in; ++r, e += WIN * E_PITCH) {
-                    const float4 x0 = *reinterpret_cast<const float4*>(e);
-                    const float4 x1 = *reinterpret_cast<const float4*>(e + E_PITCH);
-                    const float4 x2 = *reinterpret_cast<const float4*>(e + 2 * E_PITCH);
-                    fma4_acc(acc0, x0, k[6]); fma4_acc(acc0, x1, k[7]); fma4_acc(acc0, x2, k[8]);
-                    fma4_acc(acc1, x0, k[3]); fma4_acc(acc1, x1, k[4]); fma4_acc(acc1, x2, k[5]);
-                    fma4_acc(acc2, x0, k[0]); fma4_acc(acc2, x1, k[1]); fma4_acc(acc2, x2, k[2]);
-                    if (r >= 2) emit(acc0);
-                    acc0 = acc1; acc1 = acc2; acc2 = zero;
-                }
-            } else {
-                float4 p0 = *reinterpret_cast<const float4*>(e);
-                float4 p1 = *reinterpret_cast<const float4*>(e + E_PITCH);
-                float4 p2 = *reinterpret_cast<const float4*>(e + 2 * E_PITCH);
-                for (int oy = dw_oy0; oy < dw_oy1; ++oy) {
-                    e += WIN * E_PITCH;
-                    float4 acc4 = zero;
-                    fma4_acc(acc4, p0, k[0]); fma4_acc(acc4, p1, k[1]); fma4_acc(acc4, p2, k[2]);
-                    const float4 m0 = *reinterpret_cast<const float4*>(e);
-                    const float4 m1 = *reinterpret_cast<const float4*>(e + E_PITCH);
-                    const float4 m2 = *reinterpret_cast<const float4*>(e + 2 * E_PITCH);
-                    fma4_acc(acc4, m0, k[3]); fma4_acc(acc4, m1, k[4]); fma4_acc(acc4, m2, k[5]);
-                    e += WIN * E_PITCH;
-                    p0 = *reinterpret_cast<const float4*>(e);
-                    p1 = *reinterpret_cast<const float4*>(e + E_PITCH);
-                    p2 = *reinterpret_cast<const float4*>(e + 2 * E_PITCH);
-                    fma4_acc(acc4, p0, k[6]); fma4_acc(acc4, p1, k[7]); fma4_acc(acc4, p2, k[8]);
-                    emit(acc4);
-                }
-            }
-        }
+        depthwise<STRIDE>(sh.E, par, a, w, c * NC, cq, rows);
         worker_barrier();                              // E and the parameter slot are free for the next chunk
       }
+    }
+}
+
+// Pipelined, warp-specialized schedule (3xTF32).  The MMA warpgroups run chunk i's expand GEMM and phase (a) into E slot
+// i % NE, hand the slot to the depthwise warpgroup and go straight on to chunk i+1, so the tensor cores work on one chunk
+// while the FP32 pipes run the depthwise conv of the previous one.  Slot hand-offs are mbarriers (efull: 256 MMA-thread
+// arrivals, eempty: 128 depthwise-thread arrivals); a chunk's parameter block lives beside its E slot.  No CTA-wide barrier
+// inside the item loop; the E ring runs across item boundaries like the weight ring.
+template <int STRIDE, int X3, int NKB, int KSL, bool SAVE>
+__global__ void __launch_bounds__(WS_THREADS, 1)
+xdw_ws_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
+    using L = XdwSmem<NKB, X3>;
+    constexpr int TO = STRIDE == 1 ? 14 : 7, NE = L::NE;
+    constexpr int PROD_WARP = (NUM_WORKERS + DW_THREADS) / 32;
+    extern __shared__ uint8_t smem_raw[];
+    const XdwShared<NKB, X3> sh(smem_raw);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (warp == PROD_WARP && lane == 0) {
+        prefetch_tensormap(&mp.x[0]);
+        prefetch_tensormap(&mp.w[0]);
+        prefetch_tensormap(&mp.wlo[0]);
+        for (int s = 0; s < L::STAGES; ++s) { mbar_init(&sh.full[s], 1); mbar_init(&sh.empty[s], NUM_WORKERS / 32); }
+        for (int b = 0; b < L::WBUF; ++b) { mbar_init(&sh.wfull[b], 1); mbar_init(&sh.wempty[b], NUM_WORKERS / 32); }
+        for (int s = 0; s < NE; ++s) { mbar_init(&sh.efull[s], NUM_WORKERS); mbar_init(&sh.eempty[s], DW_THREADS); }
+        fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (warp >= PROD_WARP) {                           // warpgroup 3: the TMA producer
+        setmaxnreg_dec<PROD_REGS>();
+        if (warp == PROD_WARP && lane == 0) produce<STRIDE, X3, NKB>(mp, a, sh.smem, sh.full, sh.empty, sh.wfull, sh.wempty);
+        return;
+    }
+
+    if (warp >= NUM_WORKERS / 32) {                    // warpgroup 2: phase (b) of every chunk, slot by slot
+        setmaxnreg_inc<DW_REGS>();
+        const int d = threadIdx.x - NUM_WORKERS, cq = d & 7;
+        unsigned role[DW_ROLES];
+#pragma unroll
+        for (int j = 0; j < DW_ROLES; ++j) role[j] = dw_role<TO>(a, (d >> 3) + j * (DW_THREADS / 8));
+        int cc = 0;
+        for (ItemIter ii(a); ii.item < a.n_items; ii.next(a)) {
+            const Item w = ii.decode<TO>(a);
+            DwRows rows[DW_ROLES];
+#pragma unroll
+            for (int j = 0; j < DW_ROLES; ++j) rows[j] = dw_rows<TO>(a, ii, role[j]);
+            for (int c = w.c_begin; c < w.c_end; ++c, ++cc) {
+                const int s = cc % NE;
+                mbar_wait(&sh.efull[s], (uint32_t)(cc / NE) & 1u);
+#pragma unroll 1
+                for (int j = 0; j < DW_ROLES; ++j) depthwise<STRIDE>(sh.E + s * E_FLOATS, sh.PAR + s * PAR_FLOATS, a, w, c * NC, cq, rows[j]);
+                mbar_arrive(&sh.eempty[s]);
+            }
+        }
+        return;
+    }
+
+    // warpgroups 0-1: expand GEMM of window half `half`, then phase (a) into the next free E slot
+    setmaxnreg_inc<MMA_REGS>();
+    const int half = warp >> 2, wq = warp & 3;
+    const ParLoader pl(a, threadIdx.x);
+    int cc = 0, it = 0, n = 0;
+    for (ItemIter ii(a); ii.item < a.n_items; ii.next(a), ++n) {
+        const Item w = ii.decode<TO>(a);
+        const int wb = n % L::WBUF;
+        const uint8_t* win = sh.smem + wb * L::WIN_BYTES + half * HALF_BYTES;
+        mbar_wait(&sh.wfull[wb], (uint32_t)(n / L::WBUF) & 1u);
+        for (int c = w.c_begin; c < w.c_end; ++c, ++cc) {
+            const int s = cc % NE;
+            float* par = sh.PAR + s * PAR_FLOATS;
+            const float2 pf = pl.load(a, w.prob, c);
+            float acc[2][NC / 2];
+            expand_gemm<X3, NKB, KSL>(acc, win, sh.smem + L::RING, sh.full, sh.empty, it, wq, lane);
+            mbar_arrive_if(&sh.wempty[wb], lane == 0 && c + 1 == w.c_end);
+            mbar_wait(&sh.eempty[s], ((uint32_t)(cc / NE) & 1u) ^ 1u);     // phase (b) of chunk cc - NE has drained the slot
+            pl.park(par, pf);
+            worker_barrier();                          // the parameter block is complete before phase (a) reads BN1 from it
+            bn1_relu<STRIDE, SAVE>(acc, sh.E + s * E_FLOATS, par, a, w, c * NC, half, wq, lane);
+            mbar_arrive(&sh.efull[s]);
+        }
     }
 }
 
 template <int STRIDE, int X3, int NKB, int KSL, bool SAVE>
 int launch(const XdwMaps& mp, const XdwArgs& a, int grid, cudaStream_t st) {
     constexpr size_t smem = XdwSmem<NKB, X3>::SMEM;
-    SMK_CHECK_CUDA((set_max_dynamic_smem<xdw_kernel<STRIDE, X3, NKB, KSL, SAVE>>((int)smem)));
-    SMK_LAUNCH((xdw_kernel<STRIDE, X3, NKB, KSL, SAVE>), dim3(grid), dim3(NUM_THREADS), smem, st, mp, a);
+    if constexpr (X3 != 0) {
+        SMK_CHECK_CUDA((set_max_dynamic_smem<xdw_ws_kernel<STRIDE, X3, NKB, KSL, SAVE>>((int)smem)));
+        SMK_LAUNCH((xdw_ws_kernel<STRIDE, X3, NKB, KSL, SAVE>), dim3(grid), dim3(WS_THREADS), smem, st, mp, a);
+    } else {
+        SMK_CHECK_CUDA((set_max_dynamic_smem<xdw_kernel<STRIDE, X3, NKB, KSL, SAVE>>((int)smem)));
+        SMK_LAUNCH((xdw_kernel<STRIDE, X3, NKB, KSL, SAVE>), dim3(grid), dim3(NUM_THREADS), smem, st, mp, a);
+    }
     SMK_CHECK_LAUNCH();
     return 0;
 }
