@@ -62,4 +62,7 @@ int smk_encoder_backward_train(const SmkEncoder* h, const SmkEncoderTrainArgs* a
 }
 #endif
 
+/* Test entry points of the train-mode kernels (not part of the drop-in surface): include/smirk_b200_train_debug.h. */
+#include "smirk_b200_train_debug.h"
+
 #endif /* SMIRK_B200_TRAIN_H */

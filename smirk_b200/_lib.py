@@ -1,4 +1,5 @@
-"""ctypes binding of libsmirk_b200.so (the C ABI declared in include/smirk_b200.h and include/smirk_b200_train.h).
+"""ctypes binding of libsmirk_b200.so (the C ABI declared in include/smirk_b200.h, include/smirk_b200_train.h and
+include/smirk_b200_train_debug.h).
 
 There is deliberately no fallback: if the shared library is missing or a call fails, the product
 path raises.  Build with ``python -m smirk_b200.build`` (or ``__graft_entry__.build()``).
@@ -145,7 +146,19 @@ TRAIN_BINDINGS = [
     ("smk_encoder_backward_train", _i, [_vp, C.POINTER(SmkEncoderTrainArgs), _vp, _i, _vp, _sz, _vp, _vp, _vp, _vp,
                                         C.POINTER(SmkEncoderTrainGrads), _vp, _sz, STREAM]),
 ]
-_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS + TRAIN_BINDINGS if args[-1:] == [STREAM])
+# The same for include/smirk_b200_train_debug.h (test entry points of the train-mode kernels), in that header's order.
+TRAIN_DEBUG_BINDINGS = [
+    ("smk_debug_train_bn_forward", _i, [_vp, _i, _i, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_debug_train_bn_backward", _i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_debug_train_pw_wgrad", _i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, STREAM]),
+    ("smk_debug_train_dw_forward", _i, [_vp, _vp, _i, _i, _i, _i, _vp, STREAM]),
+    ("smk_debug_train_dw_wgrad", _i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _sz, STREAM]),
+    ("smk_debug_train_dw_dgrad", _i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, STREAM]),
+    ("smk_debug_train_stem_forward", _i, [_vp, _vp, _i, _i, _i, _vp, STREAM]),
+    ("smk_debug_train_stem_wgrad", _i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, STREAM]),
+    ("smk_debug_train_head_backward", _i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, STREAM]),
+]
+_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS + TRAIN_BINDINGS + TRAIN_DEBUG_BINDINGS if args[-1:] == [STREAM])
 
 
 def lib():
@@ -157,7 +170,7 @@ def lib():
         raise RuntimeError("smirk_b200: %s not found — build it with `python -m smirk_b200.build` "
                            "(there is no CPU / PyTorch fallback)" % LIB_PATH)
     L = C.CDLL(LIB_PATH)
-    for name, restype, argtypes in BINDINGS + TRAIN_BINDINGS:
+    for name, restype, argtypes in BINDINGS + TRAIN_BINDINGS + TRAIN_DEBUG_BINDINGS:
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, [_vp if a is STREAM else a for a in argtypes]
     if L.smk_version() != 100:

@@ -630,6 +630,43 @@ int dw_dgrad(const float* g, const float* w, const float* res, int B, int H, int
     return 0;
 }
 
+// The stem conv (3x3 stride 2 TF-SAME, one padding for both axes): img [B,3,H,W] -> z [B,Ho,Wo,16].
+int stem_forward(const float* img, const float* w, int B, int H, int W, float* z, cudaStream_t st) {
+    const int Ho = (H + 1) / 2, Wo = (W + 1) / 2;
+    const long M = (long)B * Ho * Wo;
+    SMK_TAG("stem_fwd", 4.0 * ((double)B * 3 * H * W + M * 16), 2.0 * 27 * 16 * M, st);
+    SMK_LAUNCH(stem_fwd_kernel, dim3(cdiv(M, 128)), dim3(128), 0, st, img, w, B, H, W, Ho, Wo, same_pad_begin(H, 2), z);
+    SMK_CHECK_LAUNCH();
+    return 0;
+}
+
+// The stem's weight gradient from g [B,Ho,Wo,16] (gradient of z): split K over at most 512 chunks of >= 1024 pixels.
+int stem_wgrad(const float* g, const float* img, int B, int H, int W, float* part, float* out, cudaStream_t st) {
+    const int Ho = (H + 1) / 2, Wo = (W + 1) / 2;
+    const long M = (long)B * Ho * Wo;
+    const int nch = (int)std::min<long>(cdiv(M, 1024), 512);
+    SMK_TAG("stem_wgrad", 4.0 * ((double)M * 16 + (double)B * 3 * H * W), 2.0 * 432 * M, st);
+    SMK_LAUNCH(stem_wgrad_kernel, dim3(nch), dim3(448), 0, st, g, img, B, H, W, Ho, Wo, same_pad_begin(H, 2), cdiv(M, nch), part);
+    SMK_CHECK_LAUNCH();
+    return sum_chunks(part, nch, 432, out, st);
+}
+
+// The head's backward: g [B][n_out] (gradient of the clamped output) -> gp (gradient of the pre-clamp output), gy
+// [B,HW,C] (of the features before the pool), and the head's weight gradients gw [n_out][C] / gbias [n_out] (either may
+// be null) from the pooled features [B][C].
+int head_backward(const float* g, const float* raw, const uint8_t* codes, const float* w, const float* pooled, int B, int n_out, int HW, int C,
+                  float* gp, float* gy, float* gw, float* gbias, cudaStream_t st) {
+    SMK_TAG("train_head_bwd", 4.0 * ((double)B * HW * C + (double)n_out * C + 3.0 * B * n_out), 2.0 * B * C * n_out, st);
+    SMK_LAUNCH(head_bwd_train_kernel, dim3(B, cdiv(C, 256)), dim3(256), (size_t)n_out * 4, st, g, raw, codes, w, n_out, HW, C, gp, gy);
+    SMK_CHECK_LAUNCH();
+    if (gw || gbias) {
+        SMK_TAG("train_head_wgrad", 4.0 * ((double)B * (n_out + C) + (double)n_out * C), 2.0 * B * C * n_out, st);
+        SMK_LAUNCH(head_wgrad_kernel, dim3(cdiv((long)n_out * (C + 1), 256)), dim3(256), 0, st, gp, pooled, B, n_out, C, gw, gbias);
+        SMK_CHECK_LAUNCH();
+    }
+    return 0;
+}
+
 // Topology of a train handle: the layer list, activation sizes and the saved layout (names: the reference's module paths
 // — a conv's pre-BN output under the conv, a ReLU output under its BatchNorm as in the eval layout, a block's output
 // under the block, the pooled features under `<encoder>.pooled`, a head's pre-clamp output under the head).
@@ -789,9 +826,7 @@ extern "C" int smk_encoder_forward_train(const SmkEncoder* h, const SmkEncoderTr
         // the stem
         {
             const long M = (long)B * 112 * 112;
-            SMK_TAG("stem_fwd", 4.0 * ((double)B * 3 * 224 * 224 + M * 16), 2.0 * 27 * 16 * M, st);
-            SMK_LAUNCH(stem_fwd_kernel, dim3(cdiv(M, 128)), dim3(128), 0, st, img, v.bn(0).w, B, 224, 224, 112, 112, same_pad_begin(224, 2), SV(bb.sv_zstem));
-            SMK_CHECK_LAUNCH();
+            if (int rc = stem_forward(img, v.bn(0).w, B, 224, 224, SV(bb.sv_zstem), st)) return rc;
             if (int rc = bn_forward(v.bn(0), SV(bb.sv_zstem), M, 16, eps, mom, st_i, st_i + 16, nullptr, true, false, SV(bb.sv_stem), W.part, st)) return rc;
             st_i += 32;
         }
@@ -896,18 +931,9 @@ extern "C" int smk_encoder_backward_train(const SmkEncoder* h, const SmkEncoderT
         float *gy = W.buf[0], *t1 = W.buf[1], *t2 = W.buf[2];
         int res = 7;
         {   // head -> gradient of the cn output (t1); head weight gradients
-            const int C = bb.feat;
-            SMK_TAG("train_head_bwd", 4.0 * ((double)B * res * res * C + (double)bb.n_out * C + 3.0 * B * bb.n_out), 2.0 * B * C * bb.n_out, st);
-            SMK_LAUNCH(head_bwd_train_kernel, dim3(B, cdiv(C, 256)), dim3(256), (size_t)bb.n_out * 4, st, g_out[i], SV(bb.sv_head), bb.codes,
-                       args->head_w[i], bb.n_out, res * res, C, W.gp, t1);
-            SMK_CHECK_LAUNCH();
-            float* gw = grads ? grads->head_w[i] : nullptr;
-            float* gb = grads ? grads->head_b[i] : nullptr;
-            if (gw || gb) {
-                SMK_TAG("train_head_wgrad", 4.0 * ((double)B * (bb.n_out + C) + (double)bb.n_out * C), 2.0 * B * C * bb.n_out, st);
-                SMK_LAUNCH(head_wgrad_kernel, dim3(cdiv((long)bb.n_out * (C + 1), 256)), dim3(256), 0, st, W.gp, SV(bb.sv_pool), B, bb.n_out, C, gw, gb);
-                SMK_CHECK_LAUNCH();
-            }
+            if (int rc = head_backward(g_out[i], SV(bb.sv_head), bb.codes, args->head_w[i], SV(bb.sv_pool), B, bb.n_out, res * res, bb.feat, W.gp, t1,
+                                       grads ? grads->head_w[i] : nullptr, grads ? grads->head_b[i] : nullptr, st))
+                return rc;
         }
         int p = (int)pk.size();
         for (int bi = (int)bb.blocks.size() - 1; bi >= 0; --bi) {
@@ -952,15 +978,120 @@ extern "C" int smk_encoder_backward_train(const SmkEncoder* h, const SmkEncoderT
         const long M = (long)B * 112 * 112;
         if (int rc = bnb(0, t1, SV(bb.sv_stem), SV(bb.sv_zstem), M, t1)) return rc;
         if (r0.gw) {
-            const int nch = (int)std::min<long>(cdiv(M, 1024), 512);
-            SMK_TAG("stem_wgrad", 4.0 * ((double)M * 16 + (double)B * 3 * 224 * 224), 2.0 * 432 * M, st);
-            SMK_LAUNCH(stem_wgrad_kernel, dim3(nch), dim3(448), 0, st, t1, img, B, 224, 224, 112, 112, same_pad_begin(224, 2), cdiv(M, nch), W.wpart);
-            SMK_CHECK_LAUNCH();
-            if (int rc = sum_chunks(W.wpart, nch, 432, r0.gw, st)) return rc;
+            if (int rc = stem_wgrad(t1, img, B, 224, 224, W.wpart, r0.gw, st)) return rc;
         }
         g_stem[i] = t1; w_stem[i] = W.stem_t;
         return 0;
     });
     if (rc || !g_img) return rc;
     return enc::stem_dgrad(g_stem, w_stem, B, g_img, main_st);
+}
+
+// ---- test entry points (include/smirk_b200_train_debug.h): each runs the host helper of the train path ----------------
+
+namespace {
+
+BnRef debug_bn(const float* gamma, const float* beta, float* rmean, float* rvar, int64_t* nbt, float* g_gamma, float* g_beta) {
+    BnRef r{};
+    r.gamma = const_cast<float*>(gamma); r.beta = const_cast<float*>(beta); r.rmean = rmean; r.rvar = rvar; r.nbt = (long long*)nbt;
+    r.ggamma = g_gamma; r.gbeta = g_beta;
+    return r;
+}
+
+int check_dw(const char* fn, int B, int H, int C, int stride) {
+    SMK_REQUIRE(B > 0 && H > 0 && C > 0, "%s: B, H and C must be positive", fn);
+    SMK_REQUIRE(stride == 1 || stride == 2, "%s: stride must be 1 or 2", fn);
+    return 0;
+}
+
+}  // namespace
+
+extern "C" int smk_debug_train_bn_forward(const float* z, int M, int C, float eps, float momentum, const float* gamma, const float* beta,
+                                          float* rmean, float* rvar, int64_t* nbt, const float* res, int relu, int round, float* mean,
+                                          float* invstd, float* y, void* ws, size_t ws_bytes, void* stream) {
+    const char* fn = "smk_debug_train_bn_forward";
+    SMK_REQUIRE(z && gamma && beta && rmean && rvar && nbt && mean && invstd && y && ws, "%s: null argument", fn);
+    SMK_REQUIRE(M > 0 && C > 0 && C % 4 == 0, "%s: M > 0 and C > 0 with C %% 4 == 0 (the apply reads float4)", fn);
+    SMK_REQUIRE(momentum <= 1.f && eps > 0.f, "%s: momentum must be in [0, 1] (or negative for None) and eps > 0", fn);
+    smk::Workspace w(ws, ws_bytes);
+    double2* part = w.take<double2>((size_t)kMaxChunks * C);
+    SMK_REQUIRE(part, "%s: workspace too small", fn);
+    return bn_forward(debug_bn(gamma, beta, rmean, rvar, nbt, nullptr, nullptr), z, M, C, eps, momentum, mean, invstd, res, relu != 0, round != 0, y,
+                      part, (cudaStream_t)stream);
+}
+
+extern "C" int smk_debug_train_bn_backward(const float* g, const float* y, const float* z, const float* mean, const float* invstd,
+                                           const float* gamma, int M, int C, int round, float* gz, float* g_gamma, float* g_beta, void* ws,
+                                           size_t ws_bytes, void* stream) {
+    const char* fn = "smk_debug_train_bn_backward";
+    SMK_REQUIRE(g && z && mean && invstd && gamma && gz && ws, "%s: null argument", fn);
+    SMK_REQUIRE(M > 0 && C > 0, "%s: M and C must be positive", fn);
+    smk::Workspace w(ws, ws_bytes);
+    double2* part = w.take<double2>((size_t)kMaxChunks * C);
+    float* gb = w.take<float>(2 * (size_t)C);
+    SMK_REQUIRE(part && gb, "%s: workspace too small", fn);
+    return bn_backward(debug_bn(gamma, nullptr, nullptr, nullptr, nullptr, g_gamma, g_beta), g, y, z, mean, invstd, M, C, round != 0, gz, part, gb,
+                       (cudaStream_t)stream);
+}
+
+extern "C" int smk_debug_train_pw_wgrad(const float* g, const float* a, int M, int Co, int Ci, float* out, void* ws, size_t ws_bytes, void* stream) {
+    const char* fn = "smk_debug_train_pw_wgrad";
+    SMK_REQUIRE(g && a && out && ws, "%s: null argument", fn);
+    SMK_REQUIRE(M > 0 && Co > 0 && Ci > 0, "%s: M, Co and Ci must be positive", fn);
+    smk::Workspace w(ws, ws_bytes);
+    float* part = w.take<float>(kWgradPart);
+    SMK_REQUIRE(part, "%s: workspace too small", fn);
+    return pw_wgrad(g, a, M, Co, Ci, part, out, (cudaStream_t)stream);
+}
+
+extern "C" int smk_debug_train_dw_forward(const float* a, const float* w, int B, int H, int C, int stride, float* z, void* stream) {
+    const char* fn = "smk_debug_train_dw_forward";
+    SMK_REQUIRE(a && w && z, "%s: null argument", fn);
+    if (int rc = check_dw(fn, B, H, C, stride)) return rc;
+    return dw_forward(a, w, B, H, C, stride, z, (cudaStream_t)stream);
+}
+
+extern "C" int smk_debug_train_dw_wgrad(const float* g, const float* a, int B, int H, int C, int stride, float* out, void* ws, size_t ws_bytes,
+                                        void* stream) {
+    const char* fn = "smk_debug_train_dw_wgrad";
+    SMK_REQUIRE(g && a && out && ws, "%s: null argument", fn);
+    if (int rc = check_dw(fn, B, H, C, stride)) return rc;
+    smk::Workspace w(ws, ws_bytes);
+    float* part = w.take<float>(kWgradPart);
+    SMK_REQUIRE(part, "%s: workspace too small", fn);
+    return dw_wgrad(g, a, B, H, C, stride, part, out, (cudaStream_t)stream);
+}
+
+extern "C" int smk_debug_train_dw_dgrad(const float* g, const float* w, const float* res, int B, int H, int C, int stride, float* out, void* stream) {
+    const char* fn = "smk_debug_train_dw_dgrad";
+    SMK_REQUIRE(g && w && out, "%s: null argument", fn);
+    if (int rc = check_dw(fn, B, H, C, stride)) return rc;
+    return dw_dgrad(g, w, res, B, H, C, stride, out, (cudaStream_t)stream);
+}
+
+extern "C" int smk_debug_train_stem_forward(const float* img, const float* w, int B, int H, int W, float* z, void* stream) {
+    const char* fn = "smk_debug_train_stem_forward";
+    SMK_REQUIRE(img && w && z, "%s: null argument", fn);
+    SMK_REQUIRE(B > 0 && H > 0 && W > 0, "%s: B, H and W must be positive", fn);
+    SMK_REQUIRE(same_pad_begin(H, 2) == same_pad_begin(W, 2), "%s: H and W must have the same parity (one TF-SAME padding)", fn);
+    return stem_forward(img, w, B, H, W, z, (cudaStream_t)stream);
+}
+
+extern "C" int smk_debug_train_stem_wgrad(const float* g, const float* img, int B, int H, int W, float* out, void* ws, size_t ws_bytes, void* stream) {
+    const char* fn = "smk_debug_train_stem_wgrad";
+    SMK_REQUIRE(g && img && out && ws, "%s: null argument", fn);
+    SMK_REQUIRE(B > 0 && H > 0 && W > 0, "%s: B, H and W must be positive", fn);
+    SMK_REQUIRE(same_pad_begin(H, 2) == same_pad_begin(W, 2), "%s: H and W must have the same parity (one TF-SAME padding)", fn);
+    smk::Workspace w(ws, ws_bytes);
+    float* part = w.take<float>(kWgradPart);
+    SMK_REQUIRE(part, "%s: workspace too small", fn);
+    return stem_wgrad(g, img, B, H, W, part, out, (cudaStream_t)stream);
+}
+
+extern "C" int smk_debug_train_head_backward(const float* g, const float* raw, const uint8_t* codes, const float* w, const float* pooled, int B,
+                                             int n_out, int HW, int C, float* gp, float* g_feat, float* g_w, float* g_b, void* stream) {
+    const char* fn = "smk_debug_train_head_backward";
+    SMK_REQUIRE(g && raw && w && pooled && gp && g_feat, "%s: null argument", fn);
+    SMK_REQUIRE(B > 0 && n_out > 0 && n_out <= 4096 && HW > 0 && C > 0, "%s: B, HW and C must be positive and n_out in [1, 4096]", fn);
+    return head_backward(g, raw, codes, w, pooled, B, n_out, HW, C, gp, g_feat, g_w, g_b, (cudaStream_t)stream);
 }

@@ -60,6 +60,55 @@ def test_train_entry_points_reject_bad_arguments(native_lib):
     assert L.smk_encoder_train_workspace_bytes(nul, 4) == 0
 
 
+def test_train_debug_header_prototypes_are_exported_and_bound(native_lib):
+    """include/smirk_b200_train_debug.h (the train-kernel test entry points) is included by smirk_b200_train.h; the
+    library exports each of its 9 prototypes, and each has exactly one row in _lib.TRAIN_DEBUG_BINDINGS (header order, no
+    row shared with the other tables) with the same return type and parameters, the trailing stream included."""
+    from smirk_b200 import _lib
+    train = open(os.path.join(ROOT, "include", "smirk_b200_train.h")).read()
+    assert '#include "smirk_b200_train_debug.h"' in train
+    hdr = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "smirk_b200_train_debug.h")).read(), flags=re.S)
+    protos = re.findall(r"^\s*([A-Za-z_][\w ]*?\**)\s*\b(smk_\w+)\s*\(([^)]*)\)\s*;", hdr, flags=re.M)
+    assert [name for _, name, _ in protos] == [name for name, _, _ in _lib.TRAIN_DEBUG_BINDINGS] and len(protos) == 9
+    names = {name for name, _, _ in _lib.TRAIN_DEBUG_BINDINGS}
+    assert not names & {name for name, _, _ in _lib.BINDINGS + _lib.TRAIN_BINDINGS}
+    table = {name: (restype, args) for name, restype, args in _lib.TRAIN_DEBUG_BINDINGS}
+    for ret, name, params in protos:
+        assert hasattr(native_lib, name), "missing export: " + name
+        restype, args = table[name]
+        assert ret.strip() == "int" and restype is C.c_int, name
+        params = [q.strip() for q in params.split(",") if q.strip()]
+        assert len(args) == len(params), name
+        for q, a in zip(params, args):
+            if q.endswith("stream"):
+                assert a is _lib.STREAM, (name, q)
+            elif "*" in q:
+                assert a in (C.c_void_p, C.c_char_p) or issubclass(a, C._Pointer), (name, q)
+            else:
+                assert a is {"int": C.c_int, "size_t": C.c_size_t, "float": C.c_float}[q.rsplit(None, 1)[0]], (name, q)
+        assert name in _lib._TAKES_STREAM and args[-1:] == [_lib.STREAM], name
+
+
+def test_train_debug_entry_points_reject_bad_arguments(native_lib):
+    """The train-kernel test entry points check their arguments before they launch anything."""
+    L = native_lib
+    buf, nul, n64 = C.c_void_p(16), C.c_void_p(0), C.c_void_p(64)
+    rc = L.smk_debug_train_bn_forward(buf, 100, 6, 1e-3, 0.1, buf, buf, buf, buf, buf, nul, 1, 0, buf, buf, buf, buf, 1 << 24, nul)
+    assert rc < 0 and b"C % 4 == 0" in L.smk_last_error()
+    rc = L.smk_debug_train_bn_forward(buf, 100, 8, 1e-3, 1.5, buf, buf, buf, buf, buf, nul, 1, 0, buf, buf, buf, buf, 1 << 24, nul)
+    assert rc < 0 and b"momentum" in L.smk_last_error()
+    rc = L.smk_debug_train_bn_forward(buf, 100, 8, 1e-3, 0.1, buf, buf, buf, buf, nul, nul, 1, 0, buf, buf, buf, buf, 1 << 24, nul)
+    assert rc < 0 and b"null argument" in L.smk_last_error()
+    rc = L.smk_debug_train_bn_backward(buf, nul, buf, buf, buf, buf, 100, 8, 0, buf, nul, nul, n64, 64, nul)
+    assert rc < 0 and b"workspace too small" in L.smk_last_error()
+    assert L.smk_debug_train_pw_wgrad(buf, buf, 100, 8, 8, buf, n64, 64, nul) < 0 and b"workspace too small" in L.smk_last_error()
+    assert L.smk_debug_train_dw_forward(buf, buf, 1, 8, 8, 3, buf, nul) < 0 and b"stride" in L.smk_last_error()
+    assert L.smk_debug_train_dw_dgrad(buf, nul, nul, 1, 8, 8, 1, buf, nul) < 0 and b"null argument" in L.smk_last_error()
+    assert L.smk_debug_train_stem_forward(buf, buf, 1, 16, 15, buf, nul) < 0 and b"parity" in L.smk_last_error()
+    rc = L.smk_debug_train_head_backward(buf, buf, nul, buf, buf, 2, 0, 49, 8, buf, buf, nul, nul, nul)
+    assert rc < 0 and b"n_out" in L.smk_last_error()
+
+
 def _encoder():
     import smirk_b200
     return smirk_b200.SmirkEncoder()
