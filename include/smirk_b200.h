@@ -184,6 +184,49 @@ int smk_encoder_saved_tensor(const SmkEncoder* h, int B, int i, const char** nam
 size_t smk_encoder_backward_workspace_bytes(const SmkEncoder* h, int B);
 int smk_encoder_backward(const SmkEncoder* h, int B, const float* saved, size_t saved_bytes, const float* g_pose_cam,
                          const float* g_shape, const float* g_expr, float* g_img, void* ws, size_t ws_bytes, void* stream);
+/* Train mode (BatchNorm over batch statistics, the reference trainer's encoder.train(), base_trainer.py:108-111) and the
+ * gradients of every parameter (src/smirk_trainer.py:34-73).
+ * A train handle holds the topology only — the backbones in `backbones` (bit set: 1 pose, 2 shape, 4 expression), the head
+ * widths and the precision (as SmkEncoderDesc's; precision 2 computes as 1, there is no fused train kernel) — and is
+ * destroyed by smk_encoder_destroy.  Every call reads the parameters through the device pointers of SmkEncoderTrainArgs and
+ * repacks the 1x1 weights into the workspace, so an optimizer step needs no new handle.  Calls never allocate or
+ * synchronise, use no float atomics (bitwise reproducible) and are CUDA-graph capturable; the eval entry points above reject
+ * a train handle.  BatchNorm couples the images of a batch: outputs are not independent of the other images. */
+typedef struct {
+    /* Per backbone, DEVICE pointers of its `encoder.*` tensors in the order of SmkEncoderDesc.tensors (per conv: weight,
+     * BN weight, bias, running_mean, running_var); running_mean / running_var are updated in place.                   */
+    float* const* tensors[3];
+    int n_tensors[3];
+    int64_t* const* num_batches_tracked[3];   /* one per BatchNorm, in the same order; each is incremented by one     */
+    const float* head_w[3];
+    const float* head_b[3];
+    float momentum[3];         /* running-statistics factor; negative = None (cumulative average, 1 / num_batches_tracked) */
+    float eps[3];
+} SmkEncoderTrainArgs;
+typedef struct {
+    /* Gradient outputs (written, not accumulated), NULL = not wanted.  tensors[i][j] is the gradient of
+     * SmkEncoderTrainArgs.tensors[i][j]; the running-statistics entries must be NULL.  tensors[i] itself may be NULL.  */
+    float* const* tensors[3];
+    float* head_w[3];
+    float* head_b[3];
+} SmkEncoderTrainGrads;
+int smk_encoder_train_create(int backbones, int n_shape, int n_exp, int precision, SmkEncoder** out);
+/* Workspace of both train calls.  smk_encoder_saved_bytes / smk_encoder_saved_tensor describe the train handle's saved
+ * buffer: per BatchNorm the conv's pre-BN output (named after the conv, e.g. "shape_encoder.encoder.blocks.2.1.conv_pw"),
+ * every ReLU output (named as in eval mode), every block output ("...blocks.2.1"), the pooled features
+ * ("shape_encoder.pooled", [B,feat]) and the heads' pre-clamp outputs, followed by the batch statistics (not listed). */
+size_t smk_encoder_train_workspace_bytes(const SmkEncoder* h, int B);
+/* Train-mode forward: outputs as smk_encoder_forward; updates the running statistics and num_batches_tracked of every
+ * BatchNorm.  saved (>= smk_encoder_saved_bytes) keeps the activations for smk_encoder_backward_train; with saved == NULL
+ * they live in ws, which must then hold smk_encoder_saved_bytes more. */
+int smk_encoder_forward_train(const SmkEncoder* h, const SmkEncoderTrainArgs* args, const float* img, int B, float* pose_cam,
+                              float* shape, float* expr, float* saved, size_t saved_bytes, void* ws, size_t ws_bytes, void* stream);
+/* Train-mode backward from the forward's saved buffer (args and img: those of the forward).  Upstream gradients may be
+ * NULL: a backbone without one, or whose parameters want no gradient while g_img is NULL, launches nothing (and writes
+ * none of its gradients).  g_img [B,3,224,224] (NULL: not wanted) is written. */
+int smk_encoder_backward_train(const SmkEncoder* h, const SmkEncoderTrainArgs* args, const float* img, int B, const float* saved,
+                               size_t saved_bytes, const float* g_pose_cam, const float* g_shape, const float* g_expr, float* g_img,
+                               const SmkEncoderTrainGrads* grads, void* ws, size_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * SmirkGenerator — replaces SmirkGenerator.forward (src/smirk_generator.py:51-86), eval-mode BN.
@@ -368,11 +411,44 @@ int smk_debug_stem_ds(const float* img, int B, int H, int W, const float* stem_w
                       const float* dw_w, const float* dw_s, const float* dw_b, const float* pw_w, const float* pw_s,
                       const float* pw_b, int stride, int round_out, float* out, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Train-kernel test entry points (used by tests/ to check the train-mode kernels one at a time against torch; not
+ * part of the drop-in surface).  All pointers are device pointers; each calls the host helper the train calls use, so
+ * the launches are theirs.  Activations are NHWC [M = B*H*W, C]; weights are in torch's layout.  ws / ws_bytes: scratch
+ * for the partial sums, at least 512 * C * 16 bytes for bn_forward, that + 8 * C for bn_backward, and 16 MiB (4M
+ * floats) for the weight gradients.
+ *   bn_forward   : batch statistics of z -> mean, invstd; running_mean / running_var / num_batches_tracked updated as
+ *                  the train forward does (momentum < 0: None); y = gamma * (z - mean) * invstd + beta (+ res) (ReLU when
+ *                  relu) (TF32-rounded when round).  C % 4 == 0.
+ *   bn_backward  : g (gradient of y; masked by [y > 0] when y is given) -> gz, which may alias g; g_gamma / g_beta
+ *                  (either may be NULL).
+ *   pw_wgrad     : out [Co][Ci] = sum over the M pixels of g[p][co] * a[p][ci].
+ *   dw_*         : the 3x3 depthwise conv (TF-SAME, stride 1 or 2) of a [B,H,H,C] with w [C][1][3][3]; dgrad adds res
+ *                  (may be NULL) to the input gradient [B,H,H,C].
+ *   stem_*       : the stem conv of img [B,3,H,W] (3x3 stride 2 TF-SAME, 3 -> 16; H and W of one parity), z and its
+ *                  gradient g [B,ceil(H/2),ceil(W/2),16]; out [16][3][3][3].
+ *   head_backward: codes [n_out] (NULL: all 0) per output: 0 pass, 1 clamp [0, 1], 2 ReLU, 3 clamp [-0.2, 0.2], judged
+ *                  on the pre-clamp output raw [B][n_out]; gp [B][n_out] (gradient of raw), g_feat [B,HW,C] (of the
+ *                  features before the global pool), g_w [n_out][C] and g_b [n_out] (either may be NULL) from pooled [B][C].
+ * ---------------------------------------------------------------------------------------------- */
+int smk_debug_train_bn_forward(const float* z, int M, int C, float eps, float momentum, const float* gamma, const float* beta,
+                               float* rmean, float* rvar, int64_t* nbt, const float* res, int relu, int round, float* mean,
+                               float* invstd, float* y, void* ws, size_t ws_bytes, void* stream);
+int smk_debug_train_bn_backward(const float* g, const float* y, const float* z, const float* mean, const float* invstd,
+                                const float* gamma, int M, int C, int round, float* gz, float* g_gamma, float* g_beta, void* ws,
+                                size_t ws_bytes, void* stream);
+int smk_debug_train_pw_wgrad(const float* g, const float* a, int M, int Co, int Ci, float* out, void* ws, size_t ws_bytes, void* stream);
+int smk_debug_train_dw_forward(const float* a, const float* w, int B, int H, int C, int stride, float* z, void* stream);
+int smk_debug_train_dw_wgrad(const float* g, const float* a, int B, int H, int C, int stride, float* out, void* ws, size_t ws_bytes,
+                             void* stream);
+int smk_debug_train_dw_dgrad(const float* g, const float* w, const float* res, int B, int H, int C, int stride, float* out, void* stream);
+int smk_debug_train_stem_forward(const float* img, const float* w, int B, int H, int W, float* z, void* stream);
+int smk_debug_train_stem_wgrad(const float* g, const float* img, int B, int H, int W, float* out, void* ws, size_t ws_bytes, void* stream);
+int smk_debug_train_head_backward(const float* g, const float* raw, const uint8_t* codes, const float* w, const float* pooled, int B,
+                                  int n_out, int HW, int C, float* gp, float* g_feat, float* g_w, float* g_b, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
-
-/* SmirkEncoder train mode (batch-statistics BatchNorm and parameter gradients): include/smirk_b200_train.h. */
-#include "smirk_b200_train.h"
 
 #endif /* SMIRK_B200_H */

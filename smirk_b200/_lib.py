@@ -1,5 +1,4 @@
-"""ctypes binding of libsmirk_b200.so (the C ABI declared in include/smirk_b200.h, include/smirk_b200_train.h and
-include/smirk_b200_train_debug.h).
+"""ctypes binding of libsmirk_b200.so (the C ABI declared in include/smirk_b200.h).
 
 There is deliberately no fallback: if the shared library is missing or a call fails, the product
 path raises.  Build with ``python -m smirk_b200.build`` (or ``__graft_entry__.build()``).
@@ -95,6 +94,11 @@ BINDINGS = [
     ("smk_encoder_saved_tensor", _i, [_vp, _i, _i, C.POINTER(C.c_char_p), C.POINTER(_sz), C.POINTER(C.c_int)]),
     ("smk_encoder_backward_workspace_bytes", _sz, [_vp, _i]),
     ("smk_encoder_backward", _i, [_vp, _i, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_encoder_train_create", _i, [_i, _i, _i, _i, _vpp]),
+    ("smk_encoder_train_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_encoder_forward_train", _i, [_vp, C.POINTER(SmkEncoderTrainArgs), _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp, _sz, STREAM]),
+    ("smk_encoder_backward_train", _i, [_vp, C.POINTER(SmkEncoderTrainArgs), _vp, _i, _vp, _sz, _vp, _vp, _vp, _vp,
+                                        C.POINTER(SmkEncoderTrainGrads), _vp, _sz, STREAM]),
     ("smk_generator_create", _i, [C.POINTER(SmkGeneratorDesc), _vpp]),
     ("smk_generator_destroy", None, [_vp]),
     ("smk_generator_workspace_bytes", _sz, [_vp, _i]),
@@ -137,17 +141,6 @@ BINDINGS = [
     ("smk_debug_gemm_tc3x", _i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _vp, _i, STREAM]),
     ("smk_debug_xdw3x", _i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _vp, STREAM]),
     ("smk_debug_stem_ds", _i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, STREAM]),
-]
-# The same for include/smirk_b200_train.h (SmirkEncoder train mode), in that header's order.
-TRAIN_BINDINGS = [
-    ("smk_encoder_train_create", _i, [_i, _i, _i, _i, _vpp]),
-    ("smk_encoder_train_workspace_bytes", _sz, [_vp, _i]),
-    ("smk_encoder_forward_train", _i, [_vp, C.POINTER(SmkEncoderTrainArgs), _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp, _sz, STREAM]),
-    ("smk_encoder_backward_train", _i, [_vp, C.POINTER(SmkEncoderTrainArgs), _vp, _i, _vp, _sz, _vp, _vp, _vp, _vp,
-                                        C.POINTER(SmkEncoderTrainGrads), _vp, _sz, STREAM]),
-]
-# The same for include/smirk_b200_train_debug.h (test entry points of the train-mode kernels), in that header's order.
-TRAIN_DEBUG_BINDINGS = [
     ("smk_debug_train_bn_forward", _i, [_vp, _i, _i, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _sz, STREAM]),
     ("smk_debug_train_bn_backward", _i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _sz, STREAM]),
     ("smk_debug_train_pw_wgrad", _i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, STREAM]),
@@ -158,7 +151,7 @@ TRAIN_DEBUG_BINDINGS = [
     ("smk_debug_train_stem_wgrad", _i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, STREAM]),
     ("smk_debug_train_head_backward", _i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, STREAM]),
 ]
-_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS + TRAIN_BINDINGS + TRAIN_DEBUG_BINDINGS if args[-1:] == [STREAM])
+_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS if args[-1:] == [STREAM])
 
 
 def lib():
@@ -170,7 +163,7 @@ def lib():
         raise RuntimeError("smirk_b200: %s not found — build it with `python -m smirk_b200.build` "
                            "(there is no CPU / PyTorch fallback)" % LIB_PATH)
     L = C.CDLL(LIB_PATH)
-    for name, restype, argtypes in BINDINGS + TRAIN_BINDINGS + TRAIN_DEBUG_BINDINGS:
+    for name, restype, argtypes in BINDINGS:
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, [_vp if a is STREAM else a for a in argtypes]
     if L.smk_version() != 100:

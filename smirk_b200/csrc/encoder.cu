@@ -18,7 +18,6 @@
 #include "gemm_tc.cuh"
 #include "xdw_tc.cuh"
 #include <math.h>
-#include <string>
 
 namespace {
 
@@ -103,41 +102,33 @@ extern "C" int smk_encoder_create(const SmkEncoderDesc* desc, SmkEncoder** out) 
     SmkEncoder* h = new SmkEncoder();
     h->n_shape = desc->n_shape; h->n_exp = desc->n_exp; h->precision = tc ? 1 : 0; h->fuse_xdw = desc->precision >= 2; h->x3 = desc->precision == 3;
     const bool x3 = h->x3;
-    const int n_outs[3] = {6, desc->n_shape, desc->n_exp + 5};
     cudaError_t e = cudaSuccess;
+    // saved-tensor layout: forward order within a backbone (names: the reference's module paths)
+    auto add = [h](const std::string& name, int H, int C) { return h->saved.add(name, H, H, C); };
     for (int i = 0; i < 3; ++i) {
-        const BlockDef* defs = i == 0 ? kSmall : kLarge;
-        const int nb = i == 0 ? (int)(sizeof(kSmall) / sizeof(BlockDef)) : (int)(sizeof(kLarge) / sizeof(BlockDef));
         Backbone& bb = h->bb[i];
         if (desc->n_tensors[i] == 0 || desc->tensors[i] == nullptr) continue;        // backbone not part of this handle
         h->present[i] = true;
+        build_backbone(h, i);
         TensorCursor cur{desc->tensors[i], desc->n_tensors[i]};
         bool ok = fold_conv(cur, 2, 3, 16, false, h->arena, &bb.stem, &e, false, &bb.stem_d);
-        int cin = 16, res = 112;
-        size_t max_act = (size_t)112 * 112 * 16;
-        for (int k = 0; ok && k < nb; ++k) {
-            Block b{};
-            b.kind = defs[k].kind; b.stride = defs[k].stride; b.cin = cin; b.cout = defs[k].cout;
-            b.skip = b.kind != CN && b.stride == 1 && b.cin == b.cout;
+        bb.sv_stem = add(std::string(kEncName[i]) + ".encoder.bn1", 112, 16);
+        for (Block& b : bb.blocks) {
+            if (!ok) break;
             if (b.kind == DS) {
-                b.mid = cin;
-                ok = fold_conv(cur, 1, cin, cin, false, h->arena, &b.dw, &e, false, &b.dw_d);
-                if (ok && tc) { TensorCursor again = cur; ok = fold_conv(again, 0, cin, b.cout, false, h->arena, &b.pw_f32, &e); }
-                ok = ok && fold_conv(cur, 0, cin, b.cout, tc, h->arena, &b.pw, &e, x3, &b.pw_d);
+                ok = fold_conv(cur, 1, b.cin, b.cin, false, h->arena, &b.dw, &e, false, &b.dw_d);
+                if (ok && tc) { TensorCursor again = cur; ok = fold_conv(again, 0, b.cin, b.cout, false, h->arena, &b.pw_f32, &e); }
+                ok = ok && fold_conv(cur, 0, b.cin, b.cout, tc, h->arena, &b.pw, &e, x3, &b.pw_d);
+                b.sv_a = add(b.path + ".bn1", b.hout, b.cin);
             } else if (b.kind == IR) {
-                b.mid = make_divisible((double)cin * defs[k].exp);
-                ok = fold_conv(cur, 0, cin, b.mid, tc, h->arena, &b.pw, &e, x3, &b.pw_d) &&
+                ok = fold_conv(cur, 0, b.cin, b.mid, tc, h->arena, &b.pw, &e, x3, &b.pw_d) &&
                      fold_conv(cur, 1, b.mid, b.mid, false, h->arena, &b.dw, &e, false, &b.dw_d) &&
                      fold_conv(cur, 0, b.mid, b.cout, tc, h->arena, &b.pwl, &e, x3, &b.pwl_d);
+                b.sv_a = add(b.path + ".bn1", b.hin, b.mid); b.sv_b = add(b.path + ".bn2", b.hout, b.mid);
             } else {
-                b.mid = cin;
-                ok = fold_conv(cur, 0, cin, b.cout, tc, h->arena, &b.pw, &e, x3, &b.pw_d);
+                ok = fold_conv(cur, 0, b.cin, b.cout, tc, h->arena, &b.pw, &e, x3, &b.pw_d);
+                b.sv_a = add(b.path + ".bn1", b.hout, b.cout);
             }
-            max_act = std::max(max_act, (size_t)res * res * b.mid);           // expanded tensor at input resolution
-            res = (res + b.stride - 1) / b.stride;
-            max_act = std::max(max_act, (size_t)res * res * std::max(b.mid, b.cout));
-            cin = b.cout;
-            bb.blocks.push_back(b);
         }
         if (!ok || cur.i != cur.n) {
             if (e != cudaSuccess) smk::set_error("smk_encoder_create: upload failed: %s", cudaGetErrorString(e));
@@ -145,46 +136,14 @@ extern "C" int smk_encoder_create(const SmkEncoderDesc* desc, SmkEncoder** out) 
                                 i, cur.i, cur.n);
             delete h; return e != cudaSuccess ? (int)e : -1;
         }
-        bb.feat = cin; bb.n_out = n_outs[i];
-        h->max_act = std::max(h->max_act, max_act);
         e = h->arena.upload(desc->head_w[i], (size_t)bb.n_out * bb.feat, &bb.head_w);
         if (e == cudaSuccess) e = h->arena.upload(desc->head_b[i], (size_t)bb.n_out, &bb.head_b);
-        if (i == 2 && e == cudaSuccess) {                  // smirk_encoder.py:105-108
-            std::vector<uint8_t> codes(bb.n_out, 0);
-            int ne = desc->n_exp;
-            codes[ne] = codes[ne + 1] = 1; codes[ne + 2] = 2; codes[ne + 3] = codes[ne + 4] = 3;
-            e = h->arena.upload(codes, &bb.codes);
-        }
         if (e != cudaSuccess) { smk::set_error("smk_encoder_create: upload failed: %s", cudaGetErrorString(e)); delete h; return (int)e; }
+        bb.sv_head = add(std::string(kEncName[i]) + "." + kHeadName[i], 1, bb.n_out);
     }
     if (!h->present[0] && !h->present[1] && !h->present[2]) { smk::set_error("smk_encoder_create: no backbone given"); delete h; return -1; }
-    {   // dgrad epilogue constants and the saved-tensor layout (names: the reference's module paths)
-        std::vector<float> ones(1024, 1.f), zeros(1024, 0.f);
-        e = h->arena.upload(ones, &h->ones);
-        if (e == cudaSuccess) e = h->arena.upload(zeros, &h->zeros);
-        if (e != cudaSuccess) { smk::set_error("smk_encoder_create: upload failed: %s", cudaGetErrorString(e)); delete h; return (int)e; }
-        auto add = [h](const std::string& name, int H, int W, int C) { return h->saved.add(name, H, W, C); };
-        for (int i = 0; i < 3; ++i) {
-            if (!h->present[i]) continue;
-            Backbone& bb = h->bb[i];
-            const std::string enc = std::string(kEncName[i]) + ".encoder.";
-            const int* stages = i == 0 ? kStageSmall : kStageLarge;
-            bb.sv_stem = add(enc + "bn1", 112, 112, 16);
-            int res = 112, stage = 0, in_stage = 0;
-            for (Block& b : bb.blocks) {
-                const std::string pre = enc + "blocks." + std::to_string(stage) + "." + std::to_string(in_stage) + ".";
-                const int ro = (res + b.stride - 1) / b.stride;
-                if (b.kind == DS) b.sv_a = add(pre + "bn1", ro, ro, b.cin);
-                else if (b.kind == IR) { b.sv_a = add(pre + "bn1", res, res, b.mid); b.sv_b = add(pre + "bn2", ro, ro, b.mid); }
-                else b.sv_a = add(pre + "bn1", ro, ro, b.cout);
-                res = ro;
-                if (++in_stage == stages[stage]) { ++stage; in_stage = 0; }
-            }
-            bb.sv_head = add(std::string(kEncName[i]) + "." + kHeadName[i], 1, 1, bb.n_out);
-        }
-    }
-    e = create_forks(h);
-    if (e != cudaSuccess) { smk::set_error("smk_encoder_create: stream/event creation failed: %s", cudaGetErrorString(e)); delete h; return (int)e; }
+    e = finish_create(h);
+    if (e != cudaSuccess) { smk::set_error("smk_encoder_create: upload or stream/event creation failed: %s", cudaGetErrorString(e)); delete h; return (int)e; }
     *out = h;
     return 0;
 }

@@ -1,29 +1,43 @@
 // The encoder handle shared by the eval path (encoder.cu) and the train-mode path (encoder_train.cu): the MobileNetV3
-// "minimal" layer lists, the per-backbone topology, and the fork/join walk over the backbones.
+// "minimal" layer lists, the per-backbone topology and its one builder, and the fork/join walk over the backbones.
 #pragma once
 #include "common.cuh"
+#include <string>
 
 namespace enc {
 
 struct ConvW { float* w = nullptr; float* wt = nullptr; float* wt_lo = nullptr; float* scale = nullptr; float* bias = nullptr; int cin = 0, cout = 0; };   // w: [K][N] fp32 path, wt: [N][K] tensor-core path (TF32 heads), wt_lo: TF32 tails (3xTF32 path)
 enum Kind { DS = 0, IR = 1, CN = 2 };
 struct BlockDef { Kind kind; int stride; float exp; int cout; };
+// path: the block's module path, <encoder>.encoder.blocks.<stage>.<i>; hin / hout: input / output resolution.
 // pw_f32: fp32 [K][N] copy of a DS block's 1x1 (fused stem path).  *_d: dgrad weights (see fold_conv).
-// sv_a / sv_b: saved-tensor indices of the block's ReLU outputs (IR: expand, depthwise; DS: depthwise; CN: its output).
-// Train handles only: sv_z[j] the pre-BN output of the block's j-th conv, sv_out the block output (DS / IR), bn0 the
-// index of the block's first BatchNorm within its backbone.
-struct Block { Kind kind; int stride, cin, mid, cout; bool skip; ConvW pw, dw, pwl; ConvW pw_f32; ConvW pw_d, dw_d, pwl_d; int sv_a = -1, sv_b = -1;
-               int sv_z[3] = {-1, -1, -1}, sv_out = -1, bn0 = 0; };
+// sv_a / sv_b: saved-tensor indices of the block's ReLU outputs (IR: expand, depthwise; DS: depthwise; CN: its output); eval handles.
+struct Block { Kind kind; int stride, cin, mid, cout; bool skip; std::string path; int hin, hout;
+               ConvW pw, dw, pwl; ConvW pw_f32; ConvW pw_d, dw_d, pwl_d; int sv_a = -1, sv_b = -1; };
+
+// Train handles walk a backbone as a flat list, in forward order, of conv + BatchNorm (+ skip) (+ ReLU) layers.  The stem is
+// entry 0, so the index is the BatchNorm's index in the tensor list (5 tensors per entry, one num_batches_tracked).
+enum Op { STEM, PW, DW };
+struct Layer {
+    Op op; int cin, cout, stride, hin, hout;
+    int sv_in, sv_z, sv_y;   // saved-tensor indices of the input (-1: the image), the pre-BN output, the BN (+ skip, ReLU) output
+    bool relu;               // ReLU after the BatchNorm
+    bool first;              // first layer of its block
+    int skip;                // last layer of a block with a skip connection: saved index of the block input; otherwise -1
+    size_t stats;            // offset in floats, within the handle's statistics area, of mean[cout]; invstd[cout] follows
+    int pw;                  // PW: index among the backbone's 1x1 convs (its slot of the per-call weight pack); otherwise -1
+};
 
 struct Backbone {
     ConvW stem, stem_d;
     std::vector<Block> blocks;
+    std::vector<Layer> layers;                 // train handles
     int feat = 0;
     float *head_w = nullptr, *head_b = nullptr;
     int n_out = 0;
     uint8_t* codes = nullptr;
-    int sv_stem = -1, sv_head = -1;
-    int sv_zstem = -1, sv_pool = -1;           // train handles: the stem's pre-BN output, the pooled features [B, feat]
+    int sv_stem = -1, sv_head = -1;            // sv_stem: eval handles (a train handle's is layers[0].sv_y)
+    int sv_pool = -1;                          // train handles: the pooled features [B, feat]
     size_t max_act = 0;                        // floats per image of the largest activation
 };
 
@@ -95,6 +109,49 @@ inline cudaError_t create_forks(SmkEncoder* h) {
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&f.fork, cudaEventDisableTiming);
     }
     return e;
+}
+
+// Everything about backbone i that follows from its layer list and the head widths: the blocks (channels, resolutions,
+// module paths), feat, n_out and the activation sizes.  Weights and saved tensors are the caller's.
+inline void build_backbone(SmkEncoder* h, int i) {
+    Backbone& bb = h->bb[i];
+    const BlockDef* defs = i == 0 ? kSmall : kLarge;
+    const int nb = i == 0 ? (int)(sizeof(kSmall) / sizeof(BlockDef)) : (int)(sizeof(kLarge) / sizeof(BlockDef));
+    const int* stages = i == 0 ? kStageSmall : kStageLarge;
+    int cin = 16, res = 112, stage = 0, in_stage = 0;
+    bb.max_act = (size_t)112 * 112 * 16;
+    for (int k = 0; k < nb; ++k) {
+        Block b{};
+        b.kind = defs[k].kind; b.stride = defs[k].stride; b.cin = cin; b.cout = defs[k].cout;
+        b.skip = b.kind != CN && b.stride == 1 && b.cin == b.cout;
+        b.mid = b.kind == IR ? make_divisible((double)cin * defs[k].exp) : cin;
+        b.hin = res; b.hout = (res + b.stride - 1) / b.stride;
+        b.path = std::string(kEncName[i]) + ".encoder.blocks." + std::to_string(stage) + "." + std::to_string(in_stage);
+        if (++in_stage == stages[stage]) { ++stage; in_stage = 0; }
+        bb.max_act = std::max(bb.max_act, (size_t)b.hin * b.hin * b.mid);           // expanded tensor at input resolution
+        bb.max_act = std::max(bb.max_act, (size_t)b.hout * b.hout * std::max(b.mid, b.cout));
+        res = b.hout; cin = b.cout;
+        bb.blocks.push_back(b);
+    }
+    bb.feat = cin;
+    bb.n_out = i == 0 ? 6 : i == 1 ? h->n_shape : h->n_exp + 5;
+    h->max_act = std::max(h->max_act, bb.max_act);
+}
+
+// The device state every handle has besides its layers: the expression head's clamp codes (smirk_encoder.py:105-108), the
+// unit scale / zero bias of the dgrad GEMM epilogues, and the fork/join streams and events; -> cudaSuccess or the first error.
+inline cudaError_t finish_create(SmkEncoder* h) {
+    cudaError_t e = cudaSuccess;
+    if (h->present[2]) {
+        const int ne = h->n_exp;
+        std::vector<uint8_t> codes(h->bb[2].n_out, 0);
+        codes[ne] = codes[ne + 1] = 1; codes[ne + 2] = 2; codes[ne + 3] = codes[ne + 4] = 3;
+        e = h->arena.upload(codes, &h->bb[2].codes);
+    }
+    std::vector<float> ones(1024, 1.f), zeros(1024, 0.f);
+    if (e == cudaSuccess) e = h->arena.upload(ones, &h->ones);
+    if (e == cudaSuccess) e = h->arena.upload(zeros, &h->zeros);
+    return e == cudaSuccess ? create_forks(h) : e;
 }
 
 // One unit of work: n = 1 backbone, or the pair idx = {1, 2}, on stream st.

@@ -2,18 +2,19 @@
 // head gradients, for the reference trainer's encoder steps (src/smirk_trainer.py:34-73 with base_trainer.py:108-111's
 // .train()).
 //
-// A train handle holds the topology only; every call reads the module's current parameters through device pointers
-// (SmkEncoderTrainArgs) and repacks the 1x1 weights into the workspace, so an optimizer step needs no new handle.  The
-// forward runs the unfused layer sequence (BN cannot be folded): per conv the pre-BN output z, then per BatchNorm a
-// per-channel reduction over fixed pixel chunks (fp64 partial sums), a one-CTA finalise (mean, invstd, running stats,
-// num_batches_tracked), and an apply step (gamma * xhat + beta, + skip, ReLU).  The backward walks each backbone in
-// reverse: BN backward (fixed-order fp64 sums of g and g * xhat, then g_z), 1x1 dgrads through smk::conv over W^T, a
-// depthwise transposed conv, and weight gradients as split-K reductions over fixed pixel chunks with a fixed-order
-// reduce.  No atomics: results are bitwise reproducible, and every call is CUDA-graph capturable.
+// A train handle holds the topology only: per backbone a flat list of conv + BatchNorm layers (enc::Layer, built from the
+// blocks of enc::build_backbone), which the forward walks front to back and the backward back to front.  Every call reads
+// the module's current parameters through device pointers (SmkEncoderTrainArgs) and repacks the 1x1 weights into the
+// workspace, so an optimizer step needs no new handle.  The forward runs the unfused layer sequence (BN cannot be
+// folded): per conv the pre-BN output z, then per BatchNorm a per-channel reduction over fixed pixel chunks (fp64 partial
+// sums), a one-CTA finalise (mean, invstd, running stats, num_batches_tracked), and an apply step (gamma * xhat + beta,
+// + skip, ReLU).  The backward runs per layer the BN backward (fixed-order fp64 sums of g and g * xhat, then g_z), the
+// weight gradient as a split-K reduction over fixed pixel chunks with a fixed-order reduce, and the dgrad: a 1x1 through
+// smk::conv over W^T, or a depthwise transposed conv.  No atomics: results are bitwise reproducible, and every call is
+// CUDA-graph capturable.
 #include "encoder.cuh"
 #include "nn_kernels.cuh"
 #include "gemm_tc.cuh"
-#include <string>
 
 namespace {
 
@@ -451,20 +452,15 @@ struct View {
     }
 };
 
-int n_bn(const Backbone& bb) {
-    int n = 1;
-    for (const Block& b : bb.blocks) n += b.kind == IR ? 3 : b.kind == DS ? 2 : 1;
-    return n;
-}
 // floats of one copy of a backbone's 1x1 weights
 size_t pw_floats(const Backbone& bb) {
     size_t n = 0;
-    for (const Block& b : bb.blocks) n += b.kind == IR ? (size_t)b.cin * b.mid + (size_t)b.mid * b.cout : (size_t)b.cin * b.cout;
+    for (const Layer& L : bb.layers) if (L.op == PW) n += (size_t)L.cin * L.cout;
     return n;
 }
 int max_channels(const Backbone& bb) {
-    int c = 16;
-    for (const Block& b : bb.blocks) c = std::max(c, std::max(b.mid, b.cout));
+    int c = 0;
+    for (const Layer& L : bb.layers) c = std::max(c, L.cout);
     return c;
 }
 
@@ -493,14 +489,13 @@ bool carve(smk::Workspace& w, const SmkEncoder* h, const Backbone& bb, int B, Ba
 struct PwPack { const float* w; const float* wt; const float* wt_lo; };
 
 // Packs the backbone's 1x1 weights for the forward (dgrad = false) or the dgrad (true), and the stem's dgrad weights, in
-// one launch.  packed[k]: where the k-th 1x1 conv's copy went.
+// one launch.  packed[Layer::pw]: where that 1x1 conv's copy went.
 int pack_weights(const SmkEncoder* h, const View& v, const BackboneWs& ws, bool dgrad, std::vector<PwPack>& packed, cudaStream_t st) {
     const Backbone& bb = h->bb[v.i];
     const bool tc = h->precision >= 1;
     PackJobs jobs{};
     int nj = 0, max_n = 432;
     float* dst = ws.pw;
-    int bn = 1;
     packed.clear();
     auto add = [&](const float* w, int cin, int cout) {
         const size_t n = (size_t)cin * cout;
@@ -513,11 +508,8 @@ int pack_weights(const SmkEncoder* h, const View& v, const BackboneWs& ws, bool 
         packed.push_back(tc ? PwPack{nullptr, j.hi, j.lo} : PwPack{j.hi, nullptr, nullptr});
         dst += n * (j.lo ? 2 : 1);
     };
-    for (const Block& b : bb.blocks) {
-        if (b.kind == DS) { add(v.bn(bn + 1).w, b.cin, b.cout); bn += 2; }
-        else if (b.kind == IR) { add(v.bn(bn).w, b.cin, b.mid); add(v.bn(bn + 2).w, b.mid, b.cout); bn += 3; }
-        else { add(v.bn(bn).w, b.cin, b.cout); bn += 1; }
-    }
+    for (size_t k = 0; k < bb.layers.size(); ++k)
+        if (bb.layers[k].op == PW) add(v.bn((int)k).w, bb.layers[k].cin, bb.layers[k].cout);
     if (dgrad) {                                          // stem [16][27] -> [27][16], the layout of stem_dgrad
         PackJob& j = jobs.j[nj++];
         j.src = v.bn(0).w; j.rows = 16; j.cols = 27; j.hi = ws.stem_t; j.lo = nullptr; j.transpose = 1; j.split = 0;
@@ -667,64 +659,40 @@ int head_backward(const float* g, const float* raw, const uint8_t* codes, const 
     return 0;
 }
 
-// Topology of a train handle: the layer list, activation sizes and the saved layout (names: the reference's module paths
-// — a conv's pre-BN output under the conv, a ReLU output under its BatchNorm as in the eval layout, a block's output
-// under the block, the pooled features under `<encoder>.pooled`, a head's pre-clamp output under the head).
-void build_topology(SmkEncoder* h) {
-    for (int i = 0; i < 3; ++i) {
-        if (!h->present[i]) continue;
-        Backbone& bb = h->bb[i];
-        const BlockDef* defs = i == 0 ? kSmall : kLarge;
-        const int nb = i == 0 ? (int)(sizeof(kSmall) / sizeof(BlockDef)) : (int)(sizeof(kLarge) / sizeof(BlockDef));
-        const int* stages = i == 0 ? kStageSmall : kStageLarge;
-        const std::string enc = std::string(kEncName[i]) + ".encoder.";
-        auto add = [h](const std::string& name, int H, int C) { return h->saved.add(name, H, H, C); };
-        bb.sv_zstem = add(enc + "conv_stem", 112, 16);
-        bb.sv_stem = add(enc + "bn1", 112, 16);
-        int cin = 16, res = 112, stage = 0, in_stage = 0, bn = 1;
-        size_t max_act = (size_t)112 * 112 * 16;
-        for (int k = 0; k < nb; ++k) {
-            Block b{};
-            b.kind = defs[k].kind; b.stride = defs[k].stride; b.cin = cin; b.cout = defs[k].cout;
-            b.skip = b.kind != CN && b.stride == 1 && b.cin == b.cout;
-            b.mid = b.kind == IR ? make_divisible((double)cin * defs[k].exp) : cin;
-            b.bn0 = bn;
-            const int ro = (res + b.stride - 1) / b.stride;
-            const std::string pre = enc + "blocks." + std::to_string(stage) + "." + std::to_string(in_stage);
-            if (b.kind == DS) {
-                b.sv_z[0] = add(pre + ".conv_dw", ro, cin); b.sv_a = add(pre + ".bn1", ro, cin);
-                b.sv_z[1] = add(pre + ".conv_pw", ro, b.cout); b.sv_out = add(pre, ro, b.cout);
-                bn += 2;
-            } else if (b.kind == IR) {
-                b.sv_z[0] = add(pre + ".conv_pw", res, b.mid); b.sv_a = add(pre + ".bn1", res, b.mid);
-                b.sv_z[1] = add(pre + ".conv_dw", ro, b.mid); b.sv_b = add(pre + ".bn2", ro, b.mid);
-                b.sv_z[2] = add(pre + ".conv_pwl", ro, b.cout); b.sv_out = add(pre, ro, b.cout);
-                bn += 3;
-            } else {
-                b.sv_z[0] = add(pre + ".conv", ro, b.cout); b.sv_a = add(pre + ".bn1", ro, b.cout);
-                bn += 1;
-            }
-            max_act = std::max(max_act, (size_t)res * res * b.mid);
-            max_act = std::max(max_act, (size_t)ro * ro * std::max(b.mid, b.cout));
-            res = ro; cin = b.cout;
-            if (++in_stage == stages[stage]) { ++stage; in_stage = 0; }
-            bb.blocks.push_back(b);
-        }
-        bb.feat = cin;
-        bb.n_out = i == 0 ? 6 : i == 1 ? h->n_shape : h->n_exp + 5;
-        bb.max_act = max_act;
-        h->max_act = std::max(h->max_act, max_act);
-        bb.sv_pool = h->saved.add(std::string(kEncName[i]) + ".pooled", 1, 1, bb.feat);
-        bb.sv_head = h->saved.add(std::string(kEncName[i]) + "." + kHeadName[i], 1, 1, bb.n_out);
+// Backbone i of a train handle: the layer list, and with it the saved layout (names: the reference's module paths — a
+// conv's pre-BN output under the conv, a ReLU output under its BatchNorm as in the eval layout, a block's output under the
+// block, the pooled features under `<encoder>.pooled`, a head's pre-clamp output under the head) and the BatchNorm
+// statistics after the saved tensors (backbones in slot order; per BatchNorm mean[C], then invstd[C]).
+void build_layers(SmkEncoder* h, int i) {
+    build_backbone(h, i);
+    Backbone& bb = h->bb[i];
+    const std::string enc = std::string(kEncName[i]) + ".";
+    int n_pw = 0;
+    // One conv (cin -> cout at resolution hin) + BatchNorm, fed by the previous layer; y: the name of the BatchNorm's output.
+    auto add = [&](Op op, int cin, int cout, int stride, int hin, const std::string& conv, const std::string& y, bool relu) {
+        Layer L{};
+        L.op = op; L.cin = cin; L.cout = cout; L.stride = stride; L.hin = hin; L.hout = (hin + stride - 1) / stride;
+        L.sv_in = bb.layers.empty() ? -1 : bb.layers.back().sv_y;
+        L.sv_z = h->saved.add(conv, L.hout, L.hout, cout);
+        L.sv_y = h->saved.add(y, L.hout, L.hout, cout);
+        L.relu = relu; L.skip = -1;
+        L.stats = h->stats_floats; h->stats_floats += 2 * (size_t)cout;
+        L.pw = op == PW ? n_pw++ : -1;
+        bb.layers.push_back(L);
+    };
+    add(STEM, 3, 16, 2, 224, enc + "encoder.conv_stem", enc + "encoder.bn1", true);
+    for (const Block& b : bb.blocks) {
+        const size_t first = bb.layers.size();
+        const int block_in = bb.layers.back().sv_y;
+        if (b.kind == IR) add(PW, b.cin, b.mid, 1, b.hin, b.path + ".conv_pw", b.path + ".bn1", true);
+        if (b.kind != CN) add(DW, b.mid, b.mid, b.stride, b.hin, b.path + ".conv_dw", b.path + (b.kind == IR ? ".bn2" : ".bn1"), true);
+        if (b.kind == CN) add(PW, b.cin, b.cout, 1, b.hout, b.path + ".conv", b.path + ".bn1", true);
+        else add(PW, b.mid, b.cout, 1, b.hout, b.path + (b.kind == IR ? ".conv_pwl" : ".conv_pw"), b.path, false);
+        bb.layers[first].first = true;
+        if (b.skip) bb.layers.back().skip = block_in;
     }
-    // BatchNorm statistics after the saved tensors: per backbone, per BN, mean[C] then invstd[C]
-    for (int i = 0; i < 3; ++i) {
-        if (!h->present[i]) continue;
-        const Backbone& bb = h->bb[i];
-        size_t n = 2 * 16;
-        for (const Block& b : bb.blocks) n += b.kind == IR ? 2 * (2 * (size_t)b.mid + b.cout) : b.kind == DS ? 2 * ((size_t)b.cin + b.cout) : 2 * (size_t)b.cout;
-        h->stats_floats += n;
-    }
+    bb.sv_pool = h->saved.add(enc + "pooled", 1, 1, bb.feat);
+    bb.sv_head = h->saved.add(enc + kHeadName[i], 1, 1, bb.n_out);
 }
 
 }  // namespace
@@ -738,18 +706,11 @@ extern "C" int smk_encoder_train_create(int backbones, int n_shape, int n_exp, i
     SmkEncoder* h = new SmkEncoder();
     h->train = true;
     h->n_shape = n_shape; h->n_exp = n_exp; h->precision = precision >= 1 ? 1 : 0; h->x3 = precision == 3;
-    for (int i = 0; i < 3; ++i) h->present[i] = (backbones >> i) & 1;
-    build_topology(h);
-    cudaError_t e = cudaSuccess;
-    if (h->present[2]) {                                  // smirk_encoder.py:105-108
-        std::vector<uint8_t> codes(h->bb[2].n_out, 0);
-        codes[n_exp] = codes[n_exp + 1] = 1; codes[n_exp + 2] = 2; codes[n_exp + 3] = codes[n_exp + 4] = 3;
-        e = h->arena.upload(codes, &h->bb[2].codes);
+    for (int i = 0; i < 3; ++i) {
+        h->present[i] = (backbones >> i) & 1;
+        if (h->present[i]) build_layers(h, i);
     }
-    std::vector<float> ones(1024, 1.f), zeros(1024, 0.f);
-    if (e == cudaSuccess) e = h->arena.upload(ones, &h->ones);
-    if (e == cudaSuccess) e = h->arena.upload(zeros, &h->zeros);
-    if (e == cudaSuccess) e = create_forks(h);
+    const cudaError_t e = finish_create(h);
     if (e != cudaSuccess) { smk::set_error("smk_encoder_train_create: %s", cudaGetErrorString(e)); delete h; return (int)e; }
     *out = h;
     return 0;
@@ -764,23 +725,12 @@ extern "C" size_t smk_encoder_train_workspace_bytes(const SmkEncoder* h, int B) 
 
 namespace {
 
-// Statistics offset (floats, from the start of the stats area) of backbone i's first BN.
-size_t stats_base(const SmkEncoder* h, int i) {
-    size_t o = 0;
-    for (int j = 0; j < i; ++j) {
-        if (!h->present[j]) continue;
-        o += 2 * 16;
-        for (const Block& b : h->bb[j].blocks) o += b.kind == IR ? 2 * (2 * (size_t)b.mid + b.cout) : b.kind == DS ? 2 * ((size_t)b.cin + b.cout) : 2 * (size_t)b.cout;
-    }
-    return o;
-}
-
 int check_args(const SmkEncoder* h, const SmkEncoderTrainArgs* a, const char* fn) {
     SMK_REQUIRE(h && h->train, "%s: not a train-mode handle (smk_encoder_train_create)", fn);
     SMK_REQUIRE(a, "%s: null args", fn);
     for (int i = 0; i < 3; ++i) {
         if (!h->present[i]) continue;
-        const int nbn = n_bn(h->bb[i]);
+        const int nbn = (int)h->bb[i].layers.size();
         SMK_REQUIRE(a->tensors[i] && a->n_tensors[i] == 5 * nbn, "%s: backbone %d expects %d tensors (conv weight + 4 BN tensors per conv), got %d",
                     fn, i, 5 * nbn, a->n_tensors[i]);
         SMK_REQUIRE(a->num_batches_tracked[i] && a->head_w[i] && a->head_b[i], "%s: backbone %d: null num_batches_tracked or head", fn, i);
@@ -820,49 +770,25 @@ extern "C" int smk_encoder_forward_train(const SmkEncoder* h, const SmkEncoderTr
         const View v{h, args, nullptr, i};
         const BackboneWs& W = bw[i];
         const float eps = args->eps[i], mom = args->momentum[i];
-        float* st_i = stats + stats_base(h, i);
         std::vector<PwPack> pk;
         if (int rc = pack_weights(h, v, W, false, pk, st)) return rc;
-        // the stem
-        {
-            const long M = (long)B * 112 * 112;
-            if (int rc = stem_forward(img, v.bn(0).w, B, 224, 224, SV(bb.sv_zstem), st)) return rc;
-            if (int rc = bn_forward(v.bn(0), SV(bb.sv_zstem), M, 16, eps, mom, st_i, st_i + 16, nullptr, true, false, SV(bb.sv_stem), W.part, st)) return rc;
-            st_i += 32;
-        }
-        const float* x = SV(bb.sv_stem);
-        int res = 112, p = 0;
-        for (const Block& b : bb.blocks) {
-            const int ro = (res + b.stride - 1) / b.stride;
-            const long Mi = (long)B * res * res, Mo = (long)B * ro * ro;
-            auto bnf = [&](int j, const float* z, long M, int C, const float* skip, bool relu, float* y) {
-                const int rc = bn_forward(v.bn(b.bn0 + j), z, M, C, eps, mom, st_i, st_i + C, skip, relu, rnd, y, W.part, st);
-                st_i += 2 * C;
-                return rc;
-            };
-            int rc = 0;
-            if (b.kind == DS) {
-                rc = dw_forward(x, v.bn(b.bn0).w, B, res, b.cin, b.stride, SV(b.sv_z[0]), st);
-                if (!rc) rc = bnf(0, SV(b.sv_z[0]), Mo, b.cin, nullptr, true, SV(b.sv_a));
-                if (!rc) rc = conv1x1(h, pk[p++], SV(b.sv_a), b.cin, b.cout, B, ro, nullptr, SV(b.sv_z[1]), false, "train_pw", st);
-                if (!rc) rc = bnf(1, SV(b.sv_z[1]), Mo, b.cout, b.skip ? x : nullptr, false, SV(b.sv_out));
-                x = SV(b.sv_out);
-            } else if (b.kind == IR) {
-                rc = conv1x1(h, pk[p++], x, b.cin, b.mid, B, res, nullptr, SV(b.sv_z[0]), false, "train_pw", st);
-                if (!rc) rc = bnf(0, SV(b.sv_z[0]), Mi, b.mid, nullptr, true, SV(b.sv_a));
-                if (!rc) rc = dw_forward(SV(b.sv_a), v.bn(b.bn0 + 1).w, B, res, b.mid, b.stride, SV(b.sv_z[1]), st);
-                if (!rc) rc = bnf(1, SV(b.sv_z[1]), Mo, b.mid, nullptr, true, SV(b.sv_b));
-                if (!rc) rc = conv1x1(h, pk[p++], SV(b.sv_b), b.mid, b.cout, B, ro, nullptr, SV(b.sv_z[2]), false, "train_pw", st);
-                if (!rc) rc = bnf(2, SV(b.sv_z[2]), Mo, b.cout, b.skip ? x : nullptr, false, SV(b.sv_out));
-                x = SV(b.sv_out);
-            } else {
-                rc = conv1x1(h, pk[p++], x, b.cin, b.cout, B, res, nullptr, SV(b.sv_z[0]), false, "train_pw", st);
-                if (!rc) rc = bnf(0, SV(b.sv_z[0]), Mo, b.cout, nullptr, true, SV(b.sv_a));
-                x = SV(b.sv_a);
-            }
+        for (size_t k = 0; k < bb.layers.size(); ++k) {
+            const Layer& L = bb.layers[k];
+            const BnRef r = v.bn((int)k);
+            int rc;
+            if (L.op == STEM) rc = stem_forward(img, r.w, B, L.hin, L.hin, SV(L.sv_z), st);
+            else if (L.op == PW) rc = conv1x1(h, pk[L.pw], SV(L.sv_in), L.cin, L.cout, B, L.hin, nullptr, SV(L.sv_z), false, "train_pw", st);
+            else rc = dw_forward(SV(L.sv_in), r.w, B, L.hin, L.cin, L.stride, SV(L.sv_z), st);
             if (rc) return rc;
-            res = ro;
+            // At precisions 1-2 every BatchNorm output inside a block is TF32-rounded, also one that feeds the depthwise conv,
+            // while the stem's never is, and no 1x1 conv rounds its own output: results stay bitwise what they have been.
+            float* mean = stats + L.stats;
+            rc = bn_forward(r, SV(L.sv_z), (long)B * L.hout * L.hout, L.cout, eps, mom, mean, mean + L.cout, L.skip >= 0 ? SV(L.skip) : nullptr,
+                            L.relu, rnd && L.op != STEM, SV(L.sv_y), W.part, st);
+            if (rc) return rc;
         }
+        const float* x = SV(bb.layers.back().sv_y);
+        const int res = bb.layers.back().hout;
         // global average pool, then the head on the pooled features (HW = 1)
         SMK_TAG("train_pool", 4.0 * B * bb.feat * (res * res + 1), (double)B * bb.feat * res * res, st);
         SMK_LAUNCH(pool_kernel, dim3(cdiv((long)B * bb.feat, 256)), dim3(256), 0, st, x, B, res * res, bb.feat, SV(bb.sv_pool));
@@ -912,82 +838,46 @@ extern "C" int smk_encoder_backward_train(const SmkEncoder* h, const SmkEncoderT
         const BackboneWs& W = bw[i];
         std::vector<PwPack> pk;
         if (int rc = pack_weights(h, v, W, true, pk, st)) return rc;
-        // statistics of each BN, in forward order
-        std::vector<const float*> mean;
-        std::vector<int> chans;
-        {
-            const float* s = stats + stats_base(h, i);
-            auto push = [&](int C) { mean.push_back(s); chans.push_back(C); s += 2 * C; };
-            push(16);
-            for (const Block& b : bb.blocks) {
-                if (b.kind == DS) { push(b.cin); push(b.cout); }
-                else if (b.kind == IR) { push(b.mid); push(b.mid); push(b.cout); }
-                else push(b.cout);
-            }
-        }
-        auto bnb = [&](int k, const float* g, const float* y, const float* z, long M, float* gz) {
-            return bn_backward(v.bn(k), g, y, z, mean[k], mean[k] + chans[k], M, chans[k], rnd, gz, W.part, W.gb, st);
-        };
-        float *gy = W.buf[0], *t1 = W.buf[1], *t2 = W.buf[2];
-        int res = 7;
-        {   // head -> gradient of the cn output (t1); head weight gradients
-            if (int rc = head_backward(g_out[i], SV(bb.sv_head), bb.codes, args->head_w[i], SV(bb.sv_pool), B, bb.n_out, res * res, bb.feat, W.gp, t1,
-                                       grads ? grads->head_w[i] : nullptr, grads ? grads->head_b[i] : nullptr, st))
-                return rc;
-        }
-        int p = (int)pk.size();
-        for (int bi = (int)bb.blocks.size() - 1; bi >= 0; --bi) {
-            const Block& b = bb.blocks[bi];
-            const int ro = res, ri = bi == 0 ? 112 : ro * b.stride;
-            const long Mi = (long)B * ri * ri, Mo = (long)B * ro * ro;
-            const float* x = bi == 0 ? SV(bb.sv_stem) : SV(bb.blocks[bi - 1].sv_out);     // the block input
-            int rc = 0;
-            if (b.kind == CN) {                      // t1: gradient of the cn output -> gy: of the block input
-                const BnRef r = v.bn(b.bn0);
-                rc = bnb(b.bn0, t1, SV(b.sv_a), SV(b.sv_z[0]), Mo, t1);
-                if (!rc && r.gw) rc = pw_wgrad(t1, x, Mo, b.cout, b.cin, W.wpart, r.gw, st);
-                if (!rc) rc = conv1x1(h, pk[--p], t1, b.cout, b.cin, B, ro, nullptr, gy, false, "train_pw_dgrad", st);
-            } else if (b.kind == IR) {               // gy: gradient of the block output -> gy: of the block input
-                const BnRef rp = v.bn(b.bn0), rd = v.bn(b.bn0 + 1), rl = v.bn(b.bn0 + 2);
-                const PwPack& wl = pk[--p];
-                const PwPack& we = pk[--p];
-                rc = bnb(b.bn0 + 2, gy, nullptr, SV(b.sv_z[2]), Mo, t1);
-                if (!rc && rl.gw) rc = pw_wgrad(t1, SV(b.sv_b), Mo, b.cout, b.mid, W.wpart, rl.gw, st);
-                if (!rc) rc = conv1x1(h, wl, t1, b.cout, b.mid, B, ro, nullptr, t2, false, "train_pw_dgrad", st);
-                if (!rc) rc = bnb(b.bn0 + 1, t2, SV(b.sv_b), SV(b.sv_z[1]), Mo, t2);
-                if (!rc && rd.gw) rc = dw_wgrad(t2, SV(b.sv_a), B, ri, b.mid, b.stride, W.wpart, rd.gw, st);
-                if (!rc) rc = dw_dgrad(t2, rd.w, nullptr, B, ri, b.mid, b.stride, t1, st);
-                if (!rc) rc = bnb(b.bn0, t1, SV(b.sv_a), SV(b.sv_z[0]), Mi, t1);
-                if (!rc && rp.gw) rc = pw_wgrad(t1, x, Mi, b.mid, b.cin, W.wpart, rp.gw, st);
-                if (!rc) rc = conv1x1(h, we, t1, b.mid, b.cin, B, ri, b.skip ? gy : nullptr, t2, false, "train_pw_dgrad", st);
-                std::swap(gy, t2);
-            } else {                                 // DS block 0: gy -> t1: gradient of the stem output
-                const BnRef rd = v.bn(b.bn0), rp = v.bn(b.bn0 + 1);
-                rc = bnb(b.bn0 + 1, gy, nullptr, SV(b.sv_z[1]), Mo, t1);
-                if (!rc && rp.gw) rc = pw_wgrad(t1, SV(b.sv_a), Mo, b.cout, b.cin, W.wpart, rp.gw, st);
-                if (!rc) rc = conv1x1(h, pk[--p], t1, b.cout, b.cin, B, ro, nullptr, t2, false, "train_pw_dgrad", st);
-                if (!rc) rc = bnb(b.bn0, t2, SV(b.sv_a), SV(b.sv_z[0]), Mo, t2);
-                if (!rc && rd.gw) rc = dw_wgrad(t2, x, B, ri, b.cin, b.stride, W.wpart, rd.gw, st);
-                if (!rc) rc = dw_dgrad(t2, rd.w, b.skip ? gy : nullptr, B, ri, b.cin, b.stride, t1, st);
-            }
+        // g: the gradient of the current layer's output; out: where its dgrad goes; held: the gradient of a block's output, kept
+        // from the block's last layer to its first, where the skip connection adds it to the gradient of the block's input
+        float *g = W.buf[0], *out = W.buf[1], *spare = W.buf[2], *held = nullptr;
+        const Layer& top = bb.layers.back();
+        if (int rc = head_backward(g_out[i], SV(bb.sv_head), bb.codes, args->head_w[i], SV(bb.sv_pool), B, bb.n_out, top.hout * top.hout, bb.feat, W.gp, g,
+                                   grads ? grads->head_w[i] : nullptr, grads ? grads->head_b[i] : nullptr, st))
+            return rc;
+        for (int k = (int)bb.layers.size() - 1; k >= 0; --k) {
+            const Layer& L = bb.layers[k];
+            const BnRef r = v.bn(k);
+            const long M = (long)B * L.hout * L.hout;
+            const float* mean = stats + L.stats;
+            float* gz = L.skip >= 0 ? out : g;        // in place, unless g is to be held
+            // Every BatchNorm backward rounds its result at precisions 1-2, whatever consumes it, and no 1x1 dgrad rounds
+            // its own: results stay bitwise what they have been.
+            int rc = bn_backward(r, g, L.relu ? SV(L.sv_y) : nullptr, SV(L.sv_z), mean, mean + L.cout, M, L.cout, rnd, gz, W.part, W.gb, st);
             if (rc) return rc;
-            res = ri;
+            if (L.skip >= 0) { held = g; g = out; out = spare; }
+            if (r.gw) {
+                if (L.op == STEM) rc = stem_wgrad(g, img, B, L.hin, L.hin, W.wpart, r.gw, st);
+                else if (L.op == PW) rc = pw_wgrad(g, SV(L.sv_in), M, L.cout, L.cin, W.wpart, r.gw, st);
+                else rc = dw_wgrad(g, SV(L.sv_in), B, L.hin, L.cin, L.stride, W.wpart, r.gw, st);
+                if (rc) return rc;
+            }
+            if (L.op == STEM) break;                  // g: the gradient of the stem's pre-BN output; its dgrad runs after the join
+            const float* res = L.first ? held : nullptr;
+            if (L.op == PW) rc = conv1x1(h, pk[L.pw], g, L.cout, L.cin, B, L.hin, res, out, false, "train_pw_dgrad", st);
+            else rc = dw_dgrad(g, r.w, res, B, L.hin, L.cin, L.stride, out, st);
+            if (rc) return rc;
+            std::swap(g, out);
+            if (res) { spare = held; held = nullptr; }
         }
-        // the stem: t1 -> gradient of its pre-BN output (t1); its weight gradient; the image gradient after the join
-        const BnRef r0 = v.bn(0);
-        const long M = (long)B * 112 * 112;
-        if (int rc = bnb(0, t1, SV(bb.sv_stem), SV(bb.sv_zstem), M, t1)) return rc;
-        if (r0.gw) {
-            if (int rc = stem_wgrad(t1, img, B, 224, 224, W.wpart, r0.gw, st)) return rc;
-        }
-        g_stem[i] = t1; w_stem[i] = W.stem_t;
+        g_stem[i] = g; w_stem[i] = W.stem_t;
         return 0;
     });
     if (rc || !g_img) return rc;
     return enc::stem_dgrad(g_stem, w_stem, B, g_img, main_st);
 }
 
-// ---- test entry points (include/smirk_b200_train_debug.h): each runs the host helper of the train path ----------------
+// ---- test entry points (smk_debug_train_*): each runs the host helper of the train path ------------------------------
 
 namespace {
 

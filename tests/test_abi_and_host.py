@@ -11,9 +11,10 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_every_header_prototype_is_exported_and_bound(native_lib):
-    """The library exports every prototype in include/smirk_b200.h (all 70 entry points, the input gradients and the
-    video grid included), and each has exactly one row in _lib.BINDINGS with the same return type and the same
+def test_every_header_prototype_is_exported_and_bound_in_header_order(native_lib):
+    """The library exports every prototype in include/smirk_b200.h (all 83 entry points: the input gradients, the
+    video grid, the encoder's train mode and its kernel test entry points included), and each has exactly one row in
+    _lib.BINDINGS, in the header's order, with the same return type and the same
     parameters: count, pointer / value kind, and the trailing stream where the header has one (which is what makes
     `_lib.call` append the current stream)."""
     import ctypes as C
@@ -27,8 +28,8 @@ def test_every_header_prototype_is_exported_and_bound(native_lib):
     assert native_lib.smk_version() == 100
     protos = re.findall(r"^\s*([A-Za-z_][\w ]*?\**)\s*\b(smk_\w+)\s*\(([^)]*)\)\s*;", hdr, flags=re.M)
     table = {name: (restype, args) for name, restype, args in _lib.BINDINGS}
-    assert len(protos) == 70 and len(table) == len(_lib.BINDINGS)
-    assert {name for _, name, _ in protos} == set(table)
+    assert len(protos) == 83 and len(table) == len(_lib.BINDINGS)
+    assert [name for _, name, _ in protos] == [name for name, _, _ in _lib.BINDINGS]
     returns = {"int": C.c_int, "size_t": C.c_size_t, "void": None, "const char*": C.c_char_p, "unsigned long long": C.c_ulonglong}
     values = {"int": C.c_int, "size_t": C.c_size_t, "float": C.c_float}
     for ret, name, params in protos:

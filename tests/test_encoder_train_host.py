@@ -1,10 +1,9 @@
-"""CPU suite of the train-mode encoder: the C ABI with the train entry points, their argument checks, the opt-in and mode
+"""CPU suite of the train-mode encoder: the argument checks of the train entry points, the opt-in and mode
 checks of the module, the dropin runner's --train flag, and the train-mode restatement (tests/encoder_train_ref.py)
 against the reference's own SmirkEncoder (when the reference checkout is present)."""
 import copy
 import ctypes as C
 import os
-import re
 
 import pytest
 import torch
@@ -13,35 +12,6 @@ import torch.nn as nn
 import encoder_train_ref as tr
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def test_train_header_prototypes_are_exported_and_bound(native_lib):
-    """include/smirk_b200_train.h is included by smirk_b200.h; the library exports each of its 4 prototypes, and each has
-    exactly one row in _lib.TRAIN_BINDINGS (header order, no row shared with BINDINGS) with the same return type and
-    parameters: count, pointer / value kind, and the trailing stream, which `_lib.call` fills in."""
-    from smirk_b200 import _lib
-    main = open(os.path.join(ROOT, "include", "smirk_b200.h")).read()
-    assert '#include "smirk_b200_train.h"' in main
-    hdr = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "smirk_b200_train.h")).read(), flags=re.S)
-    protos = re.findall(r"^\s*([A-Za-z_][\w ]*?\**)\s*\b(smk_\w+)\s*\(([^)]*)\)\s*;", hdr, flags=re.M)
-    assert [name for _, name, _ in protos] == [name for name, _, _ in _lib.TRAIN_BINDINGS] and len(protos) == 4
-    assert not {name for name, _, _ in _lib.TRAIN_BINDINGS} & {name for name, _, _ in _lib.BINDINGS}
-    table = {name: (restype, args) for name, restype, args in _lib.TRAIN_BINDINGS}
-    returns = {"int": C.c_int, "size_t": C.c_size_t}
-    for ret, name, params in protos:
-        assert hasattr(native_lib, name), "missing export: " + name
-        restype, args = table[name]
-        assert restype is returns[ret.strip()], name
-        params = [q.strip() for q in params.split(",") if q.strip()]
-        assert len(args) == len(params), name
-        for q, a in zip(params, args):
-            if q.endswith("stream"):
-                assert a is _lib.STREAM, (name, q)
-            elif "*" in q:
-                assert a in (C.c_void_p, C.c_char_p) or issubclass(a, C._Pointer), (name, q)
-            else:
-                assert a is {"int": C.c_int, "size_t": C.c_size_t}[q.rsplit(None, 1)[0]], (name, q)
-        assert (name in _lib._TAKES_STREAM) == (args[-1:] == [_lib.STREAM]), name
 
 
 def test_train_entry_points_reject_bad_arguments(native_lib):
@@ -58,35 +28,6 @@ def test_train_entry_points_reject_bad_arguments(native_lib):
     rc = L.smk_encoder_backward_train(nul, C.byref(args), buf, 2, buf, 1 << 20, buf, buf, buf, buf, None, buf, 1 << 20, nul)
     assert rc < 0 and b"not a train-mode handle" in L.smk_last_error()
     assert L.smk_encoder_train_workspace_bytes(nul, 4) == 0
-
-
-def test_train_debug_header_prototypes_are_exported_and_bound(native_lib):
-    """include/smirk_b200_train_debug.h (the train-kernel test entry points) is included by smirk_b200_train.h; the
-    library exports each of its 9 prototypes, and each has exactly one row in _lib.TRAIN_DEBUG_BINDINGS (header order, no
-    row shared with the other tables) with the same return type and parameters, the trailing stream included."""
-    from smirk_b200 import _lib
-    train = open(os.path.join(ROOT, "include", "smirk_b200_train.h")).read()
-    assert '#include "smirk_b200_train_debug.h"' in train
-    hdr = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "smirk_b200_train_debug.h")).read(), flags=re.S)
-    protos = re.findall(r"^\s*([A-Za-z_][\w ]*?\**)\s*\b(smk_\w+)\s*\(([^)]*)\)\s*;", hdr, flags=re.M)
-    assert [name for _, name, _ in protos] == [name for name, _, _ in _lib.TRAIN_DEBUG_BINDINGS] and len(protos) == 9
-    names = {name for name, _, _ in _lib.TRAIN_DEBUG_BINDINGS}
-    assert not names & {name for name, _, _ in _lib.BINDINGS + _lib.TRAIN_BINDINGS}
-    table = {name: (restype, args) for name, restype, args in _lib.TRAIN_DEBUG_BINDINGS}
-    for ret, name, params in protos:
-        assert hasattr(native_lib, name), "missing export: " + name
-        restype, args = table[name]
-        assert ret.strip() == "int" and restype is C.c_int, name
-        params = [q.strip() for q in params.split(",") if q.strip()]
-        assert len(args) == len(params), name
-        for q, a in zip(params, args):
-            if q.endswith("stream"):
-                assert a is _lib.STREAM, (name, q)
-            elif "*" in q:
-                assert a in (C.c_void_p, C.c_char_p) or issubclass(a, C._Pointer), (name, q)
-            else:
-                assert a is {"int": C.c_int, "size_t": C.c_size_t, "float": C.c_float}[q.rsplit(None, 1)[0]], (name, q)
-        assert name in _lib._TAKES_STREAM and args[-1:] == [_lib.STREAM], name
 
 
 def test_train_debug_entry_points_reject_bad_arguments(native_lib):
