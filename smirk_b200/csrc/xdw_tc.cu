@@ -54,11 +54,11 @@ constexpr int PAR_ROWS = 13;                     // scale1, bias1, 9 depthwise t
 constexpr int PAR_FLOATS = PAR_ROWS * NC, PAR_SLOT_BYTES = PAR_FLOATS * 4;   // one chunk's parameters: 1664 B
 constexpr int NUM_WORKERS = 256;                // serial schedule: 8 worker warps; pipelined: the 8 warps of the two MMA warpgroups
 constexpr int NUM_THREADS = NUM_WORKERS + 32;   // serial schedule: + the TMA producer warp
-// Pipelined schedule: warpgroups 0-1 expand GEMM + phase (a), warpgroup 2 depthwise (each thread plays DW_ROLES of the
-// serial schedule's 256 depthwise roles), warpgroup 3 the TMA producer (one warp works, three exit).  Every warp starts
+// Pipelined schedule: warpgroups 0-1 expand GEMM + phase (a), warpgroup 2 depthwise (one role per thread, cut for 128
+// threads), warpgroup 3 the TMA producer (one warp works, three exit).  Every warp starts
 // with WS_LAUNCH_REGS; the producer warpgroup gives registers back (setmaxnreg.dec, which may only lower the count) and the
 // other three take them (setmaxnreg.inc, which may only raise it).  The budgets fill the 64 K register file exactly.
-constexpr int DW_THREADS = 128, DW_ROLES = NUM_WORKERS / DW_THREADS, WS_THREADS = NUM_WORKERS + DW_THREADS + 128;
+constexpr int DW_THREADS = 128, WS_THREADS = NUM_WORKERS + DW_THREADS + 128;
 constexpr int WS_LAUNCH_REGS = 65536 / WS_THREADS, MMA_REGS = 168, DW_REGS = 136, PROD_REGS = 40;
 static_assert(NUM_WORKERS * MMA_REGS + DW_THREADS * DW_REGS + 128 * PROD_REGS == 65536, "register budgets of the pipelined schedule");
 static_assert(MMA_REGS >= WS_LAUNCH_REGS && DW_REGS >= WS_LAUNCH_REGS && PROD_REGS <= WS_LAUNCH_REGS,
@@ -69,16 +69,17 @@ constexpr int SMEM_PER_SM = 228 * 1024, SMEM_PER_CTA = 227 * 1024, SMEM_RESERVED
 // Shared-memory plan of one window size.  3xTF32 (X3) runs the pipelined schedule, plain TF32 the serial one.
 // MINB: resident CTAs per SM the kernel is built for — two for plain TF32 wherever a single window leaves room for them, one for
 // 3xTF32 (the pipelined schedule takes the whole register file) and for the deep plain-TF32 windows.
-// NE: E slots (each with its parameter block).  Pipelined: two where they fit beside one window and a 2-stage weight ring, so
-// the MMA warpgroups fill one slot while the depthwise warpgroup drains the other; one for NKB = 5 (Cin 160).  Serial: one E,
-// two parameter blocks (chunk parity).
+// NE: E slots.  Pipelined: two where they fit beside one window and a 2-stage weight ring, so the MMA warpgroups fill one slot
+// while the depthwise warpgroup drains the other; one for NKB = 5 (Cin 160); 2 NE parameter blocks (chunk i's in block
+// i % 2NE), so the depthwise warpgroup can stage chunk i + NE's while chunk i's is still in use.  Serial: one E, two parameter
+// blocks (chunk parity).
 // STAGES: weight stages; NKB where they fit, so the next chunk's weights all load during this chunk's phases (a)/(b).
 // WBUF: windows, two where they fit beside MINB CTAs.
 template <int NKB, int X3> struct XdwSmem {
     static constexpr int WIN_BYTES = NKB * KB_BYTES;
     static constexpr int STAGE_BYTES = X3 ? 2 * B_BYTES : B_BYTES;      // [w heads] (+ [w tails])
     static constexpr size_t bytes(int wbuf, int stages, int ne) {
-        return (size_t)wbuf * WIN_BYTES + stages * STAGE_BYTES + ne * E_BYTES + (X3 ? ne : 2) * PAR_SLOT_BYTES + 256 + 1024;   // + barriers, alignment slack
+        return (size_t)wbuf * WIN_BYTES + stages * STAGE_BYTES + ne * E_BYTES + (X3 ? 2 * ne : 2) * PAR_SLOT_BYTES + 256 + 1024;   // + barriers, alignment slack
     }
     static constexpr bool fits(int wbuf, int stages, int ne, int minb) {
         return bytes(wbuf, stages, ne) <= SMEM_PER_CTA && minb * (bytes(wbuf, stages, ne) + SMEM_RESERVED) <= SMEM_PER_SM;
@@ -89,7 +90,7 @@ template <int NKB, int X3> struct XdwSmem {
     static constexpr int WBUF = fits(2, STAGES, NE, MINB) ? 2 : 1;
     static constexpr size_t SMEM = bytes(WBUF, STAGES, NE);
     static constexpr int RING = WBUF * WIN_BYTES, E_OFF = RING + STAGES * STAGE_BYTES, PAR_OFF = E_OFF + NE * E_BYTES,
-                         BAR_OFF = PAR_OFF + (X3 ? NE : 2) * PAR_SLOT_BYTES;
+                         BAR_OFF = PAR_OFF + (X3 ? 2 * NE : 2) * PAR_SLOT_BYTES;
     static_assert(fits(WBUF, STAGES, NE, MINB), "shared-memory budget");
     static_assert(2 * (STAGES + WBUF + NE) * 8 <= 256, "barrier block");
 };
@@ -145,6 +146,19 @@ struct ItemIter {
         return w;
     }
 };
+// The chunk sequence of a CTA, (problem, chunk) in the order every role walks it (every item has at least one chunk).
+template <int TO> struct ChunkIter {
+    ItemIter ii;
+    int prob, c, c_end;
+    __device__ explicit ChunkIter(const XdwArgs& a) : ii(a) { start(a); }
+    __device__ bool valid(const XdwArgs& a) const { return ii.item < a.n_items; }
+    __device__ void start(const XdwArgs& a) {
+        if (valid(a)) { const Item w = ii.decode<TO>(a); prob = w.prob; c = w.c_begin; c_end = w.c_end; }
+    }
+    __device__ void next(const XdwArgs& a) {
+        if (valid(a) && ++c == c_end) { ii.next(a); start(a); }
+    }
+};
 
 // TMA producer: the x window once per item, then the W1 rows of every (chunk, k-block).
 template <int STRIDE, int X3, int NKB>
@@ -179,9 +193,10 @@ __device__ __forceinline__ void produce(const XdwMaps& mp, const XdwArgs& a, uin
 }
 
 // Per-chunk parameters (BN1 scale/bias, nine depthwise taps, BN2 scale/bias: 13 rows of 32 channels) are staged through a
-// shared-memory block: worker t < 208 owns one float2 of it, loads it from global memory before it starts the chunk's MMAs
-// (or, serial schedule, the previous chunk's) and parks it once the block is free, so the global-load latency is off the
-// critical path and phases (a)/(b) read parameters with LDS.  Channels past `mid` get zero scale and bias.
+// shared-memory block: thread t < 208 owns one float2 of it, loads it from global memory ahead of time and parks it once the
+// block is free, so the global-load latency is off the critical path and phases (a)/(b) read parameters with LDS.  Serial
+// schedule: the 256 workers, one chunk ahead, before the MMAs of the previous chunk.  Pipelined: the 128 depthwise threads
+// (two float2 each for the first 80), NE chunks ahead, during a depthwise conv.  Channels past `mid` get zero scale and bias.
 struct ParLoader {
     const float* src[2];
     int prow, pcol;
@@ -194,9 +209,11 @@ struct ParLoader {
                                                                                   : a.wdw[q] + (size_t)(prow - 2) * a.mid) + pcol;
         }
     }
-    __device__ float2 load(const XdwArgs& a, int prob, int c) const {
+    // SELECT: pick the problem's pointer with a select rather than an index, which keeps src out of local memory in the
+    // pipelined kernel's depthwise warpgroup; the serial kernel's 96-register allocation spills less with the index.
+    template <bool SELECT = false> __device__ float2 load(const XdwArgs& a, int prob, int c) const {
         float2 v = make_float2(0.f, 0.f);
-        if (owner && c * NC + pcol < a.mid) v = __ldg(reinterpret_cast<const float2*>(src[prob] + c * NC));
+        if (owner && c * NC + pcol < a.mid) v = __ldg(reinterpret_cast<const float2*>((SELECT ? (prob ? src[1] : src[0]) : src[prob]) + c * NC));
         return v;
     }
     __device__ void park(float* par, const float2& v) const {
@@ -302,32 +319,48 @@ __device__ __forceinline__ void bn1_relu(const float (&acc)[2][NC / 2], float* E
         }
 }
 
-// Depthwise role: output column ox and row group rg of the tile's valid columns x as many row groups as fit in the 32 slots.
+// Depthwise role: a run of DWC adjacent output columns starting at ox (dw_cols: two in the pipelined schedule at stride 1,
+// else one), and row group rg, of one channel quad.  The tile's column runs x as many row groups as fit in the schedule's
+// slots (depthwise threads / 8 channel quads: 32 serial, 16 pipelined), so every slot gets about the same number of outputs.
 // A tile has TO columns / rows except in the last tile column / row: the role for both column counts is worked out once
 // (bytes: ox full, rg full, ox edge, rg edge), the row grouping of the four tile kinds comes from the host (a.geom); the item
 // loop only selects (dw_rows).
-template <int TO> __device__ __forceinline__ unsigned dw_role(const XdwArgs& a, int slot) {
-    const int ncols_e = a.Wo - (a.tiles_x - 1) * TO;
-    return (unsigned)(slot % TO) | (unsigned)(slot / TO) << 8 | (unsigned)(slot % ncols_e) << 16 | (unsigned)(slot / ncols_e) << 24;
+__host__ __device__ constexpr int dw_cols(int stride, bool pipelined) { return stride == 1 && pipelined ? 2 : 1; }
+template <int STRIDE, int DWC> __device__ __forceinline__ unsigned dw_role(const XdwArgs& a, int slot) {
+    constexpr int TO = STRIDE == 1 ? 14 : 7, NCR = (TO + DWC - 1) / DWC;
+    const int ncr_e = (a.Wo - (a.tiles_x - 1) * TO + DWC - 1) / DWC;   // column runs of an edge tile
+    return (unsigned)(slot % NCR * DWC) | (unsigned)(slot / NCR) << 8 | (unsigned)(slot % ncr_e * DWC) << 16 | (unsigned)(slot / ncr_e) << 24;
 }
-struct DwRows { int ox, oy0, oy1; };            // output column and output rows [oy0, oy1) of the tile
-template <int TO> __device__ __forceinline__ DwRows dw_rows(const XdwArgs& a, const ItemIter& ii, unsigned role) {
+struct DwRows { int ox, ncol, oy0, oy1; };      // output columns [ox, ox + ncol) and output rows [oy0, oy1) of the tile
+template <int STRIDE, int DWC> __device__ __forceinline__ DwRows dw_rows(const XdwArgs& a, const ItemIter& ii, unsigned role) {
+    constexpr int TO = STRIDE == 1 ? 14 : 7;
     const bool col_e = ii.tx == a.tiles_x - 1, row_e = ii.ty == a.tiles_y - 1;
-    const int nrows = row_e ? a.Ho - (a.tiles_y - 1) * TO : TO;
+    const int nrows = row_e ? a.Ho - (a.tiles_y - 1) * TO : TO, ncols = col_e ? a.Wo - (a.tiles_x - 1) * TO : TO;
     const unsigned g8 = a.geom >> ((col_e ? 16 : 0) + (row_e ? 8 : 0));
     const int rpt = (int)(g8 & 15u), n_rg = (int)((g8 >> 4) & 15u);
     const unsigned r16 = role >> (col_e ? 16 : 0);
     const int rg = (int)((r16 >> 8) & 255u);
     DwRows d;
-    d.ox = (int)(r16 & 255u); d.oy0 = rg * rpt; d.oy1 = rg < n_rg ? min(nrows, d.oy0 + rpt) : 0;
+    d.ox = (int)(r16 & 255u); d.ncol = min(DWC, ncols - d.ox);
+    d.oy0 = rg * rpt; d.oy1 = rg < n_rg ? min(nrows, d.oy0 + rpt) : 0;
     return d;
 }
 
-// Phase (b): depthwise 3x3 over E, BN2 + ReLU, optional TF32 rounding, store of d.  One thread owns one output column of one
-// channel quad and walks down its rows, so every E row it reads is shared by the (up to three) output rows it feeds: 3 LDS.128
-// per input row instead of 9 per output.  Tap order per output stays (ky, kx) ascending -> same rounding as the unfused path.
-template <int STRIDE>
+// Phase (b): depthwise 3x3 over E, BN2 + ReLU, optional TF32 rounding, store of d.  Tap order per output stays (ky, kx)
+// ascending, one fmaf chain from zero -> same rounding as the unfused path.
+// Stride 1: one thread owns DWC adjacent output columns of one channel quad and walks down their rows; every E row it reads
+// feeds those columns and the up to three output rows that use it, through rolling accumulators.
+//   DWC = 1 (serial schedule): 3 LDS.128 per input row; the accumulators of the two rows above oy0 are computed and dropped,
+//     which keeps the loop within the 96 registers of the two-CTA serial kernel.
+//   DWC = 2 (pipelined schedule): 4 LDS.128 per input row for both columns; p = output r-2 (gets its ky=2 taps from row r,
+//     then is stored), q = output r-1 (ky=1, then becomes p), and a fresh one for output r (ky=0, then becomes q).  The first
+//     two and the last two input rows are peeled, so no accumulator is started for an output outside [oy0, oy1).  A run cut
+//     short by the tile edge (ncol = 1) still computes its second column, which lies inside the 16-pixel window, and does
+//     not store it.
+// Stride 2: one thread owns one output column; a row of E is shared by two output rows at most.
+template <int STRIDE, int DWC>
 __device__ __forceinline__ void depthwise(const float* E, const float* par, const XdwArgs& a, const Item& w, int ch0, int cq, const DwRows& rows) {
+    static_assert(STRIDE == 1 || DWC == 1, "stride 2 runs one column per role");
     if (cq * 4 < a.mid - ch0 && rows.oy0 < rows.oy1) {
         const int ch = ch0 + cq * 4;
         float4 k[9];
@@ -337,16 +370,19 @@ __device__ __forceinline__ void depthwise(const float* E, const float* par, cons
         const float4 b2 = *reinterpret_cast<const float4*>(par + 12 * NC + cq * 4);
         float* orow = a.out[w.prob] + (((size_t)w.img * a.Ho + w.oh0 + rows.oy0) * a.Wo + w.ow0 + rows.ox) * a.mid + ch;
         const size_t orow_stride = (size_t)a.Wo * a.mid;
-        auto emit = [&](const float4& acc4) {
+        auto bn2 = [&](const float4& acc4) {
             float4 o = fma4(acc4, s2, b2);
             o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
             if (a.round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
-            *reinterpret_cast<float4*>(orow) = o;
+            return o;
+        };
+        auto emit = [&](const float4& acc4) {
+            *reinterpret_cast<float4*>(orow) = bn2(acc4);
             orow += orow_stride;
         };
         const float* e = E + (size_t)((rows.oy0 * STRIDE) * WIN + rows.ox * STRIDE) * E_PITCH + cq * 4;
         const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (STRIDE == 1) {
+        if (STRIDE == 1 && DWC == 1) {
             float4 acc0 = zero, acc1 = zero, acc2 = zero;          // outputs r-2 (gets ky=2), r-1 (ky=1), r (ky=0)
             const int n_in = rows.oy1 - rows.oy0 + 2;
 #pragma unroll 3
@@ -360,6 +396,45 @@ __device__ __forceinline__ void depthwise(const float* E, const float* par, cons
                 if (r >= 2) emit(acc0);
                 acc0 = acc1; acc1 = acc2; acc2 = zero;
             }
+        } else if (STRIDE == 1) {
+            struct Acc { float4 c[DWC]; };             // the DWC columns of one output row
+            float4 x[DWC + 2];
+            auto load = [&](int r) {
+#pragma unroll
+                for (int j = 0; j < DWC + 2; ++j) x[j] = *reinterpret_cast<const float4*>(e + (r * WIN + j) * E_PITCH);
+            };
+            auto fresh = [&]() {
+                Acc acc;
+#pragma unroll
+                for (int j = 0; j < DWC; ++j) acc.c[j] = zero;
+                return acc;
+            };
+            auto taps = [&](Acc& acc, int ky) {    // acc += the ky row of taps over the loaded E row, every column
+#pragma unroll
+                for (int kx = 0; kx < 3; ++kx)
+#pragma unroll
+                    for (int j = 0; j < DWC; ++j) fma4_acc(acc.c[j], x[kx + j], k[3 * ky + kx]);
+            };
+            auto store = [&](const Acc& acc) {
+#pragma unroll
+                for (int j = 0; j < DWC; ++j)
+                    if (j == 0 || j < rows.ncol) *reinterpret_cast<float4*>(orow + j * a.mid) = bn2(acc.c[j]);
+                orow += orow_stride;
+            };
+            const int n_out = rows.oy1 - rows.oy0;
+            Acc p, q = fresh();
+            load(0); taps(q, 0);                                            // output 0: ky=0
+            load(1); p = q; taps(p, 1);                                     // output 0: ky=1
+            if (n_out > 1) { q = fresh(); taps(q, 0); }                     // output 1: ky=0
+#pragma unroll 2
+            for (int r = 2; r < n_out; ++r) {                               // outputs r-2 (done), r-1, r
+                load(r);
+                taps(p, 2); store(p);
+                p = q; taps(p, 1);
+                q = fresh(); taps(q, 0);
+            }
+            if (n_out > 1) { load(n_out); taps(p, 2); store(p); p = q; taps(p, 1); }
+            load(n_out + 1); taps(p, 2); store(p);                          // the last output: ky=2
         } else {
             float4 p0 = *reinterpret_cast<const float4*>(e);
             float4 p1 = *reinterpret_cast<const float4*>(e + E_PITCH);
@@ -388,7 +463,7 @@ template <int NKB, int X3> struct XdwShared {
     using L = XdwSmem<NKB, X3>;
     uint8_t* smem;
     float* E;                   // [NE][256][E_PITCH]
-    float* PAR;                 // [X3 ? NE : 2][PAR_ROWS][NC]
+    float* PAR;                 // [X3 ? 2 NE : 2][PAR_ROWS][NC]
     uint64_t *full, *empty;     // weight stage s loaded / free
     uint64_t *wfull, *wempty;   // window b loaded (TMA transaction count) / free: its item's last chunk has finished its MMAs
     uint64_t *efull, *eempty;   // pipelined: E slot s written by phase (a) / drained by phase (b)
@@ -440,14 +515,15 @@ xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
     ItemIter ii(a);
     if (ii.item < a.n_items) { const Item w0 = ii.decode<TO>(a); pl.park(sh.PAR, pl.load(a, w0.prob, w0.c_begin)); }
     worker_barrier();
-    const unsigned role = dw_role<TO>(a, t >> 3);
+    constexpr int DWC = dw_cols(STRIDE, false);
+    const unsigned role = dw_role<STRIDE, DWC>(a, t >> 3);
     int cc = 0, it = 0;
     for (int n = 0; ii.item < a.n_items; ++n) {
       const Item w = ii.decode<TO>(a);
       const int wb = n % L::WBUF;
       const uint8_t* win = sh.smem + wb * L::WIN_BYTES + half * HALF_BYTES;     // this warpgroup's half of k-block 0
       mbar_wait(&sh.wfull[wb], (uint32_t)(n / L::WBUF) & 1u);
-      const DwRows rows = dw_rows<TO>(a, ii, role);
+      const DwRows rows = dw_rows<STRIDE, DWC>(a, ii, role);
       int next_first = -1, next_prob = 0;              // first chunk (and problem) of this CTA's next item (-1: none)
       ii.next(a);
       if (ii.item < a.n_items) { const Item wn = ii.decode<TO>(a); next_first = wn.c_begin; next_prob = wn.prob; }
@@ -463,7 +539,7 @@ xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
         bn1_relu<STRIDE, SAVE>(acc, sh.E, par, a, w, c * NC, half, wq, lane);
         if (c_next >= 0) pl.park(sh.PAR + (buf ^ 1) * PAR_FLOATS, pf);     // slot buf^1 was last read in the previous chunk's phase (b)
         worker_barrier();
-        depthwise<STRIDE>(sh.E, par, a, w, c * NC, cq, rows);
+        depthwise<STRIDE, DWC>(sh.E, par, a, w, c * NC, cq, rows);
         worker_barrier();                              // E and the parameter slot are free for the next chunk
       }
     }
@@ -472,8 +548,10 @@ xdw_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
 // Pipelined, warp-specialized schedule (3xTF32).  The MMA warpgroups run chunk i's expand GEMM and phase (a) into E slot
 // i % NE, hand the slot to the depthwise warpgroup and go straight on to chunk i+1, so the tensor cores work on one chunk
 // while the FP32 pipes run the depthwise conv of the previous one.  Slot hand-offs are mbarriers (efull: 256 MMA-thread
-// arrivals, eempty: 128 depthwise-thread arrivals); a chunk's parameter block lives beside its E slot.  No CTA-wide barrier
-// inside the item loop; the E ring runs across item boundaries like the weight ring.
+// arrivals, eempty: 128 depthwise-thread arrivals).  The depthwise warpgroup, which has slack on most layer shapes, also
+// stages the parameter blocks, so an eempty phase means "slot free and the next chunk's parameters in place" and the MMA
+// warpgroups go from their GEMM to phase (a) without a barrier between them.  No CTA-wide barrier inside the item loop; the E
+// ring runs across item boundaries like the weight ring.
 template <int STRIDE, int X3, int NKB, int KSL, bool SAVE>
 __global__ void __launch_bounds__(WS_THREADS, 1)
 xdw_ws_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
@@ -503,30 +581,45 @@ xdw_ws_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
     if (warp >= NUM_WORKERS / 32) {                    // warpgroup 2: phase (b) of every chunk, slot by slot
         setmaxnreg_inc<DW_REGS>();
         const int d = threadIdx.x - NUM_WORKERS, cq = d & 7;
-        unsigned role[DW_ROLES];
-#pragma unroll
-        for (int j = 0; j < DW_ROLES; ++j) role[j] = dw_role<TO>(a, (d >> 3) + j * (DW_THREADS / 8));
+        constexpr int DWC = dw_cols(STRIDE, true);
+        const unsigned role = dw_role<STRIDE, DWC>(a, d >> 3);
+        // The parameter block of chunk i + NE is staged here: its global loads are issued before chunk i's depthwise conv and
+        // parked after it, then the eempty arrival publishes slot and block together.  Block (i + NE) % (2 NE) was last read
+        // by chunk i - NE, whose phase (a) and (b) are complete for every thread once chunk i's efull has completed.
+        const ParLoader pl0(a, d), pl1(a, d + DW_THREADS);               // float2 owners d and d + 128 of the 208
+        ChunkIter<TO> ahead(a);
+        for (int j = 0; j < NE; ++j, ahead.next(a)) {                     // blocks of the first NE chunks, then free slots
+            if (ahead.valid(a)) {
+                float* par = sh.PAR + j * PAR_FLOATS;
+                pl0.park(par, pl0.load<true>(a, ahead.prob, ahead.c)); pl1.park(par, pl1.load<true>(a, ahead.prob, ahead.c));
+            }
+            mbar_arrive(&sh.eempty[j]);
+        }
         int cc = 0;
         for (ItemIter ii(a); ii.item < a.n_items; ii.next(a)) {
             const Item w = ii.decode<TO>(a);
-            DwRows rows[DW_ROLES];
-#pragma unroll
-            for (int j = 0; j < DW_ROLES; ++j) rows[j] = dw_rows<TO>(a, ii, role[j]);
-            for (int c = w.c_begin; c < w.c_end; ++c, ++cc) {
+            const DwRows rows = dw_rows<STRIDE, DWC>(a, ii, role);
+            for (int c = w.c_begin; c < w.c_end; ++c, ++cc, ahead.next(a)) {
                 const int s = cc % NE;
+                const bool stage = ahead.valid(a);
+                float2 pf0 = make_float2(0.f, 0.f), pf1 = pf0;
+                if (stage) { pf0 = pl0.load<true>(a, ahead.prob, ahead.c); pf1 = pl1.load<true>(a, ahead.prob, ahead.c); }
                 mbar_wait(&sh.efull[s], (uint32_t)(cc / NE) & 1u);
-#pragma unroll 1
-                for (int j = 0; j < DW_ROLES; ++j) depthwise<STRIDE>(sh.E + s * E_FLOATS, sh.PAR + s * PAR_FLOATS, a, w, c * NC, cq, rows[j]);
-                mbar_arrive(&sh.eempty[s]);
+                depthwise<STRIDE, DWC>(sh.E + s * E_FLOATS, sh.PAR + (cc % (2 * NE)) * PAR_FLOATS, a, w, c * NC, cq, rows);
+                if (stage) {
+                    float* par = sh.PAR + ((cc + NE) % (2 * NE)) * PAR_FLOATS;
+                    pl0.park(par, pf0); pl1.park(par, pf1);
+                }
+                mbar_arrive(&sh.eempty[s]);            // slot s drained, chunk cc + NE's parameters staged
             }
         }
         return;
     }
 
-    // warpgroups 0-1: expand GEMM of window half `half`, then phase (a) into the next free E slot
+    // warpgroups 0-1: expand GEMM of window half `half`, then phase (a) into the next free E slot.  The two warpgroups
+    // share no barrier in the loop: each waits for its weights, its window and the E slot on its own.
     setmaxnreg_inc<MMA_REGS>();
     const int half = warp >> 2, wq = warp & 3;
-    const ParLoader pl(a, threadIdx.x);
     int cc = 0, it = 0, n = 0;
     for (ItemIter ii(a); ii.item < a.n_items; ii.next(a), ++n) {
         const Item w = ii.decode<TO>(a);
@@ -535,15 +628,11 @@ xdw_ws_kernel(const __grid_constant__ XdwMaps mp, const XdwArgs a) {
         mbar_wait(&sh.wfull[wb], (uint32_t)(n / L::WBUF) & 1u);
         for (int c = w.c_begin; c < w.c_end; ++c, ++cc) {
             const int s = cc % NE;
-            float* par = sh.PAR + s * PAR_FLOATS;
-            const float2 pf = pl.load(a, w.prob, c);
             float acc[2][NC / 2];
             expand_gemm<X3, NKB, KSL>(acc, win, sh.smem + L::RING, sh.full, sh.empty, it, wq, lane);
             mbar_arrive_if(&sh.wempty[wb], lane == 0 && c + 1 == w.c_end);
-            mbar_wait(&sh.eempty[s], ((uint32_t)(cc / NE) & 1u) ^ 1u);     // phase (b) of chunk cc - NE has drained the slot
-            pl.park(par, pf);
-            worker_barrier();                          // the parameter block is complete before phase (a) reads BN1 from it
-            bn1_relu<STRIDE, SAVE>(acc, sh.E + s * E_FLOATS, par, a, w, c * NC, half, wq, lane);
+            mbar_wait(&sh.eempty[s], (uint32_t)(cc / NE) & 1u);     // slot drained by chunk cc - NE, chunk cc's parameters staged
+            bn1_relu<STRIDE, SAVE>(acc, sh.E + s * E_FLOATS, sh.PAR + (cc % (2 * NE)) * PAR_FLOATS, a, w, c * NC, half, wq, lane);
             mbar_arrive(&sh.efull[s]);
         }
     }
@@ -642,9 +731,13 @@ int xdw_conv(const XdwConv& p, cudaStream_t st, const XdwConv* p2) {
     }
     a.B = p.B;
     a.n_items = nprob * a.tiles_x * a.tiles_y * p.B * a.groups;
-    {
+    {   // depthwise row grouping (dw_role): column runs x row groups over the slots of the schedule's depthwise threads
         const int ncols_e = Wo - (a.tiles_x - 1) * TO, nrows_e = Ho - (a.tiles_y - 1) * TO;
-        auto group = [](int ncols, int nrows) { const int n_rg = std::min(32 / ncols, nrows); return (unsigned)((nrows + n_rg - 1) / n_rg) | (unsigned)n_rg << 4; };
+        const int dw_slots = (p.w1t_lo ? DW_THREADS : NUM_WORKERS) / (NC / 4), dwc = dw_cols(p.stride, p.w1t_lo != nullptr);
+        auto group = [&](int ncols, int nrows) {
+            const int n_rg = std::min(dw_slots / cdiv(ncols, dwc), nrows);
+            return (unsigned)cdiv(nrows, n_rg) | (unsigned)n_rg << 4;
+        };
         a.geom = group(TO, TO) | group(TO, nrows_e) << 8 | group(ncols_e, TO) << 16 | group(ncols_e, nrows_e) << 24;
     }
     const int grid = std::min(a.n_items, slots);         // persistent
