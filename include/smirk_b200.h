@@ -238,7 +238,9 @@ typedef struct {
     /* fp32 tensors of the module's state_dict in state_dict order, `num_batches_tracked` removed.    */
     const float* const* tensors;
     int n_tensors;
-    int precision;             /* 0 = fp32 CUDA-core implicit GEMM, 1 = TF32 wgmma implicit GEMM */
+    int precision;             /* 0 = fp32 CUDA-core implicit GEMM, 1 = TF32 wgmma implicit GEMM,
+                                  3 = 1 with 3xTF32 error-compensated arithmetic (fp32-equivalent forward and input
+                                  gradient on the tensor cores; the same launches as 1).  2 is not a generator precision. */
 } SmkGeneratorDesc;
 
 int smk_generator_create(const SmkGeneratorDesc* desc, SmkGenerator** out);

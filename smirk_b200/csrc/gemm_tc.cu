@@ -1,8 +1,8 @@
 // TF32 tensor-core implicit-GEMM convolution for sm_90a (Hopper wgmma):  C[M,N] = epi( A[M,K] * W[N,K]^T ).
 //
 // This is the tensor-core path of the generator's 3x3 convolutions / transposed convolutions and of
-// the encoder's 1x1 convolutions (precision = 1).  The reference executes these layers as cuDNN
-// TF32 implicit GEMMs (src/smirk_generator.py:56-76,147-178; torch default cudnn.allow_tf32=True);
+// the encoder's 1x1 convolutions (precision = 1; the 3xTF32 instantiations at precision 3).  The reference executes
+// these layers as cuDNN TF32 implicit GEMMs (src/smirk_generator.py:56-76,147-178; torch default cudnn.allow_tf32=True);
 // here they are one hand-written kernel:
 //
 //   * A (activations, NHWC fp32) is fetched tile-by-tile by TMA: `cp.async.bulk.tensor.2d` for 1x1
@@ -82,6 +82,11 @@ gemm_tc_kernel(const __grid_constant__ TcMaps mp, const TcArgs a) {
     //                    Weights are split on the host (TcMaps::blo maps the tails).  The activation tile is split in
     //                    registers by the consumers (A fragments of the register form of wgmma), so shared memory holds
     //                    only the plain kernel's tiles plus the weight tails.
+    //   X3 = 3         : 3xTF32 for deep K (the generator's convolutions, K up to 4608).  The tensor core's accumulator
+    //                    truncates at every wgmma update, and with 3 K / 8 updates into one running sum those losses add
+    //                    up to ~2^-22 K / 8 of the output scale (1e-4 at K = 4608, TF32's order over a network).  Here each
+    //                    k-block's 12 updates go into a fresh register tile that is then added to the running sum by an
+    //                    fp32 (round-to-nearest) add: the truncation only ever sees one k-block's partial sum.
     //   EXTRA = true     : the epilogue also applies `mask` and writes `out2` (backward / grad-mode forward); the forward-only
     //                    instantiations are compiled without them.
     static_assert(!X3 || !PERSIST, "3xTF32 runs single-tile CTAs");
@@ -170,7 +175,7 @@ gemm_tc_kernel(const __grid_constant__ TcMaps mp, const TcArgs a) {
             uint8_t* st = smem + s * STAGE_BYTES;
             const uint32_t sa = smem_u32(st) + (uint32_t)(wg * 64 * BKB);
             const uint32_t sb = smem_u32(st) + A_STAGE_BYTES;
-            if constexpr (X3 != 0) {
+            if constexpr (X3 == 2) {
                 uint32_t hi[BK / MMA_K][4], lo[BK / MMA_K][4];
 #pragma unroll
                 for (int k = 0; k < BK / MMA_K; ++k) {
@@ -191,6 +196,33 @@ gemm_tc_kernel(const __grid_constant__ TcMaps mp, const TcArgs a) {
                 wgmma_wait<0>();
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&empty[s]);
+            } else if constexpr (X3 == 3) {
+                // as X3 = 2, into a zeroed tile dk, then d += dk in fp32
+                float dk[BN / 2];
+                uint32_t hi[BK / MMA_K][4], lo[BK / MMA_K][4];
+#pragma unroll
+                for (int k = 0; k < BK / MMA_K; ++k) {
+                    float v[4];
+                    load_a_frag(st, wg * 64, k * MMA_K, wq, lane, v);
+                    split_frag(v, hi[k], lo[k]);
+                }
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) dk[i] = 0.f;
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / MMA_K; ++k) {
+                    const uint64_t db = make_smem_desc(sb + k * MMA_K * 4);
+                    const uint64_t dbl = make_smem_desc(smem_u32(st) + BLO_OFF + k * MMA_K * 4);
+                    Wgmma<BN>::rs(dk, hi[k], db, 1u);
+                    Wgmma<BN>::rs(dk, lo[k], db, 1u);
+                    Wgmma<BN>::rs(dk, hi[k], dbl, 1u);
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[s]);
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) d[i] += dk[i];
             } else {
                 wgmma_fence();
 #pragma unroll
@@ -420,7 +452,7 @@ int launch_kernel(const TcMaps& mp, const TcArgs& a_in, cudaStream_t st, int gro
 
 template <int BN, int STAGES, int MINB, bool PERSIST, int X3 = 0>
 int launch(const TcMaps& mp, const TcArgs& a, cudaStream_t st, int groups) {
-    if constexpr (X3 == 0) {
+    if constexpr (X3 != 2) {                            // X3 = 2 runs plain GEMMs only (tc_conv)
         if (a.mask || a.out2) return launch_kernel<BN, STAGES, MINB, PERSIST, X3, true>(mp, a, st, groups);
     }
     return launch_kernel<BN, STAGES, MINB, PERSIST, X3, false>(mp, a, st, groups);
@@ -444,6 +476,10 @@ int tc_conv(const Conv& p, cudaStream_t st, const Conv* p2) {
     // halves the A-operand bytes wgmma pulls from shared memory per FLOP (TF32 operands are 4 bytes; at BN = 128 the
     // operand reads ask for more than an SM's shared-memory bandwidth).  One persistent CTA per SM, 4-stage ring.
     if (p.mode != 0 && p.N % 256 == 0 && !p.wt_lo) BN = 256;
+    // 3xTF32: plain 1x1 GEMMs (the encoder's 1x1 convs, K <= 960) run X3 = 2; every other problem (3x3 convs, the shuffled
+    // store, the mask / second store: the generator's convolutions, K up to 4608) X3 = 3, with 64-wide tiles at most.
+    const int x3 = !p.wt_lo ? 0 : (p.mode == 0 && p.store == 0 && !p.mask && !p.out2) ? 2 : 3;
+    if (x3 == 3) BN = std::min(BN, 64);
     TcMaps mp;
     TcArgs a{};
     a.M = M; a.N = p.N; a.nkb = cdiv(p.K, BK); a.mode = p.mode == 0 ? 0 : 1; a.H = p.H; a.W = p.W;
@@ -452,10 +488,9 @@ int tc_conv(const Conv& p, cudaStream_t st, const Conv* p2) {
     a.ld_out = p.ld_out; a.store = p.store; a.round_out = p.round_out;
     a.head_w = p.head_w; a.head_b = p.head_b; a.head_c = p.head_c;
     SMK_REQUIRE(p.store != 3 || (p.N == 32 && p.mode != 0 && p.head_w && p.head_b && p.head_c >= 1 && p.head_c <= 4 && !p.res && !p2),
-                "tc_conv: the fused 1x1 head needs a 3x3 conv with N == 32 (persistent kernel, one full column tile) and 1..4 head channels");
-    SMK_REQUIRE(!p.wt_lo || (p.mode == 0 && p.store == 0), "tc_conv: the 3xTF32 path covers plain 1x1 convolutions / GEMMs");
-    SMK_REQUIRE((!p.mask || p.store == 0) && (!p.out2 || p.store != 1) && (!(p.mask || p.out2) || (!p2 && !p.wt_lo)),
-                "tc_conv: the mask needs store 0, the second store a non-shuffled store, both a single TF32 problem");
+                "tc_conv: the fused 1x1 head needs a 3x3 conv with N == 32 (one full column tile) and 1..4 head channels");
+    SMK_REQUIRE((!p.mask || p.store == 0) && (!p.out2 || p.store != 1) && (!(p.mask || p.out2) || !p2),
+                "tc_conv: the mask needs store 0, the second store a non-shuffled store, both a single problem");
     a.mask = p.mask; a.ld_mask = p.ld_mask; a.out2 = p.out2; a.ld_out2 = p.ld_out2;
     for (int g = 0; g < groups; ++g) {
         const Conv& q = g ? *p2 : p;
@@ -474,8 +509,10 @@ int tc_conv(const Conv& p, cudaStream_t st, const Conv* p2) {
     if (groups == 1) { mp.a[1] = mp.a[0]; mp.b[1] = mp.b[0]; mp.blo[1] = mp.blo[0]; a.scale[1] = a.scale[0]; a.bias[1] = a.bias[0]; a.res[1] = a.res[0]; a.out[1] = a.out[0]; }
     {
         const double cin_eff = p.mode == 0 ? p.K : p.Cin;
-        const char* tag = p.tag ? p.tag : p.mode == 0 ? (p.store == 1 ? "upconv_gemm_tc" : (p.wt_lo ? "pw_gemm_tc3x" : "pw_gemm_tc"))
-                                      : (p.store == 3 ? "conv3x3_head_gemm_tc" : "conv3x3_gemm_tc");
+        const char* tag = p.tag ? p.tag
+                        : p.mode == 0 ? (p.store == 1 ? (p.wt_lo ? "upconv_gemm_tc3x" : "upconv_gemm_tc") : (p.wt_lo ? "pw_gemm_tc3x" : "pw_gemm_tc"))
+                        : p.store == 3 ? (p.wt_lo ? "conv3x3_head_gemm_tc3x" : "conv3x3_head_gemm_tc")
+                                       : (p.wt_lo ? "conv3x3_gemm_tc3x" : "conv3x3_gemm_tc");
         if (g_prof_detail) tag = prof_shape_tag(tag, (long)groups * M, p.K, p.N);
         SMK_TAG(tag,
                 groups * 4.0 * ((double)M * cin_eff + (double)p.K * p.N + (double)M * p.N * (1 + !!p.res + !!p.mask + !!p.out2) + 2.0 * p.N),
@@ -486,7 +523,15 @@ int tc_conv(const Conv& p, cudaStream_t st, const Conv* p2) {
     // <64,2,3> spill (16-220 B) and the 3xTF32 <32,2,3> serialises its wgmmas; spill-free budgets (lower MINB) were measured
     // slower end to end on H100 (fewer CTAs of the concurrent pipeline share an SM), and 128-wide tiles in place of
     // <256,...> much slower, so the spills stay.
-    if (p.wt_lo) {                                      // 3xTF32: fp32-equivalent arithmetic (encoder precision 3)
+    // 3xTF32: fp32-equivalent arithmetic (encoder and generator precision 3).  Every mode and store, one tile per CTA (the fused
+    // head loads its constants per CTA); the EXTRA instantiations carry the generator's grad-mode forward and dgrads.
+    // X3 = 3 holds BN / 2 more accumulators: one step lower MINB, and 64-wide tiles at most (a 128-wide tile needs more than
+    // the 168 registers of MINB = 1 and spills); ptxas: <32, 2, 2> 80 / 77 registers, <64, 2, 1> 132 / 126, no spills.
+    if (x3 == 3) {
+        if (BN == 32) return launch<32, 2, 2, false, 3>(mp, a, st, groups);
+        return launch<64, 2, 1, false, 3>(mp, a, st, groups);
+    }
+    if (p.wt_lo) {
         if (BN == 32) return launch<32, 2, 3, false, 2>(mp, a, st, groups);
         if (BN == 64) return launch<64, 2, 2, false, 2>(mp, a, st, groups);
         return launch<128, 2, 1, false, 2>(mp, a, st, groups);
@@ -533,6 +578,25 @@ extern "C" int smk_debug_gemm_tc3x(const float* in, int ld_in, int M, const floa
     smk::Conv p{};
     p.in = in; p.ld_in = ld_in; p.B = 1; p.H = 1; p.W = M; p.Cin = K; p.wt = wt_hi; p.wt_lo = wt_lo; p.scale = scale; p.bias = bias; p.N = N; p.K = K;
     p.mode = 0; p.relu = relu; p.res = res; p.ld_res = ld_res; p.res_pad = 0; p.out = out; p.ld_out = ld_out; p.store = 0; p.round_out = 0;
+    return smk::tc_conv(p, (cudaStream_t)stream);
+}
+// smk_debug_conv_tc on the 3xTF32 path, with every epilogue option of the generator's convolutions: mask [M, ld_mask]
+// (zero outputs whose mask <= 0; store 0), out2 [M, ld_out2] (the stored activations again, compact; stores 0, 2, 3) and
+// the fused head of store 3 (head_w [N][head_c], head_b [head_c], out [B, head_c, H, W] NCHW, N == 32, 1 <= head_c <= 4).
+// Null mask / out2 / head pointers: not used.  Nothing is rounded to TF32.  Each 32-deep k-block is summed apart (X3 = 3),
+// except for a plain 1x1 GEMM (mode 0, store 0, no mask / out2), which runs smk_debug_gemm_tc3x's arithmetic.
+// A kernel-test entry point: it is exported but not part of include/smirk_b200.h, and tests/test_gpu_generator_x3.py
+// declares its argument types itself.
+extern "C" int smk_debug_conv_tc3x(const float* in, int ld_in, int B, int H, int W, int Cin, const float* wt_hi, const float* wt_lo,
+                                   const float* scale, const float* bias, int N, int K, int mode, int relu, const float* res, int ld_res,
+                                   int res_pad, float* out, int ld_out, int store, const float* mask, int ld_mask, float* out2, int ld_out2,
+                                   const float* head_w, const float* head_b, int head_c, void* stream) {
+    SMK_REQUIRE(wt_hi && wt_lo, "smk_debug_conv_tc3x: the weight heads and tails are both required");
+    smk::Conv p{};
+    p.in = in; p.ld_in = ld_in; p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.wt = wt_hi; p.wt_lo = wt_lo; p.scale = scale; p.bias = bias;
+    p.N = N; p.K = K; p.mode = mode; p.relu = relu; p.res = res; p.ld_res = ld_res; p.res_pad = res_pad; p.out = out; p.ld_out = ld_out;
+    p.store = store; p.round_out = 0; p.mask = mask; p.ld_mask = ld_mask; p.out2 = out2; p.ld_out2 = ld_out2;
+    p.head_w = head_w; p.head_b = head_b; p.head_c = head_c;
     return smk::tc_conv(p, (cudaStream_t)stream);
 }
 extern "C" int smk_debug_reflect_halo(float* buf, int B, int H, int W, int C, void* stream) {

@@ -15,6 +15,9 @@
 //              reflection-padded [B,16,16,512] buffers: each conv's epilogue writes the interior, a
 //              tiny kernel mirrors the 1-pixel halo, and the next conv's im2col TMA reads it with no
 //              padding — the hardware cannot reflect, so the halo is made explicit once per layer.
+// precision 3: precision 1's launches with 3xTF32 arithmetic (gemm_tc's X3 = 3 instantiations): every weight, forward and
+//              dgrad, is packed as a TF32 head plus a TF32 tail, the kernels split the activations themselves, and nothing
+//              is rounded to TF32 between layers — fp32-equivalent results on the tensor cores.
 //
 // Input gradient (frozen weights, eval BN): smk_generator_forward_saved runs the same launches with the post-ReLU outputs
 // of every block conv and ResNet conv1 written to a caller-owned `saved` buffer (by redirecting the store, or by a second
@@ -35,54 +38,70 @@ using smk::grid_of;
 constexpr float kBnEps = 1e-5f;
 
 // dw: dgrad weights, W' scaled by the folded BN scale: [9*cout][cin_p] (fp32) or [cin_p][9*cout] (TF32), k = tap' * cout + co
-struct Conv3 { float* w; float* wt; float* scale; float* bias; float* dw; int cin, cin_p, cout; };  // w: [9*cin_p][cout]; wt: [cout][9*cin_p]
+// wt_lo / dw_lo (precision 3): the TF32 tails of wt / dw, which then hold the TF32 heads
+struct Conv3 { float* w; float* wt; float* wt_lo; float* scale; float* bias; float* dw; float* dw_lo; int cin, cin_p, cout; };  // w: [9*cin_p][cout]; wt: [cout][9*cin_p]
 // dw: [4*cout][cin] (fp32) or [cin][4*cout] (TF32), k = (dy*2+dx) * cout + co
-struct UpConv { float* w; float* wt; float* scale; float* bias; float* dw; int cin, cout; };         // w: [cin][4*cout];   wt: [4*cout][cin]
+struct UpConv { float* w; float* wt; float* wt_lo; float* scale; float* bias; float* dw; float* dw_lo; int cin, cout; };         // w: [cin][4*cout];   wt: [4*cout][cin]
 
-bool fold_conv3(TensorCursor& cur, int cin, int cin_p, int cout, bool tc, smk::DeviceArena& arena, Conv3* out, cudaError_t* err) {
+// Tensor-core weight v at index i: the TF32 head, and with x3 the TF32 tail of what the head leaves (v = head + tail up to
+// 2^-22 |v|), the split encoder.cu packs for its 3xTF32 1x1 convs.
+void pack_tc(std::vector<float>& hi, std::vector<float>& lo, size_t i, float v, bool x3) {
+    hi[i] = smk::round_tf32_host(v);
+    if (x3) lo[i] = smk::round_tf32_host(v - hi[i]);
+}
+
+bool fold_conv3(TensorCursor& cur, int cin, int cin_p, int cout, bool tc, bool x3, smk::DeviceArena& arena, Conv3* out, cudaError_t* err) {
     const float* w = cur.next(); const float* g = cur.next(); const float* b = cur.next();
     const float* mu = cur.next(); const float* var = cur.next();
     if (!w || !g || !b || !mu || !var) return false;
     const size_t K = (size_t)9 * cin_p, Kd = (size_t)9 * cout;
-    std::vector<float> W(K * cout, 0.f), D(Kd * cin_p, 0.f), S(cout), Bi(cout);
+    std::vector<float> W(K * cout, 0.f), D(Kd * cin_p, 0.f), S(cout), Bi(cout), Wlo, Dlo;
+    if (x3) { Wlo.assign(W.size(), 0.f); Dlo.assign(D.size(), 0.f); }
     smk::fold_bn(g, b, mu, var, cout, kBnEps, S.data(), Bi.data());
     for (int o = 0; o < cout; ++o)
         for (int c = 0; c < cin; ++c)
             for (int k = 0; k < 9; ++k) {
                 float v = w[((size_t)o * cin + c) * 9 + k];
-                if (tc) W[(size_t)o * K + (size_t)k * cin_p + c] = smk::round_tf32_host(v);   // [N][K], TF32-rounded
+                if (tc) pack_tc(W, Wlo, (size_t)o * K + (size_t)k * cin_p + c, v, x3);   // [N][K], TF32 heads (+ tails)
                 else W[((size_t)k * cin_p + c) * cout + o] = v;                // [K][N]
-                const float vd = v * S[o];
+                const float vd = v * S[o];                                     // split after the BN-scale multiply
                 const size_t kd = (size_t)(8 - k) * cout + o;                  // rotated tap
-                if (tc) D[(size_t)c * Kd + kd] = smk::round_tf32_host(vd);
+                if (tc) pack_tc(D, Dlo, (size_t)c * Kd + kd, vd, x3);
                 else D[kd * cin_p + c] = vd;
             }
-    out->cin = cin; out->cin_p = cin_p; out->cout = cout; out->w = out->wt = nullptr;
+    out->cin = cin; out->cin_p = cin_p; out->cout = cout;
+    out->w = out->wt = out->wt_lo = out->dw_lo = nullptr;
     cudaError_t e = arena.upload(W, tc ? &out->wt : &out->w);
+    if (e == cudaSuccess && x3) e = arena.upload(Wlo, &out->wt_lo);
     if (e == cudaSuccess) e = arena.upload(D, &out->dw);
+    if (e == cudaSuccess && x3) e = arena.upload(Dlo, &out->dw_lo);
     if (e == cudaSuccess) e = arena.upload(S, &out->scale);
     if (e == cudaSuccess) e = arena.upload(Bi, &out->bias);
     *err = e;
     return e == cudaSuccess;
 }
 
-bool fold_upconv(TensorCursor& cur, int cin, int cout, bool tc, smk::DeviceArena& arena, UpConv* out, cudaError_t* err) {
+bool fold_upconv(TensorCursor& cur, int cin, int cout, bool tc, bool x3, smk::DeviceArena& arena, UpConv* out, cudaError_t* err) {
     const float* w = cur.next(); const float* b = cur.next();        // weight [cin, cout, 2, 2], bias [cout]
     if (!w || !b) return false;
-    std::vector<float> W((size_t)cin * 4 * cout), D((size_t)cin * 4 * cout), S((size_t)4 * cout, 1.f), Bi((size_t)4 * cout);
+    std::vector<float> W((size_t)cin * 4 * cout), D((size_t)cin * 4 * cout), S((size_t)4 * cout, 1.f), Bi((size_t)4 * cout), Wlo, Dlo;
+    if (x3) { Wlo.assign(W.size(), 0.f); Dlo.assign(D.size(), 0.f); }
     for (int c = 0; c < cin; ++c)
         for (int o = 0; o < cout; ++o)
             for (int q = 0; q < 4; ++q) {
                 float v = w[((size_t)c * cout + o) * 4 + q];
-                if (tc) W[((size_t)q * cout + o) * cin + c] = smk::round_tf32_host(v);   // [N = 4*cout][K = cin]
+                if (tc) pack_tc(W, Wlo, ((size_t)q * cout + o) * cin + c, v, x3);   // [N = 4*cout][K = cin]
                 else W[(size_t)c * 4 * cout + q * cout + o] = v;               // [K][N]
-                if (tc) D[(size_t)c * 4 * cout + q * cout + o] = smk::round_tf32_host(v);  // dgrad [N = cin][K = 4*cout]
+                if (tc) pack_tc(D, Dlo, (size_t)c * 4 * cout + q * cout + o, v, x3);  // dgrad [N = cin][K = 4*cout]
                 else D[((size_t)q * cout + o) * cin + c] = v;                  // dgrad [K][N]
             }
     for (int q = 0; q < 4; ++q) for (int o = 0; o < cout; ++o) Bi[q * cout + o] = b[o];
-    out->cin = cin; out->cout = cout; out->w = out->wt = nullptr;
+    out->cin = cin; out->cout = cout;
+    out->w = out->wt = out->wt_lo = out->dw_lo = nullptr;
     cudaError_t e = arena.upload(W, tc ? &out->wt : &out->w);
+    if (e == cudaSuccess && x3) e = arena.upload(Wlo, &out->wt_lo);
     if (e == cudaSuccess) e = arena.upload(D, &out->dw);
+    if (e == cudaSuccess && x3) e = arena.upload(Dlo, &out->dw_lo);
     if (e == cudaSuccess) e = arena.upload(S, &out->scale);
     if (e == cudaSuccess) e = arena.upload(Bi, &out->bias);
     *err = e;
@@ -105,33 +124,34 @@ struct SmkGenerator {
 
 extern "C" int smk_generator_create(const SmkGeneratorDesc* desc, SmkGenerator** out) {
     SMK_REQUIRE(desc && out && desc->tensors, "smk_generator_create: null argument");
-    SMK_REQUIRE(desc->precision == 0 || desc->precision == 1, "smk_generator_create: precision must be 0 (fp32) or 1 (tf32 wgmma)");
+    SMK_REQUIRE(desc->precision == 0 || desc->precision == 1 || desc->precision == 3,
+                "smk_generator_create: precision must be 0, 1 or 3 (0 = fp32 CUDA cores, 1 = TF32 wgmma, 3 = 3xTF32 wgmma: fp32-equivalent)");
     SMK_REQUIRE(desc->init_features % 8 == 0 && desc->out_channels <= 4 && desc->in_channels >= 1,
                 "smk_generator_create: need init_features %% 8 == 0 and out_channels <= 4");
     SMK_REQUIRE(desc->precision == 0 || desc->init_features % 32 == 0, "smk_generator_create: the tensor-core path needs init_features %% 32 == 0");
-    if (desc->precision == 1) { if (int rc = smk::tc_init()) return rc; }
+    const bool tc = desc->precision != 0, x3 = desc->precision == 3;     // tensor cores; 3xTF32 arithmetic on them
+    if (tc) { if (int rc = smk::tc_init()) return rc; }
     SmkGenerator* h = new SmkGenerator();
     h->cin = desc->in_channels; h->cout = desc->out_channels;
-    h->cin_p = desc->precision == 1 ? (desc->in_channels + 31) & ~31 : (desc->in_channels + 7) & ~7;
+    h->cin_p = tc ? (desc->in_channels + 31) & ~31 : (desc->in_channels + 7) & ~7;
     h->f = desc->init_features; h->nres = desc->res_blocks; h->precision = desc->precision;
     const int f = h->f;
-    const bool tc = h->precision == 1;
     TensorCursor cur{desc->tensors, desc->n_tensors};
     cudaError_t e = cudaSuccess;
     bool ok = true;
     int c_in = h->cin, c_in_p = h->cin_p;
     for (int l = 0; ok && l < 5; ++l) {
         int co = f << l;
-        ok = fold_conv3(cur, c_in, c_in_p, co, tc, h->arena, &h->enc[l][0], &e) &&
-             fold_conv3(cur, co, co, co, tc, h->arena, &h->enc[l][1], &e);
+        ok = fold_conv3(cur, c_in, c_in_p, co, tc, x3, h->arena, &h->enc[l][0], &e) &&
+             fold_conv3(cur, co, co, co, tc, x3, h->arena, &h->enc[l][1], &e);
         c_in = c_in_p = co;
     }
     h->res.resize((size_t)2 * h->nres);
-    for (int r = 0; ok && r < 2 * h->nres; ++r) ok = fold_conv3(cur, 16 * f, 16 * f, 16 * f, tc, h->arena, &h->res[r], &e);
+    for (int r = 0; ok && r < 2 * h->nres; ++r) ok = fold_conv3(cur, 16 * f, 16 * f, 16 * f, tc, x3, h->arena, &h->res[r], &e);
     for (int l = 0; ok && l < 4; ++l) {          // level 4 -> 1
         int ci = (16 * f) >> l, co = ci / 2;
-        ok = fold_upconv(cur, ci, co, tc, h->arena, &h->up[l], &e) && fold_conv3(cur, 2 * co, 2 * co, co, tc, h->arena, &h->dec[l][0], &e) &&
-             fold_conv3(cur, co, co, co, tc, h->arena, &h->dec[l][1], &e);
+        ok = fold_upconv(cur, ci, co, tc, x3, h->arena, &h->up[l], &e) && fold_conv3(cur, 2 * co, 2 * co, co, tc, x3, h->arena, &h->dec[l][0], &e) &&
+             fold_conv3(cur, co, co, co, tc, x3, h->arena, &h->dec[l][1], &e);
     }
     if (ok) {
         const float* w = cur.next(); const float* b = cur.next();
@@ -186,22 +206,23 @@ Plan make_plan(const SmkGenerator* h) {
     }
     size_t sb = S >> 4, cb = (size_t)h->f * 16;
     P.tb = P.b0 = P.b1 = sb * sb * cb;
-    P.pad[0] = P.pad[1] = P.pad[2] = h->precision == 1 ? (sb + 2) * (sb + 2) * cb : 0;
+    P.pad[0] = P.pad[1] = P.pad[2] = h->precision != 0 ? (sb + 2) * (sb + 2) * cb : 0;
     return P;
 }
 
 // One 3x3 convolution, dispatched on the handle's precision.
-//   refl   : reflection padding (ResNet blocks).  At precision 1 `in` must then be a padded buffer.
-//   store  : 0 plain / slice, 2 interior of a padded buffer (precision 1 only)
+//   refl   : reflection padding (ResNet blocks).  At precisions 1 and 3 `in` must then be a padded buffer.
+//   store  : 0 plain / slice, 2 interior of a padded buffer (precisions 1 and 3 only)
 //   out2   : optional second, compact [B,S,S,cout] store of the activations (the grad-mode forward's saved copy)
 int conv3(const SmkGenerator* h, const Conv3& c, const float* in, int ld_in, int B, int S, bool refl, bool relu,
           const float* res, int res_pad, float* out, int ld_out, int store, cudaStream_t st, bool fuse_head = false,
           float* out2 = nullptr) {
     smk::Conv p{};
     if (fuse_head) { p.head_w = h->fw; p.head_b = h->fb; p.head_c = h->cout; }
-    p.in = in; p.ld_in = ld_in; p.B = B; p.H = S; p.W = S; p.Cin = c.cin_p; p.w = c.w; p.wt = c.wt; p.scale = c.scale; p.bias = c.bias;
+    p.in = in; p.ld_in = ld_in; p.B = B; p.H = S; p.W = S; p.Cin = c.cin_p; p.w = c.w; p.wt = c.wt; p.wt_lo = c.wt_lo; p.scale = c.scale; p.bias = c.bias;
     p.N = c.cout; p.K = 9 * c.cin_p; p.mode = refl ? 2 : 1; p.relu = relu ? 1 : 0;
-    p.res = res; p.ld_res = c.cout; p.res_pad = res_pad; p.out = out; p.ld_out = ld_out; p.store = store; p.round_out = c.wt ? 1 : 0;
+    p.res = res; p.ld_res = c.cout; p.res_pad = res_pad; p.out = out; p.ld_out = ld_out; p.store = store;
+    p.round_out = c.wt && !c.wt_lo ? 1 : 0;        // TF32 consumers; 3xTF32 consumers split full fp32 activations themselves
     p.out2 = out2; p.ld_out2 = c.cout;
     return smk::conv(p, st);
 }
@@ -219,7 +240,7 @@ int generator_forward(const SmkGenerator* h, const float* x, int B, float* y, fl
     smk::Workspace w(ws, ws_bytes);
     const Plan P = make_plan(h);
     const int f = h->f;
-    const bool tc = h->precision == 1;
+    const bool tc = h->precision != 0;             // tensor cores (TF32 or 3xTF32): padded ResNet stream, fused head
     auto SV = [&](int i) -> float* { return sv ? sv + (size_t)B * h->saved.off[i] : nullptr; };
     float* x8 = w.take<float>(P.x8 * B);
     float *cat[4], *t[4], *d[4], *p[4];
@@ -231,7 +252,7 @@ int generator_forward(const SmkGenerator* h, const float* x, int B, float* y, fl
     float* pad[3] = {nullptr, nullptr, nullptr};
     if (tc) for (int i = 0; i < 3; ++i) pad[i] = w.take<float>(P.pad[i] * B);
     SMK_REQUIRE(b1 != nullptr && (!tc || pad[2] != nullptr), "smk_generator_forward: workspace carve-up failed");
-    int rc = smk::nchw_to_nhwc_pad(x, B, h->cin, 224, 224, h->cin_p, x8, st, tc);
+    int rc = smk::nchw_to_nhwc_pad(x, B, h->cin, 224, 224, h->cin_p, x8, st, h->precision == 1);
     if (rc) return rc;
     // encoder levels: conv1 -> t[l]; conv2 -> upper half of cat[l] (the skip); pool -> p[l]
     const float* in = x8; int ld = h->cin_p;
@@ -279,8 +300,8 @@ int generator_forward(const SmkGenerator* h, const float* x, int B, float* y, fl
         int lvl = 3 - l;                            // index into cat/t/d (3 = 28x28 ... 0 = 224x224)
         const UpConv& u = h->up[l];
         smk::Conv q{};
-        q.in = din; q.ld_in = u.cin; q.B = B; q.H = dS; q.W = dS; q.Cin = u.cin; q.w = u.w; q.wt = u.wt; q.scale = u.scale; q.bias = u.bias;
-        q.N = 4 * u.cout; q.K = u.cin; q.mode = 0; q.out = cat[lvl]; q.ld_out = 2 * u.cout; q.store = 1; q.round_out = u.wt ? 1 : 0;
+        q.in = din; q.ld_in = u.cin; q.B = B; q.H = dS; q.W = dS; q.Cin = u.cin; q.w = u.w; q.wt = u.wt; q.wt_lo = u.wt_lo; q.scale = u.scale; q.bias = u.bias;
+        q.N = 4 * u.cout; q.K = u.cin; q.mode = 0; q.out = cat[lvl]; q.ld_out = 2 * u.cout; q.store = 1; q.round_out = u.wt && !u.wt_lo ? 1 : 0;
         if ((rc = smk::conv(q, st))) return rc;
         dS *= 2;
         float* dt = sv ? SV(sv_dec(h, lvl, 0)) : t[lvl];
@@ -432,22 +453,24 @@ nhwc_to_nchw_kernel(const float* __restrict__ in, int B, int HW, int Cp, int C, 
 // dgrad of a 3x3 conv (zero padding 1): g_in = conv3x3(g, W') over S x S, * [mask > 0] (mask: the saved input activation).
 int dgrad3(const SmkGenerator* h, const Conv3& c, const float* g, int B, int S, const float* mask, float* out, int ld_out, bool round,
            cudaStream_t st) {
-    const bool tc = h->precision == 1;
+    const bool tc = h->precision != 0;
     smk::Conv p{};
-    p.in = g; p.ld_in = c.cout; p.B = B; p.H = S; p.W = S; p.Cin = c.cout; p.w = tc ? nullptr : c.dw; p.wt = tc ? c.dw : nullptr; p.scale = h->ones; p.bias = h->zeros;
+    p.in = g; p.ld_in = c.cout; p.B = B; p.H = S; p.W = S; p.Cin = c.cout; p.w = tc ? nullptr : c.dw; p.wt = tc ? c.dw : nullptr; p.wt_lo = c.dw_lo;
+    p.scale = h->ones; p.bias = h->zeros;
     p.N = c.cin_p; p.K = 9 * c.cout; p.mode = 1; p.out = out; p.ld_out = ld_out; p.round_out = round ? 1 : 0;
-    p.mask = mask; p.ld_mask = c.cin_p; p.tag = tc ? "conv3x3_dgrad_tc" : "conv3x3_dgrad_f32";
+    p.mask = mask; p.ld_mask = c.cin_p; p.tag = c.dw_lo ? "conv3x3_dgrad_tc3x" : tc ? "conv3x3_dgrad_tc" : "conv3x3_dgrad_f32";
     return smk::conv(p, st);
 }
 
 // dgrad of ConvTranspose2d(k2, s2): g_in[S x S, cin] = s2d(g_out)[S x S, 4 cout] . W'^T, * [mask > 0].
 int dgrad_up(const SmkGenerator* h, const UpConv& u, const float* s2d, int B, int S, const float* mask, float* out, bool round, cudaStream_t st) {
-    const bool tc = h->precision == 1;
+    const bool tc = h->precision != 0;
     const int K = 4 * u.cout;
     smk::Conv p{};
-    p.in = s2d; p.ld_in = K; p.B = B; p.H = S; p.W = S; p.Cin = K; p.w = tc ? nullptr : u.dw; p.wt = tc ? u.dw : nullptr; p.scale = h->ones; p.bias = h->zeros;
+    p.in = s2d; p.ld_in = K; p.B = B; p.H = S; p.W = S; p.Cin = K; p.w = tc ? nullptr : u.dw; p.wt = tc ? u.dw : nullptr; p.wt_lo = u.dw_lo;
+    p.scale = h->ones; p.bias = h->zeros;
     p.N = u.cin; p.K = K; p.mode = 0; p.out = out; p.ld_out = u.cin; p.round_out = round ? 1 : 0;
-    p.mask = mask; p.ld_mask = u.cin; p.tag = tc ? "upconv_dgrad_tc" : "upconv_dgrad_f32";
+    p.mask = mask; p.ld_mask = u.cin; p.tag = u.dw_lo ? "upconv_dgrad_tc3x" : tc ? "upconv_dgrad_tc" : "upconv_dgrad_f32";
     return smk::conv(p, st);
 }
 
@@ -519,7 +542,7 @@ extern "C" int smk_generator_backward(const SmkGenerator* h, int B, const float*
     SMK_REQUIRE(ws && ws_bytes > 0 && ws_bytes >= smk_generator_backward_workspace_bytes(h, B), "smk_generator_backward: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     const int f = h->f, cb = 16 * f;
-    const bool tc = h->precision == 1;
+    const bool rnd = h->precision == 1;            // TF32 rounding of every gradient a TF32 dgrad reads (not at 3xTF32)
     auto SV = [&](int i) -> const float* { return saved + (size_t)B * h->saved.off[i]; };
     const GradPlan P = make_grad_plan(h);
     smk::Workspace w(ws, ws_bytes);
@@ -536,14 +559,14 @@ extern "C" int smk_generator_backward(const SmkGenerator* h, int B, const float*
         const long total = (long)B * 224 * 224 * (f / 4);
         SMK_TAG("head_dgrad", 4.0 * B * 224.0 * 224.0 * (2.0 * h->cout + 2.0 * f), 2.0 * B * 224.0 * 224.0 * f * h->cout, st);
         SMK_LAUNCH(head_bwd_kernel, dim3(smk::cdiv(total, 256)), dim3(256), 0, st, g_y, y, B, 224 * 224, h->cout, h->fw,
-                   SV(sv_dec(h, 0, 1)), f, tc ? 1 : 0, A);
+                   SV(sv_dec(h, 0, 1)), f, rnd ? 1 : 0, A);
         SMK_CHECK_LAUNCH();
     }
     // decoder levels 1..4: conv2, conv1 (both halves of the concat), up-convolution
     for (int lvl = 0; lvl < 4; ++lvl) {
         const int i = 3 - lvl, S = 224 >> lvl, c = f << lvl;
-        if ((rc = dgrad3(h, h->dec[i][1], A, B, S, SV(sv_dec(h, lvl, 0)), Bf, c, tc, st))) return rc;
-        if ((rc = dgrad3(h, h->dec[i][0], Bf, B, S, nullptr, gcat[lvl], 2 * c, tc, st))) return rc;
+        if ((rc = dgrad3(h, h->dec[i][1], A, B, S, SV(sv_dec(h, lvl, 0)), Bf, c, rnd, st))) return rc;
+        if ((rc = dgrad3(h, h->dec[i][0], Bf, B, S, nullptr, gcat[lvl], 2 * c, rnd, st))) return rc;
         {
             const long total = (long)B * (S / 2) * (S / 2) * 4 * (c / 4);
             SMK_TAG("upconv_s2d", 8.0 * B * S * S * c, 0.0, st);
@@ -551,37 +574,37 @@ extern "C" int smk_generator_backward(const SmkGenerator* h, int B, const float*
             SMK_CHECK_LAUNCH();
         }
         const float* m = lvl < 3 ? SV(sv_dec(h, lvl + 1, 1)) : (h->nres == 0 ? SV(sv_bott(1)) : nullptr);
-        if ((rc = dgrad_up(h, h->up[i], s2d, B, S / 2, m, A, tc, st))) return rc;
+        if ((rc = dgrad_up(h, h->up[i], s2d, B, S / 2, m, A, rnd, st))) return rc;
     }
     // ResNet blocks, last to first, over zero-haloed 16 x 16 gradient buffers: g_x = fold(conv(G(fold(conv(G(g)) * [u > 0])))) + g
     float* g = A;                                    // gradient of the bottleneck's conv2 output, [B,14,14,cb]
     if (h->nres > 0) {
         float *cur = pad[0], *nxt = pad[1], *gP = pad[2], *gu = pad[3];
-        if ((rc = fold(nullptr, A, 0, nullptr, B, cb, tc, cur, 1, st))) return rc;
+        if ((rc = fold(nullptr, A, 0, nullptr, B, cb, rnd, cur, 1, st))) return rc;
         for (int r = h->nres - 1; r >= 0; --r) {
-            if ((rc = dgrad3(h, h->res[2 * r + 1], cur, B, 16, nullptr, gP, cb, tc, st))) return rc;
-            if ((rc = fold(gP, nullptr, 0, SV(sv_res(r)), B, cb, tc, gu, 1, st))) return rc;
-            if ((rc = dgrad3(h, h->res[2 * r], gu, B, 16, nullptr, gP, cb, tc, st))) return rc;
-            if (r == 0) { if ((rc = fold(gP, cur, 1, SV(sv_bott(1)), B, cb, tc, Bf, 0, st))) return rc; }
-            else { if ((rc = fold(gP, cur, 1, nullptr, B, cb, tc, nxt, 1, st))) return rc; std::swap(cur, nxt); }
+            if ((rc = dgrad3(h, h->res[2 * r + 1], cur, B, 16, nullptr, gP, cb, rnd, st))) return rc;
+            if ((rc = fold(gP, nullptr, 0, SV(sv_res(r)), B, cb, rnd, gu, 1, st))) return rc;
+            if ((rc = dgrad3(h, h->res[2 * r], gu, B, 16, nullptr, gP, cb, rnd, st))) return rc;
+            if (r == 0) { if ((rc = fold(gP, cur, 1, SV(sv_bott(1)), B, cb, rnd, Bf, 0, st))) return rc; }
+            else { if ((rc = fold(gP, cur, 1, nullptr, B, cb, rnd, nxt, 1, st))) return rc; std::swap(cur, nxt); }
         }
         g = Bf;
     }
     float* o = g == A ? Bf : A;
-    if ((rc = dgrad3(h, h->enc[4][1], g, B, 14, SV(sv_bott(0)), o, cb, tc, st))) return rc;
-    if ((rc = dgrad3(h, h->enc[4][0], o, B, 14, nullptr, g, 8 * f, tc, st))) return rc;
+    if ((rc = dgrad3(h, h->enc[4][1], g, B, 14, SV(sv_bott(0)), o, cb, rnd, st))) return rc;
+    if ((rc = dgrad3(h, h->enc[4][0], o, B, 14, nullptr, g, 8 * f, rnd, st))) return rc;
     // encoder levels 4..1: pool (+ skip gradient), conv2, conv1
     for (int lvl = 3; lvl >= 0; --lvl) {
         const int S = 224 >> lvl, c = f << lvl;
         {
             const long total = (long)B * (S / 2) * (S / 2) * (c / 4);
             SMK_TAG("maxpool_dgrad", 4.0 * B * ((double)S * S * c * 3 + (S / 2.0) * (S / 2.0) * c), 0.0, st);
-            SMK_LAUNCH(pool_bwd_kernel, dim3(grid_of(total)), dim3(256), 0, st, SV(sv_enc(lvl, 1)), g, gcat[lvl] + c, 2 * c, B, S, c, tc ? 1 : 0, o);
+            SMK_LAUNCH(pool_bwd_kernel, dim3(grid_of(total)), dim3(256), 0, st, SV(sv_enc(lvl, 1)), g, gcat[lvl] + c, 2 * c, B, S, c, rnd ? 1 : 0, o);
             SMK_CHECK_LAUNCH();
         }
-        if ((rc = dgrad3(h, h->enc[lvl][1], o, B, S, SV(sv_enc(lvl, 0)), g, c, tc, st))) return rc;
+        if ((rc = dgrad3(h, h->enc[lvl][1], o, B, S, SV(sv_enc(lvl, 0)), g, c, rnd, st))) return rc;
         const int n_in = lvl > 0 ? c / 2 : h->cin_p;
-        if ((rc = dgrad3(h, h->enc[lvl][0], g, B, S, nullptr, o, n_in, tc && lvl > 0, st))) return rc;
+        if ((rc = dgrad3(h, h->enc[lvl][0], g, B, S, nullptr, o, n_in, rnd && lvl > 0, st))) return rc;
         std::swap(g, o);
     }
     const long total = (long)B * h->cin * 224 * 224;

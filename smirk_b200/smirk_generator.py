@@ -8,6 +8,10 @@ With grad mode on and an input that requires grad, a frozen (``requires_grad_(Fa
 gradient to its input, as the reference trainer's emotion loss and photometric fitting need: the forward then keeps
 its activations (``smk_generator_forward_saved``) and the backward runs ``smk_generator_backward``.  Weight gradients
 are not implemented.
+
+``precision`` (part of the native handle's key, so it may change between calls): 0 = fp32 CUDA cores, 1 = TF32 tensor cores,
+3 = 3xTF32 tensor cores (each operand split into a TF32 head and tail, three products per term: fp32-equivalent forward and
+input gradient, the same launches as 1).  Precisions 1 and 3 need ``init_features % 32 == 0``.
 """
 import ctypes as C
 from collections import OrderedDict

@@ -1,6 +1,6 @@
 """Device time of the SmirkGenerator forward alone, the grad-mode forward (which also stores the activations the
-backward needs) and the input-gradient backward alone, frozen weights, at B = 32 and B = 256, precision 1 (TF32 wgmma)
-and precision 0 (fp32 CUDA cores) for reference.  CUDA-event mean over `--reps` iterations after warm-up; inputs resident
+backward needs) and the input-gradient backward alone, frozen weights, at B = 32 and B = 256, by default precision 1 (TF32 wgmma)
+and precision 0 (fp32 CUDA cores) for reference; `--precisions 3 1 0` adds the 3xTF32 tensor-core path.  CUDA-event mean over `--reps` iterations after warm-up; inputs resident
 on the device.  Prints the card name and power limit read in the same run, then the per-kernel breakdown of one grad-mode
 forward + backward from the library's event profiler (smk_profiler_*), with TFLOP/s per tag."""
 import argparse
