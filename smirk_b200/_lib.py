@@ -1,4 +1,4 @@
-"""ctypes binding of libsmirk_b200.so (the C ABI declared in include/smirk_b200.h).
+"""ctypes binding of libsmirk_b200.so (the C ABI declared in include/smirk_b200.h and include/smirk_b200_loss.h).
 
 There is deliberately no fallback: if the shared library is missing or a call fails, the product
 path raises.  Build with ``python -m smirk_b200.build`` (or ``__graft_entry__.build()``).
@@ -53,6 +53,10 @@ class SmkGeneratorDesc(C.Structure):
     _fields_ = [("in_channels", C.c_int), ("out_channels", C.c_int), ("init_features", C.c_int),
                 ("res_blocks", C.c_int), ("tensors", C.POINTER(c_f32p)), ("n_tensors", C.c_int),
                 ("precision", C.c_int)]
+
+
+class SmkVggLossDesc(C.Structure):
+    _fields_ = [("tensors", C.POINTER(c_f32p)), ("n_tensors", C.c_int), ("precision", C.c_int)]
 
 
 class SmkMaskingDesc(C.Structure):
@@ -151,7 +155,19 @@ BINDINGS = [
     ("smk_debug_train_stem_wgrad", _i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, STREAM]),
     ("smk_debug_train_head_backward", _i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, STREAM]),
 ]
-_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS if args[-1:] == [STREAM])
+# The binding table of include/smirk_b200_loss.h (the trainer's losses), in that header's order, by the same rules.
+LOSS_BINDINGS = [
+    ("smk_vgg_loss_create", _i, [C.POINTER(SmkVggLossDesc), _vpp]),
+    ("smk_vgg_loss_destroy", None, [_vp]),
+    ("smk_vgg_loss_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_vgg_loss_forward", _i, [_vp, _vp, _vp, _i, _vp, _vp, _sz, STREAM]),
+    ("smk_vgg_loss_saved_bytes", _sz, [_vp, _i, _i]),
+    ("smk_vgg_loss_forward_saved", _i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _sz, _vp, _sz, STREAM]),
+    ("smk_vgg_loss_saved_tensor", _i, [_vp, _i, _i, _i, C.POINTER(C.c_char_p), C.POINTER(_sz), C.POINTER(C.c_int)]),
+    ("smk_vgg_loss_backward_workspace_bytes", _sz, [_vp, _i, _i]),
+    ("smk_vgg_loss_backward", _i, [_vp, _i, _i, _vp, _sz, _vp, _vp, _vp, _vp, _sz, STREAM]),
+]
+_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS + LOSS_BINDINGS if args[-1:] == [STREAM])
 
 
 def lib():
@@ -163,7 +179,7 @@ def lib():
         raise RuntimeError("smirk_b200: %s not found — build it with `python -m smirk_b200.build` "
                            "(there is no CPU / PyTorch fallback)" % LIB_PATH)
     L = C.CDLL(LIB_PATH)
-    for name, restype, argtypes in BINDINGS:
+    for name, restype, argtypes in BINDINGS + LOSS_BINDINGS:
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, [_vp if a is STREAM else a for a in argtypes]
     if L.smk_version() != 100:

@@ -52,6 +52,7 @@ struct WinArgs {
     const float* head_w; const float* head_b; int head_c;
     const float* mask; int ld_mask;   // store 0: zero outputs whose mask[pixel, n] <= 0 (ReLU backward)
     float* out2; int ld_out2;         // the stored activations again, compact NHWC (store 3: the activations it does not store)
+    int out2_rows;                    // out2 takes the pixels m < out2_rows
 };
 
 // RES = true : the layer's whole weight matrix stays in shared memory, shared by both pipelines (<= 72 KB);
@@ -216,8 +217,9 @@ conv3_win_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
                                 xs[e] = x;
                                 a0 = fmaf(x, p0.z, a0); a1 = fmaf(x, p0.w, a1); a2 = fmaf(x, p1.x, a2); a3 = fmaf(x, p1.y, a3);
                             }
-                            if (EXTRA && a.out2)
-                                *reinterpret_cast<float4*>(a.out2 + ((size_t)(img * a.H + oh) * a.W + ow) * a.ld_out2 + 4 * j) = make_float4(xs[0], xs[1], xs[2], xs[3]);
+                            const size_t px = (size_t)(img * a.H + oh) * a.W + ow;
+                            if (EXTRA && a.out2 && px < (size_t)a.out2_rows)
+                                *reinterpret_cast<float4*>(a.out2 + px * a.ld_out2 + 4 * j) = make_float4(xs[0], xs[1], xs[2], xs[3]);
                         }
                         const int hw_px = a.H * a.W;
                         float* dst = a.out + (size_t)img * a.head_c * hw_px + (size_t)oh * a.W + ow;
@@ -250,7 +252,7 @@ conv3_win_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
                         }
                         if (a.round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
                         *reinterpret_cast<float4*>(a.out + pix * a.ld_out + nc) = o;
-                        if (EXTRA && a.out2) *reinterpret_cast<float4*>(a.out2 + pix * a.ld_out2 + nc) = o;
+                        if (EXTRA && a.out2 && pix < (size_t)a.out2_rows) *reinterpret_cast<float4*>(a.out2 + pix * a.ld_out2 + nc) = o;
                     }
                 }
                 __syncwarp();
@@ -303,6 +305,7 @@ int conv3_win(const Conv& p, cudaStream_t st) {
     a.scale = p.scale; a.bias = p.bias; a.relu = p.relu; a.round_out = p.round_out;
     a.out = p.out; a.ld_out = p.ld_out; a.store = p.store; a.head_w = p.head_w; a.head_b = p.head_b; a.head_c = p.head_c;
     a.mask = p.mask; a.ld_mask = p.ld_mask; a.out2 = p.out2; a.ld_out2 = p.ld_out2;
+    a.out2_rows = p.out2_rows > 0 ? p.out2_rows : p.B * p.H * p.W;
     {
         const double M = (double)p.B * p.H * p.W;
         const char* tag = p.tag ? p.tag : p.store == 3 ? "conv3x3_win_head_tc" : "conv3x3_win_tc";

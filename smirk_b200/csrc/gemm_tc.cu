@@ -62,6 +62,7 @@ struct TcArgs {
     const float* head_w; const float* head_b; int head_c;      // store 3: 1x1 head weights [N][head_c], bias [head_c], head_c <= 4
     const float* mask; int ld_mask;    // zero outputs whose mask[m, n] <= 0 (single problem, store 0)
     float* out2; int ld_out2;          // second store of the activations, compact at pixel m (single problem, store 0 / 2 / 3)
+    int out2_rows;                     // out2 takes the pixels m < out2_rows
 };
 
 struct TcMaps { CUtensorMap a[2], b[2], blo[2]; };       // per problem: activations, weights (TF32 heads), weight tails (3xTF32)
@@ -289,7 +290,7 @@ gemm_tc_kernel(const __grid_constant__ TcMaps mp, const TcArgs a) {
                             xs[e] = x;
                             a0 = fmaf(x, p0.z, a0); a1 = fmaf(x, p0.w, a1); a2 = fmaf(x, p1.x, a2); a3 = fmaf(x, p1.y, a3);
                         }
-                        if (EXTRA && a.out2) *reinterpret_cast<float4*>(a.out2 + (size_t)m * a.ld_out2 + 4 * j) = make_float4(xs[0], xs[1], xs[2], xs[3]);
+                        if (EXTRA && a.out2 && m < a.out2_rows) *reinterpret_cast<float4*>(a.out2 + (size_t)m * a.ld_out2 + 4 * j) = make_float4(xs[0], xs[1], xs[2], xs[3]);
                     }
                     const int hw_px = a.H * a.W, b = m / hw_px, rem = m - b * hw_px;
                     float* dst = g_out + (size_t)b * a.head_c * hw_px + rem;
@@ -328,7 +329,7 @@ gemm_tc_kernel(const __grid_constant__ TcMaps mp, const TcArgs a) {
                     }
                     if (a.round_out) { o.x = smk::round_tf32(o.x); o.y = smk::round_tf32(o.y); o.z = smk::round_tf32(o.z); o.w = smk::round_tf32(o.w); }
                     *reinterpret_cast<float4*>(g_out + (size_t)(opix[i] + pix_off) * a.ld_out + col) = o;
-                    if (EXTRA && a.out2) *reinterpret_cast<float4*>(a.out2 + mc * a.ld_out2 + nc) = o;
+                    if (EXTRA && a.out2 && mc < (size_t)a.out2_rows) *reinterpret_cast<float4*>(a.out2 + mc * a.ld_out2 + nc) = o;
                 }
             }
             __syncwarp();
@@ -491,7 +492,7 @@ int tc_conv(const Conv& p, cudaStream_t st, const Conv* p2) {
                 "tc_conv: the fused 1x1 head needs a 3x3 conv with N == 32 (one full column tile) and 1..4 head channels");
     SMK_REQUIRE((!p.mask || p.store == 0) && (!p.out2 || p.store != 1) && (!(p.mask || p.out2) || !p2),
                 "tc_conv: the mask needs store 0, the second store a non-shuffled store, both a single problem");
-    a.mask = p.mask; a.ld_mask = p.ld_mask; a.out2 = p.out2; a.ld_out2 = p.ld_out2;
+    a.mask = p.mask; a.ld_mask = p.ld_mask; a.out2 = p.out2; a.ld_out2 = p.ld_out2; a.out2_rows = p.out2_rows > 0 ? p.out2_rows : M;
     for (int g = 0; g < groups; ++g) {
         const Conv& q = g ? *p2 : p;
         a.scale[g] = q.scale; a.bias[g] = q.bias; a.res[g] = q.res; a.out[g] = q.out;

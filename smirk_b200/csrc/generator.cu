@@ -43,38 +43,18 @@ struct Conv3 { float* w; float* wt; float* wt_lo; float* scale; float* bias; flo
 // dw: [4*cout][cin] (fp32) or [cin][4*cout] (TF32), k = (dy*2+dx) * cout + co
 struct UpConv { float* w; float* wt; float* wt_lo; float* scale; float* bias; float* dw; float* dw_lo; int cin, cout; };         // w: [cin][4*cout];   wt: [4*cout][cin]
 
-// Tensor-core weight v at index i: the TF32 head, and with x3 the TF32 tail of what the head leaves (v = head + tail up to
-// 2^-22 |v|), the split encoder.cu packs for its 3xTF32 1x1 convs.
-void pack_tc(std::vector<float>& hi, std::vector<float>& lo, size_t i, float v, bool x3) {
-    hi[i] = smk::round_tf32_host(v);
-    if (x3) lo[i] = smk::round_tf32_host(v - hi[i]);
-}
+using smk::pack_tc;
 
 bool fold_conv3(TensorCursor& cur, int cin, int cin_p, int cout, bool tc, bool x3, smk::DeviceArena& arena, Conv3* out, cudaError_t* err) {
     const float* w = cur.next(); const float* g = cur.next(); const float* b = cur.next();
     const float* mu = cur.next(); const float* var = cur.next();
     if (!w || !g || !b || !mu || !var) return false;
-    const size_t K = (size_t)9 * cin_p, Kd = (size_t)9 * cout;
-    std::vector<float> W(K * cout, 0.f), D(Kd * cin_p, 0.f), S(cout), Bi(cout), Wlo, Dlo;
-    if (x3) { Wlo.assign(W.size(), 0.f); Dlo.assign(D.size(), 0.f); }
+    std::vector<float> S(cout), Bi(cout);
     smk::fold_bn(g, b, mu, var, cout, kBnEps, S.data(), Bi.data());
-    for (int o = 0; o < cout; ++o)
-        for (int c = 0; c < cin; ++c)
-            for (int k = 0; k < 9; ++k) {
-                float v = w[((size_t)o * cin + c) * 9 + k];
-                if (tc) pack_tc(W, Wlo, (size_t)o * K + (size_t)k * cin_p + c, v, x3);   // [N][K], TF32 heads (+ tails)
-                else W[((size_t)k * cin_p + c) * cout + o] = v;                // [K][N]
-                const float vd = v * S[o];                                     // split after the BN-scale multiply
-                const size_t kd = (size_t)(8 - k) * cout + o;                  // rotated tap
-                if (tc) pack_tc(D, Dlo, (size_t)c * Kd + kd, vd, x3);
-                else D[kd * cin_p + c] = vd;
-            }
     out->cin = cin; out->cin_p = cin_p; out->cout = cout;
-    out->w = out->wt = out->wt_lo = out->dw_lo = nullptr;
-    cudaError_t e = arena.upload(W, tc ? &out->wt : &out->w);
-    if (e == cudaSuccess && x3) e = arena.upload(Wlo, &out->wt_lo);
-    if (e == cudaSuccess) e = arena.upload(D, &out->dw);
-    if (e == cudaSuccess && x3) e = arena.upload(Dlo, &out->dw_lo);
+    smk::Conv3Weights pk;                          // the dgrad weights carry the BN scale
+    cudaError_t e = smk::pack_conv3(w, S.data(), cin, cin_p, cout, tc, x3, arena, &pk);
+    out->w = pk.w; out->wt = pk.wt; out->wt_lo = pk.wt_lo; out->dw = pk.dw; out->dw_lo = pk.dw_lo;
     if (e == cudaSuccess) e = arena.upload(S, &out->scale);
     if (e == cudaSuccess) e = arena.upload(Bi, &out->bias);
     *err = e;

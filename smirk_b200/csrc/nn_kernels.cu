@@ -126,7 +126,7 @@ conv_gemm_kernel(Conv p, int M) {
             if (p.relu) v = fmaxf(v, 0.f);
             if (p.mask && !(p.mask[(size_t)m * p.ld_mask + n] > 0.f)) v = 0.f;
             if (p.round_out) v = round_tf32(v);
-            if (p.out2) p.out2[(size_t)m * p.ld_out2 + n] = v;
+            if (p.out2 && (p.out2_rows <= 0 || m < p.out2_rows)) p.out2[(size_t)m * p.ld_out2 + n] = v;
             if (p.store == 1) {
                 int cout = p.N >> 2, q = n / cout, co = n - q * cout;
                 int b = m / HW, r = m - b * HW, h = r / p.W, w = r - h * p.W;

@@ -7,16 +7,17 @@
 (``smirk_encoder.set_train_mode_default(True)``): the trainer's ``.train()`` encoder then runs with batch statistics
 and gets its weight gradients.  Without it a train-mode encoder raises, as before.
 
-``install()`` registers our modules under the four names the reference imports its hot-path classes
-from (``demo.py:5-7,62``, ``src/smirk_trainer.py:3-6``):
+``install()`` registers our modules under the five names the reference imports its hot-path classes
+from (``demo.py:5-7,62``, ``src/smirk_trainer.py:3-6``, ``src/base_trainer.py``):
 
     src.smirk_encoder      -> smirk_b200.smirk_encoder    (SmirkEncoder, create_backbone, ...)
     src.FLAME.FLAME        -> smirk_b200.flame            (FLAME)
     src.renderer.renderer  -> smirk_b200.renderer         (Renderer)
     src.smirk_generator    -> smirk_b200.smirk_generator  (SmirkGenerator, ResnetBlock)
+    src.losses.VGGPerceptualLoss -> smirk_b200.vgg_loss   (VGGPerceptualLoss)
 
-Everything else under ``src`` (``src.FLAME.lbs``, ``src.renderer.util``, ``src.utils.*``, losses, trainers)
-still resolves to the reference's files: the real ``src`` package is imported first and only these four
+Everything else under ``src`` (``src.FLAME.lbs``, ``src.renderer.util``, ``src.utils.*``, the other losses,
+trainers) still resolves to the reference's files: the real ``src`` package is imported first and only these five
 submodules are replaced in ``sys.modules`` (and as attributes of their parent packages).
 """
 import importlib
@@ -30,6 +31,7 @@ _MAP = {
     "src.FLAME.FLAME": "smirk_b200.flame",
     "src.renderer.renderer": "smirk_b200.renderer",
     "src.smirk_generator": "smirk_b200.smirk_generator",
+    "src.losses.VGGPerceptualLoss": "smirk_b200.vgg_loss",
 }
 
 
@@ -48,12 +50,13 @@ def _ensure_package(name, path_hint):
 
 
 def install(reference_root=None):
-    """Alias the four hot-path modules.  ``reference_root`` (default: cwd) is put on sys.path so the
+    """Alias the five hot-path modules.  ``reference_root`` (default: cwd) is put on sys.path so the
     rest of the reference package keeps importing normally."""
     root = os.path.abspath(reference_root or os.getcwd())
     if root not in sys.path:
         sys.path.insert(0, root)
-    for parent, sub in (("src", "src"), ("src.FLAME", "src/FLAME"), ("src.renderer", "src/renderer")):
+    for parent, sub in (("src", "src"), ("src.FLAME", "src/FLAME"), ("src.renderer", "src/renderer"),
+                        ("src.losses", "src/losses")):
         pkg = _ensure_package(parent, os.path.join(root, sub))
         if "." in parent:
             setattr(sys.modules[parent.rsplit(".", 1)[0]], parent.rsplit(".", 1)[1], pkg)
