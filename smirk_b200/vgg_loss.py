@@ -122,10 +122,15 @@ class VGGPerceptualLoss(_lib.NativeModule, nn.Module):
         The forward is deterministic and batch-independent, so these are the tensors an autograd context holds."""
         self._check_inputs(x, y)
         h, _, saved = self._forward_saved(x, y, 3)
+        return self._saved_views(h, saved, x.shape[0], 3)
+
+    @staticmethod
+    def _saved_views(h, saved, B, need):
+        """{name: [B',C,H,W] view of ``saved``} for the buffer of a grad-mode forward with ``need``, B' = B per saved half."""
         fn = getattr(_lib.lib(), "smk_vgg_loss_saved_tensor")
         name, off, dims = C.c_char_p(), C.c_size_t(), (C.c_int * 4)()
-        out, i, B = {}, 0, x.shape[0]
-        while fn(h, B, 3, i, C.byref(name), C.byref(off), dims) == 0:         # non-zero past the last tensor
+        out, i = {}, 0
+        while fn(h, B, need, i, C.byref(name), C.byref(off), dims) == 0:      # non-zero past the last tensor
             b, hh, ww, c = dims
             n, key = b * hh * ww * c, name.value.decode()
             if key.startswith("sign"):

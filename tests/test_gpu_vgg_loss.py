@@ -89,9 +89,10 @@ def test_loss_vs_restatement(native_lib, precision, B):
 
 @pytest.mark.parametrize("precision", [0, 1, 3])
 @pytest.mark.parametrize("need", [1, 2, 3])
-def test_input_grads_vs_replay_oracle(native_lib, precision, need):
+@pytest.mark.parametrize("B", [1, 2, 3])
+def test_input_grads_vs_replay_oracle(native_lib, precision, need, B):
     m = vgg(precision)
-    x, y = inputs(2, 600 + need)
+    x, y = inputs(B, 600 + need)
     loss, gx, gy = device_loss_and_grads(m, x, y, need)
     with torch.no_grad():
         assert torch.equal(loss, m(x.to(DEV), y.to(DEV)))            # the grad-mode forward's loss is the forward's
@@ -101,7 +102,7 @@ def test_input_grads_vs_replay_oracle(native_lib, precision, need):
         if want:
             assert torch.isfinite(got).all()
             err = rel_close(got, ref, TOL[precision])
-            print("precision %d need %d: max-abs err / max-abs %.2e" % (precision, need, err / float(ref.abs().max())))
+            print("precision %d need %d B %d: max-abs err / max-abs %.2e" % (precision, need, B, err / float(ref.abs().max())))
         else:
             assert got is None
 
@@ -136,6 +137,8 @@ def test_x_is_y_gives_exact_zeros(native_lib):
 
 
 def test_deterministic_and_batch_independent(native_lib):
+    """Also the gradients: at B = 32 each tap's scale g / numel is exactly 2^-5 of B = 1's, and fp32 and TF32 rounding
+    commute with a power of two, so 32 times an image's B = 32 gradient is its B = 1 gradient bit for bit."""
     for precision in (0, 1, 3):
         m = vgg(precision)
         x, y = inputs(32, 710)
@@ -144,6 +147,8 @@ def test_deterministic_and_batch_independent(native_lib):
         assert all(torch.equal(p, q) for p, q in zip(a, b))
         full = m.saved_activations(x.to(DEV), y.to(DEV))
         for i in (0, 17):
+            _, gx, gy = device_loss_and_grads(m, x[i:i + 1], y[i:i + 1], 3)
+            assert torch.equal(a[1][i] * 32, gx[0]) and torch.equal(a[2][i] * 32, gy[0]), (precision, i)
             one = m.saved_activations(x[i:i + 1].to(DEV), y[i:i + 1].to(DEV))
             for k, v in one.items():
                 if k.startswith("sign"):

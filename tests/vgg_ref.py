@@ -72,16 +72,57 @@ def replay_activations(sd, v, saved_half):
     return out
 
 
-def vgg_loss_replay_ref(sd, x, y, saved):
-    """saved: {"relu*": [2B,C,H,W] (x's images, then y's), "sign*": [B,C,H,W]} as VGGPerceptualLoss.saved_activations."""
+def vgg_loss_replay_ref(sd, x, y, saved, record=None):
+    """saved: {"relu*": [2B,C,H,W] (x's images, then y's), "sign*": [B,C,H,W]} as VGGPerceptualLoss.saved_activations.
+    record (optional list): receives the tensors of the graph a gradient passes through, x's normalised input and ten
+    post-ReLU outputs, then y's."""
     B = x.shape[0]
-    ax = replay_activations(sd, normalise(sd, x), {k: saved[k][:B] for k in NAMES})
-    ay = replay_activations(sd, normalise(sd, y), {k: saved[k][B:] for k in NAMES})
+    nx, ny = normalise(sd, x), normalise(sd, y)
+    ax = replay_activations(sd, nx, {k: saved[k][:B] for k in NAMES})
+    ay = replay_activations(sd, ny, {k: saved[k][B:] for k in NAMES})
+    if record is not None:
+        record += [nx] + ax + [ny] + ay
     loss = 0.0
     for t, l in enumerate(TAP_CONVS):
         s = saved[SIGNS[t]].to(ax[l].dtype)
         loss = loss + (s * (ax[l] - ay[l])).sum() / ax[l].numel()
     return loss
+
+
+CHANNELS = [(3, 64), (64, 64), (64, 128), (128, 128), (128, 256), (256, 256), (256, 256), (256, 512), (512, 512), (512, 512)]
+
+
+def integer_state_dict(seed):
+    """A VGGPerceptualLoss state_dict on which every quantity of the forward and the input gradient is a small multiple
+    of 0.5 (tests/test_vgg_loss_layers_host.py checks it): output channel co of each conv has weight +1 on input channel
+    co mod cin at a random tap and -1 at a random other (channel, tap), all other weights 0; biases in {0, 1}; mean and
+    std distinct per channel (a channel mix-up in the normalisation shows) and such that the normalised input of
+    integer_inputs is a multiple of 0.5 in [-3, 3]."""
+    g = torch.Generator().manual_seed(seed)
+    sd = {"mean": torch.tensor([0.5, 0.25, 0.75]).view(1, 3, 1, 1), "std": torch.tensor([0.5, 0.25, 0.25]).view(1, 3, 1, 1)}
+    for k, (cin, cout) in zip(CONVS, CHANNELS):
+        w = torch.zeros(cout, cin * 9)
+        co = torch.arange(cout)
+        plus = (co % cin) * 9 + torch.randint(0, 9, (cout,), generator=g)
+        minus = (plus + torch.randint(1, cin * 9, (cout,), generator=g)) % (cin * 9)       # any other (channel, tap)
+        w[co, plus], w[co, minus] = 1.0, -1.0
+        sd[k + ".weight"] = w.view(cout, cin, 3, 3)
+        sd[k + ".bias"] = torch.randint(0, 2, (cout,), generator=g).float()
+    return sd
+
+
+def integer_inputs(B, seed):
+    """x, y [B,3,224,224] in {-1, -0.5, 0, 0.5, 1}; y is x with 30 % of its entries drawn again."""
+    g = torch.Generator().manual_seed(seed)
+    draw = lambda: torch.randint(-2, 3, (B, 3, 224, 224), generator=g).float() * 0.5
+    x = draw()
+    y = torch.where(torch.rand(B, 3, 224, 224, generator=g) < 0.3, draw(), x)
+    return x, y
+
+
+def integer_upstream(B):
+    """The loss's upstream gradient B * 224^2 * 64: tap t's L1 gradient g / numel_t is then exactly 2^t."""
+    return float(B * 224 * 224 * 64)
 
 
 def oracle_saved(sd, x, y):
