@@ -1,9 +1,17 @@
-// One descriptor for the GEMM-shaped convolutions of the encoder and the generator, and the one place that picks
-// their kernel: the fp32 CUDA-core `conv_gemm` (nn_kernels.cu) or the TF32 wgmma `tc_conv` (gemm_tc.cu).
+// One descriptor for the GEMM-shaped convolutions of the encoder, the generator and the VGG loss, the one place that picks
+// their kernel: the fp32 CUDA-core `conv_gemm` (nn_kernels.cu) or the TF32 wgmma `tc_conv` (gemm_tc.cu), and the one
+// packer of their weights.
 #pragma once
 #include "common.cuh"
 
 namespace smk {
+
+// The weight operand W(k, n) of a problem, in the layout of the kernel that reads it: exactly one of w / wt is set.
+//   w      fp32 [K][N], n fastest (conv_gemm)
+//   wt     TF32 [N][K], k fastest (tc_conv): the weights rounded to TF32, or with wt_lo their TF32 heads
+//   wt_lo  optional: the TF32 tails, v - head rounded to TF32 (v = head + tail up to 2^-22 |v|) -> 3xTF32 arithmetic
+// pack_gemm below packs one from the logical [N][K] matrix.
+struct GemmW { const float* w; const float* wt; const float* wt_lo; };
 
 // One convolution / GEMM problem:  out[m, n] = epi( sum_k A(m, k) * W(k, n) )
 //   m indexes the output pixels (b, h, w) of an NHWC tensor, n the output channels.  Stride 1: H x W are the output dims.
@@ -15,9 +23,7 @@ struct Conv {
     const float* in; int ld_in;          // NHWC input, pixel stride ld_in (>= Cin; lets us read a channel slice)
     int B, H, W, Cin;
     int N, K, mode;
-    const float* w;                      // fp32 weights [K][N], n fastest (conv_gemm)
-    const float* wt;                     // TF32 weights [N][K], k fastest (tc_conv)
-    const float* wt_lo;                  // optional: TF32 tails of the weights (wt holds the heads) -> 3xTF32 arithmetic
+    GemmW wgt;                           // the weights W(k, n)
     const float* scale; const float* bias;   // folded BN (or 1 / conv bias), per n
     int relu;
     const float* res; int ld_res; int res_pad;   // optional residual, added before the ReLU; res_pad: read it from the
@@ -34,6 +40,9 @@ struct Conv {
     const char* tag;                     // profiler tag (null: derived from the problem)
 };
 
+// conv_gemm_kernel takes Conv by value: its parameter layout is pinned.
+static_assert(offsetof(Conv, wgt) == 40 && offsetof(Conv, scale) == 64 && sizeof(Conv) == 184, "smk::Conv layout moved");
+
 // fp32 CUDA cores: modes 0-2, stores 0 and 1; no TF32 weights, padded residual or paired problem.
 int conv_gemm(const Conv& p, cudaStream_t st);
 // TF32 tensor cores.  p2 (optional): a second problem of identical shape sharing the launch (tiles of both in one grid).
@@ -41,45 +50,53 @@ int tc_conv(const Conv& p, cudaStream_t st, const Conv* p2 = nullptr);
 
 // TF32 weights (wt) run tc_conv, fp32 weights (w) conv_gemm.
 inline int conv(const Conv& p, cudaStream_t st, const Conv* p2 = nullptr) {
-    if (p.wt) return tc_conv(p, st, p2);
+    if (p.wgt.wt) return tc_conv(p, st, p2);
     SMK_REQUIRE(!p2, "conv: paired problems need TF32 weights");
     return conv_gemm(p, st);
 }
 
-// Tensor-core weight v at index i: the TF32 head, and with x3 the TF32 tail of what the head leaves (v = head + tail up to
-// 2^-22 |v|), the split encoder.cu packs for its 3xTF32 1x1 convs.
-inline void pack_tc(std::vector<float>& hi, std::vector<float>& lo, size_t i, float v, bool x3) {
-    hi[i] = round_tf32_host(v);
-    if (x3) lo[i] = round_tf32_host(v - hi[i]);
+// Packs the logical weight matrix W[n][k] = v(n, k), n < N, k < K, as smk::conv's operand: fp32 [K][N] (tc false), or
+// TF32 [N][K] (tc), as heads plus tails when x3.  Where a matrix comes from a reordered or scaled tensor, v does that
+// before the split.
+template <typename V>
+cudaError_t pack_gemm(DeviceArena& arena, int N, int K, bool tc, bool x3, V&& v, GemmW* out) {
+    std::vector<float> hi((size_t)N * K), lo(tc && x3 ? hi.size() : 0);
+    for (int n = 0; n < N; ++n)
+        for (int k = 0; k < K; ++k) {
+            const float x = v(n, k);
+            if (!tc) { hi[(size_t)k * N + n] = x; continue; }
+            const size_t i = (size_t)n * K + k;
+            hi[i] = round_tf32_host(x);
+            if (!lo.empty()) lo[i] = round_tf32_host(x - hi[i]);
+        }
+    float *d = nullptr, *d_lo = nullptr;
+    cudaError_t e = arena.upload(hi, &d);
+    if (e == cudaSuccess && !lo.empty()) e = arena.upload(lo, &d_lo);
+    *out = tc ? GemmW{nullptr, d, d_lo} : GemmW{d, nullptr, nullptr};
+    return e;
+}
+// The same from a dense [N][K] matrix.
+inline cudaError_t pack_gemm(DeviceArena& arena, int N, int K, bool tc, bool x3, const float* nk, GemmW* out) {
+    return pack_gemm(arena, N, K, tc, x3, [nk, K](int n, int k) { return nk[(size_t)n * K + k]; }, out);
 }
 
 // One 3x3 convolution's weights (PyTorch [cout][cin][3][3]) packed for smk::conv, forward and input gradient:
-//   forward  w [9*cin_p][cout] (fp32) or wt [cout][9*cin_p] (TF32 heads, + wt_lo tails with x3), k = tap * cin_p + ci;
-//   dgrad    W'[ci][8 - tap][co] = dscale[co] * W[co][ci][tap]: dw [9*cout][cin_p] (fp32) or [cin_p][9*cout] (TF32, + dw_lo),
-//            the forward's GEMM kernels run it as a 3x3 conv of the output gradient.
-// Input channels cin..cin_p-1 are zero.  dscale (null: 1) is multiplied in before the TF32 split.  Unused pointers are null.
-struct Conv3Weights { float* w; float* wt; float* wt_lo; float* dw; float* dw_lo; };
+//   forward  N = cout, K = 9*cin_p:  W(k = tap * cin_p + ci, co) = W[co][ci][tap];
+//   dgrad    N = cin_p, K = 9*cout:  W'(k = (8 - tap) * cout + co, ci) = dscale[co] * W[co][ci][tap], the rotated taps: the
+//            forward's GEMM kernels run it as a 3x3 conv of the output gradient.
+// Input channels cin..cin_p-1 are zero.  dscale (null: 1) is multiplied in before the TF32 split.
 inline cudaError_t pack_conv3(const float* w, const float* dscale, int cin, int cin_p, int cout, bool tc, bool x3,
-                              DeviceArena& arena, Conv3Weights* out) {
-    const size_t K = (size_t)9 * cin_p, Kd = (size_t)9 * cout;
-    std::vector<float> W(K * cout, 0.f), D(Kd * cin_p, 0.f), Wlo, Dlo;
-    if (x3) { Wlo.assign(W.size(), 0.f); Dlo.assign(D.size(), 0.f); }
-    for (int o = 0; o < cout; ++o)
-        for (int c = 0; c < cin; ++c)
-            for (int k = 0; k < 9; ++k) {
-                const float v = w[((size_t)o * cin + c) * 9 + k];
-                if (tc) pack_tc(W, Wlo, (size_t)o * K + (size_t)k * cin_p + c, v, x3);   // [N][K], TF32 heads (+ tails)
-                else W[((size_t)k * cin_p + c) * cout + o] = v;                // [K][N]
-                const float vd = dscale ? v * dscale[o] : v;                   // split after the scale multiply
-                const size_t kd = (size_t)(8 - k) * cout + o;                  // rotated tap
-                if (tc) pack_tc(D, Dlo, (size_t)c * Kd + kd, vd, x3);
-                else D[kd * cin_p + c] = vd;
-            }
-    *out = Conv3Weights{};
-    cudaError_t e = arena.upload(W, tc ? &out->wt : &out->w);
-    if (e == cudaSuccess && x3) e = arena.upload(Wlo, &out->wt_lo);
-    if (e == cudaSuccess) e = arena.upload(D, &out->dw);
-    if (e == cudaSuccess && x3) e = arena.upload(Dlo, &out->dw_lo);
+                              DeviceArena& arena, GemmW* fwd, GemmW* dgrad) {
+    cudaError_t e = pack_gemm(arena, cout, 9 * cin_p, tc, x3, [&](int o, int k) {
+        const int tap = k / cin_p, c = k % cin_p;
+        return c < cin ? w[((size_t)o * cin + c) * 9 + tap] : 0.f;
+    }, fwd);
+    if (e == cudaSuccess) e = pack_gemm(arena, cin_p, 9 * cout, tc, x3, [&](int c, int k) {
+        const int tap = 8 - k / cout, o = k % cout;
+        if (c >= cin) return 0.f;
+        const float v = w[((size_t)o * cin + c) * 9 + tap];
+        return dscale ? v * dscale[o] : v;
+    }, dgrad);
     return e;
 }
 

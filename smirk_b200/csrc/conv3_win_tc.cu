@@ -285,7 +285,7 @@ int launch(const CUtensorMap& tmX, const CUtensorMap& tmW, const WinArgs& a, cud
 }  // namespace
 
 bool conv3_win_supported(const Conv& p) {
-    if (p.mode != 1 || p.res || p.wt_lo || (p.store != 0 && p.store != 3) || (p.store == 3 && (p.N != 32 || p.mask))) return false;
+    if (p.mode != 1 || p.res || p.wgt.wt_lo || (p.store != 0 && p.store != 3) || (p.store == 3 && (p.N != 32 || p.mask))) return false;
     if (p.Cin % 32 != 0 || p.K != 9 * p.Cin || (p.N != 32 && p.N != 64)) return false;
     return p.W >= 56;                                             // low-resolution layers are MMA-bound: gemm_tc's wide tiles win there
 }
@@ -298,7 +298,7 @@ int conv3_win(const Conv& p, cudaStream_t st) {
     const int BN = p.N <= 32 ? 32 : 64;
     CUtensorMap tmX, tmW;
     if (int rc = encode_nhwc(&tmX, p.in, p.B, p.H, p.W, p.Cin, p.ld_in, PW, TH + 2, "conv3_win(x)")) return rc;
-    if (int rc = encode_2d(&tmW, p.wt, (uint64_t)p.N, (uint64_t)p.K, (uint64_t)p.K, (uint32_t)BN, "conv3_win(w)")) return rc;
+    if (int rc = encode_2d(&tmW, p.wgt.wt, (uint64_t)p.N, (uint64_t)p.K, (uint64_t)p.K, (uint32_t)BN, "conv3_win(w)")) return rc;
     WinArgs a{};
     a.H = p.H; a.W = p.W; a.N = p.N; a.nchunks = p.Cin / 32;
     a.tiles_x = cdiv(p.W, TW); a.tiles_y = cdiv(p.H, TH); a.n_tiles = a.tiles_x * a.tiles_y * p.B;
@@ -323,7 +323,7 @@ int conv3_win(const Conv& p, cudaStream_t st) {
 extern "C" int smk_debug_conv3_win(const float* in, int ld_in, int B, int H, int W, int Cin, const float* wt, const float* scale,
                                    const float* bias, int N, int relu, float* out, int ld_out, void* stream) {
     smk::Conv p{};
-    p.in = in; p.ld_in = ld_in; p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.wt = wt; p.scale = scale; p.bias = bias; p.N = N; p.K = 9 * Cin;
+    p.in = in; p.ld_in = ld_in; p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.wgt = smk::GemmW{nullptr, wt, nullptr}; p.scale = scale; p.bias = bias; p.N = N; p.K = 9 * Cin;
     p.mode = 1; p.relu = relu; p.out = out; p.ld_out = ld_out; p.store = 0;
     return smk::conv3_win(p, (cudaStream_t)stream);
 }

@@ -28,63 +28,38 @@ using smk::same_pad_begin;
 
 constexpr float kBnEps = 1e-3f;
 
-// Consumes (conv weight, bn gamma, beta, mean, var) from the tensor list.
-// kind: 0 = 1x1 [Cout,Cin,1,1] -> W[Cin][Cout]; 1 = depthwise [C,1,3,3] -> W[9][C]; 2 = stem [16,3,3,3] -> W[27][16]
-// dg (optional): the dgrad weights with the folded BN scale s multiplied in.  1x1: (diag(s) W)^T as a GEMM with K = cout,
-// N = cin — fp32 [K][N], or TF32 [N][K] (+ tails when x3); depthwise: flipped taps, Wd[8 - k][c] = s[c] W[c][k];
-// stem: Wd[k][o] = s[o] W[o][k] (the forward layout).
-bool fold_conv(TensorCursor& cur, int kind, int cin, int cout, bool tc, smk::DeviceArena& arena, ConvW* out, cudaError_t* err, bool x3 = false,
-               ConvW* dg = nullptr) {
+// Consumes (conv weight, bn gamma, beta, mean, var) from the tensor list: the folded BN scale s and bias, the forward
+// weights, and the dgrad weights, which carry s.
+//   kind 0 = 1x1 [Cout,Cin,1,1]: smk::pack_gemm operands, the forward's N = cout, K = cin, the dgrad's (diag(s) W)^T,
+//            N = cin, K = cout.  f32 (optional): an fp32 copy of the forward weights as well.
+//   kind 1 = depthwise [C,1,3,3] -> W[9][C]; dgrad: flipped taps, Wd[8 - k][c] = s[c] W[c][k]
+//   kind 2 = stem [16,3,3,3] -> W[27][16]; dgrad: Wd[k][o] = s[o] W[o][k] (the forward layout)
+bool fold_conv(TensorCursor& cur, int kind, int cin, int cout, bool tc, bool x3, smk::DeviceArena& arena, ConvW* out, cudaError_t* err,
+               smk::GemmW* f32 = nullptr) {
     const float* w = cur.next(); const float* g = cur.next(); const float* b = cur.next();
     const float* mu = cur.next(); const float* var = cur.next();
     if (!w || !g || !b || !mu || !var) return false;
-    std::vector<float> W, Wlo, S(cout), Bi(cout), D, Dlo;
-    if (kind == 0 && tc) {
-        W.resize((size_t)cin * cout);                        // torch layout [Cout][Cin] is already [N][K]
-        for (size_t i = 0; i < W.size(); ++i) W[i] = smk::round_tf32_host(w[i]);
-        if (x3) {                                            // w = head + tail exactly; the tail is itself a TF32 number up to 2^-22 |w|
-            Wlo.resize(W.size());
-            for (size_t i = 0; i < W.size(); ++i) Wlo[i] = smk::round_tf32_host(w[i] - W[i]);
-        }
-    } else if (kind == 0) {
-        W.resize((size_t)cin * cout);
-        for (int o = 0; o < cout; ++o) for (int c = 0; c < cin; ++c) W[(size_t)c * cout + o] = w[(size_t)o * cin + c];
-    } else if (kind == 1) {
-        W.resize((size_t)9 * cout);
-        for (int c = 0; c < cout; ++c) for (int k = 0; k < 9; ++k) W[(size_t)k * cout + c] = w[(size_t)c * 9 + k];
-    } else {
-        W.resize((size_t)27 * cout);
-        for (int o = 0; o < cout; ++o) for (int k = 0; k < 27; ++k) W[(size_t)k * cout + o] = w[(size_t)o * 27 + k];
-    }
+    std::vector<float> S(cout), Bi(cout);
     smk::fold_bn(g, b, mu, var, cout, kBnEps, S.data(), Bi.data());
     out->cin = cin; out->cout = cout;
-    cudaError_t e = arena.upload(W, (kind == 0 && tc) ? &out->wt : &out->w);
-    if (e == cudaSuccess && !Wlo.empty()) e = arena.upload(Wlo, &out->wt_lo);
-    if (e == cudaSuccess) e = arena.upload(S, &out->scale);
+    cudaError_t e = arena.upload(S, &out->scale);
     if (e == cudaSuccess) e = arena.upload(Bi, &out->bias);
-    if (e == cudaSuccess && dg) {
-        const bool dtc = kind == 0 && tc;
-        if (kind == 0) {
-            D.resize((size_t)cin * cout);
-            if (dtc && x3) Dlo.resize(D.size());
-            for (int o = 0; o < cout; ++o)
-                for (int c = 0; c < cin; ++c) {
-                    const float v = S[o] * w[(size_t)o * cin + c];
-                    if (!dtc) { D[(size_t)o * cin + c] = v; continue; }
-                    const size_t i = (size_t)c * cout + o;
-                    D[i] = smk::round_tf32_host(v);
-                    if (x3) Dlo[i] = smk::round_tf32_host(v - D[i]);
-                }
-        } else if (kind == 1) {
-            D.resize((size_t)9 * cout);
-            for (int c = 0; c < cout; ++c) for (int k = 0; k < 9; ++k) D[(size_t)(8 - k) * cout + c] = S[c] * w[(size_t)c * 9 + k];
-        } else {
-            D.resize((size_t)27 * cout);
-            for (int o = 0; o < cout; ++o) for (int k = 0; k < 27; ++k) D[(size_t)k * cout + o] = S[o] * w[(size_t)o * 27 + k];
-        }
-        dg->cin = cout; dg->cout = cin;                     // the dgrad maps the conv's output channels to its input channels
-        e = arena.upload(D, dtc ? &dg->wt : &dg->w);
-        if (e == cudaSuccess && !Dlo.empty()) e = arena.upload(Dlo, &dg->wt_lo);
+    if (kind == 0) {                                          // torch's [Cout][Cin] is the forward's [N][K]
+        if (e == cudaSuccess) e = smk::pack_gemm(arena, cout, cin, tc, x3, w, &out->fwd);
+        if (e == cudaSuccess) e = smk::pack_gemm(arena, cin, cout, tc, x3, [&](int c, int o) { return S[o] * w[(size_t)o * cin + c]; }, &out->dgrad);
+        if (e == cudaSuccess && f32) e = smk::pack_gemm(arena, cout, cin, false, false, w, f32);
+    } else {
+        const int K = kind == 1 ? 9 : 27;
+        std::vector<float> W((size_t)K * cout), D(W.size());
+        for (int o = 0; o < cout; ++o)
+            for (int k = 0; k < K; ++k) {
+                W[(size_t)k * cout + o] = w[(size_t)o * K + k];
+                D[(size_t)(kind == 1 ? 8 - k : k) * cout + o] = S[o] * w[(size_t)o * K + k];
+            }
+        float *fw = nullptr, *dw = nullptr;
+        if (e == cudaSuccess) e = arena.upload(W, &fw);
+        if (e == cudaSuccess) e = arena.upload(D, &dw);
+        out->fwd = smk::GemmW{fw, nullptr, nullptr}; out->dgrad = smk::GemmW{dw, nullptr, nullptr};
     }
     *err = e;
     return e == cudaSuccess;
@@ -111,22 +86,21 @@ extern "C" int smk_encoder_create(const SmkEncoderDesc* desc, SmkEncoder** out) 
         h->present[i] = true;
         build_backbone(h, i);
         TensorCursor cur{desc->tensors[i], desc->n_tensors[i]};
-        bool ok = fold_conv(cur, 2, 3, 16, false, h->arena, &bb.stem, &e, false, &bb.stem_d);
+        bool ok = fold_conv(cur, 2, 3, 16, false, false, h->arena, &bb.stem, &e);
         bb.sv_stem = add(std::string(kEncName[i]) + ".encoder.bn1", 112, 16);
         for (Block& b : bb.blocks) {
             if (!ok) break;
             if (b.kind == DS) {
-                ok = fold_conv(cur, 1, b.cin, b.cin, false, h->arena, &b.dw, &e, false, &b.dw_d);
-                if (ok && tc) { TensorCursor again = cur; ok = fold_conv(again, 0, b.cin, b.cout, false, h->arena, &b.pw_f32, &e); }
-                ok = ok && fold_conv(cur, 0, b.cin, b.cout, tc, h->arena, &b.pw, &e, x3, &b.pw_d);
+                ok = fold_conv(cur, 1, b.cin, b.cin, false, false, h->arena, &b.dw, &e) &&
+                     fold_conv(cur, 0, b.cin, b.cout, tc, x3, h->arena, &b.pw, &e, tc ? &b.pw_f32 : nullptr);
                 b.sv_a = add(b.path + ".bn1", b.hout, b.cin);
             } else if (b.kind == IR) {
-                ok = fold_conv(cur, 0, b.cin, b.mid, tc, h->arena, &b.pw, &e, x3, &b.pw_d) &&
-                     fold_conv(cur, 1, b.mid, b.mid, false, h->arena, &b.dw, &e, false, &b.dw_d) &&
-                     fold_conv(cur, 0, b.mid, b.cout, tc, h->arena, &b.pwl, &e, x3, &b.pwl_d);
+                ok = fold_conv(cur, 0, b.cin, b.mid, tc, x3, h->arena, &b.pw, &e) &&
+                     fold_conv(cur, 1, b.mid, b.mid, false, false, h->arena, &b.dw, &e) &&
+                     fold_conv(cur, 0, b.mid, b.cout, tc, x3, h->arena, &b.pwl, &e);
                 b.sv_a = add(b.path + ".bn1", b.hin, b.mid); b.sv_b = add(b.path + ".bn2", b.hout, b.mid);
             } else {
-                ok = fold_conv(cur, 0, b.cin, b.cout, tc, h->arena, &b.pw, &e, x3, &b.pw_d);
+                ok = fold_conv(cur, 0, b.cin, b.cout, tc, x3, h->arena, &b.pw, &e);
                 b.sv_a = add(b.path + ".bn1", b.hout, b.cout);
             }
         }
@@ -162,10 +136,10 @@ static int pointwise(int n, const ConvW* const* c, float* const* in, int B, int 
     for (int k = 0; k < n; ++k) {
         q[k] = smk::Conv{};
         q[k].in = in[k]; q[k].ld_in = c[k]->cin; q[k].B = B; q[k].H = H; q[k].W = W; q[k].Cin = c[k]->cin;
-        q[k].w = c[k]->w; q[k].wt = c[k]->wt; q[k].wt_lo = c[k]->wt_lo; q[k].scale = c[k]->scale; q[k].bias = c[k]->bias;
+        q[k].wgt = c[k]->fwd; q[k].scale = c[k]->scale; q[k].bias = c[k]->bias;
         q[k].N = c[k]->cout; q[k].K = c[k]->cin; q[k].mode = 0; q[k].relu = relu ? 1 : 0;
         q[k].res = res ? res[k] : nullptr; q[k].ld_res = c[k]->cout; q[k].out = out[k]; q[k].ld_out = c[k]->cout;
-        q[k].round_out = c[k]->wt && !c[k]->wt_lo;      // 3xTF32 consumers split full fp32 activations themselves
+        q[k].round_out = c[k]->fwd.wt && !c[k]->fwd.wt_lo;      // 3xTF32 consumers split full fp32 activations themselves
     }
     return smk::conv(q[0], st, n == 2 ? &q[1] : nullptr);
 }
@@ -189,11 +163,11 @@ static int encoder_forward(const SmkEncoder* h, const float* img, int B, float* 
     const bool fuse_stem = h->fuse_xdw;                           // every backbone starts with a DS block
     if (!fuse_stem && n_present == 3) {   // all three stems in one pass over the image (it is the only tensor the backbones share)
         const float* sw[3]; const float* ss[3]; const float* sb[3]; float* so[3];
-        for (int i = 0; i < 3; ++i) { sw[i] = h->bb[i].stem.w; ss[i] = h->bb[i].stem.scale; sb[i] = h->bb[i].stem.bias; so[i] = stem_out[i]; }
+        for (int i = 0; i < 3; ++i) { sw[i] = h->bb[i].stem.fwd.w; ss[i] = h->bb[i].stem.scale; sb[i] = h->bb[i].stem.bias; so[i] = stem_out[i]; }
         if (int rc = smk::stem_conv3(img, B, 224, 224, sw, ss, sb, so, main_st)) return rc;
     } else if (!fuse_stem) {
         for (int i = 0; i < 3; ++i)
-            if (h->present[i]) { if (int rc = smk::stem_conv(img, B, 224, 224, h->bb[i].stem.w, h->bb[i].stem.scale, h->bb[i].stem.bias, stem_out[i], main_st)) return rc; }
+            if (h->present[i]) { if (int rc = smk::stem_conv(img, B, 224, 224, h->bb[i].stem.fwd.w, h->bb[i].stem.scale, h->bb[i].stem.bias, stem_out[i], main_st)) return rc; }
     }
     // the stems above run on main_st before the fork
     return for_each_unit(h, h->present, main_st, "smk_encoder_forward", [&](const Unit& unit) {
@@ -213,8 +187,8 @@ static int encoder_forward(const SmkEncoder* h, const float* img, int B, float* 
             smk::StemDsProblem sp[2];
             for (int k = 0; k < n; ++k) {
                 const Block& bk = bb[k]->blocks[0];
-                sp[k] = smk::StemDsProblem{bb[k]->stem.w, bb[k]->stem.scale, bb[k]->stem.bias, bk.dw.w, bk.dw.scale, bk.dw.bias,
-                                           bk.pw_f32.w, bk.pw_f32.scale, bk.pw_f32.bias, x[k], SV(bb[k]->sv_stem), SV(bk.sv_a)};
+                sp[k] = smk::StemDsProblem{bb[k]->stem.fwd.w, bb[k]->stem.scale, bb[k]->stem.bias, bk.dw.fwd.w, bk.dw.scale, bk.dw.bias,
+                                           bk.pw_f32.w, bk.pw.scale, bk.pw.bias, x[k], SV(bb[k]->sv_stem), SV(bk.sv_a)};
                 cur[k] = x[k];
             }
             rc = smk::stem_ds(img, B, 224, 224, sp, n, b0.stride, h->x3 ? 0 : 1, st);
@@ -237,19 +211,19 @@ static int encoder_forward(const SmkEncoder* h, const float* img, int B, float* 
             }
             if (b0.kind == DS) {
                 for (int k = 0; k < n && !rc; ++k)
-                    rc = smk::dwconv3x3(cur[k], B, res, res, b[k]->cin, b[k]->stride, b[k]->dw.w, b[k]->dw.scale, b[k]->dw.bias, d[k], st, rnd);
+                    rc = smk::dwconv3x3(cur[k], B, res, res, b[k]->cin, b[k]->stride, b[k]->dw.fwd.w, b[k]->dw.scale, b[k]->dw.bias, d[k], st, rnd);
                 if (!rc) rc = pointwise(n, pw, d, B, ro, ro, false, b0.skip ? cur : nullptr, out, st);
             } else if (b0.kind == IR) {
                 // The 7x7 layers (a 16x16 window holds 81 useful pixels, 49 outputs) run as 1x1 GEMM + depthwise kernels:
                 // most of a window would be halo; every other resolution runs fused.
                 constexpr int kXdwMinRes = 8;
-                if (h->fuse_xdw && b0.pw.wt && res >= kXdwMinRes) {
+                if (h->fuse_xdw && b0.pw.fwd.wt && res >= kXdwMinRes) {
                     // expand 1x1 + depthwise 3x3 in one kernel: the expanded tensor never leaves the SM
                     smk::XdwConv q[2];
                     for (int k = 0; k < n; ++k) {
                         q[k] = smk::XdwConv{};
-                        q[k].x = cur[k]; q[k].B = B; q[k].H = res; q[k].W = res; q[k].Cin = b[k]->cin; q[k].w1t = b[k]->pw.wt; q[k].w1t_lo = b[k]->pw.wt_lo;
-                        q[k].scale1 = b[k]->pw.scale; q[k].bias1 = b[k]->pw.bias; q[k].mid = b[k]->mid; q[k].wdw = b[k]->dw.w;
+                        q[k].x = cur[k]; q[k].B = B; q[k].H = res; q[k].W = res; q[k].Cin = b[k]->cin; q[k].w1t = b[k]->pw.fwd.wt; q[k].w1t_lo = b[k]->pw.fwd.wt_lo;
+                        q[k].scale1 = b[k]->pw.scale; q[k].bias1 = b[k]->pw.bias; q[k].mid = b[k]->mid; q[k].wdw = b[k]->dw.fwd.w;
                         q[k].scale2 = b[k]->dw.scale; q[k].bias2 = b[k]->dw.bias; q[k].stride = b[k]->stride; q[k].round_out = h->x3 ? 0 : 1; q[k].out = d[k];
                         q[k].e_out = sv ? e[k] : nullptr;
                     }
@@ -257,7 +231,7 @@ static int encoder_forward(const SmkEncoder* h, const float* img, int B, float* 
                 } else {
                     rc = pointwise(n, pw, cur, B, res, res, true, nullptr, e, st);
                     for (int k = 0; k < n && !rc; ++k)
-                        rc = smk::dwconv3x3(e[k], B, res, res, b[k]->mid, b[k]->stride, b[k]->dw.w, b[k]->dw.scale, b[k]->dw.bias, d[k], st, rnd);
+                        rc = smk::dwconv3x3(e[k], B, res, res, b[k]->mid, b[k]->stride, b[k]->dw.fwd.w, b[k]->dw.scale, b[k]->dw.bias, d[k], st, rnd);
                 }
                 if (!rc) rc = pointwise(n, pwl, d, B, ro, ro, false, b0.skip ? cur : nullptr, out, st);
             } else {
@@ -414,16 +388,17 @@ stem_dgrad_kernel(const __grid_constant__ StemDgrad p, int B, int H, int W, int 
     for (int c = 0; c < 3; ++c) out[(((size_t)b * 3 + c) * H + ih) * W + iw] = acc[c];
 }
 
-// 1x1 dgrad of n = 1 or 2 backbones: out[m, :N] = g[m, :K] . Wd (+ res), K = the conv's cout, N = its cin.
+// 1x1 dgrad of n = 1 or 2 backbones over their convs' dgrad weights: out[m, :N] = g[m, :K] . Wd (+ res), K = the conv's
+// cout, N = its cin.
 int dgrad_pw(const SmkEncoder* h, int n, const ConvW* const* c, const float* const* g, int B, int H, int W, const float* const* res,
              float* const* out, bool round, const char* tag, cudaStream_t st) {
     smk::Conv q[2];
     for (int k = 0; k < n; ++k) {
         q[k] = smk::Conv{};
-        q[k].in = g[k]; q[k].ld_in = c[k]->cin; q[k].B = B; q[k].H = H; q[k].W = W; q[k].Cin = c[k]->cin;
-        q[k].w = c[k]->w; q[k].wt = c[k]->wt; q[k].wt_lo = c[k]->wt_lo; q[k].scale = h->ones; q[k].bias = h->zeros;
-        q[k].N = c[k]->cout; q[k].K = c[k]->cin; q[k].mode = 0;
-        q[k].res = res ? res[k] : nullptr; q[k].ld_res = c[k]->cout; q[k].out = out[k]; q[k].ld_out = c[k]->cout;
+        q[k].in = g[k]; q[k].ld_in = c[k]->cout; q[k].B = B; q[k].H = H; q[k].W = W; q[k].Cin = c[k]->cout;
+        q[k].wgt = c[k]->dgrad; q[k].scale = h->ones; q[k].bias = h->zeros;
+        q[k].N = c[k]->cin; q[k].K = c[k]->cout; q[k].mode = 0;
+        q[k].res = res ? res[k] : nullptr; q[k].ld_res = c[k]->cin; q[k].out = out[k]; q[k].ld_out = c[k]->cin;
         q[k].round_out = round ? 1 : 0; q[k].tag = tag;
     }
     return smk::conv(q[0], st, n == 2 ? &q[1] : nullptr);
@@ -434,7 +409,7 @@ int dgrad_dw(int n, const Block* const* b, const float* const* g, const float* c
     DwDgrad p{};
     for (int k = 0; k < 2; ++k) {
         const int j = k < n ? k : n - 1;
-        p.g[k] = g[j]; p.d[k] = d[j]; p.a[k] = a[j]; p.res[k] = res ? res[j] : nullptr; p.w[k] = b[j]->dw_d.w; p.out[k] = out[j];
+        p.g[k] = g[j]; p.d[k] = d[j]; p.a[k] = a[j]; p.res[k] = res ? res[j] : nullptr; p.w[k] = b[j]->dw.dgrad.w; p.out[k] = out[j];
     }
     const int C = b[0]->mid, S = b[0]->stride, Ho = (H + S - 1) / S;
     SMK_REQUIRE(C % 4 == 0 && (S == 1 || H % 2 == 0), "dw_dgrad: C must be a multiple of 4 and stride-2 maps even");
@@ -529,11 +504,11 @@ extern "C" int smk_encoder_backward(const SmkEncoder* h, int B, const float* sav
             // input resolution of the block: the output resolution times the stride, 112 at block 0
             const int ro = res, ri = bi == 0 ? 112 : ro * bk.stride;
             if (bk.kind == CN) {
-                const ConvW* c[2] = {&b[0]->pw_d, &b[1]->pw_d};
+                const ConvW* c[2] = {&b[0]->pw, &b[1]->pw};
                 rc = dgrad_pw(h, n, c, t1, B, ro, ro, nullptr, gy, rnd, tc ? "cn_dgrad_tc" : "cn_dgrad_f32", st);
             } else if (bk.kind == IR) {
-                const ConvW* cl[2] = {&b[0]->pwl_d, &b[1]->pwl_d};
-                const ConvW* cp[2] = {&b[0]->pw_d, &b[1]->pw_d};
+                const ConvW* cl[2] = {&b[0]->pwl, &b[1]->pwl};
+                const ConvW* cp[2] = {&b[0]->pw, &b[1]->pw};
                 const float *dm[2], *am[2];
                 for (int k = 0; k < n; ++k) { dm[k] = SV(b[k]->sv_b); am[k] = SV(b[k]->sv_a); }
                 rc = dgrad_pw(h, n, cl, gy, B, ro, ro, nullptr, t1, false, tc ? "pwl_dgrad_tc" : "pwl_dgrad_f32", st);
@@ -541,7 +516,7 @@ extern "C" int smk_encoder_backward(const SmkEncoder* h, int B, const float* sav
                 if (!rc) rc = dgrad_pw(h, n, cp, t2, B, ri, ri, bk.skip ? gy : nullptr, t1, rnd, tc ? "pw_dgrad_tc" : "pw_dgrad_f32", st);
                 for (int k = 0; k < n; ++k) std::swap(gy[k], t1[k]);
             } else {                                 // DS block 0: the gradient of the stem pre-activation lands in t2
-                const ConvW* cp[2] = {&b[0]->pw_d, &b[1]->pw_d};
+                const ConvW* cp[2] = {&b[0]->pw, &b[1]->pw};
                 const float *dm[2], *am[2];
                 for (int k = 0; k < n; ++k) { dm[k] = SV(b[k]->sv_a); am[k] = SV(bb[k]->sv_stem); }
                 rc = dgrad_pw(h, n, cp, gy, B, ro, ro, nullptr, t1, false, tc ? "ds_pw_dgrad_tc" : "ds_pw_dgrad_f32", st);
@@ -554,7 +529,7 @@ extern "C" int smk_encoder_backward(const SmkEncoder* h, int B, const float* sav
     });
     if (rc) return rc;
     const float* w_stem[3];
-    for (int i = 0; i < 3; ++i) w_stem[i] = g_stem[i] ? h->bb[i].stem_d.w : nullptr;
+    for (int i = 0; i < 3; ++i) w_stem[i] = g_stem[i] ? h->bb[i].stem.dgrad.w : nullptr;
     return enc::stem_dgrad(g_stem, w_stem, B, g_img, main_st);
 }
 

@@ -1,19 +1,21 @@
 // The encoder handle shared by the eval path (encoder.cu) and the train-mode path (encoder_train.cu): the MobileNetV3
 // "minimal" layer lists, the per-backbone topology and its one builder, and the fork/join walk over the backbones.
 #pragma once
-#include "common.cuh"
+#include "conv.cuh"
 #include <string>
 
 namespace enc {
 
-struct ConvW { float* w = nullptr; float* wt = nullptr; float* wt_lo = nullptr; float* scale = nullptr; float* bias = nullptr; int cin = 0, cout = 0; };   // w: [K][N] fp32 path, wt: [N][K] tensor-core path (TF32 heads), wt_lo: TF32 tails (3xTF32 path)
+// A conv with its folded BatchNorm.  fwd / dgrad: the weights of the forward and of the input gradient (see fold_conv): a 1x1
+// conv's are smk::conv operands, a depthwise or stem conv's are fp32 in fwd.w / dgrad.w, in layouts of their own.
+struct ConvW { smk::GemmW fwd{}, dgrad{}; float* scale = nullptr; float* bias = nullptr; int cin = 0, cout = 0; };
 enum Kind { DS = 0, IR = 1, CN = 2 };
 struct BlockDef { Kind kind; int stride; float exp; int cout; };
 // path: the block's module path, <encoder>.encoder.blocks.<stage>.<i>; hin / hout: input / output resolution.
-// pw_f32: fp32 [K][N] copy of a DS block's 1x1 (fused stem path).  *_d: dgrad weights (see fold_conv).
+// pw_f32: fp32 [K][N] copy of a DS block's 1x1 forward weights (fused stem path; pw's scale and bias).
 // sv_a / sv_b: saved-tensor indices of the block's ReLU outputs (IR: expand, depthwise; DS: depthwise; CN: its output); eval handles.
 struct Block { Kind kind; int stride, cin, mid, cout; bool skip; std::string path; int hin, hout;
-               ConvW pw, dw, pwl; ConvW pw_f32; ConvW pw_d, dw_d, pwl_d; int sv_a = -1, sv_b = -1; };
+               ConvW pw, dw, pwl; smk::GemmW pw_f32{}; int sv_a = -1, sv_b = -1; };
 
 // Train handles walk a backbone as a flat list, in forward order, of conv + BatchNorm (+ skip) (+ ReLU) layers.  The stem is
 // entry 0, so the index is the BatchNorm's index in the tensor list (5 tensors per entry, one num_batches_tracked).
@@ -29,7 +31,7 @@ struct Layer {
 };
 
 struct Backbone {
-    ConvW stem, stem_d;
+    ConvW stem;
     std::vector<Block> blocks;
     std::vector<Layer> layers;                 // train handles
     int feat = 0;

@@ -484,13 +484,9 @@ bool carve(smk::Workspace& w, const SmkEncoder* h, const Backbone& bb, int B, Ba
     return o->buf[2] != nullptr;
 }
 
-// Forward and dgrad copies of a 1x1 weight W [cout][cin] in the packed buffer: conv_gemm reads [K][N], tc_conv [N][K]
-// (+ tails).  fwd: K = cin, N = cout; dgrad: K = cout, N = cin.
-struct PwPack { const float* w; const float* wt; const float* wt_lo; };
-
-// Packs the backbone's 1x1 weights for the forward (dgrad = false) or the dgrad (true), and the stem's dgrad weights, in
-// one launch.  packed[Layer::pw]: where that 1x1 conv's copy went.
-int pack_weights(const SmkEncoder* h, const View& v, const BackboneWs& ws, bool dgrad, std::vector<PwPack>& packed, cudaStream_t st) {
+// Packs the backbone's 1x1 weights for the forward (dgrad = false: N = cout, K = cin) or the dgrad (true: N = cin,
+// K = cout), and the stem's dgrad weights, in one launch.  packed[Layer::pw]: that 1x1 conv's operand.
+int pack_weights(const SmkEncoder* h, const View& v, const BackboneWs& ws, bool dgrad, std::vector<smk::GemmW>& packed, cudaStream_t st) {
     const Backbone& bb = h->bb[v.i];
     const bool tc = h->precision >= 1;
     PackJobs jobs{};
@@ -500,12 +496,14 @@ int pack_weights(const SmkEncoder* h, const View& v, const BackboneWs& ws, bool 
     auto add = [&](const float* w, int cin, int cout) {
         const size_t n = (size_t)cin * cout;
         max_n = std::max(max_n, (int)n);
-        if (!tc && dgrad) { packed.push_back(PwPack{w, nullptr, nullptr}); return; }   // torch's [cout][cin] is the dgrad's [K][N]
+        // The layout rule of smk::pack_gemm: fp32 [K][N], or TF32 [N][K] split into heads (+ tails).  Torch's [cout][cin] is
+        // the forward's [N][K] and the dgrad's [K][N], so it is transposed exactly when that is not the layout wanted.
+        const bool torch_nk = !dgrad;
+        if (!tc && !torch_nk) { packed.push_back(smk::GemmW{w, nullptr, nullptr}); return; }   // the fp32 dgrad reads it as is
         PackJob& j = jobs.j[nj++];
         j.src = w; j.rows = cout; j.cols = cin; j.hi = dst; j.lo = tc && h->x3 ? dst + n : nullptr;
-        // fp32 forward: [cin][cout]; tensor-core forward: torch's own layout, split; tensor-core dgrad: [cin][cout], split
-        j.transpose = !tc || dgrad; j.split = tc;
-        packed.push_back(tc ? PwPack{nullptr, j.hi, j.lo} : PwPack{j.hi, nullptr, nullptr});
+        j.transpose = torch_nk != tc; j.split = tc;
+        packed.push_back(tc ? smk::GemmW{nullptr, j.hi, j.lo} : smk::GemmW{j.hi, nullptr, nullptr});
         dst += n * (j.lo ? 2 : 1);
     };
     for (size_t k = 0; k < bb.layers.size(); ++k)
@@ -522,11 +520,11 @@ int pack_weights(const SmkEncoder* h, const View& v, const BackboneWs& ws, bool 
 }
 
 // One 1x1 conv through smk::conv: out[m, :N] = in[m, :K] . W (+ res), unit scale and zero bias.
-int conv1x1(const SmkEncoder* h, const PwPack& w, const float* in, int K, int N, int B, int H, const float* res, float* out, bool round, const char* tag,
+int conv1x1(const SmkEncoder* h, const smk::GemmW& w, const float* in, int K, int N, int B, int H, const float* res, float* out, bool round, const char* tag,
             cudaStream_t st) {
     smk::Conv q{};
     q.in = in; q.ld_in = K; q.B = B; q.H = H; q.W = H; q.Cin = K; q.N = N; q.K = K; q.mode = 0;
-    q.w = w.w; q.wt = w.wt; q.wt_lo = w.wt_lo; q.scale = h->ones; q.bias = h->zeros;
+    q.wgt = w; q.scale = h->ones; q.bias = h->zeros;
     q.res = res; q.ld_res = N; q.out = out; q.ld_out = N; q.round_out = round ? 1 : 0; q.tag = tag;
     return smk::conv(q, st);
 }
@@ -770,7 +768,7 @@ extern "C" int smk_encoder_forward_train(const SmkEncoder* h, const SmkEncoderTr
         const View v{h, args, nullptr, i};
         const BackboneWs& W = bw[i];
         const float eps = args->eps[i], mom = args->momentum[i];
-        std::vector<PwPack> pk;
+        std::vector<smk::GemmW> pk;
         if (int rc = pack_weights(h, v, W, false, pk, st)) return rc;
         for (size_t k = 0; k < bb.layers.size(); ++k) {
             const Layer& L = bb.layers[k];
@@ -836,7 +834,7 @@ extern "C" int smk_encoder_backward_train(const SmkEncoder* h, const SmkEncoderT
         const Backbone& bb = h->bb[i];
         const View v{h, args, grads, i};
         const BackboneWs& W = bw[i];
-        std::vector<PwPack> pk;
+        std::vector<smk::GemmW> pk;
         if (int rc = pack_weights(h, v, W, true, pk, st)) return rc;
         // g: the gradient of the current layer's output; out: where its dgrad goes; held: the gradient of a block's output, kept
         // from the block's last layer to its first, where the skip connection adds it to the gradient of the block's input

@@ -470,16 +470,16 @@ int tc_conv(const Conv& p, cudaStream_t st, const Conv* p2) {
     SMK_REQUIRE(p.store != 1 || ((p.N / 4) % 32 == 0), "tc_conv: pixel-shuffle store needs Cout %% 32 == 0");
     SMK_REQUIRE(!p2 || (p2->B == p.B && p2->H == p.H && p2->W == p.W && p2->Cin == p.Cin && p2->N == p.N && p2->K == p.K && p2->mode == p.mode &&
                         p2->relu == p.relu && p2->ld_in == p.ld_in && p2->ld_out == p.ld_out && p2->ld_res == p.ld_res && p2->store == p.store &&
-                        p2->res_pad == p.res_pad && p2->round_out == p.round_out && !p2->wt_lo == !p.wt_lo && !p2->res == !p.res && p.store != 3),
+                        p2->res_pad == p.res_pad && p2->round_out == p.round_out && !p2->wgt.wt_lo == !p.wgt.wt_lo && !p2->res == !p.res && p.store != 3),
                 "tc_conv: paired problems must have identical shapes and epilogue options");
     int BN = p.N <= 32 ? 32 : (p.N <= 64 ? 64 : 128);
     // Wide 3x3 layers (N a multiple of 256: the generator's 28^2 / 14^2 convolutions, most of its FLOPs): a 128 x 256 tile
     // halves the A-operand bytes wgmma pulls from shared memory per FLOP (TF32 operands are 4 bytes; at BN = 128 the
     // operand reads ask for more than an SM's shared-memory bandwidth).  One persistent CTA per SM, 4-stage ring.
-    if (p.mode != 0 && p.N % 256 == 0 && !p.wt_lo) BN = 256;
+    if (p.mode != 0 && p.N % 256 == 0 && !p.wgt.wt_lo) BN = 256;
     // 3xTF32: plain 1x1 GEMMs (the encoder's 1x1 convs, K <= 960) run X3 = 2; every other problem (3x3 convs, the shuffled
     // store, the mask / second store: the generator's convolutions, K up to 4608) X3 = 3, with 64-wide tiles at most.
-    const int x3 = !p.wt_lo ? 0 : (p.mode == 0 && p.store == 0 && !p.mask && !p.out2) ? 2 : 3;
+    const int x3 = !p.wgt.wt_lo ? 0 : (p.mode == 0 && p.store == 0 && !p.mask && !p.out2) ? 2 : 3;
     if (x3 == 3) BN = std::min(BN, 64);
     TcMaps mp;
     TcArgs a{};
@@ -503,17 +503,17 @@ int tc_conv(const Conv& p, cudaStream_t st, const Conv* p2) {
         } else {                                            // input buffer is [B, H+2, W+2, C], already reflection padded
             if (int rc = encode_im2col(&mp.a[g], q.in, q.B, q.H + 2, q.W + 2, q.Cin, q.ld_in, 0, "tc_conv(A)")) return rc;
         }
-        if (int rc = encode_2d(&mp.b[g], q.wt, (uint64_t)q.N, (uint64_t)q.K, (uint64_t)q.K, (uint32_t)BN, "tc_conv(W)")) return rc;
-        if (q.wt_lo) { if (int rc = encode_2d(&mp.blo[g], q.wt_lo, (uint64_t)q.N, (uint64_t)q.K, (uint64_t)q.K, (uint32_t)BN, "tc_conv(W tails)")) return rc; }
+        if (int rc = encode_2d(&mp.b[g], q.wgt.wt, (uint64_t)q.N, (uint64_t)q.K, (uint64_t)q.K, (uint32_t)BN, "tc_conv(W)")) return rc;
+        if (q.wgt.wt_lo) { if (int rc = encode_2d(&mp.blo[g], q.wgt.wt_lo, (uint64_t)q.N, (uint64_t)q.K, (uint64_t)q.K, (uint32_t)BN, "tc_conv(W tails)")) return rc; }
         else mp.blo[g] = mp.b[g];
     }
     if (groups == 1) { mp.a[1] = mp.a[0]; mp.b[1] = mp.b[0]; mp.blo[1] = mp.blo[0]; a.scale[1] = a.scale[0]; a.bias[1] = a.bias[0]; a.res[1] = a.res[0]; a.out[1] = a.out[0]; }
     {
         const double cin_eff = p.mode == 0 ? p.K : p.Cin;
         const char* tag = p.tag ? p.tag
-                        : p.mode == 0 ? (p.store == 1 ? (p.wt_lo ? "upconv_gemm_tc3x" : "upconv_gemm_tc") : (p.wt_lo ? "pw_gemm_tc3x" : "pw_gemm_tc"))
-                        : p.store == 3 ? (p.wt_lo ? "conv3x3_head_gemm_tc3x" : "conv3x3_head_gemm_tc")
-                                       : (p.wt_lo ? "conv3x3_gemm_tc3x" : "conv3x3_gemm_tc");
+                        : p.mode == 0 ? (p.store == 1 ? (p.wgt.wt_lo ? "upconv_gemm_tc3x" : "upconv_gemm_tc") : (p.wgt.wt_lo ? "pw_gemm_tc3x" : "pw_gemm_tc"))
+                        : p.store == 3 ? (p.wgt.wt_lo ? "conv3x3_head_gemm_tc3x" : "conv3x3_head_gemm_tc")
+                                       : (p.wgt.wt_lo ? "conv3x3_gemm_tc3x" : "conv3x3_gemm_tc");
         if (g_prof_detail) tag = prof_shape_tag(tag, (long)groups * M, p.K, p.N);
         SMK_TAG(tag,
                 groups * 4.0 * ((double)M * cin_eff + (double)p.K * p.N + (double)M * p.N * (1 + !!p.res + !!p.mask + !!p.out2) + 2.0 * p.N),
@@ -532,7 +532,7 @@ int tc_conv(const Conv& p, cudaStream_t st, const Conv* p2) {
         if (BN == 32) return launch<32, 2, 2, false, 3>(mp, a, st, groups);
         return launch<64, 2, 1, false, 3>(mp, a, st, groups);
     }
-    if (p.wt_lo) {
+    if (p.wgt.wt_lo) {
         if (BN == 32) return launch<32, 2, 3, false, 2>(mp, a, st, groups);
         if (BN == 64) return launch<64, 2, 2, false, 2>(mp, a, st, groups);
         return launch<128, 2, 1, false, 2>(mp, a, st, groups);
@@ -569,7 +569,7 @@ extern "C" int smk_debug_conv_tc(const float* in, int ld_in, int B, int H, int W
                                  const float* bias, int N, int K, int mode, int relu, const float* res, int ld_res, int res_pad,
                                  float* out, int ld_out, int store, void* stream) {
     smk::Conv p{};
-    p.in = in; p.ld_in = ld_in; p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.wt = wt; p.scale = scale; p.bias = bias; p.N = N; p.K = K;
+    p.in = in; p.ld_in = ld_in; p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.wgt = smk::GemmW{nullptr, wt, nullptr}; p.scale = scale; p.bias = bias; p.N = N; p.K = K;
     p.mode = mode; p.relu = relu; p.res = res; p.ld_res = ld_res; p.res_pad = res_pad; p.out = out; p.ld_out = ld_out; p.store = store;
     return smk::tc_conv(p, (cudaStream_t)stream);
 }
@@ -577,7 +577,7 @@ extern "C" int smk_debug_conv_tc(const float* in, int ld_in, int B, int H, int W
 extern "C" int smk_debug_gemm_tc3x(const float* in, int ld_in, int M, const float* wt_hi, const float* wt_lo, const float* scale,
                                    const float* bias, int N, int K, int relu, const float* res, int ld_res, float* out, int ld_out, void* stream) {
     smk::Conv p{};
-    p.in = in; p.ld_in = ld_in; p.B = 1; p.H = 1; p.W = M; p.Cin = K; p.wt = wt_hi; p.wt_lo = wt_lo; p.scale = scale; p.bias = bias; p.N = N; p.K = K;
+    p.in = in; p.ld_in = ld_in; p.B = 1; p.H = 1; p.W = M; p.Cin = K; p.wgt = smk::GemmW{nullptr, wt_hi, wt_lo}; p.scale = scale; p.bias = bias; p.N = N; p.K = K;
     p.mode = 0; p.relu = relu; p.res = res; p.ld_res = ld_res; p.res_pad = 0; p.out = out; p.ld_out = ld_out; p.store = 0; p.round_out = 0;
     return smk::tc_conv(p, (cudaStream_t)stream);
 }
@@ -594,7 +594,7 @@ extern "C" int smk_debug_conv_tc3x(const float* in, int ld_in, int B, int H, int
                                    const float* head_w, const float* head_b, int head_c, void* stream) {
     SMK_REQUIRE(wt_hi && wt_lo, "smk_debug_conv_tc3x: the weight heads and tails are both required");
     smk::Conv p{};
-    p.in = in; p.ld_in = ld_in; p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.wt = wt_hi; p.wt_lo = wt_lo; p.scale = scale; p.bias = bias;
+    p.in = in; p.ld_in = ld_in; p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.wgt = smk::GemmW{nullptr, wt_hi, wt_lo}; p.scale = scale; p.bias = bias;
     p.N = N; p.K = K; p.mode = mode; p.relu = relu; p.res = res; p.ld_res = ld_res; p.res_pad = res_pad; p.out = out; p.ld_out = ld_out;
     p.store = store; p.round_out = 0; p.mask = mask; p.ld_mask = ld_mask; p.out2 = out2; p.ld_out2 = ld_out2;
     p.head_w = head_w; p.head_b = head_b; p.head_c = head_c;

@@ -37,13 +37,10 @@ using smk::TensorCursor;
 using smk::grid_of;
 constexpr float kBnEps = 1e-5f;
 
-// dw: dgrad weights, W' scaled by the folded BN scale: [9*cout][cin_p] (fp32) or [cin_p][9*cout] (TF32), k = tap' * cout + co
-// wt_lo / dw_lo (precision 3): the TF32 tails of wt / dw, which then hold the TF32 heads
-struct Conv3 { float* w; float* wt; float* wt_lo; float* scale; float* bias; float* dw; float* dw_lo; int cin, cin_p, cout; };  // w: [9*cin_p][cout]; wt: [cout][9*cin_p]
-// dw: [4*cout][cin] (fp32) or [cin][4*cout] (TF32), k = (dy*2+dx) * cout + co
-struct UpConv { float* w; float* wt; float* wt_lo; float* scale; float* bias; float* dw; float* dw_lo; int cin, cout; };         // w: [cin][4*cout];   wt: [4*cout][cin]
-
-using smk::pack_tc;
+// fwd / dgrad: the weight operands of the forward and of the input gradient (smk::pack_conv3; the dgrad's carry the BN scale)
+struct Conv3 { smk::GemmW fwd, dgrad; float* scale; float* bias; int cin, cin_p, cout; };
+// fwd: N = 4*cout (n = (dy*2+dx) * cout + co), K = cin; dgrad: N = cin, K = 4*cout
+struct UpConv { smk::GemmW fwd, dgrad; float* scale; float* bias; int cin, cout; };
 
 bool fold_conv3(TensorCursor& cur, int cin, int cin_p, int cout, bool tc, bool x3, smk::DeviceArena& arena, Conv3* out, cudaError_t* err) {
     const float* w = cur.next(); const float* g = cur.next(); const float* b = cur.next();
@@ -52,9 +49,7 @@ bool fold_conv3(TensorCursor& cur, int cin, int cin_p, int cout, bool tc, bool x
     std::vector<float> S(cout), Bi(cout);
     smk::fold_bn(g, b, mu, var, cout, kBnEps, S.data(), Bi.data());
     out->cin = cin; out->cin_p = cin_p; out->cout = cout;
-    smk::Conv3Weights pk;                          // the dgrad weights carry the BN scale
-    cudaError_t e = smk::pack_conv3(w, S.data(), cin, cin_p, cout, tc, x3, arena, &pk);
-    out->w = pk.w; out->wt = pk.wt; out->wt_lo = pk.wt_lo; out->dw = pk.dw; out->dw_lo = pk.dw_lo;
+    cudaError_t e = smk::pack_conv3(w, S.data(), cin, cin_p, cout, tc, x3, arena, &out->fwd, &out->dgrad);
     if (e == cudaSuccess) e = arena.upload(S, &out->scale);
     if (e == cudaSuccess) e = arena.upload(Bi, &out->bias);
     *err = e;
@@ -64,24 +59,12 @@ bool fold_conv3(TensorCursor& cur, int cin, int cin_p, int cout, bool tc, bool x
 bool fold_upconv(TensorCursor& cur, int cin, int cout, bool tc, bool x3, smk::DeviceArena& arena, UpConv* out, cudaError_t* err) {
     const float* w = cur.next(); const float* b = cur.next();        // weight [cin, cout, 2, 2], bias [cout]
     if (!w || !b) return false;
-    std::vector<float> W((size_t)cin * 4 * cout), D((size_t)cin * 4 * cout), S((size_t)4 * cout, 1.f), Bi((size_t)4 * cout), Wlo, Dlo;
-    if (x3) { Wlo.assign(W.size(), 0.f); Dlo.assign(D.size(), 0.f); }
-    for (int c = 0; c < cin; ++c)
-        for (int o = 0; o < cout; ++o)
-            for (int q = 0; q < 4; ++q) {
-                float v = w[((size_t)c * cout + o) * 4 + q];
-                if (tc) pack_tc(W, Wlo, ((size_t)q * cout + o) * cin + c, v, x3);   // [N = 4*cout][K = cin]
-                else W[(size_t)c * 4 * cout + q * cout + o] = v;               // [K][N]
-                if (tc) pack_tc(D, Dlo, (size_t)c * 4 * cout + q * cout + o, v, x3);  // dgrad [N = cin][K = 4*cout]
-                else D[((size_t)q * cout + o) * cin + c] = v;                  // dgrad [K][N]
-            }
+    const int N = 4 * cout;                                         // n = q * cout + o, q = dy*2+dx
+    std::vector<float> S((size_t)N, 1.f), Bi((size_t)N);
     for (int q = 0; q < 4; ++q) for (int o = 0; o < cout; ++o) Bi[q * cout + o] = b[o];
     out->cin = cin; out->cout = cout;
-    out->w = out->wt = out->wt_lo = out->dw_lo = nullptr;
-    cudaError_t e = arena.upload(W, tc ? &out->wt : &out->w);
-    if (e == cudaSuccess && x3) e = arena.upload(Wlo, &out->wt_lo);
-    if (e == cudaSuccess) e = arena.upload(D, &out->dw);
-    if (e == cudaSuccess && x3) e = arena.upload(Dlo, &out->dw_lo);
+    cudaError_t e = smk::pack_gemm(arena, N, cin, tc, x3, [&](int n, int c) { return w[((size_t)c * cout + n % cout) * 4 + n / cout]; }, &out->fwd);
+    if (e == cudaSuccess) e = smk::pack_gemm(arena, cin, N, tc, x3, [&](int c, int k) { return w[((size_t)c * cout + k % cout) * 4 + k / cout]; }, &out->dgrad);
     if (e == cudaSuccess) e = arena.upload(S, &out->scale);
     if (e == cudaSuccess) e = arena.upload(Bi, &out->bias);
     *err = e;
@@ -199,10 +182,10 @@ int conv3(const SmkGenerator* h, const Conv3& c, const float* in, int ld_in, int
           float* out2 = nullptr) {
     smk::Conv p{};
     if (fuse_head) { p.head_w = h->fw; p.head_b = h->fb; p.head_c = h->cout; }
-    p.in = in; p.ld_in = ld_in; p.B = B; p.H = S; p.W = S; p.Cin = c.cin_p; p.w = c.w; p.wt = c.wt; p.wt_lo = c.wt_lo; p.scale = c.scale; p.bias = c.bias;
+    p.in = in; p.ld_in = ld_in; p.B = B; p.H = S; p.W = S; p.Cin = c.cin_p; p.wgt = c.fwd; p.scale = c.scale; p.bias = c.bias;
     p.N = c.cout; p.K = 9 * c.cin_p; p.mode = refl ? 2 : 1; p.relu = relu ? 1 : 0;
     p.res = res; p.ld_res = c.cout; p.res_pad = res_pad; p.out = out; p.ld_out = ld_out; p.store = store;
-    p.round_out = c.wt && !c.wt_lo ? 1 : 0;        // TF32 consumers; 3xTF32 consumers split full fp32 activations themselves
+    p.round_out = c.fwd.wt && !c.fwd.wt_lo ? 1 : 0;    // TF32 consumers; 3xTF32 consumers split full fp32 activations themselves
     p.out2 = out2; p.ld_out2 = c.cout;
     return smk::conv(p, st);
 }
@@ -280,8 +263,8 @@ int generator_forward(const SmkGenerator* h, const float* x, int B, float* y, fl
         int lvl = 3 - l;                            // index into cat/t/d (3 = 28x28 ... 0 = 224x224)
         const UpConv& u = h->up[l];
         smk::Conv q{};
-        q.in = din; q.ld_in = u.cin; q.B = B; q.H = dS; q.W = dS; q.Cin = u.cin; q.w = u.w; q.wt = u.wt; q.wt_lo = u.wt_lo; q.scale = u.scale; q.bias = u.bias;
-        q.N = 4 * u.cout; q.K = u.cin; q.mode = 0; q.out = cat[lvl]; q.ld_out = 2 * u.cout; q.store = 1; q.round_out = u.wt && !u.wt_lo ? 1 : 0;
+        q.in = din; q.ld_in = u.cin; q.B = B; q.H = dS; q.W = dS; q.Cin = u.cin; q.wgt = u.fwd; q.scale = u.scale; q.bias = u.bias;
+        q.N = 4 * u.cout; q.K = u.cin; q.mode = 0; q.out = cat[lvl]; q.ld_out = 2 * u.cout; q.store = 1; q.round_out = u.fwd.wt && !u.fwd.wt_lo ? 1 : 0;
         if ((rc = smk::conv(q, st))) return rc;
         dS *= 2;
         float* dt = sv ? SV(sv_dec(h, lvl, 0)) : t[lvl];
@@ -433,24 +416,22 @@ nhwc_to_nchw_kernel(const float* __restrict__ in, int B, int HW, int Cp, int C, 
 // dgrad of a 3x3 conv (zero padding 1): g_in = conv3x3(g, W') over S x S, * [mask > 0] (mask: the saved input activation).
 int dgrad3(const SmkGenerator* h, const Conv3& c, const float* g, int B, int S, const float* mask, float* out, int ld_out, bool round,
            cudaStream_t st) {
-    const bool tc = h->precision != 0;
     smk::Conv p{};
-    p.in = g; p.ld_in = c.cout; p.B = B; p.H = S; p.W = S; p.Cin = c.cout; p.w = tc ? nullptr : c.dw; p.wt = tc ? c.dw : nullptr; p.wt_lo = c.dw_lo;
+    p.in = g; p.ld_in = c.cout; p.B = B; p.H = S; p.W = S; p.Cin = c.cout; p.wgt = c.dgrad;
     p.scale = h->ones; p.bias = h->zeros;
     p.N = c.cin_p; p.K = 9 * c.cout; p.mode = 1; p.out = out; p.ld_out = ld_out; p.round_out = round ? 1 : 0;
-    p.mask = mask; p.ld_mask = c.cin_p; p.tag = c.dw_lo ? "conv3x3_dgrad_tc3x" : tc ? "conv3x3_dgrad_tc" : "conv3x3_dgrad_f32";
+    p.mask = mask; p.ld_mask = c.cin_p; p.tag = c.dgrad.wt_lo ? "conv3x3_dgrad_tc3x" : c.dgrad.wt ? "conv3x3_dgrad_tc" : "conv3x3_dgrad_f32";
     return smk::conv(p, st);
 }
 
 // dgrad of ConvTranspose2d(k2, s2): g_in[S x S, cin] = s2d(g_out)[S x S, 4 cout] . W'^T, * [mask > 0].
 int dgrad_up(const SmkGenerator* h, const UpConv& u, const float* s2d, int B, int S, const float* mask, float* out, bool round, cudaStream_t st) {
-    const bool tc = h->precision != 0;
     const int K = 4 * u.cout;
     smk::Conv p{};
-    p.in = s2d; p.ld_in = K; p.B = B; p.H = S; p.W = S; p.Cin = K; p.w = tc ? nullptr : u.dw; p.wt = tc ? u.dw : nullptr; p.wt_lo = u.dw_lo;
+    p.in = s2d; p.ld_in = K; p.B = B; p.H = S; p.W = S; p.Cin = K; p.wgt = u.dgrad;
     p.scale = h->ones; p.bias = h->zeros;
     p.N = u.cin; p.K = K; p.mode = 0; p.out = out; p.ld_out = u.cin; p.round_out = round ? 1 : 0;
-    p.mask = mask; p.ld_mask = u.cin; p.tag = u.dw_lo ? "upconv_dgrad_tc3x" : tc ? "upconv_dgrad_tc" : "upconv_dgrad_f32";
+    p.mask = mask; p.ld_mask = u.cin; p.tag = u.dgrad.wt_lo ? "upconv_dgrad_tc3x" : u.dgrad.wt ? "upconv_dgrad_tc" : "upconv_dgrad_f32";
     return smk::conv(p, st);
 }
 

@@ -66,7 +66,7 @@ conv_gemm_kernel(Conv p, int M) {
             int kk = idx / (BN / 4), nq = idx - kk * (BN / 4);
             float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
             if (kk < BK && k0 + kk < p.K && n0 + nq * 4 < p.N)
-                v = *reinterpret_cast<const float4*>(p.w + (size_t)(k0 + kk) * p.N + n0 + nq * 4);
+                v = *reinterpret_cast<const float4*>(p.wgt.w + (size_t)(k0 + kk) * p.N + n0 + nq * 4);
             b_reg[j] = v;
         }
     };
@@ -404,7 +404,7 @@ conv1x1_sigmoid_kernel(const float* __restrict__ in, int B, int HW, int Cin, con
 
 int conv_gemm(const Conv& p, cudaStream_t st) {
     const int M = p.B * p.H * p.W;
-    SMK_REQUIRE(!p.wt && !p.wt_lo, "conv_gemm: TF32 weights need tc_conv");
+    SMK_REQUIRE(!p.wgt.wt && !p.wgt.wt_lo, "conv_gemm: TF32 weights need tc_conv");
     SMK_REQUIRE(!p.res_pad && (p.store == 0 || p.store == 1), "conv_gemm: padded residuals and stores 2 / 3 need tc_conv");
     SMK_REQUIRE(p.K % 4 == 0 && p.N % 4 == 0 && p.ld_in % 4 == 0, "conv_gemm: K, N, ld_in must be multiples of 4");
     SMK_REQUIRE(p.mode == 0 || p.Cin % 4 == 0, "conv_gemm: Cin must be a multiple of 4");
@@ -715,7 +715,7 @@ extern "C" int smk_debug_conv_f32(const float* in, int ld_in, int B, int H, int 
                                   const float* bias, int N, int K, int mode, int relu, const float* res, int ld_res,
                                   float* out, int ld_out, int shuffle, void* stream) {
     smk::Conv p{};
-    p.in = in; p.ld_in = ld_in; p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.w = w_kn; p.scale = scale; p.bias = bias; p.N = N; p.K = K;
+    p.in = in; p.ld_in = ld_in; p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.wgt = smk::GemmW{w_kn, nullptr, nullptr}; p.scale = scale; p.bias = bias; p.N = N; p.K = K;
     p.mode = mode; p.relu = relu; p.res = res; p.ld_res = ld_res; p.out = out; p.ld_out = ld_out; p.store = shuffle;
     return smk::conv_gemm(p, (cudaStream_t)stream);
 }

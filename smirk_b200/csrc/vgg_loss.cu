@@ -35,7 +35,7 @@ constexpr int kChunk4 = 4096;                                       // float4s p
 
 struct Norm { float mean[3], std[3]; };
 
-struct VggConv { smk::Conv3Weights pk; float* bias; int cin, cin_p, cout, S; };
+struct VggConv { smk::GemmW fwd, dgrad; float* bias; int cin, cin_p, cout, S; };   // fwd / dgrad: smk::pack_conv3
 
 int tap_S(int t) { return 224 >> t; }
 int tap_C(int t) { return 64 << t; }
@@ -215,7 +215,7 @@ extern "C" int smk_vgg_loss_create(const SmkVggLossDesc* desc, SmkVggLoss** out)
         c.S = 224 >> kStage[l]; c.cout = 64 << kStage[l];
         c.cin = l == 0 ? 3 : h->conv[l - 1].cout;
         c.cin_p = l > 0 ? c.cin : tc ? 32 : 8;         // the tensor-core path reads 128-byte pixel rows
-        e = smk::pack_conv3(desc->tensors[2 + 2 * l], nullptr, c.cin, c.cin_p, c.cout, tc, x3, h->arena, &c.pk);
+        e = smk::pack_conv3(desc->tensors[2 + 2 * l], nullptr, c.cin, c.cin_p, c.cout, tc, x3, h->arena, &c.fwd, &c.dgrad);
         if (e == cudaSuccess) e = h->arena.upload(desc->tensors[3 + 2 * l], (size_t)c.cout, &c.bias);
     }
     const std::vector<float> one(512, 1.f), zero(512, 0.f);
@@ -251,7 +251,7 @@ int conv_fwd(const SmkVggLoss* h, const VggConv& c, const float* in, int B2, flo
              cudaStream_t st) {
     smk::Conv p{};
     p.in = in; p.ld_in = c.cin_p; p.B = B2; p.H = c.S; p.W = c.S; p.Cin = c.cin_p;
-    p.w = c.pk.w; p.wt = c.pk.wt; p.wt_lo = c.pk.wt_lo; p.scale = h->ones; p.bias = c.bias;
+    p.wgt = c.fwd; p.scale = h->ones; p.bias = c.bias;
     p.N = c.cout; p.K = 9 * c.cin_p; p.mode = 1; p.relu = 1; p.out = out; p.ld_out = c.cout;
     p.round_out = round ? 1 : 0;
     p.out2 = out2; p.ld_out2 = c.cout; p.out2_rows = out2_imgs * c.S * c.S;
@@ -260,14 +260,12 @@ int conv_fwd(const SmkVggLoss* h, const VggConv& c, const float* in, int B2, flo
 
 // dgrad of conv c over Bc images: g_in = conv3x3(g, W') * [mask > 0] (mask: the saved input activation, or null).
 int conv_dgrad(const SmkVggLoss* h, const VggConv& c, const float* g, int Bc, const float* mask, float* out, bool round, cudaStream_t st) {
-    const bool tc = h->precision != 0;
     smk::Conv p{};
-    p.in = g; p.ld_in = c.cout; p.B = Bc; p.H = c.S; p.W = c.S; p.Cin = c.cout;
-    p.w = tc ? nullptr : c.pk.dw; p.wt = tc ? c.pk.dw : nullptr; p.wt_lo = c.pk.dw_lo;
+    p.in = g; p.ld_in = c.cout; p.B = Bc; p.H = c.S; p.W = c.S; p.Cin = c.cout; p.wgt = c.dgrad;
     p.scale = h->ones; p.bias = h->zeros;
     p.N = c.cin_p; p.K = 9 * c.cout; p.mode = 1; p.out = out; p.ld_out = c.cin_p; p.round_out = round ? 1 : 0;
     p.mask = mask; p.ld_mask = c.cin_p;
-    p.tag = c.pk.dw_lo ? "vgg_conv_dgrad_tc3x" : tc ? "vgg_conv_dgrad_tc" : "vgg_conv_dgrad_f32";
+    p.tag = c.dgrad.wt_lo ? "vgg_conv_dgrad_tc3x" : c.dgrad.wt ? "vgg_conv_dgrad_tc" : "vgg_conv_dgrad_f32";
     return smk::conv(p, st);
 }
 
