@@ -10,6 +10,7 @@ from .renderer import Renderer              # noqa: F401
 from .smirk_encoder import SmirkEncoder     # noqa: F401
 from .smirk_generator import SmirkGenerator # noqa: F401
 from .vgg_loss import VGGPerceptualLoss     # noqa: F401
+from .mica import MICA                      # noqa: F401
 
-__all__ = ["FLAME", "Renderer", "SmirkEncoder", "SmirkGenerator", "VGGPerceptualLoss"]
+__all__ = ["FLAME", "Renderer", "SmirkEncoder", "SmirkGenerator", "VGGPerceptualLoss", "MICA"]
 __version__ = "0.1.0"

@@ -59,6 +59,10 @@ class SmkVggLossDesc(C.Structure):
     _fields_ = [("tensors", C.POINTER(c_f32p)), ("n_tensors", C.c_int), ("precision", C.c_int)]
 
 
+class SmkMicaDesc(C.Structure):
+    _fields_ = [("tensors", C.POINTER(c_f32p)), ("n_tensors", C.c_int), ("precision", C.c_int)]
+
+
 class SmkMaskingDesc(C.Structure):
     _fields_ = [("n_verts", C.c_int), ("n_faces", C.c_int), ("faces", c_i32p)]
 
@@ -167,7 +171,16 @@ LOSS_BINDINGS = [
     ("smk_vgg_loss_backward_workspace_bytes", _sz, [_vp, _i, _i]),
     ("smk_vgg_loss_backward", _i, [_vp, _i, _i, _vp, _sz, _vp, _vp, _vp, _vp, _sz, STREAM]),
 ]
-_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS + LOSS_BINDINGS if args[-1:] == [STREAM])
+# The binding table of include/smirk_b200_mica.h (MICA and its shape loss), in that header's order, by the same rules.
+MICA_BINDINGS = [
+    ("smk_mica_create", _i, [C.POINTER(SmkMicaDesc), _vpp]),
+    ("smk_mica_destroy", None, [_vp]),
+    ("smk_mica_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_mica_forward", _i, [_vp, _vp, _i, _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_mica_shape_loss_forward", _i, [_vp, _vp, _i, _i, _i, _vp, STREAM]),
+    ("smk_mica_shape_loss_backward", _i, [_vp, _vp, _i, _i, _i, _vp, _vp, STREAM]),
+]
+_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS + LOSS_BINDINGS + MICA_BINDINGS if args[-1:] == [STREAM])
 
 
 def lib():
@@ -179,7 +192,7 @@ def lib():
         raise RuntimeError("smirk_b200: %s not found — build it with `python -m smirk_b200.build` "
                            "(there is no CPU / PyTorch fallback)" % LIB_PATH)
     L = C.CDLL(LIB_PATH)
-    for name, restype, argtypes in BINDINGS + LOSS_BINDINGS:
+    for name, restype, argtypes in BINDINGS + LOSS_BINDINGS + MICA_BINDINGS:
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, [_vp if a is STREAM else a for a in argtypes]
     if L.smk_version() != 100:

@@ -38,10 +38,18 @@ struct Conv {
     float* out2; int ld_out2;            // optional (no pixel shuffle): the stored activations again, compact NHWC at pixel m
     int out2_rows;                       // out2 takes only the pixels m < out2_rows (0: every pixel), e.g. the first images
     const char* tag;                     // profiler tag (null: derived from the problem)
+    // The fields below run on their own kernel instantiations (store 0, a single problem, N >= 64), so the kernels of
+    // problems that leave them null are the ones compiled without them.
+    const float* prelu;                  // optional: per-n PReLU slope, v < 0 -> v * prelu[n], after the residual and ReLU
+    const float* scale2; const float* bias2;   // optional (with out2): out2 = scale2[n] * v + bias2[n] of the unrounded v,
+                                               // e.g. the next layer's BatchNorm, whose zero padding forbids folding it
+    int round_out2;                      // with scale2: round out2 to TF32 (round_out then rounds `out` alone)
 };
 
-// conv_gemm_kernel takes Conv by value: its parameter layout is pinned.
-static_assert(offsetof(Conv, wgt) == 40 && offsetof(Conv, scale) == 64 && sizeof(Conv) == 184, "smk::Conv layout moved");
+// conv_gemm_kernel takes Conv by value: its parameter layout is pinned, and fields are only ever appended.
+static_assert(offsetof(Conv, wgt) == 40 && offsetof(Conv, scale) == 64 && offsetof(Conv, tag) == 176 && sizeof(Conv) == 216,
+              "smk::Conv layout moved");
+inline bool conv_aff(const Conv& p) { return p.prelu || p.scale2; }
 
 // fp32 CUDA cores: modes 0-2, stores 0 and 1; no TF32 weights, padded residual or paired problem.
 int conv_gemm(const Conv& p, cudaStream_t st);

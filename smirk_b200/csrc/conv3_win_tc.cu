@@ -285,7 +285,7 @@ int launch(const CUtensorMap& tmX, const CUtensorMap& tmW, const WinArgs& a, cud
 }  // namespace
 
 bool conv3_win_supported(const Conv& p) {
-    if (p.mode != 1 || p.res || p.wgt.wt_lo || (p.store != 0 && p.store != 3) || (p.store == 3 && (p.N != 32 || p.mask))) return false;
+    if (p.mode != 1 || p.res || p.wgt.wt_lo || conv_aff(p) || (p.store != 0 && p.store != 3) || (p.store == 3 && (p.N != 32 || p.mask))) return false;
     if (p.Cin % 32 != 0 || p.K != 9 * p.Cin || (p.N != 32 && p.N != 64)) return false;
     return p.W >= 56;                                             // low-resolution layers are MMA-bound: gemm_tc's wide tiles win there
 }

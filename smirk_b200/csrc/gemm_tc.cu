@@ -63,11 +63,13 @@ struct TcArgs {
     const float* mask; int ld_mask;    // zero outputs whose mask[m, n] <= 0 (single problem, store 0)
     float* out2; int ld_out2;          // second store of the activations, compact at pixel m (single problem, store 0 / 2 / 3)
     int out2_rows;                     // out2 takes the pixels m < out2_rows
+    const float* prelu;                // PReLU slope per column (AFF instantiations; store 0)
+    const float* scale2; const float* bias2; int round_out2;   // out2 = scale2 * v + bias2 of the unrounded v (AFF)
 };
 
 struct TcMaps { CUtensorMap a[2], b[2], blo[2]; };       // per problem: activations, weights (TF32 heads), weight tails (3xTF32)
 
-template <int BN, int STAGES, int MINB, bool PERSIST, int X3, bool EXTRA>
+template <int BN, int STAGES, int MINB, bool PERSIST, int X3, bool EXTRA, bool AFF = false>
 __global__ void __launch_bounds__(NUM_THREADS, MINB)
 gemm_tc_kernel(const __grid_constant__ TcMaps mp, const TcArgs a) {
     // Output tiles (128 rows x BN columns) are strided over the grid.
@@ -90,6 +92,7 @@ gemm_tc_kernel(const __grid_constant__ TcMaps mp, const TcArgs a) {
     //                    fp32 (round-to-nearest) add: the truncation only ever sees one k-block's partial sum.
     //   EXTRA = true     : the epilogue also applies `mask` and writes `out2` (backward / grad-mode forward); the forward-only
     //                    instantiations are compiled without them.
+    //   AFF = true       : (with EXTRA) also the per-column PReLU and the second store's own affine (MICA's residual blocks).
     static_assert(!X3 || !PERSIST, "3xTF32 runs single-tile CTAs");
     constexpr int B_STAGE_BYTES = BN * BKB;
     constexpr int HALF_STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
@@ -322,14 +325,34 @@ gemm_tc_kernel(const __grid_constant__ TcMaps mp, const TcArgs a) {
                         o.x += r4.x; o.y += r4.y; o.z += r4.z; o.w += r4.w;
                     }
                     if (a.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
+                    if constexpr (AFF) {
+                        if (a.prelu) {
+                            const float4 w4 = __ldg(reinterpret_cast<const float4*>(a.prelu + nc));
+                            o.x = o.x < 0.f ? o.x * w4.x : o.x; o.y = o.y < 0.f ? o.y * w4.y : o.y;
+                            o.z = o.z < 0.f ? o.z * w4.z : o.z; o.w = o.w < 0.f ? o.w * w4.w : o.w;
+                        }
+                    }
                     const size_t mc = (size_t)(row0 + 4 * i + sub);            // compact pixel (mask, second store)
                     if (EXTRA && a.mask) {
                         const float4 k4 = __ldg(reinterpret_cast<const float4*>(a.mask + mc * a.ld_mask + nc));
                         o.x = k4.x > 0.f ? o.x : 0.f; o.y = k4.y > 0.f ? o.y : 0.f; o.z = k4.z > 0.f ? o.z : 0.f; o.w = k4.w > 0.f ? o.w : 0.f;
                     }
+                    float4 o2 = o;
+                    if constexpr (AFF) {
+                        if (a.scale2) {
+                            const float4 s2 = __ldg(reinterpret_cast<const float4*>(a.scale2 + nc));
+                            const float4 b2 = __ldg(reinterpret_cast<const float4*>(a.bias2 + nc));
+                            o2.x = fmaf(o.x, s2.x, b2.x); o2.y = fmaf(o.y, s2.y, b2.y); o2.z = fmaf(o.z, s2.z, b2.z); o2.w = fmaf(o.w, s2.w, b2.w);
+                            if (a.round_out2) { o2.x = smk::round_tf32(o2.x); o2.y = smk::round_tf32(o2.y); o2.z = smk::round_tf32(o2.z); o2.w = smk::round_tf32(o2.w); }
+                        }
+                    }
                     if (a.round_out) { o.x = smk::round_tf32(o.x); o.y = smk::round_tf32(o.y); o.z = smk::round_tf32(o.z); o.w = smk::round_tf32(o.w); }
                     *reinterpret_cast<float4*>(g_out + (size_t)(opix[i] + pix_off) * a.ld_out + col) = o;
-                    if (EXTRA && a.out2 && mc < (size_t)a.out2_rows) *reinterpret_cast<float4*>(a.out2 + mc * a.ld_out2 + nc) = o;
+                    if constexpr (AFF) {
+                        if (a.out2 && mc < (size_t)a.out2_rows) *reinterpret_cast<float4*>(a.out2 + mc * a.ld_out2 + nc) = a.scale2 ? o2 : o;
+                    } else {
+                        if (EXTRA && a.out2 && mc < (size_t)a.out2_rows) *reinterpret_cast<float4*>(a.out2 + mc * a.ld_out2 + nc) = o;
+                    }
                 }
             }
             __syncwarp();
@@ -434,19 +457,19 @@ int encode_im2col(CUtensorMap* map, const float* base, int B, int H, int W, int 
 
 namespace {
 
-template <int BN, int STAGES, int MINB, bool PERSIST, int X3, bool EXTRA>
+template <int BN, int STAGES, int MINB, bool PERSIST, int X3, bool EXTRA, bool AFF = false>
 int launch_kernel(const TcMaps& mp, const TcArgs& a_in, cudaStream_t st, int groups) {
     constexpr size_t stage = X3 ? A_STAGE_BYTES + 2 * BN * BKB : A_STAGE_BYTES + BN * BKB;
     constexpr size_t smem = (size_t)STAGES * stage + (PERSIST ? SLAB_BYTES : 0) + BAR_BYTES + HEAD_PAR_BYTES + 1024;
     static_assert(PERSIST || (size_t)STAGES * stage >= SLAB_BYTES, "single-tile CTAs stage the epilogue in ring stage 0");
     static_assert(MINB * (smem + 1024) <= 228 * 1024, "shared memory budget of MINB resident CTAs");
-    SMK_CHECK_CUDA((set_max_dynamic_smem<gemm_tc_kernel<BN, STAGES, MINB, PERSIST, X3, EXTRA>>((int)smem)));
+    SMK_CHECK_CUDA((set_max_dynamic_smem<gemm_tc_kernel<BN, STAGES, MINB, PERSIST, X3, EXTRA, AFF>>((int)smem)));
     TcArgs a = a_in;
     a.tiles_n = cdiv(a.N, BN);
     a.n_tiles_g = cdiv(a.M, BM) * a.tiles_n;
     a.n_tiles = groups * a.n_tiles_g;
     dim3 grid((unsigned)(PERSIST ? std::min(a.n_tiles, MINB * num_sms()) : a.n_tiles));
-    SMK_LAUNCH((gemm_tc_kernel<BN, STAGES, MINB, PERSIST, X3, EXTRA>), dim3(grid), dim3(NUM_THREADS), smem, st, mp, a);
+    SMK_LAUNCH((gemm_tc_kernel<BN, STAGES, MINB, PERSIST, X3, EXTRA, AFF>), dim3(grid), dim3(NUM_THREADS), smem, st, mp, a);
     SMK_CHECK_LAUNCH();
     return 0;
 }
@@ -454,6 +477,9 @@ int launch_kernel(const TcMaps& mp, const TcArgs& a_in, cudaStream_t st, int gro
 template <int BN, int STAGES, int MINB, bool PERSIST, int X3 = 0>
 int launch(const TcMaps& mp, const TcArgs& a, cudaStream_t st, int groups) {
     if constexpr (X3 != 2) {                            // X3 = 2 runs plain GEMMs only (tc_conv)
+        if constexpr (BN >= 64) {                       // PReLU / second-store affine: N >= 64 (tc_conv checks)
+            if (a.prelu || a.scale2) return launch_kernel<BN, STAGES, MINB, PERSIST, X3, true, true>(mp, a, st, groups);
+        }
         if (a.mask || a.out2) return launch_kernel<BN, STAGES, MINB, PERSIST, X3, true>(mp, a, st, groups);
     }
     return launch_kernel<BN, STAGES, MINB, PERSIST, X3, false>(mp, a, st, groups);
@@ -478,8 +504,10 @@ int tc_conv(const Conv& p, cudaStream_t st, const Conv* p2) {
     // operand reads ask for more than an SM's shared-memory bandwidth).  One persistent CTA per SM, 4-stage ring.
     if (p.mode != 0 && p.N % 256 == 0 && !p.wgt.wt_lo) BN = 256;
     // 3xTF32: plain 1x1 GEMMs (the encoder's 1x1 convs, K <= 960) run X3 = 2; every other problem (3x3 convs, the shuffled
-    // store, the mask / second store: the generator's convolutions, K up to 4608) X3 = 3, with 64-wide tiles at most.
-    const int x3 = !p.wgt.wt_lo ? 0 : (p.mode == 0 && p.store == 0 && !p.mask && !p.out2) ? 2 : 3;
+    // store, the mask / second store: the generator's convolutions, K up to 4608; MICA's PReLU / affine epilogues and its
+    // K = 25088 fc) X3 = 3, with 64-wide tiles at most.
+    const bool plain = p.mode == 0 && p.store == 0 && !p.mask && !p.out2 && !conv_aff(p) && p.K <= 1024;
+    const int x3 = !p.wgt.wt_lo ? 0 : plain ? 2 : 3;
     if (x3 == 3) BN = std::min(BN, 64);
     TcMaps mp;
     TcArgs a{};
@@ -493,6 +521,9 @@ int tc_conv(const Conv& p, cudaStream_t st, const Conv* p2) {
     SMK_REQUIRE((!p.mask || p.store == 0) && (!p.out2 || p.store != 1) && (!(p.mask || p.out2) || !p2),
                 "tc_conv: the mask needs store 0, the second store a non-shuffled store, both a single problem");
     a.mask = p.mask; a.ld_mask = p.ld_mask; a.out2 = p.out2; a.ld_out2 = p.ld_out2; a.out2_rows = p.out2_rows > 0 ? p.out2_rows : M;
+    SMK_REQUIRE(!conv_aff(p) || (p.store == 0 && p.N >= 64 && !p2 && (!p.scale2 || (p.bias2 && p.out2))),
+                "tc_conv: PReLU / second-store affine need store 0, N >= 64, a single problem, and scale2 with bias2 and out2");
+    a.prelu = p.prelu; a.scale2 = p.scale2; a.bias2 = p.bias2; a.round_out2 = p.round_out2;
     for (int g = 0; g < groups; ++g) {
         const Conv& q = g ? *p2 : p;
         a.scale[g] = q.scale; a.bias[g] = q.bias; a.res[g] = q.res; a.out[g] = q.out;

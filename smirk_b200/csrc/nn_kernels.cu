@@ -10,7 +10,8 @@ constexpr int NT = 256;
 // ---------------------------------------------------------------------------------------------------
 // Implicit-GEMM convolution, BMxBN tile, BK = 16, 256 threads as a 16x16 grid of (BM/16)x(BN/16)
 // register tiles; global->register prefetch of the next k-slab overlaps the FMAs of the current one.
-template <int BM, int BN>
+// AFF: the epilogue also applies p.prelu and writes out2 through p.scale2 / p.bias2 (smk::conv_aff problems only).
+template <int BM, int BN, bool AFF = false>
 __global__ void __launch_bounds__(NT)
 conv_gemm_kernel(Conv p, int M) {
     constexpr int TM = BM / 16, TN = BN / 16;
@@ -124,9 +125,18 @@ conv_gemm_kernel(Conv p, int M) {
             float v = fmaf(acc[i][j], p.scale[n], p.bias[n]);
             if (p.res) v += p.res[(size_t)m * p.ld_res + n];
             if (p.relu) v = fmaxf(v, 0.f);
+            if constexpr (AFF) { if (p.prelu && v < 0.f) v *= p.prelu[n]; }
             if (p.mask && !(p.mask[(size_t)m * p.ld_mask + n] > 0.f)) v = 0.f;
+            float v2 = 0.f;
+            if constexpr (AFF) {
+                if (p.scale2) { v2 = fmaf(v, p.scale2[n], p.bias2[n]); if (p.round_out2) v2 = round_tf32(v2); }
+            }
             if (p.round_out) v = round_tf32(v);
-            if (p.out2 && (p.out2_rows <= 0 || m < p.out2_rows)) p.out2[(size_t)m * p.ld_out2 + n] = v;
+            if constexpr (AFF) {
+                if (p.out2 && (p.out2_rows <= 0 || m < p.out2_rows)) p.out2[(size_t)m * p.ld_out2 + n] = p.scale2 ? v2 : v;
+            } else {
+                if (p.out2 && (p.out2_rows <= 0 || m < p.out2_rows)) p.out2[(size_t)m * p.ld_out2 + n] = v;
+            }
             if (p.store == 1) {
                 int cout = p.N >> 2, q = n / cout, co = n - q * cout;
                 int b = m / HW, r = m - b * HW, h = r / p.W, w = r - h * p.W;
@@ -409,6 +419,8 @@ int conv_gemm(const Conv& p, cudaStream_t st) {
     SMK_REQUIRE(p.K % 4 == 0 && p.N % 4 == 0 && p.ld_in % 4 == 0, "conv_gemm: K, N, ld_in must be multiples of 4");
     SMK_REQUIRE(p.mode == 0 || p.Cin % 4 == 0, "conv_gemm: Cin must be a multiple of 4");
     SMK_REQUIRE(!p.out2 || p.store != 1, "conv_gemm: the second store does not support the pixel-shuffle layout");
+    SMK_REQUIRE(!conv_aff(p) || (p.store == 0 && p.N > 32 && (!p.scale2 || (p.bias2 && p.out2))),
+                "conv_gemm: PReLU / second-store affine need store 0, N > 32, and scale2 with bias2 and out2");
     {
         const double cin_eff = p.mode == 0 ? p.K : p.Cin;       // unique input bytes (not im2col-expanded)
         const char* tag = p.tag ? p.tag : p.mode == 0 ? (p.store == 1 ? "upconv_gemm_f32" : "pw_gemm_f32") : "conv3x3_gemm_f32";
@@ -422,7 +434,8 @@ int conv_gemm(const Conv& p, cudaStream_t st) {
         SMK_LAUNCH((conv_gemm_kernel<128, 32>), dim3(grid), dim3(NT), 0, st, p, M);
     } else {
         dim3 grid(cdiv(M, 64), cdiv(p.N, 64));
-        SMK_LAUNCH((conv_gemm_kernel<64, 64>), dim3(grid), dim3(NT), 0, st, p, M);
+        if (conv_aff(p)) SMK_LAUNCH((conv_gemm_kernel<64, 64, true>), dim3(grid), dim3(NT), 0, st, p, M);
+        else SMK_LAUNCH((conv_gemm_kernel<64, 64>), dim3(grid), dim3(NT), 0, st, p, M);
     }
     SMK_CHECK_LAUNCH();
     return 0;
