@@ -158,14 +158,25 @@ static int encoder_forward(const SmkEncoder* h, const float* img, int B, float* 
     float* stem_out[3];                                           // where each backbone's stem writes
     for (int i = 0; i < 3; ++i) stem_out[i] = sv && h->present[i] ? SV(h->bb[i].sv_stem) : bufs[i][0];
     const int n_present = (int)h->present[0] + (int)h->present[1] + (int)h->present[2];
-    // precision 2: stem + block 0 (depthwise-separable, 16 channels at 112 x 112) run as one kernel per backbone —
-    // the three largest activations never reach HBM.
+    // precision 2: stem + block 0 (depthwise-separable, 16 channels at 112 x 112) of every backbone run as one kernel
+    // that reads the image once — the three largest activations never reach HBM.  Each unit's walk starts at block 1.
     const bool fuse_stem = h->fuse_xdw;                           // every backbone starts with a DS block
-    if (!fuse_stem && n_present == 3) {   // all three stems in one pass over the image (it is the only tensor the backbones share)
+    if (fuse_stem) {
+        smk::StemDsProblem sp[3];
+        int n = 0;
+        for (int i = 0; i < 3; ++i) {
+            if (!h->present[i]) continue;
+            const enc::Backbone& bb = h->bb[i];
+            const Block& b0 = bb.blocks[0];
+            sp[n++] = smk::StemDsProblem{bb.stem.fwd.w, bb.stem.scale, bb.stem.bias, b0.dw.fwd.w, b0.dw.scale, b0.dw.bias,
+                                         b0.pw_f32.w, b0.pw.scale, b0.pw.bias, bufs[i][0], SV(bb.sv_stem), SV(b0.sv_a), b0.stride};
+        }
+        if (int rc = smk::stem_ds(img, B, 224, 224, sp, n, h->x3 ? 0 : 1, main_st)) return rc;
+    } else if (n_present == 3) {   // all three stems in one pass over the image (it is the only tensor the backbones share)
         const float* sw[3]; const float* ss[3]; const float* sb[3]; float* so[3];
         for (int i = 0; i < 3; ++i) { sw[i] = h->bb[i].stem.fwd.w; ss[i] = h->bb[i].stem.scale; sb[i] = h->bb[i].stem.bias; so[i] = stem_out[i]; }
         if (int rc = smk::stem_conv3(img, B, 224, 224, sw, ss, sb, so, main_st)) return rc;
-    } else if (!fuse_stem) {
+    } else {
         for (int i = 0; i < 3; ++i)
             if (h->present[i]) { if (int rc = smk::stem_conv(img, B, 224, 224, h->bb[i].stem.fwd.w, h->bb[i].stem.scale, h->bb[i].stem.bias, stem_out[i], main_st)) return rc; }
     }
@@ -182,17 +193,9 @@ static int encoder_forward(const SmkEncoder* h, const float* img, int B, float* 
         }
         int res = 112;
         size_t first = 0;
-        if (fuse_stem) {
-            const Block& b0 = bb[0]->blocks[0];
-            smk::StemDsProblem sp[2];
-            for (int k = 0; k < n; ++k) {
-                const Block& bk = bb[k]->blocks[0];
-                sp[k] = smk::StemDsProblem{bb[k]->stem.fwd.w, bb[k]->stem.scale, bb[k]->stem.bias, bk.dw.fwd.w, bk.dw.scale, bk.dw.bias,
-                                           bk.pw_f32.w, bk.pw.scale, bk.pw.bias, x[k], SV(bb[k]->sv_stem), SV(bk.sv_a)};
-                cur[k] = x[k];
-            }
-            rc = smk::stem_ds(img, B, 224, 224, sp, n, b0.stride, h->x3 ? 0 : 1, st);
-            res = 112 / b0.stride; first = 1;
+        if (fuse_stem) {                                  // block 0's output is in x
+            for (int k = 0; k < n; ++k) cur[k] = x[k];
+            res = 112 / bb[0]->blocks[0].stride; first = 1;
         }
         for (size_t bi = first; bi < bb[0]->blocks.size() && !rc; ++bi) {
             const Block* b[2] = {&bb[0]->blocks[bi], &bb[n - 1]->blocks[bi]};

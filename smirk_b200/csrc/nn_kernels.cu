@@ -482,123 +482,64 @@ int stem_conv3(const float* img, int B, int H, int W, const float* const w[3], c
 // conv_stem 3x3 s2 (3 -> 16) + BN + ReLU  ->  block 0 of tf_mobilenetv3_*_minimal_100, a depthwise-separable
 // block (depthwise 3x3 s{1,2} + BN + ReLU -> 1x1 16 -> 16 + BN, + skip when stride 1); reference
 // src/smirk_encoder.py:7-12 -> timm MobileNetV3.conv_stem/bn1 + DepthwiseSeparableConv.  These are the three
-// largest activations of a backbone (112 x 112 x 16); unfused they cost a 96 MB stem pass plus a depthwise and
-// a 1x1 kernel per backbone.  Here a CTA owns a 16 x 16 tile of the stem output (+1 halo = 18 x 18):
-//   1. stage the 37 x 37 x 3 image patch in shared memory, even/odd columns de-interleaved so the stride-2 taps
-//      of neighbouring pixels hit neighbouring banks;
-//   2. stem conv: thread = two stem pixels x 16 channels (the tap weights, broadcast from shared memory, are
-//      used twice), BN + ReLU, zero outside the 112 x 112 map (= the depthwise conv's zero padding) -> S;
-//   3. depthwise 3x3 over S: thread = (pixel, channel quad), taps in registers, BN + ReLU -> D (aliases the patch);
-//   4. 1x1 conv on D: thread = (pixel, output-channel quad), 16 x 4 weights in registers, BN, + S (skip),
-//      optional TF32 rounding, one coalesced 16-byte store per thread.
-// All arithmetic is fp32 FMA in the reference's tap order; the image is the only HBM read, the block output the
-// only write.
+// largest activations of a backbone (112 x 112 x 16).  One launch runs every backbone the handle holds (up to three,
+// each with its own block-0 stride) from one pass over the image.  Persistent CTAs walk 16 x 16 tiles of the stem
+// output; a tile's stem region carries a one-pixel halo on every side (18 x 18, stem rows / columns 16 t - 1 ...
+// 16 t + 16), which covers the depthwise window of both strides (TF-SAME pads 1 before at stride 1, 0 at stride 2).
+//   1. the 37 x 37 x 3 image patch of the NEXT tile is fetched by 4-byte cp.async into the other half of a double
+//      buffer, rows and columns de-interleaved by parity (zero-filled outside the image), while this tile computes;
+//   2. stem convs: thread = (backbone, 4 stem pixels (sy, sx) + {0, 9} x {0, 9}) x 16 channels, 81 threads per
+//      backbone, BN + ReLU, zero outside the 112 x 112 map (= the depthwise conv's zero padding) -> S (one per backbone);
+//   3. per backbone: depthwise 3x3 over S: thread = (pixel, channel quad), taps in registers, BN + ReLU -> D (aliases
+//      the consumed patch);
+//   4. 1x1 conv on D: thread = (pixel, output-channel quad), BN, + S (skip), optional TF32 rounding, one coalesced
+//      16-byte store per thread.
+// All arithmetic is fp32 FMA in the reference's tap order; the image is the only HBM read, the block outputs the only
+// writes.
 namespace {
 constexpr int SD_T = 16, SD_ST = SD_T + 2;                 // stem-resolution tile edge, with halo
 constexpr int SD_PR = 2 * SD_ST + 1;                       // image patch rows / cols (37)
-constexpr int SD_PP = 20;                                  // patch row pitch per column parity (19 even + 18 odd columns)
-struct StemDs {                              // one or two backbones share a launch (blockIdx.z selects; both read the same image)
-    StemDsProblem q[2];
-    int round_out;
-};
+// Patch word of (channel c, row r, column x): [c][r & 1][r >> 1][x & 1][x >> 1], column-parity pitch SD_PC, row pitch
+// SD_PU.  SD_PU = 9 (mod 32): the quarter-grid pixel j = 9 sy + sx of a stem thread reads word SD_PU sy + sx + const,
+// so a warp's 32 threads of one backbone hit 32 consecutive banks on every tap.
+constexpr int SD_PC = 20, SD_PU = 41, SD_PH = (SD_PR + 1) / 2;
+constexpr int SD_PATCH = (3 * 2 * SD_PH * SD_PU + 3) / 4 * 4;  // floats per patch buffer (16-byte multiple: D is float4)
+constexpr int SD_STILE = SD_ST * SD_ST * 16;               // floats of one backbone's stem tile
+constexpr int SD_WK = 9 * 16 + 16 * 16;                    // depthwise taps + 1x1 weights of one backbone
+constexpr int SD_Q = SD_ST / 2;                            // stem threads per backbone: SD_Q x SD_Q, 4 pixels each
+constexpr int SD_SMEM = 4 * (2 * SD_PATCH + 3 * (SD_STILE + 27 * 16 + SD_WK + 6 * 16));
+static_assert(2 * (SD_SMEM + 1024) <= 228 * 1024, "stem_ds: shared memory of two resident CTAs");
+static_assert(SD_PC >= SD_PH && SD_PU >= SD_PC + SD_PH && SD_PU % 32 == SD_Q, "stem_ds: patch layout");
+static_assert(16 * 16 * 16 <= SD_PATCH && 3 * SD_Q * SD_Q <= 256, "stem_ds: D fits a patch buffer; one stem pass");
 
-// SAVE: also store the stem output of the tile's own 16 x 16 pixels (s_out) and the depthwise output (d_out), the ReLU
-// outputs the backward masks with.
+struct StemDs { StemDsProblem q[3]; int n, round_out; };
+
+__device__ __forceinline__ int sd_patch_idx(int c, int r, int x) {
+    return ((c * 2 + (r & 1)) * SD_PH + (r >> 1)) * SD_PU + (x & 1) * SD_PC + (x >> 1);
+}
+__device__ __forceinline__ void cp_async4(float* dst, const float* src, int src_bytes) {   // src_bytes 0: zero fill
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;\n" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src),
+                 "r"(src_bytes) : "memory");
+}
+
+// Steps 3 and 4 for one backbone.  S: its stem tile, K / Bv: its taps, weights, scales and biases, D: scratch.
 template <int STRIDE, bool SAVE>
-__global__ void __launch_bounds__(256, 3)
-stem_ds_kernel(const float* __restrict__ img, int H, int W, int Hs, int Ws, int pad, const __grid_constant__ StemDs pp) {
-    struct { const float *stem_w, *stem_s, *stem_b, *dw_w, *dw_s, *dw_b, *pw_w, *pw_s, *pw_b; float* out; int round_out; float *s_out, *d_out; } p;
-    {
-        const StemDsProblem& q = pp.q[blockIdx.z];
-        p.stem_w = q.stem_w; p.stem_s = q.stem_s; p.stem_b = q.stem_b; p.dw_w = q.dw_w; p.dw_s = q.dw_s; p.dw_b = q.dw_b;
-        p.pw_w = q.pw_w; p.pw_s = q.pw_s; p.pw_b = q.pw_b; p.out = q.out; p.round_out = pp.round_out;
-        if (SAVE) { p.s_out = q.s_out; p.d_out = q.d_out; }
-    }
-    constexpr int PADO = STRIDE == 1 ? 1 : 0;              // depthwise TF-SAME pad_begin on an even-sized map
-    constexpr int TO = SD_T / STRIDE;                      // output tile edge
-    __shared__ __align__(16) float sP[3 * SD_PR * 2 * SD_PP];          // image patch [c][row][parity][col/2]; later D [256][16]
-    __shared__ __align__(16) float sS[SD_ST * SD_ST * 16];             // stem tile [pixel][16]
-    __shared__ __align__(16) float sW[27 * 16];
-    __shared__ __align__(16) float sK[9 * 16 + 16 * 16];               // depthwise taps, 1x1 weights
-    __shared__ __align__(16) float sB[6 * 16];                         // stem / dw / pw scale, bias
-    const int tid = threadIdx.x, b = blockIdx.y;
-    const int tiles_x = Ws / SD_T;
-    const int ty = blockIdx.x / tiles_x, tx = blockIdx.x - ty * tiles_x;
-    const int sy0 = ty * SD_T - PADO, sx0 = tx * SD_T - PADO;          // stem-tile origin
-    const int iy0 = 2 * sy0 - pad, ix0 = 2 * sx0 - pad;                // image-patch origin
-    for (int i = tid; i < 27 * 16; i += 256) sW[i] = p.stem_w[i];
-    for (int i = tid; i < 9 * 16; i += 256) sK[i] = p.dw_w[i];
-    sK[9 * 16 + tid] = p.pw_w[tid];
-    if (tid < 16) {
-        sB[tid] = p.stem_s[tid]; sB[16 + tid] = p.stem_b[tid]; sB[32 + tid] = p.dw_s[tid]; sB[48 + tid] = p.dw_b[tid];
-        sB[64 + tid] = p.pw_s[tid]; sB[80 + tid] = p.pw_b[tid];
-    }
-    // ix0 and W are even: one 8-byte load fetches an (even, odd) column pair — exactly the de-interleaved layout.
-    // 19 pairs per row cover the 37 columns (the odd half of the last pair is never read).
-    constexpr int SD_PAIRS = (SD_PR + 1) / 2;
-#pragma unroll 4
-    for (int i = tid; i < 3 * SD_PR * SD_PAIRS; i += 256) {
-        const int row = i / SD_PAIRS, j = i - row * SD_PAIRS, c = row / SD_PR, r = row - c * SD_PR;
-        const int iy = iy0 + r, ix = ix0 + 2 * j;
-        float2 v = make_float2(0.f, 0.f);
-        if (iy >= 0 && iy < H && ix >= 0 && ix < W) v = __ldg(reinterpret_cast<const float2*>(img + (((size_t)b * 3 + c) * H + iy) * W + ix));
-        sP[(row * 2) * SD_PP + j] = v.x;
-        sP[(row * 2 + 1) * SD_PP + j] = v.y;
-    }
-    __syncthreads();
-    // -- 2. stem conv: pixels (syp, sx) and (syp + 9, sx)
-    if (tid < SD_ST * SD_ST / 2) {
-        const int syp = tid / SD_ST, sx = tid - syp * SD_ST;
-        float4 a0[4], a1[4];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) a0[q] = a1[q] = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-        for (int c = 0; c < 3; ++c)
-#pragma unroll
-            for (int ky = 0; ky < 3; ++ky)
-#pragma unroll
-                for (int kx = 0; kx < 3; ++kx) {
-                    const int off = (kx & 1) * SD_PP + sx + (kx >> 1);
-                    const float x0 = sP[(c * SD_PR + 2 * syp + ky) * 2 * SD_PP + off];
-                    const float x1 = sP[(c * SD_PR + 2 * (syp + SD_ST / 2) + ky) * 2 * SD_PP + off];
-                    const float4* wk = reinterpret_cast<const float4*>(sW + ((c * 3 + ky) * 3 + kx) * 16);
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) { const float4 w4 = wk[q]; fma4_s(a0[q], x0, w4); fma4_s(a1[q], x1, w4); }
-                }
-        const bool in_x = sx0 + sx >= 0 && sx0 + sx < Ws;
-        const bool v0 = in_x && sy0 + syp >= 0 && sy0 + syp < Hs;
-        const bool v1 = in_x && sy0 + syp + SD_ST / 2 >= 0 && sy0 + syp + SD_ST / 2 < Hs;
-        float4* s0 = reinterpret_cast<float4*>(sS + (syp * SD_ST + sx) * 16);
-        float4* s1 = reinterpret_cast<float4*>(sS + ((syp + SD_ST / 2) * SD_ST + sx) * 16);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            const float4 sc = *reinterpret_cast<const float4*>(sB + 4 * q), bi = *reinterpret_cast<const float4*>(sB + 16 + 4 * q);
-            float4 o0 = fma4(a0[q], sc, bi), o1 = fma4(a1[q], sc, bi);
-            o0.x = v0 ? fmaxf(o0.x, 0.f) : 0.f; o0.y = v0 ? fmaxf(o0.y, 0.f) : 0.f; o0.z = v0 ? fmaxf(o0.z, 0.f) : 0.f; o0.w = v0 ? fmaxf(o0.w, 0.f) : 0.f;
-            o1.x = v1 ? fmaxf(o1.x, 0.f) : 0.f; o1.y = v1 ? fmaxf(o1.y, 0.f) : 0.f; o1.z = v1 ? fmaxf(o1.z, 0.f) : 0.f; o1.w = v1 ? fmaxf(o1.w, 0.f) : 0.f;
-            s0[q] = o0; s1[q] = o1;
-            if (SAVE) {                                    // the tile's own pixels: stem rows / columns [PADO, PADO + 16) of S
-                const bool own_x = sx >= PADO && sx < PADO + SD_T;
-                if (own_x && syp >= PADO)
-                    reinterpret_cast<float4*>(p.s_out + (((size_t)b * Hs + sy0 + syp) * Ws + sx0 + sx) * 16)[q] = o0;
-                if (own_x && syp + SD_ST / 2 < PADO + SD_T)
-                    reinterpret_cast<float4*>(p.s_out + (((size_t)b * Hs + sy0 + syp + SD_ST / 2) * Ws + sx0 + sx) * 16)[q] = o1;
-            }
-        }
-    }
-    __syncthreads();
-    // -- 3. depthwise 3x3: thread = (pixel, channel quad)
-    float* sD = sP;
-    const int q = tid & 3;
+__device__ __forceinline__ void sd_block(const StemDsProblem& p, const float* S, const float* K, const float* Bv, float* D,
+                                         int b, int ty, int tx, int Hs, int Ws, int round_out) {
+    constexpr int TO = SD_T / STRIDE, NJ = TO * TO / 64;  // output tile edge, pixels per thread
+    constexpr int O = STRIDE - 1;                         // local stem row / column of the depthwise window's first tap
+    const int tid = threadIdx.x, q = tid & 3;
+    const int Ho = Hs / STRIDE, Wo = Ws / STRIDE;
+    __syncthreads();                                      // S complete; D's previous readers done
     {
         float4 k[9];
 #pragma unroll
-        for (int t = 0; t < 9; ++t) k[t] = *reinterpret_cast<const float4*>(sK + t * 16 + 4 * q);
-        const float4 sc = *reinterpret_cast<const float4*>(sB + 32 + 4 * q), bi = *reinterpret_cast<const float4*>(sB + 48 + 4 * q);
+        for (int t = 0; t < 9; ++t) k[t] = *reinterpret_cast<const float4*>(K + t * 16 + 4 * q);
+        const float4 sc = *reinterpret_cast<const float4*>(Bv + 32 + 4 * q), bi = *reinterpret_cast<const float4*>(Bv + 48 + 4 * q);
 #pragma unroll
-        for (int j = 0; j < TO * TO / 64; ++j) {
+        for (int j = 0; j < NJ; ++j) {
             const int px = (tid >> 2) + 64 * j, oy = px / TO, ox = px - oy * TO;
-            const float* s = sS + ((oy * STRIDE) * SD_ST + ox * STRIDE) * 16 + 4 * q;
+            const float* s = S + ((oy * STRIDE + O) * SD_ST + ox * STRIDE + O) * 16 + 4 * q;
             float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
             for (int ky = 0; ky < 3; ++ky)
@@ -607,17 +548,14 @@ stem_ds_kernel(const float* __restrict__ img, int H, int W, int Hs, int Ws, int 
                     fma4_acc(acc, *reinterpret_cast<const float4*>(s + (ky * SD_ST + kx) * 16), k[ky * 3 + kx]);
             float4 o = fma4(acc, sc, bi);
             o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
-            *reinterpret_cast<float4*>(sD + px * 16 + 4 * q) = o;
+            *reinterpret_cast<float4*>(D + px * 16 + 4 * q) = o;
             if (SAVE)
-                *reinterpret_cast<float4*>(p.d_out + (((size_t)b * (Hs / STRIDE) + ty * TO + oy) * (Ws / STRIDE) + tx * TO + ox) * 16 + 4 * q) = o;
+                *reinterpret_cast<float4*>(p.d_out + (((size_t)b * Ho + ty * TO + oy) * Wo + tx * TO + ox) * 16 + 4 * q) = o;
         }
     }
     __syncthreads();
-    // -- 4. 1x1 conv: thread = (pixel, output-channel quad)
     {
-        constexpr int NJ = TO * TO / 64;                   // pixels per thread
-        const float4 sc = *reinterpret_cast<const float4*>(sB + 64 + 4 * q), bi = *reinterpret_cast<const float4*>(sB + 80 + 4 * q);
-        const int Ho = Hs / STRIDE, Wo = Ws / STRIDE;
+        const float4 sc = *reinterpret_cast<const float4*>(Bv + 64 + 4 * q), bi = *reinterpret_cast<const float4*>(Bv + 80 + 4 * q);
         float4 accs[NJ];
 #pragma unroll
         for (int j = 0; j < NJ; ++j) accs[j] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -625,10 +563,10 @@ stem_ds_kernel(const float* __restrict__ img, int H, int W, int Hs, int Ws, int 
         for (int g = 0; g < 4; ++g) {                      // four input channels at a time: their weights serve all NJ pixels
             float4 w[4];
 #pragma unroll
-            for (int ci = 0; ci < 4; ++ci) w[ci] = *reinterpret_cast<const float4*>(sK + 9 * 16 + (4 * g + ci) * 16 + 4 * q);
+            for (int ci = 0; ci < 4; ++ci) w[ci] = *reinterpret_cast<const float4*>(K + 9 * 16 + (4 * g + ci) * 16 + 4 * q);
 #pragma unroll
             for (int j = 0; j < NJ; ++j) {
-                const float4 d = *reinterpret_cast<const float4*>(sD + ((tid >> 2) + 64 * j) * 16 + 4 * g);
+                const float4 d = *reinterpret_cast<const float4*>(D + ((tid >> 2) + 64 * j) * 16 + 4 * g);
                 fma4_s(accs[j], d.x, w[0]); fma4_s(accs[j], d.y, w[1]); fma4_s(accs[j], d.z, w[2]); fma4_s(accs[j], d.w, w[3]);
             }
         }
@@ -637,39 +575,140 @@ stem_ds_kernel(const float* __restrict__ img, int H, int W, int Hs, int Ws, int 
             const int px = (tid >> 2) + 64 * j, oy = px / TO, ox = px - oy * TO;
             float4 o = fma4(accs[j], sc, bi);
             if (STRIDE == 1) {                             // skip connection: block input = stem output at the same pixel
-                const float4 r = *reinterpret_cast<const float4*>(sS + ((oy + 1) * SD_ST + ox + 1) * 16 + 4 * q);
+                const float4 r = *reinterpret_cast<const float4*>(S + ((oy + 1) * SD_ST + ox + 1) * 16 + 4 * q);
                 o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
             }
-            if (p.round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
-            const int oh = ty * TO + oy, ow = tx * TO + ox;
-            *reinterpret_cast<float4*>(p.out + (((size_t)b * Ho + oh) * Wo + ow) * 16 + 4 * q) = o;
+            if (round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
+            *reinterpret_cast<float4*>(p.out + (((size_t)b * Ho + ty * TO + oy) * Wo + tx * TO + ox) * 16 + 4 * q) = o;
+        }
+    }
+}
+
+// SAVE: also store the stem output of the tile's own 16 x 16 pixels (s_out) and the depthwise output (d_out), the ReLU
+// outputs the backward masks with.
+template <bool SAVE>
+__global__ void __launch_bounds__(256, 2)
+stem_ds_kernel(const float* __restrict__ img, int H, int W, int Hs, int Ws, int pad, int n_tiles, const __grid_constant__ StemDs pp) {
+    extern __shared__ __align__(16) float sd_smem[];
+    float* sP = sd_smem;                                   // [2][SD_PATCH] image patches; the consumed one is D
+    float* sS = sP + 2 * SD_PATCH;                         // [3][SD_ST * SD_ST][16] stem tiles
+    float* sW = sS + 3 * SD_STILE;                         // [3][27][16] stem weights
+    float* sK = sW + 3 * 27 * 16;                          // [3][SD_WK] depthwise taps, 1x1 weights [ci][co]
+    float* sB = sK + 3 * SD_WK;                            // [3][6][16] stem / dw / pw scale, bias
+    const int tid = threadIdx.x, n = pp.n;
+    for (int g = 0; g < n; ++g) {
+        const StemDsProblem& p = pp.q[g];
+        for (int i = tid; i < 27 * 16; i += 256) sW[g * 27 * 16 + i] = p.stem_w[i];
+        for (int i = tid; i < 9 * 16; i += 256) sK[g * SD_WK + i] = p.dw_w[i];
+        sK[g * SD_WK + 9 * 16 + tid] = p.pw_w[tid];
+        if (tid < 16) {
+            float* B6 = sB + g * 96;
+            B6[tid] = p.stem_s[tid]; B6[16 + tid] = p.stem_b[tid]; B6[32 + tid] = p.dw_s[tid]; B6[48 + tid] = p.dw_b[tid];
+            B6[64 + tid] = p.pw_s[tid]; B6[80 + tid] = p.pw_b[tid];
+        }
+    }
+    const int tiles_x = Ws / SD_T, tiles_img = (Hs / SD_T) * tiles_x;
+    auto stage = [&](int t, float* dst) {                  // issue the patch of tile t (one cp.async group)
+        const int b = t / tiles_img, r = t - b * tiles_img, ty = r / tiles_x, tx = r - ty * tiles_x;
+        const int iy0 = 2 * (ty * SD_T - 1) - pad, ix0 = 2 * (tx * SD_T - 1) - pad;
+        for (int i = tid; i < 3 * SD_PR * SD_PR; i += 256) {
+            const int row = i / SD_PR, x = i - row * SD_PR, c = row / SD_PR, y = row - c * SD_PR;
+            const int iy = iy0 + y, ix = ix0 + x;
+            const bool in = iy >= 0 && iy < H && ix >= 0 && ix < W;
+            cp_async4(dst + sd_patch_idx(c, y, x), in ? img + (((size_t)b * 3 + c) * H + iy) * W + ix : img, in ? 4 : 0);
+        }
+        asm volatile("cp.async.commit_group;\n" ::: "memory");
+    };
+    int buf = 0;
+    if ((int)blockIdx.x < n_tiles) stage(blockIdx.x, sP);
+    for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, buf ^= 1) {
+        const int b = t / tiles_img, r = t - b * tiles_img, ty = r / tiles_x, tx = r - ty * tiles_x;
+        const int sy0 = ty * SD_T - 1, sx0 = tx * SD_T - 1;          // stem-tile origin
+        float* P = sP + buf * SD_PATCH;
+        asm volatile("cp.async.wait_group 0;\n" ::: "memory");
+        __syncthreads();                                   // this tile's patch landed; the previous tile is done with S / D
+        if (t + (int)gridDim.x < n_tiles) stage(t + gridDim.x, sP + (buf ^ 1) * SD_PATCH);
+        // -- 2. stem convs
+        if (tid < n * SD_Q * SD_Q) {
+            const int g = tid / (SD_Q * SD_Q), j = tid - g * (SD_Q * SD_Q), sy = j / SD_Q, sx = j - sy * SD_Q;
+            const float* Wg = sW + g * 27 * 16;
+            float4 a[4][4];                                // [pixel (dy, dx) = (a >> 1, a & 1) * SD_Q][channel quad]
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int qq = 0; qq < 4; ++qq) a[i][qq] = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+            for (int c = 0; c < 3; ++c)
+#pragma unroll
+                for (int ky = 0; ky < 3; ++ky)
+#pragma unroll
+                    for (int kx = 0; kx < 3; ++kx) {
+                        const float* x0 = P + sd_patch_idx(c, 2 * sy + ky, 2 * sx + kx);
+                        float x[4];
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) x[i] = x0[(i >> 1) * SD_Q * SD_PU + (i & 1) * SD_Q];
+                        const float4* wk = reinterpret_cast<const float4*>(Wg + ((c * 3 + ky) * 3 + kx) * 16);
+#pragma unroll
+                        for (int qq = 0; qq < 4; ++qq) {
+                            const float4 w4 = wk[qq];
+#pragma unroll
+                            for (int i = 0; i < 4; ++i) fma4_s(a[i][qq], x[i], w4);
+                        }
+                    }
+            const float* Bg = sB + g * 96;
+            float* Sg = sS + g * SD_STILE;
+            float* s_out = SAVE ? pp.q[g].s_out : nullptr;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int ly = sy + (i >> 1) * SD_Q, lx = sx + (i & 1) * SD_Q;           // local stem pixel
+                const int gy = sy0 + ly, gx = sx0 + lx;
+                const bool v = gy >= 0 && gy < Hs && gx >= 0 && gx < Ws;
+                const bool own = ly >= 1 && ly <= SD_T && lx >= 1 && lx <= SD_T;
+#pragma unroll
+                for (int qq = 0; qq < 4; ++qq) {
+                    const float4 sc = *reinterpret_cast<const float4*>(Bg + 4 * qq), bi = *reinterpret_cast<const float4*>(Bg + 16 + 4 * qq);
+                    float4 o = fma4(a[i][qq], sc, bi);
+                    o.x = v ? fmaxf(o.x, 0.f) : 0.f; o.y = v ? fmaxf(o.y, 0.f) : 0.f; o.z = v ? fmaxf(o.z, 0.f) : 0.f; o.w = v ? fmaxf(o.w, 0.f) : 0.f;
+                    reinterpret_cast<float4*>(Sg + (ly * SD_ST + lx) * 16)[qq] = o;
+                    if (SAVE && own) reinterpret_cast<float4*>(s_out + (((size_t)b * Hs + gy) * Ws + gx) * 16)[qq] = o;
+                }
+            }
+        }
+        // -- 3, 4. depthwise + 1x1 per backbone
+        for (int g = 0; g < n; ++g) {
+            if (pp.q[g].stride == 1)
+                sd_block<1, SAVE>(pp.q[g], sS + g * SD_STILE, sK + g * SD_WK, sB + g * 96, P, b, ty, tx, Hs, Ws, pp.round_out);
+            else
+                sd_block<2, SAVE>(pp.q[g], sS + g * SD_STILE, sK + g * SD_WK, sB + g * 96, P, b, ty, tx, Hs, Ws, pp.round_out);
         }
     }
 }
 }  // namespace
 
-int stem_ds(const float* img, int B, int H, int W, const StemDsProblem* probs, int n, int stride, int round_out, cudaStream_t st) {
+int stem_ds(const float* img, int B, int H, int W, const StemDsProblem* probs, int n, int round_out, cudaStream_t st) {
     const int Hs = (H + 1) / 2, Ws = (W + 1) / 2;
-    SMK_REQUIRE(n == 1 || n == 2, "stem_ds: one or two backbones per launch");
-    SMK_REQUIRE(stride == 1 || stride == 2, "stem_ds: stride must be 1 or 2");
+    SMK_REQUIRE(n >= 1 && n <= 3, "stem_ds: one to three backbones per launch");
     SMK_REQUIRE(H % 2 == 0 && W % 2 == 0 && Hs % SD_T == 0 && Ws % SD_T == 0, "stem_ds: image size %dx%d must be a multiple of 32", H, W);
-    SMK_REQUIRE(((uintptr_t)img & 7) == 0, "stem_ds: image pointer must be 8-byte aligned");
     const bool save = probs[0].s_out != nullptr;
-    SMK_REQUIRE(((probs[0].s_out && probs[0].d_out) || (!probs[0].s_out && !probs[0].d_out)) &&
-                (!probs[n - 1].s_out == !save) && (!probs[n - 1].d_out == !save), "stem_ds: s_out and d_out are given together, for every problem or none");
     StemDs p{};
-    p.q[0] = probs[0]; p.q[1] = probs[n - 1]; p.round_out = round_out;
-    const double px_o = (double)B * (Hs / stride) * (Ws / stride);
-    SMK_TAG("stem_ds_fused", 4.0 * ((double)B * 3 * H * W + n * (px_o * 16 + 27 * 16 + 9 * 16 + 256 + 96)),
-            n * 2.0 * ((double)B * Hs * Ws * 16 * 27 + px_o * 16 * (9 + 16)), st);
-    dim3 grid((Hs / SD_T) * (Ws / SD_T), B, n);
-    if (save) {
-        if (stride == 1) SMK_LAUNCH((stem_ds_kernel<1, true>), grid, dim3(256), 0, st, img, H, W, Hs, Ws, same_pad_begin(H, 2), p);
-        else SMK_LAUNCH((stem_ds_kernel<2, true>), grid, dim3(256), 0, st, img, H, W, Hs, Ws, same_pad_begin(H, 2), p);
-    } else {
-        if (stride == 1) SMK_LAUNCH((stem_ds_kernel<1, false>), grid, dim3(256), 0, st, img, H, W, Hs, Ws, same_pad_begin(H, 2), p);
-        else SMK_LAUNCH((stem_ds_kernel<2, false>), grid, dim3(256), 0, st, img, H, W, Hs, Ws, same_pad_begin(H, 2), p);
+    double bytes = 4.0 * B * 3 * H * W, flops = 0;
+    for (int k = 0; k < n; ++k) {
+        const StemDsProblem& q = probs[k];
+        SMK_REQUIRE(q.stride == 1 || q.stride == 2, "stem_ds: stride must be 1 or 2");
+        SMK_REQUIRE(!q.s_out == !save && !q.d_out == !save, "stem_ds: s_out and d_out are given together, for every problem or none");
+        p.q[k] = q;
+        const double px_o = (double)B * (Hs / q.stride) * (Ws / q.stride);
+        bytes += 4.0 * (px_o * 16 + 27 * 16 + 9 * 16 + 256 + 96);
+        flops += 2.0 * ((double)B * Hs * Ws * 16 * 27 + px_o * 16 * (9 + 16));
     }
+    p.n = n; p.round_out = round_out;
+    const int n_tiles = B * (Hs / SD_T) * (Ws / SD_T);
+    SMK_CHECK_CUDA(set_max_dynamic_smem<stem_ds_kernel<true>>(SD_SMEM));
+    SMK_CHECK_CUDA(set_max_dynamic_smem<stem_ds_kernel<false>>(SD_SMEM));
+    SMK_TAG("stem_ds_fused", bytes, flops, st);
+    const dim3 grid((unsigned)std::min(n_tiles, 2 * num_sms()));
+    if (save) SMK_LAUNCH(stem_ds_kernel<true>, grid, dim3(256), SD_SMEM, st, img, H, W, Hs, Ws, same_pad_begin(H, 2), n_tiles, p);
+    else SMK_LAUNCH(stem_ds_kernel<false>, grid, dim3(256), SD_SMEM, st, img, H, W, Hs, Ws, same_pad_begin(H, 2), n_tiles, p);
     SMK_CHECK_LAUNCH();
     return 0;
 }
@@ -738,6 +777,6 @@ extern "C" int smk_debug_stem_ds(const float* img, int B, int H, int W, const fl
                                  const float* pw_b, int stride, int round_out, float* out, void* stream) {
     if (B == 0) return 0;
     SMK_REQUIRE(img && stem_w && stem_s && stem_b && dw_w && dw_s && dw_b && pw_w && pw_s && pw_b && out, "smk_debug_stem_ds: null argument");
-    const smk::StemDsProblem q{stem_w, stem_s, stem_b, dw_w, dw_s, dw_b, pw_w, pw_s, pw_b, out};
-    return smk::stem_ds(img, B, H, W, &q, 1, stride, round_out, (cudaStream_t)stream);
+    const smk::StemDsProblem q{stem_w, stem_s, stem_b, dw_w, dw_s, dw_b, pw_w, pw_s, pw_b, out, nullptr, nullptr, stride};
+    return smk::stem_ds(img, B, H, W, &q, 1, round_out, (cudaStream_t)stream);
 }

@@ -25,9 +25,10 @@ struct StemDsProblem {
     const float* pw_w; const float* pw_s; const float* pw_b;            // [16 ci][16 co]
     float* out;
     float* s_out; float* d_out;          // optional, together: also store the stem output [B,112,112,16] and the depthwise output
+    int stride;                          // of block 0's depthwise conv: 1 or 2
 };
-// n = 1 or 2 backbones of the same block-0 stride in one launch (they read the same image).
-int stem_ds(const float* img_nchw, int B, int H, int W, const StemDsProblem* probs, int n, int stride, int round_out, cudaStream_t st);
+// n = 1 to 3 backbones in one launch, each with its own stride; the image is read once for all of them.
+int stem_ds(const float* img_nchw, int B, int H, int W, const StemDsProblem* probs, int n, int round_out, cudaStream_t st);
 int maxpool2x2(const float* in, int ld_in, int B, int H, int W, int C, float* out, cudaStream_t st);
 // NCHW -> NHWC with the channel count zero-padded to Cp (a multiple of 4); round_out rounds to TF32 for a tensor-core consumer.
 int nchw_to_nhwc_pad(const float* in, int B, int C, int H, int W, int Cp, float* out, cudaStream_t st, bool round_out = false);
