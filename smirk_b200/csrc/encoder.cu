@@ -31,11 +31,11 @@ constexpr float kBnEps = 1e-3f;
 // Consumes (conv weight, bn gamma, beta, mean, var) from the tensor list: the folded BN scale s and bias, the forward
 // weights, and the dgrad weights, which carry s.
 //   kind 0 = 1x1 [Cout,Cin,1,1]: smk::pack_gemm operands, the forward's N = cout, K = cin, the dgrad's (diag(s) W)^T,
-//            N = cin, K = cout.  f32 (optional): an fp32 copy of the forward weights as well.
+//            N = cin, K = cout.  fwd_f32: the forward weights in fp32 even when tc (a DS block's 1x1 that stem_ds runs).
 //   kind 1 = depthwise [C,1,3,3] -> W[9][C]; dgrad: flipped taps, Wd[8 - k][c] = s[c] W[c][k]
 //   kind 2 = stem [16,3,3,3] -> W[27][16]; dgrad: Wd[k][o] = s[o] W[o][k] (the forward layout)
 bool fold_conv(TensorCursor& cur, int kind, int cin, int cout, bool tc, bool x3, smk::DeviceArena& arena, ConvW* out, cudaError_t* err,
-               smk::GemmW* f32 = nullptr) {
+               bool fwd_f32 = false) {
     const float* w = cur.next(); const float* g = cur.next(); const float* b = cur.next();
     const float* mu = cur.next(); const float* var = cur.next();
     if (!w || !g || !b || !mu || !var) return false;
@@ -45,9 +45,8 @@ bool fold_conv(TensorCursor& cur, int kind, int cin, int cout, bool tc, bool x3,
     cudaError_t e = arena.upload(S, &out->scale);
     if (e == cudaSuccess) e = arena.upload(Bi, &out->bias);
     if (kind == 0) {                                          // torch's [Cout][Cin] is the forward's [N][K]
-        if (e == cudaSuccess) e = smk::pack_gemm(arena, cout, cin, tc, x3, w, &out->fwd);
+        if (e == cudaSuccess) e = smk::pack_gemm(arena, cout, cin, tc && !fwd_f32, x3, w, &out->fwd);
         if (e == cudaSuccess) e = smk::pack_gemm(arena, cin, cout, tc, x3, [&](int c, int o) { return S[o] * w[(size_t)o * cin + c]; }, &out->dgrad);
-        if (e == cudaSuccess && f32) e = smk::pack_gemm(arena, cout, cin, false, false, w, f32);
     } else {
         const int K = kind == 1 ? 9 : 27;
         std::vector<float> W((size_t)K * cout), D(W.size());
@@ -64,6 +63,9 @@ bool fold_conv(TensorCursor& cur, int kind, int cin, int cout, bool tc, bool x3,
     *err = e;
     return e == cudaSuccess;
 }
+
+// Stem + block 0 run as one fp32 kernel (stem_ds) at every precision but 1, whose block-0 1x1 runs on TF32 tensor cores.
+bool fuse_stem(const SmkEncoder* h) { return h->precision == 0 || h->fuse_xdw; }
 
 }  // namespace
 
@@ -92,7 +94,7 @@ extern "C" int smk_encoder_create(const SmkEncoderDesc* desc, SmkEncoder** out) 
             if (!ok) break;
             if (b.kind == DS) {
                 ok = fold_conv(cur, 1, b.cin, b.cin, false, false, h->arena, &b.dw, &e) &&
-                     fold_conv(cur, 0, b.cin, b.cout, tc, x3, h->arena, &b.pw, &e, tc ? &b.pw_f32 : nullptr);
+                     fold_conv(cur, 0, b.cin, b.cout, tc, x3, h->arena, &b.pw, &e, fuse_stem(h));
                 b.sv_a = add(b.path + ".bn1", b.hout, b.cin);
             } else if (b.kind == IR) {
                 ok = fold_conv(cur, 0, b.cin, b.mid, tc, x3, h->arena, &b.pw, &e) &&
@@ -155,32 +157,26 @@ static int encoder_forward(const SmkEncoder* h, const float* img, int B, float* 
     SMK_REQUIRE(bufs[2][3] != nullptr, "smk_encoder_forward: workspace carve-up failed");
     float* outs[3] = {pose_cam, shape, expr};
     auto SV = [&](int i) -> float* { return sv ? sv + (size_t)B * h->saved.off[i] : nullptr; };
-    float* stem_out[3];                                           // where each backbone's stem writes
-    for (int i = 0; i < 3; ++i) stem_out[i] = sv && h->present[i] ? SV(h->bb[i].sv_stem) : bufs[i][0];
-    const int n_present = (int)h->present[0] + (int)h->present[1] + (int)h->present[2];
-    // precision 2: stem + block 0 (depthwise-separable, 16 channels at 112 x 112) of every backbone run as one kernel
-    // that reads the image once — the three largest activations never reach HBM.  Each unit's walk starts at block 1.
-    const bool fuse_stem = h->fuse_xdw;                           // every backbone starts with a DS block
-    if (fuse_stem) {
-        smk::StemDsProblem sp[3];
-        int n = 0;
-        for (int i = 0; i < 3; ++i) {
-            if (!h->present[i]) continue;
-            const enc::Backbone& bb = h->bb[i];
-            const Block& b0 = bb.blocks[0];
-            sp[n++] = smk::StemDsProblem{bb.stem.fwd.w, bb.stem.scale, bb.stem.bias, b0.dw.fwd.w, b0.dw.scale, b0.dw.bias,
-                                         b0.pw_f32.w, b0.pw.scale, b0.pw.bias, bufs[i][0], SV(bb.sv_stem), SV(b0.sv_a), b0.stride};
-        }
-        if (int rc = smk::stem_ds(img, B, 224, 224, sp, n, h->x3 ? 0 : 1, main_st)) return rc;
-    } else if (n_present == 3) {   // all three stems in one pass over the image (it is the only tensor the backbones share)
-        const float* sw[3]; const float* ss[3]; const float* sb[3]; float* so[3];
-        for (int i = 0; i < 3; ++i) { sw[i] = h->bb[i].stem.fwd.w; ss[i] = h->bb[i].stem.scale; sb[i] = h->bb[i].stem.bias; so[i] = stem_out[i]; }
-        if (int rc = smk::stem_conv3(img, B, 224, 224, sw, ss, sb, so, main_st)) return rc;
-    } else {
-        for (int i = 0; i < 3; ++i)
-            if (h->present[i]) { if (int rc = smk::stem_conv(img, B, 224, 224, h->bb[i].stem.fwd.w, h->bb[i].stem.scale, h->bb[i].stem.bias, stem_out[i], main_st)) return rc; }
+    const bool fused = fuse_stem(h);
+    const bool rnd = h->precision == 1 && !h->x3;                 // activations that feed a plain TF32 layer are rounded
+    // Before the fork, on main_st, one pass over the image (the only tensor the backbones share) for every backbone: stem
+    // + block 0 (depthwise-separable, 16 channels at 112 x 112) as one kernel, so the three largest activations never
+    // reach HBM and each unit's walk starts at block 1; at precision 1 the stems alone.
+    float* in0[3];                        // what the walk's first block reads: block 0's output, or the stem's
+    smk::StemDsProblem sp[3];
+    smk::StemProblem sq[3];
+    int n_present = 0;
+    for (int i = 0; i < 3; ++i) {
+        if (!h->present[i]) continue;
+        const Backbone& bb = h->bb[i];
+        const Block& b0 = bb.blocks[0];
+        in0[i] = sv && !fused ? SV(bb.sv_stem) : bufs[i][0];
+        sp[n_present] = smk::StemDsProblem{bb.stem.fwd.w, bb.stem.scale, bb.stem.bias, b0.dw.fwd.w, b0.dw.scale, b0.dw.bias,
+                                           b0.pw.fwd.w, b0.pw.scale, b0.pw.bias, in0[i], SV(bb.sv_stem), SV(b0.sv_a), b0.stride};
+        sq[n_present++] = smk::StemProblem{bb.stem.fwd.w, bb.stem.scale, bb.stem.bias, in0[i]};
     }
-    // the stems above run on main_st before the fork
+    if (int rc = fused ? smk::stem_ds(img, B, 224, 224, sp, n_present, rnd ? 1 : 0, main_st)
+                       : smk::stem_conv(img, B, 224, 224, sq, n_present, main_st)) return rc;
     return for_each_unit(h, h->present, main_st, "smk_encoder_forward", [&](const Unit& unit) {
         const int n = unit.n;
         cudaStream_t st = unit.st;
@@ -189,19 +185,14 @@ static int encoder_forward(const SmkEncoder* h, const float* img, int B, float* 
         const Backbone* bb[2]; float *x[2], *y[2], *e[2], *d[2], *cur[2];
         for (int k = 0; k < n; ++k) {
             const int i = unit.idx[k];
-            bb[k] = &h->bb[i]; x[k] = bufs[i][0]; y[k] = bufs[i][1]; e[k] = bufs[i][2]; d[k] = bufs[i][3]; cur[k] = stem_out[i];
+            bb[k] = &h->bb[i]; x[k] = bufs[i][0]; y[k] = bufs[i][1]; e[k] = bufs[i][2]; d[k] = bufs[i][3]; cur[k] = in0[i];
         }
-        int res = 112;
-        size_t first = 0;
-        if (fuse_stem) {                                  // block 0's output is in x
-            for (int k = 0; k < n; ++k) cur[k] = x[k];
-            res = 112 / bb[0]->blocks[0].stride; first = 1;
-        }
+        const size_t first = fused ? 1 : 0;
+        int res = 112 / (fused ? bb[0]->blocks[0].stride : 1);
         for (size_t bi = first; bi < bb[0]->blocks.size() && !rc; ++bi) {
             const Block* b[2] = {&bb[0]->blocks[bi], &bb[n - 1]->blocks[bi]};
             const Block& b0 = *b[0];
             const int ro = (res + b0.stride - 1) / b0.stride;
-            const bool rnd = h->precision == 1 && !h->x3;
             const ConvW* pw[2] = {&b[0]->pw, &b[1]->pw};
             const ConvW* pwl[2] = {&b[0]->pwl, &b[1]->pwl};
             float* out[2] = {y[0], y[1]};                // the block's output
@@ -212,7 +203,7 @@ static int encoder_forward(const SmkEncoder* h, const float* img, int B, float* 
                     else out[k] = SV(b[k]->sv_a);
                 }
             }
-            if (b0.kind == DS) {
+            if (b0.kind == DS) {                         // block 0 at precision 1 (stem_ds runs it at the others)
                 for (int k = 0; k < n && !rc; ++k)
                     rc = smk::dwconv3x3(cur[k], B, res, res, b[k]->cin, b[k]->stride, b[k]->dw.fwd.w, b[k]->dw.scale, b[k]->dw.bias, d[k], st, rnd);
                 if (!rc) rc = pointwise(n, pw, d, B, ro, ro, false, b0.skip ? cur : nullptr, out, st);

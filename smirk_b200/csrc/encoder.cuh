@@ -12,10 +12,9 @@ struct ConvW { smk::GemmW fwd{}, dgrad{}; float* scale = nullptr; float* bias = 
 enum Kind { DS = 0, IR = 1, CN = 2 };
 struct BlockDef { Kind kind; int stride; float exp; int cout; };
 // path: the block's module path, <encoder>.encoder.blocks.<stage>.<i>; hin / hout: input / output resolution.
-// pw_f32: fp32 [K][N] copy of a DS block's 1x1 forward weights (fused stem path; pw's scale and bias).
 // sv_a / sv_b: saved-tensor indices of the block's ReLU outputs (IR: expand, depthwise; DS: depthwise; CN: its output); eval handles.
 struct Block { Kind kind; int stride, cin, mid, cout; bool skip; std::string path; int hin, hout;
-               ConvW pw, dw, pwl; smk::GemmW pw_f32{}; int sv_a = -1, sv_b = -1; };
+               ConvW pw, dw, pwl; int sv_a = -1, sv_b = -1; };
 
 // Train handles walk a backbone as a flat list, in forward order, of conv + BatchNorm (+ skip) (+ ReLU) layers.  The stem is
 // entry 0, so the index is the BatchNorm's index in the tensor list (5 tensors per entry, one num_batches_tracked).

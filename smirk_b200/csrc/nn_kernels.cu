@@ -457,24 +457,24 @@ int dwconv3x3(const float* in, int B, int H, int W, int C, int stride, const flo
     return 0;
 }
 
-int stem_conv(const float* img, int B, int H, int W, const float* w, const float* scale, const float* bias, float* out,
-              cudaStream_t st) {
-    int Ho = (H + 1) / 2, Wo = (W + 1) / 2;
-    SMK_TAG("stem_conv", 4.0 * ((double)B * 3 * H * W + (double)B * Ho * Wo * 16 + 27 * 16 + 32), 2.0 * 27 * 16 * (double)B * Ho * Wo, st);
-    SMK_LAUNCH(stem_conv_kernel, dim3(cdiv((long)B * Ho * Wo, 128)), dim3(128), 0, st, img, B, H, W, Ho, Wo, same_pad_begin(H, 2), w, scale, bias, out);
-    SMK_CHECK_LAUNCH();
-    return 0;
-}
-
-int stem_conv3(const float* img, int B, int H, int W, const float* const w[3], const float* const scale[3],
-               const float* const bias[3], float* const out[3], cudaStream_t st) {
-    int Ho = (H + 1) / 2, Wo = (W + 1) / 2;
-    Stem3 p;
-    for (int g = 0; g < 3; ++g) { p.w[g] = w[g]; p.scale[g] = scale[g]; p.bias[g] = bias[g]; p.out[g] = out[g]; }
-    SMK_TAG("stem_conv3", 4.0 * ((double)B * 3 * H * W + (double)B * Ho * Wo * 48 + 27 * 48 + 96), 2.0 * 27 * 48 * (double)B * Ho * Wo, st);
-    SMK_REQUIRE(W % 4 == 0 && W + 8 <= STEM_MAXW && same_pad_begin(H, 2) <= 1, "stem_conv3: unsupported image width %d", W);
-    SMK_LAUNCH(stem_conv3_kernel, dim3(B * Ho), dim3(128), 0, st, img, B, H, W, Ho, Wo, same_pad_begin(H, 2), p);
-    SMK_CHECK_LAUNCH();
+int stem_conv(const float* img, int B, int H, int W, const StemProblem* probs, int n, cudaStream_t st) {
+    SMK_REQUIRE(n >= 1 && n <= 3, "stem_conv: one to three backbones");
+    const int Ho = (H + 1) / 2, Wo = (W + 1) / 2, pad = same_pad_begin(H, 2);
+    if (n == 3) {
+        Stem3 p;
+        for (int g = 0; g < 3; ++g) { p.w[g] = probs[g].w; p.scale[g] = probs[g].scale; p.bias[g] = probs[g].bias; p.out[g] = probs[g].out; }
+        SMK_TAG("stem_conv3", 4.0 * ((double)B * 3 * H * W + (double)B * Ho * Wo * 48 + 27 * 48 + 96), 2.0 * 27 * 48 * (double)B * Ho * Wo, st);
+        SMK_REQUIRE(W % 4 == 0 && W + 8 <= STEM_MAXW && pad <= 1, "stem_conv: unsupported image width %d", W);
+        SMK_LAUNCH(stem_conv3_kernel, dim3(B * Ho), dim3(128), 0, st, img, B, H, W, Ho, Wo, pad, p);
+        SMK_CHECK_LAUNCH();
+        return 0;
+    }
+    for (int g = 0; g < n; ++g) {
+        const StemProblem& q = probs[g];
+        SMK_TAG("stem_conv", 4.0 * ((double)B * 3 * H * W + (double)B * Ho * Wo * 16 + 27 * 16 + 32), 2.0 * 27 * 16 * (double)B * Ho * Wo, st);
+        SMK_LAUNCH(stem_conv_kernel, dim3(cdiv((long)B * Ho * Wo, 128)), dim3(128), 0, st, img, B, H, W, Ho, Wo, pad, q.w, q.scale, q.bias, q.out);
+        SMK_CHECK_LAUNCH();
+    }
     return 0;
 }
 

@@ -11,12 +11,11 @@ namespace smk {
 // Depthwise 3x3, TF-"SAME" padding (pad_beg = pad_total/2), stride 1 or 2, fused scale/bias/ReLU.
 int dwconv3x3(const float* in, int B, int H, int W, int C, int stride, const float* w9c /*[9][C]*/,
               const float* scale, const float* bias, float* out, cudaStream_t st, bool round_out = false);
-// Stem: NCHW fp32 image -> NHWC, 3x3 stride 2 TF-SAME, Cout = 16, fused scale/bias/ReLU.
-int stem_conv(const float* img_nchw, int B, int H, int W, const float* w /*[27][16]*/, const float* scale,
-              const float* bias, float* out, cudaStream_t st);
-// Three 16-channel stems over the same image in one pass (the encoder's three backbones).
-int stem_conv3(const float* img_nchw, int B, int H, int W, const float* const w[3], const float* const scale[3],
-               const float* const bias[3], float* const out[3], cudaStream_t st);
+// Stems (NCHW fp32 image -> NHWC, 3x3 stride 2 TF-SAME, Cout = 16, fused scale/bias/ReLU) of n = 1 to 3 backbones.  Three
+// run as one pass over the image (a CTA stages the input rows of one output row); fewer run a thread-per-pixel launch
+// each, which is faster for one backbone than the one-pass kernel.
+struct StemProblem { const float* w /*[27][16]*/; const float* scale; const float* bias; float* out; };
+int stem_conv(const float* img_nchw, int B, int H, int W, const StemProblem* probs, int n, cudaStream_t st);
 // Fused stem (3x3 s2, 3 -> 16, BN, ReLU) + depthwise-separable block 0 (dw 3x3 s{1,2} + BN + ReLU, 1x1 16 -> 16 + BN,
 // + skip when stride 1) of one backbone: image NCHW fp32 -> [B, 112/stride, 112/stride, 16] NHWC.  pw_w is [ci][co] fp32.
 struct StemDsProblem {

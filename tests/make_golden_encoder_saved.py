@@ -1,8 +1,9 @@
 """Writes tests/golden/encoder_saved_digests.json: SHA-256 digests of what the grad-mode encoder forward
-(``smk_encoder_forward_saved``, precision 3 as benched, seeded weights and images) returns on an H100 — the raw outputs of
-every backbone the module holds and every tensor of the saved-activation buffer — for SmirkEncoder and each sub-encoder alone at
-B = 1, 7 and 32.  The forward has no atomics and no data-dependent reduction order, so its bytes are a function of its
-inputs: a kernel change that keeps the arithmetic must keep every digest.
+(``smk_encoder_forward_saved``, seeded weights and images) returns on an H100 — the raw outputs of every backbone the module
+holds and every tensor of the saved-activation buffer — for SmirkEncoder and each sub-encoder alone at B = 1, 7 and 32, at
+every precision (0 fp32, 1 TF32 with the stem and block 0 unfused, 2 TF32, 3 3xTF32 as benched).  The forward has no
+atomics and no data-dependent reduction order, so its bytes are a function of its inputs: a kernel change that keeps the
+arithmetic must keep every digest.
 
 Re-run on an H100 at the commit whose bytes are the reference: ``python tests/make_golden_encoder_saved.py [out.json]``.
 """
@@ -20,14 +21,20 @@ from smirk_b200 import synth_inputs  # noqa: E402
 GOLD = os.path.join(HERE, "golden", "encoder_saved_digests.json")
 MODULES = ("SmirkEncoder", "PoseEncoder", "ShapeEncoder", "ExpressionEncoder")
 BATCHES = (1, 7, 32)
+PRECISIONS = (0, 1, 2, 3)
 
 
-def make_module(name, dev="cuda"):
+def key(precision, name, B):
+    """The digests' key; precision 3's carry no prefix."""
+    return "%s%s/B%d" % ("" if precision == 3 else "p%d/" % precision, name, B)
+
+
+def make_module(name, precision=3, dev="cuda"):
     from smirk_b200 import smirk_encoder
     m = getattr(smirk_encoder, name)()
     m.load_state_dict(synth_inputs.random_state_dict(m.state_dict(), seed=7))
     m = m.eval().requires_grad_(False).to(dev)
-    m.precision = 3
+    m.precision = precision
     return m
 
 
@@ -49,7 +56,7 @@ def digests(m, B):
 
 
 def all_digests():
-    return {"%s/B%d" % (name, B): digests(make_module(name), B) for name in MODULES for B in BATCHES}
+    return {key(p, name, B): digests(make_module(name, p), B) for p in PRECISIONS for name in MODULES for B in BATCHES}
 
 
 if __name__ == "__main__":
