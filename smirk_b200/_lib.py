@@ -1,4 +1,5 @@
-"""ctypes binding of libsmirk_b200.so (the C ABI declared in include/smirk_b200.h and include/smirk_b200_loss.h).
+"""ctypes binding of libsmirk_b200.so (the C ABI declared in include/smirk_b200.h, include/smirk_b200_loss.h,
+include/smirk_b200_mica.h and include/smirk_b200_expression.h).
 
 There is deliberately no fallback: if the shared library is missing or a call fails, the product
 path raises.  Build with ``python -m smirk_b200.build`` (or ``__graft_entry__.build()``).
@@ -60,6 +61,10 @@ class SmkVggLossDesc(C.Structure):
 
 
 class SmkMicaDesc(C.Structure):
+    _fields_ = [("tensors", C.POINTER(c_f32p)), ("n_tensors", C.c_int), ("precision", C.c_int)]
+
+
+class SmkExpressionLossDesc(C.Structure):
     _fields_ = [("tensors", C.POINTER(c_f32p)), ("n_tensors", C.c_int), ("precision", C.c_int)]
 
 
@@ -180,7 +185,20 @@ MICA_BINDINGS = [
     ("smk_mica_shape_loss_forward", _i, [_vp, _vp, _i, _i, _i, _vp, STREAM]),
     ("smk_mica_shape_loss_backward", _i, [_vp, _vp, _i, _i, _i, _vp, _vp, STREAM]),
 ]
-_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS + LOSS_BINDINGS + MICA_BINDINGS if args[-1:] == [STREAM])
+# The binding table of include/smirk_b200_expression.h (the emotion loss), in that header's order, by the same rules.
+EXPRESSION_BINDINGS = [
+    ("smk_expression_loss_create", _i, [C.POINTER(SmkExpressionLossDesc), _vpp]),
+    ("smk_expression_loss_destroy", None, [_vp]),
+    ("smk_expression_loss_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_expression_loss_forward", _i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_expression_loss_saved_bytes", _sz, [_vp, _i, _i]),
+    ("smk_expression_loss_forward_saved", _i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp, _sz, STREAM]),
+    ("smk_expression_loss_saved_tensor", _i, [_vp, _i, _i, _i, C.POINTER(C.c_char_p), C.POINTER(_sz), C.POINTER(C.c_int)]),
+    ("smk_expression_loss_backward_workspace_bytes", _sz, [_vp, _i, _i]),
+    ("smk_expression_loss_backward", _i, [_vp, _i, _i, _i, _i, _vp, _sz, _vp, _vp, _vp, _vp, _sz, STREAM]),
+]
+_ALL_BINDINGS = BINDINGS + LOSS_BINDINGS + MICA_BINDINGS + EXPRESSION_BINDINGS
+_TAKES_STREAM = frozenset(name for name, _, args in _ALL_BINDINGS if args[-1:] == [STREAM])
 
 
 def lib():
@@ -192,7 +210,7 @@ def lib():
         raise RuntimeError("smirk_b200: %s not found — build it with `python -m smirk_b200.build` "
                            "(there is no CPU / PyTorch fallback)" % LIB_PATH)
     L = C.CDLL(LIB_PATH)
-    for name, restype, argtypes in BINDINGS + LOSS_BINDINGS + MICA_BINDINGS:
+    for name, restype, argtypes in _ALL_BINDINGS:
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, [_vp if a is STREAM else a for a in argtypes]
     if L.smk_version() != 100:

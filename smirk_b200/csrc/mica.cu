@@ -15,7 +15,7 @@
 // bn1(x), not x), so the epilogue that writes a block's output y also writes bn1_next(y), the next conv1's input, as its
 // second store with its own affine (smk::Conv::scale2 / bias2); the stem and every conv1 apply their PReLU there too
 // (smk::Conv::prelu).  The stride-2 layers (four 3x3 and four 1x1, 3.8 % of the MACs) gather their receptive fields into a
-// dense [M, 9 Cin] (or [M, Cin]) matrix that a plain GEMM then reads (mica_gather_s2_kernel): one simple kernel serves the
+// dense [M, 9 Cin] (or [M, Cin]) matrix that a plain GEMM then reads (smk::gather_s2): one simple kernel serves the
 // fp32 and tensor-core paths alike, at the cost of one extra pass over those eight layers' inputs.
 //
 // Precision 1 rounds every stored activation that another tensor-core layer reads to TF32 (conv1's output, bn1(y), the
@@ -60,28 +60,6 @@ mica_prep_kernel(const float* __restrict__ x, int B, int HW, int Cp, int round, 
         v[k] = t;
     }
     reinterpret_cast<float4*>(out)[i] = make_float4(v[0], v[1], v[2], v[3]);
-}
-
-// Stride-2 receptive fields of in [B,H,W,C] as a dense matrix out [B*(H/2)*(W/2), taps*C]:
-//   taps 9: the 3x3 conv with zero padding 1, column (ky*3 + kx)*C + c = in[b, 2h+ky-1, 2w+kx-1, c] (0 outside);
-//   taps 1: the 1x1 conv, column c = in[b, 2h, 2w, c].
-__global__ void __launch_bounds__(256)
-mica_gather_s2_kernel(const float4* __restrict__ in, int B, int H, int W, int C, int taps, int round, float4* __restrict__ out) {
-    const int C4 = C >> 2, Ho = H >> 1, Wo = W >> 1;
-    const long total = (long)B * Ho * Wo * taps * C4;
-    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-        const int c4 = (int)(i % C4); long t = i / C4;
-        const int tap = (int)(t % taps); const long m = t / taps;
-        const int wo = (int)(m % Wo); const long t2 = m / Wo; const int ho = (int)(t2 % Ho); const int b = (int)(t2 / Ho);
-        const int ky = taps == 9 ? tap / 3 : 1, kx = taps == 9 ? tap % 3 : 1;
-        const int h = 2 * ho + ky - 1, w = 2 * wo + kx - 1;
-        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (h >= 0 && h < H && w >= 0 && w < W) {
-            v = __ldg(in + (((size_t)b * H + h) * W + w) * C4 + c4);
-            if (round) { v.x = smk::round_tf32(v.x); v.y = smk::round_tf32(v.y); v.z = smk::round_tf32(v.z); v.w = smk::round_tf32(v.w); }
-        }
-        out[i] = v;
-    }
 }
 
 // Sum over the 256 threads of a block in a fixed order; the result is valid in every thread.
@@ -302,12 +280,7 @@ const char* tag_of(int precision, const char* f32, const char* tc, const char* t
 }
 
 int gather_s2(const float* in, int B, int H, int C, int taps, bool round, float* out, cudaStream_t st) {
-    const long total = (long)B * (H / 2) * (H / 2) * taps * (C / 4);
-    SMK_TAG(taps == 9 ? "mica_gather3x3_s2" : "mica_gather1x1_s2", 4.0 * total * 4 + (taps == 9 ? 4.0 * B * H * H * C : total * 4.0 * 4), 0.0, st);
-    SMK_LAUNCH(mica_gather_s2_kernel, dim3(smk::grid_of(total)), dim3(256), 0, st, reinterpret_cast<const float4*>(in), B, H, H, C, taps,
-               round ? 1 : 0, reinterpret_cast<float4*>(out));
-    SMK_CHECK_LAUNCH();
-    return 0;
+    return smk::gather_s2(in, B, H, C, taps, round, out, taps == 9 ? "mica_gather3x3_s2" : "mica_gather1x1_s2", st);
 }
 
 }  // namespace
@@ -441,7 +414,7 @@ extern "C" int smk_debug_mica_conv(const float* in, int ld_in, int B, int H, int
     p.scale2 = scale2; p.bias2 = bias2; p.round_out2 = round_out2;
     return smk::conv(p, (cudaStream_t)stream);
 }
-// mica_gather_s2_kernel: in [B,H,H,C] -> out [B*(H/2)^2, taps*C], taps 9 (3x3, zero padding 1) or 1.
+// smk::gather_s2: in [B,H,H,C] -> out [B*(H/2)^2, taps*C], taps 9 (3x3, zero padding 1) or 1.
 extern "C" int smk_debug_mica_gather_s2(const float* in, int B, int H, int C, int taps, int round, float* out, void* stream) {
     SMK_REQUIRE(in && out && B > 0 && H % 2 == 0 && C % 4 == 0 && (taps == 1 || taps == 9), "smk_debug_mica_gather_s2: bad arguments");
     return gather_s2(in, B, H, C, taps, round != 0, out, (cudaStream_t)stream);

@@ -761,6 +761,41 @@ int gap_head(const GapHeadProblem* probs, int n, int B, int HW, int C, cudaStrea
     return 0;
 }
 
+namespace {
+
+// Stride-2 receptive fields of in [B,H,W,C] as a dense matrix out [B*(H/2)*(W/2), taps*C]:
+//   taps 9: the 3x3 conv with zero padding 1, column (ky*3 + kx)*C + c = in[b, 2h+ky-1, 2w+kx-1, c] (0 outside);
+//   taps 1: the 1x1 conv, column c = in[b, 2h, 2w, c].
+__global__ void __launch_bounds__(256)
+gather_s2_kernel(const float4* __restrict__ in, int B, int H, int W, int C, int taps, int round, float4* __restrict__ out) {
+    const int C4 = C >> 2, Ho = H >> 1, Wo = W >> 1;
+    const long total = (long)B * Ho * Wo * taps * C4;
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+        const int c4 = (int)(i % C4); long t = i / C4;
+        const int tap = (int)(t % taps); const long m = t / taps;
+        const int wo = (int)(m % Wo); const long t2 = m / Wo; const int ho = (int)(t2 % Ho); const int b = (int)(t2 / Ho);
+        const int ky = taps == 9 ? tap / 3 : 1, kx = taps == 9 ? tap % 3 : 1;
+        const int h = 2 * ho + ky - 1, w = 2 * wo + kx - 1;
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (h >= 0 && h < H && w >= 0 && w < W) {
+            v = __ldg(in + (((size_t)b * H + h) * W + w) * C4 + c4);
+            if (round) { v.x = round_tf32(v.x); v.y = round_tf32(v.y); v.z = round_tf32(v.z); v.w = round_tf32(v.w); }
+        }
+        out[i] = v;
+    }
+}
+
+}  // namespace
+
+int gather_s2(const float* in, int B, int H, int C, int taps, bool round, float* out, const char* tag, cudaStream_t st) {
+    const long total = (long)B * (H / 2) * (H / 2) * taps * (C / 4);
+    SMK_TAG(tag, 4.0 * total * 4 + (taps == 9 ? 4.0 * B * H * H * C : total * 4.0 * 4), 0.0, st);
+    SMK_LAUNCH(gather_s2_kernel, dim3(grid_of(total)), dim3(256), 0, st, reinterpret_cast<const float4*>(in), B, H, H, C, taps,
+               round ? 1 : 0, reinterpret_cast<float4*>(out));
+    SMK_CHECK_LAUNCH();
+    return 0;
+}
+
 }  // namespace smk
 
 extern "C" int smk_debug_conv_f32(const float* in, int ld_in, int B, int H, int W, int Cin, const float* w_kn, const float* scale,

@@ -2,7 +2,7 @@
 //
 // The fp32 implicit-GEMM convolution `conv_gemm` (precision 0; declared with its descriptor in conv.cuh) with fused
 // BN / ReLU / residual / pixel-shuffle epilogues, depthwise 3x3, the stem convolutions and the fused stem + first block,
-// 2x2 max-pool, layout conversion, the final 1x1 + sigmoid and the fused global-average-pool + linear heads.
+// 2x2 max-pool, the stride-2 gather, layout conversion, the final 1x1 + sigmoid and the fused global-average-pool + linear heads.
 #pragma once
 #include "conv.cuh"
 
@@ -29,6 +29,10 @@ struct StemDsProblem {
 // n = 1 to 3 backbones in one launch, each with its own stride; the image is read once for all of them.
 int stem_ds(const float* img_nchw, int B, int H, int W, const StemDsProblem* probs, int n, int round_out, cudaStream_t st);
 int maxpool2x2(const float* in, int ld_in, int B, int H, int W, int C, float* out, cudaStream_t st);
+// The receptive fields of a stride-2 conv (MICA's and the expression loss's stride-2 layers) as a dense matrix that a plain
+// GEMM reads: in [B,H,H,C] -> out [B*(H/2)^2, taps*C]; taps 9: 3x3 with zero padding 1, column (ky*3 + kx)*C + c; taps 1:
+// the 1x1 conv's even pixels.  round: TF32 for a TF32 consumer.  tag: the profiler tag of the launch.
+int gather_s2(const float* in, int B, int H, int C, int taps, bool round, float* out, const char* tag, cudaStream_t st);
 // NCHW -> NHWC with the channel count zero-padded to Cp (a multiple of 4); round_out rounds to TF32 for a tensor-core consumer.
 int nchw_to_nhwc_pad(const float* in, int B, int C, int H, int W, int Cp, float* out, cudaStream_t st, bool round_out = false);
 // out[b, co, h, w] = sigmoid(bias[co] + sum_c in[b,h,w,c] * w[c][co])   (NHWC -> NCHW)

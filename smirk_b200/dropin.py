@@ -7,7 +7,7 @@
 (``smirk_encoder.set_train_mode_default(True)``): the trainer's ``.train()`` encoder then runs with batch statistics
 and gets its weight gradients.  Without it a train-mode encoder raises, as before.
 
-``install()`` registers our modules under the six names the reference imports its hot-path classes
+``install()`` registers our modules under the seven names the reference imports its hot-path classes
 from (``demo.py:5-7,62``, ``src/smirk_trainer.py:3-6``, ``src/base_trainer.py``):
 
     src.smirk_encoder      -> smirk_b200.smirk_encoder    (SmirkEncoder, create_backbone, ...)
@@ -16,9 +16,10 @@ from (``demo.py:5-7,62``, ``src/smirk_trainer.py:3-6``, ``src/base_trainer.py``)
     src.smirk_generator    -> smirk_b200.smirk_generator  (SmirkGenerator, ResnetBlock)
     src.losses.VGGPerceptualLoss -> smirk_b200.vgg_loss   (VGGPerceptualLoss)
     src.models.MICA.mica   -> smirk_b200.mica             (MICA; src.models.MICA.arcface stays the reference's)
+    src.losses.ExpressionLoss -> smirk_b200.expression_loss (ExpressionLoss; src.losses.resnet stays the reference's)
 
 Everything else under ``src`` (``src.FLAME.lbs``, ``src.renderer.util``, ``src.utils.*``, the other losses,
-trainers) still resolves to the reference's files: the real ``src`` package is imported first and only these six
+trainers) still resolves to the reference's files: the real ``src`` package is imported first and only these seven
 submodules are replaced in ``sys.modules`` (and as attributes of their parent packages).
 """
 import importlib
@@ -34,6 +35,7 @@ _MAP = {
     "src.smirk_generator": "smirk_b200.smirk_generator",
     "src.losses.VGGPerceptualLoss": "smirk_b200.vgg_loss",
     "src.models.MICA.mica": "smirk_b200.mica",
+    "src.losses.ExpressionLoss": "smirk_b200.expression_loss",
 }
 
 
@@ -52,7 +54,7 @@ def _ensure_package(name, path_hint):
 
 
 def install(reference_root=None):
-    """Alias the six hot-path modules.  ``reference_root`` (default: cwd) is put on sys.path so the
+    """Alias the seven hot-path modules.  ``reference_root`` (default: cwd) is put on sys.path so the
     rest of the reference package keeps importing normally."""
     root = os.path.abspath(reference_root or os.getcwd())
     if root not in sys.path:
