@@ -1,5 +1,5 @@
 """ctypes binding of libsmirk_b200.so (the C ABI declared in include/smirk_b200.h, include/smirk_b200_loss.h,
-include/smirk_b200_mica.h and include/smirk_b200_expression.h).
+include/smirk_b200_mica.h, include/smirk_b200_expression.h and include/smirk_b200_generator_train.h).
 
 There is deliberately no fallback: if the shared library is missing or a call fails, the product
 path raises.  Build with ``python -m smirk_b200.build`` (or ``__graft_entry__.build()``).
@@ -14,6 +14,19 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libsmirk_b200.so")
 _lib = None
+_TRAIN_MODE_DEFAULT = False
+
+
+def set_train_mode_default(on):
+    """Process-wide default of the train-mode opt-in of the encoder and the generator (off until set; a module's
+    ``allow_train_mode_`` overrides it)."""
+    global _TRAIN_MODE_DEFAULT
+    _TRAIN_MODE_DEFAULT = bool(on)
+
+
+def train_mode_default():
+    return _TRAIN_MODE_DEFAULT
+
 
 c_f32p = C.POINTER(C.c_float)
 c_i32p = C.POINTER(C.c_int32)
@@ -54,6 +67,15 @@ class SmkGeneratorDesc(C.Structure):
     _fields_ = [("in_channels", C.c_int), ("out_channels", C.c_int), ("init_features", C.c_int),
                 ("res_blocks", C.c_int), ("tensors", C.POINTER(c_f32p)), ("n_tensors", C.c_int),
                 ("precision", C.c_int)]
+
+
+class SmkGeneratorTrainArgs(C.Structure):
+    _fields_ = [("tensors", C.POINTER(c_f32p)), ("n_tensors", C.c_int), ("num_batches_tracked", C.POINTER(C.POINTER(C.c_int64))),
+                ("momentum", C.c_float), ("eps", C.c_float)]
+
+
+class SmkGeneratorTrainGrads(C.Structure):
+    _fields_ = [("tensors", C.POINTER(c_f32p))]
 
 
 class SmkVggLossDesc(C.Structure):
@@ -197,7 +219,16 @@ EXPRESSION_BINDINGS = [
     ("smk_expression_loss_backward_workspace_bytes", _sz, [_vp, _i, _i]),
     ("smk_expression_loss_backward", _i, [_vp, _i, _i, _i, _i, _vp, _sz, _vp, _vp, _vp, _vp, _sz, STREAM]),
 ]
-_ALL_BINDINGS = BINDINGS + LOSS_BINDINGS + MICA_BINDINGS + EXPRESSION_BINDINGS
+# The binding table of include/smirk_b200_generator_train.h (the generator's train mode), in that header's order, by the same rules.
+GENERATOR_TRAIN_BINDINGS = [
+    ("smk_generator_train_create", _i, [_i, _i, _i, _i, _i, _vpp]),
+    ("smk_generator_train_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_generator_forward_train", _i, [_vp, C.POINTER(SmkGeneratorTrainArgs), _vp, _i, _vp, _vp, _sz, _vp, _sz, STREAM]),
+    ("smk_generator_backward_train", _i, [_vp, C.POINTER(SmkGeneratorTrainArgs), _i, _vp, _vp, _sz, _vp, _vp,
+                                          C.POINTER(SmkGeneratorTrainGrads), _vp, _sz, STREAM]),
+    ("smk_debug_train_conv3_wgrad", _i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _sz, STREAM]),
+]
+_ALL_BINDINGS = BINDINGS + LOSS_BINDINGS + MICA_BINDINGS + EXPRESSION_BINDINGS + GENERATOR_TRAIN_BINDINGS
 _TAKES_STREAM = frozenset(name for name, _, args in _ALL_BINDINGS if args[-1:] == [STREAM])
 
 
@@ -343,7 +374,7 @@ class NativeState:
 
     def __init__(self):
         self.handle, self.key, self.workspaces, self.per_device = None, None, {}, {}
-        self.train_handle, self.train_key = None, None        # the encoder's train-mode handle (topology only)
+        self.train_handle, self.train_key = None, None        # the train-mode handle (topology only) of the encoder or generator
 
 
 class NativeModule:

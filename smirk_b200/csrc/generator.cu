@@ -27,6 +27,7 @@
 // by the epilogue of the kernel that produces g, and ConvTranspose2d's dgrad is a GEMM over a space-to-depth copy of g.
 #include "nn_kernels.cuh"
 #include "gemm_tc.cuh"
+#include "generator.cuh"
 #include <math.h>
 #include <algorithm>
 #include <string>
@@ -36,11 +37,6 @@ namespace {
 using smk::TensorCursor;
 using smk::grid_of;
 constexpr float kBnEps = 1e-5f;
-
-// fwd / dgrad: the weight operands of the forward and of the input gradient (smk::pack_conv3; the dgrad's carry the BN scale)
-struct Conv3 { smk::GemmW fwd, dgrad; float* scale; float* bias; int cin, cin_p, cout; };
-// fwd: N = 4*cout (n = (dy*2+dx) * cout + co), K = cin; dgrad: N = cin, K = 4*cout
-struct UpConv { smk::GemmW fwd, dgrad; float* scale; float* bias; int cin, cout; };
 
 bool fold_conv3(TensorCursor& cur, int cin, int cin_p, int cout, bool tc, bool x3, smk::DeviceArena& arena, Conv3* out, cudaError_t* err) {
     const float* w = cur.next(); const float* g = cur.next(); const float* b = cur.next();
@@ -72,18 +68,6 @@ bool fold_upconv(TensorCursor& cur, int cin, int cout, bool tc, bool x3, smk::De
 }
 
 }  // namespace
-
-struct SmkGenerator {
-    int cin, cin_p, cout, f, nres, precision;
-    Conv3 enc[5][2];                 // encoder1..4, bottleneck
-    std::vector<Conv3> res;          // 2 per ResnetBlock
-    UpConv up[4];                    // upconv4..1  (index 0 = level 4)
-    Conv3 dec[4][2];                 // decoder4..1
-    float *fw = nullptr, *fb = nullptr;   // final 1x1: W[f][cout], bias
-    float *ones = nullptr, *zeros = nullptr;   // unit scale / zero bias of the dgrad epilogues
-    smk::SavedLayout saved;          // activations of the grad-mode forward, forward order
-    smk::DeviceArena arena;
-};
 
 extern "C" int smk_generator_create(const SmkGeneratorDesc* desc, SmkGenerator** out) {
     SMK_REQUIRE(desc && out && desc->tensors, "smk_generator_create: null argument");
@@ -314,7 +298,7 @@ head_bwd_kernel(const float* __restrict__ gy, const float* __restrict__ y, int B
 // MaxPool 2x2 backward + skip gradient + ReLU mask of the pool input e (= the encoder's conv2 output = the skip):
 // g_e = (g_skip + [first maximum of the window, row-major] * g_p) * [e > 0].
 __global__ void __launch_bounds__(256)
-pool_bwd_kernel(const float* __restrict__ e, const float* __restrict__ gp, const float* __restrict__ gskip, int ld_skip,
+pool_bwd_kernel(const float* __restrict__ e, int ld_e, const float* __restrict__ gp, const float* __restrict__ gskip, int ld_skip,
                 int B, int S, int C, int round, float* __restrict__ out) {
     const int Ho = S >> 1, C4 = C >> 2;
     const long total = (long)B * Ho * Ho * C4;
@@ -326,7 +310,7 @@ pool_bwd_kernel(const float* __restrict__ e, const float* __restrict__ gp, const
         float v[4][4], g[4][4];
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-            const float4 a = __ldg(reinterpret_cast<const float4*>(e + px[k] * C) + c4);
+            const float4 a = __ldg(reinterpret_cast<const float4*>(e + px[k] * ld_e) + c4);
             const float4 s = __ldg(reinterpret_cast<const float4*>(gskip + px[k] * ld_skip) + c4);
             v[k][0] = a.x; v[k][1] = a.y; v[k][2] = a.z; v[k][3] = a.w;
             g[k][0] = s.x; g[k][1] = s.y; g[k][2] = s.z; g[k][3] = s.w;
@@ -413,36 +397,15 @@ nhwc_to_nchw_kernel(const float* __restrict__ in, int B, int HW, int Cp, int C, 
     out[i] = __ldg(in + ((size_t)b * HW + r) * Cp + c);
 }
 
-// dgrad of a 3x3 conv (zero padding 1): g_in = conv3x3(g, W') over S x S, * [mask > 0] (mask: the saved input activation).
+// The eval handle's dgrads: its packed dgrad weights, which carry the folded BN scale.
 int dgrad3(const SmkGenerator* h, const Conv3& c, const float* g, int B, int S, const float* mask, float* out, int ld_out, bool round,
            cudaStream_t st) {
-    smk::Conv p{};
-    p.in = g; p.ld_in = c.cout; p.B = B; p.H = S; p.W = S; p.Cin = c.cout; p.wgt = c.dgrad;
-    p.scale = h->ones; p.bias = h->zeros;
-    p.N = c.cin_p; p.K = 9 * c.cout; p.mode = 1; p.out = out; p.ld_out = ld_out; p.round_out = round ? 1 : 0;
-    p.mask = mask; p.ld_mask = c.cin_p; p.tag = c.dgrad.wt_lo ? "conv3x3_dgrad_tc3x" : c.dgrad.wt ? "conv3x3_dgrad_tc" : "conv3x3_dgrad_f32";
-    return smk::conv(p, st);
+    return gen::dgrad3(c.dgrad, c.cin_p, c.cout, h->ones, h->zeros, g, B, S, mask, out, ld_out, round, st);
 }
-
-// dgrad of ConvTranspose2d(k2, s2): g_in[S x S, cin] = s2d(g_out)[S x S, 4 cout] . W'^T, * [mask > 0].
 int dgrad_up(const SmkGenerator* h, const UpConv& u, const float* s2d, int B, int S, const float* mask, float* out, bool round, cudaStream_t st) {
-    const int K = 4 * u.cout;
-    smk::Conv p{};
-    p.in = s2d; p.ld_in = K; p.B = B; p.H = S; p.W = S; p.Cin = K; p.wgt = u.dgrad;
-    p.scale = h->ones; p.bias = h->zeros;
-    p.N = u.cin; p.K = K; p.mode = 0; p.out = out; p.ld_out = u.cin; p.round_out = round ? 1 : 0;
-    p.mask = mask; p.ld_mask = u.cin; p.tag = u.dgrad.wt_lo ? "upconv_dgrad_tc3x" : u.dgrad.wt ? "upconv_dgrad_tc" : "upconv_dgrad_f32";
-    return smk::conv(p, st);
+    return gen::dgrad_up(u.dgrad, u.cin, u.cout, h->ones, h->zeros, s2d, B, S, mask, out, round, st);
 }
-
-int fold(const float* gP, const float* res, int res_pad, const float* mask, int B, int C, bool round, float* out, int out_pad, cudaStream_t st) {
-    const int H = 14, Ho = H + 2 * out_pad;
-    const long total = (long)B * Ho * Ho * (C / 4);
-    SMK_TAG("reflect_fold", 4.0 * B * C * ((gP ? 16.0 * 16 : 0.0) + (res ? 196.0 : 0.0) + (mask ? 196.0 : 0.0) + Ho * Ho), (gP ? 1.0 : 0.0) * B * C * 256, st);
-    SMK_LAUNCH(fold_kernel, dim3(grid_of(total)), dim3(256), 0, st, gP, res, res_pad, mask, B, H, H, C, round ? 1 : 0, out, out_pad);
-    SMK_CHECK_LAUNCH();
-    return 0;
-}
+using gen::fold;
 
 // floats per image of the backward's workspace buffers
 struct GradPlan {
@@ -459,6 +422,72 @@ GradPlan make_grad_plan(const SmkGenerator* h) {
 }
 }  // namespace
 
+namespace gen {
+
+int dgrad3(const smk::GemmW& w, int cin_p, int cout, const float* ones, const float* zeros, const float* g, int B, int S, const float* mask,
+           float* out, int ld_out, bool round, cudaStream_t st) {
+    smk::Conv p{};
+    p.in = g; p.ld_in = cout; p.B = B; p.H = S; p.W = S; p.Cin = cout; p.wgt = w;
+    p.scale = ones; p.bias = zeros;
+    p.N = cin_p; p.K = 9 * cout; p.mode = 1; p.out = out; p.ld_out = ld_out; p.round_out = round ? 1 : 0;
+    p.mask = mask; p.ld_mask = cin_p; p.tag = w.wt_lo ? "conv3x3_dgrad_tc3x" : w.wt ? "conv3x3_dgrad_tc" : "conv3x3_dgrad_f32";
+    return smk::conv(p, st);
+}
+
+int dgrad_up(const smk::GemmW& w, int cin, int cout, const float* ones, const float* zeros, const float* s2d, int B, int S, const float* mask,
+             float* out, bool round, cudaStream_t st) {
+    const int K = 4 * cout;
+    smk::Conv p{};
+    p.in = s2d; p.ld_in = K; p.B = B; p.H = S; p.W = S; p.Cin = K; p.wgt = w;
+    p.scale = ones; p.bias = zeros;
+    p.N = cin; p.K = K; p.mode = 0; p.out = out; p.ld_out = cin; p.round_out = round ? 1 : 0;
+    p.mask = mask; p.ld_mask = cin; p.tag = w.wt_lo ? "upconv_dgrad_tc3x" : w.wt ? "upconv_dgrad_tc" : "upconv_dgrad_f32";
+    return smk::conv(p, st);
+}
+
+int s2d(const float* in, int ld_in, int B, int S, int C, float* out, cudaStream_t st) {
+    const long total = (long)B * S * S * 4 * (C / 4);
+    SMK_TAG("upconv_s2d", 32.0 * B * S * S * C, 0.0, st);
+    SMK_LAUNCH(s2d_kernel, dim3(grid_of(total)), dim3(256), 0, st, in, ld_in, B, S, C, out);
+    SMK_CHECK_LAUNCH();
+    return 0;
+}
+
+int fold(const float* gP, const float* res, int res_pad, const float* mask, int B, int C, bool round, float* out, int out_pad, cudaStream_t st) {
+    const int H = 14, Ho = H + 2 * out_pad;
+    const long total = (long)B * Ho * Ho * (C / 4);
+    SMK_TAG("reflect_fold", 4.0 * B * C * ((gP ? 16.0 * 16 : 0.0) + (res ? 196.0 : 0.0) + (mask ? 196.0 : 0.0) + Ho * Ho), (gP ? 1.0 : 0.0) * B * C * 256, st);
+    SMK_LAUNCH(fold_kernel, dim3(grid_of(total)), dim3(256), 0, st, gP, res, res_pad, mask, B, H, H, C, round ? 1 : 0, out, out_pad);
+    SMK_CHECK_LAUNCH();
+    return 0;
+}
+
+int pool_bwd(const float* e, int ld_e, const float* gp, const float* gskip, int ld_skip, int B, int S, int C, bool round, float* out, cudaStream_t st) {
+    const long total = (long)B * (S / 2) * (S / 2) * (C / 4);
+    SMK_TAG("maxpool_dgrad", 4.0 * B * ((double)S * S * C * 3 + (S / 2.0) * (S / 2.0) * C), 0.0, st);
+    SMK_LAUNCH(pool_bwd_kernel, dim3(grid_of(total)), dim3(256), 0, st, e, ld_e, gp, gskip, ld_skip, B, S, C, round ? 1 : 0, out);
+    SMK_CHECK_LAUNCH();
+    return 0;
+}
+
+int head_bwd(const float* gy, const float* y, int B, int HW, int cout, const float* w, const float* d, int f, bool round, float* out, cudaStream_t st) {
+    const long total = (long)B * HW * (f / 4);
+    SMK_TAG("head_dgrad", 4.0 * B * HW * (2.0 * cout + 2.0 * f), 2.0 * B * HW * f * cout, st);
+    SMK_LAUNCH(head_bwd_kernel, dim3(smk::cdiv(total, 256)), dim3(256), 0, st, gy, y, B, HW, cout, w, d, f, round ? 1 : 0, out);
+    SMK_CHECK_LAUNCH();
+    return 0;
+}
+
+int nhwc_to_nchw(const float* in, int B, int HW, int Cp, int C, float* out, cudaStream_t st) {
+    const long total = (long)B * C * HW;
+    SMK_TAG("nhwc_to_nchw", 4.0 * (double)B * HW * (C + Cp), 0.0, st);
+    SMK_LAUNCH(nhwc_to_nchw_kernel, dim3(smk::cdiv(total, 256)), dim3(256), 0, st, in, B, HW, Cp, C, out);
+    SMK_CHECK_LAUNCH();
+    return 0;
+}
+
+}  // namespace gen
+
 extern "C" size_t smk_generator_workspace_bytes(const SmkGenerator* h, int B) {
     return (make_plan(h).total() * (size_t)B * sizeof(float)) + 40 * 256;
 }
@@ -469,10 +498,13 @@ extern "C" int smk_generator_forward(const SmkGenerator* h, const float* x, int 
     SMK_REQUIRE(h && x && y, "smk_generator_forward: null argument");
     SMK_REQUIRE(B > 0, "smk_generator_forward: negative batch");
     SMK_REQUIRE(ws && ws_bytes >= smk_generator_workspace_bytes(h, B), "smk_generator_forward: workspace too small");
+    SMK_REQUIRE(!h->train, "smk_generator_forward: a train handle has no packed weights (smk_generator_forward_train)");
     return generator_forward(h, x, B, y, nullptr, ws, ws_bytes, (cudaStream_t)stream);
 }
 
-extern "C" size_t smk_generator_saved_bytes(const SmkGenerator* h, int B) { return h ? h->saved.bytes(B) : 0; }
+extern "C" size_t smk_generator_saved_bytes(const SmkGenerator* h, int B) {
+    return h ? h->saved.bytes(B) + smk::ws_round(h->topo.stats_floats * sizeof(float)) : 0;     // stats: train handles only
+}
 
 extern "C" int smk_generator_saved_tensor(const SmkGenerator* h, int B, int i, const char** name, size_t* offset, int* dims) {
     return smk::saved_tensor(h ? &h->saved : nullptr, "smk_generator_saved_tensor", B, i, name, offset, dims);
@@ -486,6 +518,7 @@ extern "C" int smk_generator_forward_saved(const SmkGenerator* h, const float* x
     SMK_REQUIRE(x && y && saved, "smk_generator_forward_saved: null argument");
     SMK_REQUIRE(saved_bytes > 0 && saved_bytes >= smk_generator_saved_bytes(h, B), "smk_generator_forward_saved: saved buffer too small");
     SMK_REQUIRE(ws && ws_bytes > 0 && ws_bytes >= smk_generator_workspace_bytes(h, B), "smk_generator_forward_saved: workspace too small");
+    SMK_REQUIRE(!h->train, "smk_generator_forward_saved: a train handle has no packed weights (smk_generator_forward_train)");
     return generator_forward(h, x, B, y, saved, ws, ws_bytes, (cudaStream_t)stream);
 }
 
@@ -501,6 +534,7 @@ extern "C" int smk_generator_backward(const SmkGenerator* h, int B, const float*
     SMK_REQUIRE(y && saved && g_y && g_x, "smk_generator_backward: null argument");
     SMK_REQUIRE(saved_bytes > 0 && saved_bytes >= smk_generator_saved_bytes(h, B), "smk_generator_backward: saved buffer too small");
     SMK_REQUIRE(ws && ws_bytes > 0 && ws_bytes >= smk_generator_backward_workspace_bytes(h, B), "smk_generator_backward: workspace too small");
+    SMK_REQUIRE(!h->train, "smk_generator_backward: a train handle (smk_generator_backward_train)");
     cudaStream_t st = (cudaStream_t)stream;
     const int f = h->f, cb = 16 * f;
     const bool rnd = h->precision == 1;            // TF32 rounding of every gradient a TF32 dgrad reads (not at 3xTF32)
@@ -516,24 +550,13 @@ extern "C" int smk_generator_backward(const SmkGenerator* h, int B, const float*
     SMK_REQUIRE(s2d && (h->nres == 0 || pad[3]), "smk_generator_backward: workspace carve-up failed");
     int rc;
     // head: sigmoid and the 1x1 conv, through dec1conv2's ReLU
-    {
-        const long total = (long)B * 224 * 224 * (f / 4);
-        SMK_TAG("head_dgrad", 4.0 * B * 224.0 * 224.0 * (2.0 * h->cout + 2.0 * f), 2.0 * B * 224.0 * 224.0 * f * h->cout, st);
-        SMK_LAUNCH(head_bwd_kernel, dim3(smk::cdiv(total, 256)), dim3(256), 0, st, g_y, y, B, 224 * 224, h->cout, h->fw,
-                   SV(sv_dec(h, 0, 1)), f, rnd ? 1 : 0, A);
-        SMK_CHECK_LAUNCH();
-    }
+    if ((rc = gen::head_bwd(g_y, y, B, 224 * 224, h->cout, h->fw, SV(sv_dec(h, 0, 1)), f, rnd, A, st))) return rc;
     // decoder levels 1..4: conv2, conv1 (both halves of the concat), up-convolution
     for (int lvl = 0; lvl < 4; ++lvl) {
         const int i = 3 - lvl, S = 224 >> lvl, c = f << lvl;
         if ((rc = dgrad3(h, h->dec[i][1], A, B, S, SV(sv_dec(h, lvl, 0)), Bf, c, rnd, st))) return rc;
         if ((rc = dgrad3(h, h->dec[i][0], Bf, B, S, nullptr, gcat[lvl], 2 * c, rnd, st))) return rc;
-        {
-            const long total = (long)B * (S / 2) * (S / 2) * 4 * (c / 4);
-            SMK_TAG("upconv_s2d", 8.0 * B * S * S * c, 0.0, st);
-            SMK_LAUNCH(s2d_kernel, dim3(grid_of(total)), dim3(256), 0, st, gcat[lvl], 2 * c, B, S / 2, c, s2d);
-            SMK_CHECK_LAUNCH();
-        }
+        if ((rc = gen::s2d(gcat[lvl], 2 * c, B, S / 2, c, s2d, st))) return rc;
         const float* m = lvl < 3 ? SV(sv_dec(h, lvl + 1, 1)) : (h->nres == 0 ? SV(sv_bott(1)) : nullptr);
         if ((rc = dgrad_up(h, h->up[i], s2d, B, S / 2, m, A, rnd, st))) return rc;
     }
@@ -557,20 +580,11 @@ extern "C" int smk_generator_backward(const SmkGenerator* h, int B, const float*
     // encoder levels 4..1: pool (+ skip gradient), conv2, conv1
     for (int lvl = 3; lvl >= 0; --lvl) {
         const int S = 224 >> lvl, c = f << lvl;
-        {
-            const long total = (long)B * (S / 2) * (S / 2) * (c / 4);
-            SMK_TAG("maxpool_dgrad", 4.0 * B * ((double)S * S * c * 3 + (S / 2.0) * (S / 2.0) * c), 0.0, st);
-            SMK_LAUNCH(pool_bwd_kernel, dim3(grid_of(total)), dim3(256), 0, st, SV(sv_enc(lvl, 1)), g, gcat[lvl] + c, 2 * c, B, S, c, rnd ? 1 : 0, o);
-            SMK_CHECK_LAUNCH();
-        }
+        if ((rc = gen::pool_bwd(SV(sv_enc(lvl, 1)), c, g, gcat[lvl] + c, 2 * c, B, S, c, rnd, o, st))) return rc;
         if ((rc = dgrad3(h, h->enc[lvl][1], o, B, S, SV(sv_enc(lvl, 0)), g, c, rnd, st))) return rc;
         const int n_in = lvl > 0 ? c / 2 : h->cin_p;
         if ((rc = dgrad3(h, h->enc[lvl][0], g, B, S, nullptr, o, n_in, rnd && lvl > 0, st))) return rc;
         std::swap(g, o);
     }
-    const long total = (long)B * h->cin * 224 * 224;
-    SMK_TAG("nhwc_to_nchw", 4.0 * (double)B * 224 * 224 * (h->cin + h->cin_p), 0.0, st);
-    SMK_LAUNCH(nhwc_to_nchw_kernel, dim3(smk::cdiv(total, 256)), dim3(256), 0, st, g, B, 224 * 224, h->cin_p, h->cin, g_x);
-    SMK_CHECK_LAUNCH();
-    return 0;
+    return gen::nhwc_to_nchw(g, B, 224 * 224, h->cin_p, h->cin, g_x, st);
 }

@@ -3,9 +3,11 @@
     cd <reference checkout>;  python -m smirk_b200.dropin demo.py --input_path ... [script args]
     cd <reference checkout>;  python -m smirk_b200.dropin --train train.py configs/config_pretrain.yaml
 
-``--train`` (before the script) turns on the encoder's train-mode opt-in for the whole process
-(``smirk_encoder.set_train_mode_default(True)``): the trainer's ``.train()`` encoder then runs with batch statistics
-and gets its weight gradients.  Without it a train-mode encoder raises, as before.
+    cd <reference checkout>;  python -m smirk_b200.dropin --train train.py configs/config_train.yaml
+
+``--train`` (before the script) turns on the train-mode opt-in of SmirkEncoder and SmirkGenerator for the whole process
+(``smirk_encoder.set_train_mode_default(True)``, one flag for both): the trainer's ``.train()`` encoder and generator
+then run with batch statistics and get their weight gradients.  Without it a train-mode encoder or generator raises.
 
 ``install()`` registers our modules under the seven names the reference imports its hot-path classes
 from (``demo.py:5-7,62``, ``src/smirk_trainer.py:3-6``, ``src/base_trainer.py``):

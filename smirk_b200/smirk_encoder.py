@@ -24,17 +24,9 @@ import torch.nn as nn
 from . import _lib
 
 BN_EPS = 1e-3          # timm tf_* models (BN_EPS_TF_DEFAULT)
-_TRAIN_MODE_DEFAULT = False
-
-
-def set_train_mode_default(on):
-    """Process-wide default of the train-mode opt-in (off until set; ``allow_train_mode_`` overrides it per module)."""
-    global _TRAIN_MODE_DEFAULT
-    _TRAIN_MODE_DEFAULT = bool(on)
-
-
-def train_mode_default():
-    return _TRAIN_MODE_DEFAULT
+# The process-wide train-mode opt-in, one flag shared with SmirkGenerator (it lives in _lib).
+set_train_mode_default = _lib.set_train_mode_default
+train_mode_default = _lib.train_mode_default
 
 # (kind, stride, expansion, out_channels) per block, grouped per stage — timm 0.9.16
 # tf_mobilenetv3_{large,small}_minimal_100 with features_only=True (stops after the `cn` stage).
@@ -178,7 +170,7 @@ class _NativeEncoder(_lib.NativeModule, nn.Module):
 
     def _train_allowed(self):
         on = self.__dict__.get("_allow_train")
-        return _TRAIN_MODE_DEFAULT if on is None else on
+        return _lib.train_mode_default() if on is None else on
 
     def _check(self, img):
         """Device, shape and mode checks of every call -> True for a train-mode call.  The mode is that of the BatchNorms

@@ -6,8 +6,15 @@ parameter containers; the forward pass runs in ``csrc/generator.cu`` through ``s
 
 With grad mode on and an input that requires grad, a frozen (``requires_grad_(False)``) eval-mode generator passes the
 gradient to its input, as the reference trainer's emotion loss and photometric fitting need: the forward then keeps
-its activations (``smk_generator_forward_saved``) and the backward runs ``smk_generator_backward``.  Weight gradients
-are not implemented.
+its activations (``smk_generator_forward_saved``) and the backward runs ``smk_generator_backward``.  Eval-mode weight
+gradients are not implemented.
+
+Train mode (``.train()``, what the reference trainer's generator steps run) is opt-in, as the encoder's: per module with
+``allow_train_mode_(True)``, or process-wide with ``smirk_encoder.set_train_mode_default(True)`` (one flag for both
+modules; ``python -m smirk_b200.dropin --train``).  Then the BatchNorms normalise with batch statistics and update their
+running statistics (``smk_generator_forward_train``, also under ``torch.no_grad()``), and every parameter that requires
+grad, and the input when it requires grad, gets its gradient (``smk_generator_backward_train``).  Batch statistics couple
+the images of a batch.  Without the opt-in a train-mode generator raises.
 
 ``precision`` (part of the native handle's key, so it may change between calls): 0 = fp32 CUDA cores, 1 = TF32 tensor cores,
 3 = 3xTF32 tensor cores (each operand split into a TF32 head and tail, three products per term: fp32-equivalent forward and
@@ -92,10 +99,33 @@ class SmirkGenerator(_lib.NativeModule, nn.Module):
         if x.dim() != 4 or tuple(x.shape[1:]) != (cin, 224, 224):
             raise RuntimeError("smirk_b200.SmirkGenerator: expected x [B,%d,224,224], got %s" % (cin, tuple(x.shape)))
 
+    def allow_train_mode_(self, on=True):
+        """Opt this module in to (or out of) train mode; returns the module."""
+        self._allow_train = bool(on)
+        return self
+
+    def _train_allowed(self):
+        on = self.__dict__.get("_allow_train")
+        return _lib.train_mode_default() if on is None else on
+
+    def _is_train(self):
+        """True when the BatchNorms are in train mode (checked on every call: .train() after the first forward must not
+        silently run eval BN)."""
+        modes = {m.training for m in self.modules() if isinstance(m, nn.BatchNorm2d)}
+        if True not in modes:
+            return False
+        if not self._train_allowed():
+            raise RuntimeError("smirk_b200.SmirkGenerator: train-mode BatchNorm runs only with the opt-in: call "
+                               ".allow_train_mode_(True) on the generator or run under `python -m smirk_b200.dropin --train`")
+        if modes != {True}:
+            raise RuntimeError("smirk_b200.SmirkGenerator: its BatchNorms mix train and eval mode")
+        return True
+
     def forward(self, x):
         _lib.require_cuda(x, "x")
-        if self.training:                      # checked on every call: .train() after the first forward must not silently run eval BN
-            raise RuntimeError("smirk_b200.SmirkGenerator: train-mode BatchNorm is not implemented (forward/eval only)")
+        if self._is_train():
+            self._check_input(x)
+            return self._run_train(x)
         if torch.is_grad_enabled() and x.requires_grad:
             if any(p.requires_grad for p in self.parameters()):
                 raise RuntimeError("smirk_b200.SmirkGenerator: weight gradients are not implemented; to pass a gradient to the "
@@ -133,8 +163,94 @@ class SmirkGenerator(_lib.NativeModule, nn.Module):
         context of the same input holds."""
         _lib.require_cuda(x, "x")
         self._check_input(x)
-        h, _, saved = self._forward_saved(x)
+        if self._is_train():                 # train mode: on copies of the running statistics, which stay untouched
+            h, _, saved = self._forward_train(x, list(self.parameters()), True, copy_stats=True)
+        else:
+            h, _, saved = self._forward_saved(x)
         return _lib.saved_views("generator", h, saved, x.shape[0])
+
+    # ---- train mode ---------------------------------------------------------------------------------------------------
+    def _train_handle(self, dev):
+        st = self._native
+        key = (str(dev), self._cfg, int(self.precision))          # topology only: an optimizer step builds nothing
+        if st.train_handle is None or st.train_key != key:
+            st.train_handle = None
+            h = C.c_void_p()
+            _lib.call("smk_generator_train_create", dev, *self._cfg, int(self.precision), C.byref(h))
+            st.train_handle, st.train_key = _lib.NativeHandle(h, "smk_generator_destroy"), key
+        return st.train_handle
+
+    def _bn_settings(self):
+        bns = [m for m in self.modules() if isinstance(m, nn.BatchNorm2d)]
+        settings = {(m.momentum, m.eps) for m in bns}
+        if len(settings) != 1 or not all(m.affine and m.track_running_stats for m in bns):
+            raise RuntimeError("smirk_b200.SmirkGenerator: train mode needs affine BatchNorms that track running statistics, "
+                               "with one momentum and one eps, got %s" % sorted(settings, key=str))
+        momentum, eps = settings.pop()
+        if (momentum is not None and not 0.0 <= momentum <= 1.0) or not eps > 0:
+            raise RuntimeError("smirk_b200.SmirkGenerator: train mode takes momentum in [0, 1] or None and eps > 0, got "
+                               "momentum %r, eps %r" % (momentum, eps))
+        return momentum, eps
+
+    def _train_args(self, dev, params, copy_stats=False):
+        """-> (SmkGeneratorTrainArgs, keep-alive list, [running statistics and counters], {parameter index: tensor
+        index}).  params: ``list(self.parameters())`` (or the tensors an autograd context saved).  copy_stats: point at
+        copies of the running statistics (a forward that must leave the module untouched)."""
+        momentum, eps = self._bn_settings()
+        names = [k for k, _ in self.named_parameters()]
+        it = iter(params)
+        ts, nbt, stats, where = [], [], [], {}
+        for k, v in self.state_dict(keep_vars=True).items():
+            if k.endswith("num_batches_tracked"):
+                n = v.clone() if copy_stats else v
+                if n.device != dev or n.dtype != torch.int64:
+                    raise RuntimeError("smirk_b200: num_batches_tracked must be an int64 tensor on %s" % dev)
+                nbt.append(n); stats.append(n)
+                continue
+            if k in names:
+                where[names.index(k)] = len(ts)
+                t = next(it)
+            else:
+                t = v.clone() if copy_stats else v
+                stats.append(t)
+            if t.device != dev or t.dtype != torch.float32 or not t.is_contiguous():
+                raise RuntimeError("smirk_b200: train mode needs contiguous float32 parameters and buffers on %s" % dev)
+            ts.append(t)
+        a = _lib.SmkGeneratorTrainArgs()
+        arr = (_lib.c_f32p * len(ts))(*[C.cast(t.data_ptr(), _lib.c_f32p) for t in ts])
+        narr = (C.POINTER(C.c_int64) * len(nbt))(*[C.cast(t.data_ptr(), C.POINTER(C.c_int64)) for t in nbt])
+        a.tensors, a.n_tensors = C.cast(arr, C.POINTER(_lib.c_f32p)), len(ts)
+        a.num_batches_tracked = C.cast(narr, C.POINTER(C.POINTER(C.c_int64)))
+        a.momentum, a.eps = -1.0 if momentum is None else momentum, eps
+        return a, [arr, narr, ts, nbt], stats, where
+
+    def _forward_train(self, x, params, with_saved, copy_stats=False):
+        """-> (handle, y, saved | None): one train-mode forward, which updates the running statistics (of copies, with
+        copy_stats)."""
+        dev = x.device
+        h = self._train_handle(dev)
+        x = _lib.dev_f32(x, "x")
+        B = x.shape[0]
+        y = torch.empty(B, self._cfg[1], 224, 224, dtype=torch.float32, device=dev)
+        args, keep, stats, _ = self._train_args(dev, params, copy_stats)
+        nbytes = _lib.call("smk_generator_train_workspace_bytes", dev, h, B)
+        saved = _lib.saved_buffer("generator", h, B, dev) if with_saved else None
+        if saved is None:
+            nbytes += _lib.call("smk_generator_saved_bytes", dev, h, B)
+        ws = self._native_workspace("train", nbytes, dev)
+        _lib.call("smk_generator_forward_train", dev, h, C.byref(args), x, B, y, saved, 0 if saved is None else saved.numel() * 4,
+                  ws, ws.numel())
+        if not copy_stats:                  # the eval handle repacks, and copies see the new statistics
+            for t in stats:
+                torch.autograd.graph.increment_version(t)
+        return h, y, saved
+
+    def _run_train(self, x):
+        params = list(self.parameters())
+        if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params)):
+            return _GeneratorTrainFunction.apply(x, self, *params)
+        with torch.no_grad():
+            return self._forward_train(x, params, False)[1]
 
 
 class _GeneratorFunction(torch.autograd.Function):
@@ -158,3 +274,36 @@ class _GeneratorFunction(torch.autograd.Function):
         ws = m._native_workspace("backward", _lib.call("smk_generator_backward_workspace_bytes", dev, ctx.handle, B), dev)
         _lib.call("smk_generator_backward", dev, ctx.handle, B, y, saved, saved.numel() * 4, g_y, g_x, ws, ws.numel())
         return g_x.to(ctx.dtype), None
+
+
+class _GeneratorTrainFunction(torch.autograd.Function):
+    """Train-mode generator: y = G(x), and the gradients of x and of every parameter in ``parameters()`` order (those
+    autograd asks for).  The activations and batch statistics are saved per call, so several forwards may share one
+    backward."""
+
+    @staticmethod
+    def forward(ctx, x, module, *params):
+        h, y, saved = module._forward_train(x, params, True)
+        ctx.handle, ctx.module, ctx.dtype = h, module, x.dtype
+        ctx.save_for_backward(y, saved, *params)
+        return y
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_y):
+        y, saved, *params = ctx.saved_tensors
+        m, dev, B = ctx.module, y.device, y.shape[0]
+        g_y = _lib.dev_f32(g_y, "g_y")
+        args, keep, _, where = m._train_args(dev, params)
+        out = [torch.empty_like(p) if ctx.needs_input_grad[2 + i] else None for i, p in enumerate(params)]
+        ptrs = [None] * args.n_tensors
+        for i, t in enumerate(out):
+            ptrs[where[i]] = t
+        arr = (_lib.c_f32p * len(ptrs))(*[C.cast(t.data_ptr(), _lib.c_f32p) if t is not None else None for t in ptrs])
+        gr = _lib.SmkGeneratorTrainGrads()
+        gr.tensors = C.cast(arr, C.POINTER(_lib.c_f32p))
+        g_x = torch.empty(B, m._cfg[0], 224, 224, dtype=torch.float32, device=dev) if ctx.needs_input_grad[0] else None
+        ws = m._native_workspace("train", _lib.call("smk_generator_train_workspace_bytes", dev, ctx.handle, B), dev)
+        _lib.call("smk_generator_backward_train", dev, ctx.handle, C.byref(args), B, y, saved, saved.numel() * 4, g_y, g_x,
+                  C.byref(gr), ws, ws.numel())
+        return (None if g_x is None else g_x.to(ctx.dtype), None, *out)
