@@ -1,5 +1,6 @@
 """ctypes binding of libsmirk_b200.so (the C ABI declared in include/smirk_b200.h, include/smirk_b200_loss.h,
-include/smirk_b200_mica.h, include/smirk_b200_expression.h and include/smirk_b200_generator_train.h).
+include/smirk_b200_mica.h, include/smirk_b200_expression.h, include/smirk_b200_generator_train.h and
+include/smirk_b200_cycle.h).
 
 There is deliberately no fallback: if the shared library is missing or a call fails, the product
 path raises.  Build with ``python -m smirk_b200.build`` (or ``__graft_entry__.build()``).
@@ -92,6 +93,17 @@ class SmkExpressionLossDesc(C.Structure):
 
 class SmkMaskingDesc(C.Structure):
     _fields_ = [("n_verts", C.c_int), ("n_faces", C.c_int), ("faces", c_i32p)]
+
+
+class SmkCycleDesc(C.Structure):
+    _fields_ = [("n_keys", C.c_int), ("row_offset", c_i32p), ("rows", c_f32p), ("n_exp", C.c_int)]
+
+
+class SmkCycleDraws(C.Structure):
+    """Device pointers of the augmentation's exported draws (include/smirk_b200_cycle.h), in the header's field order."""
+    FIELDS = ("gids", "perm1", "param_mask", "jaw_mask", "randn0a", "randn0b", "randn1", "randn2", "randn3", "randn_jaw",
+              "rand0a", "rand0b", "rand1a", "rand1b", "rand2a", "rand2b", "rand3", "rand_eyelid", "rand3_eyelid", "tmpl_key", "tmpl_row")
+    _fields_ = [(f, C.c_void_p) for f in FIELDS]
 
 
 # The binding table: one (name, return type, argument types) row per entry point of include/smirk_b200.h, in the
@@ -228,7 +240,17 @@ GENERATOR_TRAIN_BINDINGS = [
                                           C.POINTER(SmkGeneratorTrainGrads), _vp, _sz, STREAM]),
     ("smk_debug_train_conv3_wgrad", _i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _sz, STREAM]),
 ]
-_ALL_BINDINGS = BINDINGS + LOSS_BINDINGS + MICA_BINDINGS + EXPRESSION_BINDINGS + GENERATOR_TRAIN_BINDINGS
+# The binding table of include/smirk_b200_cycle.h (the trainer's masking and the cycle augmentation), in that header's order,
+# by the same rules.
+CYCLE_BINDINGS = [
+    ("smk_masking_train_workspace_bytes", _sz, [_vp, _i, _i, _i, _i]),
+    ("smk_masking_train_forward", _i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp,
+                                       _vp, _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_cycle_create", _i, [C.POINTER(SmkCycleDesc), _vpp]),
+    ("smk_cycle_destroy", None, [_vp]),
+    ("smk_cycle_augment", _i, [_vp, _vpp, _vpp, C.POINTER(C.c_int), _i, _i, _i, _vp, C.POINTER(SmkCycleDraws), STREAM]),
+]
+_ALL_BINDINGS = BINDINGS + LOSS_BINDINGS + MICA_BINDINGS + EXPRESSION_BINDINGS + GENERATOR_TRAIN_BINDINGS + CYCLE_BINDINGS
 _TAKES_STREAM = frozenset(name for name, _, args in _ALL_BINDINGS if args[-1:] == [STREAM])
 
 

@@ -19,13 +19,21 @@
 // what IS exact: given the draws this call exports (optional debug outputs), the masked image equals the reference's
 // `masking()` fed the same draws.  The counter lives in device memory and is advanced by the last kernel, so a captured
 // CUDA graph produces fresh draws on every replay.
+// (3) smk_masking_train_forward (include/smirk_b200_cycle.h) runs the trainer's step1 / step2 masking on the same kernels:
+// every sampled point kept (no rbound), transfer_pixels between two meshes, Ke repeats read as row r mod B (`Bsrc`).
 // All of it is HBM-bound byte/float shuffling over [B,3,224,224] images (602 KB per face in, 602 KB out).
 #include "common.cuh"
+#include "philox.cuh"
+#include "../../include/smirk_b200_cycle.h"
 #include <math.h>
 #include <algorithm>
 #include <vector>
 
 namespace {
+
+using smk::U4;
+using smk::philox;
+using smk::u01;
 
 struct MaskDev {
     int V, F;
@@ -82,13 +90,14 @@ mask_face_weights_kernel(MaskDev d, const float* __restrict__ tv, const float* _
 
 __global__ void __launch_bounds__(256)
 mask_points_kernel(MaskDev d, const float* __restrict__ tv, const int64_t* __restrict__ fidx, const float* __restrict__ bary,
-                   int B, int N, int S, int64_t* __restrict__ npoints) {
+                   int B, int Bsrc, int N, int S, int64_t* __restrict__ npoints) {
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long)B * N) return;
     const int b = (int)(i / N);
-    const int32_t* tri = d.faces + (size_t)fidx[i] * 3;
+    const long src = (long)(b % Bsrc) * N + (i - (long)b * N);                          // draws of row b mod Bsrc
+    const int32_t* tri = d.faces + (size_t)fidx[src] * 3;
     const float* vb = tv + (size_t)b * d.V * 3;
-    const float b0 = bary[i * 3], b1 = bary[i * 3 + 1], b2 = bary[i * 3 + 2];
+    const float b0 = bary[src * 3], b1 = bary[src * 3 + 1], b2 = bary[src * 3 + 2];
 #pragma unroll
     for (int k = 0; k < 2; ++k) {
         float p = __fmul_rn(vb[(size_t)tri[0] * 3 + k], b0);
@@ -113,12 +122,13 @@ mask_scatter_kernel(const int64_t* __restrict__ npoints, const int64_t* __restri
 // horizontal halves of the two max-pools: th = max_{|dx|<=wr}(1 - hull), tc = max_{|dx|<=5} centres (OOB ignored, like
 // max_pool2d's -inf padding)
 __global__ void __launch_bounds__(256)
-mask_hmax_kernel(const float* __restrict__ hull, const float* __restrict__ centres, int B, int S, int wr,
+mask_hmax_kernel(const float* __restrict__ hull, const float* __restrict__ centres, int B, int Bsrc, int S, int wr,
                  float* __restrict__ th, float* __restrict__ tc) {
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long)B * S * S) return;
     const int x = (int)(i % S);
-    const float* hr = hull + (i - x);
+    const long plane = (long)S * S, b = i / plane;
+    const float* hr = hull + (b % Bsrc) * plane + (i - b * plane - x);                  // hull of image b mod Bsrc
     float m = -INFINITY;
     for (int dx = -wr; dx <= wr; ++dx) { const int xx = x + dx; if (xx >= 0 && xx < S) m = fmaxf(m, __fsub_rn(1.0f, hr[xx])); }
     th[i] = m;
@@ -134,7 +144,7 @@ mask_hmax_kernel(const float* __restrict__ hull, const float* __restrict__ centr
 __global__ void __launch_bounds__(256)
 mask_compose_kernel(const float* __restrict__ img, const float* __restrict__ th, const float* __restrict__ tc,
                     const uint8_t* __restrict__ pm, const float* __restrict__ extra, const float* __restrict__ rendered_mask,
-                    const float* __restrict__ noise_mult, int B, int S, int wr, float* __restrict__ out) {
+                    const float* __restrict__ noise_mult, int B, int Bsrc, int S, int wr, float* __restrict__ out) {
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long)B * S * S) return;
     const int b = (int)(i / ((long)S * S));
@@ -155,7 +165,7 @@ mask_compose_kernel(const float* __restrict__ img, const float* __restrict__ th,
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) {
         const size_t o = ((size_t)b * 3 + ch) * S * S + pix;
-        const float v = img[o];
+        const float v = img[((size_t)(b % Bsrc) * 3 + ch) * S * S + pix];              // image b mod Bsrc
         float e = extra ? extra[o] : __fmul_rn(v, on);                // extra_points: given (masking.py:71), or img * pmask (demo.py:162)
         if (noise_mult) e = __fmul_rn(e, noise_mult[o]);
         if (tc) e = __fmul_rn(e, keep);
@@ -163,22 +173,6 @@ mask_compose_kernel(const float* __restrict__ img, const float* __restrict__ th,
     }
 }
 
-
-// ---- counter-based RNG: Philox4x32-10 (Salmon et al. 2011), key = seed, counter = (element, stream, call counter) ----
-struct U4 { uint32_t x, y, z, w; };
-__device__ __forceinline__ U4 philox(uint64_t seed, uint64_t ctr, uint32_t stream, uint32_t elem_hi, uint32_t elem_lo) {
-    uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
-    U4 c{elem_lo, elem_hi, (uint32_t)ctr ^ (stream << 28), (uint32_t)(ctr >> 32)};
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
-        const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
-        c = U4{hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0};
-        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-    }
-    return c;
-}
-__device__ __forceinline__ float u01(uint32_t r) { return (float)(r >> 8) * (1.0f / 16777216.0f); }          // [0, 1)
 
 // one CTA per image: inclusive CDF of the face weights in shared memory, N inverse-CDF samples, barycentrics, rbound
 __global__ void __launch_bounds__(512)
@@ -222,7 +216,7 @@ mask_sample_kernel(const float* __restrict__ w, int F, int N, float ratio_mul, c
         fidx[o] = f;
         bary[o * 3] = 1.f - (u + v); bary[o * 3 + 1] = u; bary[o * 3 + 2] = v;
     }
-    if (t == 0) {                                       // demo.py:151-153
+    if (t == 0 && rbound) {                             // demo.py:151-153
         const U4 r = philox(seed, ctr, 1u, (uint32_t)b, 0u);
         const float rsign = (r.x & 1u) ? 1.f : -1.f;
         const float rscale = u01(r.y) * (ratio_mul - 1.f) + 1.f;
@@ -249,14 +243,18 @@ mask_rng_fill_kernel(int B, int S, float p_centre, const uint64_t* __restrict__ 
     centres[i] = u01(q.x) < p_centre ? 1.f : 0.f;
 }
 
-// rendered_mask = 1 - all(rendered == 0 over channels)   (demo.py:146)
+// all_positive = 0: rendered_mask = 1 - all(rendered == 0 over channels)   (demo.py:146, smirk_trainer.py:77)
+// all_positive = 1: rendered_mask = all(rendered > 0 over channels)          (smirk_trainer.py:290)
+// Neither is the complement of the other: a pixel with one zero channel is 1 under the first rule and 0 under the second.
 __global__ void __launch_bounds__(256)
-mask_rendered_kernel(const float* __restrict__ rendered, int B, int S, float* __restrict__ rmask) {
+mask_rendered_kernel(const float* __restrict__ rendered, int B, int S, int all_positive, float* __restrict__ rmask) {
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long)B * S * S) return;
     const int b = (int)(i / ((long)S * S)); const long pix = i - (long)b * S * S;
     const float* r = rendered + (size_t)b * 3 * S * S + pix;
-    const bool bg = r[0] == 0.f && r[(size_t)S * S] == 0.f && r[(size_t)2 * S * S] == 0.f;
+    const float r0 = r[0], r1 = r[(size_t)S * S], r2 = r[(size_t)2 * S * S];
+    if (all_positive) { rmask[i] = (r0 > 0.f && r1 > 0.f && r2 > 0.f) ? 1.f : 0.f; return; }
+    const bool bg = r0 == 0.f && r1 == 0.f && r2 == 0.f;
     rmask[i] = bg ? 0.f : 1.f;
 }
 
@@ -276,18 +274,18 @@ mask_transfer_winner_kernel(const int64_t* __restrict__ p2, const int64_t* __res
     atomicMax(winner + ((size_t)b * S + y) * S + x, j);
 }
 __global__ void __launch_bounds__(256)
-mask_transfer_copy_kernel(const float* __restrict__ img, const int64_t* __restrict__ p1, const int* __restrict__ winner, int B, int N, int S,
+mask_transfer_copy_kernel(const float* __restrict__ img, const int64_t* __restrict__ p1, const int* __restrict__ winner, int B, int Bsrc, int N, int S,
                           float* __restrict__ out) {
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long)B * S * S) return;
     const int b = (int)(i / ((long)S * S)); const long pix = i - (long)b * S * S;
+    const int bs = b % Bsrc;                            // source image and points1 of row b: row b mod Bsrc
     const int j = winner[i];
     int64_t sx = 0, sy = 0;
-    if (j >= 0) { sx = p1[((size_t)b * N + j) * 2]; sy = p1[((size_t)b * N + j) * 2 + 1]; }
+    if (j >= 0) { sx = p1[((size_t)bs * N + j) * 2]; sy = p1[((size_t)bs * N + j) * 2 + 1]; }
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) {
-        const size_t o = ((size_t)b * 3 + ch) * S * S;
-        out[o + pix] = j >= 0 ? img[o + (size_t)sy * S + sx] : 0.f;
+        out[((size_t)b * 3 + ch) * S * S + pix] = j >= 0 ? img[((size_t)bs * 3 + ch) * S * S + (size_t)sy * S + sx] : 0.f;
     }
 }
 
@@ -345,24 +343,19 @@ extern "C" int smk_masking_face_weights(const SmkMasking* h, const float* trans_
     return 0;
 }
 
-extern "C" int smk_masking_points(const SmkMasking* h, const float* trans_verts, const int64_t* face_idx, const float* bary,
-                                  int B, int N, int image_size, int64_t* npoints, void* stream) {
-    if (B == 0 || N == 0) return 0;
-    SMK_REQUIRE(h && trans_verts && face_idx && bary && npoints && image_size > 0, "smk_masking_points: bad argument");
-    cudaStream_t st = (cudaStream_t)stream;
+namespace {
+
+int points_impl(const SmkMasking* h, const float* tv, const int64_t* fidx, const float* bary, int B, int Bsrc, int N, int S,
+                int64_t* npoints, cudaStream_t st) {
     SMK_TAG("mask_points", 36.0 * B * N, 0.0, st);
-    SMK_LAUNCH(mask_points_kernel, dim3(smk::cdiv((long)B * N, 256)), dim3(256), 0, st, h->d, trans_verts, face_idx, bary, B, N, image_size, npoints);
+    SMK_LAUNCH(mask_points_kernel, dim3(smk::cdiv((long)B * N, 256)), dim3(256), 0, st, h->d, tv, fidx, bary, B, Bsrc, N, S, npoints);
     SMK_CHECK_LAUNCH();
     return 0;
 }
 
-extern "C" int smk_masking_transfer_pixels(const float* img, const int64_t* points1, const int64_t* points2, const int64_t* rbound,
-                                           int B, int N, int S, float* out, void* ws, size_t ws_bytes, void* stream) {
-    if (B == 0) return 0;
-    SMK_REQUIRE(img && out && (N == 0 || (points1 && points2)) && S > 0, "smk_masking_transfer_pixels: bad argument");
-    SMK_REQUIRE(ws && ws_bytes >= (size_t)B * S * S * sizeof(int), "smk_masking_transfer_pixels: workspace too small (B*S*S ints)");
-    cudaStream_t st = (cudaStream_t)stream;
-    int* winner = reinterpret_cast<int*>(ws);
+// winner: B*S*S ints of scratch
+int transfer_impl(const float* img, const int64_t* points1, const int64_t* points2, const int64_t* rbound, int B, int Bsrc, int N, int S,
+                  float* out, int* winner, cudaStream_t st) {
     SMK_CHECK_CUDA(cudaMemsetAsync(winner, 0xFF, (size_t)B * S * S * sizeof(int), st));        // -1
     if (N > 0) {
         SMK_TAG("mask_transfer_winner", 20.0 * B * N, 0.0, st);
@@ -370,19 +363,16 @@ extern "C" int smk_masking_transfer_pixels(const float* img, const int64_t* poin
         SMK_CHECK_LAUNCH();
     }
     SMK_TAG("mask_transfer_copy", 4.0 * B * S * S * 5.0, 0.0, st);
-    SMK_LAUNCH(mask_transfer_copy_kernel, dim3(smk::cdiv((long)B * S * S, 256)), dim3(256), 0, st, img, points1, (const int*)winner, B, N, S, out);
+    SMK_LAUNCH(mask_transfer_copy_kernel, dim3(smk::cdiv((long)B * S * S, 256)), dim3(256), 0, st, img, points1, (const int*)winner, B, Bsrc, N, S, out);
     SMK_CHECK_LAUNCH();
     return 0;
 }
 
-extern "C" int smk_masking_compose(const SmkMasking* h, const float* img, const float* hull, const int64_t* npoints, const int64_t* rbound,
-                                   int N, const float* extra_points, const float* rendered_mask, const float* noise_mult, const float* random_centres,
-                                   int wr, int B, int S, float* masked, void* ws, size_t ws_bytes, void* stream) {
-    if (B == 0) return 0;
-    SMK_REQUIRE(h && img && hull && masked && (N == 0 || extra_points || (npoints && rbound)) && wr >= 0 && S > 0, "smk_masking_compose: bad argument");
+// ws: smk_masking_workspace_bytes(h, B, S); img and hull rows are those of image b mod Bsrc
+int compose_impl(const SmkMasking* h, const float* img, const float* hull, const int64_t* npoints, const int64_t* rbound, int N,
+                 const float* extra_points, const float* rendered_mask, const float* noise_mult, const float* random_centres,
+                 int wr, int B, int Bsrc, int S, float* masked, void* ws, size_t ws_bytes, cudaStream_t st) {
     if (extra_points) N = 0;                            // the caller supplies extra_points (masking.py:71); no point mask to build
-    SMK_REQUIRE(ws && ws_bytes >= smk_masking_workspace_bytes(h, B, S), "smk_masking_compose: workspace too small");
-    cudaStream_t st = (cudaStream_t)stream;
     smk::Workspace w(ws, ws_bytes);
     w.take<float>((size_t)B * h->d.V * 3);                              // (normals slot, unused here)
     float* th = w.take<float>((size_t)B * S * S);
@@ -397,13 +387,53 @@ extern "C" int smk_masking_compose(const SmkMasking* h, const float* img, const 
         SMK_CHECK_LAUNCH();
     }
     SMK_TAG("mask_hmax", 16.0 * npx, 0.0, st);
-    SMK_LAUNCH(mask_hmax_kernel, dim3(smk::cdiv(npx, 256)), dim3(256), 0, st, hull, random_centres, B, S, wr, th, tc);
+    SMK_LAUNCH(mask_hmax_kernel, dim3(smk::cdiv(npx, 256)), dim3(256), 0, st, hull, random_centres, B, Bsrc, S, wr, th, tc);
     SMK_CHECK_LAUNCH();
     SMK_TAG("mask_compose", 4.0 * npx * (3 + 3 + 2 + (noise_mult ? 3 : 0)), 0.0, st);
     SMK_LAUNCH(mask_compose_kernel, dim3(smk::cdiv(npx, 256)), dim3(256), 0, st, img, (const float*)th, (const float*)(random_centres ? tc : nullptr),
-               (const uint8_t*)pm, extra_points, rendered_mask, noise_mult, B, S, wr, masked);
+               (const uint8_t*)pm, extra_points, rendered_mask, noise_mult, B, Bsrc, S, wr, masked);
     SMK_CHECK_LAUNCH();
     return 0;
+}
+
+// The face weights of trans_verts [B] and N inverse-CDF samples per image into fidx / bary; rbound NULL = keep every point.
+int sample_impl(const SmkMasking* h, const float* tv, const float* base_prob, int B, int N, float ratio_mul, const uint64_t* rng,
+                float* weights, int64_t* fidx, float* bary, int64_t* rbound, void* ws, size_t ws_bytes, cudaStream_t st) {
+    const MaskDev& d = h->d;
+    if (int rc = smk_masking_face_weights(h, tv, base_prob, B, weights, ws, ws_bytes, st)) return rc;
+    SMK_CHECK_CUDA(smk::set_max_dynamic_smem<mask_sample_kernel>(160 * 1024));
+    SMK_TAG("mask_sample", 4.0 * B * d.F + 36.0 * B * N, 0.0, st);
+    SMK_LAUNCH(mask_sample_kernel, dim3(B), dim3(512), (size_t)d.F * sizeof(float), st, (const float*)weights, d.F, N, ratio_mul,
+               rng, fidx, bary, rbound);
+    SMK_CHECK_LAUNCH();
+    return 0;
+}
+
+}  // namespace
+
+extern "C" int smk_masking_points(const SmkMasking* h, const float* trans_verts, const int64_t* face_idx, const float* bary,
+                                  int B, int N, int image_size, int64_t* npoints, void* stream) {
+    if (B == 0 || N == 0) return 0;
+    SMK_REQUIRE(h && trans_verts && face_idx && bary && npoints && image_size > 0, "smk_masking_points: bad argument");
+    return points_impl(h, trans_verts, face_idx, bary, B, B, N, image_size, npoints, (cudaStream_t)stream);
+}
+
+extern "C" int smk_masking_transfer_pixels(const float* img, const int64_t* points1, const int64_t* points2, const int64_t* rbound,
+                                           int B, int N, int S, float* out, void* ws, size_t ws_bytes, void* stream) {
+    if (B == 0) return 0;
+    SMK_REQUIRE(img && out && (N == 0 || (points1 && points2)) && S > 0, "smk_masking_transfer_pixels: bad argument");
+    SMK_REQUIRE(ws && ws_bytes >= (size_t)B * S * S * sizeof(int), "smk_masking_transfer_pixels: workspace too small (B*S*S ints)");
+    return transfer_impl(img, points1, points2, rbound, B, B, N, S, out, reinterpret_cast<int*>(ws), (cudaStream_t)stream);
+}
+
+extern "C" int smk_masking_compose(const SmkMasking* h, const float* img, const float* hull, const int64_t* npoints, const int64_t* rbound,
+                                   int N, const float* extra_points, const float* rendered_mask, const float* noise_mult, const float* random_centres,
+                                   int wr, int B, int S, float* masked, void* ws, size_t ws_bytes, void* stream) {
+    if (B == 0) return 0;
+    SMK_REQUIRE(h && img && hull && masked && (N == 0 || extra_points || (npoints && rbound)) && wr >= 0 && S > 0, "smk_masking_compose: bad argument");
+    SMK_REQUIRE(ws && ws_bytes >= smk_masking_workspace_bytes(h, B, S), "smk_masking_compose: workspace too small");
+    return compose_impl(h, img, hull, npoints, rbound, N, extra_points, rendered_mask, noise_mult, random_centres, wr, B, B, S, masked, ws,
+                        ws_bytes, (cudaStream_t)stream);
 }
 
 extern "C" size_t smk_masking_forward_workspace_bytes(const SmkMasking* h, int B, int S, int N) {
@@ -435,21 +465,76 @@ extern "C" int smk_masking_forward(const SmkMasking* h, const float* img, const 
     float* centres = dbg_centres ? dbg_centres : w.take<float>((size_t)npx);
     float* rmask = w.take<float>((size_t)npx);
     SMK_REQUIRE(rmask != nullptr, "smk_masking_forward: workspace carve-up failed");
-    if (int rc = smk_masking_face_weights(h, trans_verts, base_prob, B, weights, ws, base, stream)) return rc;
-    SMK_CHECK_CUDA(smk::set_max_dynamic_smem<mask_sample_kernel>(160 * 1024));
-    SMK_TAG("mask_sample", 4.0 * B * d.F + 36.0 * B * N, 0.0, st);
-    SMK_LAUNCH(mask_sample_kernel, dim3(B), dim3(512), (size_t)d.F * sizeof(float), st, (const float*)weights, d.F, N, ratio_mul,
-               (const uint64_t*)rng_state, fidx, bary, rbound);
-    SMK_CHECK_LAUNCH();
-    if (int rc = smk_masking_points(h, trans_verts, fidx, bary, B, N, S, npoints, stream)) return rc;
+    if (int rc = sample_impl(h, trans_verts, base_prob, B, N, ratio_mul, rng_state, weights, fidx, bary, rbound, ws, base, st)) return rc;
+    if (int rc = points_impl(h, trans_verts, fidx, bary, B, B, N, S, npoints, st)) return rc;
     SMK_TAG("mask_rng_fill", 16.0 * npx, 0.0, st);
     SMK_LAUNCH(mask_rng_fill_kernel, dim3(smk::cdiv(npx, 256)), dim3(256), 0, st, B, S, p_centre, (const uint64_t*)rng_state, noise, centres);
     SMK_CHECK_LAUNCH();
     SMK_TAG("mask_rendered", 16.0 * npx, 0.0, st);
-    SMK_LAUNCH(mask_rendered_kernel, dim3(smk::cdiv(npx, 256)), dim3(256), 0, st, rendered, B, S, rmask);
+    SMK_LAUNCH(mask_rendered_kernel, dim3(smk::cdiv(npx, 256)), dim3(256), 0, st, rendered, B, S, 0, rmask);
     SMK_CHECK_LAUNCH();
-    if (int rc = smk_masking_compose(h, img, hull, npoints, rbound, N, nullptr, rmask, extra_noise ? noise : nullptr, p_centre > 0.f ? centres : nullptr,
-                                     wr, B, S, masked, ws, base, stream)) return rc;
+    if (int rc = compose_impl(h, img, hull, npoints, rbound, N, nullptr, rmask, extra_noise ? noise : nullptr, p_centre > 0.f ? centres : nullptr,
+                              wr, B, B, S, masked, ws, base, st)) return rc;
+    SMK_TAG("mask_rng_advance", 16.0, 0.0, st);
+    SMK_LAUNCH(mask_rng_advance_kernel, dim3(1), dim3(32), 0, st, rng_state);
+    SMK_CHECK_LAUNCH();
+    return 0;
+}
+
+// ---- the trainer's masking (include/smirk_b200_cycle.h) ----
+extern "C" size_t smk_masking_train_workspace_bytes(const SmkMasking* h, int B, int Ke, int S, int N) {
+    if (!h) return 0;
+    const size_t b = (size_t)(B > 0 ? B : 1), r = b * (size_t)(Ke > 0 ? Ke : 1), px = r * S * S, n = (size_t)(N > 0 ? N : 1);
+    return smk_masking_workspace_bytes(h, (int)r, S) + smk::ws_round(b * h->d.F * sizeof(float)) + smk::ws_round(b * n * 8) +
+           smk::ws_round(b * n * 12) + smk::ws_round(b * n * 16) + smk::ws_round(r * n * 16) + smk::ws_round(px * 12) +
+           smk::ws_round(px * 12) + 3 * smk::ws_round(px * 4) + 4096;
+}
+
+extern "C" int smk_masking_train_forward(const SmkMasking* h, int step, const float* img, const float* hull, const float* tv_first,
+                                         const float* tv_second, const float* rendered, const float* base_prob, int B, int Ke, int S, int N,
+                                         int wr, float p_centre, uint64_t* rng_state, float* masked, int64_t* dbg_face_idx, float* dbg_bary,
+                                         int64_t* dbg_points1, int64_t* dbg_points2, float* dbg_noise, float* dbg_centres, void* ws,
+                                         size_t ws_bytes, void* stream) {
+    SMK_REQUIRE(step == 1 || step == 2, "smk_masking_train_forward: step must be 1 or 2");
+    SMK_REQUIRE(B >= 0 && Ke >= 1 && (step == 2 || Ke == 1), "smk_masking_train_forward: bad batch (B >= 0, Ke >= 1, step 1 needs Ke == 1)");
+    if (B == 0) return 0;
+    SMK_REQUIRE(h && img && hull && tv_first && rendered && base_prob && rng_state && masked, "smk_masking_train_forward: null argument");
+    SMK_REQUIRE((step == 2) == (tv_second != nullptr), "smk_masking_train_forward: tv_second is required by step 2 and only by it");
+    SMK_REQUIRE(N > 0 && S > 0 && wr >= 0 && p_centre >= 0.f && p_centre <= 1.f, "smk_masking_train_forward: bad sizes");
+    SMK_REQUIRE(ws && ws_bytes >= smk_masking_train_workspace_bytes(h, B, Ke, S, N), "smk_masking_train_forward: workspace too small");
+    SMK_REQUIRE((size_t)h->d.F * sizeof(float) <= 160 * 1024, "smk_masking_train_forward: too many faces for the shared-memory CDF");
+    cudaStream_t st = (cudaStream_t)stream;
+    const MaskDev& d = h->d;
+    const int R = B * Ke;
+    const long npx = (long)R * S * S;
+    const size_t base = smk_masking_workspace_bytes(h, R, S);
+    smk::Workspace w((char*)ws + base, ws_bytes - base);
+    float* weights = w.take<float>((size_t)B * d.F);
+    int64_t* fidx = dbg_face_idx ? dbg_face_idx : w.take<int64_t>((size_t)B * N);
+    float* bary = dbg_bary ? dbg_bary : w.take<float>((size_t)B * N * 3);
+    int64_t* points1 = dbg_points1 ? dbg_points1 : w.take<int64_t>((size_t)B * N * 2);
+    int64_t* points2 = step == 1 ? points1 : (dbg_points2 ? dbg_points2 : w.take<int64_t>((size_t)R * N * 2));
+    float* extra = w.take<float>((size_t)npx * 3);
+    float* noise = dbg_noise ? dbg_noise : w.take<float>((size_t)npx * 3);
+    float* centres = dbg_centres ? dbg_centres : w.take<float>((size_t)npx);
+    float* rmask = w.take<float>((size_t)npx);
+    int* winner = w.take<int>((size_t)npx);
+    SMK_REQUIRE(winner != nullptr && points2 != nullptr, "smk_masking_train_forward: workspace carve-up failed");
+    // smirk_trainer.py:80-84 / 268-271: all int(mask_ratio * S^2) samples are kept (no rbound)
+    if (int rc = sample_impl(h, tv_first, base_prob, B, N, 1.f, rng_state, weights, fidx, bary, nullptr, ws, base, st)) return rc;
+    if (int rc = points_impl(h, tv_first, fidx, bary, B, B, N, S, points1, st)) return rc;
+    if (step == 2)                                      // :275-283: the same draws (repeated Ke times) on the second path's mesh
+        if (int rc = points_impl(h, tv_second, fidx, bary, R, B, N, S, points2, st)) return rc;
+    // :87 transfer_pixels(img, npoints, npoints) / :287 transfer_pixels(img.repeat(Ke), points1.repeat(Ke), points2)
+    if (int rc = transfer_impl(img, points1, points2, nullptr, R, B, N, S, extra, winner, st)) return rc;
+    SMK_TAG("mask_rng_fill", 16.0 * npx, 0.0, st);
+    SMK_LAUNCH(mask_rng_fill_kernel, dim3(smk::cdiv(npx, 256)), dim3(256), 0, st, R, S, p_centre, (const uint64_t*)rng_state, noise, centres);
+    SMK_CHECK_LAUNCH();
+    SMK_TAG("mask_rendered", 16.0 * npx, 0.0, st);
+    SMK_LAUNCH(mask_rendered_kernel, dim3(smk::cdiv(npx, 256)), dim3(256), 0, st, rendered, R, S, step == 2 ? 1 : 0, rmask);
+    SMK_CHECK_LAUNCH();
+    if (int rc = compose_impl(h, img, hull, nullptr, nullptr, 0, extra, rmask, noise, p_centre > 0.f ? centres : nullptr, wr, R, B, S,
+                              masked, ws, base, st)) return rc;
     SMK_TAG("mask_rng_advance", 16.0, 0.0, st);
     SMK_LAUNCH(mask_rng_advance_kernel, dim3(1), dim3(32), 0, st, rng_state);
     SMK_CHECK_LAUNCH();

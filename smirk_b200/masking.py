@@ -193,3 +193,82 @@ class MaskingStage(_lib.NativeModule):
         return (out, dbg) if debug else out
 
     __call__ = forward
+
+
+class TrainMaskingStage(_lib.NativeModule):
+    """The reference trainer's masking (``src/smirk_trainer.py``: step1 at :76-92, step2 at :262-293) as one capturable
+    device call per path, every random draw made on the device by the counter-based generator of ``MaskingStage``
+    (``include/smirk_b200_cycle.h``).  Unlike the demo's step it keeps all ``int(mask_ratio * S^2)`` sampled points, and
+    the second path moves the pixels under points sampled on the first path's mesh onto the augmented mesh.
+
+    ``first_path(img, hull_mask, transformed_vertices, rendered_img)``: ``masking(img, hull, transfer_pixels(img, p, p),
+    wr, rendered_mask = 1 - all(rendered == 0), random_mask = 0.01)``.
+    ``second_path(img, hull_mask, transformed_vertices, transformed_vertices_2nd, rendered_img_2nd, Ke)``: points sampled on
+    ``transformed_vertices`` [B] and placed on ``transformed_vertices_2nd`` [Ke*B]; ``transfer_pixels(img.repeat(Ke),
+    points1.repeat(Ke), points2)``, ``rendered_mask = all(rendered_2nd > 0)``, ``random_mask = 0.005``; [Ke*B,3,S,S] out.
+    ``rng_state`` = (seed, call counter) lives in device memory and each call advances the counter on the stream."""
+
+    FIRST_RANDOM_MASK, SECOND_RANDOM_MASK = 0.01, 0.005          # smirk_trainer.py:90 (masking()'s default), :293
+    DEBUG_KEYS = ("sampled_faces_indices", "barycentric_coords", "points1", "points2", "noise_mult", "random_centres")
+
+    def __init__(self, flame_faces, face_probabilities, mask_ratio=0.01, mask_dilation_radius=10, image_size=224, seed=0, n_verts=5023):
+        self.faces = flame_faces.detach().to("cpu", torch.int64)
+        self.n_verts, self.S, self.wr = int(n_verts), int(image_size), int(mask_dilation_radius)
+        self.base_prob_host = face_probabilities.detach().to("cpu", torch.float32).contiguous()
+        self.N = int(mask_ratio * image_size * image_size)                   # masking.py:140
+        self.seed = int(seed)
+
+    def _native_key(self, device):
+        return ()
+
+    def _native_create(self, device):
+        return MaskingContext(self.faces, self.n_verts, device)
+
+    _state = MaskingStage._state
+    reseed = MaskingStage.reseed
+
+    def graph_keep_alive(self):
+        return (self._native.handle,) + tuple(w.buf for w in self._native.workspaces.values())
+
+    def _check(self, name, t, shape):
+        if tuple(t.shape) != tuple(shape):
+            raise RuntimeError("smirk_b200.TrainMaskingStage: %s must be %s, got %s" % (name, list(shape), list(t.shape)))
+
+    @torch.no_grad()
+    def _run(self, step, img, hull_mask, tv, tv2, rendered, Ke, debug):
+        _lib.require_cuda(img, "img")
+        dev = img.device
+        img, hull, tv, rend = (_lib.dev_f32(t, n) for t, n in ((img, "img"), (hull_mask, "hull_mask"), (tv, "transformed_vertices"),
+                                                                (rendered, "rendered_img")))
+        B, S, N, R = img.shape[0], self.S, self.N, img.shape[0] * Ke
+        self._check("img", img, (B, 3, S, S))
+        self._check("hull_mask", hull, (B, 1, S, S))
+        self._check("transformed_vertices", tv, (B, self.n_verts, 3))
+        self._check("rendered_img", rend, (R, 3, S, S))
+        if tv2 is not None:
+            tv2 = _lib.dev_f32(tv2, "transformed_vertices_2nd")
+            self._check("transformed_vertices_2nd", tv2, (R, self.n_verts, 3))
+        ctx, base_prob, rng = self._state(dev)
+        out = torch.empty(R, 3, S, S, dtype=torch.float32, device=dev)
+        dbg = {}
+        if debug:
+            i64 = lambda *s: torch.empty(*s, dtype=torch.int64, device=dev)
+            f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+            dbg = dict(sampled_faces_indices=i64(B, N), barycentric_coords=f32(B, N, 3), points1=i64(B, N, 2),
+                       noise_mult=f32(R, 3, S, S), random_centres=f32(R, 1, S, S))
+            if step == 2:
+                dbg["points2"] = i64(R, N, 2)
+        p = self.FIRST_RANDOM_MASK if step == 1 else self.SECOND_RANDOM_MASK
+        nbytes = _lib.call("smk_masking_train_workspace_bytes", dev, ctx.handle, B, Ke, S, N)
+        ws = self._native_workspace("step%d" % step, nbytes, dev)
+        _lib.call("smk_masking_train_forward", dev, ctx.handle, step, img, hull, tv, tv2, rend, base_prob, B, Ke, S, N, self.wr, p,
+                  rng, out, *[dbg.get(k) for k in self.DEBUG_KEYS], ws, ws.numel())
+        return (out, dbg) if debug else out
+
+    def first_path(self, img, hull_mask, transformed_vertices, rendered_img, debug=False):
+        return self._run(1, img, hull_mask, transformed_vertices, None, rendered_img, 1, debug)
+
+    def second_path(self, img, hull_mask, transformed_vertices, transformed_vertices_2nd, rendered_img_2nd, Ke=1, debug=False):
+        if int(Ke) < 1:
+            raise RuntimeError("smirk_b200.TrainMaskingStage: Ke must be >= 1")
+        return self._run(2, img, hull_mask, transformed_vertices, transformed_vertices_2nd, rendered_img_2nd, int(Ke), debug)
