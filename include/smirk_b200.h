@@ -267,6 +267,53 @@ size_t smk_generator_backward_workspace_bytes(const SmkGenerator* h, int B);
 int smk_generator_backward(const SmkGenerator* h, int B, const float* y, const float* saved, size_t saved_bytes,
                            const float* g_y, float* g_x, void* ws, size_t ws_bytes, void* stream);
 
+/* Train mode (BatchNorm over batch statistics, the reference trainer's generator.train(), base_trainer.py:108-111) and the
+ * gradients of every parameter (src/smirk_trainer.py:94,295).
+ * A train handle holds the topology only (the configuration and precision of SmkGeneratorDesc) and is destroyed by
+ * smk_generator_destroy.  Every call reads the parameters through the device pointers of SmkGeneratorTrainArgs and repacks
+ * the weights into the workspace, so an optimizer step needs no new handle.  Calls never allocate or synchronise, use no
+ * float atomics (bitwise reproducible) and are CUDA-graph capturable; the eval entry points above reject a train handle.
+ * BatchNorm couples the images of a batch: outputs are not independent of the other images. */
+typedef struct {
+    /* DEVICE pointers of the module's state_dict tensors in the order of SmkGeneratorDesc.tensors (num_batches_tracked
+     * removed); running_mean / running_var are updated in place.                                                      */
+    float* const* tensors;
+    int n_tensors;
+    int64_t* const* num_batches_tracked;   /* one per BatchNorm, in state_dict order; each is incremented by one */
+    float momentum;            /* running-statistics factor of every BatchNorm; negative = None (1 / num_batches_tracked) */
+    float eps;
+} SmkGeneratorTrainArgs;
+typedef struct {
+    /* Gradient outputs (written, not accumulated), NULL = not wanted: tensors[j] is the gradient of
+     * SmkGeneratorTrainArgs.tensors[j]; the running-statistics entries must be NULL.                                  */
+    float* const* tensors;
+} SmkGeneratorTrainGrads;
+int smk_generator_train_create(int in_channels, int out_channels, int init_features, int res_blocks, int precision, SmkGenerator** out);
+/* Workspace of both train calls.  smk_generator_saved_bytes / smk_generator_saved_tensor describe the train handle's saved
+ * buffer: the NHWC input ("input", channels zero-padded), per conv its pre-BN output (named after the conv, e.g.
+ * "enc1conv1", "res0conv2") and per BatchNorm its (+ residual) (+ ReLU) output (named after the BatchNorm, e.g.
+ * "enc1norm1", "res0norm2"), each decoder's input ("dec1cat": torch.cat((upconv1 output, enc1norm2 output))) and each
+ * pool's output ("pool1"), followed by the batch statistics (not listed). */
+size_t smk_generator_train_workspace_bytes(const SmkGenerator* h, int B);
+/* Train-mode forward: x [B,in_channels,224,224] -> y as smk_generator_forward; updates the running statistics and
+ * num_batches_tracked of every BatchNorm.  saved (>= smk_generator_saved_bytes) keeps the activations for
+ * smk_generator_backward_train; with saved == NULL they live in ws, which must then hold smk_generator_saved_bytes more. */
+int smk_generator_forward_train(const SmkGenerator* h, const SmkGeneratorTrainArgs* args, const float* x, int B, float* y,
+                                float* saved, size_t saved_bytes, void* ws, size_t ws_bytes, void* stream);
+/* Train-mode backward from the forward's saved buffer and output y (args: those of the forward).  g_y [B,out_channels,
+ * 224,224]; g_x [B,in_channels,224,224] (NULL: not wanted, and the first conv's dgrad does not run) is written. */
+int smk_generator_backward_train(const SmkGenerator* h, const SmkGeneratorTrainArgs* args, int B, const float* y, const float* saved,
+                                 size_t saved_bytes, const float* g_y, float* g_x, const SmkGeneratorTrainGrads* grads, void* ws,
+                                 size_t ws_bytes, void* stream);
+
+/* Test entry point of the train path's 3x3 weight gradient (tests/test_gpu_generator_train_kernels.py; not part of the
+ * drop-in surface).  Device pointers; it calls the host helper the train backward uses.  g [B,H,W,cout] (the gradient
+ * of the conv's output), a [B,H,W,lda] (the conv's input, its first cin channels) -> out [cout][cin][3][3] (torch's
+ * layout), 3x3 stride 1 with zero padding 1 (reflect 0) or ReflectionPad2d(1) (reflect 1).  ws: kWgradPart floats
+ * (16 MiB) of split-K partials. */
+int smk_debug_train_conv3_wgrad(const float* g, const float* a, int lda, int B, int H, int W, int cin, int cout, int reflect, float* out,
+                                void* ws, size_t ws_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Crop / warp front and back end (SURVEY.md 8f #2) — replaces the CPU `skimage.transform.warp` calls of
  * demo.py:97 and demo_video.py:128,149 (+ BGR->RGB, /255, HWC->CHW of demo.py:103-105) for frames that are
@@ -350,6 +397,173 @@ int smk_masking_forward(const SmkMasking* h, const float* img, const float* hull
                         const float* base_prob, int B, int S, int N, int wr, float ratio_mul, float p_centre, int extra_noise,
                         uint64_t* rng_state, float* masked, int64_t* dbg_face_idx, float* dbg_bary, int64_t* dbg_npoints,
                         int64_t* dbg_rbound, float* dbg_noise, float* dbg_centres, void* ws, size_t ws_bytes, void* stream);
+
+/* The reference trainer's masking and the cycle path's parameter augmentation, with every random draw made on the device.
+ * Randomness: a counter-based generator (Philox4x32-10) keyed by rng_state = {seed, call counter}, two uint64 in device
+ * memory.  Every call advances the counter on the stream, so a captured CUDA graph draws fresh numbers on every replay
+ * and a given (seed, counter) always gives the same bits.  The draws are equal in distribution to the reference's torch
+ * draws, not equal to them; given the draws the optional debug pointers export, every output equals the reference's
+ * fp32 arithmetic bit for bit.  Calls never allocate or synchronise with the host and are CUDA-graph capturable. */
+/* ---- the trainer's masking (src/smirk_trainer.py:76-92 step1, :262-293 step2), on a SmkMasking handle ----
+ * N = int(mask_ratio * S * S) points per image, all of them kept (no rbound budget); faces by inverse CDF of the face
+ * weights (masking.py:146-160) of tv_first [B,V,3], uniform reflected barycentrics.  R = Ke * B output rows; row r uses
+ * the draws, image, hull and tv_first points of row r mod B (torch's .repeat(Ke)).
+ *   step 1 (Ke == 1, tv_second NULL): points = points(tv_first); extra = transfer_pixels(img, points, points);
+ *           masked = masking(img, hull, extra, wr, rendered_mask = 1 - all(rendered == 0), extra_noise, random_mask = p_centre)
+ *   step 2: points1 = points(tv_first), points2 = points(tv_second [R,V,3]);
+ *           extra = transfer_pixels(img.repeat(Ke), points1.repeat(Ke), points2)   (duplicate targets: the last pair wins)
+ *           masked = masking(img.repeat(Ke), hull.repeat(Ke), extra, wr, rendered_mask = all(rendered > 0), extra_noise,
+ *                            random_mask = p_centre)
+ * img [B,3,S,S], hull [B,1,S,S], rendered [R,3,S,S] (step 2: the second path's render), base_prob [F]; masked [R,3,S,S].
+ * Debug outputs (each nullable): face_idx int64 [B,N], bary [B,N,3], points1 int64 [B,N,2] (x, y), points2 int64 [R,N,2]
+ * (step 2 only), noise_mult [R,3,S,S] (randn * 0.05 + 1), centres [R,1,S,S] (Bernoulli(p_centre) patch centres). */
+size_t smk_masking_train_workspace_bytes(const SmkMasking* h, int B, int Ke, int S, int N);
+int smk_masking_train_forward(const SmkMasking* h, int step, const float* img, const float* hull, const float* tv_first,
+                              const float* tv_second, const float* rendered, const float* base_prob, int B, int Ke, int S, int N,
+                              int wr, float p_centre, uint64_t* rng_state, float* masked, int64_t* dbg_face_idx, float* dbg_bary,
+                              int64_t* dbg_points1, int64_t* dbg_points2, float* dbg_noise, float* dbg_centres, void* ws,
+                              size_t ws_bytes, void* stream);
+
+/* ---- the cycle path's parameter augmentation (src/smirk_trainer.py:189-248) ----
+ * Templates (src/utils/utils.py:load_templates): n_keys keys in dict order; key k owns rows row_offset[k] ..
+ * row_offset[k+1]-1 of rows [total][n_exp] (fp32, each row the first n_exp values of a template cast from fp64).     */
+typedef struct SmkCycle SmkCycle;
+typedef struct {
+    int n_keys;
+    const int32_t* row_offset;   /* host [n_keys + 1], row_offset[0] = 0, strictly increasing */
+    const float* rows;           /* host [row_offset[n_keys]][n_exp]                          */
+    int n_exp;                   /* num_expression: the columns a template injection overwrites  */
+} SmkCycleDesc;
+/* Every field nullable; R = Ke * B, groups of sizes n0 = R/4, n1 = 2R/4 - R/4, n2 = 3R/4 - 2R/4, n3 = R - 3R/4 (floors),
+ * E = the expression width.  Group-indexed draws are in group order (row k of group g is output row gids[start_g + k]). */
+typedef struct {
+    int64_t* gids;          /* [R]  the group permutation (torch.randperm(R))              */
+    int64_t* perm1;         /* [n1] the in-group permutation of group 1                     */
+    float* param_mask;      /* [n0,E] Bernoulli(0.5)                                        */
+    float* jaw_mask;        /* [R]    Bernoulli(0.5) of the jaw's scale_mask                */
+    float* randn0a;         /* [n0,E] group 0: the normal of new_expressions               */
+    float* randn0b;         /* [n0,E] group 0: the normal of the extra noise               */
+    float* randn1;          /* [n1,E] */
+    float* randn2;          /* [n2,E] */
+    float* randn3;          /* [n3,E] */
+    float* randn_jaw;       /* [R,3]  */
+    float* rand0a;          /* [n0]   U(0,1) draws: group 0's scale of new_expressions (1 + 2U) */
+    float* rand0b;          /* [n0]   group 0's noise scale (0.2U)                          */
+    float* rand1a;          /* [n1]   group 1's expression scale (0.25 + 1.25U)             */
+    float* rand1b;          /* [n1]   group 1's noise scale                                 */
+    float* rand2a;          /* [n2]   group 2's template scale (0.25 + 1.25U)               */
+    float* rand2b;          /* [n2]   group 2's noise scale                                 */
+    float* rand3;           /* [n3]   group 3's noise scale                                 */
+    float* rand_eyelid;     /* [R,2]  the eyelid tweak (use_eyelids)                        */
+    float* rand3_eyelid;    /* [n3,2] group 3's eyelids                                     */
+    int64_t* tmpl_key;      /* [n2]   key index of each template pick                       */
+    int64_t* tmpl_row;      /* [n2]   row within that key                                   */
+} SmkCycleDraws;
+int smk_cycle_create(const SmkCycleDesc* desc, SmkCycle** out);
+void smk_cycle_destroy(SmkCycle* h);
+/* Encoder outputs [B, dim] (dims[0..5]: pose, cam, shape, expression, jaw (3), eyelid (2)) -> flame_feats [Ke*B, dim]:
+ * pose, cam and shape copied from row r mod B; expression, jaw and eyelid augmented as the reference does.  One launch. */
+int smk_cycle_augment(const SmkCycle* h, const float* const* in, float* const* out, const int* dims, int B, int Ke, int use_eyelids,
+                      uint64_t* rng_state, const SmkCycleDraws* dbg, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * The trainer's frozen networks: VGGPerceptualLoss, MICA and ExpressionLoss.  create takes the host fp32 tensors of the
+ * module's state_dict (which ones: at each network) and uploads them to the current device; the weights are frozen and
+ * every BatchNorm runs in eval mode.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+    const float* const* tensors;   /* host fp32 tensors, in state_dict order */
+    int n_tensors;
+    int precision;             /* 0 = fp32 CUDA-core implicit GEMM, 1 = TF32 wgmma implicit GEMM,
+                                  3 = 1 with 3xTF32 error-compensated arithmetic (fp32-equivalent).  2 is not a precision. */
+} SmkNetDesc;
+
+/* VGGPerceptualLoss (src/losses/VGGPerceptualLoss.py) — replaces VGGPerceptualLoss.forward: sum over the taps relu1_2,
+ * relu2_2, relu3_3, relu4_3 of torchvision VGG16 features[:23] of l1_loss(phi(x), phi(y)), x and y normalised as
+ * (v * 0.5 + 0.5 - mean) / std.  The input gradient goes to x, y or both.
+ * Tensors (22): mean [1,3,1,1], std [1,3,1,1], then weight [cout,cin,3,3] and bias [cout] of the ten convolutions
+ * (blocks.0.0 ... blocks.3.21). */
+typedef struct SmkVggLoss SmkVggLoss;
+int smk_vgg_loss_create(const SmkNetDesc* desc, SmkVggLoss** out);
+void smk_vgg_loss_destroy(SmkVggLoss* h);
+size_t smk_vgg_loss_workspace_bytes(const SmkVggLoss* h, int B);
+/* x, y [B,3,224,224] NCHW -> loss, one fp32 device scalar (written).  x and y may be the same tensor.  Deterministic:
+ * no atomics, fixed summation order.  An empty batch (B = 0) is an argument error: the loss of nothing is undefined. */
+int smk_vgg_loss_forward(const SmkVggLoss* h, const float* x, const float* y, int B, float* loss,
+                         void* ws, size_t ws_bytes, void* stream);
+/* Grad-mode forward: the same launches and bitwise the same loss, plus what the backward needs in `saved` (caller-owned,
+ * >= smk_vgg_loss_saved_bytes): the post-ReLU output of every convolution, fp32 NHWC, for each half whose gradient is
+ * wanted, and per tap an int8 map of sign(phi(x) - phi(y)) (-1, 0, +1).  need: 1 = gradient to x, 2 = to y, 3 = both.
+ * ws / ws_bytes: the forward workspace (smk_vgg_loss_workspace_bytes). */
+size_t smk_vgg_loss_saved_bytes(const SmkVggLoss* h, int B, int need);
+int smk_vgg_loss_forward_saved(const SmkVggLoss* h, const float* x, const float* y, int B, int need, float* loss,
+                               float* saved, size_t saved_bytes, void* ws, size_t ws_bytes, void* stream);
+/* Layout of tensor i of `saved`: its name ("relu1_1" ... "relu4_3": fp32, dims B' = B per saved half (x's first when both),
+ * "sign1_2" ... "sign4_3": int8, dims B), offset in floats, and dims [4] = B,H,W,C of the NHWC tensor.  Returns non-zero
+ * past the last tensor. */
+int smk_vgg_loss_saved_tensor(const SmkVggLoss* h, int B, int need, int i, const char** name, size_t* offset, int* dims);
+/* Input gradient of the loss times the device scalar g: g_x and g_y [B,3,224,224] NCHW (written, not accumulated; the one
+ * `need` does not ask for may be null).  `need` and `saved` are those of the grad-mode forward.
+ * ws >= smk_vgg_loss_backward_workspace_bytes. */
+size_t smk_vgg_loss_backward_workspace_bytes(const SmkVggLoss* h, int B, int need);
+int smk_vgg_loss_backward(const SmkVggLoss* h, int B, int need, const float* saved, size_t saved_bytes, const float* g,
+                          float* g_x, float* g_y, void* ws, size_t ws_bytes, void* stream);
+
+/* MICA (src/models/MICA/mica.py): the frozen ArcFace iResNet-100 and shape regressor the pretraining step's MICA shape loss
+ * runs, forward only, and that loss, mse_loss(shape_params, mica_shape), with its gradient to shape_params.
+ * Tensors (781): the state_dict without num_batches_tracked: arcface.* (conv1, bn1, prelu, layer1.0 ... layer4.2, bn2,
+ * fc, features), then regressor.* (network.0 ... network.3, output). */
+typedef struct SmkMica SmkMica;
+int smk_mica_create(const SmkNetDesc* desc, SmkMica** out);
+void smk_mica_destroy(SmkMica* h);
+size_t smk_mica_workspace_bytes(const SmkMica* h, int B);
+/* images [B,3,112,112] NCHW (RGB in [0, 1]) -> shape_params [B,300]; features (optional, null: not written) [B,512]: the
+ * ArcFace embedding before F.normalize.  Eval-mode BatchNorm throughout.  Deterministic and batch-independent. */
+int smk_mica_forward(const SmkMica* h, const float* images, int B, float* shape_params, float* features,
+                     void* ws, size_t ws_bytes, void* stream);
+/* MICA shape loss over the first D columns: loss (one fp32 device scalar, written) = mean over b < B, d < D of
+ * (shape_params[b*D + d] - mica_shape[b*ld + d])^2.  One CTA, fixed summation order, no atomics. */
+int smk_mica_shape_loss_forward(const float* shape_params, const float* mica_shape, int B, int D, int ld, float* loss,
+                                void* stream);
+/* Its gradient times the device scalar g: grad [B,D] (written) = (2 / (B*D)) * (shape_params - mica_shape) * g. */
+int smk_mica_shape_loss_backward(const float* shape_params, const float* mica_shape, int B, int D, int ld, const float* g,
+                                 float* grad, void* stream);
+
+/* ExpressionLoss (src/losses/ExpressionLoss.py) — replaces ExpressionLoss.forward(gen, tar, use_mean, metric):
+ * f = backbone(x).view(B, -1), EMOCA's eval-mode ResNet-50 (Bottleneck layers (3, 4, 6, 3), the stride of each layer's
+ * first block on its 3x3 conv) up to the 7x7 average pool, on gen and tar [B,3,224,224] as they are; per face
+ * l2 = mean((f_gen - f_tar)^2), l1 = mean(|.|) or cos = 1 - cosine_similarity (eps 1e-8); use_mean: their mean over the
+ * faces.  The input gradient goes to gen, tar or both.
+ * Tensors (265): backbone.* in state_dict order, num_batches_tracked and backbone.fc.* left out: conv1.weight, bn1
+ * (weight, bias, running_mean, running_var), then per Bottleneck conv1, conv2, bn1, bn2, conv3, bn3 and, in the first
+ * block of each layer, downsample.0 and downsample.1. */
+typedef struct SmkExpressionLoss SmkExpressionLoss;
+int smk_expression_loss_create(const SmkNetDesc* desc, SmkExpressionLoss** out);
+void smk_expression_loss_destroy(SmkExpressionLoss* h);
+size_t smk_expression_loss_workspace_bytes(const SmkExpressionLoss* h, int B);
+/* gen, tar [B,3,224,224] NCHW -> loss: [B] per-face values, or one scalar (their mean) when use_mean.  metric: 0 = l2,
+ * 1 = l1, 2 = cos.  features (optional): [2B,2048], gen's then tar's.  Deterministic: no atomics, fixed summation
+ * orders; face b's value does not depend on the other faces. */
+int smk_expression_loss_forward(const SmkExpressionLoss* h, const float* gen, const float* tar, int B, int metric, int use_mean,
+                                float* loss, float* features, void* ws, size_t ws_bytes, void* stream);
+/* Grad-mode forward: the same launches and bitwise the same loss, plus what the backward needs in `saved` (caller-owned,
+ * >= smk_expression_loss_saved_bytes): for each image whose gradient is wanted, the pool output and its int8 argmax tap,
+ * and u1, u2 (the post-ReLU outputs of conv1 and conv2) and y of every block, fp32 NHWC; then both halves' features.
+ * need: 1 = gradient to gen, 2 = to tar, 3 = both.  ws / ws_bytes: the forward workspace. */
+size_t smk_expression_loss_saved_bytes(const SmkExpressionLoss* h, int B, int need);
+int smk_expression_loss_forward_saved(const SmkExpressionLoss* h, const float* gen, const float* tar, int B, int metric, int use_mean,
+                                      int need, float* loss, float* saved, size_t saved_bytes, void* ws, size_t ws_bytes, void* stream);
+/* Layout of tensor i of `saved`: its name ("pool", "pool_argmax" (int8), "layer1.0.u1" ... "layer4.2.y", dims B' = B per
+ * saved half, gen's first when both; last "features", dims [2B,1,1,2048]), offset in floats, and dims [4] = B,H,W,C of
+ * the NHWC tensor.  Returns non-zero past the last tensor. */
+int smk_expression_loss_saved_tensor(const SmkExpressionLoss* h, int B, int need, int i, const char** name, size_t* offset, int* dims);
+/* Input gradient of the loss times g ([B], or one scalar when use_mean): g_gen and g_tar [B,3,224,224] NCHW (written,
+ * not accumulated; the one `need` does not ask for may be null).  metric, use_mean, need and saved are those of the
+ * grad-mode forward.  ws >= smk_expression_loss_backward_workspace_bytes. */
+size_t smk_expression_loss_backward_workspace_bytes(const SmkExpressionLoss* h, int B, int need);
+int smk_expression_loss_backward(const SmkExpressionLoss* h, int B, int metric, int use_mean, int need, const float* saved,
+                                 size_t saved_bytes, const float* g, float* g_gen, float* g_tar, void* ws, size_t ws_bytes,
+                                 void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Peer-mapped gather buffers: the all-gather of the final outputs across the GPUs of one node (SURVEY.md 8e; the

@@ -1,6 +1,4 @@
-"""ctypes binding of libsmirk_b200.so (the C ABI declared in include/smirk_b200.h, include/smirk_b200_loss.h,
-include/smirk_b200_mica.h, include/smirk_b200_expression.h, include/smirk_b200_generator_train.h and
-include/smirk_b200_cycle.h).
+"""ctypes binding of libsmirk_b200.so (the C ABI declared in include/smirk_b200.h).
 
 There is deliberately no fallback: if the shared library is missing or a call fails, the product
 path raises.  Build with ``python -m smirk_b200.build`` (or ``__graft_entry__.build()``).
@@ -79,16 +77,13 @@ class SmkGeneratorTrainGrads(C.Structure):
     _fields_ = [("tensors", C.POINTER(c_f32p))]
 
 
-class SmkVggLossDesc(C.Structure):
+class SmkNetDesc(C.Structure):
     _fields_ = [("tensors", C.POINTER(c_f32p)), ("n_tensors", C.c_int), ("precision", C.c_int)]
 
 
-class SmkMicaDesc(C.Structure):
-    _fields_ = [("tensors", C.POINTER(c_f32p)), ("n_tensors", C.c_int), ("precision", C.c_int)]
-
-
-class SmkExpressionLossDesc(C.Structure):
-    _fields_ = [("tensors", C.POINTER(c_f32p)), ("n_tensors", C.c_int), ("precision", C.c_int)]
+# The names of the three frozen networks' descriptors from before they shared SmkNetDesc (the same layout), kept so that
+# code written against them still builds the descriptor.
+SmkVggLossDesc = SmkMicaDesc = SmkExpressionLossDesc = SmkNetDesc
 
 
 class SmkMaskingDesc(C.Structure):
@@ -100,7 +95,7 @@ class SmkCycleDesc(C.Structure):
 
 
 class SmkCycleDraws(C.Structure):
-    """Device pointers of the augmentation's exported draws (include/smirk_b200_cycle.h), in the header's field order."""
+    """Device pointers of the augmentation's exported draws (include/smirk_b200.h), in the header's field order."""
     FIELDS = ("gids", "perm1", "param_mask", "jaw_mask", "randn0a", "randn0b", "randn1", "randn2", "randn3", "randn_jaw",
               "rand0a", "rand0b", "rand1a", "rand1b", "rand2a", "rand2b", "rand3", "rand_eyelid", "rand3_eyelid", "tmpl_key", "tmpl_row")
     _fields_ = [(f, C.c_void_p) for f in FIELDS]
@@ -155,6 +150,12 @@ BINDINGS = [
     ("smk_generator_saved_tensor", _i, [_vp, _i, _i, C.POINTER(C.c_char_p), C.POINTER(_sz), C.POINTER(C.c_int)]),
     ("smk_generator_backward_workspace_bytes", _sz, [_vp, _i]),
     ("smk_generator_backward", _i, [_vp, _i, _vp, _vp, _sz, _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_generator_train_create", _i, [_i, _i, _i, _i, _i, _vpp]),
+    ("smk_generator_train_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_generator_forward_train", _i, [_vp, C.POINTER(SmkGeneratorTrainArgs), _vp, _i, _vp, _vp, _sz, _vp, _sz, STREAM]),
+    ("smk_generator_backward_train", _i, [_vp, C.POINTER(SmkGeneratorTrainArgs), _i, _vp, _vp, _sz, _vp, _vp,
+                                          C.POINTER(SmkGeneratorTrainGrads), _vp, _sz, STREAM]),
+    ("smk_debug_train_conv3_wgrad", _i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _sz, STREAM]),
     ("smk_warp_workspace_bytes", _sz, [_i]),
     ("smk_crop_warp", _i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _sz, STREAM]),
     ("smk_warp_u8", _i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _sz, STREAM]),
@@ -172,6 +173,36 @@ BINDINGS = [
     ("smk_masking_forward_workspace_bytes", _sz, [_vp, _i, _i, _i]),
     ("smk_masking_forward", _i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _f, _i, _vp, _vp, _vp, _vp, _vp, _vp,
                                  _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_masking_train_workspace_bytes", _sz, [_vp, _i, _i, _i, _i]),
+    ("smk_masking_train_forward", _i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp,
+                                       _vp, _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_cycle_create", _i, [C.POINTER(SmkCycleDesc), _vpp]),
+    ("smk_cycle_destroy", None, [_vp]),
+    ("smk_cycle_augment", _i, [_vp, _vpp, _vpp, C.POINTER(C.c_int), _i, _i, _i, _vp, C.POINTER(SmkCycleDraws), STREAM]),
+    ("smk_vgg_loss_create", _i, [C.POINTER(SmkNetDesc), _vpp]),
+    ("smk_vgg_loss_destroy", None, [_vp]),
+    ("smk_vgg_loss_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_vgg_loss_forward", _i, [_vp, _vp, _vp, _i, _vp, _vp, _sz, STREAM]),
+    ("smk_vgg_loss_saved_bytes", _sz, [_vp, _i, _i]),
+    ("smk_vgg_loss_forward_saved", _i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _sz, _vp, _sz, STREAM]),
+    ("smk_vgg_loss_saved_tensor", _i, [_vp, _i, _i, _i, C.POINTER(C.c_char_p), C.POINTER(_sz), C.POINTER(C.c_int)]),
+    ("smk_vgg_loss_backward_workspace_bytes", _sz, [_vp, _i, _i]),
+    ("smk_vgg_loss_backward", _i, [_vp, _i, _i, _vp, _sz, _vp, _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_mica_create", _i, [C.POINTER(SmkNetDesc), _vpp]),
+    ("smk_mica_destroy", None, [_vp]),
+    ("smk_mica_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_mica_forward", _i, [_vp, _vp, _i, _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_mica_shape_loss_forward", _i, [_vp, _vp, _i, _i, _i, _vp, STREAM]),
+    ("smk_mica_shape_loss_backward", _i, [_vp, _vp, _i, _i, _i, _vp, _vp, STREAM]),
+    ("smk_expression_loss_create", _i, [C.POINTER(SmkNetDesc), _vpp]),
+    ("smk_expression_loss_destroy", None, [_vp]),
+    ("smk_expression_loss_workspace_bytes", _sz, [_vp, _i]),
+    ("smk_expression_loss_forward", _i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, STREAM]),
+    ("smk_expression_loss_saved_bytes", _sz, [_vp, _i, _i]),
+    ("smk_expression_loss_forward_saved", _i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp, _sz, STREAM]),
+    ("smk_expression_loss_saved_tensor", _i, [_vp, _i, _i, _i, C.POINTER(C.c_char_p), C.POINTER(_sz), C.POINTER(C.c_int)]),
+    ("smk_expression_loss_backward_workspace_bytes", _sz, [_vp, _i, _i]),
+    ("smk_expression_loss_backward", _i, [_vp, _i, _i, _i, _i, _vp, _sz, _vp, _vp, _vp, _vp, _sz, STREAM]),
     ("smk_peer_alloc", _i, [_sz, _vpp, C.c_char_p]),
     ("smk_peer_free", _i, [_vp]),
     ("smk_peer_open", _i, [C.c_char_p, _vpp]),
@@ -198,60 +229,7 @@ BINDINGS = [
     ("smk_debug_train_stem_wgrad", _i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, STREAM]),
     ("smk_debug_train_head_backward", _i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, STREAM]),
 ]
-# The binding table of include/smirk_b200_loss.h (the trainer's losses), in that header's order, by the same rules.
-LOSS_BINDINGS = [
-    ("smk_vgg_loss_create", _i, [C.POINTER(SmkVggLossDesc), _vpp]),
-    ("smk_vgg_loss_destroy", None, [_vp]),
-    ("smk_vgg_loss_workspace_bytes", _sz, [_vp, _i]),
-    ("smk_vgg_loss_forward", _i, [_vp, _vp, _vp, _i, _vp, _vp, _sz, STREAM]),
-    ("smk_vgg_loss_saved_bytes", _sz, [_vp, _i, _i]),
-    ("smk_vgg_loss_forward_saved", _i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _sz, _vp, _sz, STREAM]),
-    ("smk_vgg_loss_saved_tensor", _i, [_vp, _i, _i, _i, C.POINTER(C.c_char_p), C.POINTER(_sz), C.POINTER(C.c_int)]),
-    ("smk_vgg_loss_backward_workspace_bytes", _sz, [_vp, _i, _i]),
-    ("smk_vgg_loss_backward", _i, [_vp, _i, _i, _vp, _sz, _vp, _vp, _vp, _vp, _sz, STREAM]),
-]
-# The binding table of include/smirk_b200_mica.h (MICA and its shape loss), in that header's order, by the same rules.
-MICA_BINDINGS = [
-    ("smk_mica_create", _i, [C.POINTER(SmkMicaDesc), _vpp]),
-    ("smk_mica_destroy", None, [_vp]),
-    ("smk_mica_workspace_bytes", _sz, [_vp, _i]),
-    ("smk_mica_forward", _i, [_vp, _vp, _i, _vp, _vp, _vp, _sz, STREAM]),
-    ("smk_mica_shape_loss_forward", _i, [_vp, _vp, _i, _i, _i, _vp, STREAM]),
-    ("smk_mica_shape_loss_backward", _i, [_vp, _vp, _i, _i, _i, _vp, _vp, STREAM]),
-]
-# The binding table of include/smirk_b200_expression.h (the emotion loss), in that header's order, by the same rules.
-EXPRESSION_BINDINGS = [
-    ("smk_expression_loss_create", _i, [C.POINTER(SmkExpressionLossDesc), _vpp]),
-    ("smk_expression_loss_destroy", None, [_vp]),
-    ("smk_expression_loss_workspace_bytes", _sz, [_vp, _i]),
-    ("smk_expression_loss_forward", _i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, STREAM]),
-    ("smk_expression_loss_saved_bytes", _sz, [_vp, _i, _i]),
-    ("smk_expression_loss_forward_saved", _i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp, _sz, STREAM]),
-    ("smk_expression_loss_saved_tensor", _i, [_vp, _i, _i, _i, C.POINTER(C.c_char_p), C.POINTER(_sz), C.POINTER(C.c_int)]),
-    ("smk_expression_loss_backward_workspace_bytes", _sz, [_vp, _i, _i]),
-    ("smk_expression_loss_backward", _i, [_vp, _i, _i, _i, _i, _vp, _sz, _vp, _vp, _vp, _vp, _sz, STREAM]),
-]
-# The binding table of include/smirk_b200_generator_train.h (the generator's train mode), in that header's order, by the same rules.
-GENERATOR_TRAIN_BINDINGS = [
-    ("smk_generator_train_create", _i, [_i, _i, _i, _i, _i, _vpp]),
-    ("smk_generator_train_workspace_bytes", _sz, [_vp, _i]),
-    ("smk_generator_forward_train", _i, [_vp, C.POINTER(SmkGeneratorTrainArgs), _vp, _i, _vp, _vp, _sz, _vp, _sz, STREAM]),
-    ("smk_generator_backward_train", _i, [_vp, C.POINTER(SmkGeneratorTrainArgs), _i, _vp, _vp, _sz, _vp, _vp,
-                                          C.POINTER(SmkGeneratorTrainGrads), _vp, _sz, STREAM]),
-    ("smk_debug_train_conv3_wgrad", _i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _sz, STREAM]),
-]
-# The binding table of include/smirk_b200_cycle.h (the trainer's masking and the cycle augmentation), in that header's order,
-# by the same rules.
-CYCLE_BINDINGS = [
-    ("smk_masking_train_workspace_bytes", _sz, [_vp, _i, _i, _i, _i]),
-    ("smk_masking_train_forward", _i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp,
-                                       _vp, _vp, _vp, _vp, _sz, STREAM]),
-    ("smk_cycle_create", _i, [C.POINTER(SmkCycleDesc), _vpp]),
-    ("smk_cycle_destroy", None, [_vp]),
-    ("smk_cycle_augment", _i, [_vp, _vpp, _vpp, C.POINTER(C.c_int), _i, _i, _i, _vp, C.POINTER(SmkCycleDraws), STREAM]),
-]
-_ALL_BINDINGS = BINDINGS + LOSS_BINDINGS + MICA_BINDINGS + EXPRESSION_BINDINGS + GENERATOR_TRAIN_BINDINGS + CYCLE_BINDINGS
-_TAKES_STREAM = frozenset(name for name, _, args in _ALL_BINDINGS if args[-1:] == [STREAM])
+_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS if args[-1:] == [STREAM])
 
 
 def lib():
@@ -263,7 +241,7 @@ def lib():
         raise RuntimeError("smirk_b200: %s not found — build it with `python -m smirk_b200.build` "
                            "(there is no CPU / PyTorch fallback)" % LIB_PATH)
     L = C.CDLL(LIB_PATH)
-    for name, restype, argtypes in _ALL_BINDINGS:
+    for name, restype, argtypes in BINDINGS:
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, [_vp if a is STREAM else a for a in argtypes]
     if L.smk_version() != 100:
@@ -351,16 +329,19 @@ def saved_buffer(kind, handle, B, device):
     return torch.empty(max(nbytes // 4, 1), dtype=torch.float32, device=device)
 
 
-def saved_views(kind, handle, saved, B):
-    """{name: view of ``saved``} for every tensor ``smk_<kind>_saved_tensor`` lays out in it, in layout order: [B,C,H,W]
-    views of the NHWC tensors, [B,C] for 1 x 1 ones (the encoder's head outputs)."""
+def saved_views(kind, handle, saved, B, *args, int8=()):
+    """{name: view of ``saved``} for every tensor ``smk_<kind>_saved_tensor(handle, B, *args, i, ...)`` lays out in it, in
+    layout order: [B,C,H,W] views of the NHWC tensors, [B,C] for 1 x 1 ones (the encoder's head outputs, the expression
+    loss's features).  ``args``: the losses' ``need``.  The tensors named in ``int8`` are int8, at byte offset 4 * offset."""
     fn = getattr(lib(), "smk_%s_saved_tensor" % kind)
     name, off, dims = C.c_char_p(), C.c_size_t(), (C.c_int * 4)()
     out, i = {}, 0
-    while (rc := fn(handle, B, i, C.byref(name), C.byref(off), dims)) == 0:       # non-zero past the last tensor
+    while (rc := fn(handle, B, *args, i, C.byref(name), C.byref(off), dims)) == 0:       # non-zero past the last tensor
         b, h, w, c = dims
-        t = saved[off.value:off.value + b * h * w * c].view(b, h, w, c)
-        out[name.value.decode()] = t.view(b, c) if h == w == 1 else t.permute(0, 3, 1, 2)
+        key, n = name.value.decode(), b * h * w * c
+        t = saved.view(torch.int8)[4 * off.value:4 * off.value + n] if key in int8 else saved[off.value:off.value + n]
+        t = t.view(b, h, w, c)
+        out[key] = t.view(b, c) if h == w == 1 else t.permute(0, 3, 1, 2)
         i += 1
     if not out:                                 # not even tensor 0: raise with the library's message
         check(rc, "smk_%s_saved_tensor" % kind)
@@ -445,6 +426,96 @@ class NativeModule:
             if k != "_native_state":
                 new.__dict__[k] = copy.deepcopy(v, memo)
         return new
+
+
+class FrozenNet(NativeModule):
+    """Base of the trainer's frozen networks (VGGPerceptualLoss, MICA, ExpressionLoss): the handle ``smk_<_kind>_create``
+    builds from ``_native_tensors()`` at ``precision`` (0 = fp32 CUDA cores, 1 = TF32 tensor cores, 3 = 3xTF32 tensor
+    cores), and the check that the module runs as the trainer runs it.  A subclass sets ``_kind``, ``_name`` (the class in
+    messages) and ``_net`` (what the trainer calls the network, in messages)."""
+
+    def _native_extras(self):
+        return (self.precision,)
+
+    def _native_tensors(self):
+        """The tensors the handle is built from: the state_dict in its order, without num_batches_tracked."""
+        return [t for k, t in self.state_dict().items() if not k.endswith("num_batches_tracked")]
+
+    def _native_create(self, device):
+        if self.precision not in (0, 1, 3):
+            raise RuntimeError("smirk_b200.%s: precision must be 0 (fp32), 1 (TF32) or 3 (3xTF32), got %r" % (self._name, self.precision))
+        host = [f32(t) for t in self._native_tensors()]
+        arr = (c_f32p * len(host))(*[p for _, p in host])
+        d = SmkNetDesc()
+        d.tensors, d.n_tensors, d.precision = C.cast(arr, C.POINTER(c_f32p)), len(host), self.precision
+        return create(self._kind, d, device)
+
+    def _saved_views(self, h, saved, B, need):
+        """{name: view of ``saved``} for the buffer of a grad-mode forward with ``need`` (the two losses with an input
+        gradient; their int8 tensors are named in ``_int8``)."""
+        return saved_views(self._kind, h, saved, B, need, int8=self._int8)
+
+    def _check_frozen(self):
+        """BatchNorm runs in eval mode only, and weight gradients are not implemented."""
+        if any(m.training for m in self.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)):
+            raise RuntimeError("smirk_b200.%s: BatchNorm in train mode is not implemented (the trainer runs %s in eval mode); "
+                               "call .eval() on the module" % (self._name, self._net))
+        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            raise RuntimeError("smirk_b200.%s: weight gradients are not implemented (the trainer freezes %s); set "
+                               "requires_grad=False on its parameters or run it under torch.no_grad()" % (self._name, self._net))
+
+
+def check_image_pair(m, a, b):
+    """The inputs of a loss of two [B,3,224,224] images on one device (``m._inputs`` names them; ``m._why_224`` says why
+    only 224x224 is implemented)."""
+    for name, t in zip(m._inputs, (a, b)):
+        require_cuda(t, name)
+        if t.dim() != 4 or tuple(t.shape[1:]) != (3, 224, 224) or t.shape[0] < 1:
+            raise RuntimeError("smirk_b200.%s: expected %s [B,3,224,224], got %s — %s" % (m._name, name, tuple(t.shape), m._why_224))
+    if a.shape[0] != b.shape[0] or a.device != b.device:
+        raise RuntimeError("smirk_b200.%s: %s and %s must have the same batch size and device, got %s on %s and %s on %s"
+                           % ((m._name,) + tuple(m._inputs) + (tuple(a.shape), a.device, tuple(b.shape), b.device)))
+
+
+def pair_forward_saved(m, a, b, opts, need, loss_shape):
+    """-> (handle, loss, saved): the grad-mode forward ``smk_<m._kind>_forward_saved(h, a, b, B, *opts, need, loss, saved,
+    ...)`` of a two-image loss for the inputs ``need`` names (1 a, 2 b, 3 both); ``opts``: the loss's int options."""
+    dev, kind = a.device, m._kind
+    h = m._native_handle(dev)
+    a, b = dev_f32(a, m._inputs[0]), dev_f32(b, m._inputs[1])
+    B = a.shape[0]
+    loss = torch.empty(loss_shape, dtype=torch.float32, device=dev)
+    nbytes = call("smk_%s_saved_bytes" % kind, dev, h, B, need)
+    saved = torch.empty(nbytes // 4, dtype=torch.float32, device=dev)
+    ws = m._native_workspace("forward", call("smk_%s_workspace_bytes" % kind, dev, h, B), dev)
+    call("smk_%s_forward_saved" % kind, dev, h, a, b, B, *opts, need, loss, saved, saved.numel() * 4, ws, ws.numel())
+    return h, loss, saved
+
+
+class PairLossFunction(torch.autograd.Function):
+    """loss = m(a, b) of a frozen two-image loss (VGG's x / y, the expression loss's gen / tar), and its gradient to
+    whichever of a and b requires grad, through ``pair_forward_saved`` and ``smk_<m._kind>_backward(h, B, *opts, need,
+    saved, ...)``."""
+
+    @staticmethod
+    def forward(ctx, a, b, m, opts, loss_shape):
+        need = (1 if ctx.needs_input_grad[0] else 0) | (2 if ctx.needs_input_grad[1] else 0)
+        h, loss, saved = pair_forward_saved(m, a, b, opts, need, loss_shape)
+        ctx.handle, ctx.m, ctx.opts, ctx.need, ctx.B, ctx.dtypes = h, m, opts, need, a.shape[0], (a.dtype, b.dtype)
+        ctx.save_for_backward(saved)
+        return loss
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g):
+        saved, = ctx.saved_tensors
+        m, dev, B, need = ctx.m, saved.device, ctx.B, ctx.need
+        g = dev_f32(g, "g")
+        ga = torch.empty(B, 3, 224, 224, dtype=torch.float32, device=dev) if need & 1 else None
+        gb = torch.empty(B, 3, 224, 224, dtype=torch.float32, device=dev) if need & 2 else None
+        ws = m._native_workspace("backward", call("smk_%s_backward_workspace_bytes" % m._kind, dev, ctx.handle, B, need), dev)
+        call("smk_%s_backward" % m._kind, dev, ctx.handle, B, *ctx.opts, need, saved, saved.numel() * 4, g, ga, gb, ws, ws.numel())
+        return (ga.to(ctx.dtypes[0]) if ga is not None else None, gb.to(ctx.dtypes[1]) if gb is not None else None, None, None, None)
 
 
 def profiler_report():

@@ -1,12 +1,11 @@
 // The cycle path's parameter augmentation (src/smirk_trainer.py:189-248) with its random draws made on the device
-// (include/smirk_b200_cycle.h).  The reference draws a permutation on the host, loops over template rows in Python and
+// (include/smirk_b200.h).  The reference draws a permutation on the host, loops over template rows in Python and
 // issues ~30 small torch ops; here the whole augmentation of Ke*B rows is one single-CTA launch: both permutations
 // (ranks of Philox keys in shared memory), every Bernoulli / normal / uniform and the template picks come from the
 // counter-based generator of csrc/philox.cuh, and the arithmetic repeats the reference's fp32 ops one by one (explicit
 // round-to-nearest intrinsics, no FMA contraction), so given the exported draws the result is bitwise the reference's.
 #include "common.cuh"
 #include "philox.cuh"
-#include "../../include/smirk_b200_cycle.h"
 #include <math.h>
 #include <vector>
 

@@ -30,12 +30,8 @@
 // pool_out > 0, already applied), and expr_stem_dgrad_kernel is the transposed 7x7 s2 conv into NCHW.  Precision 1
 // TF32-rounds every gradient a TF32 dgrad reads.
 #include "nn_kernels.cuh"
-#include "gemm_tc.cuh"
-#include "../../include/smirk_b200_expression.h"
-#include <array>
-#include <cmath>
+#include "frozen_net.cuh"
 #include <string>
-#include <vector>
 
 namespace {
 
@@ -222,19 +218,6 @@ expr_stem_dgrad_kernel(const float4* __restrict__ g, const float4* __restrict__ 
     for (int c = 0; c < 3; ++c) o[((size_t)c * kImg + ih) * kImg + iw] = acc[c];
 }
 
-// Sum over the 256 threads of a block in a fixed order; the result is valid in every thread.
-__device__ float block_sum_all(float v) {
-    __shared__ float wsum[8];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = v;
-    __syncthreads();
-    float t = 0.f;
-    for (int w = 0; w < 8; ++w) t += wsum[w];
-    return t;
-}
-
 __device__ __forceinline__ float sgnf(float d) { return (float)((d > 0.f) - (d < 0.f)); }
 constexpr float kCosEps = 1e-8f;
 
@@ -272,11 +255,11 @@ expr_head_kernel(const float* __restrict__ y, int B, int swap, int metric, float
         float gg = 0.f, tt = 0.f;
 #pragma unroll
         for (int j = 0; j < 8; ++j) { gg = fmaf(f[0][j], f[0][j], gg); tt = fmaf(f[1][j], f[1][j], tt); }
-        const float n1 = fmaxf(sqrtf(block_sum_all(gg)), kCosEps), n2 = fmaxf(sqrtf(block_sum_all(tt)), kCosEps);
+        const float n1 = fmaxf(sqrtf(smk::block_sum(gg)), kCosEps), n2 = fmaxf(sqrtf(smk::block_sum(tt)), kCosEps);
         float s = 0.f;
 #pragma unroll
         for (int j = 0; j < 8; ++j) s = fmaf(__fdiv_rn(f[0][j], n1), __fdiv_rn(f[1][j], n2), s);
-        r = 1.f - block_sum_all(s);
+        r = 1.f - smk::block_sum(s);
     } else {
         float s = 0.f;
 #pragma unroll
@@ -284,7 +267,7 @@ expr_head_kernel(const float* __restrict__ y, int B, int swap, int metric, float
             const float d = f[0][j] - f[1][j];
             s = metric == 0 ? fmaf(d, d, s) : s + fabsf(d);
         }
-        r = __fdiv_rn(block_sum_all(s), (float)kFeat);
+        r = __fdiv_rn(smk::block_sum(s), (float)kFeat);
     }
     if (threadIdx.x == 0) lossv[b] = r;
 }
@@ -312,12 +295,12 @@ expr_head_bwd_kernel(const float* __restrict__ feat, const float* __restrict__ y
         float gg = 0.f, tt = 0.f;
 #pragma unroll
         for (int j = 0; j < 8; ++j) { gg = fmaf(fg[j], fg[j], gg); tt = fmaf(ft[j], ft[j], tt); }
-        const float ng = sqrtf(block_sum_all(gg)), nt = sqrtf(block_sum_all(tt));
+        const float ng = sqrtf(smk::block_sum(gg)), nt = sqrtf(smk::block_sum(tt));
         const float n1 = fmaxf(ng, kCosEps), n2 = fmaxf(nt, kCosEps);
         float s = 0.f;
 #pragma unroll
         for (int j = 0; j < 8; ++j) s = fmaf(__fdiv_rn(fg[j], n1), __fdiv_rn(ft[j], n2), s);
-        const float cs = block_sum_all(s);
+        const float cs = smk::block_sum(s);
         // d(1 - cos)/dx = -(o / (n_x n_o) - cos * x / (n_x |x|)), x the image's features, o the other's
         const float nx = tar ? n2 : n1, no = tar ? n1 : n2, ax = tar ? nt : ng;
 #pragma unroll
@@ -354,7 +337,7 @@ expr_head_bwd_kernel(const float* __restrict__ feat, const float* __restrict__ y
 }
 
 // ---- host -----------------------------------------------------------------------------------------------------------
-struct Affine { float* scale = nullptr; float* bias = nullptr; };
+using smk::Affine;
 
 struct ExprBlock {
     int cin, planes, H, stride;                // H: input size; conv2 and the downsample run at H / stride
@@ -381,22 +364,8 @@ struct SmkExpressionLoss {
 
 namespace {
 
-using Bn = std::array<const float*, 4>;
-
-void bn_fold(const Bn& t, int C, std::vector<double>& s, std::vector<double>& b) {
-    s.resize(C); b.resize(C);
-    for (int c = 0; c < C; ++c) {
-        s[c] = (double)t[0][c] / std::sqrt((double)t[3][c] + 1e-5);
-        b[c] = (double)t[1][c] - (double)t[2][c] * s[c];
-    }
-}
-
-cudaError_t upload_bn(smk::DeviceArena& arena, const std::vector<double>& s, const std::vector<double>& b, Affine* out) {
-    std::vector<float> sf(s.begin(), s.end()), bf(b.begin(), b.end());
-    cudaError_t e = arena.upload(sf, &out->scale);
-    if (e == cudaSuccess) e = arena.upload(bf, &out->bias);
-    return e;
-}
+using smk::bn_fold;
+using smk::upload_bn;
 
 // A 1x1 conv's weight [cout][cin] and its BN scale s: forward (N = cout, K = cin) and dgrad (N = cin, K = cout,
 // W'(k = co, n = ci) = s[co] * W[co][ci]).
@@ -409,19 +378,15 @@ cudaError_t pack1(smk::DeviceArena& A, const float* w, const std::vector<double>
 
 }  // namespace
 
-extern "C" int smk_expression_loss_create(const SmkExpressionLossDesc* desc, SmkExpressionLoss** out) {
-    SMK_REQUIRE(desc && out && desc->tensors, "smk_expression_loss_create: null argument");
-    SMK_REQUIRE(desc->precision == 0 || desc->precision == 1 || desc->precision == 3,
-                "smk_expression_loss_create: precision must be 0, 1 or 3 (0 = fp32 CUDA cores, 1 = TF32 wgmma, 3 = 3xTF32 wgmma: fp32-equivalent)");
-    SMK_REQUIRE(desc->n_tensors == kTensors, "smk_expression_loss_create: expected %d tensors (backbone.* in state_dict order without "
-                "num_batches_tracked and fc), got %d", kTensors, desc->n_tensors);
-    for (int i = 0; i < desc->n_tensors; ++i) SMK_REQUIRE(desc->tensors[i], "smk_expression_loss_create: tensor %d is null", i);
+extern "C" int smk_expression_loss_create(const SmkNetDesc* desc, SmkExpressionLoss** out) {
+    if (int rc = smk::check_net_desc(desc, out, "smk_expression_loss_create", kTensors,
+                                     "backbone.* in state_dict order without num_batches_tracked and fc"))
+        return rc;
     const bool tc = desc->precision != 0, x3 = desc->precision == 3;
-    if (tc) { if (int rc = smk::tc_init()) return rc; }
     SmkExpressionLoss* h = new SmkExpressionLoss();
     h->precision = desc->precision;
     smk::TensorCursor cur{desc->tensors, desc->n_tensors};
-    auto bn4 = [&]() { Bn t; for (auto& p : t) p = cur.next(); return t; };      // weight, bias, running mean, running var
+    auto bn4 = [&]() { return smk::next_bn(cur); };
     smk::DeviceArena& A = h->arena;
     std::vector<double> s, b;
     cudaError_t e = cudaSuccess;
@@ -487,24 +452,17 @@ extern "C" int smk_expression_loss_create(const SmkExpressionLossDesc* desc, Smk
     const std::vector<float> one(kOnes, 1.f), zero(kOnes, 0.f);
     if (e == cudaSuccess) e = A.upload(one, &h->ones);
     if (e == cudaSuccess) e = A.upload(zero, &h->zeros);
-    if (e != cudaSuccess) {
-        smk::set_error("smk_expression_loss_create: upload failed: %s", cudaGetErrorString(e));
-        delete h; return (int)e;
-    }
-    *out = h;
-    return 0;
+    return smk::finish_create(e, "smk_expression_loss_create", h, out);
 }
 
 extern "C" void smk_expression_loss_destroy(SmkExpressionLoss* h) { delete h; }
 
 namespace {
 
-int halves(int need) { return need == 3 ? 2 : 1; }
-size_t feat_floats(int B) { return (size_t)2 * B * kFeat; }
+using smk::halves;
+using smk::tag_of;
 
-const char* tag_of(int precision, const char* f32, const char* tc, const char* tc3) {
-    return precision == 0 ? f32 : precision == 1 ? tc : tc3;
-}
+size_t feat_floats(int B) { return (size_t)2 * B * kFeat; }
 
 // One smk::conv problem of the network: out = epi(in * W), scale / bias (null: 1 / 0), res, relu, mask, round, out2.
 struct Prob {
@@ -691,8 +649,9 @@ extern "C" int smk_expression_loss_forward_saved(const SmkExpressionLoss* h, con
     SMK_REQUIRE(h && gen && tar && loss && saved, "smk_expression_loss_forward_saved: null argument");
     SMK_REQUIRE(B > 0, "smk_expression_loss_forward_saved: B must be positive (got %d)", B);
     SMK_REQUIRE(metric_ok(metric), "smk_expression_loss_forward_saved: metric must be 0 (l2), 1 (l1) or 2 (cos), got %d", metric);
-    SMK_REQUIRE(need >= 1 && need <= 3, "smk_expression_loss_forward_saved: need must be 1 (gen), 2 (tar) or 3 (both), got %d", need);
-    SMK_REQUIRE(saved_bytes >= smk_expression_loss_saved_bytes(h, B, need), "smk_expression_loss_forward_saved: saved buffer too small");
+    if (int rc = smk::check_need("smk_expression_loss_forward_saved", "gen", "tar", need, saved_bytes,
+                                 smk_expression_loss_saved_bytes(h, B, need)))
+        return rc;
     SMK_REQUIRE(ws && ws_bytes >= smk_expression_loss_workspace_bytes(h, B), "smk_expression_loss_forward_saved: workspace too small");
     return expr_forward(h, gen, tar, B, metric, use_mean, need, loss, nullptr, saved, ws, ws_bytes, (cudaStream_t)stream);
 }
@@ -727,9 +686,9 @@ extern "C" int smk_expression_loss_backward(const SmkExpressionLoss* h, int B, i
     SMK_REQUIRE(h && saved && g, "smk_expression_loss_backward: null argument");
     SMK_REQUIRE(B > 0, "smk_expression_loss_backward: B must be positive (got %d)", B);
     SMK_REQUIRE(metric_ok(metric), "smk_expression_loss_backward: metric must be 0 (l2), 1 (l1) or 2 (cos), got %d", metric);
-    SMK_REQUIRE(need >= 1 && need <= 3, "smk_expression_loss_backward: need must be 1 (gen), 2 (tar) or 3 (both), got %d", need);
+    if (int rc = smk::check_need("smk_expression_loss_backward", "gen", "tar", need, saved_bytes, smk_expression_loss_saved_bytes(h, B, need)))
+        return rc;
     SMK_REQUIRE((!(need & 1) || g_gen) && (!(need & 2) || g_tar), "smk_expression_loss_backward: a gradient `need` asks for is null");
-    SMK_REQUIRE(saved_bytes >= smk_expression_loss_saved_bytes(h, B, need), "smk_expression_loss_backward: saved buffer too small");
     SMK_REQUIRE(ws && ws_bytes >= smk_expression_loss_backward_workspace_bytes(h, B, need), "smk_expression_loss_backward: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     const int P = h->precision, swap = need == 2 ? 1 : 0, Bc = halves(need) * B;
@@ -787,7 +746,7 @@ extern "C" int smk_expression_loss_backward(const SmkExpressionLoss* h, int B, i
 }
 
 // ---- kernel-test entry points (tests/test_gpu_expression_loss_layers.py) ---------------------------------------------
-// Exported but not part of include/smirk_b200_expression.h; the test declares their argument types itself.
+// Exported but not part of include/smirk_b200.h; the test declares their argument types itself.
 //
 // expr_im2col_kernel: a, b [B,3,224,224] -> out [2B*112*112, 148].
 extern "C" int smk_debug_expression_im2col(const float* a, const float* b, int B, int round, float* out, void* stream) {

@@ -18,7 +18,6 @@
 #include "gemm_tc.cuh"
 #include "generator.cuh"
 #include "train_common.cuh"
-#include "../../include/smirk_b200_generator_train.h"
 
 using namespace trn;
 using gen::TrainConv;

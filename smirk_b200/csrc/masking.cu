@@ -19,12 +19,11 @@
 // what IS exact: given the draws this call exports (optional debug outputs), the masked image equals the reference's
 // `masking()` fed the same draws.  The counter lives in device memory and is advanced by the last kernel, so a captured
 // CUDA graph produces fresh draws on every replay.
-// (3) smk_masking_train_forward (include/smirk_b200_cycle.h) runs the trainer's step1 / step2 masking on the same kernels:
+// (3) smk_masking_train_forward (include/smirk_b200.h) runs the trainer's step1 / step2 masking on the same kernels:
 // every sampled point kept (no rbound), transfer_pixels between two meshes, Ke repeats read as row r mod B (`Bsrc`).
 // All of it is HBM-bound byte/float shuffling over [B,3,224,224] images (602 KB per face in, 602 KB out).
 #include "common.cuh"
 #include "philox.cuh"
-#include "../../include/smirk_b200_cycle.h"
 #include <math.h>
 #include <algorithm>
 #include <vector>
@@ -481,7 +480,7 @@ extern "C" int smk_masking_forward(const SmkMasking* h, const float* img, const 
     return 0;
 }
 
-// ---- the trainer's masking (include/smirk_b200_cycle.h) ----
+// ---- the trainer's masking (include/smirk_b200.h) ----
 extern "C" size_t smk_masking_train_workspace_bytes(const SmkMasking* h, int B, int Ke, int S, int N) {
     if (!h) return 0;
     const size_t b = (size_t)(B > 0 ? B : 1), r = b * (size_t)(Ke > 0 ? Ke : 1), px = r * S * S, n = (size_t)(N > 0 ? N : 1);

@@ -22,11 +22,7 @@
 // gathered matrices, the last block's output); the residual stream y itself stays fp32.  Precision 3 rounds nothing, and
 // its deep problems (every 3x3 conv, the gathered stride-2 convs, the fc) sum each 32-deep k-block apart (gemm_tc X3 = 3).
 #include "nn_kernels.cuh"
-#include "gemm_tc.cuh"
-#include "../../include/smirk_b200_mica.h"
-#include <array>
-#include <cmath>
-#include <vector>
+#include "frozen_net.cuh"
 
 namespace {
 
@@ -62,19 +58,6 @@ mica_prep_kernel(const float* __restrict__ x, int B, int HW, int Cp, int round, 
     reinterpret_cast<float4*>(out)[i] = make_float4(v[0], v[1], v[2], v[3]);
 }
 
-// Sum over the 256 threads of a block in a fixed order; the result is valid in every thread.
-__device__ float block_sum_all(float v) {
-    __shared__ float wsum[8];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = v;
-    __syncthreads();
-    float t = 0.f;
-    for (int w = 0; w < 8; ++w) t += wsum[w];
-    return t;
-}
-
 struct MapW { const float* w[kMapLayers]; const float* b[kMapLayers]; };   // w: [K][N] (n fastest), b: [N]
 
 // One image per CTA: z = f / max(|f|_2, 1e-12), then the regressor's five Linears (leaky_relu 0.2 after the first four).
@@ -85,7 +68,7 @@ mica_map_kernel(const float* __restrict__ feat, MapW mw, float* __restrict__ out
     const float* f = feat + (size_t)b * kFeat;
     float ss = 0.f;
     for (int k = tid; k < kFeat; k += 256) { const float v = f[k]; ss = fmaf(v, v, ss); }
-    const float den = fmaxf(sqrtf(block_sum_all(ss)), 1e-12f);
+    const float den = fmaxf(sqrtf(smk::block_sum(ss)), 1e-12f);
     for (int k = tid; k < kFeat; k += 256) h[0][k] = __fdiv_rn(f[k], den);
     __syncthreads();
     int cur = 0, K = kFeat;
@@ -114,7 +97,7 @@ mica_mse_kernel(const float* __restrict__ s, const float* __restrict__ m, int B,
         const float e = s[i] - m[(size_t)b * ld + d];
         acc = fmaf(e, e, acc);
     }
-    acc = block_sum_all(acc);
+    acc = smk::block_sum(acc);
     if (threadIdx.x == 0) *loss = __fdiv_rn(acc, (float)n);
 }
 
@@ -129,7 +112,7 @@ mica_mse_bwd_kernel(const float* __restrict__ s, const float* __restrict__ m, in
 }
 
 // ---- host -----------------------------------------------------------------------------------------------------------
-struct Affine { float* scale = nullptr; float* bias = nullptr; };
+using smk::Affine;
 
 struct MicaBlock {
     int cin, cout, H, stride;                  // H: input size; conv2 (and the downsample) output H / stride
@@ -156,25 +139,8 @@ struct SmkMica {
 
 namespace {
 
-// Eval-mode BatchNorm (weight, bias, running_mean, running_var) as y = scale * x + bias, in float64.
-using Bn = std::array<const float*, 4>;
-
-void bn_fold(const Bn& t, int C, std::vector<double>& s, std::vector<double>& b) {
-    s.resize(C); b.resize(C);
-    for (int c = 0; c < C; ++c) {
-        s[c] = (double)t[0][c] / std::sqrt((double)t[3][c] + 1e-5);
-        b[c] = (double)t[1][c] - (double)t[2][c] * s[c];
-    }
-}
-
-cudaError_t upload_bn(smk::DeviceArena& arena, const Bn& t, int C, Affine* out) {
-    std::vector<double> s, b;
-    bn_fold(t, C, s, b);
-    std::vector<float> sf(s.begin(), s.end()), bf(b.begin(), b.end());
-    cudaError_t e = arena.upload(sf, &out->scale);
-    if (e == cudaSuccess) e = arena.upload(bf, &out->bias);
-    return e;
-}
+using smk::bn_fold;
+using smk::upload_bn;
 
 // A 3x3 conv's PyTorch weight [cout][cin][3][3] as the GEMM operand, k = tap * cin_p + c (modes 1 and the gathered matrix).
 cudaError_t pack3(smk::DeviceArena& arena, const float* w, int cin, int cin_p, int cout, bool tc, bool x3, smk::GemmW* out) {
@@ -186,20 +152,14 @@ cudaError_t pack3(smk::DeviceArena& arena, const float* w, int cin, int cin_p, i
 
 }  // namespace
 
-extern "C" int smk_mica_create(const SmkMicaDesc* desc, SmkMica** out) {
-    SMK_REQUIRE(desc && out && desc->tensors, "smk_mica_create: null argument");
-    SMK_REQUIRE(desc->precision == 0 || desc->precision == 1 || desc->precision == 3,
-                "smk_mica_create: precision must be 0, 1 or 3 (0 = fp32 CUDA cores, 1 = TF32 wgmma, 3 = 3xTF32 wgmma: fp32-equivalent)");
-    SMK_REQUIRE(desc->n_tensors == kTensors, "smk_mica_create: expected %d tensors (the state_dict without num_batches_tracked), got %d",
-                kTensors, desc->n_tensors);
-    for (int i = 0; i < desc->n_tensors; ++i) SMK_REQUIRE(desc->tensors[i], "smk_mica_create: tensor %d is null", i);
+extern "C" int smk_mica_create(const SmkNetDesc* desc, SmkMica** out) {
+    if (int rc = smk::check_net_desc(desc, out, "smk_mica_create", kTensors, "the state_dict without num_batches_tracked")) return rc;
     const bool tc = desc->precision != 0, x3 = desc->precision == 3;
-    if (tc) { if (int rc = smk::tc_init()) return rc; }
     SmkMica* h = new SmkMica();
     h->precision = desc->precision;
     h->cin_p = tc ? 32 : 4;                   // the tensor-core path reads 128-byte pixel rows
     smk::TensorCursor cur{desc->tensors, desc->n_tensors};
-    auto bn4 = [&]() { Bn t; for (auto& p : t) p = cur.next(); return t; };      // weight, bias, running mean, running var
+    auto bn4 = [&]() { return smk::next_bn(cur); };
     smk::DeviceArena& A = h->arena;
     cudaError_t e = pack3(A, cur.next(), 3, h->cin_p, 64, tc, x3, &h->stem);
     if (e == cudaSuccess) e = upload_bn(A, bn4(), 64, &h->stem_bn);
@@ -257,12 +217,7 @@ extern "C" int smk_mica_create(const SmkMicaDesc* desc, SmkMica** out) {
     }
     const std::vector<float> one(kFeat, 1.f);
     if (e == cudaSuccess) e = A.upload(one, &h->ones);
-    if (e != cudaSuccess) {
-        smk::set_error("smk_mica_create: upload failed: %s", cudaGetErrorString(e));
-        delete h; return (int)e;
-    }
-    *out = h;
-    return 0;
+    return smk::finish_create(e, "smk_mica_create", h, out);
 }
 
 extern "C" void smk_mica_destroy(SmkMica* h) { delete h; }
@@ -275,9 +230,7 @@ extern "C" size_t smk_mica_workspace_bytes(const SmkMica* h, int B) {
 
 namespace {
 
-const char* tag_of(int precision, const char* f32, const char* tc, const char* tc3) {
-    return precision == 0 ? f32 : precision == 1 ? tc : tc3;
-}
+using smk::tag_of;
 
 int gather_s2(const float* in, int B, int H, int C, int taps, bool round, float* out, cudaStream_t st) {
     return smk::gather_s2(in, B, H, C, taps, round, out, taps == 9 ? "mica_gather3x3_s2" : "mica_gather1x1_s2", st);
@@ -398,7 +351,7 @@ extern "C" int smk_mica_shape_loss_backward(const float* shape_params, const flo
 }
 
 // ---- kernel-test entry points (tests/test_gpu_mica_layers.py) ---------------------------------------------------------
-// Exported but not part of include/smirk_b200_mica.h; the test declares their argument types itself.
+// Exported but not part of include/smirk_b200.h; the test declares their argument types itself.
 //
 // One smk::conv problem with MICA's epilogue options: w_kn fp32 [K][N] (conv_gemm), or wt_hi [N][K] TF32 (tc_conv) with
 // optional tails wt_lo (3xTF32); res / prelu / out2 / scale2 null: not used.

@@ -18,8 +18,7 @@
 // weights (smk::pack_conv3, as the generator's) whose epilogue applies the ReLU mask of its input; vgg_input_bwd_kernel
 // undoes the normalisation into NCHW.
 #include "nn_kernels.cuh"
-#include "gemm_tc.cuh"
-#include "../../include/smirk_b200_loss.h"
+#include "frozen_net.cuh"
 #include <string>
 
 namespace {
@@ -70,20 +69,6 @@ vgg_prep_kernel(const float* __restrict__ x, const float* __restrict__ y, int B,
     reinterpret_cast<float4*>(out)[i] = make_float4(v[0], v[1], v[2], v[3]);
 }
 
-// Sum over the 256 threads of a block in a fixed order; the result is valid in thread 0.
-__device__ float block_sum(float v) {
-    __shared__ float wsum[8];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = v;
-    __syncthreads();
-    float t = 0.f;
-    if (threadIdx.x == 0)
-        for (int w = 0; w < 8; ++w) t += wsum[w];
-    __syncthreads();
-    return t;
-}
-
 __device__ __forceinline__ signed char sgn(float d) { return (signed char)((d > 0.f) - (d < 0.f)); }
 
 // One tap: partial[cta] = sum of |d| over the CTA's chunk of kChunk4 float4s, d = phi(x) - phi(y); a holds the batch's first
@@ -102,7 +87,7 @@ vgg_l1_kernel(const float4* __restrict__ a, const float4* __restrict__ b, long n
         s += fabsf(d.x); s += fabsf(d.y); s += fabsf(d.z); s += fabsf(d.w);
         if (sign) sign[i] = make_char4(sgn(d.x), sgn(d.y), sgn(d.z), sgn(d.w));
     }
-    s = block_sum(s);
+    s = smk::block_sum(s);
     if (threadIdx.x == 0) partial[blockIdx.x] = s;
 }
 
@@ -115,7 +100,7 @@ vgg_l1_finalize_kernel(const float* __restrict__ partial, TapSums ts, float* __r
     for (int t = 0; t < kTaps; ++t) {
         float s = 0.f;
         for (int i = threadIdx.x; i < ts.count[t]; i += 256) s += partial[i];
-        s = block_sum(s);
+        s = smk::block_sum(s);
         if (threadIdx.x == 0) total = t == 0 ? s / ts.numel[t] : total + s / ts.numel[t];
         partial += ts.count[t];
     }
@@ -197,15 +182,10 @@ struct SmkVggLoss {
     smk::DeviceArena arena;
 };
 
-extern "C" int smk_vgg_loss_create(const SmkVggLossDesc* desc, SmkVggLoss** out) {
-    SMK_REQUIRE(desc && out && desc->tensors, "smk_vgg_loss_create: null argument");
-    SMK_REQUIRE(desc->precision == 0 || desc->precision == 1 || desc->precision == 3,
-                "smk_vgg_loss_create: precision must be 0, 1 or 3 (0 = fp32 CUDA cores, 1 = TF32 wgmma, 3 = 3xTF32 wgmma: fp32-equivalent)");
-    SMK_REQUIRE(desc->n_tensors == 2 + 2 * kConvs,
-                "smk_vgg_loss_create: expected %d tensors (mean, std, then weight and bias of 10 convs), got %d", 2 + 2 * kConvs, desc->n_tensors);
-    for (int i = 0; i < desc->n_tensors; ++i) SMK_REQUIRE(desc->tensors[i], "smk_vgg_loss_create: tensor %d is null", i);
+extern "C" int smk_vgg_loss_create(const SmkNetDesc* desc, SmkVggLoss** out) {
+    if (int rc = smk::check_net_desc(desc, out, "smk_vgg_loss_create", 2 + 2 * kConvs, "mean, std, then weight and bias of 10 convs"))
+        return rc;
     const bool tc = desc->precision != 0, x3 = desc->precision == 3;
-    if (tc) { if (int rc = smk::tc_init()) return rc; }
     SmkVggLoss* h = new SmkVggLoss();
     h->precision = desc->precision;
     for (int c = 0; c < 3; ++c) { h->norm.mean[c] = desc->tensors[0][c]; h->norm.std[c] = desc->tensors[1][c]; }
@@ -221,24 +201,19 @@ extern "C" int smk_vgg_loss_create(const SmkVggLossDesc* desc, SmkVggLoss** out)
     const std::vector<float> one(512, 1.f), zero(512, 0.f);
     if (e == cudaSuccess) e = h->arena.upload(one, &h->ones);
     if (e == cudaSuccess) e = h->arena.upload(zero, &h->zeros);
-    if (e != cudaSuccess) {
-        smk::set_error("smk_vgg_loss_create: upload failed: %s", cudaGetErrorString(e));
-        delete h; return (int)e;
-    }
     for (int l = 0; l < kConvs; ++l) {               // every size is a multiple of 64 floats
         h->act_off[l] = h->act_total;
         h->act_total += (size_t)h->conv[l].S * h->conv[l].S * h->conv[l].cout;
     }
     for (int t = 0; t < kTaps; ++t) { h->sign_off[t] = h->sign_total; h->sign_total += tap_elems(t) / 4; }
-    *out = h;
-    return 0;
+    return smk::finish_create(e, "smk_vgg_loss_create", h, out);
 }
 
 extern "C" void smk_vgg_loss_destroy(SmkVggLoss* h) { delete h; }
 
 namespace {
 
-int halves(int need) { return need == 3 ? 2 : 1; }
+using smk::halves;
 
 size_t total_partials(int B) {
     size_t n = 0;
@@ -346,8 +321,7 @@ extern "C" int smk_vgg_loss_forward_saved(const SmkVggLoss* h, const float* x, c
                                           float* saved, size_t saved_bytes, void* ws, size_t ws_bytes, void* stream) {
     SMK_REQUIRE(h && x && y && loss && saved, "smk_vgg_loss_forward_saved: null argument");
     SMK_REQUIRE(B > 0, "smk_vgg_loss_forward_saved: B must be positive (got %d)", B);
-    SMK_REQUIRE(need >= 1 && need <= 3, "smk_vgg_loss_forward_saved: need must be 1 (x), 2 (y) or 3 (both), got %d", need);
-    SMK_REQUIRE(saved_bytes >= smk_vgg_loss_saved_bytes(h, B, need), "smk_vgg_loss_forward_saved: saved buffer too small");
+    if (int rc = smk::check_need("smk_vgg_loss_forward_saved", "x", "y", need, saved_bytes, smk_vgg_loss_saved_bytes(h, B, need))) return rc;
     SMK_REQUIRE(ws && ws_bytes >= smk_vgg_loss_workspace_bytes(h, B), "smk_vgg_loss_forward_saved: workspace too small");
     return vgg_forward(h, x, y, B, need, loss, saved, ws, ws_bytes, (cudaStream_t)stream);
 }
@@ -377,9 +351,8 @@ extern "C" int smk_vgg_loss_backward(const SmkVggLoss* h, int B, int need, const
                                      float* g_x, float* g_y, void* ws, size_t ws_bytes, void* stream) {
     SMK_REQUIRE(h && saved && g, "smk_vgg_loss_backward: null argument");
     SMK_REQUIRE(B > 0, "smk_vgg_loss_backward: B must be positive (got %d)", B);
-    SMK_REQUIRE(need >= 1 && need <= 3, "smk_vgg_loss_backward: need must be 1 (x), 2 (y) or 3 (both), got %d", need);
+    if (int rc = smk::check_need("smk_vgg_loss_backward", "x", "y", need, saved_bytes, smk_vgg_loss_saved_bytes(h, B, need))) return rc;
     SMK_REQUIRE((!(need & 1) || g_x) && (!(need & 2) || g_y), "smk_vgg_loss_backward: a gradient `need` asks for is null");
-    SMK_REQUIRE(saved_bytes >= smk_vgg_loss_saved_bytes(h, B, need), "smk_vgg_loss_backward: saved buffer too small");
     SMK_REQUIRE(ws && ws_bytes >= smk_vgg_loss_backward_workspace_bytes(h, B, need), "smk_vgg_loss_backward: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     const bool swap = need == 2, rnd = h->precision == 1;     // TF32 rounding of every gradient a TF32 dgrad reads

@@ -198,7 +198,7 @@ class MaskingStage(_lib.NativeModule):
 class TrainMaskingStage(_lib.NativeModule):
     """The reference trainer's masking (``src/smirk_trainer.py``: step1 at :76-92, step2 at :262-293) as one capturable
     device call per path, every random draw made on the device by the counter-based generator of ``MaskingStage``
-    (``include/smirk_b200_cycle.h``).  Unlike the demo's step it keeps all ``int(mask_ratio * S^2)`` sampled points, and
+    (``include/smirk_b200.h``).  Unlike the demo's step it keeps all ``int(mask_ratio * S^2)`` sampled points, and
     the second path moves the pixels under points sampled on the first path's mesh onto the augmented mesh.
 
     ``first_path(img, hull_mask, transformed_vertices, rendered_img)``: ``masking(img, hull, transfer_pixels(img, p, p),

@@ -3,7 +3,7 @@ step's ``mica_loss``.
 
 Same module tree and ``state_dict`` keys (``arcface.*``: an ArcFace iResNet-100 with ``IBasicBlock`` layers (3, 13, 30, 3);
 ``regressor.*``: ``MappingNetwork(512, 300, 300, hidden=3)``), with plain ``nn`` containers whose own ``forward`` is never
-called: the network runs in ``csrc/mica.cu`` through ``smk_mica_forward`` (include/smirk_b200_mica.h).
+called: the network runs in ``csrc/mica.cu`` through ``smk_mica_forward`` (include/smirk_b200.h).
 
 - ``MICA()`` loads ``assets/mica.tar`` relative to the current directory as the reference does: ``checkpoint['arcface']``
   strictly, and from ``checkpoint['flameModel']`` the keys that contain ``network`` or ``output``, ``regressor.`` stripped.
@@ -16,8 +16,6 @@ The network is frozen: BatchNorm runs in eval mode only (a module in train mode 
 that requires grad raises, since weight gradients are not implemented.  ``precision`` (part of the native handle's key):
 0 = fp32 CUDA cores, 1 = TF32 tensor cores, 3 = 3xTF32 tensor cores (fp32-equivalent), as for ``VGGPerceptualLoss``.
 """
-import ctypes as C
-
 import torch
 import torch.nn as nn
 
@@ -79,7 +77,9 @@ class MappingNetwork(nn.Module):
         self.output = nn.Linear(hidden_dim, out_dim)
 
 
-class MICA(_lib.NativeModule, nn.Module):
+class MICA(_lib.FrozenNet, nn.Module):
+    _kind, _name, _net = "mica", "MICA", "MICA"
+
     def __init__(self, checkpoint="assets/mica.tar"):
         """``checkpoint``: the path the reference loads (relative to the current directory), or None: untrained
         containers for ``load_state_dict``."""
@@ -93,30 +93,8 @@ class MICA(_lib.NativeModule, nn.Module):
             keys = {k.replace("regressor.", ""): v for k, v in ck["flameModel"].items() if "network" in k or "output" in k}
             self.regressor.load_state_dict(keys, strict=True)
 
-    def _native_extras(self):
-        return (self.precision,)
-
-    def _native_create(self, device):
-        if self.precision not in (0, 1, 3):
-            raise RuntimeError("smirk_b200.MICA: precision must be 0 (fp32), 1 (TF32) or 3 (3xTF32), got %r" % (self.precision,))
-        keep = []
-        ts = [t for k, t in self.state_dict().items() if not k.endswith("num_batches_tracked")]
-        arr = (_lib.c_f32p * len(ts))()
-        for j, t in enumerate(ts):
-            a, p = _lib.f32(t)
-            keep.append(a)
-            arr[j] = p
-        d = _lib.SmkMicaDesc()
-        d.tensors, d.n_tensors, d.precision = C.cast(arr, C.POINTER(_lib.c_f32p)), len(ts), self.precision
-        return _lib.create("mica", d, device)
-
     def _check(self, images):
-        if any(m.training for m in self.modules() if isinstance(m, nn.modules.batchnorm._BatchNorm)):
-            raise RuntimeError("smirk_b200.MICA: BatchNorm in train mode is not implemented (the trainer runs MICA in eval "
-                               "mode); call .eval() on the module")
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            raise RuntimeError("smirk_b200.MICA: weight gradients are not implemented (the trainer freezes MICA); set "
-                               "requires_grad=False on its parameters or run it under torch.no_grad()")
+        self._check_frozen()
         _lib.require_cuda(images, "images")
         if images.dim() != 4 or tuple(images.shape[1:]) != (3, 112, 112) or images.shape[0] < 1:
             raise RuntimeError("smirk_b200.MICA: expected images [B,3,112,112] (the 112x112 ArcFace crops), got %s"

@@ -12,11 +12,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def test_every_header_prototype_is_exported_and_bound_in_header_order(native_lib):
-    """The library exports every prototype in include/smirk_b200.h (all 83 entry points: the input gradients, the
-    video grid, the encoder's train mode and its kernel test entry points included), and each has exactly one row in
+    """The library exports every prototype in include/smirk_b200.h (all 117 entry points: the input gradients, the
+    video grid, the encoder's and the generator's train modes and their kernel test entry points, the trainer's masking
+    and cycle augmentation, and the VGG, MICA and expression losses included), and each has exactly one row in
     _lib.BINDINGS, in the header's order, with the same return type and the same
     parameters: count, pointer / value kind, and the trailing stream where the header has one (which is what makes
-    `_lib.call` append the current stream)."""
+    `_lib.call` append the current stream).  The ctypes structure of the augmentation's draws has the header's fields in
+    its order, and the kernel test entry points of the expression loss, which the header leaves out, are exported."""
     import ctypes as C
     from smirk_b200 import _lib
     hdr = open(os.path.join(ROOT, "include", "smirk_b200.h")).read()
@@ -28,7 +30,7 @@ def test_every_header_prototype_is_exported_and_bound_in_header_order(native_lib
     assert native_lib.smk_version() == 100
     protos = re.findall(r"^\s*([A-Za-z_][\w ]*?\**)\s*\b(smk_\w+)\s*\(([^)]*)\)\s*;", hdr, flags=re.M)
     table = {name: (restype, args) for name, restype, args in _lib.BINDINGS}
-    assert len(protos) == 83 and len(table) == len(_lib.BINDINGS)
+    assert len(protos) == 117 and len(table) == len(_lib.BINDINGS)
     assert [name for _, name, _ in protos] == [name for name, _, _ in _lib.BINDINGS]
     returns = {"int": C.c_int, "size_t": C.c_size_t, "void": None, "const char*": C.c_char_p, "unsigned long long": C.c_ulonglong}
     values = {"int": C.c_int, "size_t": C.c_size_t, "float": C.c_float}
@@ -45,6 +47,10 @@ def test_every_header_prototype_is_exported_and_bound_in_header_order(native_lib
             else:
                 assert a is values[q.rsplit(None, 1)[0]], (name, q)
         assert (name in _lib._TAKES_STREAM) == (args[-1:] == [_lib.STREAM]), name
+    draws = hdr[hdr.index("int64_t* gids"):hdr.index("} SmkCycleDraws")]
+    assert [f for f, _ in _lib.SmkCycleDraws._fields_] == re.findall(r"\*\s*(\w+);", draws)
+    for k in ("im2col", "maxpool", "maxpool_bwd", "col2im", "stem_dgrad", "head", "head_bwd"):
+        assert hasattr(native_lib, "smk_debug_expression_" + k)
 
 
 def test_create_rejects_bad_arguments_without_gpu(native_lib):

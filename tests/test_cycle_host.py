@@ -1,10 +1,8 @@
 """CPU suite of the trainer's masking and cycle augmentation: the restatement of tests/cycle_ref.py against the reference
-trainer's own step1 / step2 (live where the reference checkout is importable, and against tests/golden/cycle.npz), the C
-ABI of include/smirk_b200_cycle.h and the argument checks of its entry points."""
+trainer's own step1 / step2 (live where the reference checkout is importable, and against tests/golden/cycle.npz) and the
+argument checks of its entry points."""
 import ctypes as C
-import os
 import random
-import re
 
 import numpy as np
 import pytest
@@ -13,7 +11,6 @@ import torch
 import cycle_ref
 import make_golden_cycle as mgc
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 N_POINTS = int(0.01 * 224 * 224)
 
 
@@ -87,22 +84,6 @@ def test_rendered_mask_rules_differ_on_one_zero_channel():
     r[0, :, 1, 1] = 0.0
     assert cycle_ref.rendered_mask_first(r).flatten().tolist() == [1, 1, 1, 0]
     assert cycle_ref.rendered_mask_second(r).flatten().tolist() == [0, 1, 1, 0]
-
-
-def test_cycle_header_prototypes_are_exported_and_bound_in_order(native_lib):
-    from smirk_b200 import _lib
-    hdr = open(os.path.join(ROOT, "include", "smirk_b200_cycle.h")).read()
-    hdr = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
-    protos = re.findall(r"^\s*([A-Za-z_][\w ]*?\**)\s*\b(smk_\w+)\s*\(([^)]*)\)\s*;", hdr, flags=re.M)
-    assert [name for _, name, _ in protos] == [name for name, _, _ in _lib.CYCLE_BINDINGS]
-    for ret, name, params in protos:
-        assert hasattr(native_lib, name), name
-        _, restype, args = next(b for b in _lib.CYCLE_BINDINGS if b[0] == name)
-        assert (restype is C.c_int) == (ret.strip() == "int") and (restype is C.c_size_t) == (ret.strip() == "size_t"), name
-        params = [q.strip() for q in params.split(",") if q.strip()]
-        assert len(args) == len(params), name
-        assert (args[-1] is _lib.STREAM) == params[-1].endswith("stream"), name
-    assert [f for f, _ in _lib.SmkCycleDraws._fields_] == re.findall(r"\*\s*(\w+);", hdr[hdr.index("int64_t* gids"):hdr.index("} SmkCycleDraws")])
 
 
 def test_cycle_entry_points_reject_bad_arguments(native_lib):

@@ -1,10 +1,8 @@
 """CPU suite for smirk_b200.ExpressionLoss: the torch restatement (tests/expression_ref.py) against the reference class
 and its golden fixture, the replay oracle against plain autograd, the module tree and state_dict keys, checkpoint
-loading, the ABI of include/smirk_b200_expression.h, the arguments the module rejects without a GPU, and the drop-in
-alias."""
+loading, the arguments the module rejects without a GPU, and the drop-in alias."""
 import ctypes as C
 import os
-import re
 import sys
 import tempfile
 
@@ -14,7 +12,6 @@ import torch
 import expression_ref
 import make_golden_expression_loss as mg
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 METRICS = ("l2", "l1", "cos")
 
 
@@ -120,35 +117,6 @@ def test_checkpoint_loads_as_the_reference_does(sd):
             os.chdir(old)
 
 
-def test_expression_header_prototypes_are_exported_and_bound_in_header_order(native_lib):
-    """Every prototype of include/smirk_b200_expression.h is exported and has one row in _lib.EXPRESSION_BINDINGS, in
-    the header's order, with the same return type and parameter kinds, and the trailing stream where the header has one."""
-    from smirk_b200 import _lib
-    hdr = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "smirk_b200_expression.h")).read(), flags=re.S)
-    protos = re.findall(r"^\s*([A-Za-z_][\w ]*?\**)\s*\b(smk_\w+)\s*\(([^)]*)\)\s*;", hdr, flags=re.M)
-    assert len(protos) == 9 and [n for _, n, _ in protos] == [n for n, _, _ in _lib.EXPRESSION_BINDINGS]
-    assert not {n for n, _, _ in _lib.EXPRESSION_BINDINGS} & {n for n, _, _ in _lib.BINDINGS + _lib.LOSS_BINDINGS + _lib.MICA_BINDINGS}
-    returns = {"int": C.c_int, "size_t": C.c_size_t, "void": None}
-    values = {"int": C.c_int, "size_t": C.c_size_t, "float": C.c_float}
-    table = {name: (restype, args) for name, restype, args in _lib.EXPRESSION_BINDINGS}
-    for ret, name, params in protos:
-        assert hasattr(native_lib, name), "missing export: " + name
-        restype, args = table[name]
-        assert restype is returns[ret.strip()], name
-        params = [q.strip() for q in params.split(",") if q.strip() not in ("", "void")]
-        assert len(args) == len(params), name
-        for q, a in zip(params, args):
-            if q.endswith("stream"):
-                assert a is _lib.STREAM, (name, q)
-            elif "*" in q:
-                assert a in (C.c_void_p, C.c_char_p) or issubclass(a, C._Pointer), (name, q)
-            else:
-                assert a is values[q.rsplit(None, 1)[0]], (name, q)
-        assert (name in _lib._TAKES_STREAM) == (args[-1:] == [_lib.STREAM]), name
-    for k in ("im2col", "maxpool", "maxpool_bwd", "col2im", "stem_dgrad", "head", "head_bwd"):
-        assert hasattr(native_lib, "smk_debug_expression_" + k)
-
-
 def test_arguments_rejected_without_a_gpu(native_lib, monkeypatch):
     import smirk_b200
     from smirk_b200 import _lib
@@ -181,7 +149,7 @@ def test_arguments_rejected_without_a_gpu(native_lib, monkeypatch):
     keep = [_lib.f32(torch.ones(2048 * 512)) for _ in range(265)]
     arr = (_lib.c_f32p * 265)(*[k[1] for k in keep])
     for precision, n, what in ((2, 265, b"precision"), (0, 264, b"265 tensors")):
-        d = _lib.SmkExpressionLossDesc()
+        d = _lib.SmkNetDesc()
         d.tensors, d.n_tensors, d.precision = C.cast(arr, C.POINTER(_lib.c_f32p)), n, precision
         h = C.c_void_p()
         assert native_lib.smk_expression_loss_create(C.byref(d), C.byref(h)) < 0

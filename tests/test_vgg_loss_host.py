@@ -1,17 +1,13 @@
 """CPU suite for smirk_b200.VGGPerceptualLoss: the module tree and state_dict keys of the reference class, the torch
 restatement (tests/vgg_ref.py) against the reference class and its golden fixture, the replay oracle against plain
-autograd, the ABI of include/smirk_b200_loss.h, and the arguments the module rejects."""
+autograd, and the arguments the module rejects."""
 import ctypes as C
-import os
-import re
 
 import pytest
 import torch
 
 import make_golden_vgg_loss as mg
 import vgg_ref
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def rel_err(a, b):
@@ -74,33 +70,6 @@ def test_replay_with_the_oracles_own_choices_is_plain_autograd():
     assert rel_err(rgx, gx) <= 1e-6 and rel_err(rgy, gy) <= 1e-6
 
 
-def test_loss_header_prototypes_are_exported_and_bound_in_header_order(native_lib):
-    """Every prototype of include/smirk_b200_loss.h is exported and has one row in _lib.LOSS_BINDINGS, in the header's
-    order, with the same return type and parameter kinds, and the trailing stream where the header has one."""
-    from smirk_b200 import _lib
-    hdr = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "smirk_b200_loss.h")).read(), flags=re.S)
-    protos = re.findall(r"^\s*([A-Za-z_][\w ]*?\**)\s*\b(smk_\w+)\s*\(([^)]*)\)\s*;", hdr, flags=re.M)
-    assert len(protos) == 9 and [n for _, n, _ in protos] == [n for n, _, _ in _lib.LOSS_BINDINGS]
-    assert not {n for n, _, _ in _lib.LOSS_BINDINGS} & {n for n, _, _ in _lib.BINDINGS}
-    returns = {"int": C.c_int, "size_t": C.c_size_t, "void": None}
-    values = {"int": C.c_int, "size_t": C.c_size_t, "float": C.c_float}
-    table = {name: (restype, args) for name, restype, args in _lib.LOSS_BINDINGS}
-    for ret, name, params in protos:
-        assert hasattr(native_lib, name), "missing export: " + name
-        restype, args = table[name]
-        assert restype is returns[ret.strip()], name
-        params = [q.strip() for q in params.split(",") if q.strip() not in ("", "void")]
-        assert len(args) == len(params), name
-        for q, a in zip(params, args):
-            if q.endswith("stream"):
-                assert a is _lib.STREAM, (name, q)
-            elif "*" in q:
-                assert a in (C.c_void_p, C.c_char_p) or issubclass(a, C._Pointer), (name, q)
-            else:
-                assert a is values[q.rsplit(None, 1)[0]], (name, q)
-        assert (name in _lib._TAKES_STREAM) == (args[-1:] == [_lib.STREAM]), name
-
-
 def test_bad_arguments_raise(native_lib, monkeypatch):
     import smirk_b200
     from smirk_b200 import _lib
@@ -122,7 +91,7 @@ def test_bad_arguments_raise(native_lib, monkeypatch):
     keep = [_lib.f32(torch.ones(512 * 512 * 9)) for _ in range(22)]
     arr = (_lib.c_f32p * 22)(*[k[1] for k in keep])
     for precision, n, what in ((2, 22, b"precision"), (0, 21, b"22 tensors")):
-        d = _lib.SmkVggLossDesc()
+        d = _lib.SmkNetDesc()
         d.tensors, d.n_tensors, d.precision = C.cast(arr, C.POINTER(_lib.c_f32p)), n, precision
         h = C.c_void_p()
         assert native_lib.smk_vgg_loss_create(C.byref(d), C.byref(h)) < 0
