@@ -229,7 +229,14 @@ BINDINGS = [
     ("smk_debug_train_stem_wgrad", _i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, STREAM]),
     ("smk_debug_train_head_backward", _i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, STREAM]),
 ]
-_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS if args[-1:] == [STREAM])
+# The live eval handles of include/smirk_b200_live.h, in that header's order.
+LIVE_BINDINGS = [
+    ("smk_encoder_live_create", _i, [_i, _i, _i, _i, _vpp]),
+    ("smk_encoder_refresh", _i, [_vp, C.POINTER(SmkEncoderTrainArgs), STREAM]),
+    ("smk_generator_live_create", _i, [_i, _i, _i, _i, _i, _vpp]),
+    ("smk_generator_refresh", _i, [_vp, C.POINTER(SmkGeneratorTrainArgs), STREAM]),
+]
+_TAKES_STREAM = frozenset(name for name, _, args in BINDINGS + LIVE_BINDINGS if args[-1:] == [STREAM])
 
 
 def lib():
@@ -241,7 +248,7 @@ def lib():
         raise RuntimeError("smirk_b200: %s not found — build it with `python -m smirk_b200.build` "
                            "(there is no CPU / PyTorch fallback)" % LIB_PATH)
     L = C.CDLL(LIB_PATH)
-    for name, restype, argtypes in BINDINGS:
+    for name, restype, argtypes in BINDINGS + LIVE_BINDINGS:
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, [_vp if a is STREAM else a for a in argtypes]
     if L.smk_version() != 100:
@@ -295,6 +302,26 @@ def require_cuda(t, name):
 def dev_f32(t, name):
     require_cuda(t, name)
     return t.detach().to(torch.float32).contiguous()
+
+
+def live_handle(module, kind, dev, key, create_args):
+    """The live eval handle ``smk_<kind>_live_create(*create_args)`` of ``module``, kept in its NativeState for ``key``
+    (topology and precision: an optimizer step builds nothing).  ``generation`` counts its refreshes."""
+    st = module._native
+    key = (str(dev),) + tuple(key)
+    if st.live_handle is None or st.live_key != key:
+        st.live_handle = None
+        h = C.c_void_p()
+        call("smk_%s_live_create" % kind, dev, *create_args, C.byref(h))
+        st.live_handle, st.live_key = NativeHandle(h, "smk_%s_destroy" % kind), key
+        st.live_handle.generation = 0
+    return st.live_handle
+
+
+def refresh(kind, h, dev, args):
+    """``smk_<kind>_refresh(h, &args)`` on the current stream; bumps the handle's generation."""
+    call("smk_%s_refresh" % kind, dev, h, C.byref(args))
+    h.generation += 1
 
 
 class NativeHandle:
@@ -378,6 +405,7 @@ class NativeState:
     def __init__(self):
         self.handle, self.key, self.workspaces, self.per_device = None, None, {}, {}
         self.train_handle, self.train_key = None, None        # the train-mode handle (topology only) of the encoder or generator
+        self.live_handle, self.live_key = None, None          # the live eval handle (weights refreshed on the device per call)
 
 
 class NativeModule:
@@ -416,7 +444,8 @@ class NativeModule:
         """What a CUDA graph captured over this module must keep alive: the handle (packed weights) and the forward
         workspace it was recorded with."""
         ws = self._native.workspaces.get("forward")
-        return self._native.handle, ws.buf if ws is not None else None
+        h = self._native.live_handle if self.__dict__.get("_live") else self._native.handle
+        return h, ws.buf if ws is not None else None
 
     def __deepcopy__(self, memo):
         """Same parameter and buffer values; the copy builds its own native state on first use."""

@@ -56,6 +56,15 @@ struct DeviceArena {
     }
     template <typename T>
     cudaError_t upload(const std::vector<T>& v, T** out) { return upload(v.data(), v.size(), out); }
+    template <typename T>
+    cudaError_t alloc(size_t n, T** out) {                  // unset: a live handle's weights, written on the device
+        void* d = nullptr;
+        cudaError_t e = cudaMalloc(&d, n * sizeof(T) + 16);
+        if (e != cudaSuccess) return e;
+        ptrs.push_back(d);
+        *out = (T*)d;
+        return e;
+    }
 };
 
 // Bump allocator over the caller-provided workspace (256-byte aligned slices).

@@ -17,6 +17,7 @@
 #include "nn_kernels.cuh"
 #include "gemm_tc.cuh"
 #include "xdw_tc.cuh"
+#include "../../include/smirk_b200_live.h"
 #include <math.h>
 
 namespace {
@@ -28,25 +29,34 @@ using smk::same_pad_begin;
 
 constexpr float kBnEps = 1e-3f;
 
-// Consumes (conv weight, bn gamma, beta, mean, var) from the tensor list: the folded BN scale s and bias, the forward
-// weights, and the dgrad weights, which carry s.
+// The operands of one conv, decided once for the host fold (smk_encoder_create) and the device refresh
+// (smk_encoder_live_create):
 //   kind 0 = 1x1 [Cout,Cin,1,1]: smk::pack_gemm operands, the forward's N = cout, K = cin, the dgrad's (diag(s) W)^T,
-//            N = cin, K = cout.  fwd_f32: the forward weights in fp32 even when tc (a DS block's 1x1 that stem_ds runs).
+//            N = cin, K = cout.  fwd_tc / dgrad_tc: TF32 [N][K] (with tails when x3), otherwise fp32 [K][N]; the forward
+//            is fp32 even when tc for a DS block's 1x1 that stem_ds runs (fwd_f32).
 //   kind 1 = depthwise [C,1,3,3] -> W[9][C]; dgrad: flipped taps, Wd[8 - k][c] = s[c] W[c][k]
 //   kind 2 = stem [16,3,3,3] -> W[27][16]; dgrad: Wd[k][o] = s[o] W[o][k] (the forward layout)
-bool fold_conv(TensorCursor& cur, int kind, int cin, int cout, bool tc, bool x3, smk::DeviceArena& arena, ConvW* out, cudaError_t* err,
-               bool fwd_f32 = false) {
+struct ConvOps { int kind, cin, cout; bool fwd_tc, dgrad_tc, x3; };
+ConvOps conv_ops(int kind, int cin, int cout, bool tc, bool x3, bool fwd_f32 = false) {
+    const bool pw = kind == 0;
+    return ConvOps{kind, cin, cout, pw && tc && !fwd_f32, pw && tc, pw && tc && x3};
+}
+
+// Consumes (conv weight, bn gamma, beta, mean, var) from the tensor list: the folded BN scale s and bias, the forward
+// weights, and the dgrad weights, which carry s.
+bool fold_conv(TensorCursor& cur, const ConvOps& c, smk::DeviceArena& arena, ConvW* out, cudaError_t* err) {
     const float* w = cur.next(); const float* g = cur.next(); const float* b = cur.next();
     const float* mu = cur.next(); const float* var = cur.next();
     if (!w || !g || !b || !mu || !var) return false;
+    const int cin = c.cin, cout = c.cout, kind = c.kind;
     std::vector<float> S(cout), Bi(cout);
     smk::fold_bn(g, b, mu, var, cout, kBnEps, S.data(), Bi.data());
     out->cin = cin; out->cout = cout;
     cudaError_t e = arena.upload(S, &out->scale);
     if (e == cudaSuccess) e = arena.upload(Bi, &out->bias);
     if (kind == 0) {                                          // torch's [Cout][Cin] is the forward's [N][K]
-        if (e == cudaSuccess) e = smk::pack_gemm(arena, cout, cin, tc && !fwd_f32, x3, w, &out->fwd);
-        if (e == cudaSuccess) e = smk::pack_gemm(arena, cin, cout, tc, x3, [&](int c, int o) { return S[o] * w[(size_t)o * cin + c]; }, &out->dgrad);
+        if (e == cudaSuccess) e = smk::pack_gemm(arena, cout, cin, c.fwd_tc, c.x3, w, &out->fwd);
+        if (e == cudaSuccess) e = smk::pack_gemm(arena, cin, cout, c.dgrad_tc, c.x3, [&](int ci, int o) { return S[o] * w[(size_t)o * cin + ci]; }, &out->dgrad);
     } else {
         const int K = kind == 1 ? 9 : 27;
         std::vector<float> W((size_t)K * cout), D(W.size());
@@ -64,8 +74,81 @@ bool fold_conv(TensorCursor& cur, int kind, int cin, int cout, bool tc, bool x3,
     return e == cudaSuccess;
 }
 
+// The live counterpart of fold_conv for the conv whose weight is tensor t of backbone i: allocates its buffers and records
+// the refresh's fold and pack jobs in the layouts of fold_conv (trn::PackJob: MAT transposes torch's [cout][cols] where
+// the operand is not torch-ordered, DW_DGRAD flips the depthwise taps; the dgrad jobs multiply in the folded scale).
+cudaError_t live_conv(const ConvOps& c, int i, int t, smk::DeviceArena& arena, trn::LivePlan& plan, ConvW* out) {
+    const int cin = c.cin, cout = c.cout, cols = c.kind == 0 ? cin : c.kind == 1 ? 9 : 27;
+    out->cin = cin; out->cout = cout;
+    cudaError_t e = arena.alloc((size_t)cout, &out->scale);
+    if (e == cudaSuccess) e = arena.alloc((size_t)cout, &out->bias);
+    if (e != cudaSuccess) return e;
+    plan.folds.push_back(trn::LiveFold{i, t, trn::FoldJob{nullptr, nullptr, nullptr, nullptr, out->scale, out->bias, cout, 0.f}});
+    // One operand of torch's [cout][cols] weight: transposed unless torch-ordered, split into TF32 heads (+ tails) when tc.
+    auto add = [&](int kind, bool transpose, bool tc, const float* scale, smk::GemmW* w) {
+        trn::PackJob j{};
+        j.kind = kind; j.rows = cout; j.cols = cols; j.transpose = transpose ? 1 : 0; j.split = tc ? 1 : 0; j.cout = cout; j.scale = scale;
+        const size_t n = (size_t)cout * cols;
+        float *hi = nullptr, *lo = nullptr;
+        cudaError_t r = arena.alloc(n, &hi);
+        if (r == cudaSuccess && tc && c.x3) r = arena.alloc(n, &lo);
+        j.hi = hi; j.lo = lo;
+        plan.jobs.push_back(trn::LiveJob{i, t, j});
+        plan.bytes += 4.0 * n * (2 + (lo ? 1 : 0));
+        *w = tc ? smk::GemmW{nullptr, hi, lo} : smk::GemmW{hi, nullptr, nullptr};
+        return r;
+    };
+    if (c.kind == 0) {          // forward [N = cout][K = cin] is torch's order; the dgrad's [N = cin][K = cout] is its transpose
+        e = add(trn::MAT, !c.fwd_tc, c.fwd_tc, nullptr, &out->fwd);
+        if (e == cudaSuccess) e = add(trn::MAT, c.dgrad_tc, c.dgrad_tc, out->scale, &out->dgrad);
+    } else {                    // fp32 [K][N] = torch's [cout][K] transposed; the depthwise dgrad flips its taps
+        e = add(trn::MAT, true, false, nullptr, &out->fwd);
+        if (e == cudaSuccess) e = add(c.kind == 1 ? trn::DW_DGRAD : trn::MAT, c.kind != 1, false, out->scale, &out->dgrad);
+    }
+    return e;
+}
+
 // Stem + block 0 run as one fp32 kernel (stem_ds) at every precision but 1, whose block-0 1x1 runs on TF32 tensor cores.
 bool fuse_stem(const SmkEncoder* h) { return h->precision == 0 || h->fuse_xdw; }
+
+// Every conv of backbone i in tensor-list order with its operands: visit(ConvOps, ConvW*) -> false stops the walk.
+template <typename Visit>
+bool for_each_conv(SmkEncoder* h, int i, Visit&& visit) {
+    const bool tc = h->precision >= 1, x3 = h->x3;
+    Backbone& bb = h->bb[i];
+    if (!visit(conv_ops(2, 3, 16, false, false), &bb.stem)) return false;
+    for (Block& b : bb.blocks) {
+        bool ok;
+        if (b.kind == DS) ok = visit(conv_ops(1, b.cin, b.cin, false, false), &b.dw) && visit(conv_ops(0, b.cin, b.cout, tc, x3, fuse_stem(h)), &b.pw);
+        else if (b.kind == IR) ok = visit(conv_ops(0, b.cin, b.mid, tc, x3), &b.pw) && visit(conv_ops(1, b.mid, b.mid, false, false), &b.dw) &&
+                                    visit(conv_ops(0, b.mid, b.cout, tc, x3), &b.pwl);
+        else ok = visit(conv_ops(0, b.cin, b.cout, tc, x3), &b.pw);
+        if (!ok) return false;
+    }
+    return true;
+}
+
+// The saved-tensor layout of backbone i's eval path: forward order (names: the reference's module paths).
+void add_saved(SmkEncoder* h, int i) {
+    Backbone& bb = h->bb[i];
+    auto add = [h](const std::string& name, int H, int C) { return h->saved.add(name, H, H, C); };
+    bb.sv_stem = add(std::string(kEncName[i]) + ".encoder.bn1", 112, 16);
+    for (Block& b : bb.blocks) {
+        if (b.kind == DS) b.sv_a = add(b.path + ".bn1", b.hout, b.cin);
+        else if (b.kind == IR) { b.sv_a = add(b.path + ".bn1", b.hin, b.mid); b.sv_b = add(b.path + ".bn2", b.hout, b.mid); }
+        else b.sv_a = add(b.path + ".bn1", b.hout, b.cout);
+    }
+    bb.sv_head = add(std::string(kEncName[i]) + "." + kHeadName[i], 1, bb.n_out);
+}
+
+// Precision 0-3 of SmkEncoderDesc -> the handle's flags.
+void set_precision(SmkEncoder* h, int precision) {
+    h->precision = precision >= 1 ? 1 : 0; h->fuse_xdw = precision >= 2; h->x3 = precision == 3;
+}
+
+// A handle refreshed on the device must have been refreshed once before the eval path reads its weights.
+#define SMK_REQUIRE_WEIGHTS(h, fn) \
+    SMK_REQUIRE(!(h)->live || (h)->refreshed, "%s: a live handle whose weights were never set: call smk_encoder_refresh first", fn)
 
 }  // namespace
 
@@ -75,37 +158,17 @@ extern "C" int smk_encoder_create(const SmkEncoderDesc* desc, SmkEncoder** out) 
                 "smk_encoder_create: precision must be 0 (fp32 CUDA cores), 1 (tf32 wgmma 1x1 convs), 2 (1 + fused expand/depthwise blocks) or "
                 "3 (2 with 3xTF32 error-compensated tensor-core arithmetic: fp32-equivalent results)");
     if (desc->precision >= 1) { if (int rc = smk::tc_init()) return rc; }
-    const bool tc = desc->precision >= 1;
     SmkEncoder* h = new SmkEncoder();
-    h->n_shape = desc->n_shape; h->n_exp = desc->n_exp; h->precision = tc ? 1 : 0; h->fuse_xdw = desc->precision >= 2; h->x3 = desc->precision == 3;
-    const bool x3 = h->x3;
+    h->n_shape = desc->n_shape; h->n_exp = desc->n_exp;
+    set_precision(h, desc->precision);
     cudaError_t e = cudaSuccess;
-    // saved-tensor layout: forward order within a backbone (names: the reference's module paths)
-    auto add = [h](const std::string& name, int H, int C) { return h->saved.add(name, H, H, C); };
     for (int i = 0; i < 3; ++i) {
         Backbone& bb = h->bb[i];
         if (desc->n_tensors[i] == 0 || desc->tensors[i] == nullptr) continue;        // backbone not part of this handle
         h->present[i] = true;
         build_backbone(h, i);
         TensorCursor cur{desc->tensors[i], desc->n_tensors[i]};
-        bool ok = fold_conv(cur, 2, 3, 16, false, false, h->arena, &bb.stem, &e);
-        bb.sv_stem = add(std::string(kEncName[i]) + ".encoder.bn1", 112, 16);
-        for (Block& b : bb.blocks) {
-            if (!ok) break;
-            if (b.kind == DS) {
-                ok = fold_conv(cur, 1, b.cin, b.cin, false, false, h->arena, &b.dw, &e) &&
-                     fold_conv(cur, 0, b.cin, b.cout, tc, x3, h->arena, &b.pw, &e, fuse_stem(h));
-                b.sv_a = add(b.path + ".bn1", b.hout, b.cin);
-            } else if (b.kind == IR) {
-                ok = fold_conv(cur, 0, b.cin, b.mid, tc, x3, h->arena, &b.pw, &e) &&
-                     fold_conv(cur, 1, b.mid, b.mid, false, false, h->arena, &b.dw, &e) &&
-                     fold_conv(cur, 0, b.mid, b.cout, tc, x3, h->arena, &b.pwl, &e);
-                b.sv_a = add(b.path + ".bn1", b.hin, b.mid); b.sv_b = add(b.path + ".bn2", b.hout, b.mid);
-            } else {
-                ok = fold_conv(cur, 0, b.cin, b.cout, tc, x3, h->arena, &b.pw, &e);
-                b.sv_a = add(b.path + ".bn1", b.hout, b.cout);
-            }
-        }
+        const bool ok = for_each_conv(h, i, [&](const ConvOps& c, ConvW* w) { return fold_conv(cur, c, h->arena, w, &e); });
         if (!ok || cur.i != cur.n) {
             if (e != cudaSuccess) smk::set_error("smk_encoder_create: upload failed: %s", cudaGetErrorString(e));
             else smk::set_error("smk_encoder_create: backbone %d expects %d tensors (conv weight + 4 BN tensors per conv), got %d",
@@ -115,12 +178,68 @@ extern "C" int smk_encoder_create(const SmkEncoderDesc* desc, SmkEncoder** out) 
         e = h->arena.upload(desc->head_w[i], (size_t)bb.n_out * bb.feat, &bb.head_w);
         if (e == cudaSuccess) e = h->arena.upload(desc->head_b[i], (size_t)bb.n_out, &bb.head_b);
         if (e != cudaSuccess) { smk::set_error("smk_encoder_create: upload failed: %s", cudaGetErrorString(e)); delete h; return (int)e; }
-        bb.sv_head = add(std::string(kEncName[i]) + "." + kHeadName[i], 1, bb.n_out);
+        add_saved(h, i);
     }
     if (!h->present[0] && !h->present[1] && !h->present[2]) { smk::set_error("smk_encoder_create: no backbone given"); delete h; return -1; }
     e = finish_create(h);
     if (e != cudaSuccess) { smk::set_error("smk_encoder_create: upload or stream/event creation failed: %s", cudaGetErrorString(e)); delete h; return (int)e; }
     *out = h;
+    return 0;
+}
+
+extern "C" int smk_encoder_live_create(int backbones, int n_shape, int n_exp, int precision, SmkEncoder** out) {
+    SMK_REQUIRE(out, "smk_encoder_live_create: null argument");
+    SMK_REQUIRE(backbones > 0 && backbones < 8, "smk_encoder_live_create: backbones is a non-empty bit set of {1 pose, 2 shape, 4 expression}");
+    SMK_REQUIRE(precision >= 0 && precision <= 3, "smk_encoder_live_create: precision must be 0, 1, 2 or 3");
+    SMK_REQUIRE(n_shape > 0 && n_exp >= 0 && n_shape <= 4096 && n_exp <= 4096, "smk_encoder_live_create: bad head widths");
+    if (precision >= 1) { if (int rc = smk::tc_init()) return rc; }
+    SmkEncoder* h = new SmkEncoder();
+    h->live = true;
+    h->n_shape = n_shape; h->n_exp = n_exp;
+    set_precision(h, precision);
+    cudaError_t e = cudaSuccess;
+    for (int i = 0; i < 3 && e == cudaSuccess; ++i) {
+        if (!((backbones >> i) & 1)) continue;
+        Backbone& bb = h->bb[i];
+        h->present[i] = true;
+        build_backbone(h, i);
+        int t = 0;
+        for_each_conv(h, i, [&](const ConvOps& c, ConvW* w) { e = live_conv(c, i, t, h->arena, h->plan, w); t += 5; return e == cudaSuccess; });
+        h->live_tensors[i] = t;
+        for (int k = 0; k < 2 && e == cudaSuccess; ++k) {             // the heads, copied as they are
+            float* dst = nullptr;
+            const int n = k == 0 ? bb.n_out * bb.feat : bb.n_out;
+            e = h->arena.alloc((size_t)n, &dst);
+            trn::PackJob j{};
+            j.kind = trn::MAT; j.rows = 1; j.cols = n; j.hi = dst;
+            h->plan.jobs.push_back(trn::LiveJob{i, -1 - k, j});
+            h->plan.bytes += 8.0 * n;
+            (k == 0 ? bb.head_w : bb.head_b) = dst;
+        }
+        add_saved(h, i);
+    }
+    if (e == cudaSuccess) e = finish_create(h);
+    if (e != cudaSuccess) { smk::set_error("smk_encoder_live_create: allocation or stream/event creation failed: %s", cudaGetErrorString(e)); delete h; return (int)e; }
+    *out = h;
+    return 0;
+}
+
+extern "C" int smk_encoder_refresh(SmkEncoder* h, const SmkEncoderTrainArgs* a, void* stream) {
+    const char* fn = "smk_encoder_refresh";
+    SMK_REQUIRE(h && h->live, "%s: not a live handle (smk_encoder_live_create)", fn);
+    SMK_REQUIRE(a, "%s: null args", fn);
+    for (int i = 0; i < 3; ++i) {
+        if (!h->present[i]) continue;
+        const int n = h->live_tensors[i];
+        SMK_REQUIRE(a->tensors[i] && a->n_tensors[i] == n, "%s: backbone %d expects %d tensors (conv weight + 4 BN tensors per conv), got %d",
+                    fn, i, n, a->n_tensors[i]);
+        for (int k = 0; k < n; ++k) SMK_REQUIRE(a->tensors[i][k], "%s: backbone %d: null tensor %d", fn, i, k);
+        SMK_REQUIRE(a->head_w[i] && a->head_b[i], "%s: backbone %d: null head", fn, i);
+        SMK_REQUIRE(a->eps[i] > 0.f, "%s: backbone %d: eps must be positive", fn, i);
+    }
+    const float* const* t[3] = {a->tensors[0], a->tensors[1], a->tensors[2]};
+    if (int rc = trn::refresh(h->plan, t, a->head_w, a->head_b, a->eps, (cudaStream_t)stream)) return rc;
+    h->refreshed = true;
     return 0;
 }
 
@@ -258,6 +377,7 @@ extern "C" int smk_encoder_forward(const SmkEncoder* h, const float* img, int B,
     SMK_REQUIRE(B > 0, "smk_encoder_forward: negative batch");
     SMK_REQUIRE(ws && ws_bytes >= smk_encoder_workspace_bytes(h, B), "smk_encoder_forward: workspace too small");
     SMK_REQUIRE(!h->train, "smk_encoder_forward: a train-mode handle runs smk_encoder_forward_train");
+    SMK_REQUIRE_WEIGHTS(h, "smk_encoder_forward");
     return encoder_forward(h, img, B, pose_cam, shape, expr, nullptr, ws, ws_bytes, (cudaStream_t)stream);
 }
 
@@ -437,6 +557,7 @@ extern "C" int smk_encoder_forward_saved(const SmkEncoder* h, const float* img, 
                 "smk_encoder_forward_saved: null output for a backbone this handle holds");
     SMK_REQUIRE(ws && ws_bytes >= smk_encoder_workspace_bytes(h, B), "smk_encoder_forward_saved: workspace too small");
     SMK_REQUIRE(!h->train, "smk_encoder_forward_saved: a train-mode handle runs smk_encoder_forward_train");
+    SMK_REQUIRE_WEIGHTS(h, "smk_encoder_forward_saved");
     return encoder_forward(h, img, B, pose_cam, shape, expr, saved, ws, ws_bytes, (cudaStream_t)stream);
 }
 
@@ -453,6 +574,7 @@ extern "C" int smk_encoder_backward(const SmkEncoder* h, int B, const float* sav
     SMK_REQUIRE(saved_bytes > 0 && saved_bytes >= smk_encoder_saved_bytes(h, B), "smk_encoder_backward: saved buffer too small");
     SMK_REQUIRE(ws && ws_bytes >= smk_encoder_backward_workspace_bytes(h, B), "smk_encoder_backward: workspace too small");
     SMK_REQUIRE(!h->train, "smk_encoder_backward: a train-mode handle runs smk_encoder_backward_train");
+    SMK_REQUIRE_WEIGHTS(h, "smk_encoder_backward");
     cudaStream_t main_st = (cudaStream_t)stream;
     const float* g_out[3] = {g_pose_cam, g_shape, g_expr};
     bool active[3];

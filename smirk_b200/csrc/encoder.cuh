@@ -1,7 +1,7 @@
 // The encoder handle shared by the eval path (encoder.cu) and the train-mode path (encoder_train.cu): the MobileNetV3
 // "minimal" layer lists, the per-backbone topology and its one builder, and the fork/join walk over the backbones.
 #pragma once
-#include "conv.cuh"
+#include "train_common.cuh"
 #include <string>
 
 namespace enc {
@@ -78,6 +78,10 @@ struct SmkEncoder {
     bool x3 = false;             // precision 3: 3xTF32 error-compensated tensor-core arithmetic (fp32-equivalent), no TF32 rounding of activations
     bool train = false;          // a train-mode handle (smk_encoder_train_create): topology only, no packed weights
     size_t stats_floats = 0;     // train handles: floats of BatchNorm statistics after the saved tensors (mean, invstd per BN)
+    bool live = false;           // a live eval handle (smk_encoder_live_create): weights set on the device by smk_encoder_refresh
+    bool refreshed = false;      // live handles: refreshed at least once
+    trn::LivePlan plan;          // live handles: the refresh's folds and pack jobs (lists = backbones)
+    int live_tensors[3] = {0, 0, 0};           // live handles: tensors per backbone the refresh reads
     bool present[3] = {false, false, false};   // a handle may hold a subset of the backbones (PoseEncoder / ShapeEncoder / ExpressionEncoder alone)
     float *ones = nullptr, *zeros = nullptr;   // unit scale / zero bias of the dgrad GEMM epilogues
     smk::SavedLayout saved;                    // of the grad-mode forward: forward order within a backbone, backbones in slot order

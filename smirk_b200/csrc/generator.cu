@@ -28,6 +28,7 @@
 #include "nn_kernels.cuh"
 #include "gemm_tc.cuh"
 #include "generator.cuh"
+#include "../../include/smirk_b200_live.h"
 #include <math.h>
 #include <algorithm>
 #include <string>
@@ -67,6 +68,95 @@ bool fold_upconv(TensorCursor& cur, int cin, int cout, bool tc, bool x3, smk::De
     return e == cudaSuccess;
 }
 
+// The live counterparts, for the layer whose first tensor is t: the buffers of fold_conv3 / fold_upconv, and the refresh's
+// jobs that fill them in their layouts (trn::PackJob's CONV3_* kinds are smk::pack_conv3's, the UP_* kinds the up-convolution's).
+struct LiveGen {
+    SmkGenerator* h; bool tc, x3;
+    cudaError_t op(int kind, int t, int cin, int cin_p, int cout, bool split, const float* scale, smk::GemmW* w) {
+        trn::PackJob j{};
+        j.kind = kind; j.cin = cin; j.cin_p = cin_p; j.cout = cout; j.split = split ? 1 : 0; j.scale = scale;
+        const size_t n = trn::pack_floats(j);
+        float *hi = nullptr, *lo = nullptr;
+        cudaError_t e = h->arena.alloc(n, &hi);
+        if (e == cudaSuccess && split && x3) e = h->arena.alloc(n, &lo);
+        j.hi = hi; j.lo = lo;
+        h->plan.jobs.push_back(trn::LiveJob{0, t, j});
+        h->plan.bytes += 4.0 * n * (2 + (lo ? 1 : 0));
+        *w = split ? smk::GemmW{nullptr, hi, lo} : smk::GemmW{hi, nullptr, nullptr};
+        return e;
+    }
+    cudaError_t conv3(int t, int cin, int cin_p, int cout, Conv3* out) {
+        out->cin = cin; out->cin_p = cin_p; out->cout = cout;
+        cudaError_t e = h->arena.alloc((size_t)cout, &out->scale);
+        if (e == cudaSuccess) e = h->arena.alloc((size_t)cout, &out->bias);
+        if (e != cudaSuccess) return e;
+        h->plan.folds.push_back(trn::LiveFold{0, t, trn::FoldJob{nullptr, nullptr, nullptr, nullptr, out->scale, out->bias, cout, 0.f}});
+        e = op(trn::CONV3_FWD, t, cin, cin_p, cout, tc, nullptr, &out->fwd);
+        return e == cudaSuccess ? op(trn::CONV3_DGRAD, t, cin, cin_p, cout, tc, out->scale, &out->dgrad) : e;
+    }
+    cudaError_t upconv(int t, int cin, int cout, UpConv* out) {
+        out->cin = cin; out->cout = cout;
+        const std::vector<float> one((size_t)4 * cout, 1.f);
+        cudaError_t e = h->arena.upload(one, &out->scale);
+        if (e == cudaSuccess) e = op(trn::UP_FWD, t, cin, cin, cout, tc, nullptr, &out->fwd);
+        if (e == cudaSuccess) e = op(trn::UP_DGRAD, t, cin, cin, cout, tc, nullptr, &out->dgrad);
+        smk::GemmW b{};
+        if (e == cudaSuccess) e = op(trn::UP_BIAS, t + 1, cin, cin, cout, false, nullptr, &b);
+        out->bias = const_cast<float*>(b.w);
+        return e;
+    }
+};
+
+// The handle's configuration, the same for every kind of handle: tensor-core operands unless precision 0, 3xTF32 at 3,
+// and the input channels padded for the first conv's kernel.
+void configure(SmkGenerator* h, int in_channels, int out_channels, int init_features, int res_blocks, int precision) {
+    h->cin = in_channels; h->cout = out_channels;
+    h->cin_p = precision != 0 ? (in_channels + 31) & ~31 : (in_channels + 7) & ~7;
+    h->f = init_features; h->nres = res_blocks; h->precision = precision;
+}
+
+// Every layer in state_dict order: conv3(cin, cin_p, cout, Conv3*) and up(cin, cout, UpConv*) -> false stops the walk.
+template <typename C3, typename Up>
+bool for_each_layer(SmkGenerator* h, C3&& conv3, Up&& up) {
+    const int f = h->f;
+    int c_in = h->cin, c_in_p = h->cin_p;
+    for (int l = 0; l < 5; ++l) {
+        const int co = f << l;
+        if (!conv3(c_in, c_in_p, co, &h->enc[l][0]) || !conv3(co, co, co, &h->enc[l][1])) return false;
+        c_in = c_in_p = co;
+    }
+    h->res.resize((size_t)2 * h->nres);
+    for (int r = 0; r < 2 * h->nres; ++r) if (!conv3(16 * f, 16 * f, 16 * f, &h->res[r])) return false;
+    for (int l = 0; l < 4; ++l) {          // level 4 -> 1
+        const int ci = (16 * f) >> l, co = ci / 2;
+        if (!up(ci, co, &h->up[l]) || !conv3(2 * co, 2 * co, co, &h->dec[l][0]) || !conv3(co, co, co, &h->dec[l][1])) return false;
+    }
+    return true;
+}
+
+// The saved-tensor layout of the grad-mode forward; every size is a multiple of 64 floats (init_features % 8 == 0), so the
+// tensors are packed with no gaps.
+void add_saved(SmkGenerator* h) {
+    const int f = h->f;
+    auto add = [h](const std::string& name, int S, int C) { h->saved.add(name, S, S, C); };
+    for (int l = 0; l < 4; ++l)
+        for (int j = 1; j <= 2; ++j) add("enc" + std::to_string(l + 1) + "conv" + std::to_string(j), 224 >> l, f << l);
+    add("bottleneckconv1", 14, 16 * f); add("bottleneckconv2", 14, 16 * f);
+    for (int r = 0; r < h->nres; ++r) add("res" + std::to_string(r) + "conv1", 14, 16 * f);
+    for (int l = 3; l >= 0; --l)
+        for (int j = 1; j <= 2; ++j) add("dec" + std::to_string(l + 1) + "conv" + std::to_string(j), 224 >> l, f << l);
+}
+
+// The unit scales / zero biases of the dgrad epilogues.
+cudaError_t upload_units(SmkGenerator* h) {
+    const std::vector<float> one((size_t)std::max(16 * h->f, h->cin_p), 1.f), zero(one.size(), 0.f);
+    cudaError_t e = h->arena.upload(one, &h->ones);
+    return e == cudaSuccess ? h->arena.upload(zero, &h->zeros) : e;
+}
+
+#define SMK_REQUIRE_WEIGHTS(h, fn) \
+    SMK_REQUIRE(!(h)->live || (h)->refreshed, "%s: a live handle whose weights were never set: call smk_generator_refresh first", fn)
+
 }  // namespace
 
 extern "C" int smk_generator_create(const SmkGeneratorDesc* desc, SmkGenerator** out) {
@@ -79,27 +169,12 @@ extern "C" int smk_generator_create(const SmkGeneratorDesc* desc, SmkGenerator**
     const bool tc = desc->precision != 0, x3 = desc->precision == 3;     // tensor cores; 3xTF32 arithmetic on them
     if (tc) { if (int rc = smk::tc_init()) return rc; }
     SmkGenerator* h = new SmkGenerator();
-    h->cin = desc->in_channels; h->cout = desc->out_channels;
-    h->cin_p = tc ? (desc->in_channels + 31) & ~31 : (desc->in_channels + 7) & ~7;
-    h->f = desc->init_features; h->nres = desc->res_blocks; h->precision = desc->precision;
+    configure(h, desc->in_channels, desc->out_channels, desc->init_features, desc->res_blocks, desc->precision);
     const int f = h->f;
     TensorCursor cur{desc->tensors, desc->n_tensors};
     cudaError_t e = cudaSuccess;
-    bool ok = true;
-    int c_in = h->cin, c_in_p = h->cin_p;
-    for (int l = 0; ok && l < 5; ++l) {
-        int co = f << l;
-        ok = fold_conv3(cur, c_in, c_in_p, co, tc, x3, h->arena, &h->enc[l][0], &e) &&
-             fold_conv3(cur, co, co, co, tc, x3, h->arena, &h->enc[l][1], &e);
-        c_in = c_in_p = co;
-    }
-    h->res.resize((size_t)2 * h->nres);
-    for (int r = 0; ok && r < 2 * h->nres; ++r) ok = fold_conv3(cur, 16 * f, 16 * f, 16 * f, tc, x3, h->arena, &h->res[r], &e);
-    for (int l = 0; ok && l < 4; ++l) {          // level 4 -> 1
-        int ci = (16 * f) >> l, co = ci / 2;
-        ok = fold_upconv(cur, ci, co, tc, x3, h->arena, &h->up[l], &e) && fold_conv3(cur, 2 * co, 2 * co, co, tc, x3, h->arena, &h->dec[l][0], &e) &&
-             fold_conv3(cur, co, co, co, tc, x3, h->arena, &h->dec[l][1], &e);
-    }
+    bool ok = for_each_layer(h, [&](int cin, int cin_p, int cout, Conv3* c) { return fold_conv3(cur, cin, cin_p, cout, tc, x3, h->arena, c, &e); },
+                             [&](int cin, int cout, UpConv* u) { return fold_upconv(cur, cin, cout, tc, x3, h->arena, u, &e); });
     if (ok) {
         const float* w = cur.next(); const float* b = cur.next();
         ok = w && b;
@@ -108,9 +183,7 @@ extern "C" int smk_generator_create(const SmkGeneratorDesc* desc, SmkGenerator**
             for (int o = 0; o < h->cout; ++o) for (int c = 0; c < f; ++c) W[(size_t)c * h->cout + o] = w[(size_t)o * f + c];
             e = h->arena.upload(W, &h->fw);
             if (e == cudaSuccess) e = h->arena.upload(b, (size_t)h->cout, &h->fb);
-            const std::vector<float> one((size_t)std::max(16 * f, h->cin_p), 1.f), zero(one.size(), 0.f);
-            if (e == cudaSuccess) e = h->arena.upload(one, &h->ones);
-            if (e == cudaSuccess) e = h->arena.upload(zero, &h->zeros);
+            if (e == cudaSuccess) e = upload_units(h);
             ok = e == cudaSuccess;
         }
     }
@@ -119,15 +192,56 @@ extern "C" int smk_generator_create(const SmkGeneratorDesc* desc, SmkGenerator**
         else smk::set_error("smk_generator_create: consumed %d tensors but %d were given (state_dict order, num_batches_tracked removed)", cur.i, cur.n);
         delete h; return e != cudaSuccess ? (int)e : -1;
     }
-    // every size is a multiple of 64 floats (init_features % 8 == 0), so the tensors are packed with no gaps
-    auto add = [h](const std::string& name, int S, int C) { h->saved.add(name, S, S, C); };
-    for (int l = 0; l < 4; ++l)
-        for (int j = 1; j <= 2; ++j) add("enc" + std::to_string(l + 1) + "conv" + std::to_string(j), 224 >> l, f << l);
-    add("bottleneckconv1", 14, 16 * f); add("bottleneckconv2", 14, 16 * f);
-    for (int r = 0; r < h->nres; ++r) add("res" + std::to_string(r) + "conv1", 14, 16 * f);
-    for (int l = 3; l >= 0; --l)
-        for (int j = 1; j <= 2; ++j) add("dec" + std::to_string(l + 1) + "conv" + std::to_string(j), 224 >> l, f << l);
+    add_saved(h);
     *out = h;
+    return 0;
+}
+
+extern "C" int smk_generator_live_create(int in_channels, int out_channels, int init_features, int res_blocks, int precision, SmkGenerator** out) {
+    SMK_REQUIRE(out, "smk_generator_live_create: null argument");
+    SMK_REQUIRE(precision == 0 || precision == 1 || precision == 3, "smk_generator_live_create: precision must be 0, 1 or 3");
+    SMK_REQUIRE(init_features > 0 && init_features % 8 == 0 && out_channels >= 1 && out_channels <= 4 && in_channels >= 1 && res_blocks >= 0,
+                "smk_generator_live_create: need init_features %% 8 == 0, out_channels in [1, 4], in_channels >= 1, res_blocks >= 0");
+    SMK_REQUIRE(precision == 0 || init_features % 32 == 0, "smk_generator_live_create: the tensor-core path needs init_features %% 32 == 0");
+    if (precision != 0) { if (int rc = smk::tc_init()) return rc; }
+    SmkGenerator* h = new SmkGenerator();
+    h->live = true;
+    configure(h, in_channels, out_channels, init_features, res_blocks, precision);
+    LiveGen L{h, precision != 0, precision == 3};
+    cudaError_t e = cudaSuccess;
+    int t = 0;
+    for_each_layer(h, [&](int cin, int cin_p, int cout, Conv3* c) { e = L.conv3(t, cin, cin_p, cout, c); t += 5; return e == cudaSuccess; },
+                   [&](int cin, int cout, UpConv* u) { e = L.upconv(t, cin, cout, u); t += 2; return e == cudaSuccess; });
+    if (e == cudaSuccess) {                           // the head: W[f][cout] from torch's [cout][f], and its bias
+        trn::PackJob j{};
+        j.kind = trn::MAT; j.rows = h->cout; j.cols = h->f; j.transpose = 1;
+        e = h->arena.alloc((size_t)h->f * h->cout, &h->fw);
+        j.hi = h->fw;
+        h->plan.jobs.push_back(trn::LiveJob{0, t, j});
+        if (e == cudaSuccess) e = h->arena.alloc((size_t)h->cout, &h->fb);
+        j.rows = 1; j.cols = h->cout; j.transpose = 0; j.hi = h->fb;
+        h->plan.jobs.push_back(trn::LiveJob{0, t + 1, j});
+        h->plan.bytes += 8.0 * (h->f + 1) * h->cout;
+        h->live_tensors = t + 2;
+    }
+    if (e == cudaSuccess) e = upload_units(h);
+    if (e != cudaSuccess) { smk::set_error("smk_generator_live_create: allocation failed: %s", cudaGetErrorString(e)); delete h; return (int)e; }
+    add_saved(h);
+    *out = h;
+    return 0;
+}
+
+extern "C" int smk_generator_refresh(SmkGenerator* h, const SmkGeneratorTrainArgs* a, void* stream) {
+    const char* fn = "smk_generator_refresh";
+    SMK_REQUIRE(h && h->live, "%s: not a live handle (smk_generator_live_create)", fn);
+    SMK_REQUIRE(a && a->tensors, "%s: null args", fn);
+    SMK_REQUIRE(a->n_tensors == h->live_tensors, "%s: expects %d tensors (state_dict order, num_batches_tracked removed), got %d", fn,
+                h->live_tensors, a->n_tensors);
+    for (int k = 0; k < a->n_tensors; ++k) SMK_REQUIRE(a->tensors[k], "%s: null tensor %d", fn, k);
+    SMK_REQUIRE(a->eps > 0.f, "%s: eps must be positive", fn);
+    const float* const* t[1] = {a->tensors};
+    if (int rc = trn::refresh(h->plan, t, nullptr, nullptr, &a->eps, (cudaStream_t)stream)) return rc;
+    h->refreshed = true;
     return 0;
 }
 
@@ -499,6 +613,7 @@ extern "C" int smk_generator_forward(const SmkGenerator* h, const float* x, int 
     SMK_REQUIRE(B > 0, "smk_generator_forward: negative batch");
     SMK_REQUIRE(ws && ws_bytes >= smk_generator_workspace_bytes(h, B), "smk_generator_forward: workspace too small");
     SMK_REQUIRE(!h->train, "smk_generator_forward: a train handle has no packed weights (smk_generator_forward_train)");
+    SMK_REQUIRE_WEIGHTS(h, "smk_generator_forward");
     return generator_forward(h, x, B, y, nullptr, ws, ws_bytes, (cudaStream_t)stream);
 }
 
@@ -519,6 +634,7 @@ extern "C" int smk_generator_forward_saved(const SmkGenerator* h, const float* x
     SMK_REQUIRE(saved_bytes > 0 && saved_bytes >= smk_generator_saved_bytes(h, B), "smk_generator_forward_saved: saved buffer too small");
     SMK_REQUIRE(ws && ws_bytes > 0 && ws_bytes >= smk_generator_workspace_bytes(h, B), "smk_generator_forward_saved: workspace too small");
     SMK_REQUIRE(!h->train, "smk_generator_forward_saved: a train handle has no packed weights (smk_generator_forward_train)");
+    SMK_REQUIRE_WEIGHTS(h, "smk_generator_forward_saved");
     return generator_forward(h, x, B, y, saved, ws, ws_bytes, (cudaStream_t)stream);
 }
 
@@ -535,6 +651,7 @@ extern "C" int smk_generator_backward(const SmkGenerator* h, int B, const float*
     SMK_REQUIRE(saved_bytes > 0 && saved_bytes >= smk_generator_saved_bytes(h, B), "smk_generator_backward: saved buffer too small");
     SMK_REQUIRE(ws && ws_bytes > 0 && ws_bytes >= smk_generator_backward_workspace_bytes(h, B), "smk_generator_backward: workspace too small");
     SMK_REQUIRE(!h->train, "smk_generator_backward: a train handle (smk_generator_backward_train)");
+    SMK_REQUIRE_WEIGHTS(h, "smk_generator_backward");
     cudaStream_t st = (cudaStream_t)stream;
     const int f = h->f, cb = 16 * f;
     const bool rnd = h->precision == 1;            // TF32 rounding of every gradient a TF32 dgrad reads (not at 3xTF32)

@@ -1,7 +1,7 @@
 // The generator's backward building blocks (generator.cu), shared by the input gradient of the eval path and the train path
 // (generator_train.cu).  NHWC fp32 activations; `round` rounds the result to TF32 for a TF32 consumer.
 #pragma once
-#include "conv.cuh"
+#include "train_common.cuh"
 
 // fwd / dgrad: the weight operands of the forward and of the input gradient (smk::pack_conv3; the dgrad's carry the BN scale)
 struct Conv3 { smk::GemmW fwd, dgrad; float* scale; float* bias; int cin, cin_p, cout; };
@@ -40,6 +40,10 @@ struct SmkGenerator {
     smk::DeviceArena arena;
     bool train = false;              // a train handle (smk_generator_train_create): topology only, no packed weights
     gen::TrainTopo topo;             // train handles
+    bool live = false;               // a live eval handle (smk_generator_live_create): weights set by smk_generator_refresh
+    bool refreshed = false;          // live handles: refreshed at least once
+    trn::LivePlan plan;              // live handles: the refresh's folds and pack jobs (one list: the state_dict tensors)
+    int live_tensors = 0;            // live handles: tensors the refresh reads
 };
 
 namespace gen {

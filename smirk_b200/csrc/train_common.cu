@@ -185,8 +185,8 @@ sum_chunks_kernel(const float* __restrict__ part, int n, long len, float* __rest
 
 // ---- per-call weight packing ------------------------------------------------------------------------------------------
 
-constexpr int kMaxPackJobs = 40;           // jobs per launch (the kernel takes them by value)
 struct PackJobs { PackJob j[kMaxPackJobs]; };
+static_assert(sizeof(PackJobs) <= 4096, "pack_kernel's job array must fit the classic 4 KB of kernel parameters");
 
 __host__ __device__ inline void pack_dims(const PackJob& q, int* N, int* K) {
     switch (q.kind) {
@@ -195,6 +195,7 @@ __host__ __device__ inline void pack_dims(const PackJob& q, int* N, int* K) {
         case UP_FWD: *N = 4 * q.cout; *K = q.cin; break;
         case UP_DGRAD: *N = q.cin; *K = 4 * q.cout; break;
         case UP_BIAS: *N = 4 * q.cout; *K = 1; break;
+        case DW_DGRAD: *N = q.cout; *K = 9; break;
         default: *N = q.rows; *K = q.cols; break;
     }
 }
@@ -206,9 +207,13 @@ __device__ inline float pack_value(const PackJob& q, int n, int k) {
         case CONV3_DGRAD: { const int tap = 8 - k / q.cout, co = k % q.cout; return n < q.cin ? __ldg(q.src + ((size_t)co * q.cin + n) * 9 + tap) : 0.f; }
         case UP_FWD: return __ldg(q.src + ((size_t)k * q.cout + n % q.cout) * 4 + n / q.cout);
         case UP_DGRAD: return __ldg(q.src + ((size_t)n * q.cout + k % q.cout) * 4 + k / q.cout);
+        case DW_DGRAD: return __ldg(q.src + (size_t)n * 9 + 8 - k);
         default: return __ldg(q.src + n % q.cout);                 // UP_BIAS
     }
 }
+
+// The output channel of W[n][k] that a job's scale belongs to.
+__device__ inline int pack_channel(const PackJob& q, int n, int k) { return q.kind == CONV3_DGRAD ? k % q.cout : n; }
 
 __global__ void __launch_bounds__(256)
 pack_kernel(const __grid_constant__ PackJobs p) {
@@ -217,7 +222,8 @@ pack_kernel(const __grid_constant__ PackJobs p) {
         const int n = q.rows * q.cols;
         for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
             const int r = i / q.cols, c = i % q.cols;
-            const float v = __ldg(q.src + i);
+            float v = __ldg(q.src + i);
+            if (q.scale) v = __fmul_rn(__ldg(q.scale + r), v);
             const int d = q.transpose ? c * q.rows + r : i;
             const float hi = q.split ? smk::round_tf32(v) : v;
             q.hi[d] = hi;
@@ -230,10 +236,25 @@ pack_kernel(const __grid_constant__ PackJobs p) {
     const int n_all = N * K;
     for (int d = blockIdx.x * blockDim.x + threadIdx.x; d < n_all; d += gridDim.x * blockDim.x) {
         const int n = q.split ? d / K : d % N, k = q.split ? d % K : d / N;    // TF32 [N][K] or fp32 [K][N]
-        const float v = pack_value(q, n, k);
+        float v = pack_value(q, n, k);
+        if (q.scale) v = __fmul_rn(__ldg(q.scale + pack_channel(q, n, k)), v);
         const float hi = q.split ? smk::round_tf32(v) : v;
         q.hi[d] = hi;
         if (q.lo) q.lo[d] = smk::round_tf32(v - hi);
+    }
+}
+
+struct FoldJobs { FoldJob j[kMaxFoldJobs]; };
+static_assert(sizeof(FoldJobs) <= 32764, "fold_kernel's job array must fit the kernel parameter space");
+
+// CTA = one BatchNorm.  The arithmetic of smk::fold_bn, each step correctly rounded and nothing contracted into an FMA.
+__global__ void __launch_bounds__(128)
+fold_kernel(const __grid_constant__ FoldJobs p) {
+    const FoldJob& q = p.j[blockIdx.x];
+    for (int o = threadIdx.x; o < q.n; o += blockDim.x) {
+        const float s = __fdiv_rn(q.gamma[o], __fsqrt_rn(__fadd_rn(q.var[o], q.eps)));
+        q.scale[o] = s;
+        q.bias[o] = __fsub_rn(q.beta[o], __fmul_rn(q.mean[o], s));
     }
 }
 
@@ -324,6 +345,40 @@ int pack(const std::vector<PackJob>& jobs, double bytes, cudaStream_t st) {
         SMK_CHECK_LAUNCH();
     }
     return 0;
+}
+
+int fold_bns(const std::vector<FoldJob>& jobs, cudaStream_t st) {
+    for (size_t j0 = 0; j0 < jobs.size(); j0 += kMaxFoldJobs) {
+        const int nj = (int)std::min<size_t>(kMaxFoldJobs, jobs.size() - j0);
+        FoldJobs p{};
+        long n = 0;
+        for (int j = 0; j < nj; ++j) { p.j[j] = jobs[j0 + j]; n += p.j[j].n; }
+        SMK_TAG("live_fold", 24.0 * n, 4.0 * n, st);
+        SMK_LAUNCH(fold_kernel, dim3(nj), dim3(128), 0, st, p);
+        SMK_CHECK_LAUNCH();
+    }
+    return 0;
+}
+
+int refresh(const LivePlan& p, const float* const* const* tensors, const float* const* head_w, const float* const* head_b, const float* eps,
+            cudaStream_t st) {
+    std::vector<FoldJob> folds;
+    folds.reserve(p.folds.size());
+    for (const LiveFold& f : p.folds) {
+        const float* const* t = tensors[f.list] + f.t;
+        FoldJob j = f.job;
+        j.gamma = t[1]; j.beta = t[2]; j.mean = t[3]; j.var = t[4]; j.eps = eps[f.list];
+        folds.push_back(j);
+    }
+    std::vector<PackJob> jobs;
+    jobs.reserve(p.jobs.size());
+    for (const LiveJob& l : p.jobs) {
+        PackJob j = l.job;
+        j.src = l.t == -1 ? head_w[l.list] : l.t == -2 ? head_b[l.list] : tensors[l.list][l.t];
+        jobs.push_back(j);
+    }
+    if (int rc = fold_bns(folds, st)) return rc;
+    return pack(jobs, p.bytes, st);
 }
 
 }  // namespace trn

@@ -48,12 +48,36 @@ int pw_wgrad(const float* g, const float* a, long M, int Co, int Ci, float* part
 //   UP_FWD       torch [cin][cout][2][2]   N = 4 cout,   K = cin:     W(k = c, n = q cout + o) = w[c][o][q]
 //   UP_DGRAD     the same                  N = cin,      K = 4 cout:  W'(k = q cout + o, c) = w[c][o][q]
 //   UP_BIAS      bias [cout]               N = 4 cout,   K = 1:       b[n % cout] (split 0)
-// Input channels cin..cin_p-1 are zero.
-enum PackKind { MAT = 0, CONV3_FWD, CONV3_DGRAD, UP_FWD, UP_DGRAD, UP_BIAS };
-struct PackJob { const float* src; float* hi; float* lo; int rows, cols, transpose, split; int kind, cin, cin_p, cout; };
+//   DW_DGRAD     depthwise [cout][1][3][3] N = cout,     K = 9:       W'(k, c) = w[c][8 - k] (flipped taps)
+// Input channels cin..cin_p-1 are zero.  scale (optional, null: none): a per-output-channel factor multiplied in (fp32,
+// uncontracted) before the split: MAT's row r, CONV3_DGRAD's co, DW_DGRAD's c (the folded BN scale of a dgrad operand).
+enum PackKind { MAT = 0, CONV3_FWD, CONV3_DGRAD, UP_FWD, UP_DGRAD, UP_BIAS, DW_DGRAD };
+struct PackJob { const float* src; float* hi; float* lo; int rows, cols, transpose, split; int kind, cin, cin_p, cout; const float* scale; };
 // Floats of a job's output (per copy: lo takes as many again).
 size_t pack_floats(const PackJob& j);
 // Runs the jobs, as many launches as the job list needs.  bytes: the profiler's byte count of the whole pack.
 int pack(const std::vector<PackJob>& jobs, double bytes, cudaStream_t st);
+constexpr int kMaxPackJobs = 40;           // jobs per pack launch (the kernel takes them by value)
+
+// Eval-mode BatchNorm folded on the device: scale = gamma / sqrt(var + eps), bias = beta - mean * scale, bit for bit the
+// host's smk::fold_bn.
+struct FoldJob { const float *gamma, *beta, *mean, *var; float *scale, *bias; int n; float eps; };
+constexpr int kMaxFoldJobs = 160;          // BatchNorms per fold launch (by value: > 4 KB of parameters, sm_70+ / CUDA 12.1+)
+int fold_bns(const std::vector<FoldJob>& jobs, cudaStream_t st);
+
+// The device refresh of a live eval handle, recorded at create time: per BatchNorm a fold and per operand a pack job whose
+// source is tensor t of list `list` of the caller's tensor lists (t = -1 / -2: the list's head weight / bias).  A refresh
+// fills in the pointers, folds every BatchNorm, then packs (the dgrad jobs read the scales the fold wrote).
+struct LiveFold { int list, t; FoldJob job; };        // job.gamma.. = tensors[list][t + 1 .. t + 4] (t: the conv weight)
+struct LiveJob { int list, t; PackJob job; };
+struct LivePlan { std::vector<LiveFold> folds; std::vector<LiveJob> jobs; double bytes = 0; };
+// Launches of one refresh: the fold batches, then the pack batches.
+inline int refresh_launches(const LivePlan& p) {
+    return (int)((p.folds.size() + kMaxFoldJobs - 1) / kMaxFoldJobs + (p.jobs.size() + kMaxPackJobs - 1) / kMaxPackJobs);
+}
+// tensors[list]: the caller's device tensor list; head_w / head_b[list]: its heads (null when the plan reads none); eps[list]:
+// the epsilon of its BatchNorms.
+int refresh(const LivePlan& p, const float* const* const* tensors, const float* const* head_w, const float* const* head_b, const float* eps,
+            cudaStream_t st);
 
 }  // namespace trn

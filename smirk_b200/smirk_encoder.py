@@ -15,6 +15,13 @@ process-wide with ``set_train_mode_default(True)`` (``python -m smirk_b200.dropi
 normalise with batch statistics and update their running statistics (``smk_encoder_forward_train``), and every parameter
 that requires grad gets its gradient (``smk_encoder_backward_train``).  Batch statistics couple the images of a batch.
 Without the opt-in a train-mode encoder raises; eval-mode weight gradients are not implemented.
+
+Live weights (``live_weights_(True)``, off by default) run the eval path on a handle whose folded BatchNorms and packed
+operands are refreshed on the device from the module's own tensors at every call (``smk_encoder_refresh``), instead of
+a handle packed on the host whenever a parameter or buffer changes: no host round trip, no allocation, and a CUDA graph of
+the call reads the weights and running statistics of replay time.  It suits a frozen encoder whose weights another path
+keeps training (the second path of the trainer's step); fixed inference weights keep the host-packed handle, which a
+captured graph (``SmirkPipeline.capture``) holds at the weights of capture time.
 """
 import ctypes as C
 
@@ -168,6 +175,65 @@ class _NativeEncoder(_lib.NativeModule, nn.Module):
                 m._allow_train = bool(on)
         return self
 
+    def live_weights_(self, on=True):
+        """Run the eval path of this module and its sub-encoders on weights refreshed on the device at every call (see the
+        module docstring); returns the module."""
+        for m in self.modules():
+            if isinstance(m, _NativeEncoder):
+                m._live = bool(on)
+        return self
+
+    def _live_tensors(self):
+        """The tensors a refresh reads, flat: per backbone its ``encoder`` tensors in state_dict order without
+        num_batches_tracked (conv weight, BN weight, bias, running_mean, running_var per conv), then the head's weight and
+        bias."""
+        out = []
+        for part in self._parts():
+            if part is not None:
+                enc, head = part
+                out += [v for k, v in enc.encoder.state_dict(keep_vars=True).items() if not k.endswith("num_batches_tracked")]
+                out += [head.weight, head.bias]
+        return out
+
+    def _live_handle(self, dev):
+        present = tuple(p is not None for p in self._parts())
+        mask = sum(1 << i for i, p in enumerate(present) if p)
+        return _lib.live_handle(self, "encoder", dev, (present, self.n_shape, self.n_exp, int(self.precision)),
+                                (mask, self.n_shape, self.n_exp, int(self.precision)))
+
+    def _refresh(self, h, dev, tensors):
+        """smk_encoder_refresh of live handle h from ``_live_tensors()`` (or the tensors an autograd context saved)."""
+        a, keep = _lib.SmkEncoderTrainArgs(), []
+        it = iter(tensors)
+        ptr = lambda t: C.cast(t.data_ptr(), _lib.c_f32p)
+        for i, part in enumerate(self._parts()):
+            if part is None:
+                continue
+            bns = [m for m in part[0].encoder.modules() if isinstance(m, nn.BatchNorm2d)]
+            eps = {m.eps for m in bns}
+            if len(eps) != 1:
+                raise RuntimeError("smirk_b200.%s: live weights need one eps for all BatchNorms of a backbone, got %s"
+                                   % (type(self).__name__, sorted(eps)))
+            ts = [next(it) for _ in range(5 * len(bns) + 2)]
+            for t in ts:
+                _check_param(t, dev)
+            arr = (_lib.c_f32p * (len(ts) - 2))(*[ptr(t) for t in ts[:-2]])
+            keep.append(arr)
+            a.tensors[i] = C.cast(arr, C.POINTER(_lib.c_f32p))
+            a.n_tensors[i] = len(ts) - 2
+            a.head_w[i], a.head_b[i] = ptr(ts[-2]), ptr(ts[-1])
+            a.eps[i] = eps.pop()
+        _lib.refresh("encoder", h, dev, a)
+
+    def _eval_handle(self, dev):
+        """-> (handle, tensors): the host-packed eval handle and None, or with live weights the live handle, refreshed
+        from the tensors returned."""
+        if not self.__dict__.get("_live"):
+            return self._native_handle(dev), None
+        h, tensors = self._live_handle(dev), self._live_tensors()
+        self._refresh(h, dev, tensors)
+        return h, tensors
+
     def _train_allowed(self):
         on = self.__dict__.get("_allow_train")
         return _lib.train_mode_default() if on is None else on
@@ -216,7 +282,7 @@ class _NativeEncoder(_lib.NativeModule, nn.Module):
             return [next(it) if p is not None else None for p in self._parts()]
         with torch.no_grad():
             dev = img.device
-            h = self._native_handle(dev)
+            h = self._eval_handle(dev)[0]
             x = _lib.dev_f32(img, "img")
             B = x.shape[0]
             outs = self._outputs(B, dev)
@@ -225,16 +291,21 @@ class _NativeEncoder(_lib.NativeModule, nn.Module):
             return outs
 
     def _forward_saved(self, img):
-        """-> (handle, [raw outputs | None], saved): the grad-mode forward, its activations in a buffer of their own."""
+        """-> (handle, outputs, saved) of ``_forward_saved_live``."""
+        return self._forward_saved_live(img)[:3]
+
+    def _forward_saved_live(self, img):
+        """-> (handle, [raw outputs | None], saved, live tensors | None): the grad-mode forward, its activations in a buffer
+        of their own."""
         dev = img.device
-        h = self._native_handle(dev)
+        h, tensors = self._eval_handle(dev)
         x = _lib.dev_f32(img, "img")
         B = x.shape[0]
         outs = self._outputs(B, dev)
         saved = _lib.saved_buffer("encoder", h, B, dev)
         ws = self._native_workspace("forward", _lib.call("smk_encoder_workspace_bytes", dev, h, B), dev)
         _lib.call("smk_encoder_forward_saved", dev, h, x, B, *outs, saved, saved.numel() * 4, ws, ws.numel())
-        return h, outs, saved
+        return h, outs, saved, tensors
 
     @torch.no_grad()
     def saved_activations(self, img):
@@ -364,22 +435,29 @@ def _check_param(t, dev):
 class _EncoderFunction(torch.autograd.Function):
     """Frozen encoder: the raw outputs (pose_cam, shape, expr: those the module holds) of img, and the gradient with
     respect to img only.  An output that receives no gradient arrives as None and its backbone's backward launches
-    nothing.  The activations are saved per call, so several forwards may share one backward."""
+    nothing.  The activations are saved per call, so several forwards may share one backward.  With live weights the
+    tensors the refresh read are saved too (autograd raises if one is modified in place before the backward), and the
+    backward refreshes the handle from them again when another call has refreshed it since."""
 
     @staticmethod
     def forward(ctx, img, module):
-        h, outs, saved = module._forward_saved(img)
+        h, outs, saved, tensors = module._forward_saved_live(img)
         ctx.set_materialize_grads(False)
         ctx.handle, ctx.module, ctx.dtype, ctx.B = h, module, img.dtype, img.shape[0]
         ctx.present = [o is not None for o in outs]
-        ctx.save_for_backward(saved)
+        ctx.live = tensors is not None
+        ctx.generation = h.generation if ctx.live else None
+        ctx.save_for_backward(saved, *(tensors or ()))
         return tuple(o for o in outs if o is not None)
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, *grads):
-        saved, = ctx.saved_tensors
+        saved, *tensors = ctx.saved_tensors
         m, dev, B = ctx.module, saved.device, ctx.B
+        if ctx.live and ctx.handle.generation != ctx.generation:
+            m._refresh(ctx.handle, dev, tensors)
+            ctx.generation = ctx.handle.generation
         it = iter(grads)
         g = [next(it) if p else None for p in ctx.present]
         g = [None if t is None else _lib.dev_f32(t, "grad") for t in g]

@@ -16,6 +16,10 @@ running statistics (``smk_generator_forward_train``, also under ``torch.no_grad(
 grad, and the input when it requires grad, gets its gradient (``smk_generator_backward_train``).  Batch statistics couple
 the images of a batch.  Without the opt-in a train-mode generator raises.
 
+Live weights (``live_weights_(True)``, off by default) run the eval path on a handle refreshed on the device from the
+module's own tensors at every call (``smk_generator_refresh``), as the encoder's: for a frozen generator whose weights
+another path keeps training.  Fixed inference weights keep the host-packed handle.
+
 ``precision`` (part of the native handle's key, so it may change between calls): 0 = fp32 CUDA cores, 1 = TF32 tensor cores,
 3 = 3xTF32 tensor cores (each operand split into a TF32 head and tail, three products per term: fp32-equivalent forward and
 input gradient, the same launches as 1).  Precisions 1 and 3 need ``init_features % 32 == 0``.
@@ -104,6 +108,39 @@ class SmirkGenerator(_lib.NativeModule, nn.Module):
         self._allow_train = bool(on)
         return self
 
+    def live_weights_(self, on=True):
+        """Run the eval path on weights refreshed on the device at every call (see the module docstring); returns the
+        module."""
+        self._live = bool(on)
+        return self
+
+    def _live_tensors(self):
+        """The tensors a refresh reads: the state_dict's in its order, without num_batches_tracked."""
+        return [v for k, v in self.state_dict(keep_vars=True).items() if not k.endswith("num_batches_tracked")]
+
+    def _refresh(self, h, dev, tensors):
+        """smk_generator_refresh of live handle h from ``_live_tensors()`` (or the tensors an autograd context saved)."""
+        eps = {m.eps for m in self.modules() if isinstance(m, nn.BatchNorm2d)}
+        if len(eps) != 1:
+            raise RuntimeError("smirk_b200.SmirkGenerator: live weights need one eps for all BatchNorms, got %s" % sorted(eps))
+        for t in tensors:
+            if t.device != dev or t.dtype != torch.float32 or not t.is_contiguous():
+                raise RuntimeError("smirk_b200: live weights need contiguous float32 parameters and buffers on %s" % dev)
+        arr = (_lib.c_f32p * len(tensors))(*[C.cast(t.data_ptr(), _lib.c_f32p) for t in tensors])
+        a = _lib.SmkGeneratorTrainArgs()
+        a.tensors, a.n_tensors, a.eps = C.cast(arr, C.POINTER(_lib.c_f32p)), len(tensors), eps.pop()
+        _lib.refresh("generator", h, dev, a)
+
+    def _eval_handle(self, dev):
+        """-> (handle, tensors): the host-packed eval handle and None, or with live weights the live handle (keyed on the
+        configuration and precision only), refreshed from the tensors returned."""
+        if not self.__dict__.get("_live"):
+            return self._native_handle(dev), None
+        h = _lib.live_handle(self, "generator", dev, (self._cfg, int(self.precision)), self._cfg + (int(self.precision),))
+        tensors = self._live_tensors()
+        self._refresh(h, dev, tensors)
+        return h, tensors
+
     def _train_allowed(self):
         on = self.__dict__.get("_allow_train")
         return _lib.train_mode_default() if on is None else on
@@ -134,7 +171,7 @@ class SmirkGenerator(_lib.NativeModule, nn.Module):
             return _GeneratorFunction.apply(x, self)
         with torch.no_grad():
             dev = x.device
-            h = self._native_handle(dev)
+            h = self._eval_handle(dev)[0]
             x = _lib.dev_f32(x, "x")
             self._check_input(x)
             B = x.shape[0]
@@ -144,16 +181,20 @@ class SmirkGenerator(_lib.NativeModule, nn.Module):
             return y
 
     def _forward_saved(self, x):
-        """-> (handle, y, saved): the grad-mode forward, its activations in a buffer of their own."""
+        """-> (handle, outputs, saved) of ``_forward_saved_live``."""
+        return self._forward_saved_live(x)[:3]
+
+    def _forward_saved_live(self, x):
+        """-> (handle, y, saved, live tensors | None): the grad-mode forward, its activations in a buffer of their own."""
         dev = x.device
-        h = self._native_handle(dev)
+        h, tensors = self._eval_handle(dev)
         x = _lib.dev_f32(x, "x")
         B = x.shape[0]
         y = torch.empty(B, self._cfg[1], 224, 224, dtype=torch.float32, device=dev)
         saved = _lib.saved_buffer("generator", h, B, dev)
         ws = self._native_workspace("forward", _lib.call("smk_generator_workspace_bytes", dev, h, B), dev)
         _lib.call("smk_generator_forward_saved", dev, h, x, B, y, saved, saved.numel() * 4, ws, ws.numel())
-        return h, y, saved
+        return h, y, saved, tensors
 
     @torch.no_grad()
     def saved_activations(self, x):
@@ -255,20 +296,27 @@ class SmirkGenerator(_lib.NativeModule, nn.Module):
 
 class _GeneratorFunction(torch.autograd.Function):
     """Frozen generator: y = G(x), and the gradient with respect to x only.  The activations are saved per call, so
-    several forwards may share one backward."""
+    several forwards may share one backward.  With live weights the tensors the refresh read are saved too (autograd
+    raises if one is modified in place before the backward), and the backward refreshes the handle from them again when
+    another call has refreshed it since."""
 
     @staticmethod
     def forward(ctx, x, module):
-        h, y, saved = module._forward_saved(x)
+        h, y, saved, tensors = module._forward_saved_live(x)
         ctx.handle, ctx.module, ctx.dtype = h, module, x.dtype    # the handle the activations were computed with
-        ctx.save_for_backward(y, saved)
+        ctx.live = tensors is not None
+        ctx.generation = h.generation if ctx.live else None
+        ctx.save_for_backward(y, saved, *(tensors or ()))
         return y
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, g_y):
-        y, saved = ctx.saved_tensors
+        y, saved, *tensors = ctx.saved_tensors
         m, dev, B = ctx.module, y.device, y.shape[0]
+        if ctx.live and ctx.handle.generation != ctx.generation:
+            m._refresh(ctx.handle, dev, tensors)
+            ctx.generation = ctx.handle.generation
         g_y = _lib.dev_f32(g_y, "g_y")
         g_x = torch.empty(B, m._cfg[0], 224, 224, dtype=torch.float32, device=dev)
         ws = m._native_workspace("backward", _lib.call("smk_generator_backward_workspace_bytes", dev, ctx.handle, B), dev)

@@ -11,12 +11,22 @@ B = 32, Ke = 1, on one GPU, in three arms:
   graph   the device arm with path1 captured once in a CUDA graph (the second path's frozen network runs the eval path,
           whose handle folds BatchNorm statistics on the host, so it is not captured; its rows repeat the device arm).
 
+Then SmirkTrainer.step as the trainer runs it (tests/test_gpu_train_flow_live.py's Trainer: step1's forward, backward and
+Adam steps, then step2 at the batch's freeze parity with its Adam step, the generator's gradient clipped at parity 0),
+parities alternating, in three more arms:
+
+  step_host   eager, the second path's frozen network on the host-packed eval handle, rebuilt on every step because the
+              first path changed its weights and running statistics;
+  step_live   eager, the frozen network on live weights (``live_weights_(True)``: folded and repacked on the device);
+  step_graph  step_live captured as two CUDA graphs, one per freeze parity, replayed alternately.
+
 The arms alternate in each of --rounds rounds after --warmup steps; each time is the median over rounds of CUDA-event
-times over --iters calls, with [min, max].  Then per arm and path the CUDA activities of one call (torch.profiler), and
+times over --iters calls, with [min, max] (the trainer-step arms: per step, over --iters pairs of steps).
+--trainer-step-only skips the path arms.  Then per arm and path the CUDA activities of one call (torch.profiler), and
 for the device arm the library's event-profiler tags of one whole step (the stages' own times, the largest tags).  The
 GPU's name and power limit are read in the same call.  Prints one JSON line.
 
-    python tools/bench_train_step.py [--iters 5] [--warmup 2] [--rounds 5] [--batch 32]
+    python tools/bench_train_step.py [--iters 5] [--warmup 2] [--rounds 5] [--batch 32] [--trainer-step-only]
 """
 import argparse
 import json
@@ -97,6 +107,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--batch", type=int, default=32)
+    ap.add_argument("--trainer-step-only", action="store_true")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_train_step needs a GPU"
     import tempfile
@@ -111,6 +122,11 @@ def main():
     finally:
         os.chdir(old)
     B = args.batch
+    gpu = {"gpu": torch.cuda.get_device_properties(0).name, "power_limit_w": power_limit_w(), "B": B, "Ke": 1, "precision": 3}
+    step_ms = trainer_steps(tf, bases, B, args)
+    if args.trainer_step_only:
+        print(json.dumps(dict(gpu, trainer_step_ms_median_min_max=step_ms)))
+        return
     batch = tf.make_batch(B, 7)
     flows = {"torch": tf.TrainFlow(bases, 3, seed=1), "device": tf.TrainFlow(bases, 3, seed=1), "graph": tf.TrainFlow(bases, 3, seed=1)}
     flows["torch"].masking = TorchMasking(bases["faces"], bases["base_prob"])
@@ -165,9 +181,46 @@ def main():
     rep = _lib.profiler_report()
     stage = {k: round(v["ms"], 4) for k, v in rep.items() if k.startswith(("mask_", "cycle_"))}
     top = dict(sorted(((k, round(v["ms"], 3)) for k, v in rep.items()), key=lambda kv: -kv[1])[:8])
-    print(json.dumps({"gpu": torch.cuda.get_device_properties(0).name, "power_limit_w": power_limit_w(), "B": B, "Ke": 1,
-                      "precision": 3, "ms_median_min_max": ms, "cuda_activities_per_call": activities,
-                      "device_step_stage_ms": stage, "device_step_top_tags_ms": top}))
+    print(json.dumps(dict(gpu, ms_median_min_max=ms, cuda_activities_per_call=activities, device_step_stage_ms=stage,
+                          device_step_top_tags_ms=top, trainer_step_ms_median_min_max=step_ms)))
+
+
+def trainer_steps(tf, bases, B, args):
+    """-> {arm: [median, min, max] ms per SmirkTrainer.step} of the step_host / step_live / step_graph arms."""
+    from test_gpu_train_flow_live import Trainer
+    data = [tf.make_batch(B, 70 + s) for s in range(2)]
+    trainers = {"step_host": Trainer(tf.TrainFlow(bases, 3, seed=1)), "step_live": Trainer(tf.TrainFlow(bases, 3, seed=1)),
+                "step_graph": Trainer(tf.TrainFlow(bases, 3, seed=1))}
+    for name in ("step_live", "step_graph"):
+        trainers[name].flow.enc.live_weights_(True)
+        trainers[name].flow.gen.live_weights_(True)
+    fns = {}
+    for name in ("step_host", "step_live"):
+        t = trainers[name]
+        fns[name] = lambda t=t: (t.step(data[0], 0), t.step(data[1], 1))
+    G = trainers["step_graph"]
+    static = [{k: v.clone() for k, v in d.items()} for d in data]
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        for parity in (0, 1):
+            G.step(static[parity], parity)
+    torch.cuda.current_stream().wait_stream(s)
+    graphs = []
+    for parity in (0, 1):
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, pool=graphs[0].pool() if graphs else None):     # replayed in capture order
+            G.step(static[parity], parity)
+        graphs.append(g)
+    fns["step_graph"] = lambda: (graphs[0].replay(), graphs[1].replay())
+    for fn in fns.values():
+        for _ in range(args.warmup):
+            fn()
+    times = {n: [] for n in fns}
+    for _ in range(args.rounds):
+        for n, fn in fns.items():
+            times[n].append(timed(fn, args.iters) / 2)
+    return {n: [round(statistics.median(v), 3), round(min(v), 3), round(max(v), 3)] for n, v in times.items()}
 
 
 if __name__ == "__main__":
